@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- MSCKF updates/sec on the B200 engine (and the reference arm / CPU baseline beside it).
+"""bench.py -- MSCKF updates/sec on the H100 engine (and the reference arm / CPU baseline beside it).
 
 A "step" is one pass of the hot path over one batch of synthetic input.  The unit of work is BASELINE.json configs[1]:
 ONE marginalize() (msckf.h:336-449 -> measurementUpdate :1325-1423) on 300 feature tracks x 30 camera clones, float32,
@@ -78,7 +78,7 @@ class ClockSampler(threading.Thread):
 
     def __init__(self, index):
         super().__init__(daemon=True)
-        self.index, self.samples, self.reasons, self.stop_flag, self.max_mhz = index, [], set(), False, None
+        self.index, self.samples, self.reasons, self.stop_flag, self.max_mhz, self.power_limit_w = index, [], set(), False, None, None
 
     def run(self):
         try:
@@ -86,6 +86,7 @@ class ClockSampler(threading.Thread):
             nv.nvmlInit()
             h = nv.nvmlDeviceGetHandleByIndex(self.index)
             self.max_mhz = nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM)
+            self.power_limit_w = nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
             names = {"hw_slowdown": nv.nvmlClocksThrottleReasonHwSlowdown, "hw_thermal_slowdown": nv.nvmlClocksThrottleReasonHwThermalSlowdown,
                      "sw_thermal_slowdown": nv.nvmlClocksThrottleReasonSwThermalSlowdown, "sw_power_cap": nv.nvmlClocksThrottleReasonSwPowerCap}
             while not self.stop_flag:
@@ -99,7 +100,7 @@ class ClockSampler(threading.Thread):
             self.reasons.add(f"nvml_unavailable:{type(e).__name__}")
 
     def result(self):
-        return {"sm_mhz": float(np.median(self.samples)) if self.samples else None, "sm_max_mhz": self.max_mhz,
+        return {"sm_mhz": float(np.median(self.samples)) if self.samples else None, "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w,
                 "reasons": sorted(self.reasons), "samples": len(self.samples)}
 
 
@@ -167,8 +168,8 @@ def run_reference(args, rank, world):
     if rank != 0:
         return
     # the oracle's working set (three 17100 x 195 matrices per filter) makes it memory-bandwidth bound: throughput
-    # saturates around 16 concurrent filters (measured on the 128-core GPU box: 8.1/s with 128 threads vs 2.0/s with 1),
-    # and a step must stay bounded, so a step = one update on each of min(cores, 16) threads
+    # saturates after a few concurrent filters, and a step must stay bounded, so a step = one update on each of
+    # min(cores, 16) threads
     cores = min(os.cpu_count() or 1, 16)
     from concurrent.futures import ThreadPoolExecutor
     from msckf_mono_b200 import synth
@@ -351,6 +352,31 @@ def parity_record(local_rank):
     return out
 
 
+def dump_outputs(out_dir, work, reps, max_bytes=64 << 20):
+    """What a caller of the timed batch update receives, per filter: the report (accept flags, stacked rows m, rank) and
+    the corrected filter state (IMU state, clone poses, covariance, delta-x).  About 1.5 MB at 8 filters of 300 x 30.
+    Past `max_bytes` in all, a fixed seeded sample of the filters is written (`filter_index` names them)."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    n = work[0].covariance().shape[0]
+    per_filter = 4 * (len(reps[0]["accepted"]) + 29 + 7 * work[0].num_clones() + n * n) + 8 * (2 + n)
+    keep = np.arange(len(work))
+    if per_filter * len(work) > max_bytes:
+        keep = np.sort(np.random.default_rng(0).choice(len(work), max(1, max_bytes // per_filter), replace=False))
+    work, reps = [work[i] for i in keep], [reps[i] for i in keep]
+    states = [w.state() for w in work]
+    arrays = {
+        "filter_index": keep.astype(np.float64),
+        "accepted": np.stack([r["accepted"] for r in reps]).astype(np.float32),
+        "m_rank": np.array([[r["m"], r["rank"]] for r in reps], dtype=np.float64),
+        "imu_state": np.stack([s[0] for s in states]).astype(np.float32),
+        "clone_poses": np.stack([s[1] for s in states]).astype(np.float32),
+        "covariance": np.stack([w.covariance() for w in work]).astype(np.float32),
+        "delta_x": np.stack([w.delta_x() for w in work]).astype(np.float64),
+    }
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -359,7 +385,8 @@ def main():
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--filters", type=int, default=FILTERS_PER_GPU, help="independent filters per GPU in the device batch")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
-    ap.add_argument("--skip-extras", action="store_true", help="profiling aid: only the device-timed steps (use under ncu)")
+    ap.add_argument("--skip-extras", action="store_true", help="profiling aid: only the device-timed steps")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
@@ -379,7 +406,7 @@ def main():
     from msckf_mono_b200 import capi, shard
 
     K, W, F = args.steps, args.warmup, args.filters
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 50 MB L2
 
     def flush_l2():
         flush.add_(1.0)
@@ -438,6 +465,8 @@ def main():
     t_wall = time.perf_counter() - t_wall0
     launches_timed = grp.launch_count() - l0
     assert all(r["m"] == N_FEAT * (2 * N_CLONES - 3) for r in reps), [r["m"] for r in reps]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), work, reps)
     dev_ms = float(np.sum(times))
     if args.skip_extras:
         sampler.stop_flag = True
@@ -497,15 +526,10 @@ def main():
         peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
     except Exception:
         pass
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
-    peak_src = "of measured (MEASURED_PEAKS.json hbm_gbs, burst copy)" if "hbm_gbs" in peaks else "of fallback (6.65 TB/s)"
+    hbm_peak = peaks.get("hbm_gbs", 3350.0)
+    peak_src = "of measured (MEASURED_PEAKS.json hbm_gbs, burst copy)" if "hbm_gbs" in peaks else "of the H100 SXM data sheet (3.35 TB/s)"
     bytes_alg = algorithmic_bytes(N_FEAT, N_CLONES, 4)
     achieved = F * bytes_alg / (kern_ms[dom] * 1e-3) / 1e9
-    traffic = None
-    try:
-        traffic = json.loads((ROOT / "profiles" / "traffic.json").read_text()).get(dom)
-    except Exception:
-        pass
     cpu_val, cpu_n, cpu_wall = cpu_oracle_updates(args.cpu_seconds, 1, DTYPE)
 
     value = world * F * K / (dev_ms * 1e-3)
@@ -520,12 +544,12 @@ def main():
                    "stacked_rows_m": N_FEAT * (2 * N_CLONES - 3), "state_dim_n": 15 + 6 * N_CLONES,
                    "timing": "CUDA events on the batch's stream around the update's kernels, summed over steps, max over ranks",
                    "l2": "flushed between timed iterations", "parallelism": f"independent filters, {world} GPU(s) x {F}, no data-path collective"},
-        "clocks": sampler.result(),
+        "gpu": torch.cuda.get_device_name(local_rank), "clocks": sampler.result(),
         "e2e": {"value": world * F * K / e2e_s, "unit": "updates/s", "h2d_bytes_per_step": int(h2d_bytes), "d2h_bytes_per_step": int(rep_bytes),
                 "ms_per_step": 1e3 * e2e_s / K, "e2e_over_device": (e2e_s / K) / (dev_ms * 1e-3 / K),
                 "path": "msckf_b200_batch_update (C-ABI) with host buffers: pack into pinned, one H2D, kernels, one D2H, unpack; host wall clock"},
         "gpu_launches": int(launches_timed),
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak, "traffic": traffic,
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
                      "kernel": dom, "kernel_ms": kern_ms[dom], "peak_source": peak_src, "algorithmic_bytes_per_update": bytes_alg,
                      "updates_per_launch": F, "whole_step_gbs": F * bytes_alg / (dev_ms / K * 1e-3) / 1e9,
                      "whole_step_frac": F * bytes_alg / (dev_ms / K * 1e-3) / 1e9 / hbm_peak,

@@ -1,4 +1,4 @@
-/* include/msckf_b200.h -- C-ABI of the B200 MSCKF measurement-update engine (libmsckf_b200.so).
+/* include/msckf_b200.h -- C-ABI of the H100 MSCKF measurement-update engine (libmsckf_b200.so).
  *
  * The reference (daniilidis-group/msckf_mono) has no plugin / FFI boundary: its filter is the header-only
  * C++ class template msckf_mono::MSCKF<_S> (include/msckf_mono/msckf.h:31-1512).  This C-ABI is what the
@@ -126,7 +126,7 @@ int msckf_b200_batch_destroy(msckf_b200_batch* b);
 /* tracks[n] / reports[n]: one per engine, in the order given to _create; reports may be NULL.  Up to `threads` host threads
  * share the validation and packing of the n track batches (<= 1: the calling thread does all of it); the engine uses fewer
  * for small batches -- one per 8 MB of observations: packing from several cores makes the following host-to-device copy slower
- * than the packing gets faster (measured, profiles/README.md). */
+ * than the packing gets faster (measured with scripts/e2e_breakdown.py). */
 int msckf_b200_batch_update_async(msckf_b200_batch* b, int mode, const msckf_b200_tracks* tracks, int threads);
 int msckf_b200_batch_fetch(msckf_b200_batch* b, msckf_b200_report* reports);
 int msckf_b200_batch_update(msckf_b200_batch* b, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports, int threads);

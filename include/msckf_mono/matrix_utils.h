@@ -1,6 +1,6 @@
 // include/msckf_mono/matrix_utils.h -- drop-in for the reference's include/msckf_mono/matrix_utils.h (":N" = its line N):
 // the small host helpers the reference's callers reach through this header (src/corner_detector.cpp via
-// corner_detector.h:24).  Inside the B200 filter none of them is on the numeric path any more -- the skew / Omega
+// corner_detector.h:24).  Inside the GPU filter none of them is on the numeric path any more -- the skew / Omega
 // products live in k_propagate / k_augment and the covariance slicing of the prune functions is k_gather
 // (msckf_mono_b200/csrc/state_kernels.cuh) -- so these are plain host functions over the boundary types of types.h,
 // compiled against Eigen when it is present and against the stand-ins of pod_linalg.h otherwise.

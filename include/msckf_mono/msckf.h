@@ -4,7 +4,7 @@
 // Same namespace, class name, template parameter and public member functions.  All integer bookkeeping
 // (feature tracks, clone ids, residualisation and pruning decisions) runs on the host exactly as in the
 // reference; all floating-point work goes through the C-ABI of libmsckf_b200.so (include/msckf_b200.h)
-// into hand-written sm_100a kernels, with the covariance, clone poses and IMU state device resident.
+// into hand-written sm_90a kernels, with the covariance, clone poses and IMU state device resident.
 // There is no CPU fallback: a failed device call throws std::runtime_error.
 //
 // Call-order contract (same as the reference's drivers, src/ros_interface.cpp:92-116,

@@ -1,6 +1,6 @@
-"""msckf_mono_b200 -- B200-native MSCKF measurement-update engine behind the msckf_mono::MSCKF<_S> surface.
+"""msckf_mono_b200 -- H100-native MSCKF measurement-update engine behind the msckf_mono::MSCKF<_S> surface.
 
-The product is native: hand-written sm_100a kernels + a C-ABI (include/msckf_b200.h) + the drop-in C++ class
+The product is native: hand-written sm_90a kernels + a C-ABI (include/msckf_b200.h) + the drop-in C++ class
 (include/msckf_mono/msckf.h), built in-tree as msckf_mono_b200/libmsckf_b200.so.  This Python package only
 holds the ctypes view used by the tests and bench.py, and the synthetic workload generator.
 There is no CPU fallback: if the library or a CUDA device is missing, construction fails loudly.
@@ -21,7 +21,7 @@ def lib_path() -> Path:
 
 
 def engine_filter(dtype=np.float32, device=0, max_clones=0, max_tracks=0, max_obs=0):
-    """msckf_mono::MSCKF<float|double> on the B200 engine, through the C view (include/msckf_mono_c.h)."""
+    """msckf_mono::MSCKF<float|double> on the H100 engine, through the C view (include/msckf_mono_c.h)."""
     import ctypes as C
     from .cview import CFilter
     f = CFilter(lib_path(), "msckf_mono_", dtype)

@@ -1,6 +1,6 @@
 // msckf_mono_b200/asl/asl_player.cpp
 // ROS-free ASL / EuRoC player + trajectory evaluator (SURVEY.md 8f-3): drives msckf_mono::MSCKF<_S> -- the drop-in shim
-// over the B200 engine -- with the call order of the reference's dataset front end
+// over the H100 engine -- with the call order of the reference's dataset front end
 // (/root/reference/datasets/asl_msckf.cpp:206-296: per IMU reading propagate(); per image augmentState, update,
 // addFeatures, marginalize, pruneRedundantStates, pruneEmptyStates), from a mav0 folder with PRE-EXTRACTED feature tracks
 // (cam0/tracks.csv; the FAST/KLT image front end is out of scope, SURVEY.md 8f-4).  Deliberately NOT copied: the

@@ -240,6 +240,13 @@ class Engine:
     def num_clones(self):
         return lib().msckf_b200_num_clones(self.h)
 
+    def state(self):
+        """(imu [29]: p, v, b_g, b_a, g, q_IG, p_null, v_null, q_null; clone poses [M, 7]: p, q), dtype scalars"""
+        imu = np.zeros(29, dtype=self.dtype)
+        poses = np.zeros((self.num_clones(), 7), dtype=self.dtype)
+        check(lib().msckf_b200_get_state(self.h, imu.ctypes.data_as(C.c_void_p), poses.ctypes.data_as(C.c_void_p)), "msckf_b200_get_state")
+        return imu, poses
+
     def covariance(self):
         n = 15 + 6 * self.num_clones()
         out = np.zeros((n, n), dtype=self.dtype)

@@ -1,4 +1,4 @@
-// msckf_mono_b200/csrc/common.cuh -- device helpers shared by all kernels (sm_100a).
+// msckf_mono_b200/csrc/common.cuh -- device helpers shared by all kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

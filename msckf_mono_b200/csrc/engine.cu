@@ -1,4 +1,4 @@
-// msckf_mono_b200/csrc/engine.cu -- host side of the B200 engine and the C-ABI of include/msckf_b200.h.
+// msckf_mono_b200/csrc/engine.cu -- host side of the H100 engine and the C-ABI of include/msckf_b200.h.
 // One handle = one filter: device-resident covariance / clone poses / IMU state and workspaces.  Updates run through a
 // launch context (Ctx): one stream, one packed pinned + device input arena ([UpdArgs per filter | track batches]), one packed
 // report arena, a small cache of captured CUDA graphs.  Every engine has a private context; a msckf_b200_batch is a context
@@ -36,9 +36,9 @@ int fail(int code, const std::string& msg) { g_err = msg; return code; }
 #define RC(call) do { int rc_ = (call); if (rc_ != 0) return rc_; } while (0)
 
 constexpr int kMaxSplit = 16;
-constexpr int kJacBatchGroup = 32;  // k_jac threads per track in a device batch (profiles/r02_*)
+constexpr int kJacBatchGroup = 32;  // k_jac threads per track in a device batch (DESIGN.md 4.2)
 constexpr int kTailCluster = 8;  // portable cluster size: the serial EKF tail runs on 8 SMs of one GPC
-constexpr size_t kSmemBudget = 220 * 1024;
+constexpr size_t kSmemBudget = 220 * 1024;  // dynamic shared memory per CTA, under H100's 227 KB opt-in limit
 constexpr int kMaxClonesHard = mb::kMaxKeep;  // the keep list of prune() travels as a kernel argument
 constexpr int kMaxGraphs = 8;
 
@@ -48,6 +48,14 @@ static const double kChi2_005[99] = {
 
 inline size_t up16(size_t x) { return (x + 15) & ~(size_t)15; }
 inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// SMs of a device (cached per ordinal): caps the grids of the grid-stride element-wise kernels at a few CTAs per SM
+inline int num_sms(int dev) {
+  static int n[64] = {};
+  if (dev < 0 || dev >= 64) return 132;
+  if (n[dev] == 0 && cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n[dev] = 132;
+  return n[dev];
+}
 
 // pinned host + device buffer pair that grows on demand
 struct Arena {
@@ -606,7 +614,7 @@ struct Engine : EngineBase {
     if (kchunk < mb::GK) kchunk = mb::GK;
     nsplit = std::max(1, (a.K + kchunk - 1) / kchunk);
     a.nsplit = nsplit; a.kchunk = kchunk;
-    // FP64 tensor-core Gram products where they win (measured, profiles/r02_dmma.md): >= 200 tracks.  The choice depends on the
+    // FP64 tensor-core Gram products where they win (measured, DESIGN.md 4.4): >= 200 tracks.  The choice depends on the
     // filter's own batch only, never on how many filters share a launch: a device batch stays bit-identical to separate calls.
     a.gram_mma = (gram_mma && p.N >= 200) ? 1 : 0;
     a.tail_kind = pick_tail(a.n, no_fused_tail);
@@ -645,7 +653,7 @@ struct Engine : EngineBase {
     kl.n = n_keep;
     for (int i = 0; i < n_keep; ++i) kl.idx[i] = keep[i];
     const int n_new = 15 + 6 * n_keep;
-    mb::k_gather<S><<<std::min(296, (n_new * n_new + 255) / 256), 256, 0, stream>>>(n_new, kl, d_P, d_P2, ldp, d_poses, d_poses2);
+    mb::k_gather<S><<<std::min(2 * num_sms(device), (n_new * n_new + 255) / 256), 256, 0, stream>>>(n_new, kl, d_P, d_P2, ldp, d_poses, d_poses2);
     launches++;
     CK(cudaGetLastError());
     std::swap(d_P, d_P2);      // (buffer addresses ride in UpdArgs, not in captured kernel arguments:
@@ -838,10 +846,9 @@ int Ctx<S>::stage(int mode, const msckf_b200_tracks* tracks, int threads) {
     Lmax[i] = lm;
     return 0;
   };
-  // Staging threads: `threads` is an upper bound.  Measured on the 2 x 32-core host of the B200 box (scripts/e2e_breakdown.py):
-  // spreading the pack over 4 threads saves 13 us of 58 at 8 config-B filters (150 of 300 at 32) and then costs 100 (400) us
-  // more until the results are back -- the copy engine reads lines left dirty in several cores' caches -- so a batch
-  // only gets a second thread from 8 MB of observations on.
+  // Staging threads: `threads` is an upper bound.  Spreading the pack over several threads shortens the pack itself but
+  // lengthens the time until the results are back -- the copy engine reads lines left dirty in several cores' caches -- so
+  // a batch only gets a second thread from 8 MB of observations on (scripts/e2e_breakdown.py measures both parts).
   size_t in_bytes_est = 0;
   for (int i = 0; i < nf; ++i)
     if (tracks[i].n_tracks > 0 && tracks[i].obs_offset) in_bytes_est += (size_t)tracks[i].obs_offset[tracks[i].n_tracks] * (2 * sizeof(S) + sizeof(int));
@@ -926,7 +933,7 @@ int Ctx<S>::launch() {
   sh.tri_gx = (Nr + 3) / 4; sh.jac_gx = Nr / (sh.jac_g == 128 ? 1 : 2); sh.rows_gx = Nr; sh.bd_gx = Mmax_;
   const int c = nmax_ - mb::kImuDim, ntile = (c + mb::GT - 1) / mb::GT;
   sh.gram_gx = ntile * (ntile + 1) / 2; sh.gram_gy = nsplit;
-  sh.asm_gx = std::min(592, (nmax_ * nmax_ + 255) / 256);
+  sh.asm_gx = std::min(4 * num_sms(device), (nmax_ * nmax_ + 255) / 256);
   sh.rows_smem = (unsigned)(sizeof(double) * mb::rows_smem_doubles((Lm + 7) & ~7));
   sh.gemm_g = (nmax_ + 31) / 32;
   sh.syrk_gx = sh.gemm_g * (sh.gemm_g + 1) / 2;
@@ -1150,7 +1157,7 @@ int msckf_b200_create(const msckf_b200_config* cfg, msckf_b200_engine** out) {
   if (!cfg || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-    return fail(MSCKF_B200_ERR_NO_DEVICE, "no CUDA device: the B200 engine has no CPU fallback");
+    return fail(MSCKF_B200_ERR_NO_DEVICE, "no CUDA device: the engine has no CPU fallback");
   if (cfg->device < 0 || cfg->device >= ndev) return fail(MSCKF_B200_ERR_ARG, "bad device ordinal");
   if (cfg->max_clones < 1 || cfg->max_tracks < 1 || cfg->max_obs < 1) return fail(MSCKF_B200_ERR_ARG, "bad capacities");
   if (cfg->max_clones > kMaxClonesHard) return fail(MSCKF_B200_ERR_CAPACITY, "max_clones above the engine's hard limit");

@@ -332,7 +332,7 @@ __device__ __forceinline__ void ld4(const double* p, double (&v)[4]) {
 // right-hand side: its 8 entries are final components of y);  (3) the solved panel goes to shared memory TRANSPOSED
 // ([8][Rp]: neighbouring threads touch neighbouring words), one barrier;  (4) trailing update in 4 x 4 register tiles over
 // the lower triangle, one barrier.  57 pivots cost 8 panels x 2 barriers instead of 57 dependent warp-wide steps
-// (round 1: one warp, shuffle + shared-memory round trip per pivot, ~350 ns each = 20 us of k_jac's 55).
+// (round 1: one warp, shuffle + shared-memory round trip per pivot: over a third of k_jac).
 constexpr int kPW = 8;
 template <class S, int G>
 __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restrict__ r, int L2, S* __restrict__ PnT, int Rp, int* s_fail, int grp) {
@@ -456,7 +456,7 @@ __host__ __device__ inline size_t jac_smem_bytes(int L, int M, int g) {
 }
 
 // Ordered stacking (msckf.h:433-445): the exclusive prefix sum of the accepted blocks' row counts, computed by whichever
-// CTA of k_jac finishes last (ticket counter) -- a separate 1-CTA kernel for 300 integers cost 8 us of launch latency.
+// CTA of k_jac finishes last (ticket counter) -- a separate 1-CTA kernel for 300 integers cost a launch latency.
 template <class S, int CT>
 __device__ __forceinline__ void jac_finish(const UpdArgs<S>& a, int n_cta /* CTAs of this filter that arrive here */) {
   __shared__ int s_last;

@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(256) k_gram(const UpdArgs<S>* __restrict__ arg
   const int bc = threadIdx.x & 31, bg = threadIdx.x >> 5;
   double bz = 0.0;
   // operands of the next k-slab are fetched into registers while the current one is multiplied (the slabs are L2 hits of
-  // ~1 us latency; without the prefetch the kernel sat in long-scoreboard stalls: ncu, profiles/)
+  // microsecond latency; without the prefetch the kernel sat in long-scoreboard stalls: ncu)
   constexpr int NF = GK * GT / 256;
   double fza[NF], fya[NF], fzb[NF], fyb[NF], fu = 0.0;
   auto fetch = [&](int kb) {

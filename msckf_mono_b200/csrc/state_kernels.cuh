@@ -302,7 +302,7 @@ __global__ void __launch_bounds__(256) k_propagate(const PropBatch<S> pb) {
   // multiply-subtract), arranged for a SHORT instruction stream -- this kernel's body is ~90 KB of SASS and whatever runs once
   // per reading is fetched cold: the pivot is a warp arg-max (5 shuffle steps), lane = ROW for the elimination (one division
   // per lane, a rolled loop along the row; stride 15 words: conflict-free), lane = column for the row swap and the back
-  // substitution (rolled).  (Measured: unrolled per-column register forms of this were slower, 26 vs 21 us per reading.)
+  // substitution (rolled).  (Measured: unrolled per-column register forms of this were slower.)
   if (t < 32) {
     S* Mx = (t < 15) ? Tm : Phi;
     const int j = (t < 15) ? t : ((t < 30) ? t - 15 : 0);

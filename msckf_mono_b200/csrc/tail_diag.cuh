@@ -2,16 +2,16 @@
 //
 // Round 1 factorised a diagonal block with one warp per matrix, a shuffle + shared-memory round trip per pivot and a second
 // pair of warps building the inverses one pivot behind (the S'' warp polling Gamma's keep / drop decision through a
-// volatile flag): ~540 ns per pivot, 17 us per block, half of the kernel.  Measurements that shaped this version
-// (%globaltimer stamps inside the functions, profiles/r02_tail_stamps.md):
+// volatile flag): per-pivot communication made it half of the kernel.  What shaped this version (%globaltimer stamps
+// inside the functions, scripts/tail_profile.py):
 //   * per-pivot communication is what costs: the block is itself blocked by panels, the diagonal micro-block of a panel is
 //     factorised REDUNDANTLY in registers by every thread of the warps that need it -- static indices, right-looking, so the
-//     dependent chain of a pivot is rsqrt -> multiply -> one FMA (80 cycles, scripts/fp64_latency.cu) -- and the keep / drop
+//     dependent chain of a pivot is rsqrt -> multiply -> one FMA (scripts/fp64_latency.cu measures it) -- and the keep / drop
 //     decision of each pivot (Gamma's pivot against thr x its original diagonal, the rank cap; S'' follows) is evaluated by
 //     every thread from the same numbers; two CTA barriers per panel;
-//   * code that runs once per call is bound by instruction fetch (~5-7 cycles per instruction once the body exceeds the
-//     L1.5 instruction cache; a first version with a fully unrolled 32-step inverse was 3 157 instructions and took 21 us per
-//     block): every loop here is rolled except the micro-block itself;
+//   * code that runs once per call is bound by instruction fetch once the body exceeds the instruction caches (a first
+//     version with a fully unrolled 32-step inverse was ~3 200 instructions and slower than the rolled code): every loop
+//     here is rolled except the micro-block itself;
 //   * the inverses of the factors ride along the panels as 32 extra rows (rows of the identity, solved like panel rows):
 //     no separate inverse stage.  Only the inverses leave the block -- the panels below it are X = rows x Linv^T.
 // Two entry points: tf_factor_block (Gamma and S'' together on one CTA, 4-column panels: the 8-CTA cluster form) and
@@ -20,7 +20,7 @@
 #include "common.cuh"
 
 #ifndef MSCKF_TF_PW
-#define MSCKF_TF_PW 8  // panel width of tf_factor_one (4 or 8; 8: four panels per block, 10.5 instead of 13.4 us per block)
+#define MSCKF_TF_PW 8  // panel width of tf_factor_one (4 or 8; 8: four panels per block, half the barriers of 4)
 #endif
 
 namespace mb {
@@ -58,7 +58,7 @@ __device__ __noinline__ TfRank tf_factor_block(double* __restrict__ DG, double* 
   // does to the rows below the block (micro-solve against the diagonal micro-block, then the trailing update), and
   // Y = L^-T, i.e. extra row i, column j holds Linv[j][i] -- stored transposed, straight into LIA / LIG.  Row i of the identity
   // is zero left of column i, so it only joins from the panel that contains column i.  This replaces a separate inverse
-  // stage (6 us and 7 CTA barriers per block in the first version of this file).
+  // stage (7 CTA barriers per block in the first version of this file).
   for (int e = tid; e < kFB * LD; e += nthreads) {
     const int k = e / LD, c = e % LD;
     LIA[e] = (k == c) ? 1.0 : 0.0;

@@ -9,14 +9,14 @@
 // chain of diagonal blocks, CTA 1 Gamma's, CTAs 2..8 are the workers; k_tail_fused<S, 1> -- a cluster of 8: CTA 0 runs both
 // chains (tf_factor_block), CTAs 1..7 are the workers.
 //
-// What bounds this kernel is latency, not the FP64 pipe (64 lane-FMA/clk/SM measured, scripts/fp64_rate.cu): a chain of
-// n dependent pivots at 80 cycles each (scripts/fp64_latency.cu) plus what surrounds them, and instruction fetch -- the kernel
-// is ~100 KB of SASS, the L1.5 instruction cache holds 32 KB, so every phase of every block iteration starts cold.
-// Measured (ncu source view, %globaltimer stamps, profiles/r02_tail_stamps.md) and acted upon:
+// What bounds this kernel is latency, not the FP64 pipe (scripts/fp64_rate.cu measures its rate): a chain of n dependent
+// pivots (scripts/fp64_latency.cu measures one step) plus what surrounds them, and instruction fetch -- the kernel is
+// ~100 KB of SASS, far more than the instruction caches hold, so every phase of every block iteration starts cold.
+// Measured (ncu source view, %globaltimer stamps: scripts/tail_profile.py) and acted upon:
 //   * the diagonal block (tail_diag.cuh): blocked by panels (8 columns in the two-chain form, 4 in the one-chain form), the
 //     diagonal micro-block factorised redundantly in registers by the threads that solve the panel rows, keep / drop decisions
 //     evaluated by all of them from the same numbers; the inverses ride along as 32 extra rows; loops rolled except the
-//     micro-block (a fully unrolled 32-step-inverse version was fetch-bound: 21 us per block against 8 now);
+//     micro-block (a fully unrolled 32-step-inverse version was fetch-bound);
 //   * the two chains only meet in the keep / drop flags: one 32-bit word per panel through DSMEM, S'' speculates "nothing
 //     dropped" and repeats a micro-block only when Gamma did drop (tf_factor_one);
 //   * the chain CTAs run ONE BLOCK AHEAD of the workers: they solve the 32 panel rows of the next diagonal block themselves
@@ -24,8 +24,8 @@
 //     run the trailing update (split cluster barrier: arrive early, wait late; published inverses double-buffered);
 //   * the panel below a diagonal block is X = A_panel L_kk^-T: with L_kk^-1 at hand a small GEMM shared by all 8 warps
 //     instead of a 32-step substitution per row; panel rows are dealt to the workers (no redundant solves) and exchanged
-//     through L2 (a scratch panel every worker reads back after the cluster barrier: ~64 B/clk per SM, against ~20 B/clk
-//     for pushing it into 8 shared memories through DSMEM);
+//     through L2 (a scratch panel every worker reads back after the cluster barrier: faster than pushing it into 8 shared
+//     memories through DSMEM);
 //   * shared-memory bank conflicts: tiles are dealt so that the lanes of a warp read neighbouring columns.
 // Two cluster barriers (release/acquire at cluster scope) per block order the phases.
 #pragma once
@@ -157,7 +157,7 @@ __global__ void __launch_bounds__(kTailThreads) k_tail_fused(const UpdArgs<S>* _
   if (tid < NB / 4) s_words[tid] = 0u;
   if (tid == 0) s_timeout = 0;
   // split barrier: the chain CTAs only wait for everybody's part of the Gamma patch, not for the workers' staging of the
-  // right-hand sides (7 us of strided loads that nobody needs before the first panel)
+  // right-hand sides (strided loads that nobody needs before the first panel)
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   if (crank >= NCH) {
     for (int e = tid; e < NB * n; e += kTailThreads) {  // consecutive threads -> consecutive k: conflict-free stores

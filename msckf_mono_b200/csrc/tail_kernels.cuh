@@ -13,7 +13,7 @@ namespace mb {
 // deterministic).  Operands stream through shared memory with the next slab prefetched into registers while the
 // current one is multiplied: at n <= 639 these products are bound by the latency of a slab (L2 round trip + a chain of
 // FMAs issued by one warp per sub-partition), not by the fp64 pipe, so shortening the chain per warp is what matters
-// (measured at config B: 27 us with 64 threads, 18 us with 128, see profiles/).
+// (at config B 128 threads per tile were faster than 64).
 // LA(k, a) / LB(k, b) fetch operand elements, EPI(a, b, acc) stores.
 constexpr int kGemmThreads = 256;
 constexpr int kGemmSmemDoubles = 2 * 1024 + (kGemmThreads / 64 - 1) * 1024;  // two operand slabs + the partial sums of three k-groups
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(kGemmThreads) k_gemm_s(const UpdArgs<S>* __res
 // P <- P - W^T W (lower-triangular tile pairs; written in the filter precision, exactly symmetric by construction), and in
 // the same launch  dx = W^T y  (the CTAs of the first tile column each take 32 components) followed by the state injection of
 // msckf.h:1373-1391 by whichever CTA finishes last (ticket counter) -- round 1 ran both as a separate single-CTA kernel
-// (k_inject: 20 us for a 195 x 195 mat-vec).
+// (k_inject: a whole launch for a 195 x 195 mat-vec).
 template <class S>
 __global__ void __launch_bounds__(kGemmThreads) k_syrk(const UpdArgs<S>* __restrict__ args) {
   pdl_wait();

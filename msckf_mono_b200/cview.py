@@ -1,6 +1,6 @@
 """ctypes binding of the "C view of msckf_mono::MSCKF<_S>" (include/msckf_mono_c.h).
 
-The same function set is exported by the B200 engine (libmsckf_b200.so, prefix
+The same function set is exported by the H100 engine (libmsckf_b200.so, prefix
 ``msckf_mono_``) and -- for tests and the CPU baseline only -- by the oracle
 (oracle/libmsckf_oracle.so, prefix ``msckf_oracle_``); this class is prefix-agnostic so the
 parity tests drive both through identical calls.  All scalars cross the boundary as double.

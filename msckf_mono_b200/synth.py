@@ -4,7 +4,7 @@ Nothing here is on the product path: it only manufactures inputs (IMU samples an
 normalised-coordinate feature tracks with ids) with the shape the reference front-ends
 deliver (datasets/asl_msckf.cpp:233-294: propagate per IMU sample, then per image
 augmentState / update / addFeatures / marginalize / prune*), so that the oracle and the
-B200 engine can be driven through the same MSCKF<_S> surface on identical inputs.
+H100 engine can be driven through the same MSCKF<_S> surface on identical inputs.
 
 Calibration and noise parameters are the *effective* EuRoC values of SURVEY.md section 5
 (euroc/MH_03_kalibr.yaml:6-13, launch/asl_msckf.launch:15-35, datasets/asl_msckf.cpp:73-134).

@@ -1,6 +1,6 @@
 // Micro-benchmark: DEPENDENT-chain latencies that bound the tail kernel's diagonal blocks (one warp, clock64()):
 // DFMA -> DFMA, the 1/sqrt sequence of tail_diag.cuh (MUFU.RSQ64H + two Newton steps), shared-memory load -> use, CTA barrier.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/fp64_latency.bin scripts/fp64_latency.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/fp64_latency.bin scripts/fp64_latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

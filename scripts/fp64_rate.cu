@@ -1,6 +1,6 @@
 // Micro-benchmark: issue rate of FP64 FMA (and FP32 FMA for comparison) per SM sub-partition on the GPU at hand.
 // One CTA, W warps, each lane runs 8 independent FMA chains; cycles from clock64() on warp 0.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/fp64_rate.bin scripts/fp64_rate.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/fp64_rate.bin scripts/fp64_rate.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -47,8 +47,8 @@ int main() {
   printf("%s, %d SMs, clock %d kHz\n", p.name, p.multiProcessorCount, p.clockRate);
   for (int w : {1, 2, 4, 8, 16}) run<double>("fp64", w, 32, 1);
   for (int l : {1, 4, 8, 16}) run<double>("fp64", 4, l, 1);
-  run<double>("fp64", 8, 32, 148);
-  run<double>("fp64", 8, 32, 296);
+  run<double>("fp64", 8, 32, p.multiProcessorCount);
+  run<double>("fp64", 8, 32, 2 * p.multiProcessorCount);
   for (int w : {1, 4, 8, 16}) run<float>("fp32", w, 32, 1);
   return 0;
 }

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""scripts/measure_parity.py -- runs every parity case of tests/parity_cases.py on the GPU box and writes the measured
+"""scripts/measure_parity.py -- runs every parity case of tests/parity_cases.py on the GPU and writes the measured
 numbers as JSON (stdout).  The committed copy, tests/golden/parity_measured.json, is what the GPU tests assert against
 (value <= 10 x measurement) and what DESIGN.md section 5 quotes.  Test infrastructure: engine vs CPU oracle.
 
-    python scripts/measure_parity.py [case ...] > gpurun_out/parity_measured.json
+    python scripts/measure_parity.py [case ...] > tests/golden/parity_measured.json
 """
 import json
 import sys

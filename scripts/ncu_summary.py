@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """scripts/ncu_summary.py -- selected metrics of every kernel in an .ncu-rep (ncu --set full) as JSON, plus the DRAM bytes per
-launch that bench.py reports as `roofline.traffic`.  Usage: python scripts/ncu_summary.py REP.ncu-rep > profiles/rNN_ncu_top_kernels.json"""
+launch.  Usage: python scripts/ncu_summary.py REP.ncu-rep > top_kernels.json"""
 import csv
 import json
 import subprocess

@@ -1,10 +1,10 @@
 #!/bin/bash
-# scripts/sanitize.sh -- compute-sanitizer evidence (run on the GPU box): memcheck over ALL GPU tests, racecheck over a subset
+# scripts/sanitize.sh -- compute-sanitizer evidence (needs a GPU and compute-sanitizer): memcheck over ALL GPU tests, racecheck over a subset
 # that reaches every kernel: small and config-B windows (k_tri, k_jac with the blocked gate Cholesky, Gram kernels,
 # the fused cluster tail with the ticket counters of k_jac / k_syrk), the large-window tail (L = 98), the device batch,
-# the streaming path (propagate_n / augment / gather).  Logs go to gpurun_out/; summaries are committed under profiles/.
+# the streaming path (propagate_n / augment / gather).  Logs go to the directory given as the first argument.
 set -u
-OUT=${1:-gpurun_out}
+OUT=${1:?usage: scripts/sanitize.sh OUT_DIR}
 timeout 1500 compute-sanitizer --tool memcheck --leak-check no --error-exitcode 9 --log-file $OUT/r02_memcheck.log \
   python -m pytest tests/test_engine_gpu.py tests/test_asl_gpu.py -m gpu -q -x > $OUT/r02_memcheck_pytest.log 2>&1
 echo "memcheck exit $?" >> $OUT/r02_memcheck_pytest.log

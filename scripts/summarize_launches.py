@@ -1,6 +1,6 @@
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list into per-kernel means and shares.
 
-usage: python scripts/summarize_launches.py gpurun_out/launches.csv > profiles/r01_launch_shares.json
+usage: python scripts/summarize_launches.py launches.csv > launch_shares.json
 The bench command under ncu runs the update several times (warm-up + timed steps); every kernel of the update appears
 once per step, so mean duration per kernel name x launches per step = the step's kernel time."""
 import csv

@@ -1,6 +1,6 @@
 // Stand-alone check of tf_factor_one (tail_diag.cuh) for a panel width given by -DMSCKF_TF_PW: a cluster of two CTAs
 // factorises a 32 x 32 pair (CTA 0: A following CTA 1's flags for G, G rank-deficient), compared with a host reference.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -DMSCKF_TF_PW=8 -I msckf_mono_b200/csrc -o scripts/tf_one_check8.bin scripts/tf_one_check.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DMSCKF_TF_PW=8 -I msckf_mono_b200/csrc -o scripts/tf_one_check8.bin scripts/tf_one_check.cu
 #include <cooperative_groups.h>
 #include <cmath>
 #include <cstdio>

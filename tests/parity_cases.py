@@ -1,6 +1,6 @@
 """Parity cases shared by the GPU tests and by scripts/measure_parity.py.
 
-Each case drives the B200 engine and the CPU oracle (or a committed oracle fixture) on the same seeded inputs, asserts what
+Each case drives the H100 engine and the CPU oracle (or a committed oracle fixture) on the same seeded inputs, asserts what
 must be bit-exact (flags, ids, counters) and RETURNS the floating-point differences as a dict of numbers.
 scripts/measure_parity.py runs every case on the GPU box and writes the numbers to tests/golden/parity_measured.json;
 the tests assert `value <= 10 x the committed measurement` (tests/parity_cases.py::check), so every asserted bound is a

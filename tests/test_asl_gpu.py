@@ -1,4 +1,4 @@
-"""The ROS-free ASL player (C++ host over the drop-in class shim, `msckf_mono_b200/asl/asl_player.cpp`) on a B200:
+"""The ROS-free ASL player (C++ host over the drop-in class shim, `msckf_mono_b200/asl/asl_player.cpp`) on an H100:
 the same on-disk sequence is played by the compiled player through `msckf_mono::MSCKF<_S>` and, for the check, by the
 CPU oracle driven from Python with the reference's call order.  Bar (BASELINE north star): trajectories agree to
 < 1e-4 m RMS; the clone-window size per frame (pruning bookkeeping) is identical."""

@@ -1,11 +1,11 @@
-"""GPU parity tests: the B200 engine behind the MSCKF<_S> surface (through the C view / C-ABI of
+"""GPU parity tests: the H100 engine behind the MSCKF<_S> surface (through the C view / C-ABI of
 libmsckf_b200.so) against the CPU oracle on identical seeded inputs.
 
 What is asserted:
   * integer bookkeeping (valid / accepted flags = zero accept/reject flips, clone ids, tracked ids, counters): bit-exact,
     inside every case (tests/parity_cases.py);
   * every floating-point difference against 10 x its committed measurement (tests/golden/parity_measured.json, written by
-    scripts/measure_parity.py on the B200): no hand-picked loose bounds -- a regression of more than one decade fails;
+    scripts/measure_parity.py on the H100): no hand-picked loose bounds -- a regression of more than one decade fails;
   * on top of that the contract tolerances of SURVEY.md 8d where the path meets them: fp64 vs the oracle's implementation-
     independent part (exact-subspace mode) <= 1e-9 relative on small windows; trajectory RMS < 1e-4 m.
 The oracle modes: `clean` = exact subspace (drop_null_rows), `faithful` = reference-literal compression (its rows from
@@ -294,6 +294,40 @@ def test_persistent_batch_over_a_stream_is_bit_identical():
     fb.close()
     # after the batch is gone the filters run on their own streams again
     grp[0].marginalize()
+
+
+@pytest.mark.parametrize("dtype", [np.float32, np.float64])
+def test_bench_dump_is_what_the_class_getters_return(tmp_path, dtype):
+    """bench.py --dump-outputs reads the corrected state through capi.Engine.state() / covariance() / delta_x(); the
+    arrays must be the filters' own state as the drop-in class reports it, and past the size budget a seeded subset."""
+    import bench
+    from msckf_mono_b200 import capi
+    filts, engs, reps = [], [], []
+    for seq in (3, 4, 5):
+        f = make_engine(dtype, max_clones=20, max_tracks=64, max_obs=64 * 12)
+        synth.drive(f, synth.make_window_workload(n_features=40, n_clones=12, seq=seq))
+        c = f.counters()
+        filts.append(f)
+        engs.append(capi.Engine(dtype, borrowed=f.engineHandle()))
+        reps.append({"accepted": f.lastReport()["accepted"].copy(), "m": c["m"], "rank": c["rows_kept"]})
+    n = 15 + 6 * filts[0].getNumCamStates()
+    per_filter = 4 * (len(reps[0]["accepted"]) + 29 + 7 * filts[0].getNumCamStates() + n * n) + 8 * (2 + n)
+    for max_bytes, count in ((64 << 20, 3), (2 * per_filter, 2)):
+        out = tmp_path / str(count)
+        bench.dump_outputs(out, engs, reps, max_bytes=max_bytes)
+        d = {p.stem: np.load(p) for p in out.glob("*.npy")}
+        idx = d["filter_index"].astype(int)
+        assert len(idx) == count and len(set(idx)) == count
+        assert sum(a.nbytes for k, a in d.items() if k != "filter_index") <= max_bytes
+        for row, i in enumerate(idx):
+            f, s, cs = filts[i], filts[i].getImuState(), filts[i].getCamStates()
+            imu = np.concatenate([s[k] for k in ("p_I_G", "v_I_G", "b_g", "b_a", "g", "q_IG", "p_I_G_null", "v_I_G_null", "q_IG_null")])
+            np.testing.assert_array_equal(d["imu_state"][row], imu.astype(dtype).astype(np.float32))
+            np.testing.assert_array_equal(d["clone_poses"][row], np.hstack([cs["p_C_G"], cs["q_CG"]]).astype(dtype).astype(np.float32))
+            np.testing.assert_array_equal(d["covariance"][row], f.getCovariance().astype(dtype).astype(np.float32))
+            np.testing.assert_array_equal(d["accepted"][row], reps[i]["accepted"])
+            np.testing.assert_array_equal(d["m_rank"][row], [reps[i]["m"], reps[i]["rank"]])
+            assert np.isfinite(d["delta_x"][row]).all() and d["delta_x"].shape[1] == n
 
 
 def test_window_growth_and_single_observation_tracks():
