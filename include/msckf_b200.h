@@ -137,6 +137,9 @@ int msckf_b200_batch_launch_timed(msckf_b200_batch* b, float* ms);
 /* per-kernel device times of the last batch launch (option key 1 of the FIRST engine set); returns the count */
 int msckf_b200_batch_kernel_times(msckf_b200_batch* b, float* ms, const char** names, int cap);
 long long msckf_b200_batch_launch_count(const msckf_b200_batch* b);
+/* CTAs of the feature kernel (k_jac) resident per SM at the shape of the batch's last launch: the CUDA occupancy calculator's
+ * figure for its threads per track and dynamic shared memory (0 before the first launch) */
+int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b);
 void* msckf_b200_batch_stream(msckf_b200_batch* b);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */

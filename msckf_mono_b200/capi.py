@@ -136,6 +136,10 @@ class Batch:
     def launch_count(self):
         return int(lib().msckf_b200_batch_launch_count(self.h))
 
+    def jac_occupancy(self):
+        """CTAs of k_jac resident per SM at the shape of the last launch (0 before the first)."""
+        return int(lib().msckf_b200_batch_jac_occupancy(self.h))
+
 
 def update_batch(engines, mode, batches, threads=8):
     """msckf_b200_update_batch: one update per engine (independent filters), host work on `threads` threads.

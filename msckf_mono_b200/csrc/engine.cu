@@ -118,6 +118,9 @@ struct CtxBase {
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
+  // k_jac at the last launch's shape: threads per track, dynamic shared memory, CTAs resident per SM (msckf_b200_batch_jac_occupancy)
+  int jac_g = 0, jac_ctas = 0;
+  unsigned jac_smem = 0;
 };
 
 struct EngineBase {
@@ -379,6 +382,13 @@ struct Engine : EngineBase {
   void drop_graphs() override { solo.drop_graphs(); if (group) static_cast<Ctx<S>*>(group)->drop_graphs(); }
 
   static int& tail9_clusters() { static int v = 0; return v; }  // co-resident clusters of 9 (0: not available)
+  // CTAs of k_jac with g threads per track resident per SM at `smem` bytes of dynamic shared memory (0: not available)
+  static int jac_ctas_per_sm(int g, unsigned smem) {
+    auto kj = g == 32 ? mb::k_jac<S, 32> : (g == 64 ? mb::k_jac<S, 64> : mb::k_jac<S, 128>);
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kj, g == 32 ? 64 : 128, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return n;
+  }
   static int set_func_attrs(int dev) {
     static bool done[64] = {};  // (per scalar type and device: function attributes belong to the device's context)
     if (dev < 0 || dev >= 64) return fail(MSCKF_B200_ERR_ARG, "device index");
@@ -387,6 +397,10 @@ struct Engine : EngineBase {
     CK(cudaFuncSetAttribute(mb::k_jac<S, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     CK(cudaFuncSetAttribute(mb::k_jac<S, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     CK(cudaFuncSetAttribute(mb::k_jac<S, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+    // k_jac's occupancy is set by shared memory: ask for the largest carveout, not just enough for one CTA
+    CK(cudaFuncSetAttribute(mb::k_jac<S, 128>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    CK(cudaFuncSetAttribute(mb::k_jac<S, 64>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    CK(cudaFuncSetAttribute(mb::k_jac<S, 32>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     CK(cudaFuncSetAttribute(mb::k_tail_fused<S, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     CK(cudaFuncSetAttribute(mb::k_tail_fused<S, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     // the two-chain form runs in clusters of 9 (2 chain CTAs + 7 workers): a non-portable size; use it where the device takes it
@@ -927,9 +941,14 @@ int Ctx<S>::launch() {
   if (sh.tri_smem > kSmemBudget) return fail(MSCKF_B200_ERR_CAPACITY, "k_tri shared memory");
   if (mode != MSCKF_B200_TRIANGULATE && sh.jac_smem > kSmemBudget) return fail(MSCKF_B200_ERR_CAPACITY, "k_jac shared memory");
   const int Nr = (Nmax + 15) & ~15;  // rounded track count: kernels exit on blockIdx >= their filter's own N
-  sh.tri_smem = (sh.tri_smem + 1023) & ~1023u; sh.jac_smem = (sh.jac_smem + 1023) & ~1023u;
+  // (k_jac's at the SM's allocation granularity of 128 B: a whole KB would cost a batch of 8 config-B filters its tenth CTA per SM)
+  sh.tri_smem = (sh.tri_smem + 1023) & ~1023u; sh.jac_smem = (sh.jac_smem + 127) & ~127u;
   if (sh.tri_smem > kSmemBudget) sh.tri_smem = (unsigned)kSmemBudget;
   if (sh.jac_smem > kSmemBudget) sh.jac_smem = (unsigned)kSmemBudget;
+  if (mode != MSCKF_B200_TRIANGULATE && (sh.jac_g != jac_g || sh.jac_smem != jac_smem)) {
+    jac_g = sh.jac_g; jac_smem = sh.jac_smem;
+    jac_ctas = Engine<S>::jac_ctas_per_sm(jac_g, jac_smem);
+  }
   sh.tri_gx = (Nr + 3) / 4; sh.jac_gx = Nr / (sh.jac_g == 128 ? 1 : 2); sh.rows_gx = Nr; sh.bd_gx = Mmax_;
   const int c = nmax_ - mb::kImuDim, ntile = (c + mb::GT - 1) / mb::GT;
   sh.gram_gx = ntile * (ntile + 1) / 2; sh.gram_gy = nsplit;
@@ -1257,6 +1276,7 @@ int msckf_b200_batch_update(msckf_b200_batch* b, int mode, const msckf_b200_trac
 }
 int msckf_b200_batch_kernel_times(msckf_b200_batch* b, float* ms, const char** names, int cap) { return b->ctx->kernel_times(ms, names, cap); }
 long long msckf_b200_batch_launch_count(const msckf_b200_batch* b) { return b->ctx->launches; }
+int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b) { return b->ctx->jac_ctas; }
 void* msckf_b200_batch_stream(msckf_b200_batch* b) { return (void*)b->ctx->stream; }
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

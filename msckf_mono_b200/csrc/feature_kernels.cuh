@@ -256,7 +256,7 @@ constexpr int JT = 128;  // most threads a CTA of k_jac has (see JGrp)
 template <int G>
 struct JGrp {
   static_assert(G == 32 || G == 64 || G == 128, "group size");
-  // G = 32 runs in CTAs of 64 threads (two tracks): the finer the CTA, the more tracks fit the SM's shared memory (18 at L = 30)
+  // G = 32 runs in CTAs of 64 threads (two tracks): the finer the CTA, the more tracks fit the SM's shared memory (20 at L = 30)
   static constexpr int CT = (G == 32) ? 64 : 128, NW = G / 32, TPC = CT / G;
   __device__ static __forceinline__ void sync(int grp) {
     if (G == CT) __syncthreads();
@@ -289,6 +289,16 @@ template <int G, int K, class T, class F>
 __device__ __forceinline__ void group_vsum(T (&out)[K], F part, T* red, int grp) {
   constexpr int NW = JGrp<G>::NW, R = 4 / NW;
   const int lane = threadIdx.x & 31, gw = (threadIdx.x % G) >> 5;
+  if (G == 32) {  // one warp plays all four virtual warps: ((s0 + s1) + s2) + s3 folded as they come (4 x K fewer live registers)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      T p[K];
+      part(32 * q + lane, p);
+#pragma unroll
+      for (int k = 0; k < K; ++k) { const T s = warp_sum(p[k]); out[k] = (q == 0) ? s : out[k] + s; }
+    }
+    return;
+  }
   T s[R][K];
 #pragma unroll
   for (int q = 0; q < R; ++q) {
@@ -296,11 +306,6 @@ __device__ __forceinline__ void group_vsum(T (&out)[K], F part, T* red, int grp)
     part(32 * (gw + NW * q) + lane, p);
 #pragma unroll
     for (int k = 0; k < K; ++k) s[q][k] = warp_sum(p[k]);
-  }
-  if (G == 32) {
-#pragma unroll
-    for (int k = 0; k < K; ++k) out[k] = ((s[0][k] + s[R > 1 ? 1 : 0][k]) + s[R > 2 ? 2 : 0][k]) + s[R > 3 ? 3 : 0][k];
-    return;
   }
   JGrp<G>::sync(grp);
   if (lane == 0) {
@@ -436,23 +441,39 @@ __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restri
 }
 
 // shared memory of one track's group (rounded to 16 bytes), in units of S:
-//   X 12L | r 2L | V 6L | WF 12L (+ slack) | Ypacked L(2L+1)
-// with two aliases: U (fp64 [2L][3], the first 3 columns of the feature's Q) lives at the start of WF until the compact
-// outputs are written (before the two-sided transform fills W and F), and the gate Cholesky's transposed panel PnT
-// (8 x Rp, Rp = (2L + 1) & ~3, 16-byte aligned) lives on V | WF once the transform is done.
+//   r 2L | X 12L | V 6L (+ slack) | Ypacked L(2L+1)
+// with two aliases: W | F of the two-sided transform ([2L][3] each) take X's place once the compact outputs are written,
+// and the gate Cholesky's transposed panel PnT (8 x Rp, Rp = (2L + 1) & ~3, 16-byte aligned) lives on X | V once the
+// transform is done.  U (the first 3 columns of the feature's Q, fp64) is never stored: its rows are rebuilt from V where
+// they are needed (u_row).
 template <class S>
-__host__ __device__ inline size_t jac_vwf_elems(int L) { return (size_t)(18 * L > 16 * L + 12 ? 18 * L : 16 * L + 12); }
+__host__ __device__ inline size_t jac_xv_elems(int L) { return (size_t)(18 * L > 16 * L + 12 ? 18 * L : 16 * L + 12); }
 template <class S>
 __host__ __device__ inline size_t jac_group_bytes(int L) {
-  const size_t b = sizeof(S) * ((size_t)14 * L + jac_vwf_elems<S>(L) + (size_t)L * (2 * L + 1));
+  const size_t b = sizeof(S) * ((size_t)2 * L + jac_xv_elems<S>(L) + (size_t)L * (2 * L + 1));
   return (b + 15) & ~(size_t)15;
 }
-// whole CTA: bar 16 | poses M*8 S (groups of 64 / 128 threads only: a single warp reads its few poses from global) | pad |
-// tpc groups (sized by the launch's longest track)
+// whole CTA: groups of 64 / 128 threads: bar 16 | poses M*8 S | pad 16 | the groups; a single warp reads its few poses from
+// global, so a CTA of G = 32 holds its two groups alone (sized by the launch's longest track)
 template <class S>
 __host__ __device__ inline size_t jac_smem_bytes(int L, int M, int g) {
   const int tpc = (g == 128) ? 1 : 2;
-  return 16 + (g == 32 ? 0 : sizeof(S) * kPoseStride * (size_t)M) + 16 + (size_t)tpc * jac_group_bytes<S>(L);
+  return (g == 32 ? 0 : 16 + sizeof(S) * kPoseStride * (size_t)M + 16) + (size_t)tpc * jac_group_bytes<S>(L);
+}
+
+// Row `row` of U = H0 H1 H2 [I3; 0] (fp64) after the reflectors H2 .. H_kmin have been applied to [I3; 0] in that order:
+// H_k changes rows >= k only, by  u -= sd_k v_k(row)  with  sd_k = tau64_k v_k^T U  (sd[3 k + q]).  The same operations in
+// the same order as applying them to a stored [2L][3] array, so the values are the same bits.
+template <class S>
+__device__ __forceinline__ void u_row(const S* __restrict__ V, const double* sd, int row, int kmin, double (&u)[3]) {
+#pragma unroll
+  for (int q = 0; q < 3; ++q) u[q] = (row == q) ? 1.0 : 0.0;
+#pragma unroll
+  for (int k = 2; k >= 0; --k) {
+    if (k < kmin || row < k) continue;
+    const double vk = (double)V[3 * row + k];
+    u[0] -= sd[3 * k] * vk; u[1] -= sd[3 * k + 1] * vk; u[2] -= sd[3 * k + 2] * vk;
+  }
 }
 
 // Ordered stacking (msckf.h:433-445): the exclusive prefix sum of the accepted blocks' row counts, computed by whichever
@@ -571,14 +592,13 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
     return;
   }
   // ------------------------------------------------------------------ shared-memory carve-up
-  S* X = reinterpret_cast<S*>(gmem_sm);
-  S* r = X + 12 * L;
-  S* V = r + L2;
-  S* wv = V + 3 * L2;   // [2L][3]  W = Y V
+  S* r = reinterpret_cast<S*>(gmem_sm);
+  S* X = r + L2;
+  S* V = X + 12 * L;
+  S* wv = X;            // [2L][3]  W = Y V     (X is dead by then)
   S* Fv = wv + 3 * L2;  // [2L][3]  F of the two-sided transform
-  double* U = reinterpret_cast<double*>(wv);  // [2L][3] fp64; dead before W is written
-  S* Y = V + jac_vwf_elems<S>(L);
-  S* PnT = reinterpret_cast<S*>((reinterpret_cast<uintptr_t>(V) + 15) & ~uintptr_t(15));  // [8][Rp]; V, W, F are dead by then
+  S* Y = X + jac_xv_elems<S>(L);
+  S* PnT = reinterpret_cast<S*>((reinterpret_cast<uintptr_t>(X) + 15) & ~uintptr_t(15));  // [8][Rp]; W, F, V are dead by then
   const int Rp = (L2 + 1) & ~3;  // >= rho + 1 = 2L - 2, multiple of 4
   const int* idx = a.clone_idx + o0;
   const S* z = a.obs + 2 * (size_t)o0;
@@ -642,9 +662,11 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   __shared__ S s_tau_[Gp::TPC][3];
   __shared__ S s_T_[Gp::TPC][9];
   __shared__ double s_urv_[Gp::TPC][3];
+  __shared__ double s_sd_[Gp::TPC][9];
   S* s_tau = s_tau_[grp];
   S* s_T = s_T_[grp];
   double* s_urv = s_urv_[grp];
+  double* s_sd = s_sd_[grp];
   const int warp = tid >> 5;
   if (warp == 0) {
     S tau[3];
@@ -723,30 +745,32 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
       for (int k = 0; k < 3; ++k) { vv3[k] = warp_sum_call(vv3[k]); tau64[k] = (tau[k] != S(0)) ? 2.0 / vv3[k] : 0.0; }
       vtv01 = warp_sum_call(vtv01); vtv02 = warp_sum_call(vtv02); vtv12 = warp_sum_call(vtv12);
     }
-    // ---- U = Q(:,0:3) = H0 H1 H2 [I3; 0]  (fp64)
-    _Pragma("unroll 1") for (int e = lane; e < 3 * L2; e += 32) U[e] = ((e / 3) == (e % 3)) ? 1.0 : 0.0;
-    __syncwarp();
+    // ---- U = Q(:,0:3) = H0 H1 H2 [I3; 0]  (fp64), kept as the nine coefficients sd_k of u_row
+    double sd[9];
 #pragma unroll
     for (int k = 2; k >= 0; --k) {
-      double sd[3] = {0.0, 0.0, 0.0};
+      double s3[3] = {0.0, 0.0, 0.0};
       _Pragma("unroll 1") for (int row = k + lane; row < L2; row += 32) {
         const double vk = (double)V[3 * row + k];
-        sd[0] += vk * U[3 * row]; sd[1] += vk * U[3 * row + 1]; sd[2] += vk * U[3 * row + 2];
+        double u[3];
+        u_row(V, sd, row, k + 1, u);
+        s3[0] += vk * u[0]; s3[1] += vk * u[1]; s3[2] += vk * u[2];
       }
 #pragma unroll
-      for (int q = 0; q < 3; ++q) sd[q] = warp_sum_call(sd[q]) * tau64[k];
-      _Pragma("unroll 1") for (int row = k + lane; row < L2; row += 32) {
-        const double vk = (double)V[3 * row + k];
-        U[3 * row] -= sd[0] * vk; U[3 * row + 1] -= sd[1] * vk; U[3 * row + 2] -= sd[2] * vk;
-      }
-      __syncwarp();
+      for (int q = 0; q < 3; ++q) sd[3 * k + q] = warp_sum_call(s3[q]) * tau64[k];
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int q = 0; q < 9; ++q) s_sd[q] = sd[q];
     }
     // U^T r in fp64 from the raw residual
     {
       double urv[3] = {0.0, 0.0, 0.0};
       _Pragma("unroll 1") for (int row = lane; row < L2; row += 32) {
         const double rr = (double)r[row];
-        urv[0] += U[3 * row] * rr; urv[1] += U[3 * row + 1] * rr; urv[2] += U[3 * row + 2] * rr;
+        double u[3];
+        u_row(V, sd, row, 0, u);
+        urv[0] += u[0] * rr; urv[1] += u[1] * rr; urv[2] += u[2] * rr;
       }
 #pragma unroll
       for (int q = 0; q < 3; ++q) urv[q] = warp_sum_call(urv[q]);
@@ -815,7 +839,7 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   Gp::sync(grp);
   stamp();  // QR, U, r~ (warp 0) | Y pairs (warps 1..3)
   const double urv[3] = {s_urv[0], s_urv[1], s_urv[2]};
-  // ---- compact outputs for the Gram stage, written as if accepted (U's shared memory is about to become W | F); a rejected
+  // ---- compact outputs for the Gram stage, written as if accepted (X's shared memory is about to become W | F); a rejected
   // track zeroes them again after the gate
   for (int k = tid; k < 3 * c; k += G) { Zr[k] = 0.0; Yr[k] = 0.0; }
   double Mm[6];  // M = U^T D U (3x3 symmetric), D = diag(u_var, v_var, u_var, ...)
@@ -824,7 +848,9 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
     for (int k = 0; k < 6; ++k) p[k] = 0.0;
     for (int row = v; row < L2; row += 128) {
       const double dd = (row & 1) ? dv : du;
-      const double u0 = U[3 * row], u1 = U[3 * row + 1], u2 = U[3 * row + 2];
+      double u[3];
+      u_row(V, s_sd, row, 0, u);
+      const double u0 = u[0], u1 = u[1], u2 = u[2];
       p[0] += dd * u0 * u0; p[1] += dd * u0 * u1; p[2] += dd * u0 * u2;
       p[3] += dd * u1 * u1; p[4] += dd * u1 * u2; p[5] += dd * u2 * u2;
     }
@@ -836,10 +862,12 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
       const int i = e / 6, b = e % 6;
       const int col = 6 * idx[i] + b;
       const double xa = X[12 * i + b], xb = X[12 * i + 6 + b];
-      double zb[3], yb[3];
+      double zb[3], yb[3], uA[3], uB[3];
+      u_row(V, s_sd, 2 * i, 0, uA);
+      u_row(V, s_sd, 2 * i + 1, 0, uB);
 #pragma unroll
       for (int q = 0; q < 3; ++q) {
-        const double ua = U[3 * (2 * i) + q], ub = U[3 * (2 * i + 1) + q];
+        const double ua = uA[q], ub = uB[q];
         zb[q] = ua * xa + ub * xb;
         yb[q] = du * ua * xa + dv * ub * xb;
       }
@@ -850,9 +878,9 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
       }
     }
   }
-  Gp::sync(grp);  // U is dead: W, F take its place
+  Gp::sync(grp);  // X is dead: W, F take its place
   // ---- two-sided transform in one pass: Q^T Y Q = Y - (V F^T + F V^T),  F = W T - V (T^T B T) / 2,  W = Y V,  B = V^T W
-  S* Wv = wv;  // [L2][3]  (wv and pv are contiguous: 2 * L2 each, >= 3 * L2 + ... see jac_smem_bytes)
+  S* Wv = wv;  // [L2][3]
   {
     // W = Y V: two threads per row (row part | column part of the packed symmetric storage)
     for (int base = 0; base < L2; base += G / 2) {
@@ -947,8 +975,10 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   if (a.prof && blockIdx.x == 0 && threadIdx.x == 0) a.prof[40 + prof_i] = 0ull;
 }
 
+// (G = 32, fp32: 10 CTAs = 20 tracks per SM, the 2 640 resident tracks a batch of 8 config-B filters needs to run in one
+// wave -- 96 registers and 10 x (2 x 9.7 KB) of shared memory at L = 30)
 template <class S, int G>
-__global__ void __launch_bounds__(JGrp<G>::CT, (G == 32) ? (sizeof(S) == 4 ? 9 : 5) : (sizeof(S) == 4 ? 5 : 3)) k_jac(const UpdArgs<S>* __restrict__ args) {
+__global__ void __launch_bounds__(JGrp<G>::CT, (G == 32) ? (sizeof(S) == 4 ? 10 : 5) : (sizeof(S) == 4 ? 5 : 3)) k_jac(const UpdArgs<S>* __restrict__ args) {
   pdl_wait();
   const UpdArgs<S>& a = args[blockIdx.z];
   constexpr int TPC = JGrp<G>::TPC, CT = JGrp<G>::CT;
@@ -956,19 +986,19 @@ __global__ void __launch_bounds__(JGrp<G>::CT, (G == 32) ? (sizeof(S) == 4 ? 9 :
   if ((int)blockIdx.x * TPC >= N) return;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const S* poses = a.poses;
-  unsigned char* wp = smem_raw + 16;
+  unsigned char* wp = smem_raw;
   if (G != 32) {
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
     S* ps = reinterpret_cast<S*>(smem_raw + 16);
     stage_table_tma(ps, a.poses, (unsigned)(a.M * kPoseStride * sizeof(S)), bar);
     poses = ps;
-    wp += sizeof(S) * kPoseStride * (size_t)a.M;
+    wp += 16 + sizeof(S) * kPoseStride * (size_t)a.M;
+    wp = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(wp) + 15) & ~uintptr_t(15));
   }
   __shared__ double redd[TPC * 4 * 6];
   __shared__ S reds[TPC * 4];
   __shared__ int redi[CT / 32];
   const int grp = threadIdx.x / G, t = blockIdx.x * TPC + grp;
-  wp = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(wp) + 15) & ~uintptr_t(15));
   if (t < N) jac_track<S, G>(a, t, grp, wp + (size_t)grp * jac_group_bytes<S>(a.Lmax), poses, redd, reds, redi);
   jac_finish<S, CT>(a, (N + TPC - 1) / TPC);
 }
