@@ -71,6 +71,8 @@ struct UpdArgs {
   double *G1p, *G2p;     // split-K partials of the Gram products
   double* bzp;           // split-K partials of Z^T (U^T r)  [nsplit][c], written by the diagonal tiles of the Gram kernel
   double *D1, *D2, *bb;  // per-clone 6x6 sums
+  // S2 (S'' = TP T''^T + R''): only its lower triangle, diagonal included, is defined -- k_gemm_s writes the lower 32 x 32
+  // tile pairs only, and both tail kernels (k_tail_fused, k_tail) read nothing above the diagonal
   double *T2, *R2, *r2, *TP, *S2, *W, *G, *y, *dx, *idiag;
   double* pivr;          // [n] diagnostics: Gamma's pivot / its original diagonal at the moment of the keep / drop decision
   int* keep;

@@ -955,7 +955,7 @@ int Ctx<S>::launch() {
   sh.asm_gx = std::min(4 * num_sms(device), (nmax_ * nmax_ + 255) / 256);
   sh.rows_smem = (unsigned)(sizeof(double) * mb::rows_smem_doubles((Lm + 7) & ~7));
   sh.gemm_g = (nmax_ + 31) / 32;
-  sh.syrk_gx = sh.gemm_g * (sh.gemm_g + 1) / 2;
+  sh.syrk_gx = sh.gemm_g * (sh.gemm_g + 1) / 2;  // lower 32 x 32 tile pairs (k_gemm_s, k_syrk)
   sh.inj_smem = (unsigned)(sizeof(double) * nmax_);
   sh.pdl = (eng[0]->use_pdl && !profile()) ? 1 : 0;
   sh.tail_nch = (eng[0]->tail_chains == 1 || Engine<S>::tail9_clusters() == 0) ? 1 : 2;
@@ -1072,7 +1072,7 @@ int Ctx<S>::run_kernels(const LaunchShape& sh) {
     if (fork) CK(cudaStreamWaitEvent(stream, ev_join2, 0));
     CK(launch_k(mb::k_gemm_tp<S>, dim3(sh.gemm_g, sh.gemm_g, nf), dim3(mb::kGemmThreads), 0, stream, false, 1, A));
     mark("k_gemm_tp");
-    CK(launch_k(mb::k_gemm_s<S>, dim3(sh.gemm_g, sh.gemm_g, nf), dim3(mb::kGemmThreads), 0, stream, pdl, 1, A));
+    CK(launch_k(mb::k_gemm_s<S>, dim3(sh.syrk_gx, 1, nf), dim3(mb::kGemmThreads), 0, stream, pdl, 1, A));  // lower tile pairs of S''
     mark("k_gemm_s");
     launches += 2;
     // rank decision + Cholesky + substitution: one thread-block cluster per filter (kernels of a kind no member uses are skipped)

@@ -8,52 +8,68 @@
 
 namespace mb {
 
-// One 32 x 32 output tile per CTA of 256 threads: four groups of 64 threads (4 x 4 register tile per thread) split every
-// 32-deep k-slab between them (8 k each) and are summed once at the end through shared memory (fixed order:
-// deterministic).  Operands stream through shared memory with the next slab prefetched into registers while the
-// current one is multiplied: at n <= 639 these products are bound by the latency of a slab (L2 round trip + a chain of
-// FMAs issued by one warp per sub-partition), not by the fp64 pipe, so shortening the chain per warp is what matters
-// (at config B 128 threads per tile were faster than 64).
+// One 32 x 32 output tile C[a][b] = sum_k A(k, a) B(k, b) per CTA of 256 threads: four groups of 64 threads (4 x 4 register
+// tile per thread) split every 32-deep k-slab between them (8 k each, one fp64 FMA chain per output and group) and are
+// summed once at the end through shared memory in a fixed order (deterministic; the same kernel serves one filter and a
+// batch).  Operands stream through double-buffered shared memory (one barrier per slab) with the next slab prefetched into
+// registers while the current one is multiplied; the ragged last slab is zero-padded.
+// The summation order is part of the results: the rank decision keeps or drops an index of S'' on the sign of its pivot,
+// and at config B some of those pivots are rounding noise.  An FP64 tensor-core form of this tile (mma.sync m8n8k4, one
+// chain of DMMA per output) was 3-4x further from a long-double reference than these four FMA chains, changed the rank of
+// 2 of 8 filters of the benchmark's batch and moved two fp64 parity cases past their bounds (DESIGN.md 4.5).
+// Each operand is fetched along its memory layout, chosen by its template flag, so that a warp's global load reads 32
+// consecutive elements:
+//   KA / KB = false: stored along the output index (P[k][b], W[k][a]): consecutive threads take consecutive output indices;
+//   KA / KB = true:  stored along k (T''[a][k], TP[a][k]): consecutive threads take consecutive k, and the slab is transposed
+//                    on its way into shared memory.
+// Slabs are staged k-major, s[k][i], with a row stride of 34 doubles: the transposing stores (32 lanes, 32 rows) hit 8 bank
+// pairs per half warp instead of one, and the 16-byte fragment reads stay aligned.
 // LA(k, a) / LB(k, b) fetch operand elements, EPI(a, b, acc) stores.
 constexpr int kGemmThreads = 256;
-constexpr int kGemmSmemDoubles = 2 * 1024 + (kGemmThreads / 64 - 1) * 1024;  // two operand slabs + the partial sums of three k-groups
-template <class LoadA, class LoadB, class Epi>
-__device__ __forceinline__ void gemm_tile32(double* __restrict__ sm /* kGemmSmemDoubles, 16-byte aligned */, int n, int k_begin, int a0, int b0,
-                                            LoadA LA, LoadB LB, Epi EPI) {
+constexpr int kGemmMinBlocks = 3;  // 3 CTAs per SM: a batch of 8 config-B filters (392 tiles of T''P) runs in one wave
+constexpr int kGemmLd = 34;
+constexpr int kGemmSlab = 32 * kGemmLd;  // doubles of one staged 32-deep operand slab
+template <bool KA, bool KB, class LoadA, class LoadB, class Epi>
+__device__ __forceinline__ void gemm_tile32(int n, int k_begin, int a0, int b0, LoadA LA, LoadB LB, Epi EPI) {
   constexpr int kParts = kGemmThreads / 64, kPer = 32 / kParts, kFetch = 1024 / kGemmThreads;
-  double (*sA)[32] = reinterpret_cast<double (*)[32]>(sm);
-  double (*sB)[32] = reinterpret_cast<double (*)[32]>(sm + 1024);
-  double (*red)[16][64] = reinterpret_cast<double (*)[16][64]>(sm + 2048);
+  static_assert((kParts - 1) * 1024 <= 4 * kGemmSlab, "the partial sums reuse the slab buffers");
+  __shared__ __align__(16) double sm[4 * kGemmSlab];  // [2 stages][A | B] slabs; after the loop: the partial sums of 3 k-groups
   const int tid = threadIdx.x;
   const int part = tid >> 6, t = tid & 63;
   const int tx = t & 7, ty = t >> 3;
+  // element e of a slab -> (k, i) of the operand
+  auto ek = [](bool along_k, int e) { return along_k ? (e & 31) : (e >> 5); };
+  auto ei = [](bool along_k, int e) { return along_k ? (e >> 5) : (e & 31); };
   double acc[4][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
   double pa[kFetch], pb[kFetch];
   auto fetch = [&](int k0) {
 #pragma unroll
     for (int u = 0; u < kFetch; ++u) {
-      const int e = tid + kGemmThreads * u, kk = e >> 5, cc = e & 31;
-      const int k = k0 + kk;
-      pa[u] = (k < n && a0 + cc < n) ? LA(k, a0 + cc) : 0.0;
-      pb[u] = (k < n && b0 + cc < n) ? LB(k, b0 + cc) : 0.0;
+      const int e = tid + kGemmThreads * u;
+      const int ka = k0 + ek(KA, e), ia = a0 + ei(KA, e), kb = k0 + ek(KB, e), ib = b0 + ei(KB, e);
+      pa[u] = (ka < n && ia < n) ? LA(ka, ia) : 0.0;
+      pb[u] = (kb < n && ib < n) ? LB(kb, ib) : 0.0;
     }
   };
-  fetch(k_begin);
-  for (int k0 = k_begin; k0 < n; k0 += 32) {
-    __syncthreads();
+  const int nslab = (n - k_begin + 31) / 32;
+  if (nslab > 0) fetch(k_begin);
+  for (int s = 0; s < nslab; ++s) {
+    // stage s & 1 was last read in slab s - 2, and every thread passed slab s - 1's barrier after that
+    double* __restrict__ sA = sm + (s & 1) * 2 * kGemmSlab;
+    double* __restrict__ sB = sA + kGemmSlab;
 #pragma unroll
     for (int u = 0; u < kFetch; ++u) {
-      const int e = tid + kGemmThreads * u, kk = e >> 5, cc = e & 31;
-      sA[kk][cc] = pa[u];
-      sB[kk][cc] = pb[u];
+      const int e = tid + kGemmThreads * u;
+      sA[ek(KA, e) * kGemmLd + ei(KA, e)] = pa[u];
+      sB[ek(KB, e) * kGemmLd + ei(KB, e)] = pb[u];
     }
     __syncthreads();
-    if (k0 + 32 < n) fetch(k0 + 32);
+    if (s + 1 < nslab) fetch(k_begin + 32 * (s + 1));
 #pragma unroll
     for (int q = 0; q < kPer; ++q) {
       const int kk = kPer * part + q;
-      const double2 a01 = *reinterpret_cast<const double2*>(&sA[kk][4 * ty]), a23 = *reinterpret_cast<const double2*>(&sA[kk][4 * ty + 2]);
-      const double2 b01 = *reinterpret_cast<const double2*>(&sB[kk][4 * tx]), b23 = *reinterpret_cast<const double2*>(&sB[kk][4 * tx + 2]);
+      const double2 a01 = *reinterpret_cast<const double2*>(&sA[kk * kGemmLd + 4 * ty]), a23 = *reinterpret_cast<const double2*>(&sA[kk * kGemmLd + 4 * ty + 2]);
+      const double2 b01 = *reinterpret_cast<const double2*>(&sB[kk * kGemmLd + 4 * tx]), b23 = *reinterpret_cast<const double2*>(&sB[kk * kGemmLd + 4 * tx + 2]);
       const double a[4] = {a01.x, a01.y, a23.x, a23.y}, b[4] = {b01.x, b01.y, b23.x, b23.y};
 #pragma unroll
       for (int p = 0; p < 4; ++p)
@@ -61,6 +77,8 @@ __device__ __forceinline__ void gemm_tile32(double* __restrict__ sm /* kGemmSmem
         for (int qq = 0; qq < 4; ++qq) acc[p][qq] += a[p] * b[qq];
     }
   }
+  double (*red)[16][64] = reinterpret_cast<double (*)[16][64]>(sm);
+  __syncthreads();  // the last slab is read by everybody before its buffer takes the partial sums
   if (part > 0) {
 #pragma unroll
     for (int p = 0; p < 4; ++p)
@@ -84,50 +102,42 @@ __device__ __forceinline__ void gemm_tile32(double* __restrict__ sm /* kGemmSmem
 
 // TP[a][b] = sum_k T2[a][k] * P[k][b]      (T2 columns < 15 are zero)
 template <class S>
-__device__ __forceinline__ void gemm_tp_tile(const UpdArgs<S>& A, double* __restrict__ sm, int ty, int tx) {
+__global__ void __launch_bounds__(kGemmThreads, kGemmMinBlocks) k_gemm_tp(const UpdArgs<S>* __restrict__ args) {
+  pdl_wait();
+  pdl_launch();
+  const UpdArgs<S>& A = args[blockIdx.z];
   const int n = A.n, ld = A.ld, ldp = A.ldp;
+  if ((int)blockIdx.x * 32 >= n || (int)blockIdx.y * 32 >= n || A.n_tracks == 0) return;
   const double* __restrict__ T2 = A.T2;
   const S* __restrict__ P = A.P;
   double* __restrict__ TP = A.TP;
-  gemm_tile32(sm, n, kImuDim, ty * 32, tx * 32,
-              [&](int k, int a) { return T2[(size_t)a * ld + k]; },
-              [&](int k, int b) { return (double)P[(size_t)k * ldp + b]; },
-              [&](int a, int b, double v) { TP[(size_t)a * ld + b] = v; });
+  gemm_tile32<true, false>(n, kImuDim, blockIdx.y * 32, blockIdx.x * 32,
+                           [&](int k, int a) { return T2[(size_t)a * ld + k]; },
+                           [&](int k, int b) { return (double)P[(size_t)k * ldp + b]; },
+                           [&](int a, int b, double v) { TP[(size_t)a * ld + b] = v; });
 }
-// S2[a][b] = sum_k TP[a][k] * T2[b][k] + R2[a][b]
+
+// S2[a][b] = sum_k TP[a][k] * T2[b][k] + R2[a][b] for b <= a: only the lower tile pairs (ta >= tb) run, and the diagonal
+// tiles are written in full.  Both tail kernels read S'' from its lower triangle only (common.cuh, UpdArgs::S2).
 template <class S>
-__device__ __forceinline__ void gemm_s_tile(const UpdArgs<S>& A, double* __restrict__ sm, int ty, int tx) {
+__global__ void __launch_bounds__(kGemmThreads, kGemmMinBlocks) k_gemm_s(const UpdArgs<S>* __restrict__ args) {
+  pdl_wait();
+  pdl_launch();
+  const UpdArgs<S>& A = args[blockIdx.z];
   const int n = A.n, ld = A.ld;
+  const int nt32 = (n + 31) / 32;
+  if ((int)blockIdx.x >= nt32 * (nt32 + 1) / 2 || A.n_tracks == 0) return;
+  int pidx = blockIdx.x, ta = 0;
+  while (pidx >= ta + 1) { pidx -= ta + 1; ++ta; }  // (ta >= tb)
+  const int tb = pidx;
   const double* __restrict__ TP = A.TP;
   const double* __restrict__ T2 = A.T2;
   const double* __restrict__ R2 = A.R2;
   double* __restrict__ S2 = A.S2;
-  gemm_tile32(sm, n, kImuDim, ty * 32, tx * 32,  // T2 columns < 15 are zero
-              [&](int k, int a) { return TP[(size_t)a * ld + k]; },
-              [&](int k, int b) { return T2[(size_t)b * ld + k]; },
-              [&](int a, int b, double v) { S2[(size_t)a * ld + b] = v + R2[(size_t)a * ld + b]; });
-}
-template <class S>
-__global__ void __launch_bounds__(kGemmThreads) k_gemm_tp(const UpdArgs<S>* __restrict__ args) {
-  pdl_wait();
-  pdl_launch();
-  const UpdArgs<S>& A = args[blockIdx.z];
-  const int n = A.n, ld = A.ld, ldp = A.ldp;
-  if ((int)blockIdx.x * 32 >= n || (int)blockIdx.y * 32 >= n || A.n_tracks == 0) return;
-  __shared__ __align__(16) double sm[kGemmSmemDoubles];
-  gemm_tp_tile(A, sm, blockIdx.y, blockIdx.x);
-}
-
-// S2[a][b] = sum_k TP[a][k] * T2[b][k] + R2[a][b]
-template <class S>
-__global__ void __launch_bounds__(kGemmThreads) k_gemm_s(const UpdArgs<S>* __restrict__ args) {
-  pdl_wait();
-  pdl_launch();
-  const UpdArgs<S>& A = args[blockIdx.z];
-  const int n = A.n, ld = A.ld;
-  if ((int)blockIdx.x * 32 >= n || (int)blockIdx.y * 32 >= n || A.n_tracks == 0) return;
-  __shared__ __align__(16) double sm[kGemmSmemDoubles];
-  gemm_s_tile(A, sm, blockIdx.y, blockIdx.x);
+  gemm_tile32<true, true>(n, kImuDim, ta * 32, tb * 32,  // T2 columns < 15 are zero
+                          [&](int k, int a) { return TP[(size_t)a * ld + k]; },
+                          [&](int k, int b) { return T2[(size_t)b * ld + k]; },
+                          [&](int a, int b, double v) { S2[(size_t)a * ld + b] = v + R2[(size_t)a * ld + b]; });
 }
 
 // P <- P - W^T W (lower-triangular tile pairs; written in the filter precision, exactly symmetric by construction), and in
@@ -135,7 +145,7 @@ __global__ void __launch_bounds__(kGemmThreads) k_gemm_s(const UpdArgs<S>* __res
 // msckf.h:1373-1391 by whichever CTA finishes last (ticket counter) -- round 1 ran both as a separate single-CTA kernel
 // (k_inject: a whole launch for a 195 x 195 mat-vec).
 template <class S>
-__global__ void __launch_bounds__(kGemmThreads) k_syrk(const UpdArgs<S>* __restrict__ args) {
+__global__ void __launch_bounds__(kGemmThreads, kGemmMinBlocks) k_syrk(const UpdArgs<S>* __restrict__ args) {
   pdl_wait();
   pdl_launch();
   const UpdArgs<S>& A = args[blockIdx.z];
@@ -148,18 +158,17 @@ __global__ void __launch_bounds__(kGemmThreads) k_syrk(const UpdArgs<S>* __restr
   int pidx = blockIdx.x, ta = 0;
   while (pidx >= ta + 1) { pidx -= ta + 1; ++ta; }  // (ta >= tb)
   const int tb = pidx;
-  __shared__ __align__(16) double sm[kGemmSmemDoubles];
-  gemm_tile32(sm, n, 0, ta * 32, tb * 32,
-              [&](int k, int a) { return Wm[(size_t)k * ld + a]; },
-              [&](int k, int b) { return Wm[(size_t)k * ld + b]; },
-              [&](int a, int b, double v) {
-                if (b <= a) {
-                  const S r = (S)((double)P[(size_t)a * ldp + b] - v);
-                  if (!isfinite((double)r)) A.m_out[2] = 1;  // MSCKF_B200_ERR_NUMERIC (benign race: every writer stores 1)
-                  P[(size_t)a * ldp + b] = r;
-                  P[(size_t)b * ldp + a] = r;
-                }
-              });
+  gemm_tile32<false, false>(n, 0, ta * 32, tb * 32,
+                            [&](int k, int a) { return Wm[(size_t)k * ld + a]; },
+                            [&](int k, int b) { return Wm[(size_t)k * ld + b]; },
+                            [&](int a, int b, double v) {
+                              if (b <= a) {
+                                const S r = (S)((double)P[(size_t)a * ldp + b] - v);
+                                if (!isfinite((double)r)) A.m_out[2] = 1;  // MSCKF_B200_ERR_NUMERIC (benign race: every writer stores 1)
+                                P[(size_t)a * ldp + b] = r;
+                                P[(size_t)b * ldp + a] = r;
+                              }
+                            });
   const int tid = threadIdx.x;
   __shared__ double part[kGemmThreads / 32][33];
   __shared__ int s_last;
