@@ -327,6 +327,18 @@ __device__ __forceinline__ void ld4(const double* p, double (&v)[4]) {
   const double2 t = *reinterpret_cast<const double2*>(p), u = *reinterpret_cast<const double2*>(p + 2);
   v[0] = t.x; v[1] = t.y; v[2] = u.x; v[3] = u.y;
 }
+// two elements at an even offset from an aligned base
+__device__ __forceinline__ void ld2(const float* p, float& a, float& b) { const float2 t = *reinterpret_cast<const float2*>(p); a = t.x; b = t.y; }
+__device__ __forceinline__ void ld2(const double* p, double& a, double& b) { const double2 t = *reinterpret_cast<const double2*>(p); a = t.x; b = t.y; }
+// p[0..5] of a row of P at an odd column (a clone block starts at kImuDim + 6 j; P's base and ldp are even-aligned): four
+// aligned pairs from p - 1 instead of six scalar loads.  p[6] exists: the last clone block ends at column n - 1, and ldp
+// rounds the odd capacity n_max >= n up to a multiple of 4.
+static_assert(kImuDim % 2 == 1, "clone blocks start at odd columns");
+template <class S>
+__device__ __forceinline__ void ld6_odd(const S* p, S (&v)[6]) {
+  S d;
+  ld2(p - 1, d, v[0]); ld2(p + 1, v[1], v[2]); ld2(p + 3, v[3], v[4]); ld2(p + 5, v[5], d);
+}
 
 // ---- gate Cholesky, blocked by panels of 8 columns, all G threads of the track's group.
 // The matrix is the trailing block [3:, 3:] of the packed-lower 2L x 2L array Y (rho = 2L - 3 rows); the right-hand side
@@ -799,41 +811,48 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   }
   if (G == 32 || warp != 0) {  // (a single-warp group does both, one after the other)
     // ---- gating (msckf.h:1103-1124): gamma = r_o^T (H_o P H_o^T + u_var I)^-1 r_o with H_o = (Q^T X)[3:]
-    // Y = X P_sub X^T, symmetric 2L x 2L, packed lower
-    const int npairs = L * (L + 1) / 2;
+    // Y = X P_sub X^T, symmetric 2L x 2L, packed lower, by 2 x 2 blocks (i, k), k <= i.  Block rows i and L-1-i share a pass
+    // of L + 1 blocks (lane e takes (i, e) for e <= i, else (L-1-i, e-i-1)): no pair decode, and the lanes of a pass read P
+    // along the same two block rows.  Each block's sums run in the same order whichever thread computes it.
     const S* P = a.P;
     const int ldp = a.ldp;
-    for (int p = (G == 32) ? tid : tid - 32; p < npairs; p += (G == 32) ? 32 : G - 32) {
-      int i = (int)((sqrtf(8.0f * (float)p + 1.0f) - 1.0f) * 0.5f);
-      while (i * (i + 1) / 2 > p) --i;
-      while ((i + 1) * (i + 2) / 2 <= p) ++i;
-      const int k = p - i * (i + 1) / 2;  // k <= i
-      const S* Pb = P + (size_t)(kImuDim + 6 * idx[i]) * ldp + (kImuDim + 6 * idx[k]);
-      const S* Xi = X + 12 * i;
-      const S* Xk = X + 12 * k;
-      S T0[6], T1[6];
+    constexpr int YW = (G == 32) ? 1 : G / 32 - 1;  // warps on the pairs
+    for (int ps = (G == 32) ? 0 : warp - 1; ps < (L + 1) / 2; ps += YW) {
+      const int ilo = ps, ihi = L - 1 - ps, ne = (ilo == ihi) ? ilo + 1 : L + 1;
+      for (int e = lane; e < ne; e += 32) {
+        const int i = (e <= ilo) ? ilo : ihi, k = (e <= ilo) ? e : e - ilo - 1;
+        const S* Pb = P + (ptrdiff_t)(kImuDim + 6 * idx[i]) * ldp + (kImuDim + 6 * idx[k]);
+        const S* Xi = X + 12 * i;
+        S T0[6], T1[6];
 #pragma unroll
-      for (int b = 0; b < 6; ++b) { T0[b] = S(0); T1[b] = S(0); }
+        for (int b = 0; b < 6; ++b) { T0[b] = S(0); T1[b] = S(0); }
 #pragma unroll
-      for (int q = 0; q < 6; ++q) {
-        const S x0 = Xi[q], x1 = Xi[6 + q];
+        for (int q = 0; q < 6; ++q) {
+          const S x0 = Xi[q], x1 = Xi[6 + q];
+          S pv[6];
+          ld6_odd(Pb + (ptrdiff_t)q * ldp, pv);
+#pragma unroll
+          for (int b = 0; b < 6; ++b) {
+            T0[b] += x0 * pv[b];
+            T1[b] += x1 * pv[b];
+          }
+        }
+        S xk[12];
+#pragma unroll
+        for (int h = 0; h < 6; ++h) ld2(X + 12 * k + 2 * h, xk[2 * h], xk[2 * h + 1]);
+        S y00 = 0, y01 = 0, y10 = 0, y11 = 0;
 #pragma unroll
         for (int b = 0; b < 6; ++b) {
-          const S pv_ = Pb[(size_t)q * ldp + b];
-          T0[b] += x0 * pv_;
-          T1[b] += x1 * pv_;
+          y00 += T0[b] * xk[b]; y01 += T0[b] * xk[6 + b];
+          y10 += T1[b] * xk[b]; y11 += T1[b] * xk[6 + b];
         }
+        S* y0 = Y + pk(2 * i, 2 * k);
+        S* y1 = y0 + 2 * i + 1;  // pk(2i + 1, 2k)
+        y0[0] = y00;
+        y1[0] = y10;
+        y1[1] = y11;
+        if (i != k) y0[1] = y01;
       }
-      S y00 = 0, y01 = 0, y10 = 0, y11 = 0;
-#pragma unroll
-      for (int b = 0; b < 6; ++b) {
-        y00 += T0[b] * Xk[b]; y01 += T0[b] * Xk[6 + b];
-        y10 += T1[b] * Xk[b]; y11 += T1[b] * Xk[6 + b];
-      }
-      Y[pk(2 * i, 2 * k)] = y00;
-      Y[pk(2 * i + 1, 2 * k)] = y10;
-      Y[pk(2 * i + 1, 2 * k + 1)] = y11;
-      if (i != k) Y[pk(2 * i, 2 * k + 1)] = y01;
     }
   }
   Gp::sync(grp);
@@ -882,20 +901,15 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   // ---- two-sided transform in one pass: Q^T Y Q = Y - (V F^T + F V^T),  F = W T - V (T^T B T) / 2,  W = Y V,  B = V^T W
   S* Wv = wv;  // [L2][3]
   {
-    // W = Y V: two threads per row (row part | column part of the packed symmetric storage)
-    for (int base = 0; base < L2; base += G / 2) {
-      const int ar = base + (tid >> 1), h = tid & 1;
-      S w0 = 0, w1 = 0, w2 = 0;
-      if (ar < L2) {
-        if (h == 0) {
-          const S* rowa = Y + pk(ar, 0);
-          for (int b = 0; b <= ar; ++b) { const S y = rowa[b]; w0 += y * V[3 * b]; w1 += y * V[3 * b + 1]; w2 += y * V[3 * b + 2]; }
-        } else {
-          for (int b = ar + 1; b < L2; ++b) { const S y = Y[pk(b, ar)]; w0 += y * V[3 * b]; w1 += y * V[3 * b + 1]; w2 += y * V[3 * b + 2]; }
-        }
-      }
-      w0 += __shfl_xor_sync(0xffffffffu, w0, 1); w1 += __shfl_xor_sync(0xffffffffu, w1, 1); w2 += __shfl_xor_sync(0xffffffffu, w2, 1);
-      if (ar < L2 && h == 0) { Wv[3 * ar] = w0; Wv[3 * ar + 1] = w1; Wv[3 * ar + 2] = w2; }
+    // W = Y V: a thread per row, L2 steps each (the row part b <= ar and the column part b > ar of the packed symmetric
+    // storage are summed apart, then added)
+    for (int ar = tid; ar < L2; ar += G) {
+      S w0 = 0, w1 = 0, w2 = 0, c0 = 0, c1 = 0, c2 = 0;
+      const S* y = Y + pk(ar, 0);
+      for (int b = 0; b <= ar; ++b) { const S yv = y[b]; w0 += yv * V[3 * b]; w1 += yv * V[3 * b + 1]; w2 += yv * V[3 * b + 2]; }
+      y = Y + pk(ar + 1, ar);
+      for (int b = ar + 1; b < L2; y += ++b) { const S yv = *y; c0 += yv * V[3 * b]; c1 += yv * V[3 * b + 1]; c2 += yv * V[3 * b + 2]; }
+      Wv[3 * ar] = w0 + c0; Wv[3 * ar + 1] = w1 + c1; Wv[3 * ar + 2] = w2 + c2;
     }
   }
   Gp::sync(grp);
@@ -935,10 +949,13 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   // only the trailing block [3:, 3:] is used below: S = (Q^T Y Q)[3:,3:] + u_var I, in place in the packed array
   const S uvar = st->u_var;
   const int rho = L2 - 3;
-  for (int ar = 3 + warp; ar < L2; ar += G / 32) {  // one row per warp, lanes along the row
-    const S va0 = V[3 * ar], va1 = V[3 * ar + 1], va2 = V[3 * ar + 2];
-    const S fa0 = Fv[3 * ar], fa1 = Fv[3 * ar + 1], fa2 = Fv[3 * ar + 2];
-    for (int b = 3 + lane; b <= ar; b += 32) {
+  // rows 3 + f and L2 - 1 - f share a warp pass of rho + 1 entries, lanes along the two rows
+  for (int f = warp; f < (rho + 1) / 2; f += G / 32) {
+    const int rlo = 3 + f, rhi = L2 - 1 - f, ne = (rlo == rhi) ? f + 1 : rho + 1;
+    for (int e = lane; e < ne; e += 32) {
+      const int ar = (e <= f) ? rlo : rhi, b = 3 + ((e <= f) ? e : e - f - 1);
+      const S va0 = V[3 * ar], va1 = V[3 * ar + 1], va2 = V[3 * ar + 2];
+      const S fa0 = Fv[3 * ar], fa1 = Fv[3 * ar + 1], fa2 = Fv[3 * ar + 2];
       const S val = Y[pk(ar, b)] - ((va0 * Fv[3 * b] + va1 * Fv[3 * b + 1] + va2 * Fv[3 * b + 2]) + (fa0 * V[3 * b] + fa1 * V[3 * b + 1] + fa2 * V[3 * b + 2]));
       Y[pk(ar, b)] = (b == ar) ? val + uvar : val;
     }
