@@ -535,11 +535,7 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   const int c = 6 * a.M;
   int prof_i = 0;
   auto stamp = [&]() {
-    if (a.prof && blockIdx.x == 0 && threadIdx.x == 0 && prof_i < 30) {
-      unsigned long long tt;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(tt));
-      a.prof[40 + prof_i++] = tt;
-    }
+    if (a.prof && blockIdx.x == 0 && threadIdx.x == 0 && prof_i < 30) a.prof[40 + prof_i++] = globaltimer();
   };
   stamp();
   // ------------------------------------------------------------------ loop-A bookkeeping

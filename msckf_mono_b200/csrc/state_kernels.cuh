@@ -106,7 +106,7 @@ __global__ void __launch_bounds__(256) k_propagate(const PropBatch<S> pb) {
   DevState<S>* gst = pb.st;
   int prof_i = 0;
   auto stamp = [&]() {
-    if (pb.prof && threadIdx.x == 0 && prof_i < 16) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); pb.prof[prof_i++] = t_; }
+    if (pb.prof && threadIdx.x == 0 && prof_i < 16) pb.prof[prof_i++] = globaltimer();
   };
   stamp();
   __shared__ DevState<S> s_state;

@@ -5,12 +5,12 @@
 //     S'' = L L^T over the kept indices                              }  in lockstep, blocked by NB
 //     W = L^-1 [T''P | r'']                                         (forward substitution as a second sweep, RHS columns
 //                                                                    sharded over the cluster)
-// followed by  P <- P - W^T W (k_syrk, all SMs) and dx = W^T y + state injection (k_inject)   (msckf.h:1373-1418)
+// followed by  P <- P - W^T W, dx = W^T y and the state injection (k_syrk, all SMs)   (msckf.h:1373-1418)
 // The matrices stay in global memory (they are L2 resident: n <= 639, fp64); cluster barriers (release/acquire
 // at cluster scope) order the phases.  Diagonal blocks: one warp of CTA 0; panel rows: solved redundantly by every CTA
 // (one thread per row) into a transposed shared panel; trailing update: 4x4 register tiles dealt to the CTAs.
 // This is the first-generation design; tail_fused.cuh documents what was measured on it and changed for the default
-// path.  Also shared with tail_fused.cuh: the tile helpers below and k_inject.
+// path.  Also shared with tail_fused.cuh: the tile helpers below.
 #pragma once
 #include <cooperative_groups.h>
 #include "common.cuh"
@@ -68,6 +68,29 @@ __device__ __forceinline__ void tc_tile_4x4(const double* At, const double* Bt, 
   }
 }
 
+// trailing-update tile (ti >= tj) of a symmetric matrix from its transposed panel: Mat[i][i2] -= sum_j PT[j][i] PT[j][i2]
+// over the NB panel rows, on the entries of the lower triangle with i < nr
+template <int NB>
+__device__ __forceinline__ void tc_update_tile(double* Mat, const double* PT, int ldt, int ld, int ti, int tj, int nr) {
+  double old[4][4];
+#pragma unroll
+  for (int p = 0; p < 4; ++p)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {  // issue the loads of the old values before the FMA chain
+      const int i = 4 * ti + p, i2 = 4 * tj + q;
+      old[p][q] = (i < nr && i2 <= i) ? Mat[(size_t)i * ld + i2] : 0.0;
+    }
+  double acc[4][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
+  tc_tile_4x4(PT, PT, ldt, ldt, 4 * ti, 4 * tj, NB, acc);
+#pragma unroll
+  for (int p = 0; p < 4; ++p)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int i = 4 * ti + p, i2 = 4 * tj + q;
+      if (i < nr && i2 <= i) Mat[(size_t)i * ld + i2] = old[p][q] - acc[p][q];
+    }
+}
+
 // one W row (an RHS column of the substitution, kept in shared memory): solve its NB entries of the current block in
 // registers, write them back (they are final) and, transposed, into XT for the tile update of the remaining entries
 template <int NB>
@@ -87,13 +110,6 @@ __device__ __forceinline__ void tc_w_row(double* wrow, int nb, const double* D, 
     XT[j * NB + c] = x[j];
     if (j < nb) wrow[j] = x[j];
   }
-}
-
-__device__ __forceinline__ void tc_tile_index(int tl, int& ti, int& tj) {  // tl -> (ti >= tj) of the lower triangle
-  ti = (int)((sqrtf(8.0f * (float)tl + 1.0f) - 1.0f) * 0.5f);
-  while (ti * (ti + 1) / 2 > tl) --ti;
-  while ((ti + 1) * (ti + 2) / 2 <= tl) ++ti;
-  tj = tl - ti * (ti + 1) / 2;
 }
 
 // W = L^-1 [TP | r''] as a separate sweep over the finished factor (windows too large for the fused form): RHS columns
@@ -196,11 +212,7 @@ __global__ void __launch_bounds__(kTailThreads) k_tail(const UpdArgs<S>* __restr
   cg::cluster_group cluster = cg::this_cluster();
   int prof_i = 0;
   auto stamp = [&]() {
-    if (prof && blockIdx.x == 0 && threadIdx.x == 0 && prof_i < 64) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-      prof[prof_i++] = t;
-    }
+    if (prof && blockIdx.x == 0 && threadIdx.x == 0 && prof_i < 64) prof[prof_i++] = globaltimer();
   };
   stamp();
   const int crank = (int)cluster.block_rank();
@@ -346,26 +358,8 @@ __global__ void __launch_bounds__(kTailThreads) k_tail(const UpdArgs<S>* __restr
           const int it = crank + C * q;
           const bool isG = it >= ntile;
           int ti, tj;
-          tc_tile_index(isG ? it - ntile : it, ti, tj);
-          double* Mat = (isG ? G : A) + (size_t)r0 * ld + r0;
-          const double* PT = isG ? PT_G : PT_A;
-          double old[4][4];
-#pragma unroll
-          for (int p = 0; p < 4; ++p)
-#pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {  // issue the loads of the old values before the FMA chain
-              const int i = 4 * ti + p, i2 = 4 * tj + qq;
-              old[p][qq] = (i < nr && i2 <= i) ? Mat[(size_t)i * ld + i2] : 0.0;
-            }
-          double acc[4][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
-          tc_tile_4x4(PT, PT, ldt, ldt, 4 * ti, 4 * tj, NB, acc);
-#pragma unroll
-          for (int p = 0; p < 4; ++p)
-#pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-              const int i = 4 * ti + p, i2 = 4 * tj + qq;
-              if (i < nr && i2 <= i) Mat[(size_t)i * ld + i2] = old[p][qq] - acc[p][qq];
-            }
+          tri_tile_index(isG ? it - ntile : it, ti, tj);
+          tc_update_tile<NB>((isG ? G : A) + (size_t)r0 * ld + r0, isG ? PT_G : PT_A, ldt, ld, ti, tj, nr);
         }
       }
     }

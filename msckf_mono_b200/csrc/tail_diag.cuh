@@ -19,10 +19,6 @@
 #pragma once
 #include "common.cuh"
 
-#ifndef MSCKF_TF_PW
-#define MSCKF_TF_PW 8  // panel width of tf_factor_one (4 or 8; 8: four panels per block, half the barriers of 4)
-#endif
-
 namespace mb {
 
 constexpr int kFB = 32;        // block size of the fused form
@@ -49,7 +45,7 @@ __device__ __noinline__ TfRank tf_factor_block(double* __restrict__ DG, double* 
   constexpr int LD = kFLD, PW = 4;
   int dpi = 0;
   auto dstamp = [&]() {
-    if (dprof && tid == 0 && dpi < 14) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); dprof[dpi++] = t_; }
+    if (dprof && tid == 0 && dpi < 14) dprof[dpi++] = globaltimer();
   };
   dstamp();
   const int half = (tid >> 5) & 1, lane = tid & 31;
@@ -202,9 +198,9 @@ __device__ __noinline__ int tf_factor_one(double* __restrict__ D, double* __rest
                                           const double* __restrict__ d0, int kb, int nb, double thr, int rank_cap, int role, int rk,
                                           int tid, int nthreads, unsigned tag /* > 0, grows with every block */, TfLink lk,
                                           double* __restrict__ pivr, unsigned long long* dprof = nullptr) {
-  constexpr int LD = kFLD, PW = MSCKF_TF_PW, PH = PW / 2;
+  constexpr int LD = kFLD, PW = 8, PH = PW / 2;  // 8-column panels: four per block, half the barriers of tf_factor_block's 4
   auto dstamp = [&](int slot) {  // fixed slots: 0 entry | 1 + 4 p + {0: micro + rows, 1: barrier, 2: trailing, 3: barrier} for panels p < 3 | 13 end
-    if (dprof && tid == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); dprof[slot] = t_; }
+    if (dprof && tid == 0) dprof[slot] = globaltimer();
   };
   dstamp(0);
   const int lane = tid & 31, warp = tid >> 5;

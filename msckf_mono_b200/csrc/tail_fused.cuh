@@ -98,20 +98,12 @@ __global__ void __launch_bounds__(kTailThreads) k_tail_fused(const UpdArgs<S>* _
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int prof_i = 0;
   auto stamp = [&]() {
-    if (prof && blockIdx.x == 0 && tid == 0 && prof_i < 39) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t) : : "memory");
-      prof[prof_i++] = t;
-    }
+    if (prof && blockIdx.x == 0 && tid == 0 && prof_i < 39) prof[prof_i++] = globaltimer();
   };
   stamp();
   int wprof_i = 0;
   auto wstamp = [&]() {  // the same for the first worker CTA (slots 20..39)
-    if (prof && (int)blockIdx.x == NCH && blockIdx.z == 0 && tid == 0 && wprof_i < 19) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t) : : "memory");
-      prof[20 + wprof_i++] = t;
-    }
+    if (prof && (int)blockIdx.x == NCH && blockIdx.z == 0 && tid == 0 && wprof_i < 19) prof[20 + wprof_i++] = globaltimer();
   };
   extern __shared__ __align__(16) double sm[];
   const int ldt = (n + 3) & ~3;              // row stride of the transposed panels (16-byte aligned rows)
@@ -179,56 +171,57 @@ __global__ void __launch_bounds__(kTailThreads) k_tail_fused(const UpdArgs<S>* _
   }
   __syncthreads();
   // ---------------------------------------------------------------- blocked rank-revealing Cholesky (G decides, A follows)
-  // CTA 0 factorises diagonal blocks (tf_factor_block, tail_diag.cuh: G decides keep / drop per pivot, A follows).  The
-  // blocks (lower triangles incl. the diagonal, in DG / DA) are in shared memory when this is called; the inverses end up in
-  // LIG / LIA and in the L2 scratch for the other CTAs.  Block 0 is factorised up front; block kb + 1 is factorised by CTA 0 WHILE the
-  // other CTAs run the trailing update of block kb (it only needs the leading 32 x 32 tile of that update, which CTA 0
-  // forms itself from the panel).
-  auto factor_block = [&](int kb, int nb, bool stamps, double* Lsc) {
-    if (stamps && tid == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); prof[76] = t_; }
-    TfRank rk;
-    rk.g = s_rankG; rk.a = s_rankA;
-    __syncthreads();
-    rk = tf_factor_block(DG, DA, LIG, LIA, idg, ida, d0, kb, nb, thr, rank_cap, full, rk, tid, kTailThreads, WB, DT, ua.pivr, stamps ? prof + 60 : nullptr);
-    if (tid == 0) { s_rankG = rk.g; s_rankA = rk.a; }
-    if (stamps && tid == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); prof[77] = t_; }
-    // the inverses go to the other CTAs through L2 (a DSMEM push of 2 x 8.7 KB to 7 CTAs runs at ~20 B/clk: 3 us)
-    for (int e = tid; e < NB * LD / 2; e += kTailThreads) {
-      reinterpret_cast<double2*>(Lsc)[e] = reinterpret_cast<const double2*>(LIA)[e];
-      if (!full) reinterpret_cast<double2*>(Lsc + NB * LD)[e] = reinterpret_cast<const double2*>(LIG)[e];
-    }
-  };
-  // NCH = 2: this chain CTA's own matrix lives in DA / LIA / ida whichever it is (CTA 0: S'', CTA 1: Gamma)
+  // The chain CTAs factorise the diagonal blocks: NCH = 1: CTA 0 both matrices (tf_factor_block, tail_diag.cuh: G decides
+  // keep / drop per pivot, A follows); NCH = 2: CTA 0 S'' and CTA 1 Gamma (tf_factor_one: Gamma's flags reach CTA 0 through
+  // DSMEM).  A block (lower triangle incl. the diagonal) is in shared memory when `factor` is called; the inverses end up
+  // in shared memory and in the L2 scratch for the workers.  Block 0 is factorised up front; block kb + 1 is factorised
+  // WHILE the workers run the trailing update of block kb (it only needs the leading 32 x 32 tile of that update, which the
+  // chain CTAs form themselves from the panel).
+  // The NM matrices a chain CTA carries -- NCH = 1: S'' and Gamma (Gamma's loads and arithmetic skipped when m <= n);
+  // NCH = 2: its own in DA / LIA / ida (CTA 0: S'', CTA 1: Gamma; the Gamma CTA idles when m <= n).  Matrix q is handed out
+  // by a function of q over the restrict pointer Mch, not kept in an array of pointers: with an array the one-chain form
+  // needs 6 more registers, without Mch the two-chain form spills.
+  constexpr int NM = 3 - NCH;
   const bool chainG = (NCH == 2) && crank == 1;
+  struct ChainMat { const double* M; double* D; double* LI; double* X; };  // in L2, its diagonal block, that block's inverse, X
   double* __restrict__ Mch = chainG ? G : A;
+  auto cm = [&](int q) { return q == 0 ? ChainMat{Mch, DA, LIA, WB} : ChainMat{G, DG, LIG, DT}; };
+  auto live = [&](int q) { return NCH == 2 || q == 0 || !full; };
+  auto isG = [&](int q) { return NCH == 2 ? chainG : q == 1; };
   TfLink link;
   link.words = s_words;
   link.timed_out = &s_timeout;
   if (NCH == 2 && chainG) link.words = cluster.map_shared_rank(s_words, 0);  // the Gamma CTA writes into CTA 0's array
-  auto factor_one = [&](int kb, int nb, bool stamps, double* Lsc) {
-    if (stamps && tid == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); prof[76] = t_; }
-    const int rk0 = chainG ? s_rankG : s_rankA;
-    __syncthreads();
-    const int role = full ? 2 : (chainG ? 1 : 0);
-    const int rk1 = tf_factor_one(DA, LIA, ida, d0, kb, nb, thr, rank_cap, role, rk0, tid, kTailThreads, (unsigned)(kb / NB) + 1u, link, ua.pivr, stamps ? prof + 60 : nullptr);
-    if (tid == 0) { if (chainG) s_rankG = rk1; else s_rankA = rk1; }
-    if (stamps && tid == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_) : : "memory"); prof[77] = t_; }
-    double* dst = Lsc + (chainG ? NB * LD : 0);
-    for (int e = tid; e < NB * LD / 2; e += kTailThreads) reinterpret_cast<double2*>(dst)[e] = reinterpret_cast<const double2*>(LIA)[e];
-  };
-  if (NCH == 1) {
-    if (crank == 0) {
-      const int nb0 = min(NB, n);
-      if (!full) tf_load_diag(DG, G, ld, 0, nb0, tid);
-      tf_load_diag(DA, A, ld, 0, nb0, tid);
+  auto factor = [&](int kb, int nb, bool stamps, double* Lsc) {
+    if (stamps && tid == 0) prof[76] = globaltimer();
+    if (NCH == 1) {
+      TfRank rk;
+      rk.g = s_rankG; rk.a = s_rankA;
       __syncthreads();
-      factor_block(0, nb0, prof != nullptr, Lsc_of(0));
+      rk = tf_factor_block(DG, DA, LIG, LIA, idg, ida, d0, kb, nb, thr, rank_cap, full, rk, tid, kTailThreads, WB, DT, ua.pivr, stamps ? prof + 60 : nullptr);
+      if (tid == 0) { s_rankG = rk.g; s_rankA = rk.a; }
+    } else {
+      const int rk0 = chainG ? s_rankG : s_rankA;
+      __syncthreads();
+      const int role = full ? 2 : (chainG ? 1 : 0);
+      const int rk1 = tf_factor_one(DA, LIA, ida, d0, kb, nb, thr, rank_cap, role, rk0, tid, kTailThreads, (unsigned)(kb / NB) + 1u, link, ua.pivr, stamps ? prof + 60 : nullptr);
+      if (tid == 0) { if (chainG) s_rankG = rk1; else s_rankA = rk1; }
     }
-  } else if (crank < NCH && !(chainG && full)) {
+    if (stamps && tid == 0) prof[77] = globaltimer();
+    // the inverses go to the workers through L2 (a DSMEM push of 2 x 8.7 KB to 7 CTAs runs at ~20 B/clk: 3 us)
+    for (int e = tid; e < NB * LD / 2; e += kTailThreads) {
+#pragma unroll
+      for (int q = 0; q < NM; ++q)
+        if (live(q)) reinterpret_cast<double2*>(Lsc + (isG(q) ? NB * LD : 0))[e] = reinterpret_cast<const double2*>(cm(q).LI)[e];
+    }
+  };
+  if (crank < NCH && !(chainG && full)) {
     const int nb0 = min(NB, n);
-    tf_load_diag(DA, Mch, ld, 0, nb0, tid);
+#pragma unroll
+    for (int q = 0; q < NM; ++q)
+      if (live(q)) tf_load_diag(cm(q).D, cm(q).M, ld, 0, nb0, tid);
     __syncthreads();
-    factor_one(0, nb0, prof != nullptr && crank == 0, Lsc_of(0));
+    factor(0, nb0, prof != nullptr && crank == 0, Lsc_of(0));
   }
   stamp();  // diagonal block 0 done
   for (int kb = 0; kb < n; kb += NB) {
@@ -238,158 +231,90 @@ __global__ void __launch_bounds__(kTailThreads) k_tail_fused(const UpdArgs<S>* _
     cluster.sync();  // B1: inverses of block kb in L2; trailing update of block kb - 1 complete
     const int blk = kb / NB;
     const double* Lsc = Lsc_of(blk);
-    if (NCH == 2 && crank < NCH) {
-      // ---- two chain CTAs (S'': 0, Gamma: 1), each ONE BLOCK AHEAD of the workers with its own matrix: the same steps as the
-      // single chain CTA below, for one matrix
+    if (crank < NCH) {
+      // ---- the chain CTAs run ONE BLOCK AHEAD of the workers: while those solve the panel of block kb, exchange it and run the
+      // trailing update, a chain CTA solves only the 32 panel rows of the NEXT diagonal block itself (X = rows * Linv^T with
+      // the inverses it still holds), forms that block's leading tile and factorises it, for each of its matrices.  It has
+      // nothing to contribute to the panel barrier (arrives at once, waits when done), so the workers never wait for it there.
       if (nr <= 0) break;
       asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");  // B2 of this block
       if (!(chainG && full)) {
         const int nb2 = min(NB, nr);
-        constexpr int NS = NB * NB / kTailThreads;
-        constexpr int NLd = (NB * LD + kTailThreads - 1) / kTailThreads;
-        double sa_[NS], oa_[NLd];
+        // every global load of this step in flight before the first use: the block's 32 panel rows (column block kb) and the
+        // old values of its leading tile -- one L2 round trip instead of one per loop iteration
+        constexpr int NS = NB * NB / kTailThreads;                       // 4 staged entries per thread and matrix
+        constexpr int NLd = (NB * LD + kTailThreads - 1) / kTailThreads;  // 5 leading-tile entries per thread and matrix
+        double s_[NM][NS], o_[NM][NLd];
 #pragma unroll
         for (int u = 0; u < NS; ++u) {
           const int e = tid + u * kTailThreads, l = e / NB, c = e % NB;
-          sa_[u] = (l < nb2 && c < nb) ? __ldcg(Mch + (size_t)(r0 + l) * ld + kb + c) : 0.0;
+          const bool in = (l < nb2 && c < nb);
+#pragma unroll
+          for (int q = 0; q < NM; ++q) s_[q][u] = (in && live(q)) ? __ldcg(cm(q).M + (size_t)(r0 + l) * ld + kb + c) : 0.0;
         }
 #pragma unroll
         for (int u = 0; u < NLd; ++u) {
           const int e = tid + u * kTailThreads, i = e / LD, j = e % LD;
-          oa_[u] = (e < NB * LD && i < nb2 && j <= i) ? __ldcg(Mch + (size_t)(r0 + i) * ld + r0 + j) : 0.0;
+          const bool in = (e < NB * LD && i < nb2 && j <= i);
+#pragma unroll
+          for (int q = 0; q < NM; ++q) o_[q][u] = (in && live(q)) ? __ldcg(cm(q).M + (size_t)(r0 + i) * ld + r0 + j) : 0.0;
         }
 #pragma unroll
         for (int u = 0; u < NS; ++u) {
           const int e = tid + u * kTailThreads, l = e / NB, c = e % NB;
-          DA[l * LD + c] = sa_[u];
+#pragma unroll
+          for (int q = 0; q < NM; ++q) cm(q).D[l * LD + c] = s_[q][u];
         }
         __syncthreads();
 #pragma unroll 1
-        for (int e = tid; e < NB * NB; e += kTailThreads) {  // X = rows * Linv^T
+        for (int e = tid; e < NB * NB; e += kTailThreads) {  // X = rows * Linv^T (rows of a dropped pivot of Linv are zero)
           const int l = e / NB, j = e % NB;
-          double sa[4] = {0.0, 0.0, 0.0, 0.0};
+          double s[NM][4] = {};
 #pragma unroll 2
           for (int c = 0; c < NB; c += 4) {
-            double a4[4], l4[4];
-            tf_ld4(DA + l * LD + c, a4); tf_ld4(LIA + j * LD + c, l4);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) sa[q] += a4[q] * l4[q];
+            for (int q = 0; q < NM; ++q) {
+              if (!live(q)) continue;
+              double a4[4], l4[4];
+              tf_ld4(cm(q).D + l * LD + c, a4); tf_ld4(cm(q).LI + j * LD + c, l4);
+#pragma unroll
+              for (int t = 0; t < 4; ++t) s[q][t] += a4[t] * l4[t];
+            }
           }
-          WB[l * LD + j] = (sa[0] + sa[1]) + (sa[2] + sa[3]);
+#pragma unroll
+          for (int q = 0; q < NM; ++q) cm(q).X[l * LD + j] = (s[q][0] + s[q][1]) + (s[q][2] + s[q][3]);
         }
         __syncthreads();
 #pragma unroll
         for (int u = 0; u < NLd; ++u) {  // the next diagonal block = its leading tile of the trailing update
           const int e = tid + u * kTailThreads, i = e / LD, j = e % LD;
           if (e >= NB * LD) break;
-          double va = 0.0;
+          double v[NM] = {};
           if (i < nb2 && j <= i) {
-            double sa[4] = {0.0, 0.0, 0.0, 0.0};
+            double s[NM][4] = {};
 #pragma unroll 2
             for (int c = 0; c < NB; c += 4) {
-              double a4[4], b4[4];
-              tf_ld4(WB + i * LD + c, a4); tf_ld4(WB + j * LD + c, b4);
 #pragma unroll
-              for (int q = 0; q < 4; ++q) sa[q] += a4[q] * b4[q];
+              for (int q = 0; q < NM; ++q) {
+                if (!live(q)) continue;
+                double a4[4], b4[4];
+                tf_ld4(cm(q).X + i * LD + c, a4); tf_ld4(cm(q).X + j * LD + c, b4);
+#pragma unroll
+                for (int t = 0; t < 4; ++t) s[q][t] += a4[t] * b4[t];
+              }
             }
-            va = oa_[u] - ((sa[0] + sa[1]) + (sa[2] + sa[3]));
+#pragma unroll
+            for (int q = 0; q < NM; ++q) v[q] = o_[q][u] - ((s[q][0] + s[q][1]) + (s[q][2] + s[q][3]));
           }
-          DA[e] = va;
+#pragma unroll
+          for (int q = 0; q < NM; ++q) cm(q).D[e] = v[q];
         }
         __syncthreads();
         stamp();  // next diagonal block formed (CTA 0)
-        factor_one(r0, nb2, false, Lsc_of(blk + 1));
+        factor(r0, nb2, false, Lsc_of(blk + 1));
         stamp();  // next diagonal block factorised (CTA 0)
       }
       asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");   // B2
-      continue;
-    }
-    if (NCH == 1 && crank == 0) {
-      // ---- CTA 0 runs the chain of diagonal blocks ONE BLOCK AHEAD of the other CTAs (round 2): while they solve the panel of
-      // block kb, exchange it and run the trailing update, CTA 0 solves only the 32 panel rows of the NEXT diagonal block itself
-      // (X = rows * Linv^T with the inverses it still holds), forms that block's leading tile and factorises it.  It has
-      // nothing to contribute to the panel barrier (arrives at once, waits when done), so the others never wait for it there.
-      if (nr <= 0) break;
-      asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");  // B2 of this block
-      const int nb2 = min(NB, nr);
-      // every global load of this step in flight before the first use: the block's 32 panel rows (column block kb) and the old
-      // values of its leading tile -- one L2 round trip instead of one per loop iteration
-      constexpr int NS = NB * NB / kTailThreads;                       // 4 staged entries per thread and matrix
-      constexpr int NLd = (NB * LD + kTailThreads - 1) / kTailThreads;  // 5 leading-tile entries per thread and matrix
-      double sa_[NS], sg_[NS], oa_[NLd], og_[NLd];
-#pragma unroll
-      for (int u = 0; u < NS; ++u) {
-        const int e = tid + u * kTailThreads, l = e / NB, c = e % NB;
-        const bool in = (l < nb2 && c < nb);
-        sa_[u] = in ? __ldcg(A + (size_t)(r0 + l) * ld + kb + c) : 0.0;
-        sg_[u] = (in && !full) ? __ldcg(G + (size_t)(r0 + l) * ld + kb + c) : 0.0;
-      }
-#pragma unroll
-      for (int u = 0; u < NLd; ++u) {
-        const int e = tid + u * kTailThreads, i = e / LD, j = e % LD;
-        const bool in = (e < NB * LD && i < nb2 && j <= i);
-        oa_[u] = in ? __ldcg(A + (size_t)(r0 + i) * ld + r0 + j) : 0.0;
-        og_[u] = (in && !full) ? __ldcg(G + (size_t)(r0 + i) * ld + r0 + j) : 0.0;
-      }
-#pragma unroll
-      for (int u = 0; u < NS; ++u) {
-        const int e = tid + u * kTailThreads, l = e / NB, c = e % NB;
-        DA[l * LD + c] = sa_[u];
-        DG[l * LD + c] = sg_[u];
-      }
-      __syncthreads();
-#pragma unroll 1
-      for (int e = tid; e < NB * NB; e += kTailThreads) {  // X = rows * Linv^T (rows of a dropped pivot of Linv are zero)
-        const int l = e / NB, j = e % NB;
-        double sa[4] = {0.0, 0.0, 0.0, 0.0}, sg[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll 2
-        for (int c = 0; c < NB; c += 4) {
-          double a4[4], l4[4];
-          tf_ld4(DA + l * LD + c, a4); tf_ld4(LIA + j * LD + c, l4);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) sa[q] += a4[q] * l4[q];
-          if (!full) {
-            double g4[4], h4[4];
-            tf_ld4(DG + l * LD + c, g4); tf_ld4(LIG + j * LD + c, h4);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) sg[q] += g4[q] * h4[q];
-          }
-        }
-        WB[l * LD + j] = (sa[0] + sa[1]) + (sa[2] + sa[3]);
-        DT[l * LD + j] = (sg[0] + sg[1]) + (sg[2] + sg[3]);
-      }
-      __syncthreads();
-#pragma unroll
-      for (int u = 0; u < NLd; ++u) {  // the next diagonal block = its leading tile of the trailing update
-        const int e = tid + u * kTailThreads, i = e / LD, j = e % LD;
-        if (e >= NB * LD) break;
-        double va = 0.0, vg = 0.0;
-        if (i < nb2 && j <= i) {
-          double sa[4] = {0.0, 0.0, 0.0, 0.0}, sg[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll 2
-          for (int c = 0; c < NB; c += 4) {
-            double a4[4], b4[4];
-            tf_ld4(WB + i * LD + c, a4); tf_ld4(WB + j * LD + c, b4);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) sa[q] += a4[q] * b4[q];
-            if (!full) {
-              double g4[4], h4[4];
-              tf_ld4(DT + i * LD + c, g4); tf_ld4(DT + j * LD + c, h4);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) sg[q] += g4[q] * h4[q];
-            }
-          }
-          va = oa_[u] - ((sa[0] + sa[1]) + (sa[2] + sa[3]));
-          vg = og_[u] - ((sg[0] + sg[1]) + (sg[2] + sg[3]));
-        }
-        DA[e] = va;
-        DG[e] = vg;
-      }
-      __syncthreads();
-      stamp();  // next diagonal block formed (CTA 0)
-      factor_block(r0, nb2, false, Lsc_of(blk + 1));
-      stamp();  // next diagonal block factorised (CTA 0)
-      asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");   // B2 (long complete)
       continue;
     }
     wstamp();  // B1 passed
@@ -516,26 +441,8 @@ __global__ void __launch_bounds__(kTailThreads) k_tail_fused(const UpdArgs<S>* _
           const int it = first + q;
           const bool isG = it >= nrest;
           int ti, tj;
-          tc_tile_index((isG ? it - nrest : it) + kLead, ti, tj);
-          double* Mat = (isG ? G : A) + (size_t)r0 * ld + r0;
-          const double* PT = isG ? PT_G : PT_A;
-          double old[4][4];
-#pragma unroll
-          for (int p = 0; p < 4; ++p)
-#pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {  // issue the loads of the old values before the FMA chain
-              const int i = 4 * ti + p, i2 = 4 * tj + qq;
-              old[p][qq] = (i < nr && i2 <= i) ? Mat[(size_t)i * ld + i2] : 0.0;
-            }
-          double acc[4][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
-          tc_tile_4x4(PT, PT, ldt, ldt, 4 * ti, 4 * tj, NB, acc);
-#pragma unroll
-          for (int p = 0; p < 4; ++p)
-#pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-              const int i = 4 * ti + p, i2 = 4 * tj + qq;
-              if (i < nr && i2 <= i) Mat[(size_t)i * ld + i2] = old[p][qq] - acc[p][qq];
-            }
+          tri_tile_index((isG ? it - nrest : it) + kLead, ti, tj);
+          tc_update_tile<NB>((isG ? G : A) + (size_t)r0 * ld + r0, isG ? PT_G : PT_A, ldt, ld, ti, tj, nr);
         } else {
           const int w = q - mine, ti = w % nt, c4 = w / nt;
           double acc[4][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};

@@ -1,8 +1,10 @@
 // msckf_mono_b200/csrc/tail_kernels.cuh
 // Dense n x n tail of the EKF update (msckf.h:1369-1418) in square-root form, fp64 throughout:
 //   TP  = T'' P                      S'' = TP T''^T + R''          (k_gemm_tp, k_gemm_s: this file, all SMs)
-//   S'' = L L^T over the independent rows, W = L^-1 [TP | r''], P+ = P - W^T W (== Joseph form for the optimal
-//   gain of the projected system), dx = W^T (L^-1 r''), state injection       (k_tail: tail_cluster.cuh, one cluster)
+//   S'' = L L^T over the independent rows, W = L^-1 [TP | r'']       (k_tail_fused: tail_fused.cuh, one cluster; windows
+//                                                                     past 34 clones: k_tail, tail_cluster.cuh)
+//   P+ = P - W^T W (== Joseph form for the optimal gain of the projected system), dx = W^T (L^-1 r''), state injection
+//                                                                    (k_syrk: this file, all SMs)
 #pragma once
 #include "common.cuh"
 

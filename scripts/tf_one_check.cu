@@ -1,6 +1,6 @@
-// Stand-alone check of tf_factor_one (tail_diag.cuh) for a panel width given by -DMSCKF_TF_PW: a cluster of two CTAs
-// factorises a 32 x 32 pair (CTA 0: A following CTA 1's flags for G, G rank-deficient), compared with a host reference.
-// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DMSCKF_TF_PW=8 -I msckf_mono_b200/csrc -o scripts/tf_one_check8.bin scripts/tf_one_check.cu
+// Stand-alone check of tf_factor_one (tail_diag.cuh) as the engine runs it: a cluster of two CTAs factorises a 32 x 32
+// pair (CTA 0: A following CTA 1's flags for G, G rank-deficient), compared with a host reference.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I msckf_mono_b200/csrc -o scripts/tf_one_check.bin scripts/tf_one_check.cu
 #include <cooperative_groups.h>
 #include <cmath>
 #include <cstdio>
@@ -86,7 +86,7 @@ int main() {
       ea = fmax(ea, fabs(da)); eg = fmax(eg, fabs(dg)); na = fmax(na, fabs(XA[i * n + j])); ng = fmax(ng, fabs(XG[i * n + j]));
     }
     int nk = 0; for (int k : keep) nk += k;
-    printf("PW=%d reps=%d: %s  rank A %d G %d (host %d)  max |Linv - ref| A %.3e (of %.2e)  G %.3e (of %.2e)\n", MSCKF_TF_PW, reps, cudaGetErrorString(e), rk[0], rk[1], nk, ea, na, eg, ng);
+    printf("reps=%d: %s  rank A %d G %d (host %d)  max |Linv - ref| A %.3e (of %.2e)  G %.3e (of %.2e)\n", reps, cudaGetErrorString(e), rk[0], rk[1], nk, ea, na, eg, ng);
   }
   return 0;
 }
