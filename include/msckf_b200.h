@@ -141,6 +141,26 @@ long long msckf_b200_batch_launch_count(const msckf_b200_batch* b);
  * figure for its threads per track and dynamic shared memory (0 before the first launch) */
 int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b);
 void* msckf_b200_batch_stream(msckf_b200_batch* b);
+/* The other device calls of a frame for every member at once (the per-image sequence of datasets/asl_msckf.cpp:233-294 on a
+ * batch).  Arrays have one entry per engine, in the order given to _create.  Each call validates every member before it
+ * launches anything: a bad argument returns MSCKF_B200_ERR_ARG and a member with an un-fetched update MSCKF_B200_ERR_STATE,
+ * and then no member has changed.  Every member computes exactly what its single-engine call computes, bit for bit.
+ * Up to 32 members share one launch per kernel; past 32 the members run in consecutive launches of 32.
+ * _propagate_n, _augment and _prune are asynchronous like their single-engine forms (arguments travel by value, nothing is
+ * synchronised except where _augment grows a member's clone capacity). */
+/* msckf_b200_propagate_n for every member (MSCKF::propagate msckf.h:101-145, applied reading by reading):
+ * readings[i] = [k[i]][7] scalars; k[i] may be 0 (readings[i] may then be NULL); k = NULL: no member has readings.
+ * Launches: for each step of 16 readings, one per 32 members that still have readings in that step
+ * (members with at most 16 readings each, at most 32 members: one launch). */
+int msckf_b200_batch_propagate_n(msckf_b200_batch* b, const void* const* readings, const int* k);
+/* msckf_b200_augment (MSCKF::augmentState msckf.h:148-212) for the members with which[i] != 0 (which = NULL: all) */
+int msckf_b200_batch_augment(msckf_b200_batch* b, const int* which);
+/* msckf_b200_prune per member (pruneEmptyStates msckf.h:685-761, pruneRedundantStates :616-681): keep[i][0 .. n_keep[i]-1]
+ * ascending positions; n_keep[i] < 0 or equal to the member's window: that member is left untouched */
+int msckf_b200_batch_prune(msckf_b200_batch* b, const int* const* keep, const int* n_keep);
+/* msckf_b200_get_state for every member (imu = NULL, imu[i] = NULL, clone_poses = NULL or clone_poses[i] = NULL: not wanted),
+ * with one stream synchronisation for the whole batch */
+int msckf_b200_batch_get_state(msckf_b200_batch* b, void* const* imu, void* const* clone_poses);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

@@ -30,8 +30,12 @@
 
 namespace msckf_mono {
 
+template <typename _S> class MSCKFBatch;
+
 template <typename _S>
 class MSCKF {
+  friend class MSCKFBatch<_S>;
+
  public:
   MSCKF_B200_ALIGNED_NEW
   MSCKF() {}
@@ -110,8 +114,12 @@ class MSCKF {
 
   // ref :148-212
   void augmentState(const int& state_id, const _S& time) {
-    map_.clear();
     check(msckf_b200_augment(eng()), "msckf_b200_augment");
+    augmentAbsorb(state_id, time);
+  }
+  // host part of augmentState, after the device appended the clone
+  void augmentAbsorb(const int& state_id, const _S& time) {
+    map_.clear();
     camState<_S> cam_state;
     cam_state.last_correlated_id = -1;
     cam_state.time = time;
@@ -195,149 +203,44 @@ class MSCKF {
     marginalizeCollect();
   }
 
-  // ref :453-682
+  // ref :453-682.  Phases (shared with MSCKFBatch): triangulate the uninitialised features seen by the redundant clones,
+  // residualise the observations those clones made, delete the clones.
   void pruneRedundantStates() {
-    if (cam_states_.size() < 20) return;
+    if (!redundantPruneWanted()) return;
     refreshState();
-    std::vector<size_t> rm_cam_state_ids;
-    findRedundantCamStates(rm_cam_state_ids);
-    // ---- first loop (ref :466-534): drop single observations, triangulate uninitialised features
-    std::vector<size_t> tri_feat;  // indices into feature_tracks_ that need checkMotion + initializePosition
-    std::vector<std::vector<size_t>> tri_involved;
-    std::vector<featureTrackToResidualize<_S>> tri_batch;
-    for (size_t fi = 0; fi < feature_tracks_.size(); ++fi) {
-      auto& feature = feature_tracks_[fi];
-      std::vector<size_t> involved;
-      size_t obs_id = 0;
-      for (const auto& cam_id : rm_cam_state_ids) {
-        auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
-        if (it != feature.cam_state_indices.end()) { involved.push_back(cam_id); obs_id = std::distance(feature.cam_state_indices.begin(), it); }
-      }
-      if (involved.size() == 0) continue;
-      if (involved.size() == 1) {
-        feature.observations.erase(feature.observations.begin() + obs_id);
-        feature.cam_state_indices.erase(feature.cam_state_indices.begin() + obs_id);
-        continue;
-      }
-      if (!feature.initialized) {
-        featureTrackToResidualize<_S> q;
-        q.feature_id = feature.feature_id;
-        q.observations = feature.observations;
-        for (size_t pos = 0; pos < cam_states_.size(); ++pos)
-          if (std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), (size_t)cam_states_[pos].state_id) !=
-              feature.cam_state_indices.end())
-            q.cam_state_indices.push_back(pos);
-        if (q.cam_state_indices.size() != q.observations.size())
-          throw std::logic_error("pruneRedundantStates: observations and associated clones differ in number");
-        tri_feat.push_back(fi);
-        tri_involved.push_back(involved);
-        tri_batch.push_back(q);
-      }
-    }
-    if (!tri_batch.empty()) {
-      msckf_b200_tracks tr;
-      packTracks(tri_batch, nullptr, tr);
-      const int N = (int)tri_batch.size();
-      rp_cm_.resize(N); rp_tri_.resize(N); rp_pfg_.resize(3 * (size_t)N);
-      msckf_b200_report rep = {};
-      rep.cm_ok = rp_cm_.data(); rep.tri_ok = rp_tri_.data(); rep.p_f_G = rp_pfg_.data();
+    msckf_b200_tracks tr;
+    msckf_b200_report rep = {};
+    if (redundantTriangulatePrepare(tr, rep, true)) {
       check(msckf_b200_update(eng(), MSCKF_B200_TRIANGULATE, &tr, &rep), "msckf_b200_update(TRIANGULATE)");
-      for (int k = 0; k < N; ++k) {
-        auto& feature = feature_tracks_[tri_feat[k]];
-        // checkMotion on fewer than two clones is false (ref :982-984)
-        const bool cm = tri_batch[k].cam_state_indices.size() >= 2 && rp_cm_[k];
-        if (!cm || !rp_tri_[k]) {
-          for (const auto& cam_id : tri_involved[k]) {
-            auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
-            if (it != feature.cam_state_indices.end()) {
-              const size_t oi = std::distance(feature.cam_state_indices.begin(), it);
-              feature.cam_state_indices.erase(it);
-              feature.observations.erase(feature.observations.begin() + oi);
-            }
-          }
-        } else {
-          feature.initialized = true;
-          for (int c = 0; c < 3; ++c) feature.p_f_G(c) = rp_pfg_[3 * (size_t)k + c];
-          map_.push_back(feature.p_f_G);
-        }
-      }
+      redundantTriangulateAbsorb();
     }
-    // ---- second loop (ref :545-607): residualise the involved observations
-    std::vector<featureTrackToResidualize<_S>> batch;
-    for (auto& feature : feature_tracks_) {
-      std::vector<size_t> involved;
-      aligned_vector<Vector2<_S>> involved_obs;
-      for (const auto& cam_id : rm_cam_state_ids) {
-        auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
-        if (it != feature.cam_state_indices.end()) {
-          involved.push_back(cam_id);
-          involved_obs.push_back(feature.observations[std::distance(feature.cam_state_indices.begin(), it)]);
-        }
-      }
-      if (involved.size() == 0) continue;
-      featureTrackToResidualize<_S> q;
-      q.feature_id = feature.feature_id;
-      q.observations = involved_obs;
-      for (size_t pos = 0; pos < cam_states_.size(); ++pos)
-        if (std::find(involved.begin(), involved.end(), (size_t)cam_states_[pos].state_id) != involved.end()) q.cam_state_indices.push_back(pos);
-      q.initialized = true;
-      q.p_f_G = feature.p_f_G;
-      if (q.cam_state_indices.size() != q.observations.size())
-        throw std::logic_error("pruneRedundantStates: involved observations and clones differ in number");
-      batch.push_back(q);
-      for (const auto& cam_id : involved) {
-        auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
-        if (it != feature.cam_state_indices.end()) {
-          const size_t oi = std::distance(feature.cam_state_indices.begin(), it);
-          feature.cam_state_indices.erase(it);
-          feature.observations.erase(feature.observations.begin() + oi);
-        }
-      }
-    }
-    if (!batch.empty()) {
-      msckf_b200_tracks tr;
-      packTracks(batch, &batch, tr);
-      msckf_b200_report rep = {};
+    if (redundantResidualizePrepare(tr, true)) {
+      rep = msckf_b200_report();
       checkNumeric(msckf_b200_update(eng(), MSCKF_B200_RESIDUALIZE, &tr, &rep), "msckf_b200_update(RESIDUALIZE)");
-      if (rep.m > 0) epoch_++;
-      state_dirty_ = true;
+      redundantResidualizeAbsorb(rep);
     }
-    // ---- delete the clones (ref :616-681)
     refreshState();
     std::vector<int> keep;
-    std::vector<camState<_S>> kept;
-    for (size_t pos = 0; pos < cam_states_.size(); ++pos) {
-      if (std::find(rm_cam_state_ids.begin(), rm_cam_state_ids.end(), (size_t)cam_states_[pos].state_id) != rm_cam_state_ids.end())
-        pruned_states_.push_back(cam_states_[pos]);
-      else { keep.push_back((int)pos); kept.push_back(cam_states_[pos]); }
-    }
-    if (keep.size() != cam_states_.size()) {
-      check(msckf_b200_prune(eng(), keep.data(), (int)keep.size()), "msckf_b200_prune");
-      cam_states_.swap(kept);
-    }
+    if (redundantDeletePrepare(keep)) check(msckf_b200_prune(eng(), keep.data(), (int)keep.size()), "msckf_b200_prune");
   }
 
-  // ref :685-761
+  // ref :685-761.  Phases (shared with MSCKFBatch): how many leading clones go, then (with the poses refreshed) the bookkeeping.
   void pruneEmptyStates() {
-    const int max_states = msckf_params_.max_cam_states;
-    if ((int)cam_states_.size() < max_states) return;
-    const int num_cam_states = (int)cam_states_.size();
-    int last_to_remove = num_cam_states - max_states - 1;
-    if (cam_states_.front().tracked_feature_ids.size()) return;
-    for (int i = 1; i < num_cam_states - max_states; i++)
-      if (cam_states_[i].tracked_feature_ids.size()) { last_to_remove = i - 1; break; }
-    const int ndel = last_to_remove + 1;
+    const int ndel = emptyStatesToDelete();
     if (ndel <= 0) return;
     refreshState();
-    for (int i = 0; i < ndel; ++i) pruned_states_.push_back(cam_states_[i]);
-    cam_states_.erase(cam_states_.begin(), cam_states_.begin() + ndel);
     std::vector<int> keep;
-    for (int i = ndel; i < num_cam_states; ++i) keep.push_back(i);
+    emptyStatesDelete(ndel, keep);
     check(msckf_b200_prune(eng(), keep.data(), (int)keep.size()), "msckf_b200_prune");
   }
 
   // ref :765-807
   void finish() {
+    finishQueue();
+    marginalize();
+  }
+  // the queueing half of finish(): every remaining track joins the residualisation queue
+  void finishQueue() {
     for (size_t i = 0; i < tracked_feature_ids_.size(); i++) {
       std::vector<size_t> camStateIndices;
       removeTrackedFeature(tracked_feature_ids_[i], camStateIndices);
@@ -357,7 +260,6 @@ class MSCKF {
       tracks_to_remove_.push_back(tracked_feature_ids_[i]);
     }
     epoch_at_queue_ = epoch_;
-    marginalize();
   }
 
   // ---- getters (ref :810-848), all by value like the reference
@@ -436,6 +338,147 @@ class MSCKF {
     if (rep.m > 0) epoch_++;
     state_dirty_ = true;
   }
+  // pieces of pruneRedundantStates() (ref :453-682).  The clone poses must be current (refreshState) before the first
+  // Prepare and before DeletePrepare.  A Prepare returning false has nothing for the device.
+  bool redundantPruneWanted() const { return cam_states_.size() >= 20; }
+  // ref :464-534, first loop: drop single observations, queue the uninitialised features for checkMotion + initializePosition
+  bool redundantTriangulatePrepare(msckf_b200_tracks& tr, msckf_b200_report& rep, bool in_engine_buffer) {
+    rm_cam_state_ids_.clear();
+    tri_feat_.clear(); tri_involved_.clear(); tri_batch_.clear();
+    findRedundantCamStates(rm_cam_state_ids_);
+    const auto& rm_cam_state_ids = rm_cam_state_ids_;
+    for (size_t fi = 0; fi < feature_tracks_.size(); ++fi) {
+      auto& feature = feature_tracks_[fi];
+      std::vector<size_t> involved;
+      size_t obs_id = 0;
+      for (const auto& cam_id : rm_cam_state_ids) {
+        auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
+        if (it != feature.cam_state_indices.end()) { involved.push_back(cam_id); obs_id = std::distance(feature.cam_state_indices.begin(), it); }
+      }
+      if (involved.size() == 0) continue;
+      if (involved.size() == 1) {
+        feature.observations.erase(feature.observations.begin() + obs_id);
+        feature.cam_state_indices.erase(feature.cam_state_indices.begin() + obs_id);
+        continue;
+      }
+      if (!feature.initialized) {
+        featureTrackToResidualize<_S> q;
+        q.feature_id = feature.feature_id;
+        q.observations = feature.observations;
+        for (size_t pos = 0; pos < cam_states_.size(); ++pos)
+          if (std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), (size_t)cam_states_[pos].state_id) !=
+              feature.cam_state_indices.end())
+            q.cam_state_indices.push_back(pos);
+        if (q.cam_state_indices.size() != q.observations.size())
+          throw std::logic_error("pruneRedundantStates: observations and associated clones differ in number");
+        tri_feat_.push_back(fi);
+        tri_involved_.push_back(involved);
+        tri_batch_.push_back(q);
+      }
+    }
+    if (tri_batch_.empty()) return false;
+    packTracks(tri_batch_, nullptr, tr, in_engine_buffer);
+    const int N = (int)tri_batch_.size();
+    rp_cm_.resize(N); rp_tri_.resize(N); rp_pfg_.resize(3 * (size_t)N);
+    rep = msckf_b200_report();
+    rep.cm_ok = rp_cm_.data(); rep.tri_ok = rp_tri_.data(); rep.p_f_G = rp_pfg_.data();
+    return true;
+  }
+  void redundantTriangulateAbsorb() {
+    for (size_t k = 0; k < tri_batch_.size(); ++k) {
+      auto& feature = feature_tracks_[tri_feat_[k]];
+      // checkMotion on fewer than two clones is false (ref :982-984)
+      const bool cm = tri_batch_[k].cam_state_indices.size() >= 2 && rp_cm_[k];
+      if (!cm || !rp_tri_[k]) {
+        for (const auto& cam_id : tri_involved_[k]) {
+          auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
+          if (it != feature.cam_state_indices.end()) {
+            const size_t oi = std::distance(feature.cam_state_indices.begin(), it);
+            feature.cam_state_indices.erase(it);
+            feature.observations.erase(feature.observations.begin() + oi);
+          }
+        }
+      } else {
+        feature.initialized = true;
+        for (int c = 0; c < 3; ++c) feature.p_f_G(c) = rp_pfg_[3 * k + c];
+        map_.push_back(feature.p_f_G);
+      }
+    }
+  }
+  // ref :545-607, second loop: residualise the observations of the redundant clones
+  bool redundantResidualizePrepare(msckf_b200_tracks& tr, bool in_engine_buffer) {
+    const auto& rm_cam_state_ids = rm_cam_state_ids_;
+    res_batch_.clear();
+    for (auto& feature : feature_tracks_) {
+      std::vector<size_t> involved;
+      aligned_vector<Vector2<_S>> involved_obs;
+      for (const auto& cam_id : rm_cam_state_ids) {
+        auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
+        if (it != feature.cam_state_indices.end()) {
+          involved.push_back(cam_id);
+          involved_obs.push_back(feature.observations[std::distance(feature.cam_state_indices.begin(), it)]);
+        }
+      }
+      if (involved.size() == 0) continue;
+      featureTrackToResidualize<_S> q;
+      q.feature_id = feature.feature_id;
+      q.observations = involved_obs;
+      for (size_t pos = 0; pos < cam_states_.size(); ++pos)
+        if (std::find(involved.begin(), involved.end(), (size_t)cam_states_[pos].state_id) != involved.end()) q.cam_state_indices.push_back(pos);
+      q.initialized = true;
+      q.p_f_G = feature.p_f_G;
+      if (q.cam_state_indices.size() != q.observations.size())
+        throw std::logic_error("pruneRedundantStates: involved observations and clones differ in number");
+      res_batch_.push_back(q);
+      for (const auto& cam_id : involved) {
+        auto it = std::find(feature.cam_state_indices.begin(), feature.cam_state_indices.end(), cam_id);
+        if (it != feature.cam_state_indices.end()) {
+          const size_t oi = std::distance(feature.cam_state_indices.begin(), it);
+          feature.cam_state_indices.erase(it);
+          feature.observations.erase(feature.observations.begin() + oi);
+        }
+      }
+    }
+    if (res_batch_.empty()) return false;
+    packTracks(res_batch_, &res_batch_, tr, in_engine_buffer);
+    return true;
+  }
+  void redundantResidualizeAbsorb(const msckf_b200_report& rep) {
+    if (rep.m > 0) epoch_++;
+    state_dirty_ = true;
+  }
+  // ref :616-681: the bookkeeping of deleting the redundant clones; keep = surviving positions (false: none is deleted)
+  bool redundantDeletePrepare(std::vector<int>& keep) {
+    keep.clear();
+    std::vector<camState<_S>> kept;
+    for (size_t pos = 0; pos < cam_states_.size(); ++pos) {
+      if (std::find(rm_cam_state_ids_.begin(), rm_cam_state_ids_.end(), (size_t)cam_states_[pos].state_id) != rm_cam_state_ids_.end())
+        pruned_states_.push_back(cam_states_[pos]);
+      else { keep.push_back((int)pos); kept.push_back(cam_states_[pos]); }
+    }
+    if (keep.size() == cam_states_.size()) return false;
+    cam_states_.swap(kept);
+    return true;
+  }
+  // pieces of pruneEmptyStates() (ref :685-761): the number of leading clones to delete (<= 0: none), and the bookkeeping
+  // of deleting them (the poses must be current), which gives the positions that survive
+  int emptyStatesToDelete() const {
+    const int max_states = msckf_params_.max_cam_states;
+    if ((int)cam_states_.size() < max_states) return 0;
+    const int num_cam_states = (int)cam_states_.size();
+    int last_to_remove = num_cam_states - max_states - 1;
+    if (cam_states_.front().tracked_feature_ids.size()) return 0;
+    for (int i = 1; i < num_cam_states - max_states; i++)
+      if (cam_states_[i].tracked_feature_ids.size()) { last_to_remove = i - 1; break; }
+    return last_to_remove + 1;
+  }
+  void emptyStatesDelete(int ndel, std::vector<int>& keep) {
+    const int num_cam_states = (int)cam_states_.size();
+    for (int i = 0; i < ndel; ++i) pruned_states_.push_back(cam_states_[i]);
+    cam_states_.erase(cam_states_.begin(), cam_states_.begin() + ndel);
+    keep.clear();
+    for (int i = ndel; i < num_cam_states; ++i) keep.push_back(i);
+  }
 
  private:
   Camera<_S> camera_;
@@ -460,6 +503,10 @@ class MSCKF {
   int last_m_ = 0, last_rank_ = 0;
   std::vector<int> pk_off_, pk_idx_, rp_cm_, rp_tri_, rp_valid_, rp_acc_;
   std::vector<_S> pk_obs_, pk_pfg_, rp_gamma_, rp_pfg_;
+  // pruneRedundantStates() between its phases
+  std::vector<size_t> rm_cam_state_ids_, tri_feat_;
+  std::vector<std::vector<size_t>> tri_involved_;
+  std::vector<featureTrackToResidualize<_S>> tri_batch_, res_batch_;
 
   static void check(int rc, const char* what) {
     if (rc != 0) throw std::runtime_error(std::string(what) + " failed (" + std::to_string(rc) + "): " + msckf_b200_last_error());
@@ -537,6 +584,10 @@ class MSCKF {
     _S im[29];
     std::vector<_S> poses(7 * std::max<size_t>(cam_states_.size(), 1));
     check(msckf_b200_get_state(eng(), im, poses.data()), "msckf_b200_get_state");
+    refreshAbsorb(im, poses.data());
+  }
+  // the host mirror from msckf_b200_get_state's layouts (imu: 29 scalars, poses: 7 per clone)
+  void refreshAbsorb(const _S* im, const _S* poses) const {
     for (int i = 0; i < 3; ++i) {
       imu_state_.p_I_G(i) = im[i]; imu_state_.v_I_G(i) = im[3 + i]; imu_state_.b_g(i) = im[6 + i]; imu_state_.b_a(i) = im[9 + i];
       imu_state_.g(i) = im[12 + i]; imu_state_.p_I_G_null(i) = im[19 + i]; imu_state_.v_I_G_null(i) = im[22 + i];
@@ -599,10 +650,13 @@ class MSCKF {
   }
 };
 
-// Not in the reference: marginalize() on several independent filters (sequences, Monte-Carlo trials) as ONE device batch --
-// one launch per kernel with the filter index in blockIdx.z, one CUDA graph, one packed copy each way
-// (msckf_b200_batch_* in include/msckf_b200.h).  Results are bit-identical to calling marginalize() on each filter.
-// While the object lives the filters share its CUDA stream; all their other member functions stay usable.
+// Not in the reference: the per-image step of several independent filters (sequences, Monte-Carlo trials) as ONE device
+// batch -- one launch per kernel with the filter index in the block index, one packed copy each way (msckf_b200_batch_* in
+// include/msckf_b200.h).  The member functions below mean what MSCKF's members of the same name mean, applied to every
+// filter; each filter ends bit-identical to calling them filter by filter.  The IMU readings queued by propagate() (here or
+// on the filters themselves) go to the device in one call before any batched device call.  update() and addFeatures() are
+// host bookkeeping only and stay per filter.  While the object lives the filters share its CUDA stream; all their own member
+// functions stay usable.
 template <typename _S>
 class MSCKFBatch {
  public:
@@ -615,23 +669,87 @@ class MSCKFBatch {
   ~MSCKFBatch() { if (batch_) msckf_b200_batch_destroy(batch_); }
   MSCKFBatch(const MSCKFBatch&) = delete;
   MSCKFBatch& operator=(const MSCKFBatch&) = delete;
+  size_t size() const { return filters_.size(); }
+
+  // MSCKF::propagate of filter i (queued on the host like there)
+  void propagate(size_t i, imuReading<_S>& reading) { filters_.at(i)->propagate(reading); }
+  // MSCKF::augmentState of every filter: state_ids[i] / times[i] for filter i
+  void augmentState(const std::vector<int>& state_ids, const std::vector<_S>& times) {
+    if (state_ids.size() != size() || times.size() != size()) throw std::invalid_argument("MSCKFBatch::augmentState: one state id and time per filter");
+    flushImu();
+    MSCKF<_S>::check(msckf_b200_batch_augment(batch_, nullptr), "msckf_b200_batch_augment");
+    for (size_t i = 0; i < size(); ++i) filters_[i]->augmentAbsorb(state_ids[i], times[i]);
+  }
   void marginalize() {
-    const size_t n = filters_.size();
-    tracks_.assign(n, msckf_b200_tracks());
-    reports_.assign(n, msckf_b200_report());
-    active_.assign(n, 0);
+    const size_t n = size();
+    flushImu();
+    resetUpdate();
     bool any = false;
     for (size_t i = 0; i < n; ++i) {
-      filters_[i]->engine();  // hand queued IMU readings over before the batch runs
       active_[i] = filters_[i]->marginalizePrepare(tracks_[i], false) ? 1 : 0;
-      if (active_[i]) { filters_[i]->marginalizeReport(reports_[i]); any = true; } else tracks_[i].n_tracks = 0;
+      if (active_[i]) { filters_[i]->marginalizeReport(reports_[i]); any = true; }
     }
     if (!any) return;
-    const int rc = msckf_b200_batch_update(batch_, MSCKF_B200_MARGINALIZE, tracks_.data(), reports_.data(), threads_);
-    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch update: " << msckf_b200_last_error() << std::endl;
-    else if (rc != 0) throw std::runtime_error(std::string("msckf_b200_batch_update failed: ") + msckf_b200_last_error());
+    runUpdate(MSCKF_B200_MARGINALIZE);
     for (size_t i = 0; i < n; ++i)
       if (active_[i]) filters_[i]->marginalizeAbsorb(reports_[i]);
+  }
+  void pruneRedundantStates() {
+    const size_t n = size();
+    std::vector<char> wanted(n, 0);
+    bool any = false;
+    for (size_t i = 0; i < n; ++i) any |= (wanted[i] = filters_[i]->redundantPruneWanted() ? 1 : 0) != 0;
+    if (!any) return;
+    flushImu();
+    refresh(wanted);
+    resetUpdate();
+    any = false;
+    for (size_t i = 0; i < n; ++i)
+      if (wanted[i]) any |= (active_[i] = filters_[i]->redundantTriangulatePrepare(tracks_[i], reports_[i], false) ? 1 : 0) != 0;
+    if (any) {
+      runUpdate(MSCKF_B200_TRIANGULATE);
+      for (size_t i = 0; i < n; ++i) if (active_[i]) filters_[i]->redundantTriangulateAbsorb();
+    }
+    resetUpdate();
+    any = false;
+    for (size_t i = 0; i < n; ++i)
+      if (wanted[i]) any |= (active_[i] = filters_[i]->redundantResidualizePrepare(tracks_[i], false) ? 1 : 0) != 0;
+    if (any) {
+      runUpdate(MSCKF_B200_RESIDUALIZE);
+      for (size_t i = 0; i < n; ++i) if (active_[i]) filters_[i]->redundantResidualizeAbsorb(reports_[i]);
+    }
+    refresh(wanted);
+    keep_.assign(n, std::vector<int>());
+    std::vector<int> n_keep(n, -1);
+    any = false;
+    for (size_t i = 0; i < n; ++i)
+      if (wanted[i] && filters_[i]->redundantDeletePrepare(keep_[i])) { n_keep[i] = (int)keep_[i].size(); any = true; }
+    if (any) prune(n_keep);
+  }
+  void pruneEmptyStates() {
+    const size_t n = size();
+    std::vector<int> ndel(n, 0);
+    std::vector<char> wanted(n, 0);
+    bool any = false;
+    for (size_t i = 0; i < n; ++i) any |= (wanted[i] = (ndel[i] = filters_[i]->emptyStatesToDelete()) > 0 ? 1 : 0) != 0;
+    if (!any) return;
+    flushImu();
+    refresh(wanted);
+    keep_.assign(n, std::vector<int>());
+    std::vector<int> n_keep(n, -1);
+    for (size_t i = 0; i < n; ++i)
+      if (wanted[i]) { filters_[i]->emptyStatesDelete(ndel[i], keep_[i]); n_keep[i] = (int)keep_[i].size(); }
+    prune(n_keep);
+  }
+  void finish() {
+    for (auto* f : filters_) f->finishQueue();
+    marginalize();
+  }
+  // brings every filter's host mirror of the IMU state and clone poses up to date with one synchronisation, so that the
+  // getters after a batched step do not synchronise filter by filter
+  void refreshState() {
+    flushImu();
+    refresh(std::vector<char>(size(), 1));
   }
   msckf_b200_batch* handle() { return batch_; }
 
@@ -640,8 +758,59 @@ class MSCKFBatch {
   std::vector<msckf_b200_tracks> tracks_;
   std::vector<msckf_b200_report> reports_;
   std::vector<char> active_;
+  std::vector<std::vector<int>> keep_;
   msckf_b200_batch* batch_ = nullptr;
   int threads_ = 1;
+
+  // the IMU readings queued on every filter, as one msckf_b200_batch_propagate_n
+  void flushImu() {
+    const size_t n = size();
+    std::vector<const void*> r(n, nullptr);
+    std::vector<int> k(n, 0);
+    bool any = false;
+    for (size_t i = 0; i < n; ++i) {
+      k[i] = (int)(filters_[i]->imu_queue_.size() / 7);
+      r[i] = filters_[i]->imu_queue_.data();
+      any |= k[i] > 0;
+    }
+    if (!any) return;
+    const int rc = msckf_b200_batch_propagate_n(batch_, r.data(), k.data());
+    for (auto* f : filters_) f->imu_queue_.clear();
+    MSCKF<_S>::check(rc, "msckf_b200_batch_propagate_n");
+  }
+  // MSCKF::refreshState of the filters with which[i] whose mirror is stale, as one msckf_b200_batch_get_state
+  void refresh(const std::vector<char>& which) {
+    const size_t n = size();
+    std::vector<std::vector<_S>> im(n), poses(n);
+    std::vector<void*> pi(n, nullptr), pp(n, nullptr);
+    bool any = false;
+    for (size_t i = 0; i < n; ++i) {
+      if (!which[i] || !filters_[i]->state_dirty_) continue;
+      im[i].resize(29);
+      poses[i].resize(7 * std::max<size_t>(filters_[i]->cam_states_.size(), 1));
+      pi[i] = im[i].data(); pp[i] = poses[i].data();
+      any = true;
+    }
+    if (!any) return;
+    MSCKF<_S>::check(msckf_b200_batch_get_state(batch_, pi.data(), pp.data()), "msckf_b200_batch_get_state");
+    for (size_t i = 0; i < n; ++i)
+      if (pi[i]) filters_[i]->refreshAbsorb(im[i].data(), poses[i].data());
+  }
+  void resetUpdate() {
+    tracks_.assign(size(), msckf_b200_tracks());  // (n_tracks = 0: a member with nothing to do)
+    reports_.assign(size(), msckf_b200_report());
+    active_.assign(size(), 0);
+  }
+  void runUpdate(int mode) {
+    const int rc = msckf_b200_batch_update(batch_, mode, tracks_.data(), reports_.data(), threads_);
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch update: " << msckf_b200_last_error() << std::endl;
+    else if (rc != 0) throw std::runtime_error(std::string("msckf_b200_batch_update failed: ") + msckf_b200_last_error());
+  }
+  void prune(const std::vector<int>& n_keep) {
+    std::vector<const int*> kp(size());
+    for (size_t i = 0; i < size(); ++i) kp[i] = keep_[i].data();
+    MSCKF<_S>::check(msckf_b200_batch_prune(batch_, kp.data(), n_keep.data()), "msckf_b200_batch_prune");
+  }
 };
 
 }  // namespace msckf_mono

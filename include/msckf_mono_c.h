@@ -54,6 +54,15 @@ int msckf_mono_marginalize_collect(void* h);
 int msckf_mono_batch_create(void** handles, int n, int threads, void** out);
 void msckf_mono_batch_destroy(void* batch);
 int msckf_mono_batch_marginalize(void* batch);
+/* the rest of the per-image step on every filter of the batch, same meaning as the single-filter calls above; each device
+ * operation is one batched call (datasets/asl_msckf.cpp:233-294 for n filters) */
+int msckf_mono_batch_propagate(void* batch, int member, const double* omega_a_dT);             /* msckf.h:101, filter `member` */
+int msckf_mono_batch_augment_state(void* batch, const int* state_ids, const double* times);    /* msckf.h:148, one per filter */
+int msckf_mono_batch_prune_empty_states(void* batch);                                          /* msckf.h:685 */
+int msckf_mono_batch_prune_redundant_states(void* batch);                                      /* msckf.h:453 */
+int msckf_mono_batch_finish(void* batch);                                                      /* msckf.h:765 */
+/* every filter's IMU state and clone poses fetched with one synchronisation (the getters then read the host mirror) */
+int msckf_mono_batch_refresh_state(void* batch);
 void* msckf_mono_batch_handle(void* batch); /* the msckf_b200_batch* beneath */
 int msckf_mono_marginalize_batch(void** handles, int n, int threads);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */

@@ -136,6 +136,37 @@ class Batch:
     def launch_count(self):
         return int(lib().msckf_b200_batch_launch_count(self.h))
 
+    def propagate_n(self, readings):
+        """msckf_b200_batch_propagate_n: readings[i] = [k_i, 7] array (k_i may be 0) for engine i"""
+        n = len(self.engines)
+        assert len(readings) == n
+        rs = [np.ascontiguousarray(r, dtype=e.dtype).reshape(-1, 7) for r, e in zip(readings, self.engines)]
+        ptrs = (C.c_void_p * n)(*[r.ctypes.data if len(r) else None for r in rs])
+        k = (C.c_int * n)(*[len(r) for r in rs])
+        check(lib().msckf_b200_batch_propagate_n(self.h, ptrs, k), "msckf_b200_batch_propagate_n")
+
+    def augment(self, which=None):
+        """msckf_b200_batch_augment for the engines with which[i] (None: all)"""
+        w = None if which is None else (C.c_int * len(self.engines))(*[int(bool(x)) for x in which])
+        check(lib().msckf_b200_batch_augment(self.h, w), "msckf_b200_batch_augment")
+
+    def prune(self, keeps):
+        """msckf_b200_batch_prune: keeps[i] = ascending positions to keep, or None (engine i untouched)"""
+        n = len(self.engines)
+        ks = [None if k is None else np.ascontiguousarray(k, dtype=np.int32) for k in keeps]
+        ptrs = (C.POINTER(C.c_int) * n)(*[None if k is None else k.ctypes.data_as(C.POINTER(C.c_int)) for k in ks])
+        nk = (C.c_int * n)(*[-1 if k is None else len(k) for k in ks])
+        check(lib().msckf_b200_batch_prune(self.h, ptrs, nk), "msckf_b200_batch_prune")
+
+    def state(self):
+        """msckf_b200_batch_get_state: [(imu [29], clone poses [M, 7])] per engine, with one synchronisation"""
+        n = len(self.engines)
+        out = [(np.zeros(29, dtype=e.dtype), np.zeros((e.num_clones(), 7), dtype=e.dtype)) for e in self.engines]
+        imu = (C.c_void_p * n)(*[o[0].ctypes.data for o in out])
+        poses = (C.c_void_p * n)(*[o[1].ctypes.data if o[1].size else None for o in out])
+        check(lib().msckf_b200_batch_get_state(self.h, imu, poses), "msckf_b200_batch_get_state")
+        return out
+
     def jac_occupancy(self):
         """CTAs of k_jac resident per SM at the shape of the last launch (0 before the first)."""
         return int(lib().msckf_b200_batch_jac_occupancy(self.h))

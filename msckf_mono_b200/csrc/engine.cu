@@ -115,6 +115,11 @@ struct CtxBase {
   virtual void detach(EngineBase* e) = 0;
   virtual int count() const = 0;
   virtual EngineBase* member(int i) const = 0;
+  // the state calls of every member as one launch per kernel (msckf_b200_batch_propagate_n / _augment / _prune / _get_state)
+  virtual int propagate_n(const void* const* readings, const int* k) = 0;
+  virtual int augment(const int* which) = 0;
+  virtual int prune(const int* const* keep, const int* n_keep) = 0;
+  virtual int get_state(void* const* imu, void* const* poses) = 0;
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
@@ -275,6 +280,7 @@ struct Ctx : CtxBase {
   std::vector<Engine<S>*> eng;
   std::vector<Plan<S>> plan;
   Arena in, rep;
+  Arena poses_out;  // clone poses of a batched get_state (pinned: all members' copies are asynchronous)
   size_t in_used = 0, rep_used = 0;
   int device = 0;
   bool owns_stream = false;
@@ -310,7 +316,7 @@ struct Ctx : CtxBase {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     drop_graphs();
-    in.release(); rep.release();
+    in.release(); rep.release(); poses_out.release();
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
@@ -346,6 +352,11 @@ struct Ctx : CtxBase {
   int run_kernels(const LaunchShape& sh);
   int launch_timed(float* ms) override;
   int fetch(msckf_b200_report* reports) override;
+  int members_ready(const char* what) const;
+  int propagate_n(const void* const* readings, const int* k) override;
+  int augment(const int* which) override;
+  int prune(const int* const* keep, const int* n_keep) override;
+  int get_state(void* const* imu, void* const* poses) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
@@ -592,16 +603,20 @@ struct Engine : EngineBase {
     const S* r = (const S*)r_;
     CK(cudaSetDevice(device));
     for (int k0 = 0; k0 < k; k0 += mb::kPropMax) {
-      mb::PropBatch<S> pb;
-      pb.st = d_st; pb.P = d_P; pb.ldp = ldp; pb.M = M; pb.k = std::min(mb::kPropMax, k - k0); pb.pad_ = 0;
-      pb.prof = profile ? d_prof : nullptr;
-      for (int i = 0; i < pb.k; ++i)
-        for (int j = 0; j < 7; ++j) pb.r[i][j] = r[7 * (size_t)(k0 + i) + j];
-      mb::k_propagate<S><<<1, 256, 0, stream>>>(pb);
+      mb::Members<mb::PropBatch<S>, 1> a;
+      prop_args(a.m[0], r, k0, std::min(mb::kPropMax, k - k0));
+      mb::k_propagate<S, 1><<<1, 256, 0, stream>>>(a);
       launches++;
     }
     CK(cudaGetLastError());
     return 0;
+  }
+  // k_propagate's arguments for readings k0 .. k0 + n - 1 of r (n <= kPropMax)
+  void prop_args(mb::PropBatch<S>& pb, const S* r, int k0, int n) const {
+    pb.st = d_st; pb.P = d_P; pb.ldp = ldp; pb.M = M; pb.k = n; pb.pad_ = 0;
+    pb.prof = profile ? d_prof : nullptr;
+    for (int i = 0; i < n; ++i)
+      for (int j = 0; j < 7; ++j) pb.r[i][j] = r[7 * (size_t)(k0 + i) + j];
   }
 
   int augment() override {
@@ -609,12 +624,15 @@ struct Engine : EngineBase {
     if (busy) return fail(MSCKF_B200_ERR_STATE, "augment with an un-fetched update pending");
     RC(ensure_clones(M + 1));
     CK(cudaSetDevice(device));
-    mb::k_augment<S><<<1, 256, 0, stream>>>(d_st, d_P, ldp, M, d_poses);
+    mb::Members<mb::AugArgs<S>, 1> a;
+    a.m[0] = aug_args();
+    mb::k_augment<S, 1><<<1, 256, 0, stream>>>(a);
     launches++;
     CK(cudaGetLastError());
     M += 1;
     return 0;
   }
+  mb::AugArgs<S> aug_args() const { return {d_st, d_P, d_poses, ldp, M}; }
 
   // everything the kernels need for this filter's slice of the update
   void fill_args(mb::UpdArgs<S>& a, const Plan<S>& p, int mode) const {
@@ -656,35 +674,58 @@ struct Engine : EngineBase {
   }
 
   int prune(const int* keep, int n_keep) override {
+    RC(prune_check(keep, n_keep));
+    if (n_keep == M) return 0;
+    CK(cudaSetDevice(device));
+    mb::Members<mb::GatherArgs<S>, 1> g;
+    gather_args(g.m[0], keep, n_keep);
+    mb::k_gather<S, 1><<<gather_grid(n_keep), 256, 0, stream>>>(g);
+    launches++;
+    CK(cudaGetLastError());
+    prune_swap(n_keep);
+    return 0;
+  }
+  int prune_check(const int* keep, int n_keep) const {
     if (n_keep < 0 || n_keep > M) return fail(MSCKF_B200_ERR_ARG, "prune: bad keep count");
     if (n_keep > 0 && !keep) return fail(MSCKF_B200_ERR_ARG, "prune: null keep list");
     if (busy) return fail(MSCKF_B200_ERR_STATE, "prune with an un-fetched update pending");
     for (int i = 0; i < n_keep; ++i)
       if (keep[i] < 0 || keep[i] >= M || (i && keep[i] <= keep[i - 1])) return fail(MSCKF_B200_ERR_ARG, "prune: keep[] must be ascending positions");
-    if (n_keep == M) return 0;
-    CK(cudaSetDevice(device));
-    mb::KeepList kl;
-    kl.n = n_keep;
-    for (int i = 0; i < n_keep; ++i) kl.idx[i] = keep[i];
+    return 0;
+  }
+  int gather_grid(int n_keep) const {
     const int n_new = 15 + 6 * n_keep;
-    mb::k_gather<S><<<std::min(2 * num_sms(device), (n_new * n_new + 255) / 256), 256, 0, stream>>>(n_new, kl, d_P, d_P2, ldp, d_poses, d_poses2);
-    launches++;
-    CK(cudaGetLastError());
+    return std::min(2 * num_sms(device), (n_new * n_new + 255) / 256);
+  }
+  void gather_args(mb::GatherArgs<S>& g, const int* keep, int n_keep) const {
+    g.Pold = d_P; g.Pnew = d_P2; g.poses_old = d_poses; g.poses_new = d_poses2;
+    g.n_new = 15 + 6 * n_keep; g.ldp = ldp;
+    g.kl.n = n_keep;
+    for (int i = 0; i < n_keep; ++i) g.kl.idx[i] = keep[i];
+  }
+  void prune_swap(int n_keep) {
     std::swap(d_P, d_P2);      // (buffer addresses ride in UpdArgs, not in captured kernel arguments:
     std::swap(d_poses, d_poses2);  //  no synchronisation, and captured graphs stay valid)
     M = n_keep;
-    return 0;
   }
 
   int get_state(void* imu_, void* poses_) override {
     CK(cudaSetDevice(device));
     std::vector<S> tmp;
-    if (imu_) CK(cudaMemcpyAsync(h_st, d_st, sizeof(mb::DevState<S>), cudaMemcpyDeviceToHost, stream));
-    if (poses_ && M > 0) {
-      tmp.resize((size_t)mb::kPoseStride * M);
-      CK(cudaMemcpyAsync(tmp.data(), d_poses, sizeof(S) * tmp.size(), cudaMemcpyDeviceToHost, stream));
-    }
+    if (poses_ && M > 0) tmp.resize((size_t)mb::kPoseStride * M);
+    RC(state_copy(imu_ != nullptr, tmp.empty() ? nullptr : tmp.data()));
     CK(cudaStreamSynchronize(stream));  // one synchronisation for both copies
+    state_unpack(imu_, poses_, tmp.data());
+    return 0;
+  }
+  // get_state in two halves: enqueue the copies (IMU state into h_st, kPoseStride * M clone-pose scalars into raw_poses),
+  // and, once the stream has been synchronised, convert them into the C-ABI's layouts
+  int state_copy(bool imu, S* raw_poses) {
+    if (imu) CK(cudaMemcpyAsync(h_st, d_st, sizeof(mb::DevState<S>), cudaMemcpyDeviceToHost, stream));
+    if (raw_poses && M > 0) CK(cudaMemcpyAsync(raw_poses, d_poses, sizeof(S) * mb::kPoseStride * M, cudaMemcpyDeviceToHost, stream));
+    return 0;
+  }
+  void state_unpack(void* imu_, void* poses_, const S* raw_poses) const {
     if (imu_) {
       S* o = (S*)imu_;
       const mb::DevState<S>& s = *h_st;
@@ -697,12 +738,11 @@ struct Engine : EngineBase {
     if (poses_ && M > 0) {
       S* o = (S*)poses_;
       for (int k = 0; k < M; ++k) {
-        const S* p = tmp.data() + mb::kPoseStride * k;
+        const S* p = raw_poses + mb::kPoseStride * k;
         o[7 * k] = p[4]; o[7 * k + 1] = p[5]; o[7 * k + 2] = p[6];
         o[7 * k + 3] = p[0]; o[7 * k + 4] = p[1]; o[7 * k + 5] = p[2]; o[7 * k + 6] = p[3];
       }
     }
-    return 0;
   }
 
   int get_covariance(void* out) override {
@@ -1142,6 +1182,119 @@ int Ctx<S>::fetch(msckf_b200_report* reports) {
   if (status != 0) return fail(status, "non-finite delta-x or covariance after the update (the update has been applied, like msckf.h:1369-1418 would), or the tail kernel's two chain CTAs lost their hand-off");
   return 0;
 }
+
+// ---- batched state calls.  Every member is validated before anything is launched, so a bad argument changes no member.
+// Members' arguments travel by value, mb::kBatchMembers per launch (one launch per chunk past that): no staging buffer, no
+// host synchronisation.  A member runs exactly the kernel body and arguments of its single-filter call.
+template <class S>
+int Ctx<S>::members_ready(const char* what) const {
+  for (auto* e : eng) {
+    if (!e) return fail(MSCKF_B200_ERR_STATE, "a member engine of this batch was destroyed");
+    if (!e->initialized) return fail(MSCKF_B200_ERR_STATE, std::string(what) + " before initialize");
+    if (e->busy) return fail(MSCKF_B200_ERR_STATE, std::string(what) + " with an un-fetched update pending");
+  }
+  return 0;
+}
+
+template <class S>
+int Ctx<S>::propagate_n(const void* const* readings, const int* k) {
+  RC(members_ready("batch_propagate_n"));
+  const int nf = (int)eng.size();
+  int kmax = 0;
+  for (int i = 0; i < nf; ++i) {
+    const int ki = k ? k[i] : 0;
+    if (ki < 0 || (ki > 0 && (!readings || !readings[i]))) return fail(MSCKF_B200_ERR_ARG, "batch_propagate_n: bad arguments");
+    kmax = std::max(kmax, ki);
+  }
+  CK(cudaSetDevice(device));
+  std::vector<int> idx;
+  // the same split into kPropMax readings per launch as propagate_n: step k0 runs every member with more than k0 readings
+  for (int k0 = 0; k0 < kmax; k0 += mb::kPropMax) {
+    idx.clear();
+    for (int i = 0; i < nf; ++i) if (k[i] > k0) idx.push_back(i);
+    for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
+      const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
+      mb::Members<mb::PropBatch<S>, mb::kBatchMembers> a;
+      for (int j = 0; j < nm; ++j) {
+        const int i = idx[c + j];
+        eng[i]->prop_args(a.m[j], (const S*)readings[i], k0, std::min(mb::kPropMax, k[i] - k0));
+        eng[i]->launches++;
+      }
+      mb::k_propagate<S, mb::kBatchMembers><<<nm, 256, 0, stream>>>(a);
+      launches++;
+    }
+  }
+  CK(cudaGetLastError());
+  return 0;
+}
+
+template <class S>
+int Ctx<S>::augment(const int* which) {
+  RC(members_ready("batch_augment"));
+  std::vector<int> idx;
+  for (int i = 0; i < (int)eng.size(); ++i) {
+    if (which && !which[i]) continue;
+    if (eng[i]->M + 1 > kMaxClonesHard) return fail(MSCKF_B200_ERR_CAPACITY, "sliding window exceeds the engine's hard limit of " + std::to_string(kMaxClonesHard) + " clones");
+    idx.push_back(i);
+  }
+  for (int i : idx) RC(eng[i]->ensure_clones(eng[i]->M + 1));
+  CK(cudaSetDevice(device));
+  for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
+    const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
+    mb::Members<mb::AugArgs<S>, mb::kBatchMembers> a;
+    for (int j = 0; j < nm; ++j) { a.m[j] = eng[idx[c + j]]->aug_args(); eng[idx[c + j]]->launches++; }
+    mb::k_augment<S, mb::kBatchMembers><<<nm, 256, 0, stream>>>(a);
+    launches++;
+  }
+  CK(cudaGetLastError());
+  for (int i : idx) eng[i]->M += 1;
+  return 0;
+}
+
+template <class S>
+int Ctx<S>::prune(const int* const* keep, const int* n_keep) {
+  RC(members_ready("batch_prune"));
+  if (!n_keep) return fail(MSCKF_B200_ERR_ARG, "batch_prune: null n_keep");
+  std::vector<int> idx;  // members whose window changes
+  for (int i = 0; i < (int)eng.size(); ++i) {
+    if (n_keep[i] < 0 || n_keep[i] == eng[i]->M) continue;
+    RC(eng[i]->prune_check(keep ? keep[i] : nullptr, n_keep[i]));
+    idx.push_back(i);
+  }
+  CK(cudaSetDevice(device));
+  for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
+    const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
+    mb::Members<mb::GatherArgs<S>, mb::kBatchMembers> g;
+    int gx = 1;  // the largest member's grid; smaller members' CTAs past their own grid-stride range exit at once
+    for (int j = 0; j < nm; ++j) {
+      const int i = idx[c + j];
+      eng[i]->gather_args(g.m[j], keep[i], n_keep[i]);
+      gx = std::max(gx, eng[i]->gather_grid(n_keep[i]));
+      eng[i]->launches++;
+    }
+    mb::k_gather<S, mb::kBatchMembers><<<dim3(gx, nm), 256, 0, stream>>>(g);
+    launches++;
+  }
+  CK(cudaGetLastError());
+  for (int i : idx) eng[i]->prune_swap(n_keep[i]);
+  return 0;
+}
+
+template <class S>
+int Ctx<S>::get_state(void* const* imu, void* const* poses) {
+  RC(members_ready("batch_get_state"));
+  const int nf = (int)eng.size();
+  std::vector<size_t> off(nf + 1, 0);
+  for (int i = 0; i < nf; ++i) off[i + 1] = off[i] + (poses && poses[i] ? up16(sizeof(S) * mb::kPoseStride * eng[i]->M) : 0);
+  RC(poses_out.ensure(off[nf], stream));
+  CK(cudaSetDevice(device));
+  for (int i = 0; i < nf; ++i)
+    RC(eng[i]->state_copy(imu && imu[i], off[i + 1] > off[i] ? reinterpret_cast<S*>(poses_out.h + off[i]) : nullptr));
+  CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
+  for (int i = 0; i < nf; ++i)
+    eng[i]->state_unpack(imu ? imu[i] : nullptr, off[i + 1] > off[i] ? poses[i] : nullptr, reinterpret_cast<S*>(poses_out.h + off[i]));
+  return 0;
+}
 }  // namespace
 
 struct msckf_b200_engine { EngineBase* impl; };
@@ -1278,6 +1431,22 @@ int msckf_b200_batch_kernel_times(msckf_b200_batch* b, float* ms, const char** n
 long long msckf_b200_batch_launch_count(const msckf_b200_batch* b) { return b->ctx->launches; }
 int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b) { return b->ctx->jac_ctas; }
 void* msckf_b200_batch_stream(msckf_b200_batch* b) { return (void*)b->ctx->stream; }
+int msckf_b200_batch_propagate_n(msckf_b200_batch* b, const void* const* readings, const int* k) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->propagate_n(readings, k);
+}
+int msckf_b200_batch_augment(msckf_b200_batch* b, const int* which) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->augment(which);
+}
+int msckf_b200_batch_prune(msckf_b200_batch* b, const int* const* keep, const int* n_keep) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->prune(keep, n_keep);
+}
+int msckf_b200_batch_get_state(msckf_b200_batch* b, void* const* imu, void* const* clone_poses) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->get_state(imu, clone_poses);
+}
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,
                             int threads) {

@@ -8,43 +8,15 @@
 #include <vector>
 #include <msckf_mono/msckf.h>
 #include <msckf_mono_c.h>
+#include "filter_view.hpp"
 
 using namespace msckf_mono;
-namespace {
+namespace msckf_view {
 thread_local std::string g_err;
+}  // namespace msckf_view
+using namespace msckf_view;
 
-struct Base {
-  virtual ~Base() {}
-  virtual void set_engine_options(int, int, int, int) = 0;
-  virtual void initialize(const double*, const double*, const double*, const double*) = 0;
-  virtual void propagate(const double*) = 0;
-  virtual void augment(int, double) = 0;
-  virtual void update(const double*, const uint64_t*, int) = 0;
-  virtual void add(const double*, const uint64_t*, int) = 0;
-  virtual void marginalize() = 0;
-  virtual void marginalize_launch() = 0;
-  virtual void marginalize_collect() = 0;
-  virtual void prune_redundant() = 0;
-  virtual void prune_empty() = 0;
-  virtual void finish() = 0;
-  virtual int num_cam() = 0;
-  virtual void imu_state(double*) = 0;
-  virtual void cam_states(double*, int*, double*) = 0;
-  virtual int cam_tracked(int, uint64_t*, int) = 0;
-  virtual int covariance(double*) = 0;
-  virtual int map(double*, int) = 0;
-  virtual int pruned(double*, int*, int) = 0;
-  virtual int tracked_ids(uint64_t*, int) = 0;
-  virtual int report(int*, double*, double*, int) = 0;
-  virtual int queued(uint64_t*, int*, int) = 0;
-  virtual int pack_queued(int*, double*, int*, int, int) = 0;
-  virtual msckf_b200_engine* engine() = 0;
-  virtual void* filter_ptr() = 0;
-  virtual int last_m() = 0;
-  virtual int last_rank() = 0;
-  int dtype = 0;
-};
-
+namespace {
 template <class S>
 struct Impl : Base {
   MSCKF<S> f;
@@ -177,16 +149,6 @@ struct Impl : Base {
   int last_m() override { return f.lastStackedRows(); }
   int last_rank() override { return f.lastRank(); }
 };
-
-template <class F>
-int guard(F&& fn) {
-  try {
-    return fn();
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return -1;
-  }
-}
 }  // namespace
 
 #define H ((Base*)h)
@@ -210,58 +172,6 @@ int msckf_mono_add_features(void* h, const double* z, const uint64_t* ids, int n
 int msckf_mono_marginalize(void* h) { return guard([&] { H->marginalize(); return 0; }); }
 int msckf_mono_marginalize_launch(void* h) { return guard([&] { H->marginalize_launch(); return 0; }); }
 int msckf_mono_marginalize_collect(void* h) { return guard([&] { H->marginalize_collect(); return 0; }); }
-// a persistent device batch over n filters of one scalar type (msckf_mono::MSCKFBatch<_S>)
-struct ViewBatch {
-  int dtype = 0;
-  MSCKFBatch<float>* bf = nullptr;
-  MSCKFBatch<double>* bd = nullptr;
-  ~ViewBatch() { delete bf; delete bd; }
-};
-int msckf_mono_batch_create(void** handles, int n, int threads, void** out) {
-  return guard([&] {
-    if (n <= 0 || !handles || !out) throw std::runtime_error("batch_create: bad arguments");
-    const int dtype = static_cast<Base*>(handles[0])->dtype;
-    auto* vb = new ViewBatch();
-    vb->dtype = dtype;
-    try {
-      if (dtype == 0) {
-        std::vector<MSCKF<float>*> fs;
-        for (int i = 0; i < n; ++i) { Base* b = static_cast<Base*>(handles[i]); if (b->dtype != dtype) throw std::runtime_error("batch_create: mixed scalar types"); fs.push_back(static_cast<MSCKF<float>*>(b->filter_ptr())); }
-        vb->bf = new MSCKFBatch<float>(fs, threads);
-      } else {
-        std::vector<MSCKF<double>*> fs;
-        for (int i = 0; i < n; ++i) { Base* b = static_cast<Base*>(handles[i]); if (b->dtype != dtype) throw std::runtime_error("batch_create: mixed scalar types"); fs.push_back(static_cast<MSCKF<double>*>(b->filter_ptr())); }
-        vb->bd = new MSCKFBatch<double>(fs, threads);
-      }
-    } catch (...) { delete vb; throw; }
-    *out = vb;
-    return 0;
-  });
-}
-void msckf_mono_batch_destroy(void* b) { delete static_cast<ViewBatch*>(b); }
-int msckf_mono_batch_marginalize(void* b) {
-  return guard([&] {
-    auto* vb = static_cast<ViewBatch*>(b);
-    if (vb->bf) vb->bf->marginalize(); else vb->bd->marginalize();
-    return 0;
-  });
-}
-void* msckf_mono_batch_handle(void* b) {
-  auto* vb = static_cast<ViewBatch*>(b);
-  return vb->bf ? (void*)vb->bf->handle() : (void*)vb->bd->handle();
-}
-// one-shot form: a temporary batch around one marginalize() of every filter
-int msckf_mono_marginalize_batch(void** handles, int n, int threads) {
-  if (n <= 0) return 0;
-  void* b = nullptr;
-  int rc = msckf_mono_batch_create(handles, n, threads, &b);
-  if (rc != 0) return rc;
-  rc = msckf_mono_batch_marginalize(b);
-  const std::string keep = g_err;
-  msckf_mono_batch_destroy(b);
-  g_err = keep;
-  return rc;
-}
 int msckf_mono_prune_redundant_states(void* h) { return guard([&] { H->prune_redundant(); return 0; }); }
 int msckf_mono_prune_empty_states(void* h) { return guard([&] { H->prune_empty(); return 0; }); }
 int msckf_mono_finish(void* h) { return guard([&] { H->finish(); return 0; }); }

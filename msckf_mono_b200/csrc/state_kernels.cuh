@@ -4,6 +4,7 @@
 //                 Phi = exp(F dT) with Eigen's Pade degree selection, observability constraints :116-132)
 //   k_augment   : msckf.h:148-212
 //   k_gather    : covariance slicing of pruneEmptyStates / pruneRedundantStates (matrix_utils.h:58-87)
+// Each runs one filter or, with the filter index in the block index, a device batch of filters (msckf_b200_batch_*).
 // Arithmetic is carried out in the filter precision _S like the reference.
 #pragma once
 #include "common.cuh"
@@ -86,9 +87,15 @@ __device__ __forceinline__ int warp_argmax_first(double v, bool active, int lane
   return (int)__reduce_min_sync(0xffffffffu, (c1 && lo == mlo) ? (unsigned)lane : 31u);
 }
 
-// Up to kPropMax IMU readings per launch (msckf_b200_propagate_n: the shim queues the readings between two images), passed
-// by value so that the call needs no staging buffer and stays asynchronous.  The readings are applied one after the other
-// with exactly the arithmetic of a single propagate() each.
+// The state kernels take their per-filter arguments by value, so that a call needs no staging buffer and no synchronisation.
+// One body serves a single filter (NM = 1) and a device batch (NM = kBatchMembers): the member is the block index (k_propagate,
+// k_augment: one CTA per member) or the grid row (k_gather).  A batch of more members runs as one launch per kBatchMembers.
+constexpr int kBatchMembers = 32;  // 32 fp64 propagate members are 29 952 B: under sm_90's 32 764 B of kernel parameters
+template <class T, int NM>
+struct Members { T m[NM]; };
+
+// Up to kPropMax IMU readings per launch and member (msckf_b200_propagate_n: the shim queues the readings between two images).
+// The readings are applied one after the other with exactly the arithmetic of a single propagate() each.
 constexpr int kPropMax = 16;
 template <class S>
 struct PropBatch {
@@ -98,21 +105,24 @@ struct PropBatch {
   unsigned long long* prof;  // optional %globaltimer stamps of the first reading's phases (profiling aid)
   S r[kPropMax][7];  // omega[3], a[3], dT
 };
+static_assert(sizeof(Members<PropBatch<double>, kBatchMembers>) <= 32764, "k_propagate's batched arguments exceed the parameter limit");
 
-template <class S>
-__global__ void __launch_bounds__(256) k_propagate(const PropBatch<S> pb) {
+template <class S, int NM>
+__global__ void __launch_bounds__(256) k_propagate(const Members<PropBatch<S>, NM> a) {
   // The IMU state, the 15 x 15 IMU block of P and (for windows up to 85 clones) the thread's columns of P_IC stay on chip
   // across the readings of the batch: one global round trip per launch instead of one per reading and serial section.
-  DevState<S>* gst = pb.st;
+  // (Fields are read from the parameter bank one at a time: a reference to a.m[f] would copy the member to local memory.)
+  const int f = NM == 1 ? 0 : blockIdx.x;
+  DevState<S>* gst = a.m[f].st;
   int prof_i = 0;
   auto stamp = [&]() {
-    if (pb.prof && threadIdx.x == 0 && prof_i < 16) pb.prof[prof_i++] = globaltimer();
+    if (a.m[f].prof && threadIdx.x == 0 && prof_i < 16) a.m[f].prof[prof_i++] = globaltimer();
   };
   stamp();
   __shared__ DevState<S> s_state;
   DevState<S>* st = &s_state;
-  S* __restrict__ P = pb.P;
-  const int ldp = pb.ldp, M = pb.M;
+  S* __restrict__ P = a.m[f].P;
+  const int ldp = a.m[f].ldp, M = a.m[f].M;
   {
     static_assert(sizeof(DevState<S>) % 4 == 0, "DevState is copied word-wise");
     const unsigned* src = reinterpret_cast<const unsigned*>(gst);
@@ -140,8 +150,9 @@ __global__ void __launch_bounds__(256) k_propagate(const PropBatch<S> pb) {
   __shared__ S colsum[15];
   const int t = threadIdx.x;
   stamp();  // state, P_II and P_IC columns on chip
-  for (int ir = 0; ir < pb.k; ++ir) {
-  const S wx = pb.r[ir][0], wy = pb.r[ir][1], wz = pb.r[ir][2], ax = pb.r[ir][3], ay = pb.r[ir][4], az = pb.r[ir][5], dT = pb.r[ir][6];
+  for (int ir = 0; ir < a.m[f].k; ++ir) {
+  const S wx = a.m[f].r[ir][0], wy = a.m[f].r[ir][1], wz = a.m[f].r[ir][2], ax = a.m[f].r[ir][3], ay = a.m[f].r[ir][4],
+          az = a.m[f].r[ir][5], dT = a.m[f].r[ir][6];
   __syncthreads();
   if (t < 225) { F[t] = S(0); Id[t] = ((t / 15) == (t % 15)) ? S(1) : S(0); }
   if (t < 180) G[t] = S(0);
@@ -468,7 +479,19 @@ __global__ void __launch_bounds__(256) k_propagate(const PropBatch<S> pb) {
 
 // augmentState (msckf.h:148-212): clone the IMU pose through the extrinsics and append 6 rows/columns to P.
 template <class S>
-__global__ void __launch_bounds__(256) k_augment(DevState<S>* st, S* __restrict__ P, int ldp, int M, S* __restrict__ poses) {
+struct AugArgs {
+  DevState<S>* st;
+  S* P;
+  S* poses;
+  int ldp, M;
+};
+template <class S, int NM>
+__global__ void __launch_bounds__(256) k_augment(const Members<AugArgs<S>, NM> a) {
+  const int f = NM == 1 ? 0 : blockIdx.x;
+  DevState<S>* const st = a.m[f].st;
+  S* __restrict__ const P = a.m[f].P;
+  S* __restrict__ const poses = a.m[f].poses;
+  const int ldp = a.m[f].ldp, M = a.m[f].M;
   __shared__ S J[6][6];  // the 6 nonzero columns of J: state columns {0,1,2,12,13,14}
   __shared__ S JP6[6][6];
   const int t = threadIdx.x;
@@ -524,10 +547,24 @@ __global__ void __launch_bounds__(256) k_augment(DevState<S>* st, S* __restrict_
 constexpr int kMaxKeep = 192;
 struct KeepList { int n; int idx[kMaxKeep]; };
 template <class S>
-__global__ void __launch_bounds__(256) k_gather(int n_new, const KeepList kl, const S* __restrict__ Pold,
-                                               S* __restrict__ Pnew, int ldp, const S* __restrict__ poses_old, S* __restrict__ poses_new) {
-  const int* keep_clones = kl.idx;
-  const int n_keep = kl.n;
+struct GatherArgs {
+  const S* Pold;
+  S* Pnew;
+  const S* poses_old;
+  S* poses_new;
+  int n_new, ldp;
+  KeepList kl;
+};
+static_assert(sizeof(Members<GatherArgs<double>, kBatchMembers>) <= 32764, "k_gather's batched arguments exceed the parameter limit");
+template <class S, int NM>
+__global__ void __launch_bounds__(256) k_gather(const Members<GatherArgs<S>, NM> g) {
+  const int f = NM == 1 ? 0 : blockIdx.y;
+  const int* keep_clones = g.m[f].kl.idx;
+  const int n_keep = g.m[f].kl.n, n_new = g.m[f].n_new, ldp = g.m[f].ldp;
+  const S* __restrict__ const Pold = g.m[f].Pold;
+  S* __restrict__ const Pnew = g.m[f].Pnew;
+  const S* __restrict__ const poses_old = g.m[f].poses_old;
+  S* __restrict__ const poses_new = g.m[f].poses_new;
   const size_t total = (size_t)n_new * n_new;
   for (size_t e = (size_t)blockIdx.x * 256 + threadIdx.x; e < total; e += (size_t)gridDim.x * 256) {
     const int a = (int)(e / n_new), b = (int)(e % n_new);

@@ -61,8 +61,36 @@ class FilterBatch:
         self.h = C.c_void_p()
         f0._chk(self.lib.msckf_mono_batch_create(arr, C.c_int(len(self.filters)), C.c_int(int(threads)), C.byref(self.h)), "batch_create")
 
+    def _call(self, name, *args):
+        self.filters[0]._chk(getattr(self.lib, "msckf_mono_batch_" + name)(self.h, *args), "batch_" + name)
+
+    def propagate(self, i, omega, a, dT):
+        """MSCKF::propagate of filter i (queued; the batch hands every filter's queue over in one call)"""
+        m, pm = _d(self.filters[0]._round(np.concatenate([omega, a, [dT]])))  # (one scalar type per batch)
+        self._call("propagate", C.c_int(int(i)), pm)
+
+    def augmentState(self, state_ids, times):
+        """MSCKF::augmentState of every filter: state_ids[i], times[i] for filter i"""
+        assert len(state_ids) == len(times) == len(self.filters)
+        ids = np.ascontiguousarray(state_ids, dtype=np.int32)
+        t, pt = _d([float(f._round(x)) for f, x in zip(self.filters, times)])
+        self._call("augment_state", ids.ctypes.data_as(_ip), pt)
+
     def marginalize(self):
-        self.filters[0]._chk(self.lib.msckf_mono_batch_marginalize(self.h), "batch_marginalize")
+        self._call("marginalize")
+
+    def pruneRedundantStates(self):
+        self._call("prune_redundant_states")
+
+    def pruneEmptyStates(self):
+        self._call("prune_empty_states")
+
+    def finish(self):
+        self._call("finish")
+
+    def refreshState(self):
+        """every filter's IMU state and clone poses with one synchronisation"""
+        self._call("refresh_state")
 
     def handle(self):
         fn = self.lib.msckf_mono_batch_handle
