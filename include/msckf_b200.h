@@ -161,6 +161,30 @@ int msckf_b200_batch_prune(msckf_b200_batch* b, const int* const* keep, const in
 /* msckf_b200_get_state for every member (imu = NULL, imu[i] = NULL, clone_poses = NULL or clone_poses[i] = NULL: not wanted),
  * with one stream synchronisation for the whole batch */
 int msckf_b200_batch_get_state(msckf_b200_batch* b, void* const* imu, void* const* clone_poses);
+/* ---- consistency against ground truth (simulation, Monte-Carlo trials) ----------------------------------------------------
+ * NEES = e^T P^-1 e of the filter's estimate against a caller-given truth, computed where P lives: one kernel launch (one CTA
+ * per filter), one host-to-device copy of the truth, one device-to-host copy of the results, one synchronisation.  Read-only:
+ * P, the state, the clone poses, captured graphs and launch counts are untouched.
+ * The error state is computed in fp64 for both dtypes, as the exact inverse of the state injection q+ = buildUpdateQuat(dtheta)
+ * * q (msckf.h:851-872, :1376-1390): dq = q_true * q_est^-1 (Hamilton product, true inverse conj(q)/|q|^2, dq negated when
+ * dq.w < 0), dtheta = -2 vec(dq); every other component is truth - estimate.  In the order [dtheta_I, dp_I, dv, db_g, db_a,
+ * clones (dtheta_C, dp_C)...] one fp64 Cholesky factor of P and one forward solve y = L^-1 e give every leading block's NEES
+ * as a prefix sum of y^2: orientation (3 dof), IMU pose (6), IMU state (15), whole state (15 + 6M); the position (3) has its
+ * own 3 x 3 solve.  If the factorisation meets a pivot <= 0 (P not positive definite), first_bad_pivot is its index in that
+ * order and every NEES whose block contains it is NaN; the call still succeeds. */
+typedef struct {
+  double orientation, position, pose, imu, full;
+  int dim_full;        /* 15 + 6M, or 0 without truth poses (full = NaN) */
+  int first_bad_pivot; /* -1: positive definite */
+} msckf_b200_nees_result;
+/* truth_imu: 19 doubles in the layout of msckf_b200_initialize's imu_state (g ignored); truth_poses: [M*7] doubles,
+ * p_C_G(3) q_CG(4) in window order (the layout of get_state's clone_poses), or NULL (full = NaN, dim_full = 0).
+ * A NULL or non-finite argument or a zero quaternion returns MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE;
+ * then nothing is written. */
+int msckf_b200_nees(msckf_b200_engine* e, const double* truth_imu, const double* truth_poses, msckf_b200_nees_result* out);
+/* the same for every member of a batch (truth_imu[i], truth_poses = NULL or truth_poses[i] = NULL, out[i]); every member is
+ * validated before anything is launched.  One launch per 32 members. */
+int msckf_b200_batch_nees(msckf_b200_batch* b, const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

@@ -289,6 +289,34 @@ class MSCKF {
     check(msckf_b200_get_covariance(eng(), P.data()) < 0 ? -1 : 0, "msckf_b200_get_covariance");
     return P;
   }
+  // consistency against ground truth: NEES = e^T P^-1 e of the orientation, position, IMU pose, IMU state and (with one truth
+  // pose per clone, in window order) the whole state, computed on the device (msckf_b200_nees).  Queued IMU readings are
+  // applied first, like the getters do; nothing of the filter changes.
+  msckf_b200_nees_result nees(const imuState<double>& truth, const std::vector<camState<double>>* truth_cams = nullptr) {
+    std::vector<double> im, poses;
+    neesPack(truth, truth_cams, im, poses);
+    msckf_b200_nees_result r;
+    check(msckf_b200_nees(eng(), im.data(), truth_cams ? poses.data() : nullptr, &r), "msckf_b200_nees");
+    return r;
+  }
+  // a truth in the C-ABI's layouts: imu 19 doubles (p, v, b_g, b_a, g, q_IG xyzw), poses 7 per clone (p_C_G, q_CG xyzw)
+  void neesPack(const imuState<double>& truth, const std::vector<camState<double>>* truth_cams, std::vector<double>& im,
+                std::vector<double>& poses) const {
+    if (truth_cams && truth_cams->size() != cam_states_.size())
+      throw std::invalid_argument("MSCKF::nees: one truth pose per clone of the window, in window order");
+    im.assign(19, 0.0);
+    for (int i = 0; i < 3; ++i) {
+      im[i] = truth.p_I_G(i); im[3 + i] = truth.v_I_G(i); im[6 + i] = truth.b_g(i); im[9 + i] = truth.b_a(i); im[12 + i] = truth.g(i);
+    }
+    im[15] = truth.q_IG.x(); im[16] = truth.q_IG.y(); im[17] = truth.q_IG.z(); im[18] = truth.q_IG.w();
+    poses.assign(7 * std::max<size_t>(truth_cams ? truth_cams->size() : 0, 1), 0.0);
+    if (truth_cams)
+      for (size_t k = 0; k < truth_cams->size(); ++k) {
+        const camState<double>& c = (*truth_cams)[k];
+        for (int i = 0; i < 3; ++i) poses[7 * k + i] = c.p_C_G(i);
+        poses[7 * k + 3] = c.q_CG.x(); poses[7 * k + 4] = c.q_CG.y(); poses[7 * k + 5] = c.q_CG.z(); poses[7 * k + 6] = c.q_CG.w();
+      }
+  }
   // marginalize() = launch + collect (kept separate for pipelining and for batches of filters, MSCKFBatch below).
   void marginalizeLaunch() {
     msckf_b200_tracks tr;
@@ -670,6 +698,7 @@ class MSCKFBatch {
   MSCKFBatch(const MSCKFBatch&) = delete;
   MSCKFBatch& operator=(const MSCKFBatch&) = delete;
   size_t size() const { return filters_.size(); }
+  const std::vector<MSCKF<_S>*>& filters() const { return filters_; }
 
   // MSCKF::propagate of filter i (queued on the host like there)
   void propagate(size_t i, imuReading<_S>& reading) { filters_.at(i)->propagate(reading); }
@@ -750,6 +779,26 @@ class MSCKFBatch {
   void refreshState() {
     flushImu();
     refresh(std::vector<char>(size(), 1));
+  }
+  // MSCKF::nees of every filter (truth_cams empty, or truth_cams[i] == nullptr: no truth poses for filter i), as one
+  // msckf_b200_batch_nees: one launch per 32 filters and one synchronisation
+  std::vector<msckf_b200_nees_result> nees(const std::vector<imuState<double>>& truth,
+                                           const std::vector<const std::vector<camState<double>>*>& truth_cams = {}) {
+    const size_t n = size();
+    if (truth.size() != n || (!truth_cams.empty() && truth_cams.size() != n))
+      throw std::invalid_argument("MSCKFBatch::nees: one truth (and none or one truth window) per filter");
+    flushImu();
+    std::vector<std::vector<double>> im(n), poses(n);
+    std::vector<const double*> pi(n), pp(n, nullptr);
+    for (size_t i = 0; i < n; ++i) {
+      const std::vector<camState<double>>* tc = truth_cams.empty() ? nullptr : truth_cams[i];
+      filters_[i]->neesPack(truth[i], tc, im[i], poses[i]);
+      pi[i] = im[i].data();
+      if (tc) pp[i] = poses[i].data();
+    }
+    std::vector<msckf_b200_nees_result> r(n);
+    MSCKF<_S>::check(msckf_b200_batch_nees(batch_, pi.data(), pp.data(), r.data()), "msckf_b200_batch_nees");
+    return r;
   }
   msckf_b200_batch* handle() { return batch_; }
 

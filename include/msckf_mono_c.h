@@ -65,6 +65,12 @@ int msckf_mono_batch_finish(void* batch);                                       
 int msckf_mono_batch_refresh_state(void* batch);
 void* msckf_mono_batch_handle(void* batch); /* the msckf_b200_batch* beneath */
 int msckf_mono_marginalize_batch(void** handles, int n, int threads);
+/* NEES of the estimate against ground truth (MSCKF::nees, msckf_b200_nees): truth_imu[19] p,v,b_g,b_a,g,q_IG(xyzw);
+ * truth_poses [M*7] p_C_G,q_CG(xyzw) in window order, or NULL (no whole-state NEES); out7: orientation, position, pose, imu,
+ * full, dim_full, first_bad_pivot (-1: positive definite).  _batch_nees: truth_imu[i], truth_poses NULL or [i] per filter,
+ * out7 [n][7], one device call for the batch. */
+int msckf_mono_nees(void* h, const double* truth_imu, const double* truth_poses, double* out7);
+int msckf_mono_batch_nees(void* batch, const double* const* truth_imu, const double* const* truth_poses, double* out7);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

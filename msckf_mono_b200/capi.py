@@ -25,6 +25,22 @@ class Report(C.Structure):
                 ("accepted", C.POINTER(C.c_int)), ("gamma", C.c_void_p), ("p_f_G", C.c_void_p), ("m", C.c_int), ("rank", C.c_int)]
 
 
+class NeesResult(C.Structure):
+    _fields_ = [("orientation", C.c_double), ("position", C.c_double), ("pose", C.c_double), ("imu", C.c_double),
+                ("full", C.c_double), ("dim_full", C.c_int), ("first_bad_pivot", C.c_int)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def _truth(truth_imu, truth_poses):
+    """(19 doubles: p, v, b_g, b_a, g, q_IG xyzw; [M, 7] doubles p_C_G, q_CG xyzw or None) as contiguous float64 arrays"""
+    imu = np.ascontiguousarray(truth_imu, dtype=np.float64).ravel()
+    assert imu.size == 19, imu.size
+    poses = None if truth_poses is None else np.ascontiguousarray(truth_poses, dtype=np.float64).reshape(-1, 7)
+    return imu, poses
+
+
 _lib = None
 
 
@@ -167,6 +183,19 @@ class Batch:
         check(lib().msckf_b200_batch_get_state(self.h, imu, poses), "msckf_b200_batch_get_state")
         return out
 
+    def nees(self, truth_imus, truth_poses=None):
+        """msckf_b200_batch_nees: NEES of every engine against its truth (truth_poses None, or per engine None / [M_i, 7]);
+        a list of dicts (orientation, position, pose, imu, full, dim_full, first_bad_pivot)"""
+        n = len(self.engines)
+        tp = truth_poses if truth_poses is not None else [None] * n
+        ts = [_truth(i, p) for i, p in zip(truth_imus, tp)]
+        zeros = np.zeros(7)
+        imu = (C.c_void_p * n)(*[t[0].ctypes.data for t in ts])
+        poses = None if truth_poses is None else (C.c_void_p * n)(*[None if t[1] is None else (t[1].ctypes.data if t[1].size else zeros.ctypes.data) for t in ts])
+        out = (NeesResult * n)()
+        check(lib().msckf_b200_batch_nees(self.h, imu, poses, out), "msckf_b200_batch_nees")
+        return [o.as_dict() for o in out]
+
     def jac_occupancy(self):
         """CTAs of k_jac resident per SM at the shape of the last launch (0 before the first)."""
         return int(lib().msckf_b200_batch_jac_occupancy(self.h))
@@ -281,6 +310,15 @@ class Engine:
         poses = np.zeros((self.num_clones(), 7), dtype=self.dtype)
         check(lib().msckf_b200_get_state(self.h, imu.ctypes.data_as(C.c_void_p), poses.ctypes.data_as(C.c_void_p)), "msckf_b200_get_state")
         return imu, poses
+
+    def nees(self, truth_imu, truth_poses=None):
+        """msckf_b200_nees against truth_imu (19) and, optionally, the window's truth poses [M, 7]"""
+        imu, poses = _truth(truth_imu, truth_poses)
+        zeros = np.zeros(7)
+        p = None if poses is None else C.c_void_p(poses.ctypes.data if poses.size else zeros.ctypes.data)
+        out = NeesResult()
+        check(lib().msckf_b200_nees(self.h, C.c_void_p(imu.ctypes.data), p, C.byref(out)), "msckf_b200_nees")
+        return out.as_dict()
 
     def covariance(self):
         n = 15 + 6 * self.num_clones()

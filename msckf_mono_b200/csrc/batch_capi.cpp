@@ -12,13 +12,6 @@ using namespace msckf_mono;
 using namespace msckf_view;
 
 namespace {
-// a persistent device batch over n filters of one scalar type (msckf_mono::MSCKFBatch<_S>)
-struct ViewBatch {
-  int dtype = 0;
-  MSCKFBatch<float>* bf = nullptr;
-  MSCKFBatch<double>* bd = nullptr;
-  ~ViewBatch() { delete bf; delete bd; }
-};
 template <class S>
 void batch_propagate(MSCKFBatch<S>& b, int member, const double* m) {
   imuReading<S> r;

@@ -5,6 +5,8 @@
 // shared by several engines -- the same kernels with the filter index in blockIdx.z.  No CPU fallback anywhere.
 #include <cuda_runtime.h>
 #include <algorithm>
+#include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <condition_variable>
@@ -19,6 +21,7 @@
 #include "common.cuh"
 #include "feature_kernels.cuh"
 #include "gram_kernels.cuh"
+#include "nees_kernels.cuh"
 #include "state_kernels.cuh"
 #include "tail_kernels.cuh"
 #include "tail_cluster.cuh"
@@ -120,6 +123,8 @@ struct CtxBase {
   virtual int augment(const int* which) = 0;
   virtual int prune(const int* const* keep, const int* n_keep) = 0;
   virtual int get_state(void* const* imu, void* const* poses) = 0;
+  // NEES of every member against caller-given truth (msckf_b200_nees / _batch_nees): read-only, one synchronisation
+  virtual int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) = 0;
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
@@ -281,6 +286,9 @@ struct Ctx : CtxBase {
   std::vector<Plan<S>> plan;
   Arena in, rep;
   Arena poses_out;  // clone poses of a batched get_state (pinned: all members' copies are asynchronous)
+  Arena nees_io;    // NEES: every member's truth (one host-to-device copy), then every member's result (one copy back)
+  double* nees_ws = nullptr;  // NEES: the members' fp64 Cholesky workspaces, (n + 1) x n each
+  size_t nees_ws_cap = 0;
   size_t in_used = 0, rep_used = 0;
   int device = 0;
   bool owns_stream = false;
@@ -316,7 +324,8 @@ struct Ctx : CtxBase {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     drop_graphs();
-    in.release(); rep.release(); poses_out.release();
+    in.release(); rep.release(); poses_out.release(); nees_io.release();
+    if (nees_ws) cudaFree(nees_ws);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
@@ -357,6 +366,7 @@ struct Ctx : CtxBase {
   int augment(const int* which) override;
   int prune(const int* const* keep, const int* n_keep) override;
   int get_state(void* const* imu, void* const* poses) override;
+  int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
@@ -633,6 +643,10 @@ struct Engine : EngineBase {
     return 0;
   }
   mb::AugArgs<S> aug_args() const { return {d_st, d_P, d_poses, ldp, M}; }
+  // k_nees's arguments; truth / W / out are device addresses in the calling context's buffers
+  mb::NeesArgs<S> nees_args(const double* truth, bool full, double* W, mb::NeesOut* out) const {
+    return {d_st, d_P, d_poses, truth, W, out, ldp, M, full ? 15 + 6 * M : 15, full ? 1 : 0};
+  }
 
   // everything the kernels need for this filter's slice of the update
   void fill_args(mb::UpdArgs<S>& a, const Plan<S>& p, int mode) const {
@@ -1295,6 +1309,73 @@ int Ctx<S>::get_state(void* const* imu, void* const* poses) {
     eng[i]->state_unpack(imu ? imu[i] : nullptr, off[i + 1] > off[i] ? poses[i] : nullptr, reinterpret_cast<S*>(poses_out.h + off[i]));
   return 0;
 }
+
+// Truth travels in one pinned block ([19] IMU + [M][7] poses per member) with one host-to-device copy; the results come back
+// with one copy and one synchronisation.  Nothing of the filters is written (P, state, poses, graphs, launch counts).
+static_assert(sizeof(mb::NeesOut) == sizeof(msckf_b200_nees_result) && offsetof(msckf_b200_nees_result, first_bad_pivot) == 44,
+              "mb::NeesOut must have the layout of msckf_b200_nees_result");
+template <class S>
+int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) {
+  if (!truth_imu || !out) return fail(MSCKF_B200_ERR_ARG, "nees: null argument");
+  RC(members_ready("nees"));
+  const int nf = (int)eng.size();
+  auto finite = [](const double* v, int k) { for (int i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false; return true; };
+  auto unit_ok = [](const double* q) { return q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0; };
+  std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
+  for (int i = 0; i < nf; ++i) {
+    const double* ti = truth_imu[i];
+    const double* tp = truth_poses ? truth_poses[i] : nullptr;
+    const int M = eng[i]->M;
+    if (!ti || !finite(ti, mb::kNeesTruthImu) || !unit_ok(ti + 15)) return fail(MSCKF_B200_ERR_ARG, "nees: missing or malformed truth_imu of member " + std::to_string(i));
+    if (tp) {
+      if (!finite(tp, 7 * M)) return fail(MSCKF_B200_ERR_ARG, "nees: malformed truth_poses of member " + std::to_string(i));
+      for (int k = 0; k < M; ++k)
+        if (!unit_ok(tp + 7 * k + 3)) return fail(MSCKF_B200_ERR_ARG, "nees: zero truth quaternion in member " + std::to_string(i));
+    }
+    const int n = tp ? 15 + 6 * M : 15;
+    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kNeesTruthImu + (tp ? 7 * (size_t)M : 0)));
+    woff[i + 1] = woff[i] + up256(sizeof(double) * (size_t)(n + 1) * n);
+  }
+  const size_t res_off = up256(off[nf]);
+  CK(cudaSetDevice(device));
+  RC(nees_io.ensure(res_off + sizeof(mb::NeesOut) * nf, stream));
+  if (woff[nf] > nees_ws_cap) {
+    const size_t c = std::max(woff[nf], 2 * nees_ws_cap);
+    CK(cudaStreamSynchronize(stream));
+    if (nees_ws) cudaFree(nees_ws);
+    nees_ws = nullptr; nees_ws_cap = 0;
+    CK(cudaMalloc(&nees_ws, c));
+    nees_ws_cap = c;
+  }
+  for (int i = 0; i < nf; ++i) {
+    double* h = reinterpret_cast<double*>(nees_io.h + off[i]);
+    memcpy(h, truth_imu[i], sizeof(double) * mb::kNeesTruthImu);
+    if (truth_poses && truth_poses[i] && eng[i]->M > 0) memcpy(h + mb::kNeesTruthImu, truth_poses[i], sizeof(double) * 7 * eng[i]->M);
+  }
+  CK(cudaMemcpyAsync(nees_io.d, nees_io.h, off[nf], cudaMemcpyHostToDevice, stream));
+  auto args = [&](int i) {
+    return eng[i]->nees_args(reinterpret_cast<const double*>(nees_io.d + off[i]), truth_poses && truth_poses[i],
+                             reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(nees_ws) + woff[i]),
+                             reinterpret_cast<mb::NeesOut*>(nees_io.d + res_off) + i);
+  };
+  if (nf == 1) {
+    mb::Members<mb::NeesArgs<S>, 1> a;
+    a.m[0] = args(0);
+    mb::k_nees<S, 1><<<1, 256, 0, stream>>>(a);
+  } else {
+    for (int c = 0; c < nf; c += mb::kBatchMembers) {
+      const int nm = std::min(mb::kBatchMembers, nf - c);
+      mb::Members<mb::NeesArgs<S>, mb::kBatchMembers> a;
+      for (int j = 0; j < nm; ++j) a.m[j] = args(c + j);
+      mb::k_nees<S, mb::kBatchMembers><<<nm, 256, 0, stream>>>(a);
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(nees_io.h + res_off, nees_io.d + res_off, sizeof(mb::NeesOut) * nf, cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
+  memcpy(out, nees_io.h + res_off, sizeof(mb::NeesOut) * nf);
+  return 0;
+}
 }  // namespace
 
 struct msckf_b200_engine { EngineBase* impl; };
@@ -1447,6 +1528,10 @@ int msckf_b200_batch_get_state(msckf_b200_batch* b, void* const* imu, void* cons
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->get_state(imu, clone_poses);
 }
+int msckf_b200_batch_nees(msckf_b200_batch* b, const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->nees(truth_imu, truth_poses, out);
+}
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,
                             int threads) {
@@ -1473,6 +1558,10 @@ int msckf_b200_prune(msckf_b200_engine* e, const int* keep, int n_keep) { return
 int msckf_b200_num_clones(msckf_b200_engine* e) { return e->impl->M; }
 int msckf_b200_get_state(msckf_b200_engine* e, void* imu, void* clone_poses) { return e->impl->get_state(imu, clone_poses); }
 int msckf_b200_get_covariance(msckf_b200_engine* e, void* out) { return e->impl->get_covariance(out); }
+int msckf_b200_nees(msckf_b200_engine* e, const double* truth_imu, const double* truth_poses, msckf_b200_nees_result* out) {
+  if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return e->impl->solo_ctx()->nees(&truth_imu, &truth_poses, out);
+}
 int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->impl->set_covariance(in); }
 int msckf_b200_get_counters(msckf_b200_engine* e, long long* counters) { return e->impl->get_counters(counters); }
 int msckf_b200_last_delta_x(msckf_b200_engine* e, double* out, int cap) { return e->impl->last_dx(out, cap); }

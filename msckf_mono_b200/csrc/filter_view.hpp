@@ -1,10 +1,12 @@
 // msckf_mono_b200/csrc/filter_view.hpp -- what the two translation units of the C view (include/msckf_mono_c.h) share:
-// filter_capi.cpp (one filter, msckf_mono::MSCKF<_S>) and batch_capi.cpp (device batches, msckf_mono::MSCKFBatch<_S>).
+// filter_capi.cpp (one filter, msckf_mono::MSCKF<_S>), batch_capi.cpp (device batches, msckf_mono::MSCKFBatch<_S>) and
+// nees_capi.cpp (consistency against ground truth, msckf_mono_nees / _batch_nees).
 #pragma once
 #include <cstdint>
 #include <exception>
 #include <string>
 #include <msckf_b200.h>
+#include <msckf_mono/msckf.h>
 
 namespace msckf_view {
 extern thread_local std::string g_err;  // msckf_mono_last_error()
@@ -40,6 +42,14 @@ struct Base {
   virtual int last_m() = 0;
   virtual int last_rank() = 0;
   int dtype = 0;
+};
+
+// a persistent device batch over n filters of one scalar type (msckf_mono::MSCKFBatch<_S>): a msckf_mono_batch_* handle
+struct ViewBatch {
+  int dtype = 0;
+  msckf_mono::MSCKFBatch<float>* bf = nullptr;
+  msckf_mono::MSCKFBatch<double>* bd = nullptr;
+  ~ViewBatch() { delete bf; delete bd; }
 };
 
 // runs fn(), turning an exception into -1 and its message into msckf_mono_last_error()

@@ -40,6 +40,24 @@ def pack_imu_state(s):
     return np.concatenate([np.asarray(s[k], float) for k in ("p_I_G", "v_I_G", "b_g", "b_a", "g", "q_IG")])
 
 
+NEES_KEYS = ("orientation", "position", "pose", "imu", "full", "dim_full", "first_bad_pivot")
+
+
+def _nees_dict(o):
+    d = dict(zip(NEES_KEYS, (float(x) for x in o)))
+    d["dim_full"], d["first_bad_pivot"] = int(o[5]), int(o[6])
+    return d
+
+
+def _truth(truth_imu, truth_poses):
+    imu = np.ascontiguousarray(truth_imu, dtype=np.float64).ravel()
+    assert imu.size == 19, imu.size
+    poses = None if truth_poses is None else np.ascontiguousarray(truth_poses, dtype=np.float64).reshape(-1, 7)
+    if poses is not None and poses.size == 0:
+        poses = np.zeros((1, 7))  # (an empty window: a valid pointer with nothing to read)
+    return imu, poses
+
+
 def marginalize_batch(filters, threads=8):
     """marginalize() on independent filters through the C view's batched entry point: launch on all, collect on all, the
     per-filter host work spread over `threads` host threads (engine filters only)."""
@@ -91,6 +109,18 @@ class FilterBatch:
     def refreshState(self):
         """every filter's IMU state and clone poses with one synchronisation"""
         self._call("refresh_state")
+
+    def nees(self, truth_imus, truth_poses=None):
+        """MSCKFBatch::nees: every filter against its truth (19 doubles) and, per filter, its window's truth poses [M, 7]
+        or None; one device call for the batch.  A list of dicts."""
+        n = len(self.filters)
+        tp = truth_poses if truth_poses is not None else [None] * n
+        ts = [_truth(i, p) for i, p in zip(truth_imus, tp)]
+        imu = (C.c_void_p * n)(*[t[0].ctypes.data for t in ts])
+        poses = None if truth_poses is None else (C.c_void_p * n)(*[None if t[1] is None else t[1].ctypes.data for t in ts])
+        out = np.zeros((n, 7))
+        self._call("nees", imu, poses, out.ctypes.data_as(_dp))
+        return [_nees_dict(o) for o in out]
 
     def handle(self):
         fn = self.lib.msckf_mono_batch_handle
@@ -245,6 +275,15 @@ class CFilter:
         out = np.zeros(cap, dtype=np.uint64)
         n = self._chk(self._f("get_tracked_feature_ids")(self.h, out.ctypes.data_as(_u64p), C.c_int(cap)), "get_tracked_feature_ids")
         return out[:n].copy()
+
+    def nees(self, truth_imu, truth_poses=None):
+        """MSCKF::nees against truth_imu (19 doubles: p, v, b_g, b_a, g, q_IG xyzw) and, optionally, the window's truth
+        poses [M, 7] (p_C_G, q_CG xyzw): dict of orientation, position, pose, imu, full NEES, dim_full, first_bad_pivot"""
+        imu, poses = _truth(truth_imu, truth_poses)
+        out = np.zeros(7)
+        self._chk(self._f("nees")(self.h, imu.ctypes.data_as(_dp), None if poses is None else poses.ctypes.data_as(_dp),
+                                  out.ctypes.data_as(_dp)), "nees")
+        return _nees_dict(out)
 
     # ---- test hooks --------------------------------------------------------------------
     def lastReport(self):

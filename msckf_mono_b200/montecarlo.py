@@ -1,0 +1,249 @@
+"""Monte-Carlo consistency trials of the filter on the synthetic stream (synth.make_stream_workload), measured with NEES on
+the device (MSCKFBatch::nees, msckf_b200_batch_nees).
+
+Truth: the stream built with pixel_sigma = 0 and imu_noise_frac = 0.  The generator draws its random numbers whatever the
+noise level, so the truth has the same tracks and ids, frame by frame, as the noisy stream.  Truth IMU states come from the
+trajectory at each frame's time, truth camera poses per state_id from synth.cam_pose.
+
+Trial k draws from np.random.default_rng([seed, k]) -- its inputs do not depend on how many trials run or on which rank --
+and from the noise model the filter is given: pixel noise of variance u_var' / v_var', IMU white noise of std sqrt(Q / dT),
+bias random walks of std sqrt(Q_b dT) per reading (the truth biases are recorded per frame), and an initial estimate whose
+error is drawn from P0.
+
+Error-state convention (the inverse of the filter's state injection q+ = buildUpdateQuat(dtheta) * q): dq = q_true * q_est^-1
+with the Hamilton product, dq negated when dq.w < 0, dtheta = -2 vec(dq); every other component is truth - estimate.  Host
+vectors here are in the filter's covariance order [dtheta, db_g, dv, db_a, dp, clones (dtheta_C, dp_C)...].
+"""
+from __future__ import annotations
+
+import numpy as np
+from scipy import stats
+
+from . import synth
+
+COMPONENTS = ("orientation", "position", "pose", "imu", "full")
+DOF = {"orientation": 3, "position": 3, "pose": 6, "imu": 15}
+# indices of each component in the filter's covariance order (full: the whole state)
+BLOCK = {"orientation": [0, 1, 2], "position": [12, 13, 14], "pose": [0, 1, 2, 12, 13, 14], "imu": list(range(15))}
+
+
+# ---- quaternions (x, y, z, w), Hamilton product, as the filter's quat_mul --------------------------------------------------
+def quat_mul(a, b):
+    ax, ay, az, aw = a
+    bx, by, bz, bw = b
+    return np.array([aw * bx + ax * bw + ay * bz - az * by, aw * by + ay * bw + az * bx - ax * bz,
+                     aw * bz + az * bw + ax * by - ay * bx, aw * bw - ax * bx - ay * by - az * bz])
+
+
+def quat_inv(q):
+    q = np.asarray(q, dtype=np.float64)
+    return np.array([-q[0], -q[1], -q[2], q[3]]) / np.dot(q, q)
+
+
+def quat_error(q_true, q_est):
+    """dtheta with q_true = buildUpdateQuat(dtheta) * q_est"""
+    d = quat_mul(np.asarray(q_true, dtype=np.float64), quat_inv(q_est))
+    return (2.0 if d[3] < 0 else -2.0) * d[:3]
+
+
+def quat_of_error(dth):
+    """the quaternion dq of dtheta (w >= 0): buildUpdateQuat without its renormalisation"""
+    v = -0.5 * np.asarray(dth, dtype=np.float64)
+    return np.array([v[0], v[1], v[2], np.sqrt(max(0.0, 1.0 - v @ v))])
+
+
+# ---- states: {"imu": 19 doubles (p, v, b_g, b_a, g, q_IG), "poses": [M, 7] (p_C_G, q_CG) or None} ----------------------
+def error_state(truth, est):
+    """truth - estimate in the filter's covariance order (15, or 15 + 6M when both carry poses)"""
+    t, e = np.asarray(truth["imu"], dtype=np.float64), np.asarray(est["imu"], dtype=np.float64)
+    out = [quat_error(t[15:19], e[15:19]), t[6:9] - e[6:9], t[3:6] - e[3:6], t[9:12] - e[9:12], t[0:3] - e[0:3]]
+    if truth.get("poses") is not None and est.get("poses") is not None:
+        for pt, pe in zip(np.asarray(truth["poses"], dtype=np.float64), np.asarray(est["poses"], dtype=np.float64)):
+            out += [quat_error(pt[3:7], pe[3:7]), pt[0:3] - pe[0:3]]
+    return np.concatenate(out)
+
+
+def _apply(base, e, sign):
+    b = np.asarray(base["imu"], dtype=np.float64).copy()
+    e = np.asarray(e, dtype=np.float64)
+    out = b.copy()
+    dq = quat_of_error(e[0:3])
+    out[15:19] = quat_mul(dq, b[15:19]) if sign > 0 else quat_mul(quat_inv(dq), b[15:19])
+    for dst, src in ((6, 3), (3, 6), (9, 9), (0, 12)):
+        out[dst:dst + 3] = b[dst:dst + 3] + sign * e[src:src + 3]
+    poses = None
+    if base.get("poses") is not None:
+        poses = np.asarray(base["poses"], dtype=np.float64).copy()
+        for k in range(len(poses)):
+            ek = e[15 + 6 * k:21 + 6 * k]
+            dq = quat_of_error(ek[0:3])
+            poses[k, 3:7] = quat_mul(dq, poses[k, 3:7]) if sign > 0 else quat_mul(quat_inv(dq), poses[k, 3:7])
+            poses[k, 0:3] = poses[k, 0:3] + sign * ek[3:6]
+    return {"imu": out, "poses": poses}
+
+
+def perturb(est, e):
+    """the truth whose error against est is e: error_state(perturb(est, e), est) == e"""
+    return _apply(est, e, +1)
+
+
+def estimate_of(truth, e):
+    """the estimate whose error against truth is e: error_state(truth, estimate_of(truth, e)) == e"""
+    return _apply(truth, e, -1)
+
+
+def imu_vector(s):
+    """19 doubles from a synth state dict"""
+    return np.concatenate([np.asarray(s[k], dtype=np.float64) for k in ("p_I_G", "v_I_G", "b_g", "b_a", "g", "q_IG")])
+
+
+def imu_dict(v):
+    v = np.asarray(v, dtype=np.float64)
+    return {"p_I_G": v[0:3], "v_I_G": v[3:6], "b_g": v[6:9], "b_a": v[9:12], "g": v[12:15], "q_IG": v[15:19]}
+
+
+# ---- truth and trials ------------------------------------------------------------------------------------------------------
+def make_truth(n_frames=200, seq=0, max_features=60, max_track_length=20, max_cam_states=20, noise=None):
+    """the noise-free stream, with the truth IMU state per frame (zero biases) and the truth camera pose per state_id"""
+    wl = synth.make_stream_workload(n_frames=n_frames, seq=seq, max_features=max_features, max_track_length=max_track_length,
+                                    max_cam_states=max_cam_states, pixel_sigma=0.0, imu_noise_frac=0.0)
+    wl["noise"] = synth.euroc_noise(tuned=True) if noise is None else noise
+    traj, cam = wl["traj"], wl["camera"]
+    wl["truth_imu"] = np.array([imu_vector(synth.true_imu_state(traj, fr["time"])) for fr in wl["frames"]])
+    poses = []
+    for fr in wl["frames"]:
+        C, p = synth.cam_pose(traj, fr["time"], cam)
+        poses.append(np.concatenate([p, synth.rot_to_quat(C)]))
+    wl["truth_pose"] = np.array(poses)  # row = state_id (= frame index)
+    return wl
+
+
+def make_trial(truth, k, seed=0):
+    """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise"""
+    rng = np.random.default_rng([seed, k])
+    nz = truth["noise"]
+    Q = np.asarray(nz["Q_imu"], dtype=np.float64)
+    P0 = np.asarray(nz["initial_imu_covar"], dtype=np.float64)
+    Lw, Lbg, La, Lba = (np.linalg.cholesky(Q[i:i + 3, i:i + 3]) for i in (0, 3, 6, 9))
+    e0 = np.linalg.cholesky(P0 + 0.0) @ rng.standard_normal(15)
+    imu0 = imu_vector(truth["imu_state"])
+    est0 = estimate_of({"imu": imu0, "poses": None}, e0)["imu"]
+    b_g, b_a = np.zeros(3), np.zeros(3)
+    frames, bias, inj = [], [], {"pixel": [], "gyro": [], "accel": [], "bias_g": [], "bias_a": [], "dT": []}
+    su, sv = np.sqrt(nz["u_var_prime"]), np.sqrt(nz["v_var_prime"])
+    for fr in truth["frames"]:
+        imu = []
+        for (w, a, dT) in fr["imu"]:
+            nw, na = Lw @ rng.standard_normal(3) / np.sqrt(dT), La @ rng.standard_normal(3) / np.sqrt(dT)
+            imu.append((np.asarray(w) + b_g + nw, np.asarray(a) + b_a + na, dT))
+            dbg, dba = Lbg @ rng.standard_normal(3) * np.sqrt(dT), Lba @ rng.standard_normal(3) * np.sqrt(dT)
+            b_g, b_a = b_g + dbg, b_a + dba
+            inj["gyro"].append(nw); inj["accel"].append(na); inj["bias_g"].append(dbg); inj["bias_a"].append(dba); inj["dT"].append(dT)
+        out = {"imu": imu, "state_id": fr["state_id"], "time": fr["time"]}
+        for key in ("update", "add"):
+            z, ids = fr[key]
+            n = rng.standard_normal(z.shape) * np.array([su, sv])
+            out[key] = (z + n, ids)
+            inj["pixel"].append(n)
+        frames.append(out)
+        bias.append(np.concatenate([b_g, b_a]))
+    inj = {key: (np.concatenate(v) if key == "pixel" else np.array(v)) for key, v in inj.items()}
+    return {"k": k, "frames": frames, "imu_state": imu_dict(est0), "e0": e0, "truth_bias": np.array(bias), "injected": inj}
+
+
+def truth_imu_of(truth, trial, frame):
+    """truth IMU state (19) of a trial at a frame: the trajectory's, with the trial's biases"""
+    v = truth["truth_imu"][frame].copy()
+    v[6:12] = trial["truth_bias"][frame]
+    return v
+
+
+# ---- summaries ---------------------------------------------------------------------------------------------------------------
+def trial_record(nees_rows, pos_err2):
+    """one trial's per-frame NEES (list of result dicts) and squared position errors, as plain lists"""
+    return {"nees": {c: [float(r[c]) for r in nees_rows] for c in COMPONENTS},
+            "dim": {c: [int(r["dim_full"]) if c == "full" else DOF[c] for r in nees_rows] for c in COMPONENTS},
+            "first_bad_pivot": [int(r["first_bad_pivot"]) for r in nees_rows],
+            "pos_err2": [float(x) for x in pos_err2]}
+
+
+def chi2_bounds(total_dof, n, lo=0.025, hi=0.975):
+    """two-sided 95 % bounds of the ANEES of n trials with total_dof degrees of freedom in all: chi2_{total}(q) / n"""
+    return float(stats.chi2.ppf(lo, total_dof) / n), float(stats.chi2.ppf(hi, total_dof) / n)
+
+
+def summarize(records):
+    """records {trial: trial_record}: per component, ANEES per frame with its 95 % chi^2 bounds, the run's mean ANEES and the
+    fraction of frames inside the bounds; the position RMSE over trials per frame and over the run"""
+    keys = sorted(records)
+    N = len(keys)
+    nf = len(records[keys[0]]["pos_err2"])
+    out = {"trials": N, "frames": nf, "components": {}}
+    for c in COMPONENTS:
+        V = np.array([records[k]["nees"][c] for k in keys])
+        D = np.array([records[k]["dim"][c] for k in keys])
+        anees, lo, hi, inside = [], [], [], []
+        for f in range(nf):
+            if not np.all(np.isfinite(V[:, f])) or D[:, f].sum() == 0:
+                anees.append(float("nan")); lo.append(float("nan")); hi.append(float("nan")); inside.append(False)
+                continue
+            a = float(V[:, f].mean())
+            b = chi2_bounds(int(D[:, f].sum()), N)
+            anees.append(a); lo.append(b[0]); hi.append(b[1]); inside.append(b[0] <= a <= b[1])
+        fin = [a for a in anees if np.isfinite(a)]
+        out["components"][c] = {"anees": anees, "lower": lo, "upper": hi,
+                                "mean_anees": float(np.mean(fin)) if fin else float("nan"),
+                                "mean_dof": float(D.mean()),
+                                "frames_inside": float(np.mean(inside)), "frames_finite": len(fin)}
+    E = np.array([records[k]["pos_err2"] for k in keys])
+    out["pos_rmse"] = [float(x) for x in np.sqrt(E.mean(axis=0))]
+    out["pos_rmse_run"] = float(np.sqrt(E.mean()))
+    return out
+
+
+# ---- the batched run ---------------------------------------------------------------------------------------------------------
+def run(trials, truth, dtype=np.float64, seed=0, on_frame=None):
+    """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
+    marginalize, pruneEmptyStates, refreshState, then one batched NEES with each filter's truth window looked up by the
+    state_ids of getCamStates.  Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
+    from . import engine_filter
+    from .cview import FilterBatch
+    trs = [make_trial(truth, k, seed) for k in trials]
+    fs = [engine_filter(dtype) for _ in trs]
+    for f, tr in zip(fs, trs):
+        f.initialize(truth["camera"], truth["noise"], truth["params"], tr["imu_state"])
+    fb = FilterBatch(fs)
+    rows = [[] for _ in trs]
+    err2 = [[] for _ in trs]
+    for fi in range(len(truth["frames"])):
+        frs = [tr["frames"][fi] for tr in trs]
+        for i, fr in enumerate(frs):
+            for (w, a, dT) in fr["imu"]:
+                fb.propagate(i, w, a, dT)
+        fb.augmentState([fr["state_id"] for fr in frs], [fr["time"] for fr in frs])
+        for f, fr in zip(fs, frs):
+            f.update(*fr["update"])
+            f.addFeatures(*fr["add"])
+        fb.marginalize()
+        fb.pruneEmptyStates()
+        fb.refreshState()
+        timu, tposes = [], []
+        for i, (f, tr) in enumerate(zip(fs, trs)):
+            ids = f.getCamStates()["state_id"]
+            timu.append(truth_imu_of(truth, tr, fi))
+            tposes.append(truth["truth_pose"][ids])
+            err2[i].append(float(np.sum((timu[-1][0:3] - f.getImuState()["p_I_G"]) ** 2)))
+        res = fb.nees(timu, tposes)
+        for i, r in enumerate(res):
+            rows[i].append(r)
+        if on_frame is not None:
+            on_frame(fi, fs, res)
+    fb.close()
+    records = {tr["k"]: trial_record(rows[i], err2[i]) for i, tr in enumerate(trs)}
+    final = {}
+    for f, tr in zip(fs, trs):
+        s = f.getImuState()
+        cs = f.getCamStates()
+        final[tr["k"]] = (f.getCovariance(), np.concatenate([s[key] for key in s]), np.hstack([cs["p_C_G"], cs["q_CG"]]))
+        f.close()
+    return records, final

@@ -1,0 +1,122 @@
+#!/usr/bin/env python
+"""scripts/mc_consistency.py -- Monte-Carlo consistency of the filter on the synthetic stream (msckf_mono_b200/montecarlo.py):
+`--trials` trials of the noise model the filter is given, run as one fully batched MSCKFBatch stream per process, NEES on the
+device after every frame's prune.  Prints one JSON summary: per component (orientation, position, IMU pose, IMU state, whole
+state) the run's mean ANEES, the fraction of frames inside the two-sided 95 % chi^2 bounds and the position RMSE.
+
+Under torchrun the trials are sharded with shard.sequences_of_rank; the per-trial records (a few KB) are merged with
+shard.gather_summaries -- NCCL carries nothing else.
+
+It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
+a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+ROOT = Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
+from msckf_mono_b200 import capi, montecarlo as mc, shard, synth  # noqa: E402
+
+
+def gpu_line():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
+
+
+def host_nees(e, truth_imu, truth_poses):
+    """the host path: copy P and the state back, error state and Cholesky solve in numpy"""
+    P = e.covariance().astype(np.float64)
+    imu, poses = e.state()
+    est = {"imu": np.concatenate([imu[0:15], imu[15:19]]).astype(np.float64), "poses": poses.astype(np.float64)}
+    err = mc.error_state({"imu": truth_imu, "poses": truth_poses}, est)
+    L = np.linalg.cholesky(P)
+    y = np.linalg.solve(L, err)  # (a full-state solve: the host path's cost, not its block bookkeeping)
+    return float(y @ y)
+
+
+def time_nees(n_members, reps=20):
+    wl = synth.make_window_workload(n_features=4, n_clones=2, seq=3)
+    from msckf_mono_b200 import engine_filter
+    rng = np.random.default_rng(5)
+    fs, es, truth = [], [], []
+    for i in range(n_members):
+        f = engine_filter(np.float64, max_clones=38)
+        f.initialize(wl["camera"], wl["noise"], wl["params"], wl["imu_state"])
+        e = capi.Engine(np.float64, borrowed=f.engineHandle())
+        for _ in range(30):
+            r = np.zeros((2, 7)); r[:, 3:6] = [0, 0, 9.81]; r[:, 6] = 0.005
+            e.propagate_n(r)
+            e.augment()
+        n = 15 + 6 * 30
+        A = rng.normal(size=(n, n))
+        e.set_covariance(A @ A.T / n + np.eye(n))
+        imu, poses = e.state()
+        t_imu = np.concatenate([imu[0:15], imu[15:19]]) + 1e-3
+        t_imu[15:19] /= np.linalg.norm(t_imu[15:19])
+        fs.append(f); es.append(e); truth.append((t_imu, poses.astype(np.float64) + 1e-3))
+    b = capi.Batch(es)
+    out = {}
+    for name, fn in (("device_batched_nees_ms", lambda: b.nees([t[0] for t in truth], [t[1] for t in truth])),
+                     ("host_covariance_numpy_ms", lambda: [host_nees(e, *t) for e, t in zip(es, truth)])):
+        fn()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            fn()
+            ts.append(1e3 * (time.perf_counter() - t0))
+        out[name] = float(np.median(ts))
+    b.close()
+    for f in fs:
+        f.close()
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--trials", type=int, default=32)
+    ap.add_argument("--frames", type=int, default=200)
+    ap.add_argument("--dtype", choices=("f32", "f64"), default="f64")
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--seq", type=int, default=8)
+    ap.add_argument("--no-timing", action="store_true")
+    ap.add_argument("--out", type=Path, default=None)
+    args = ap.parse_args()
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    rank = int(os.environ.get("RANK", "0"))
+    if world > 1:
+        import torch
+        import torch.distributed as dist
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
+        dist.init_process_group("nccl")
+    dtype = np.float32 if args.dtype == "f32" else np.float64
+    truth = mc.make_truth(n_frames=args.frames, seq=args.seq)
+    t0 = time.perf_counter()
+    records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed)
+    wall = time.perf_counter() - t0
+    merged = shard.gather_summaries(records)
+    s = mc.summarize(merged)
+    res = {"gpu": gpu_line(), "trials": args.trials, "frames": args.frames, "dtype": args.dtype, "seq": args.seq, "seed": args.seed,
+           "world": world, "wall_s_rank0": wall, "pos_rmse_run_m": s["pos_rmse_run"],
+           "components": {c: {k: v[k] for k in ("mean_anees", "mean_dof", "frames_inside", "frames_finite")} for c, v in s["components"].items()}}
+    for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
+        res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
+    if not args.no_timing and rank == 0:
+        res["nees_timing"] = {str(n): time_nees(n) for n in (8, 32)}
+    if rank == 0:
+        print(json.dumps(res), flush=True)
+        if args.out:
+            args.out.parent.mkdir(parents=True, exist_ok=True)
+            args.out.write_text(json.dumps({"result": res, "summary": s}, indent=1))
+    if world > 1:
+        import torch.distributed as dist
+        dist.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()
