@@ -185,6 +185,54 @@ int msckf_b200_nees(msckf_b200_engine* e, const double* truth_imu, const double*
 /* the same for every member of a batch (truth_imu[i], truth_poses = NULL or truth_poses[i] = NULL, out[i]); every member is
  * validated before anything is launched.  One launch per 32 members. */
 int msckf_b200_batch_nees(msckf_b200_batch* b, const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out);
+/* ---- aided measurements (position / pose fixes, zero-velocity updates, caller-linearised constraints) ----------------------
+ * One EKF update with residual r (m rows), Jacobian H (m x n, n = 15 + 6M, in the error-state order above) and noise R, fused
+ * where P lives: S = H P H^T + R = L L^T, W = L^-1 H P, y = L^-1 r, NIS = y^T y, dx = W^T y, P <- P - W^T W (computed in fp64,
+ * rounded to the filter's scalar type once, both halves written: exactly symmetric), then the state injection of the vision
+ * update (q_IG <- buildUpdateQuat(dtheta) * q_IG, not renormalised; clone quaternions renormalised; b_g, v, b_a, p additive;
+ * the observability copies *_null untouched).  All arithmetic is fp64 for both dtypes.
+ * Models (z in doubles; the first four compute r from the resident state, and their H selects state indices):
+ *   VELOCITY   z = v_I_G (3) -- zeros: a zero-velocity update        r = z - v          indices 6..8
+ *   POSITION   z = p_I_G (3)                                           r = z - p          indices 12..14
+ *   POSE       z = p_I_G (3), q_IG xyzw (4)                            r = [dtheta; z_p - p], dtheta of q_z against q_IG in the
+ *                                                                      convention of msckf_b200_nees   indices 0..2, 12..14
+ *   CLONE_POSE z = p_C_G (3), q_CG xyzw (4) of clone `clone` (window order, get_state's layout)   indices 15+6k .. 20+6k
+ *   LINEAR     z = r (m), H = m x n row-major (1 <= m <= 32, n must be the filter's current 15 + 6M)
+ * R is m x m row-major; only its lower triangle is read.  For the first four models m and n may be 0 or the model's own values
+ * (3, 3, 6, 6 rows).  chi2_max > 0: an update with NIS > chi2_max is not applied (applied = 0; the call succeeds).
+ * One launch (one CTA per filter), one host-to-device copy of the inputs, one device-to-host copy of the results, one
+ * synchronisation.  P is updated in place: captured update graphs stay valid.  The vision update's bookkeeping (its counters,
+ * msckf_b200_last_delta_x, rank pivots) and the launch count are not changed. */
+enum msckf_b200_aid_model {
+  MSCKF_B200_AID_VELOCITY = 0,
+  MSCKF_B200_AID_POSITION = 1,
+  MSCKF_B200_AID_POSE = 2,
+  MSCKF_B200_AID_CLONE_POSE = 3,
+  MSCKF_B200_AID_LINEAR = 4
+};
+typedef struct {
+  int model;          /* msckf_b200_aid_model; in a batch, < 0 leaves that member untouched */
+  int clone;          /* CLONE_POSE: the clone's position in the window */
+  int m, n;           /* rows and state dimension (LINEAR; 0 or the model's own for the others) */
+  const double* z;    /* the measurement (LINEAR: the residual r) */
+  const double* H;    /* LINEAR: [m][n]; else ignored */
+  const double* R;    /* [m][m], lower triangle read */
+  double chi2_max;    /* > 0: NIS gate */
+} msckf_b200_aid;
+typedef struct {
+  double nis;         /* r^T S^-1 r (NaN when S is not positive definite) */
+  double dx_norm;     /* |dx| of the applied update (0 when not applied) */
+  int dof;            /* m */
+  int applied;        /* 1: P and the state were updated */
+  int status;         /* 0: applied or gated out (see applied); 1: S not positive definite, nothing written */
+} msckf_b200_aid_result;
+/* A bad model, an out-of-window clone, an m / n mismatch, a NULL or non-finite z / H / R or a zero quaternion returns
+ * MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.  A non-finite dx or P entry returns
+ * MSCKF_B200_ERR_NUMERIC with the result filled: the update has been applied, as _fetch does for the vision update. */
+int msckf_b200_aid_update(msckf_b200_engine* e, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
+/* the same for every member of a batch (aid[i], out[i]; out[i] is not written for a member with aid[i].model < 0); every
+ * member is validated before anything is launched.  One launch per 32 updated members. */
+int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

@@ -317,6 +317,56 @@ class MSCKF {
         poses[7 * k + 3] = c.q_CG.x(); poses[7 * k + 4] = c.q_CG.y(); poses[7 * k + 5] = c.q_CG.z(); poses[7 * k + 6] = c.q_CG.w();
       }
   }
+  // aided measurements (not in the reference): one EKF update of P and the state on the device (msckf_b200_aid_update) --
+  // a position or pose fix, a zero-velocity update, a clone pose prior or a caller-linearised measurement.  Queued IMU
+  // readings are applied first; the host mirror of the state is refreshed from the device on the next getter.  An applied
+  // update between update() and marginalize() makes marginalize() refuse the queued tracks, as after a vision update.
+  msckf_b200_aid_result aidedUpdate(const msckf_b200_aid& aid) {
+    msckf_b200_aid_result r = {};
+    checkNumeric(msckf_b200_aid_update(eng(), &aid, &r), "msckf_b200_aid_update");
+    aidAbsorb(r);
+    return r;
+  }
+  // VELOCITY with z = 0: the caller knows the platform stands still
+  msckf_b200_aid_result zeroVelocityUpdate(const Matrix3<double>& R, double chi2_max = 0) {
+    const double z[3] = {0.0, 0.0, 0.0};
+    return aidedUpdate(aidModel(MSCKF_B200_AID_VELOCITY, 0, 3, z, R, chi2_max));
+  }
+  msckf_b200_aid_result positionUpdate(const Vector3<double>& p_I_G, const Matrix3<double>& R, double chi2_max = 0) {
+    const double z[3] = {p_I_G(0), p_I_G(1), p_I_G(2)};
+    return aidedUpdate(aidModel(MSCKF_B200_AID_POSITION, 0, 3, z, R, chi2_max));
+  }
+  // R: 6 x 6 over [dtheta, dp]
+  msckf_b200_aid_result poseUpdate(const Vector3<double>& p_I_G, const Quaternion<double>& q_IG, const FixedMatrix<double, 6, 6>& R,
+                                   double chi2_max = 0) {
+    const double z[7] = {p_I_G(0), p_I_G(1), p_I_G(2), q_IG.x(), q_IG.y(), q_IG.z(), q_IG.w()};
+    return aidedUpdate(aidModel(MSCKF_B200_AID_POSE, 0, 6, z, R, chi2_max));
+  }
+  // clone k of the window (window order)
+  msckf_b200_aid_result clonePoseUpdate(size_t k, const Vector3<double>& p_C_G, const Quaternion<double>& q_CG,
+                                        const FixedMatrix<double, 6, 6>& R, double chi2_max = 0) {
+    const double z[7] = {p_C_G(0), p_C_G(1), p_C_G(2), q_CG.x(), q_CG.y(), q_CG.z(), q_CG.w()};
+    return aidedUpdate(aidModel(MSCKF_B200_AID_CLONE_POSE, (int)k, 6, z, R, chi2_max));
+  }
+  // H: m x (15 + 6M) in the engine's error-state order, r: m, R: m x m (m <= 32)
+  msckf_b200_aid_result linearUpdate(const MatrixX<double>& H, const VectorX<double>& r, const MatrixX<double>& R, double chi2_max = 0) {
+    const int m = (int)H.rows(), n = (int)H.cols();
+    if ((int)r.rows() != m || (int)R.rows() != m || (int)R.cols() != m) throw std::invalid_argument("MSCKF::linearUpdate: H, r and R differ in rows");
+    std::vector<double> h((size_t)m * n), z(m);
+    for (int i = 0; i < m; ++i) {
+      z[i] = r(i);
+      for (int j = 0; j < n; ++j) h[(size_t)i * n + j] = H(i, j);
+    }
+    msckf_b200_aid a = aidModel(MSCKF_B200_AID_LINEAR, 0, m, z.data(), R, chi2_max);
+    a.n = n;
+    a.H = h.data();
+    return aidedUpdate(a);
+  }
+  // host bookkeeping after an aided update: the mirror is stale, and an applied update moves the state the queued tracks saw
+  void aidAbsorb(const msckf_b200_aid_result& r) {
+    state_dirty_ = true;
+    if (r.applied) epoch_++;
+  }
   // marginalize() = launch + collect (kept separate for pipelining and for batches of filters, MSCKFBatch below).
   void marginalizeLaunch() {
     msckf_b200_tracks tr;
@@ -535,6 +585,20 @@ class MSCKF {
   std::vector<size_t> rm_cam_state_ids_, tri_feat_;
   std::vector<std::vector<size_t>> tri_involved_;
   std::vector<featureTrackToResidualize<_S>> tri_batch_, res_batch_;
+  std::vector<double> aid_R_;  // R of the last convenience-form aided update, row-major
+
+  // a msckf_b200_aid of one of the convenience forms (z must outlive the call; R is copied row-major into aid_R_)
+  template <class Mat>
+  msckf_b200_aid aidModel(int model, int clone, int m, const double* z, const Mat& R, double chi2_max) {
+    if ((int)R.rows() != m || (int)R.cols() != m) throw std::invalid_argument("MSCKF: aided update R has the wrong shape");
+    aid_R_.resize((size_t)m * m);
+    for (int i = 0; i < m; ++i)
+      for (int j = 0; j < m; ++j) aid_R_[(size_t)i * m + j] = R(i, j);
+    msckf_b200_aid a = {};
+    a.model = model; a.clone = clone; a.m = m; a.n = 0;
+    a.z = z; a.H = nullptr; a.R = aid_R_.data(); a.chi2_max = chi2_max;
+    return a;
+  }
 
   static void check(int rc, const char* what) {
     if (rc != 0) throw std::runtime_error(std::string(what) + " failed (" + std::to_string(rc) + "): " + msckf_b200_last_error());
@@ -798,6 +862,19 @@ class MSCKFBatch {
     }
     std::vector<msckf_b200_nees_result> r(n);
     MSCKF<_S>::check(msckf_b200_batch_nees(batch_, pi.data(), pp.data(), r.data()), "msckf_b200_batch_nees");
+    return r;
+  }
+  // MSCKF::aidedUpdate of every filter (aid[i].model < 0: filter i is left alone) as one msckf_b200_batch_aid_update: one
+  // launch per 32 updated filters and one synchronisation.  result[i] of a filter left alone is value-initialised.
+  std::vector<msckf_b200_aid_result> aidedUpdate(const std::vector<msckf_b200_aid>& aid) {
+    if (aid.size() != size()) throw std::invalid_argument("MSCKFBatch::aidedUpdate: one aided measurement per filter");
+    flushImu();
+    std::vector<msckf_b200_aid_result> r(size(), msckf_b200_aid_result());
+    const int rc = msckf_b200_batch_aid_update(batch_, aid.data(), r.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch aided update: " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_update");
+    for (size_t i = 0; i < size(); ++i)
+      if (aid[i].model >= 0) filters_[i]->aidAbsorb(r[i]);
     return r;
   }
   msckf_b200_batch* handle() { return batch_; }

@@ -9,6 +9,7 @@
 #ifndef MSCKF_MONO_C_H_
 #define MSCKF_MONO_C_H_
 #include <stdint.h>
+#include <msckf_b200.h>
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -71,6 +72,11 @@ int msckf_mono_marginalize_batch(void** handles, int n, int threads);
  * out7 [n][7], one device call for the batch. */
 int msckf_mono_nees(void* h, const double* truth_imu, const double* truth_poses, double* out7);
 int msckf_mono_batch_nees(void* batch, const double* const* truth_imu, const double* const* truth_poses, double* out7);
+/* aided measurement update (MSCKF::aidedUpdate, msckf_b200_aid_update: models, layouts and errors there); the filter's host
+ * mirror is refreshed on the next getter.  _batch_aid_update: aid[i] / out[i] per filter (aid[i].model < 0: filter i is left
+ * alone), one device call for the batch. */
+int msckf_mono_aid_update(void* h, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
+int msckf_mono_batch_aid_update(void* batch, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

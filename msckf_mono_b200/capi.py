@@ -41,6 +41,35 @@ def _truth(truth_imu, truth_poses):
     return imu, poses
 
 
+AID_VELOCITY, AID_POSITION, AID_POSE, AID_CLONE_POSE, AID_LINEAR = range(5)
+
+
+class Aid(C.Structure):
+    _fields_ = [("model", C.c_int), ("clone", C.c_int), ("m", C.c_int), ("n", C.c_int), ("z", C.c_void_p), ("H", C.c_void_p),
+                ("R", C.c_void_p), ("chi2_max", C.c_double)]
+
+
+class AidResult(C.Structure):
+    _fields_ = [("nis", C.c_double), ("dx_norm", C.c_double), ("dof", C.c_int), ("applied", C.c_int), ("status", C.c_int)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def aid_struct(spec):
+    """(Aid, the float64 arrays it points into) of one aided measurement: spec = None (a batch member left alone) or a dict
+    model, z (LINEAR: the residual r), R [m, m], H [m, n] (LINEAR), clone (CLONE_POSE), chi2_max"""
+    if spec is None or spec["model"] < 0:
+        return Aid(-1, 0, 0, 0, None, None, None, 0.0), ()
+    z = np.ascontiguousarray(spec["z"], dtype=np.float64).ravel()
+    R = np.ascontiguousarray(spec["R"], dtype=np.float64)
+    H = None if spec.get("H") is None else np.ascontiguousarray(spec["H"], dtype=np.float64)
+    m, n = (H.shape[0], H.shape[1]) if H is not None else (R.shape[0], 0)
+    a = Aid(int(spec["model"]), int(spec.get("clone", 0)), m, n, z.ctypes.data, None if H is None else H.ctypes.data,
+            R.ctypes.data, float(spec.get("chi2_max", 0.0)))
+    return a, (z, R, H)
+
+
 _lib = None
 
 
@@ -196,6 +225,16 @@ class Batch:
         check(lib().msckf_b200_batch_nees(self.h, imu, poses, out), "msckf_b200_batch_nees")
         return [o.as_dict() for o in out]
 
+    def aid_update(self, specs):
+        """msckf_b200_batch_aid_update: specs[i] for engine i (see aid_struct; None leaves engine i alone); a list of result
+        dicts (None for an engine left alone)"""
+        n = len(self.engines)
+        assert len(specs) == n
+        st = [aid_struct(s) for s in specs]
+        out = (AidResult * n)()
+        check(lib().msckf_b200_batch_aid_update(self.h, (Aid * n)(*[a for a, _ in st]), out), "msckf_b200_batch_aid_update")
+        return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
+
     def jac_occupancy(self):
         """CTAs of k_jac resident per SM at the shape of the last launch (0 before the first)."""
         return int(lib().msckf_b200_batch_jac_occupancy(self.h))
@@ -318,6 +357,13 @@ class Engine:
         p = None if poses is None else C.c_void_p(poses.ctypes.data if poses.size else zeros.ctypes.data)
         out = NeesResult()
         check(lib().msckf_b200_nees(self.h, C.c_void_p(imu.ctypes.data), p, C.byref(out)), "msckf_b200_nees")
+        return out.as_dict()
+
+    def aid_update(self, model, z, R, H=None, clone=0, chi2_max=0.0):
+        """msckf_b200_aid_update: one aided measurement (see aid_struct); the result as a dict"""
+        a, keep = aid_struct({"model": model, "z": z, "R": R, "H": H, "clone": clone, "chi2_max": chi2_max})
+        out = AidResult()
+        check(lib().msckf_b200_aid_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_aid_update")
         return out.as_dict()
 
     def covariance(self):

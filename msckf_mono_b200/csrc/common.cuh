@@ -193,6 +193,70 @@ __device__ __forceinline__ void build_update_quat(const S* dth, S* u) {
   quat_normalize(u);
 }
 
+// The state injection of msckf.h:1373-1391 for delta-x component i = dx(i) (fp64): q_IG <- buildUpdateQuat(dtheta) * q_IG, not
+// renormalised; b_g, v, b_a, p additive; clone k: q <- normalise(buildUpdateQuat(dtheta_k) * q), p additive.  The observability
+// copies (*_null) are not touched.  Thread tid of nthr takes the IMU state (tid == 0) and every nthr-th clone.  (k_aid.  k_syrk
+// keeps its own inlined copy of the same arithmetic: through this function its SASS is scheduled differently, DESIGN.md 4.8)
+template <class S, class DX>
+__device__ __forceinline__ void inject_state(DevState<S>* st, S* poses, int M, int tid, int nthr, const DX& dx) {
+  if (tid == 0) {
+    const S dth[3] = {(S)dx(0), (S)dx(1), (S)dx(2)};
+    S uq[4], qn[4];
+    build_update_quat(dth, uq);
+    quat_mul(uq, st->q_IG, qn);  // not renormalised (msckf.h:1376-1378)
+    for (int i = 0; i < 4; ++i) st->q_IG[i] = qn[i];
+    for (int i = 0; i < 3; ++i) {
+      st->b_g[i] += (S)dx(3 + i);
+      st->v_I_G[i] += (S)dx(6 + i);
+      st->b_a[i] += (S)dx(9 + i);
+      st->p_I_G[i] += (S)dx(12 + i);
+    }
+  }
+  for (int ci = tid; ci < M; ci += nthr) {
+    S* ps = poses + kPoseStride * ci;
+    const S dth[3] = {(S)dx(15 + 6 * ci), (S)dx(16 + 6 * ci), (S)dx(17 + 6 * ci)};
+    S uq[4], qn[4];
+    build_update_quat(dth, uq);
+    quat_mul(uq, ps, qn);
+    quat_normalize(qn);
+    ps[0] = qn[0]; ps[1] = qn[1]; ps[2] = qn[2]; ps[3] = qn[3];
+    ps[4] += (S)dx(18 + 6 * ci); ps[5] += (S)dx(19 + 6 * ci); ps[6] += (S)dx(20 + 6 * ci);
+  }
+}
+
+// One warp (lane = row) factors the leading nb x nb block (nb <= 32) of the lower triangle of D in place, D = L L^T.  Returns
+// the number of leading pivots that were positive (nb: positive definite); idg[i] = 1 / L[i][i] for those.  (k_nees, k_aid)
+template <int LD>
+__device__ __forceinline__ int warp_chol(double (*D)[LD], int nb, double* idg, int lane) {
+  int nv = nb;
+  for (int j = 0; j < nb; ++j) {
+    const double d = D[j][j];
+    if (!(d > 0.0)) { nv = j; break; }  // (uniform across the warp: every lane read the same word)
+    const double r = sqrt(d);
+    __syncwarp();
+    if (lane == j) D[j][j] = r;
+    if (lane > j && lane < nb) D[lane][j] = D[lane][j] / r;
+    __syncwarp();
+    if (lane > j && lane < nb) {
+      const double lij = D[lane][j];
+      for (int c = j + 1; c <= lane; ++c) D[lane][c] -= lij * D[c][j];
+    }
+    __syncwarp();
+  }
+  if (lane < nv) idg[lane] = 1.0 / D[lane][lane];
+  return nv;
+}
+// One row against that factor, x <- x L^-T over the first nv columns (lane = column): a forward substitution across the warp
+template <int LD>
+__device__ __forceinline__ double warp_row_solve(double x, const double (*D)[LD], const double* idg, int nv, int lane) {
+  for (int c = 0; c < nv; ++c) {
+    const double xc = __shfl_sync(0xffffffffu, x, c) * idg[c];
+    if (lane == c) x = xc;
+    else if (lane > c) x -= xc * D[lane][c];
+  }
+  return x;
+}
+
 // ---- TMA (bulk async copy) staging of a small contiguous table into shared memory -----------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {

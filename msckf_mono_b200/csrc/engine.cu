@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/msckf_b200.h"
+#include "aid_kernels.cuh"
 #include "common.cuh"
 #include "feature_kernels.cuh"
 #include "gram_kernels.cuh"
@@ -125,6 +126,8 @@ struct CtxBase {
   virtual int get_state(void* const* imu, void* const* poses) = 0;
   // NEES of every member against caller-given truth (msckf_b200_nees / _batch_nees): read-only, one synchronisation
   virtual int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) = 0;
+  // aided measurement updates of the members (msckf_b200_aid_update / _batch_aid_update): one launch per 32, one synchronisation
+  virtual int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) = 0;
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
@@ -289,6 +292,9 @@ struct Ctx : CtxBase {
   Arena nees_io;    // NEES: every member's truth (one host-to-device copy), then every member's result (one copy back)
   double* nees_ws = nullptr;  // NEES: the members' fp64 Cholesky workspaces, (n + 1) x n each
   size_t nees_ws_cap = 0;
+  Arena aid_io;               // aided updates: every member's inputs (one host-to-device copy), then the results (one copy back)
+  double* aid_ws = nullptr;   // aided updates: W^T and dx of the members whose share does not fit in shared memory
+  size_t aid_ws_cap = 0;
   size_t in_used = 0, rep_used = 0;
   int device = 0;
   bool owns_stream = false;
@@ -324,8 +330,9 @@ struct Ctx : CtxBase {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     drop_graphs();
-    in.release(); rep.release(); poses_out.release(); nees_io.release();
+    in.release(); rep.release(); poses_out.release(); nees_io.release(); aid_io.release();
     if (nees_ws) cudaFree(nees_ws);
+    if (aid_ws) cudaFree(aid_ws);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
@@ -367,6 +374,7 @@ struct Ctx : CtxBase {
   int prune(const int* const* keep, const int* n_keep) override;
   int get_state(void* const* imu, void* const* poses) override;
   int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) override;
+  int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
@@ -646,6 +654,10 @@ struct Engine : EngineBase {
   // k_nees's arguments; truth / W / out are device addresses in the calling context's buffers
   mb::NeesArgs<S> nees_args(const double* truth, bool full, double* W, mb::NeesOut* out) const {
     return {d_st, d_P, d_poses, truth, W, out, ldp, M, full ? 15 + 6 * M : 15, full ? 1 : 0};
+  }
+  // k_aid's arguments; in / ws / out are device addresses in the calling context's buffers (ws = nullptr: shared memory)
+  mb::AidArgs<S> aid_args(const msckf_b200_aid& q, int m, const double* in, double* ws, mb::AidOut* out) const {
+    return {d_st, d_P, d_poses, in, ws, out, q.chi2_max, ldp, M, q.model, q.model == MSCKF_B200_AID_CLONE_POSE ? q.clone : 0, m, 0};
   }
 
   // everything the kernels need for this filter's slice of the update
@@ -1376,6 +1388,105 @@ int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_pose
   memcpy(out, nees_io.h + res_off, sizeof(mb::NeesOut) * nf);
   return 0;
 }
+
+// Aided updates: every updated member's inputs travel in one pinned block ([32] z, R [m][m], H [m][n] for LINEAR), the results
+// come back with one copy and one synchronisation.  W^T and dx (n (m + 1) doubles) sit in dynamic shared memory up to
+// kAidSmemMax bytes, else in a global workspace.  Nothing is launched unless every member is valid.
+static_assert(offsetof(mb::AidOut, status) == offsetof(msckf_b200_aid_result, status), "mb::AidOut must start like msckf_b200_aid_result");
+constexpr size_t kAidSmemMax = 32 * 1024;
+template <class S>
+int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
+  if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "aid_update: null argument");
+  RC(members_ready("aid_update"));
+  const int nf = (int)eng.size();
+  auto finite = [](const double* v, size_t k) { for (size_t i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false; return true; };
+  std::vector<int> idx, rows(nf, 0);
+  std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
+  for (int i = 0; i < nf; ++i) {
+    off[i + 1] = off[i];
+    woff[i + 1] = woff[i];
+    const msckf_b200_aid& q = in[i];
+    if (q.model < 0) continue;
+    const std::string who = " (member " + std::to_string(i) + ")";
+    const int M = eng[i]->M, n = 15 + 6 * M;
+    if (q.model > MSCKF_B200_AID_LINEAR) return fail(MSCKF_B200_ERR_ARG, "aid_update: unknown model" + who);
+    const bool lin = q.model == MSCKF_B200_AID_LINEAR;
+    const int m = lin ? q.m : (q.model <= MSCKF_B200_AID_POSITION ? 3 : 6);
+    if (lin ? (m < 1 || m > mb::kAidMaxRows || q.n != n) : ((q.m != 0 && q.m != m) || (q.n != 0 && q.n != n)))
+      return fail(MSCKF_B200_ERR_ARG, "aid_update: m / n do not match the model and the window" + who);
+    if (q.model == MSCKF_B200_AID_CLONE_POSE && (q.clone < 0 || q.clone >= M)) return fail(MSCKF_B200_ERR_ARG, "aid_update: clone outside the window" + who);
+    const int nz = lin ? m : (q.model <= MSCKF_B200_AID_POSITION ? 3 : 7);
+    if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing or non-finite z" + who);
+    if (!q.R) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing R" + who);
+    for (int r = 0; r < m; ++r)
+      if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, "aid_update: non-finite R" + who);
+    if (lin && (!q.H || !finite(q.H, (size_t)m * n))) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing or non-finite H" + who);
+    if (!lin && nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
+      return fail(MSCKF_B200_ERR_ARG, "aid_update: zero quaternion" + who);
+    if (std::isnan(q.chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_update: chi2_max is NaN" + who);
+    rows[i] = m;
+    idx.push_back(i);
+    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (lin ? (size_t)m * n : 0)));
+    if (mb::aid_ws_bytes(n, m) > kAidSmemMax) woff[i + 1] = woff[i] + up256(mb::aid_ws_bytes(n, m));
+  }
+  if (idx.empty()) return 0;
+  const size_t res_off = up256(off[nf]);
+  CK(cudaSetDevice(device));
+  RC(aid_io.ensure(res_off + sizeof(mb::AidOut) * nf, stream));
+  if (woff[nf] > aid_ws_cap) {
+    const size_t c = std::max(woff[nf], 2 * aid_ws_cap);
+    CK(cudaStreamSynchronize(stream));
+    if (aid_ws) cudaFree(aid_ws);
+    aid_ws = nullptr; aid_ws_cap = 0;
+    CK(cudaMalloc(&aid_ws, c));
+    aid_ws_cap = c;
+  }
+  for (int i : idx) {
+    const msckf_b200_aid& q = in[i];
+    const int m = rows[i], n = 15 + 6 * eng[i]->M;
+    double* h = reinterpret_cast<double*>(aid_io.h + off[i]);
+    memset(h, 0, sizeof(double) * mb::kAidZ);
+    memcpy(h, q.z, sizeof(double) * (q.model == MSCKF_B200_AID_LINEAR ? m : q.model <= MSCKF_B200_AID_POSITION ? 3 : 7));
+    memcpy(h + mb::kAidZ, q.R, sizeof(double) * m * m);
+    if (q.model == MSCKF_B200_AID_LINEAR) memcpy(h + mb::kAidZ + m * m, q.H, sizeof(double) * m * n);
+  }
+  CK(cudaMemcpyAsync(aid_io.d, aid_io.h, off[nf], cudaMemcpyHostToDevice, stream));
+  mb::AidOut* d_out = reinterpret_cast<mb::AidOut*>(aid_io.d + res_off);
+  // a member's arguments, and the dynamic shared memory it needs (0: its W^T and dx are in the global workspace)
+  auto args = [&](int i, size_t& smem) {
+    const int m = rows[i], n = 15 + 6 * eng[i]->M;
+    const bool global = woff[i + 1] > woff[i];
+    if (!global) smem = std::max(smem, mb::aid_ws_bytes(n, m));
+    return eng[i]->aid_args(in[i], m, reinterpret_cast<const double*>(aid_io.d + off[i]),
+                            global ? reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(aid_ws) + woff[i]) : nullptr, d_out + i);
+  };
+  if (nf == 1) {
+    mb::Members<mb::AidArgs<S>, 1> a;
+    size_t smem = 0;
+    a.m[0] = args(0, smem);
+    mb::k_aid<S, 1><<<1, mb::kAidThreads, smem, stream>>>(a);
+  } else {
+    for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
+      const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
+      mb::Members<mb::AidArgs<S>, mb::kBatchMembers> a;
+      size_t smem = 0;
+      for (int j = 0; j < nm; ++j) a.m[j] = args(idx[c + j], smem);
+      mb::k_aid<S, mb::kBatchMembers><<<nm, mb::kAidThreads, smem, stream>>>(a);
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(aid_io.h + res_off, aid_io.d + res_off, sizeof(mb::AidOut) * nf, cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
+  const mb::AidOut* h_out = reinterpret_cast<const mb::AidOut*>(aid_io.h + res_off);
+  int numeric = -1;
+  for (int i : idx) {
+    const mb::AidOut& o = h_out[i];
+    out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].applied = o.applied; out[i].status = o.status;
+    if (o.numeric && numeric < 0) numeric = i;
+  }
+  if (numeric >= 0) return fail(MSCKF_B200_ERR_NUMERIC, "aid_update: non-finite delta-x or covariance entry (member " + std::to_string(numeric) + "); the update was applied");
+  return 0;
+}
 }  // namespace
 
 struct msckf_b200_engine { EngineBase* impl; };
@@ -1532,6 +1643,10 @@ int msckf_b200_batch_nees(msckf_b200_batch* b, const double* const* truth_imu, c
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->nees(truth_imu, truth_poses, out);
 }
+int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, msckf_b200_aid_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->aid(aid, out);
+}
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,
                             int threads) {
@@ -1561,6 +1676,11 @@ int msckf_b200_get_covariance(msckf_b200_engine* e, void* out) { return e->impl-
 int msckf_b200_nees(msckf_b200_engine* e, const double* truth_imu, const double* truth_poses, msckf_b200_nees_result* out) {
   if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return e->impl->solo_ctx()->nees(&truth_imu, &truth_poses, out);
+}
+int msckf_b200_aid_update(msckf_b200_engine* e, const msckf_b200_aid* aid, msckf_b200_aid_result* out) {
+  if (!e || !aid) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (aid->model < 0) return fail(MSCKF_B200_ERR_ARG, "aid_update: unknown model");
+  return e->impl->solo_ctx()->aid(aid, out);
 }
 int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->impl->set_covariance(in); }
 int msckf_b200_get_counters(msckf_b200_engine* e, long long* counters) { return e->impl->get_counters(counters); }

@@ -101,22 +101,7 @@ __global__ void __launch_bounds__(256) k_nees(const Members<NeesArgs<S>, NM> a) 
     }
     __syncthreads();
     if (t < 32) {  // unblocked factor of the diagonal block: lane = row
-      int nv = nb;
-      for (int j = 0; j < nb; ++j) {
-        const double d = D[j][j];
-        if (!(d > 0.0)) { nv = j; break; }  // (uniform across the warp: every lane read the same word)
-        const double r = sqrt(d);
-        __syncwarp();
-        if (t == j) D[j][j] = r;
-        if (t > j && t < nb) D[t][j] = D[t][j] / r;
-        __syncwarp();
-        if (t > j && t < nb) {
-          const double lij = D[t][j];
-          for (int c = j + 1; c <= t; ++c) D[t][c] -= lij * D[c][j];
-        }
-        __syncwarp();
-      }
-      if (t < nv) idg[t] = 1.0 / D[t][t];
+      const int nv = warp_chol(D, nb, idg, t);
       if (t == 0) s_nv = nv;
     }
     __syncthreads();
@@ -126,12 +111,7 @@ __global__ void __launch_bounds__(256) k_nees(const Members<NeesArgs<S>, NM> a) 
     const int r0 = nv < nb ? n : k0 + nb, lane = t & 31;
     for (int r = r0 + (t >> 5); r <= n; r += 8) {
       double* row = W + (size_t)r * n + k0;
-      double x = lane < nv ? row[lane] : 0.0;
-      for (int c = 0; c < nv; ++c) {
-        const double xc = __shfl_sync(0xffffffffu, x, c) * idg[c];
-        if (lane == c) x = xc;
-        else if (lane > c) x -= xc * D[lane][c];
-      }
+      const double x = warp_row_solve(lane < nv ? row[lane] : 0.0, D, idg, nv, lane);
       if (lane < nv) row[lane] = x;
     }
     if (nv < nb) {

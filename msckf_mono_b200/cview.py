@@ -122,6 +122,17 @@ class FilterBatch:
         self._call("nees", imu, poses, out.ctypes.data_as(_dp))
         return [_nees_dict(o) for o in out]
 
+    def aid_update(self, specs):
+        """MSCKFBatch::aidedUpdate: specs[i] for filter i (a dict as for capi.aid_struct, or None: filter i left alone); one
+        device call for the batch.  A list of result dicts (None for a filter left alone)."""
+        from .capi import Aid, AidResult, aid_struct
+        n = len(self.filters)
+        assert len(specs) == n
+        st = [aid_struct(s) for s in specs]
+        out = (AidResult * n)()
+        self._call("aid_update", (Aid * n)(*[a for a, _ in st]), out)
+        return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
+
     def handle(self):
         fn = self.lib.msckf_mono_batch_handle
         fn.restype = C.c_void_p
@@ -284,6 +295,15 @@ class CFilter:
         self._chk(self._f("nees")(self.h, imu.ctypes.data_as(_dp), None if poses is None else poses.ctypes.data_as(_dp),
                                   out.ctypes.data_as(_dp)), "nees")
         return _nees_dict(out)
+
+    def aid_update(self, model, z, R, H=None, clone=0, chi2_max=0.0):
+        """MSCKF::aidedUpdate (include/msckf_b200.h: msckf_b200_aid_update): model, z (LINEAR: the residual), R [m, m],
+        H [m, 15 + 6M] (LINEAR), clone (CLONE_POSE), chi2_max (> 0: NIS gate).  A dict nis, dx_norm, dof, applied, status."""
+        from .capi import AidResult, aid_struct
+        a, keep = aid_struct({"model": model, "z": z, "R": R, "H": H, "clone": clone, "chi2_max": chi2_max})
+        out = AidResult()
+        self._chk(self._f("aid_update")(self.h, C.byref(a), C.byref(out)), "aid_update")
+        return out.as_dict()
 
     # ---- test hooks --------------------------------------------------------------------
     def lastReport(self):

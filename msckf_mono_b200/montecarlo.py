@@ -10,6 +10,11 @@ and from the noise model the filter is given: pixel noise of variance u_var' / v
 bias random walks of std sqrt(Q_b dT) per reading (the truth biases are recorded per frame), and an initial estimate whose
 error is drawn from P0.
 
+Optional position fixes (a GPS or motion-capture stand-in): every `fix_every` frames, after the prune, each trial fuses
+z = p_true + N(0, sigma^2 I) into its filter (MSCKFBatch::aidedUpdate, one batched call).  The fix noise of trial k comes from
+its own stream np.random.default_rng([seed, k, 1]), so the trial's other inputs are the same with fixes on or off.  The NIS
+of the fixes gives a truth-free consistency figure (ANIS against chi^2 with 3 dof per trial).
+
 Error-state convention (the inverse of the filter's state injection q+ = buildUpdateQuat(dtheta) * q): dq = q_true * q_est^-1
 with the Hamilton product, dq negated when dq.w < 0, dtheta = -2 vec(dq); every other component is truth - estimate.  Host
 vectors here are in the filter's covariance order [dtheta, db_g, dv, db_a, dp, clones (dtheta_C, dp_C)...].
@@ -118,8 +123,9 @@ def make_truth(n_frames=200, seq=0, max_features=60, max_track_length=20, max_ca
     return wl
 
 
-def make_trial(truth, k, seed=0):
-    """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise"""
+def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0):
+    """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
+    fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I)."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -148,7 +154,12 @@ def make_trial(truth, k, seed=0):
         frames.append(out)
         bias.append(np.concatenate([b_g, b_a]))
     inj = {key: (np.concatenate(v) if key == "pixel" else np.array(v)) for key, v in inj.items()}
-    return {"k": k, "frames": frames, "imu_state": imu_dict(est0), "e0": e0, "truth_bias": np.array(bias), "injected": inj}
+    out = {"k": k, "frames": frames, "imu_state": imu_dict(est0), "e0": e0, "truth_bias": np.array(bias), "injected": inj}
+    if fix_every > 0:
+        frng = np.random.default_rng([seed, k, 1])
+        out["fixes"] = [truth["truth_imu"][f][0:3] + fix_sigma * frng.standard_normal(3) if (f + 1) % fix_every == 0 else None
+                        for f in range(len(truth["frames"]))]
+    return out
 
 
 def truth_imu_of(truth, trial, frame):
@@ -159,12 +170,14 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2):
-    """one trial's per-frame NEES (list of result dicts) and squared position errors, as plain lists"""
+def trial_record(nees_rows, pos_err2, fix_nis=()):
+    """one trial's per-frame NEES (list of result dicts), squared position errors and the NIS of its position fixes, as
+    plain lists"""
     return {"nees": {c: [float(r[c]) for r in nees_rows] for c in COMPONENTS},
             "dim": {c: [int(r["dim_full"]) if c == "full" else DOF[c] for r in nees_rows] for c in COMPONENTS},
             "first_bad_pivot": [int(r["first_bad_pivot"]) for r in nees_rows],
-            "pos_err2": [float(x) for x in pos_err2]}
+            "pos_err2": [float(x) for x in pos_err2],
+            "fix_nis": [float(x) for x in fix_nis]}
 
 
 def chi2_bounds(total_dof, n, lo=0.025, hi=0.975):
@@ -198,17 +211,27 @@ def summarize(records):
     E = np.array([records[k]["pos_err2"] for k in keys])
     out["pos_rmse"] = [float(x) for x in np.sqrt(E.mean(axis=0))]
     out["pos_rmse_run"] = float(np.sqrt(E.mean()))
+    F = np.array([records[k].get("fix_nis", []) for k in keys], dtype=np.float64)
+    if F.size:  # ANIS of the position fixes: 3 dof per trial and fix
+        lo, hi = chi2_bounds(3 * N, N)
+        anis = F.mean(axis=0)
+        out["fixes"] = {"anis": [float(a) for a in anis], "lower": lo, "upper": hi, "dof": 3, "mean_anis": float(anis.mean()),
+                        "fixes_inside": float(np.mean((anis >= lo) & (anis <= hi)))}
     return out
 
 
 # ---- the batched run ---------------------------------------------------------------------------------------------------------
-def run(trials, truth, dtype=np.float64, seed=0, on_frame=None):
+def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
-    marginalize, pruneEmptyStates, refreshState, then one batched NEES with each filter's truth window looked up by the
-    state_ids of getCamStates.  Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
+    marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
+    refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.
+    Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
     from . import engine_filter
+    from .capi import AID_POSITION
     from .cview import FilterBatch
-    trs = [make_trial(truth, k, seed) for k in trials]
+    trs = [make_trial(truth, k, seed, fix_every, fix_sigma) for k in trials]
+    R_fix = (fix_sigma ** 2) * np.eye(3)
+    nis = [[] for _ in trs]
     fs = [engine_filter(dtype) for _ in trs]
     for f, tr in zip(fs, trs):
         f.initialize(truth["camera"], truth["noise"], truth["params"], tr["imu_state"])
@@ -226,6 +249,10 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None):
             f.addFeatures(*fr["add"])
         fb.marginalize()
         fb.pruneEmptyStates()
+        if fix_every > 0 and trs[0]["fixes"][fi] is not None:
+            res = fb.aid_update([{"model": AID_POSITION, "z": tr["fixes"][fi], "R": R_fix} for tr in trs])
+            for i, r in enumerate(res):
+                nis[i].append(r["nis"])
         fb.refreshState()
         timu, tposes = [], []
         for i, (f, tr) in enumerate(zip(fs, trs)):
@@ -239,7 +266,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None):
         if on_frame is not None:
             on_frame(fi, fs, res)
     fb.close()
-    records = {tr["k"]: trial_record(rows[i], err2[i]) for i, tr in enumerate(trs)}
+    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i]) for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):
         s = f.getImuState()

@@ -7,6 +7,9 @@ state) the run's mean ANEES, the fraction of frames inside the two-sided 95 % ch
 Under torchrun the trials are sharded with shard.sequences_of_rank; the per-trial records (a few KB) are merged with
 shard.gather_summaries -- NCCL carries nothing else.
 
+With --position-fix-every K, every K frames each trial also fuses a noisy position fix (standard deviation
+--position-fix-sigma, metres) after the prune, and the summary adds the fixes' ANIS against its 95 % chi^2 bounds.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -77,6 +80,37 @@ def time_nees(n_members, reps=20):
     return out
 
 
+def time_aid(n_members, reps=20):
+    """wall time of one aided call (a position fix) on n_members fp64 filters at 30 clones: msckf_b200_aid_update for one
+    filter, msckf_b200_batch_aid_update for more"""
+    wl = synth.make_window_workload(n_features=4, n_clones=2, seq=3)
+    from msckf_mono_b200 import engine_filter
+    fs, es = [], []
+    for i in range(n_members):
+        f = engine_filter(np.float64, max_clones=38)
+        f.initialize(wl["camera"], wl["noise"], wl["params"], wl["imu_state"])
+        e = capi.Engine(np.float64, borrowed=f.engineHandle())
+        for _ in range(30):
+            r = np.zeros((2, 7)); r[:, 3:6] = [0, 0, 9.81]; r[:, 6] = 0.005
+            e.propagate_n(r)
+            e.augment()
+        fs.append(f); es.append(e)
+    specs = [{"model": capi.AID_POSITION, "z": e.state()[0][0:3] + 0.01, "R": 1e6 * np.eye(3)} for e in es]  # (barely moves P)
+    b = capi.Batch(es) if n_members > 1 else None
+    fn = (lambda: b.aid_update(specs)) if b else (lambda: es[0].aid_update(**specs[0]))
+    fn()
+    ts = []
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        fn()
+        ts.append(1e3 * (time.perf_counter() - t0))
+    if b:
+        b.close()
+    for f in fs:
+        f.close()
+    return float(np.median(ts))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--trials", type=int, default=32)
@@ -84,6 +118,8 @@ def main():
     ap.add_argument("--dtype", choices=("f32", "f64"), default="f64")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--seq", type=int, default=8)
+    ap.add_argument("--position-fix-every", type=int, default=0)
+    ap.add_argument("--position-fix-sigma", type=float, default=0.1)
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -97,17 +133,22 @@ def main():
     dtype = np.float32 if args.dtype == "f32" else np.float64
     truth = mc.make_truth(n_frames=args.frames, seq=args.seq)
     t0 = time.perf_counter()
-    records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed)
+    records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed,
+                        fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
     res = {"gpu": gpu_line(), "trials": args.trials, "frames": args.frames, "dtype": args.dtype, "seq": args.seq, "seed": args.seed,
            "world": world, "wall_s_rank0": wall, "pos_rmse_run_m": s["pos_rmse_run"],
            "components": {c: {k: v[k] for k in ("mean_anees", "mean_dof", "frames_inside", "frames_finite")} for c, v in s["components"].items()}}
+    if "fixes" in s:
+        res["position_fixes"] = {"every": args.position_fix_every, "sigma_m": args.position_fix_sigma,
+                                 **{k: s["fixes"][k] for k in ("mean_anis", "lower", "upper", "fixes_inside", "dof")}}
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
         res["nees_timing"] = {str(n): time_nees(n) for n in (8, 32)}
+        res["aid_call_ms"] = {str(n): time_aid(n) for n in (1, 8, 32)}
     if rank == 0:
         print(json.dumps(res), flush=True)
         if args.out:
