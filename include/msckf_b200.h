@@ -233,6 +233,47 @@ int msckf_b200_aid_update(msckf_b200_engine* e, const msckf_b200_aid* aid, msckf
 /* the same for every member of a batch (aid[i], out[i]; out[i] is not written for a member with aid[i].model < 0); every
  * member is validated before anything is launched.  One launch per 32 updated members. */
 int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
+/* ---- mapped landmarks: image observations of landmarks whose position is known (prior map, surveyed marker, relocalisation) --
+ * Observation i is (clone[i], z[i] normalised image coordinates, p_L_G[i] landmark position in G).  With C = C(q_CG) and p_C_G of
+ * that clone: p_C = C (p_L - p_C_G), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), Jacobian the 2 x 6
+ * block [J [p_C]x, -J C] over the clone's [dtheta, dp] (msckf.h:929-936) WITHOUT the observability projection (a known landmark
+ * observes global position and yaw) and without a feature null space (the landmark is not estimated; its position is taken as
+ * exact -- inflate R to account for map uncertainty).  Noise R (2 x 2, same for every observation; NULL: diag(u_var', v_var')).
+ * Per observation: flag 2 (not used) when p_C[2] <= 0 or z^ is not finite (gamma NaN); else gamma = r^T (X P_kk X^T + R)^-1 r,
+ * flag 1 (gated out) when chi2_obs > 0 and gamma > chi2_obs, else flag 0 (used).  The used rows are whitened and compressed per
+ * clone by a Householder QR (exact: each row touches one clone), then S = T P T^T + I = L L^T, W = L^-1 T P, y = L^-1 rho,
+ * NIS = |y|^2 + the QR leftovers (equal to the NIS of the dense stacked system), dx = W^T y, P <- P - W^T W (fp64, rounded once,
+ * both halves written, in place) and the state injection of msckf_b200_aid_update.  All arithmetic is fp64 for both dtypes.
+ * Three launches per 32 members with observations, one host-to-device copy, one device-to-host copy, one synchronisation.
+ * Caps: 256 observations per clone and 4096 per member and call.  The vision update's bookkeeping and the launch count are
+ * not changed. */
+typedef struct {
+  int n_obs;             /* observations; in a batch, 0 leaves the member untouched */
+  const int* clone;      /* [n_obs] positions in the window */
+  const double* z;       /* [n_obs][2] */
+  const double* p_L_G;   /* [n_obs][3] */
+  const double* R;       /* [3]: uu, uv, vv (positive definite), or NULL: diag(u_var', v_var') of the filter */
+  double chi2_obs;       /* > 0: per-observation gate on gamma */
+  double* gamma;         /* [n_obs] out, or NULL */
+  int* flag;             /* [n_obs] out (0 used, 1 gated out, 2 behind the camera / not finite), or NULL */
+} msckf_b200_landmarks;
+typedef struct {
+  double nis;            /* NIS of the used observations (NaN when S is not positive definite) */
+  double dx_norm;        /* |dx| of the applied update (0 when not applied) */
+  int dof;               /* 2 x used */
+  int rows;              /* rows of the compressed system (sum over clones of min(2 a_k, 6)) */
+  int used;              /* observations with flag 0 */
+  int applied;           /* 1: P and the state were updated */
+  int status;            /* 0: applied, or nothing used; 1: S not positive definite, nothing written */
+} msckf_b200_landmark_result;
+/* A clone outside the window, n_obs < 0 or beyond the caps, a NULL or non-finite z / p_L_G / R, an R that is not positive
+ * definite or a NaN chi2_obs returns MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
+ * A non-finite dx or P entry returns MSCKF_B200_ERR_NUMERIC with the result filled and the update applied.  n_obs = 0 on a single
+ * engine fills out with zeros and launches nothing. */
+int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out);
+/* the same for every member of a batch (lm[i], out[i]; out[i] is not written for a member with lm[i].n_obs = 0); every member is
+ * validated before anything is launched. */
+int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

@@ -32,6 +32,14 @@ namespace msckf_mono {
 
 template <typename _S> class MSCKFBatch;
 
+// An image observation of a landmark whose position is known (a prior map, a surveyed marker, a relocalisation match; not in
+// the reference): normalised image coordinates z of the landmark at p_L_G, seen from the image whose clone has id state_id.
+struct landmarkObservation {
+  int state_id;
+  double z[2];
+  double p_L_G[3];
+};
+
 template <typename _S>
 class MSCKF {
   friend class MSCKFBatch<_S>;
@@ -367,6 +375,47 @@ class MSCKF {
     state_dirty_ = true;
     if (r.applied) epoch_++;
   }
+  // mapped landmarks (not in the reference): one EKF update with image observations of landmarks whose position is known,
+  // fused on the device (msckf_b200_landmark_update; model, gate and outcomes there).  R: 2 x 2 pixel noise in normalised
+  // coordinates (NULL: diag(u_var', v_var')); chi2_obs > 0 gates every observation on its own.  gamma / flag (optional) receive
+  // one entry per observation.  An observation of an image that is not in the window throws std::invalid_argument before any
+  // device call.  Queued IMU readings are applied first, the host mirror is refreshed on the next getter, and an applied update
+  // between update() and marginalize() makes marginalize() refuse the queued tracks, as after aidedUpdate().
+  msckf_b200_landmark_result landmarkUpdate(const std::vector<landmarkObservation>& obs, const FixedMatrix<double, 2, 2>* R = nullptr,
+                                            double chi2_obs = 0, std::vector<double>* gamma = nullptr, std::vector<int>* flag = nullptr) {
+    msckf_b200_landmarks lm;
+    landmarkPack(obs, R, chi2_obs, gamma, flag, lm);
+    msckf_b200_landmark_result r = {};
+    checkNumeric(msckf_b200_landmark_update(eng(), &lm, &r), "msckf_b200_landmark_update");
+    landmarkAbsorb(r);
+    return r;
+  }
+  // a msckf_b200_landmarks of obs with window positions from the clone list (pointers into this object's buffers)
+  void landmarkPack(const std::vector<landmarkObservation>& obs, const FixedMatrix<double, 2, 2>* R, double chi2_obs,
+                    std::vector<double>* gamma, std::vector<int>* flag, msckf_b200_landmarks& lm) {
+    const size_t n = obs.size();
+    lmk_clone_.resize(n); lmk_z_.resize(2 * n); lmk_p_.resize(3 * n);
+    for (size_t i = 0; i < n; ++i) {
+      size_t pos = 0;
+      while (pos < cam_states_.size() && cam_states_[pos].state_id != obs[i].state_id) ++pos;
+      if (pos == cam_states_.size())
+        throw std::invalid_argument("MSCKF::landmarkUpdate: state_id " + std::to_string(obs[i].state_id) + " is not in the window");
+      lmk_clone_[i] = (int)pos;
+      lmk_z_[2 * i] = obs[i].z[0]; lmk_z_[2 * i + 1] = obs[i].z[1];
+      for (int c = 0; c < 3; ++c) lmk_p_[3 * i + c] = obs[i].p_L_G[c];
+    }
+    if (R) { lmk_R_[0] = (*R)(0, 0); lmk_R_[1] = (*R)(1, 0); lmk_R_[2] = (*R)(1, 1); }
+    if (gamma) gamma->assign(n, 0.0);
+    if (flag) flag->assign(n, 0);
+    lm.n_obs = (int)n; lm.clone = lmk_clone_.data(); lm.z = lmk_z_.data(); lm.p_L_G = lmk_p_.data();
+    lm.R = R ? lmk_R_ : nullptr; lm.chi2_obs = chi2_obs;
+    lm.gamma = gamma ? gamma->data() : nullptr; lm.flag = flag ? flag->data() : nullptr;
+  }
+  // host bookkeeping after a landmark update (the same as after an aided update)
+  void landmarkAbsorb(const msckf_b200_landmark_result& r) {
+    state_dirty_ = true;
+    if (r.applied) epoch_++;
+  }
   // marginalize() = launch + collect (kept separate for pipelining and for batches of filters, MSCKFBatch below).
   void marginalizeLaunch() {
     msckf_b200_tracks tr;
@@ -586,6 +635,9 @@ class MSCKF {
   std::vector<std::vector<size_t>> tri_involved_;
   std::vector<featureTrackToResidualize<_S>> tri_batch_, res_batch_;
   std::vector<double> aid_R_;  // R of the last convenience-form aided update, row-major
+  std::vector<int> lmk_clone_;  // the last landmark update's observations in the C-ABI's layout (landmarkPack)
+  std::vector<double> lmk_z_, lmk_p_;
+  double lmk_R_[3] = {0.0, 0.0, 0.0};
 
   // a msckf_b200_aid of one of the convenience forms (z must outlive the call; R is copied row-major into aid_R_)
   template <class Mat>
@@ -875,6 +927,30 @@ class MSCKFBatch {
     else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_update");
     for (size_t i = 0; i < size(); ++i)
       if (aid[i].model >= 0) filters_[i]->aidAbsorb(r[i]);
+    return r;
+  }
+  // MSCKF::landmarkUpdate of every filter (obs[i] empty: filter i is left alone) as one msckf_b200_batch_landmark_update: three
+  // launches per 32 updated filters and one synchronisation.  gamma / flag (optional) receive one list per filter.  An unknown
+  // state_id throws before any device call.  result[i] of a filter left alone is value-initialised.
+  std::vector<msckf_b200_landmark_result> landmarkUpdate(const std::vector<std::vector<landmarkObservation>>& obs,
+                                                         const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
+                                                         std::vector<std::vector<double>>* gamma = nullptr,
+                                                         std::vector<std::vector<int>>* flag = nullptr) {
+    const size_t n = size();
+    if (obs.size() != n) throw std::invalid_argument("MSCKFBatch::landmarkUpdate: one observation list per filter");
+    if (gamma) gamma->assign(n, std::vector<double>());
+    if (flag) flag->assign(n, std::vector<int>());
+    std::vector<msckf_b200_landmarks> lm(n, msckf_b200_landmarks());
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty())
+        filters_[i]->landmarkPack(obs[i], R, chi2_obs, gamma ? &(*gamma)[i] : nullptr, flag ? &(*flag)[i] : nullptr, lm[i]);
+    flushImu();
+    std::vector<msckf_b200_landmark_result> r(n, msckf_b200_landmark_result());
+    const int rc = msckf_b200_batch_landmark_update(batch_, lm.data(), r.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch landmark update: " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_landmark_update");
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty()) filters_[i]->landmarkAbsorb(r[i]);
     return r;
   }
   msckf_b200_batch* handle() { return batch_; }

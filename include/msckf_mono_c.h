@@ -77,6 +77,14 @@ int msckf_mono_batch_nees(void* batch, const double* const* truth_imu, const dou
  * alone), one device call for the batch. */
 int msckf_mono_aid_update(void* h, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
 int msckf_mono_batch_aid_update(void* batch, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
+/* mapped-landmark update (MSCKF::landmarkUpdate, msckf_b200_landmark_update: model, gate and errors there): n_obs observations,
+ * state_ids [n] (the image's state id; an id not in the window fails before any device call), z [n][2], p_L_G [n][3];
+ * R3 = uu, uv, vv or NULL (the filter's pixel noise); gamma [n] / flag [n] out, or NULL.  _batch_landmark_update: n_obs[i] per
+ * filter (0: filter i is left alone and out[i] is not written), the other arrays concatenated in filter order, one device call. */
+int msckf_mono_landmark_update(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
+                               double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out);
+int msckf_mono_batch_landmark_update(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
+                                     const double* R3, double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

@@ -70,6 +70,39 @@ def aid_struct(spec):
     return a, (z, R, H)
 
 
+class Landmarks(C.Structure):
+    _fields_ = [("n_obs", C.c_int), ("clone", C.c_void_p), ("z", C.c_void_p), ("p_L_G", C.c_void_p), ("R", C.c_void_p),
+                ("chi2_obs", C.c_double), ("gamma", C.c_void_p), ("flag", C.c_void_p)]
+
+
+class LandmarkResult(C.Structure):
+    _fields_ = [("nis", C.c_double), ("dx_norm", C.c_double), ("dof", C.c_int), ("rows", C.c_int), ("used", C.c_int),
+                ("applied", C.c_int), ("status", C.c_int)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def landmark_struct(spec):
+    """(Landmarks, the arrays it points into) of one call's mapped-landmark observations: spec = None (a batch member left
+    alone) or a dict clone [n] (window positions), z [n, 2], p_L [n, 3], R (None: the filter's pixel noise, else 2 x 2 or
+    (uu, uv, vv)), chi2_obs.  The arrays are (clone, z, p_L, R, gamma [n] out, flag [n] out)."""
+    if spec is None or len(spec["clone"]) == 0:
+        return Landmarks(0, None, None, None, None, 0.0, None, None), ()
+    clone = np.ascontiguousarray(spec["clone"], dtype=np.int32).ravel()
+    z = np.ascontiguousarray(spec["z"], dtype=np.float64).reshape(-1, 2)
+    p = np.ascontiguousarray(spec["p_L"], dtype=np.float64).reshape(-1, 3)
+    R = spec.get("R")
+    if R is not None:
+        R = np.asarray(R, dtype=np.float64)
+        R = np.ascontiguousarray([R[0, 0], R[1, 0], R[1, 1]] if R.shape == (2, 2) else R.ravel())
+    n = len(clone)
+    gamma, flag = np.zeros(n), np.zeros(n, dtype=np.int32)
+    a = Landmarks(n, clone.ctypes.data, z.ctypes.data, p.ctypes.data, None if R is None else R.ctypes.data,
+                  float(spec.get("chi2_obs", 0.0)), gamma.ctypes.data, flag.ctypes.data)
+    return a, (clone, z, p, R, gamma, flag)
+
+
 _lib = None
 
 
@@ -235,6 +268,17 @@ class Batch:
         check(lib().msckf_b200_batch_aid_update(self.h, (Aid * n)(*[a for a, _ in st]), out), "msckf_b200_batch_aid_update")
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
+    def landmark_update(self, specs):
+        """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
+        i alone); a list of result dicts with "gamma" and "flag" arrays (None for an engine left alone)"""
+        n = len(self.engines)
+        assert len(specs) == n
+        st = [landmark_struct(s) for s in specs]
+        out = (LandmarkResult * n)()
+        check(lib().msckf_b200_batch_landmark_update(self.h, (Landmarks * n)(*[a for a, _ in st]), out),
+              "msckf_b200_batch_landmark_update")
+        return [None if not k else dict(o.as_dict(), gamma=k[4], flag=k[5]) for (a, k), o in zip(st, out)]
+
     def jac_occupancy(self):
         """CTAs of k_jac resident per SM at the shape of the last launch (0 before the first)."""
         return int(lib().msckf_b200_batch_jac_occupancy(self.h))
@@ -365,6 +409,14 @@ class Engine:
         out = AidResult()
         check(lib().msckf_b200_aid_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_aid_update")
         return out.as_dict()
+
+    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0):
+        """msckf_b200_landmark_update: observations of known landmarks p_L [n, 3] at z [n, 2] from window positions clone [n];
+        the result as a dict with the per-observation "gamma" and "flag" arrays"""
+        a, keep = landmark_struct({"clone": clone, "z": z, "p_L": p_L, "R": R, "chi2_obs": chi2_obs})
+        out = LandmarkResult()
+        check(lib().msckf_b200_landmark_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_landmark_update")
+        return dict(out.as_dict(), gamma=keep[4] if keep else np.zeros(0), flag=keep[5] if keep else np.zeros(0, np.int32))
 
     def covariance(self):
         n = 15 + 6 * self.num_clones()

@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "feature_kernels.cuh"
 #include "gram_kernels.cuh"
+#include "landmark_kernels.cuh"
 #include "nees_kernels.cuh"
 #include "state_kernels.cuh"
 #include "tail_kernels.cuh"
@@ -128,6 +129,8 @@ struct CtxBase {
   virtual int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) = 0;
   // aided measurement updates of the members (msckf_b200_aid_update / _batch_aid_update): one launch per 32, one synchronisation
   virtual int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) = 0;
+  // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
+  virtual int landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) = 0;
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
@@ -295,6 +298,9 @@ struct Ctx : CtxBase {
   Arena aid_io;               // aided updates: every member's inputs (one host-to-device copy), then the results (one copy back)
   double* aid_ws = nullptr;   // aided updates: W^T and dx of the members whose share does not fit in shared memory
   size_t aid_ws_cap = 0;
+  Arena lmk_io;               // landmark updates: every member's observations (one host-to-device copy), then results, gamma, flags (one copy back)
+  double* lmk_ws = nullptr;   // landmark updates: the members' per-clone slots, [S ; (T P)^T ; rho] factors, dx and control words
+  size_t lmk_ws_cap = 0;
   size_t in_used = 0, rep_used = 0;
   int device = 0;
   bool owns_stream = false;
@@ -330,9 +336,10 @@ struct Ctx : CtxBase {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     drop_graphs();
-    in.release(); rep.release(); poses_out.release(); nees_io.release(); aid_io.release();
+    in.release(); rep.release(); poses_out.release(); nees_io.release(); aid_io.release(); lmk_io.release();
     if (nees_ws) cudaFree(nees_ws);
     if (aid_ws) cudaFree(aid_ws);
+    if (lmk_ws) cudaFree(lmk_ws);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
@@ -375,6 +382,7 @@ struct Ctx : CtxBase {
   int get_state(void* const* imu, void* const* poses) override;
   int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) override;
   int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) override;
+  int landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
@@ -658,6 +666,15 @@ struct Engine : EngineBase {
   // k_aid's arguments; in / ws / out are device addresses in the calling context's buffers (ws = nullptr: shared memory)
   mb::AidArgs<S> aid_args(const msckf_b200_aid& q, int m, const double* in, double* ws, mb::AidOut* out) const {
     return {d_st, d_P, d_poses, in, ws, out, q.chi2_max, ldp, M, q.model, q.model == MSCKF_B200_AID_CLONE_POSE ? q.clone : 0, m, 0};
+  }
+  // the landmark kernels' arguments except the device addresses, which the calling context fills in
+  mb::LmkArgs<S> lmk_args(const msckf_b200_landmarks& q, int G, int ld) const {
+    mb::LmkArgs<S> a;
+    memset(&a, 0, sizeof(a));
+    a.st = d_st; a.P = d_P; a.poses = d_poses;
+    if (q.R) { a.R[0] = q.R[0]; a.R[1] = q.R[1]; a.R[2] = q.R[2]; a.use_R = 1; }
+    a.chi2 = q.chi2_obs; a.ldp = ldp; a.M = M; a.G = G; a.ld = ld; a.ntiles = mb::lmk_tiles(15 + 6 * M);
+    return a;
   }
 
   // everything the kernels need for this filter's slice of the update
@@ -1487,6 +1504,139 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
   if (numeric >= 0) return fail(MSCKF_B200_ERR_NUMERIC, "aid_update: non-finite delta-x or covariance entry (member " + std::to_string(numeric) + "); the update was applied");
   return 0;
 }
+
+// Mapped-landmark updates: every member with observations sends its observations (grouped by clone in window order, input
+// order kept inside a clone) and its clone table in one pinned block with one host-to-device copy; results, gamma and flags come
+// back with one copy and one synchronisation.  Three launches per chunk of 32 such members (k_lmk_clone, k_lmk_gain,
+// k_lmk_downdate), whatever the observations turn out to be.  Nothing is launched unless every member is valid.
+static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_result, status),
+              "mb::LmkOut must start like msckf_b200_landmark_result");
+template <class S>
+int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) {
+  if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "landmark_update: null argument");
+  RC(members_ready("landmark_update"));
+  const int nf = (int)eng.size();
+  auto finite = [](const double* v, size_t k) { for (size_t i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false; return true; };
+  struct LmkPlan { std::vector<int> perm, grp; int G = 0, ld = 0; size_t in_off = 0, res_off = 0, ws_off = 0; };
+  std::vector<LmkPlan> pl(nf);
+  std::vector<int> idx;
+  size_t in_bytes = 0, res_bytes = 0, ws_bytes = 0;
+  for (int i = 0; i < nf; ++i) {
+    const msckf_b200_landmarks& q = in[i];
+    const std::string who = " (member " + std::to_string(i) + ")";
+    if (q.n_obs < 0 || q.n_obs > mb::kLmkMaxObs) return fail(MSCKF_B200_ERR_ARG, "landmark_update: n_obs outside 0 .. 4096" + who);
+    if (q.n_obs == 0) continue;
+    const int M = eng[i]->M, n = 15 + 6 * M, no = q.n_obs;
+    if (!q.clone || !q.z || !q.p_L_G) return fail(MSCKF_B200_ERR_ARG, "landmark_update: missing clone, z or p_L_G" + who);
+    std::vector<int> cnt(M, 0);
+    for (int j = 0; j < no; ++j) {
+      if (q.clone[j] < 0 || q.clone[j] >= M) return fail(MSCKF_B200_ERR_ARG, "landmark_update: clone outside the window" + who);
+      if (++cnt[q.clone[j]] > mb::kLmkMaxPerClone) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 observations of one clone" + who);
+    }
+    if (!finite(q.z, 2 * (size_t)no) || !finite(q.p_L_G, 3 * (size_t)no)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: non-finite z or p_L_G" + who);
+    if (q.R && (!finite(q.R, 3) || !(q.R[0] > 0.0) || !(q.R[0] * q.R[2] - q.R[1] * q.R[1] > 0.0)))
+      return fail(MSCKF_B200_ERR_ARG, "landmark_update: R is not finite and positive definite" + who);
+    if (std::isnan(q.chi2_obs)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: chi2_obs is NaN" + who);
+    LmkPlan& p = pl[i];
+    p.perm.resize(no);
+    std::vector<int> first(M + 1, 0);
+    for (int k = 0; k < M; ++k) first[k + 1] = first[k] + cnt[k];
+    std::vector<int> fill(first.begin(), first.end() - 1);
+    for (int j = 0; j < no; ++j) p.perm[fill[q.clone[j]]++] = j;  // stable: input order inside a clone
+    for (int k = 0; k < M; ++k)
+      if (cnt[k]) { p.grp.insert(p.grp.end(), {k, first[k], cnt[k]}); p.ld += std::min(2 * cnt[k], 6); }
+    p.G = (int)p.grp.size() / 3;
+    p.in_off = in_bytes;
+    in_bytes += up16(sizeof(double) * 5 * (size_t)no) + up16(sizeof(int) * p.grp.size());
+    p.res_off = res_bytes;
+    res_bytes += up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no) + up16(sizeof(int) * (size_t)no);
+    p.ws_off = ws_bytes;
+    ws_bytes += up256(sizeof(double) * ((size_t)mb::kLmkSlot * p.G + (size_t)(p.ld + n + 1) * p.ld + n) + sizeof(mb::LmkCtl));
+    idx.push_back(i);
+  }
+  if (idx.empty()) return 0;
+  const size_t res_base = up256(in_bytes);
+  CK(cudaSetDevice(device));
+  RC(lmk_io.ensure(res_base + res_bytes, stream));
+  if (ws_bytes > lmk_ws_cap) {
+    const size_t c = std::max(ws_bytes, 2 * lmk_ws_cap);
+    CK(cudaStreamSynchronize(stream));
+    if (lmk_ws) cudaFree(lmk_ws);
+    lmk_ws = nullptr; lmk_ws_cap = 0;
+    CK(cudaMalloc(&lmk_ws, c));
+    lmk_ws_cap = c;
+  }
+  std::vector<mb::LmkArgs<S>> args(nf);
+  for (int i : idx) {
+    const msckf_b200_landmarks& q = in[i];
+    const LmkPlan& p = pl[i];
+    const int no = q.n_obs, n = 15 + 6 * eng[i]->M;
+    double* ho = reinterpret_cast<double*>(lmk_io.h + p.in_off);
+    for (int j = 0; j < no; ++j) {
+      const int s = p.perm[j];
+      ho[5 * j] = q.z[2 * s]; ho[5 * j + 1] = q.z[2 * s + 1];
+      ho[5 * j + 2] = q.p_L_G[3 * s]; ho[5 * j + 3] = q.p_L_G[3 * s + 1]; ho[5 * j + 4] = q.p_L_G[3 * s + 2];
+    }
+    const size_t goff = p.in_off + up16(sizeof(double) * 5 * (size_t)no);
+    memcpy(lmk_io.h + goff, p.grp.data(), sizeof(int) * p.grp.size());
+    mb::LmkArgs<S> a = eng[i]->lmk_args(q, p.G, p.ld);
+    a.obs = reinterpret_cast<const double*>(lmk_io.d + p.in_off);
+    a.grp = reinterpret_cast<const int*>(lmk_io.d + goff);
+    unsigned char* r = lmk_io.d + res_base + p.res_off;
+    a.out = reinterpret_cast<mb::LmkOut*>(r);
+    a.gamma = reinterpret_cast<double*>(r + up16(sizeof(mb::LmkOut)));
+    a.flag = reinterpret_cast<int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no));
+    double* w = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(lmk_ws) + p.ws_off);
+    a.slot = w;
+    a.A = w + (size_t)mb::kLmkSlot * p.G;
+    a.dx = a.A + (size_t)(p.ld + n + 1) * p.ld;
+    a.ctl = reinterpret_cast<mb::LmkCtl*>(a.dx + n);
+    args[i] = a;
+  }
+  CK(cudaMemcpyAsync(lmk_io.d, lmk_io.h, in_bytes, cudaMemcpyHostToDevice, stream));
+  if (nf == 1) {
+    mb::Members<mb::LmkArgs<S>, 1> a;
+    a.m[0] = args[0];
+    mb::k_lmk_clone<S, 1><<<dim3(a.m[0].G, 1), mb::kLmkThreads, 0, stream>>>(a);
+    mb::k_lmk_gain<S, 1><<<1, mb::kLmkThreads, 0, stream>>>(a);
+    mb::k_lmk_downdate<S, 1><<<dim3(a.m[0].ntiles, 1), mb::kLmkThreads, 0, stream>>>(a);
+  } else {
+    for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
+      const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
+      mb::Members<mb::LmkArgs<S>, mb::kBatchMembers> a;
+      int gx = 1, tx = 1;  // the largest member's grid; other members' CTAs past their own range exit at once
+      for (int j = 0; j < nm; ++j) {
+        a.m[j] = args[idx[c + j]];
+        gx = std::max(gx, a.m[j].G);
+        tx = std::max(tx, a.m[j].ntiles);
+      }
+      mb::k_lmk_clone<S, mb::kBatchMembers><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
+      mb::k_lmk_gain<S, mb::kBatchMembers><<<nm, mb::kLmkThreads, 0, stream>>>(a);
+      mb::k_lmk_downdate<S, mb::kBatchMembers><<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(a);
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(lmk_io.h + res_base, lmk_io.d + res_base, res_bytes, cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
+  int numeric = -1;
+  for (int i : idx) {
+    const msckf_b200_landmarks& q = in[i];
+    const LmkPlan& p = pl[i];
+    const unsigned char* r = lmk_io.h + res_base + p.res_off;
+    const mb::LmkOut& o = *reinterpret_cast<const mb::LmkOut*>(r);
+    const double* g = reinterpret_cast<const double*>(r + up16(sizeof(mb::LmkOut)));
+    const int* fl = reinterpret_cast<const int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)q.n_obs));
+    out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].rows = o.rows; out[i].used = o.used;
+    out[i].applied = o.applied; out[i].status = o.status;
+    for (int j = 0; j < q.n_obs; ++j) {
+      if (q.gamma) q.gamma[p.perm[j]] = g[j];
+      if (q.flag) q.flag[p.perm[j]] = fl[j];
+    }
+    if (o.numeric && numeric < 0) numeric = i;
+  }
+  if (numeric >= 0) return fail(MSCKF_B200_ERR_NUMERIC, "landmark_update: non-finite delta-x or covariance entry (member " + std::to_string(numeric) + "); the update was applied");
+  return 0;
+}
 }  // namespace
 
 struct msckf_b200_engine { EngineBase* impl; };
@@ -1647,6 +1797,10 @@ int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, 
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->aid(aid, out);
 }
+int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->landmarks(lm, out);
+}
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,
                             int threads) {
@@ -1681,6 +1835,11 @@ int msckf_b200_aid_update(msckf_b200_engine* e, const msckf_b200_aid* aid, msckf
   if (!e || !aid) return fail(MSCKF_B200_ERR_ARG, "null argument");
   if (aid->model < 0) return fail(MSCKF_B200_ERR_ARG, "aid_update: unknown model");
   return e->impl->solo_ctx()->aid(aid, out);
+}
+int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
+  if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (lm->n_obs == 0) { memset(out, 0, sizeof(*out)); return 0; }
+  return e->impl->solo_ctx()->landmarks(lm, out);
 }
 int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->impl->set_covariance(in); }
 int msckf_b200_get_counters(msckf_b200_engine* e, long long* counters) { return e->impl->get_counters(counters); }

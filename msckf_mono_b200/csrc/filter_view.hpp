@@ -1,7 +1,8 @@
 // msckf_mono_b200/csrc/filter_view.hpp -- what the two translation units of the C view (include/msckf_mono_c.h) share:
 // filter_capi.cpp (one filter, msckf_mono::MSCKF<_S>), batch_capi.cpp (device batches, msckf_mono::MSCKFBatch<_S>),
-// nees_capi.cpp (consistency against ground truth, msckf_mono_nees / _batch_nees) and aid_capi.cpp (aided measurement
-// updates, msckf_mono_aid_update / _batch_aid_update).
+// nees_capi.cpp (consistency against ground truth, msckf_mono_nees / _batch_nees), aid_capi.cpp (aided measurement
+// updates, msckf_mono_aid_update / _batch_aid_update) and landmark_capi.cpp (mapped landmarks, msckf_mono_landmark_update /
+// _batch_landmark_update).
 #pragma once
 #include <cstdint>
 #include <exception>

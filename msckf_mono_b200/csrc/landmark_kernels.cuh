@@ -1,0 +1,391 @@
+// msckf_mono_b200/csrc/landmark_kernels.cuh
+// Image observations of landmarks whose position is known (a prior map, surveyed markers, relocalisation matches), fused into
+// the device-resident filter (msckf_b200_landmark_update / _batch_landmark_update).  Observation i = (clone k_i, z_i, p_L,i):
+// p_C = C(q_CG,k) (p_L - p_C_G,k), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), and the 2 x 6 block
+// X_i = [J_i [p_C]x, -J_i C] over the clone's [dtheta, dp] (msckf.h:929-936) WITHOUT the observability projection of
+// msckf.h:938-944: that projection removes global position and yaw, which a known landmark observes.  All arithmetic in fp64.
+//   k_lmk_clone    : one CTA per (touched clone, member).  Residual, per-observation gate gamma_i = r^T (X P_kk X^T + R)^-1 r
+//                    and flag, rows whitened by R = L_R L_R^T, then a Householder QR (one warp) of the clone's used rows
+//                    [X~ | r~] (2a x 7): q = min(2a, 6) rows [T_k | rho_k] and the leftover e_k^2 go to the member's workspace.
+//   k_lmk_gain     : one CTA per member.  T P (rows of T in window order), S = T P T^T + I, and one blocked right-looking
+//                    Cholesky of [S ; (T P)^T ; rho^T]: the extra rows end as W^T = (L^-1 T P)^T and y = L^-1 rho.
+//                    NIS = |y|^2 + sum_k e_k^2 (the NIS of the dense stacked system).
+//   k_lmk_downdate : 32 x 32 tiles of the lower triangle of P - W^T W (fp64, rounded once, both halves written, in place) and
+//                    dx = W^T y on the diagonal tiles; the last tile of a member (ticket counter) runs the state injection.
+// One body for a single filter (NM = 1) and a device batch (NM = kBatchMembers), like k_aid.  Each member's arithmetic depends
+// only on its own inputs: a batch equals single calls bit for bit.
+#pragma once
+#include "common.cuh"
+#include "state_kernels.cuh"
+
+namespace mb {
+
+constexpr int kLmkMaxPerClone = 256;  // observations of one clone in one call (2 x 256 rows of 7 doubles in shared memory)
+constexpr int kLmkMaxObs = 4096;      // observations of one member in one call
+constexpr int kLmkThreads = 256;
+constexpr int kLmkSlot = 48;          // doubles per touched clone: T [6][6], rho [6], e^2, used, q
+constexpr int kLmkNB = 32;            // panel width of the blocked Cholesky and tile size of the downdate
+
+// per-member result; the first seven fields are msckf_b200_landmark_result's
+struct LmkOut {
+  double nis, dx_norm;
+  int dof, rows, used, applied, status;
+  int numeric;  // a non-finite dx or P entry was written
+};
+// per-member control words in the workspace (k_lmk_gain -> k_lmk_downdate)
+struct LmkCtl {
+  int m, apply, bad;
+  unsigned ticket;  // tiles of k_lmk_downdate done (reset by k_lmk_gain and by the last tile)
+};
+
+template <class S>
+struct LmkArgs {
+  DevState<S>* st;
+  S* P;
+  S* poses;
+  const double* obs;  // [n_obs][5]: z (2), p_L (3), grouped by clone in window order
+  const int* grp;     // [G][3]: clone, first observation, count
+  double* slot;       // [G][kLmkSlot]
+  double* A;          // [ld + n + 1][ld]: S (lower), then (T P)^T -> W^T, then rho -> y
+  double* dx;         // [n]
+  LmkCtl* ctl;
+  LmkOut* out;
+  double* gamma;      // [n_obs] (packed order)
+  int* flag;          // [n_obs]
+  double R[3];        // uu, uv, vv (use_R), else the filter's diag(u_var, v_var)
+  double chi2;        // > 0: per-observation gate
+  int ldp, M, G, ld, ntiles, use_R;
+};
+static_assert(sizeof(Members<LmkArgs<double>, kBatchMembers>) <= 32764, "the landmark kernels' batched arguments exceed the parameter limit");
+
+__host__ __device__ constexpr int lmk_tiles(int n) { return ((n + kLmkNB - 1) / kLmkNB) * ((n + kLmkNB - 1) / kLmkNB + 1) / 2; }
+
+// one observation against clone pose (C, p_C_G): rows [X | r] (2 x 7), flag (0 used, 1 gated out, 2 behind the camera or not
+// finite) and gamma = r^T (X P_kk X^T + R)^-1 r (NaN for flag 2)
+__device__ __forceinline__ double lmk_obs(const double* o, const double* Cr, const double* pc, const double (*Pk)[6], const double* Rm,
+                                          double chi2, double (&row)[2][7], int& fg) {
+  const double d[3] = {o[2] - pc[0], o[3] - pc[1], o[4] - pc[2]};
+  double p[3];
+  for (int i = 0; i < 3; ++i) p[i] = Cr[3 * i] * d[0] + Cr[3 * i + 1] * d[1] + Cr[3 * i + 2] * d[2];
+  const double zh0 = p[0] / p[2], zh1 = p[1] / p[2];
+  fg = 2;
+  if (!(p[2] > 0.0 && isfinite(zh0) && isfinite(zh1))) return __longlong_as_double(0x7ff8000000000000ll);
+  const double iz = 1.0 / p[2];
+  const double J[2][3] = {{iz, 0.0, -zh0 * iz}, {0.0, iz, -zh1 * iz}};
+  const double sk[3][3] = {{0.0, -p[2], p[1]}, {p[2], 0.0, -p[0]}, {-p[1], p[0], 0.0}};
+  for (int r = 0; r < 2; ++r)
+    for (int c = 0; c < 3; ++c) {
+      row[r][c] = J[r][0] * sk[0][c] + J[r][1] * sk[1][c] + J[r][2] * sk[2][c];
+      row[r][3 + c] = -(J[r][0] * Cr[c] + J[r][1] * Cr[3 + c] + J[r][2] * Cr[6 + c]);
+    }
+  row[0][6] = o[0] - zh0;
+  row[1][6] = o[1] - zh1;
+  double s00 = Rm[0], s10 = Rm[1], s11 = Rm[2];
+  for (int c = 0; c < 6; ++c) {
+    double x0 = 0.0, x1 = 0.0;
+    for (int j = 0; j < 6; ++j) { x0 += row[0][j] * Pk[j][c]; x1 += row[1][j] * Pk[j][c]; }
+    s00 += x0 * row[0][c];
+    s10 += x1 * row[0][c];
+    s11 += x1 * row[1][c];
+  }
+  const double r0 = row[0][6], r1 = row[1][6];
+  const double gam = (s11 * r0 * r0 - 2.0 * s10 * r0 * r1 + s00 * r1 * r1) / (s00 * s11 - s10 * s10);
+  fg = (chi2 > 0.0 && gam > chi2) ? 1 : 0;
+  return gam;
+}
+
+template <class S, int NM>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs<S>, NM> a) {
+  const int f = NM == 1 ? 0 : blockIdx.y, g = blockIdx.x;
+  if (g >= a.m[f].G) return;
+  const S* __restrict__ const P = a.m[f].P;
+  const int ldp = a.m[f].ldp, t = threadIdx.x, lane = t & 31;
+  const int k = a.m[f].grp[3 * g], i0 = a.m[f].grp[3 * g + 1], cnt = a.m[f].grp[3 * g + 2];
+  const double* __restrict__ const obs = a.m[f].obs + 5 * (size_t)(i0 + t);
+  const double chi2 = a.m[f].chi2;
+  __shared__ double Q[2 * kLmkMaxPerClone][7];  // used rows [X~ | r~], input order, then R and the Householder vectors
+  __shared__ double Pk[6][6], Cr[9], pc[3], LR[3], Rm[3];
+  __shared__ int fl[kLmkMaxPerClone], pos[kLmkMaxPerClone], s_used;
+
+  if (t < 36) Pk[t / 6][t % 6] = (double)P[(size_t)(15 + 6 * k + t / 6) * ldp + 15 + 6 * k + t % 6];
+  if (t == 0) {
+    const S* ps = a.m[f].poses + kPoseStride * k;
+    const double q[4] = {(double)ps[0], (double)ps[1], (double)ps[2], (double)ps[3]};
+    quat_to_rot(q, Cr);
+    pc[0] = (double)ps[4]; pc[1] = (double)ps[5]; pc[2] = (double)ps[6];
+    if (a.m[f].use_R) {
+      Rm[0] = a.m[f].R[0]; Rm[1] = a.m[f].R[1]; Rm[2] = a.m[f].R[2];
+    } else {
+      Rm[0] = (double)a.m[f].st->u_var; Rm[1] = 0.0; Rm[2] = (double)a.m[f].st->v_var;
+    }
+    LR[0] = sqrt(Rm[0]);
+    LR[1] = Rm[1] / LR[0];
+    LR[2] = sqrt(Rm[2] - LR[1] * LR[1]);
+  }
+  __syncthreads();
+  // ---- per observation: residual, Jacobian block, gate; then the used rows, compacted in input order (recomputed rather than
+  // kept in registers across the compaction)
+  double row[2][7];
+  int fg = 2;
+  if (t < cnt) {
+    const double gam = lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
+    a.m[f].gamma[i0 + t] = gam;
+    a.m[f].flag[i0 + t] = fg;
+    fl[t] = fg;
+  }
+  __syncthreads();
+  if (t == 0) {
+    int u = 0;
+    for (int i = 0; i < cnt; ++i) { pos[i] = u; u += fl[i] == 0; }
+    s_used = u;
+  }
+  __syncthreads();
+  if (t < cnt && fg == 0) {
+    lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
+    for (int c = 0; c < 7; ++c) {  // whiten: L_R^-1 [X | r]
+      const double y0 = row[0][c] / LR[0];
+      Q[2 * pos[t]][c] = y0;
+      Q[2 * pos[t] + 1][c] = (row[1][c] - LR[1] * y0) / LR[2];
+    }
+  }
+  __syncthreads();
+  // ---- Householder QR of the used rows (one warp): R's first q rows are [T_k | rho_k], rows q.. of column 6 give e_k^2
+  const int nr = 2 * s_used, q = min(nr, 6);
+  if (t < 32) {
+    for (int j = 0; j < q; ++j) {
+      double s = 0.0;
+      for (int r = j + lane; r < nr; r += 32) s += Q[r][j] * Q[r][j];
+      s = warp_sum(s);
+      const double x0 = Q[j][j];
+      __syncwarp();
+      if (s > 0.0) {
+        const double al = x0 >= 0.0 ? -sqrt(s) : sqrt(s);
+        const double tau = 1.0 / (s - al * x0);
+        if (lane == 0) Q[j][j] = x0 - al;
+        __syncwarp();
+        for (int c = j + 1; c < 7; ++c) {
+          double d = 0.0;
+          for (int r = j + lane; r < nr; r += 32) d += Q[r][j] * Q[r][c];
+          d = tau * warp_sum(d);
+          for (int r = j + lane; r < nr; r += 32) Q[r][c] -= d * Q[r][j];
+        }
+        __syncwarp();
+        if (lane == 0) Q[j][j] = al;
+      }
+      __syncwarp();
+    }
+    double e2 = 0.0;
+    for (int r = q + lane; r < nr; r += 32) e2 += Q[r][6] * Q[r][6];
+    e2 = warp_sum(e2);
+    double* sl = a.m[f].slot + (size_t)kLmkSlot * g;
+    for (int i = lane; i < 42; i += 32) {
+      const int r = i / 7, c = i - 7 * r;
+      const double v = (r < q && c >= r) ? Q[r][c] : 0.0;
+      if (c < 6) sl[6 * r + c] = v;
+      else sl[36 + r] = v;
+    }
+    if (lane == 0) { sl[42] = e2; sl[43] = (double)s_used; sl[44] = (double)q; }
+  }
+}
+
+template <class S, int NM>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgs<S>, NM> a) {
+  const int f = NM == 1 ? 0 : blockIdx.x;
+  const S* __restrict__ const P = a.m[f].P;
+  double* __restrict__ const A = a.m[f].A;
+  const double* __restrict__ const slot = a.m[f].slot;
+  LmkCtl* const ctl = a.m[f].ctl;
+  LmkOut* const out = a.m[f].out;
+  const int ldp = a.m[f].ldp, G = a.m[f].G, ld = a.m[f].ld, n = 15 + 6 * a.m[f].M, t = threadIdx.x, lane = t & 31;
+  __shared__ int off[kMaxKeep + 1], ck[kMaxKeep], rg[6 * kMaxKeep];
+  __shared__ double D[kLmkNB][kLmkNB + 1], B[kLmkNB][kLmkNB + 1], idg[kLmkNB];
+  __shared__ double s_e2;
+  __shared__ int s_used, s_nv;
+
+  if (t == 0) {
+    int o = 0, u = 0;
+    double e2 = 0.0;
+    for (int g = 0; g < G; ++g) {
+      off[g] = o;
+      o += (int)slot[(size_t)kLmkSlot * g + 44];
+      u += (int)slot[(size_t)kLmkSlot * g + 43];
+      e2 += slot[(size_t)kLmkSlot * g + 42];
+    }
+    off[G] = o; s_used = u; s_e2 = e2;
+    ctl->ticket = 0u; ctl->bad = 0; ctl->m = o;
+  }
+  for (int g = t; g < G; g += kLmkThreads) ck[g] = a.m[f].grp[3 * g];
+  __syncthreads();
+  const int m = off[G], Rt = m + n + 1;
+  if (s_used == 0) {  // no observation used: nothing is written
+    if (t == 0) {
+      ctl->apply = 0;
+      out->nis = 0.0; out->dx_norm = 0.0; out->dof = 0; out->rows = 0; out->used = 0; out->applied = 0; out->status = 0;
+      out->numeric = 0;
+    }
+    return;
+  }
+  for (int g = t; g < G; g += kLmkThreads)
+    for (int r = off[g]; r < off[g + 1]; ++r) rg[r] = g;
+  __syncthreads();
+  // ---- (T P)^T into rows m .. m + n - 1, rho into row m + n
+  for (int idx = t; idx < m * n; idx += kLmkThreads) {
+    const int r = idx / n, c = idx - r * n, g = rg[r], lr = r - off[g];
+    const double* T = slot + (size_t)kLmkSlot * g + 6 * lr;
+    const S* pc = P + (size_t)(15 + 6 * ck[g]) * ldp + c;
+    double s = 0.0;
+    for (int j = lr; j < 6; ++j) s += T[j] * (double)pc[(size_t)j * ldp];
+    A[(size_t)(m + c) * ld + r] = s;
+  }
+  for (int r = t; r < m; r += kLmkThreads) A[(size_t)(m + n) * ld + r] = slot[(size_t)kLmkSlot * rg[r] + 36 + r - off[rg[r]]];
+  __syncthreads();
+  // ---- S = T P T^T + I, lower triangle
+  for (int idx = t; idx < m * m; idx += kLmkThreads) {
+    const int r = idx / m, s_ = idx - r * m;
+    if (s_ > r) continue;
+    const int h = rg[s_], ls = s_ - off[h];
+    const double* T = slot + (size_t)kLmkSlot * h + 6 * ls;
+    const double* tp = A + (size_t)(m + 15 + 6 * ck[h]) * ld + r;
+    double v = r == s_ ? 1.0 : 0.0;
+    for (int j = ls; j < 6; ++j) v += tp[(size_t)j * ld] * T[j];
+    A[(size_t)r * ld + s_] = v;
+  }
+  __syncthreads();
+  // ---- blocked right-looking Cholesky of [S ; (T P)^T ; rho^T] (Rt x m): the extra rows end as W^T and y
+  int bad = 0;
+  for (int k0 = 0; k0 < m; k0 += kLmkNB) {
+    const int nb = min(kLmkNB, m - k0);
+    for (int idx = t; idx < kLmkNB * kLmkNB; idx += kLmkThreads) {
+      const int i = idx / kLmkNB, j = idx - i * kLmkNB;
+      if (j <= i) D[i][j] = (i < nb) ? A[(size_t)(k0 + i) * ld + k0 + j] : 0.0;
+    }
+    __syncthreads();
+    if (t < 32) {
+      const int nv = warp_chol(D, nb, idg, t);
+      if (t == 0) s_nv = nv;
+    }
+    __syncthreads();
+    if (s_nv < nb) { bad = 1; break; }
+    for (int r = k0 + nb + (t >> 5); r < Rt; r += kLmkThreads / 32) {
+      double* row = A + (size_t)r * ld + k0;
+      const double x = warp_row_solve(lane < nb ? row[lane] : 0.0, D, idg, nb, lane);
+      if (lane < nb) row[lane] = x;
+    }
+    __syncthreads();
+    const int k1 = k0 + nb;
+    if (k1 < m) {  // A[r, c] -= L[r, k0:k1] . L[c, k0:k1] for k1 <= c <= r, c < m, r < Rt
+      const int nti = (Rt - k1 + kLmkNB - 1) / kLmkNB, ntj = (m - k1 + kLmkNB - 1) / kLmkNB;
+      for (int ti = 0; ti < nti; ++ti)
+        for (int tj = 0; tj <= ti && tj < ntj; ++tj) {
+          const int rb = k1 + kLmkNB * ti, cb = k1 + kLmkNB * tj;
+          for (int idx = t; idx < kLmkNB * kLmkNB; idx += kLmkThreads) {
+            const int i = idx / kLmkNB, p = idx - i * kLmkNB;
+            D[i][p] = (rb + i < Rt && p < nb) ? A[(size_t)(rb + i) * ld + k0 + p] : 0.0;
+            B[i][p] = (cb + i < m && p < nb) ? A[(size_t)(cb + i) * ld + k0 + p] : 0.0;
+          }
+          __syncthreads();
+          const int i = t >> 3, r = rb + i;
+          double s[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll 8
+          for (int p = 0; p < kLmkNB; ++p) {
+            const double di = D[i][p];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) s[u] += di * B[(t & 7) + 8 * u][p];
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const int c = cb + (t & 7) + 8 * u;
+            if (r < Rt && c < m && c <= r) A[(size_t)r * ld + c] -= s[u];
+          }
+          __syncthreads();
+        }
+    }
+  }
+  if (t == 0) {
+    if (bad) {  // S not positive definite: nothing is written
+      ctl->apply = 0;
+      out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
+      out->status = 1; out->applied = 0;
+    } else {
+      const double* y = A + (size_t)(m + n) * ld;
+      double g = s_e2;
+      for (int i = 0; i < m; ++i) g += y[i] * y[i];
+      ctl->apply = 1;
+      out->nis = g; out->status = 0; out->applied = 1;
+    }
+    out->dof = 2 * s_used; out->rows = m; out->used = s_used; out->numeric = 0;
+  }
+}
+
+template <class S, int NM>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_downdate(const Members<LmkArgs<S>, NM> a) {
+  const int f = NM == 1 ? 0 : blockIdx.y, tl = blockIdx.x;
+  if (tl >= a.m[f].ntiles) return;
+  LmkCtl* const ctl = a.m[f].ctl;
+  if (!ctl->apply) return;
+  S* __restrict__ const P = a.m[f].P;
+  const int ldp = a.m[f].ldp, ld = a.m[f].ld, M = a.m[f].M, n = 15 + 6 * M, m = ctl->m, t = threadIdx.x;
+  const double* __restrict__ const Wt = a.m[f].A + (size_t)m * ld;  // row c: W[:, c]
+  const double* __restrict__ const y = a.m[f].A + (size_t)(m + n) * ld;
+  double* const dx = a.m[f].dx;
+  __shared__ double D[kLmkNB][kLmkNB + 1], B[kLmkNB][kLmkNB + 1];
+  __shared__ int s_last;
+  int ti, tj;
+  tri_tile_index(tl, ti, tj);
+  const int rb = kLmkNB * ti, cb = kLmkNB * tj, i = t >> 3, r = rb + i;
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int p0 = 0; p0 < m; p0 += kLmkNB) {
+    for (int idx = t; idx < kLmkNB * kLmkNB; idx += kLmkThreads) {
+      const int ii = idx / kLmkNB, p = idx - ii * kLmkNB;
+      D[ii][p] = (rb + ii < n && p0 + p < m) ? Wt[(size_t)(rb + ii) * ld + p0 + p] : 0.0;
+      B[ii][p] = (cb + ii < n && p0 + p < m) ? Wt[(size_t)(cb + ii) * ld + p0 + p] : 0.0;
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int p = 0; p < kLmkNB; ++p) {
+      const double di = D[i][p];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) s[u] += di * B[(t & 7) + 8 * u][p];
+    }
+    __syncthreads();
+  }
+  int bad = 0;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int c = cb + (t & 7) + 8 * u;
+    if (r < n && c < n && c <= r) {
+      const S x = (S)((double)P[(size_t)r * ldp + c] - s[u]);
+      if (!isfinite((double)x)) bad = 1;
+      P[(size_t)r * ldp + c] = x;
+      P[(size_t)c * ldp + r] = x;
+    }
+  }
+  if (ti == tj && t < kLmkNB && rb + t < n) {  // dx = W^T y for this tile's rows
+    const double* w = Wt + (size_t)(rb + t) * ld;
+    double v = 0.0;
+    for (int p = 0; p < m; ++p) v += w[p] * y[p];
+    dx[rb + t] = v;
+  }
+  __threadfence();
+  bad = __syncthreads_or(bad);
+  if (t == 0) {
+    if (bad) atomicOr(&ctl->bad, 1);
+    __threadfence();
+    s_last = atomicAdd(&ctl->ticket, 1u) == (unsigned)a.m[f].ntiles - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  // ---- the last tile of the member: the state injection of the vision update (k_syrk, k_aid)
+  __threadfence();
+  inject_state(a.m[f].st, a.m[f].poses, M, t, kLmkThreads, [&](int k) { return __ldcg(dx + k); });
+  if (t == 0) {
+    double nn = 0.0;
+    for (int k = 0; k < n; ++k) { const double v = __ldcg(dx + k); nn += v * v; }
+    LmkOut* const out = a.m[f].out;
+    out->dx_norm = sqrt(nn);
+    out->numeric = (atomicOr(&ctl->bad, 0) || !isfinite(nn)) ? 1 : 0;
+    ctl->ticket = 0u;
+  }
+}
+
+}  // namespace mb

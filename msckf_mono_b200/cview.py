@@ -133,6 +133,32 @@ class FilterBatch:
         self._call("aid_update", (Aid * n)(*[a for a, _ in st]), out)
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
+    def landmark_update(self, obs, R=None, chi2_obs=0.0):
+        """MSCKFBatch::landmarkUpdate: obs[i] = (state_ids [n], z [n, 2], p_L [n, 3]) for filter i, or None (filter i left
+        alone); R None (each filter's pixel noise) or 2 x 2; one device call for the batch.  A list of result dicts with
+        "gamma" and "flag" (None for a filter left alone)."""
+        from .capi import LandmarkResult
+        n = len(self.filters)
+        assert len(obs) == n
+        cnt = np.array([0 if o is None else len(o[0]) for o in obs], dtype=np.int32)
+        parts = [o for o in obs if o is not None and len(o[0])]
+        ids = np.ascontiguousarray(np.concatenate([np.asarray(o[0]) for o in parts]) if parts else np.zeros(1), dtype=np.int32)
+        z = np.ascontiguousarray(np.concatenate([np.asarray(o[1], float).reshape(-1, 2) for o in parts]) if parts else np.zeros((1, 2)))
+        p = np.ascontiguousarray(np.concatenate([np.asarray(o[2], float).reshape(-1, 3) for o in parts]) if parts else np.zeros((1, 3)))
+        r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
+        tot = max(int(cnt.sum()), 1)
+        gamma, flag = np.zeros(tot), np.zeros(tot, dtype=np.int32)
+        out = (LandmarkResult * n)()
+        self._call("landmark_update", cnt.ctypes.data_as(_ip), ids.ctypes.data_as(_ip), z.ctypes.data_as(_dp), p.ctypes.data_as(_dp),
+                   None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs), gamma.ctypes.data_as(_dp),
+                   flag.ctypes.data_as(_ip), out)
+        res, o0 = [], 0
+        for i in range(n):
+            c = int(cnt[i])
+            res.append(None if c == 0 else dict(out[i].as_dict(), gamma=gamma[o0:o0 + c].copy(), flag=flag[o0:o0 + c].copy()))
+            o0 += c
+        return res
+
     def handle(self):
         fn = self.lib.msckf_mono_batch_handle
         fn.restype = C.c_void_p
@@ -304,6 +330,23 @@ class CFilter:
         out = AidResult()
         self._chk(self._f("aid_update")(self.h, C.byref(a), C.byref(out)), "aid_update")
         return out.as_dict()
+
+    def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0):
+        """MSCKF::landmarkUpdate (include/msckf_b200.h: msckf_b200_landmark_update): observations of known landmarks p_L [n, 3]
+        at z [n, 2] from the images state_ids [n]; R None (the filter's pixel noise) or 2 x 2; chi2_obs > 0: per-observation
+        gate.  A dict nis, dx_norm, dof, rows, used, applied, status, gamma [n], flag [n]."""
+        from .capi import LandmarkResult
+        ids = np.ascontiguousarray(state_ids, dtype=np.int32).ravel()
+        n = len(ids)
+        z, pz = _d(np.asarray(z, float).reshape(-1, 2) if n else np.zeros((1, 2)))
+        p, pp = _d(np.asarray(p_L, float).reshape(-1, 3) if n else np.zeros((1, 3)))
+        r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
+        gamma, flag = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int32)
+        out = LandmarkResult()
+        self._chk(self._f("landmark_update")(self.h, C.c_int(n), ids.ctypes.data_as(_ip), pz, pp,
+                                             None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs),
+                                             gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip), C.byref(out)), "landmark_update")
+        return dict(out.as_dict(), gamma=gamma[:n].copy(), flag=flag[:n].copy())
 
     # ---- test hooks --------------------------------------------------------------------
     def lastReport(self):

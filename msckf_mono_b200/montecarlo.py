@@ -15,6 +15,15 @@ z = p_true + N(0, sigma^2 I) into its filter (MSCKFBatch::aidedUpdate, one batch
 its own stream np.random.default_rng([seed, k, 1]), so the trial's other inputs are the same with fixes on or off.  The NIS
 of the fixes gives a truth-free consistency figure (ANIS against chi^2 with 3 dof per trial).
 
+Optional mapped landmarks (a prior map): every `map_every` frames, after the prune (and after a position fix when both are on),
+each trial observes the map -- every `map_stride`-th landmark of the truth stream -- where it is visible from the truth pose of
+its newest clone (synth.visible, the stream's own rule), and fuses z = z_true + N(0, diag(u_var', v_var')) with known landmark
+positions (MSCKFBatch::landmarkUpdate, one batched call).  The noise of trial k comes from its own stream
+np.random.default_rng([seed, k, 2]), so the trial's other inputs are the same with the map on or off.  These map observations
+are drawn independently of the tracked-feature pixels of the same landmark in the same image: an idealisation (a real front end
+would see one pixel noise in both), which leaves the two measurements uncorrelated.  The NIS of the map updates gives another
+truth-free consistency figure (ANIS against chi^2 with 2 dof per used observation).
+
 Error-state convention (the inverse of the filter's state injection q+ = buildUpdateQuat(dtheta) * q): dq = q_true * q_est^-1
 with the Hamilton product, dq negated when dq.w < 0, dtheta = -2 vec(dq); every other component is truth - estimate.  Host
 vectors here are in the filter's covariance order [dtheta, db_g, dv, db_a, dp, clones (dtheta_C, dp_C)...].
@@ -123,9 +132,19 @@ def make_truth(n_frames=200, seq=0, max_features=60, max_track_length=20, max_ca
     return wl
 
 
-def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0):
+def map_observations(truth, frame, stride):
+    """(map indices, noise-free normalised coordinates) of the map landmarks visible from the truth camera pose of `frame`"""
+    C, p = synth.cam_pose(truth["traj"], truth["frames"][frame]["time"], truth["camera"])
+    pts = truth["landmarks"][::stride]
+    vis, xn, yn = synth.visible(C, p, pts)
+    idx = np.flatnonzero(vis)
+    return idx, np.stack([xn[idx], yn[idx]], axis=1)
+
+
+def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
-    fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I)."""
+    fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
+    map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -159,6 +178,16 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0):
         frng = np.random.default_rng([seed, k, 1])
         out["fixes"] = [truth["truth_imu"][f][0:3] + fix_sigma * frng.standard_normal(3) if (f + 1) % fix_every == 0 else None
                         for f in range(len(truth["frames"]))]
+    if map_every > 0:
+        mrng = np.random.default_rng([seed, k, 2])
+        su, sv = np.sqrt(nz["u_var_prime"]), np.sqrt(nz["v_var_prime"])
+        out["maps"] = []
+        for f in range(len(truth["frames"])):
+            if (f + 1) % map_every:
+                out["maps"].append(None)
+                continue
+            idx, z = map_observations(truth, f, map_stride)
+            out["maps"].append((idx, truth["landmarks"][::map_stride][idx], z + mrng.standard_normal(z.shape) * np.array([su, sv])))
     return out
 
 
@@ -170,14 +199,15 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2, fix_nis=()):
-    """one trial's per-frame NEES (list of result dicts), squared position errors and the NIS of its position fixes, as
-    plain lists"""
+def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=()):
+    """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes and of its
+    map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n), as plain lists"""
     return {"nees": {c: [float(r[c]) for r in nees_rows] for c in COMPONENTS},
             "dim": {c: [int(r["dim_full"]) if c == "full" else DOF[c] for r in nees_rows] for c in COMPONENTS},
             "first_bad_pivot": [int(r["first_bad_pivot"]) for r in nees_rows],
             "pos_err2": [float(x) for x in pos_err2],
-            "fix_nis": [float(x) for x in fix_nis]}
+            "fix_nis": [float(x) for x in fix_nis],
+            "map": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in map_rows] for key in ("nis", "dof", "used", "applied", "n")}}
 
 
 def chi2_bounds(total_dof, n, lo=0.025, hi=0.975):
@@ -217,21 +247,38 @@ def summarize(records):
         anis = F.mean(axis=0)
         out["fixes"] = {"anis": [float(a) for a in anis], "lower": lo, "upper": hi, "dof": 3, "mean_anis": float(anis.mean()),
                         "fixes_inside": float(np.mean((anis >= lo) & (anis <= hi)))}
+    mp = [records[k].get("map") for k in keys]
+    if all(m is not None and len(m["nis"]) for m in mp):  # ANIS of the map updates: 2 dof per used observation
+        V = np.array([m["nis"] for m in mp]); D = np.array([m["dof"] for m in mp])
+        anis, lo, hi = V.sum(axis=0) / N, [], []
+        for d in D.sum(axis=0):
+            b = chi2_bounds(int(d), N) if d > 0 else (float("nan"), float("nan"))
+            lo.append(b[0]); hi.append(b[1])
+        inside = [lo_ <= a <= hi_ for a, lo_, hi_ in zip(anis, lo, hi)]
+        tot = chi2_bounds(int(D.sum()), N * len(anis))
+        n_obs = sum(sum(m["n"]) for m in mp)
+        out["map"] = {"anis": [float(a) for a in anis], "lower": lo, "upper": hi, "dof": [int(d) for d in D.sum(axis=0)],
+                      "mean_anis": float(V.sum() / (N * len(anis))), "mean_dof": float(D.sum() / (N * len(anis))),
+                      "run_bounds": list(tot), "updates_inside": float(np.mean(inside)),
+                      "applied": float(np.mean([a for m in mp for a in m["applied"]])),
+                      "observations": int(n_obs), "gated": float(1.0 - sum(sum(m["used"]) for m in mp) / max(n_obs, 1))}
     return out
 
 
 # ---- the batched run ---------------------------------------------------------------------------------------------------------
-def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0):
+def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
+    [every map_every frames one batched mapped-landmark update from the newest clone, gated per observation at map_chi2 > 0],
     refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.
     Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
     from . import engine_filter
     from .capi import AID_POSITION
     from .cview import FilterBatch
-    trs = [make_trial(truth, k, seed, fix_every, fix_sigma) for k in trials]
+    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride) for k in trials]
     R_fix = (fix_sigma ** 2) * np.eye(3)
     nis = [[] for _ in trs]
+    maps = [[] for _ in trs]
     fs = [engine_filter(dtype) for _ in trs]
     for f, tr in zip(fs, trs):
         f.initialize(truth["camera"], truth["noise"], truth["params"], tr["imu_state"])
@@ -253,6 +300,12 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             res = fb.aid_update([{"model": AID_POSITION, "z": tr["fixes"][fi], "R": R_fix} for tr in trs])
             for i, r in enumerate(res):
                 nis[i].append(r["nis"])
+        if map_every > 0 and trs[0]["maps"][fi] is not None:
+            obs = [(np.full(len(tr["maps"][fi][0]), fr["state_id"]), tr["maps"][fi][2], tr["maps"][fi][1]) if len(tr["maps"][fi][0]) else None
+                   for tr, fr in zip(trs, frs)]
+            res = fb.landmark_update(obs, chi2_obs=map_chi2)
+            for i, r in enumerate(res):
+                maps[i].append({"nis": 0.0, "dof": 0, "used": 0, "applied": 0, "n": 0} if r is None else dict(r, n=len(r["flag"])))
         fb.refreshState()
         timu, tposes = [], []
         for i, (f, tr) in enumerate(zip(fs, trs)):
@@ -266,7 +319,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         if on_frame is not None:
             on_frame(fi, fs, res)
     fb.close()
-    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i]) for i, tr in enumerate(trs)}
+    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i]) for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):
         s = f.getImuState()

@@ -262,6 +262,21 @@ def corrupt_observations(wl, frac_gross=0.1, frac_mild=0.15, seed=0):
     return wl
 
 
+def visible(C, p, pts_G):
+    """the stream's visibility rule for a camera with rotation C (global -> cam) at p: depth in (1, 25) m and the pixel at
+    least 5 px inside the image.  Returns (vis [N] bool, xn, yn) with the normalised coordinates of every point."""
+    f_u, f_v, c_u, c_v = INTRINSICS
+    pc = (C @ (pts_G - p).T).T
+    z = pc[:, 2]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        xn = pc[:, 0] / z
+        yn = pc[:, 1] / z
+    u = f_u * xn + c_u
+    v = f_v * yn + c_v
+    vis = (z > 1.0) & (z < 25.0) & (u > 5) & (u < RESOLUTION[0] - 5) & (v > 5) & (v < RESOLUTION[1] - 5)
+    return vis, xn, yn
+
+
 def make_stream_workload(n_frames=200, seq=0, max_features=100, imu_per_frame=10, dT=0.005,
                          pixel_sigma=1.0, imu_noise_frac=0.05, n_landmarks=6000,
                          max_track_length=50, max_cam_states=30, isotropic=False, dropout=0.02):
@@ -285,8 +300,7 @@ def make_stream_workload(n_frames=200, seq=0, max_features=100, imu_per_frame=10
     rad = traj.r + rng.uniform(3.0, 15.0, n_landmarks)
     hgt = rng.uniform(-6.0, 6.0, n_landmarks)
     pts_G = np.stack([rad * np.cos(ang), rad * np.sin(ang), hgt], axis=1)
-    f_u, f_v, c_u, c_v = INTRINSICS
-    sig = pixel_sigma / f_u
+    sig = pixel_sigma / INTRINSICS[0]
     tracked = []  # landmark indices currently tracked (order = front-end order)
     next_id = 1
     lm_id = {}
@@ -294,14 +308,7 @@ def make_stream_workload(n_frames=200, seq=0, max_features=100, imu_per_frame=10
     for k in range(n_frames):
         t = t0 + k * frame_dt
         C, p = cam_pose(traj, t, cam)
-        pc = (C @ (pts_G - p).T).T
-        z = pc[:, 2]
-        with np.errstate(divide="ignore", invalid="ignore"):
-            xn = pc[:, 0] / z
-            yn = pc[:, 1] / z
-        u = f_u * xn + c_u
-        v = f_v * yn + c_v
-        vis = (z > 1.0) & (z < 25.0) & (u > 5) & (u < RESOLUTION[0] - 5) & (v > 5) & (v < RESOLUTION[1] - 5)
+        vis, xn, yn = visible(C, p, pts_G)
         still = [i for i in tracked if vis[i] and rng.random() > dropout]
         cand = np.flatnonzero(vis)
         rng.shuffle(cand)

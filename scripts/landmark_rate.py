@@ -1,0 +1,145 @@
+#!/usr/bin/env python
+"""scripts/landmark_rate.py -- call time of the mapped-landmark update (msckf_b200_landmark_update / _batch_landmark_update) in
+fp64 at 30 clones, for 1 / 8 / 32 filters and 25 / 100 / 400 observations spread over the newest 1 / 5 / 30 clones: host wall
+clock around the synchronising call, median of 20 after a warm-up.  For <= 16 observations on one filter it also times the path
+available without it: get_state, the projection linearised in numpy, then one aid_update(LINEAR).  Per-kernel device times
+(k_lmk_clone, k_lmk_gain, k_lmk_downdate) come from torch.profiler over repeated calls.  Reads the card's name and power limit
+in the same process.  Prints one JSON line."""
+import json
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+ROOT = Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
+from msckf_mono_b200 import capi, synth  # noqa: E402
+
+M = 30
+R_PIX = np.diag([2.0e-5, 2.0e-5])
+
+
+def gpu_line():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
+
+
+def rot(q):
+    x, y, z, w = q
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+def filters(n):
+    from msckf_mono_b200 import engine_filter
+    wl = synth.make_window_workload(n_features=4, n_clones=2, seq=3)
+    rng = np.random.default_rng(7)
+    fs, es = [], []
+    for _ in range(n):
+        f = engine_filter(np.float64, max_clones=M + 8)
+        f.initialize(wl["camera"], wl["noise"], wl["params"], wl["imu_state"])
+        e = capi.Engine(np.float64, borrowed=f.engineHandle())
+        for _ in range(M):
+            r = np.zeros((2, 7)); r[:, 0:3] = rng.normal(0, 0.3, (2, 3)); r[:, 3:6] = [0, 0, 9.81]; r[:, 6] = 0.005
+            e.propagate_n(r)
+            e.augment()
+        nn = 15 + 6 * M
+        A = rng.normal(size=(nn, nn))
+        e.set_covariance(1e-4 * (A @ A.T / nn + np.eye(nn)))
+        fs.append(f); es.append(e)
+    return fs, es
+
+
+def observations(rng, e, n_obs, n_clones):
+    """n_obs observations spread evenly over the newest n_clones clones, landmarks 2 .. 8 m in front, measured exactly"""
+    _, poses = e.state()
+    poses = poses.astype(np.float64)
+    clone = np.array([M - 1 - (i % n_clones) for i in range(n_obs)], dtype=np.int32)
+    d = rng.uniform(2.0, 8.0, n_obs)
+    pc = np.stack([rng.uniform(-0.4, 0.4, n_obs) * d, rng.uniform(-0.3, 0.3, n_obs) * d, d], axis=1)
+    p_L = np.array([rot(poses[k, 3:7]).T @ v + poses[k, 0:3] for k, v in zip(clone, pc)])
+    return {"clone": clone, "z": pc[:, 0:2] / pc[:, 2:3], "p_L": p_L, "R": R_PIX}
+
+
+def timed(fn, reps=20):
+    fn()
+    ts = []
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        fn()
+        ts.append(1e3 * (time.perf_counter() - t0))
+    return float(np.median(ts))
+
+
+def host_linear(e, spec):
+    """the path without the feature: get_state, numpy linearisation, one aid_update(LINEAR)"""
+    _, poses = e.state()
+    poses = poses.astype(np.float64)
+    n = 15 + 6 * M
+    m = 2 * len(spec["clone"])
+    H, r = np.zeros((m, n)), np.zeros(m)
+    for i, (k, zi, pl) in enumerate(zip(spec["clone"], spec["z"], spec["p_L"])):
+        C = rot(poses[k, 3:7])
+        X, Y, Z = C @ (pl - poses[k, 0:3])
+        J = np.array([[1, 0, -X / Z], [0, 1, -Y / Z]]) / Z
+        sk = np.array([[0, -Z, Y], [Z, 0, -X], [-Y, X, 0]])
+        H[2 * i:2 * i + 2, 15 + 6 * k:21 + 6 * k] = np.hstack([J @ sk, -J @ C])
+        r[2 * i:2 * i + 2] = zi - np.array([X, Y]) / Z
+    return e.aid_update(capi.AID_LINEAR, r, np.kron(np.eye(m // 2), spec["R"]), H=H)
+
+
+def kernel_times(fn, reps=50):
+    """mean device time per call of each landmark kernel, from torch.profiler"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            fn()
+        torch.cuda.synchronize()
+    out = {}
+    for ev in prof.key_averages():
+        for name in ("k_lmk_clone", "k_lmk_gain", "k_lmk_downdate"):
+            if name in ev.key:
+                out[name] = out.get(name, 0.0) + ev.device_time_total / 1e3 / reps  # ms per call
+    return out
+
+
+def main():
+    rng = np.random.default_rng(3)
+    res = {"gpu": gpu_line(), "dtype": "f64", "clones": M, "call_ms": {}, "host_linear_ms": {}, "kernel_ms": {}}
+    for nf in (1, 8, 32):
+        fs, es = filters(nf)
+        b = capi.Batch(es) if nf > 1 else None
+        for n_obs in (25, 100, 400):
+            for nc in (1, 5, 30):
+                key = f"{nf}x{n_obs}obs/{nc}clones"
+                if n_obs > 256 * nc:
+                    res["call_ms"][key] = "over the 256-per-clone cap"
+                    continue
+                specs = [observations(rng, e, n_obs, nc) for e in es]
+                fn = (lambda: b.landmark_update(specs)) if b else (lambda: es[0].landmark_update(**specs[0]))
+                res["call_ms"][key] = timed(fn)
+                if nf in (1, 32) and n_obs == 100 and nc == 5:
+                    try:
+                        res["kernel_ms"][key] = kernel_times(fn)
+                    except Exception as ex:  # (the profiler is an extra; the call times above stand on their own)
+                        res["kernel_ms"][key] = f"not measured: {ex}"
+        if nf == 1:
+            for n_obs in (4, 16):
+                spec = observations(rng, es[0], n_obs, 1)
+                res["host_linear_ms"][f"1x{n_obs}obs/1clone"] = timed(lambda: host_linear(es[0], spec))
+                res["call_ms"][f"1x{n_obs}obs/1clone"] = timed(lambda: es[0].landmark_update(**spec))
+        if b:
+            b.close()
+        for f in fs:
+            f.close()
+    print(json.dumps(res), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -10,6 +10,10 @@ shard.gather_summaries -- NCCL carries nothing else.
 With --position-fix-every K, every K frames each trial also fuses a noisy position fix (standard deviation
 --position-fix-sigma, metres) after the prune, and the summary adds the fixes' ANIS against its 95 % chi^2 bounds.
 
+With --map-every K, every K frames each trial also observes the map (every --map-stride-th landmark of the truth stream) from
+its newest clone and fuses the observations as mapped landmarks (after the prune and after a position fix), and the summary adds
+the map updates' ANIS against its 95 % chi^2 bounds and the fraction of observations gated out.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -120,6 +124,8 @@ def main():
     ap.add_argument("--seq", type=int, default=8)
     ap.add_argument("--position-fix-every", type=int, default=0)
     ap.add_argument("--position-fix-sigma", type=float, default=0.1)
+    ap.add_argument("--map-every", type=int, default=0)
+    ap.add_argument("--map-stride", type=int, default=20)
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -134,7 +140,8 @@ def main():
     truth = mc.make_truth(n_frames=args.frames, seq=args.seq)
     t0 = time.perf_counter()
     records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed,
-                        fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma)
+                        fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma, map_every=args.map_every,
+                        map_stride=args.map_stride)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -144,6 +151,9 @@ def main():
     if "fixes" in s:
         res["position_fixes"] = {"every": args.position_fix_every, "sigma_m": args.position_fix_sigma,
                                  **{k: s["fixes"][k] for k in ("mean_anis", "lower", "upper", "fixes_inside", "dof")}}
+    if "map" in s:
+        res["map"] = {"every": args.map_every, "stride": args.map_stride,
+                      **{k: s["map"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "observations", "gated")}}
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
