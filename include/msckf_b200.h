@@ -52,7 +52,8 @@ typedef struct {
 /* The three capacities are INITIAL sizes: like the reference, whose window and track lists are unbounded std::vectors, the
  * engine grows its device buffers on demand (x2, contents preserved).  Hard limits that remain: 98 observations per track
  * (the reference's chi-square table has 99 entries, msckf.h:91 -- longer tracks index past it there) and the window the
- * tail kernel's shared-memory panels can hold (about 135 clones): both fail with MSCKF_B200_ERR_CAPACITY / _ARG. */
+ * tail kernel's shared-memory panels can hold (136 clones; an update of a larger window fails at staging and writes nothing):
+ * they fail with MSCKF_B200_ERR_ARG / _CAPACITY. */
 
 /* One batch of feature tracks, flat SoA (types.h:102-113 featureTrackToResidualize without the clone copies:
  * the clone poses are device resident and addressed by POSITION in the sliding window, msckf.h:1481). */
@@ -140,6 +141,9 @@ long long msckf_b200_batch_launch_count(const msckf_b200_batch* b);
 /* CTAs of the feature kernel (k_jac) resident per SM at the shape of the batch's last launch: the CUDA occupancy calculator's
  * figure for its threads per track and dynamic shared memory (0 before the first launch) */
 int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b);
+/* threads per track k_jac ran with at the last update launch of the engine's context (its batch while it belongs to one):
+ * option 6's request, widened while a group of the launch's longest track does not fit in shared memory; 0 before any launch */
+int msckf_b200_jac_group(msckf_b200_engine* e);
 void* msckf_b200_batch_stream(msckf_b200_batch* b);
 /* The other device calls of a frame for every member at once (the per-image sequence of datasets/asl_msckf.cpp:233-294 on a
  * batch).  Arrays have one entry per engine, in the order given to _create.  Each call validates every member before it

@@ -142,6 +142,28 @@ class TrackBatch:
         return self.off.nbytes + self.obs.nbytes + self.idx.nbytes + (0 if self.pfg is None else self.pfg.nbytes)
 
 
+def _report(n_tracks, dtype, full=True):
+    """(Report, its per-track host arrays): accepted [n] and, with full, cm_ok, tri_ok, valid [n], gamma [n] and p_f_G [n, 3] in
+    the filter's dtype"""
+    k = max(n_tracks, 1)
+    arr = {"accepted": np.zeros(k, np.int32)}
+    if full:
+        arr.update(cm_ok=np.zeros(k, np.int32), tri_ok=np.zeros(k, np.int32), valid=np.zeros(k, np.int32),
+                   gamma=np.zeros(k, dtype), p_f_G=np.zeros((k, 3), dtype))
+    rep = Report()
+    for key in ("cm_ok", "tri_ok", "valid", "accepted"):
+        if key in arr:
+            setattr(rep, key, arr[key].ctypes.data_as(C.POINTER(C.c_int)))
+    if full:
+        rep.gamma, rep.p_f_G = arr["gamma"].ctypes.data, arr["p_f_G"].ctypes.data
+    return rep, arr
+
+
+def _result(rep, arr, n_tracks):
+    """the report as a dict: m, rank and the per-track arrays (the flags and p_f_G of the modes that compute them)"""
+    return dict({k: v[:n_tracks] for k, v in arr.items()}, m=rep.m, rank=rep.rank)
+
+
 class Batch:
     """msckf_b200_batch: n engines whose updates run as ONE device batch (filter index in blockIdx.z, one CUDA graph, one
     packed copy each way).  While it lives the engines share its stream."""
@@ -181,29 +203,22 @@ class Batch:
         check(lib().msckf_b200_batch_launch_timed(self.h, C.byref(ms)), "msckf_b200_batch_launch_timed")
         return ms.value
 
-    def fetch(self, batches=None):
-        batches = batches or self._keep
-        n = len(self.engines)
-        reps = (Report * n)()
-        accs = []
-        for i, b in enumerate(batches):
-            acc = np.zeros(max(b.n_tracks, 1), dtype=np.int32)
-            reps[i].accepted = acc.ctypes.data_as(C.POINTER(C.c_int))
-            accs.append(acc)
-        check(lib().msckf_b200_batch_fetch(self.h, reps), "msckf_b200_batch_fetch")
-        return [{"m": reps[i].m, "rank": reps[i].rank, "accepted": accs[i][:batches[i].n_tracks]} for i in range(n)]
+    def _reports(self, batches, full):
+        st = [_report(b.n_tracks, e.dtype, full) for b, e in zip(batches, self.engines)]
+        return (Report * len(st))(*[r for r, _ in st]), [a for _, a in st]
 
-    def update(self, mode, batches, threads=1):
+    def fetch(self, batches=None, full=False):
+        """per engine m, rank, accepted and, with full, the other per-track results (see Engine.update)"""
+        batches = batches or self._keep
+        reps, arrs = self._reports(batches, full)
+        check(lib().msckf_b200_batch_fetch(self.h, reps), "msckf_b200_batch_fetch")
+        return [_result(r, a, b.n_tracks) for r, a, b in zip(reps, arrs, batches)]
+
+    def update(self, mode, batches, threads=1, full=False):
         """host buffers in, reports out: packing + one H2D + kernels + one D2H (the batch's end-to-end call)."""
-        n = len(self.engines)
-        reps = (Report * n)()
-        accs = []
-        for i, b in enumerate(batches):
-            acc = np.zeros(max(b.n_tracks, 1), dtype=np.int32)
-            reps[i].accepted = acc.ctypes.data_as(C.POINTER(C.c_int))
-            accs.append(acc)
+        reps, arrs = self._reports(batches, full)
         check(lib().msckf_b200_batch_update(self.h, C.c_int(mode), self._tracks(batches), reps, C.c_int(threads)), "msckf_b200_batch_update")
-        return [{"m": reps[i].m, "rank": reps[i].rank, "accepted": accs[i][:batches[i].n_tracks]} for i in range(n)]
+        return [_result(r, a, b.n_tracks) for r, a, b in zip(reps, arrs, batches)]
 
     def kernel_times(self):
         ms = (C.c_float * 32)()
@@ -361,16 +376,16 @@ class Engine:
         check(lib().msckf_b200_prune(self.h, k.ctypes.data_as(C.POINTER(C.c_int)), C.c_int(len(k))), "msckf_b200_prune")
 
     def update(self, mode, batch):
-        rep = Report()
-        acc = np.zeros(max(batch.n_tracks, 1), dtype=np.int32)
-        rep.accepted = acc.ctypes.data_as(C.POINTER(C.c_int))
+        """one update; the report as a dict: m, rank and the per-track cm_ok, tri_ok, valid, accepted, gamma, p_f_G"""
+        rep, arr = _report(batch.n_tracks, self.dtype)
         check(lib().msckf_b200_update(self.h, C.c_int(mode), C.byref(batch.c), C.byref(rep)), "msckf_b200_update")
-        return {"m": rep.m, "rank": rep.rank, "accepted": acc[:batch.n_tracks]}
+        return _result(rep, arr, batch.n_tracks)
 
     def rank_pivots(self):
-        buf = (C.c_double * 2048)()
-        n = check(lib().msckf_b200_rank_pivots(self.h, buf, C.c_int(2048)), "msckf_b200_rank_pivots")
-        return np.array(buf[:n])
+        n = check(lib().msckf_b200_rank_pivots(self.h, None, C.c_int(0)), "msckf_b200_rank_pivots")
+        out = np.zeros(n)
+        check(lib().msckf_b200_rank_pivots(self.h, out.ctypes.data_as(C.POINTER(C.c_double)), C.c_int(n)), "msckf_b200_rank_pivots")
+        return out
 
     def set_option(self, key, value):
         check(lib().msckf_b200_set_option(self.h, C.c_int(key), C.c_double(value)), "msckf_b200_set_option")
@@ -386,6 +401,10 @@ class Engine:
 
     def num_clones(self):
         return lib().msckf_b200_num_clones(self.h)
+
+    def jac_group(self):
+        """threads per track k_jac ran with at the last update launch (after any widening; 0 before the first)"""
+        return int(lib().msckf_b200_jac_group(self.h))
 
     def state(self):
         """(imu [29]: p, v, b_g, b_a, g, q_IG, p_null, v_null, q_null; clone poses [M, 7]: p, q), dtype scalars"""
@@ -435,6 +454,6 @@ class Engine:
         self.set_covariance(P)
 
     def delta_x(self):
-        out = np.zeros(15 + 6 * 128)
+        out = np.zeros(15 + 6 * self.num_clones())
         n = check(lib().msckf_b200_last_delta_x(self.h, out.ctypes.data_as(C.POINTER(C.c_double)), C.c_int(len(out))), "last_delta_x")
         return out[:n].copy()

@@ -75,7 +75,11 @@ struct Arena {
     CK(cudaMalloc(&d, c));
     CK(cudaMallocHost(&h, c));
     memset(h, 0, c);
-    CK(cudaMemset(d, 0, c));
+    // zeroed on the stream that uses the arena: cudaMemset would run on the legacy default stream, which the engine's
+    // non-blocking streams do not wait for, so it could land after the first input copy into the arena or after the first
+    // kernels wrote their reports there (a device batch's first update then read back m = 0 for a member)
+    CK(cudaMemsetAsync(d, 0, c, s));
+    if (!s) CK(cudaStreamSynchronize(nullptr));
     cap = c;
     return 0;
   }
@@ -681,7 +685,6 @@ struct Engine : EngineBase {
   void fill_args(mb::UpdArgs<S>& a, const Plan<S>& p, int mode) const {
     memset(&a, 0, sizeof(a));
     a.n_tracks = p.N; a.M = M; a.Lmax = p.Lmax; a.ldp = ldp; a.ld = ld; a.n = 15 + 6 * M; a.mode = mode;
-    if (p.N > 0 && mode != MSCKF_B200_TRIANGULATE) pivr_n = a.n;  // (the window may shrink before msckf_b200_rank_pivots is asked)
     a.K = 3 * p.N;
     int nsplit = std::max(1, std::min(kMaxSplit, a.K / 96));
     int kchunk = (a.K + nsplit - 1) / nsplit;
@@ -1023,6 +1026,12 @@ int Ctx<S>::launch() {
   sh.jac_smem = (unsigned)mb::jac_smem_bytes<S>(jac_L, jac_M, sh.jac_g);
   if (sh.tri_smem > kSmemBudget) return fail(MSCKF_B200_ERR_CAPACITY, "k_tri shared memory");
   if (mode != MSCKF_B200_TRIANGULATE && sh.jac_smem > kSmemBudget) return fail(MSCKF_B200_ERR_CAPACITY, "k_jac shared memory");
+  // the dimension of the update whose rank decision msckf_b200_rank_pivots reports: set once the launch is committed, so that
+  // a stage or launch that fails on a capacity leaves the last update's diagnostics alone; the window may shrink before they
+  // are asked for
+  if (mode != MSCKF_B200_TRIANGULATE)
+    for (int i = 0; i < nf; ++i)
+      if (plan[i].N > 0) eng[i]->pivr_n = h_args()[i].n;
   const int Nr = (Nmax + 15) & ~15;  // rounded track count: kernels exit on blockIdx >= their filter's own N
   // (k_jac's at the SM's allocation granularity of 128 B: a whole KB would cost a batch of 8 config-B filters its tenth CTA per SM)
   sh.tri_smem = (sh.tri_smem + 1023) & ~1023u; sh.jac_smem = (sh.jac_smem + 127) & ~127u;
@@ -1772,6 +1781,10 @@ int msckf_b200_batch_update(msckf_b200_batch* b, int mode, const msckf_b200_trac
 int msckf_b200_batch_kernel_times(msckf_b200_batch* b, float* ms, const char** names, int cap) { return b->ctx->kernel_times(ms, names, cap); }
 long long msckf_b200_batch_launch_count(const msckf_b200_batch* b) { return b->ctx->launches; }
 int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b) { return b->ctx->jac_ctas; }
+int msckf_b200_jac_group(msckf_b200_engine* e) {
+  const CtxBase* c = e->impl->group ? e->impl->group : e->impl->solo_ctx();
+  return c->jac_g;
+}
 void* msckf_b200_batch_stream(msckf_b200_batch* b) { return (void*)b->ctx->stream; }
 int msckf_b200_batch_propagate_n(msckf_b200_batch* b, const void* const* readings, const int* k) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
