@@ -88,7 +88,39 @@ struct Arena {
     if (h) cudaFreeHost(h);
     d = h = nullptr; cap = 0;
   }
+  ~Arena() { release(); }
 };
+
+// device-only workspace that grows on demand (at least x2); the stream is synchronised before the old block is freed
+struct DevBuf {
+  unsigned char* d = nullptr;
+  size_t cap = 0;
+  int ensure(size_t need, cudaStream_t s) {
+    if (need <= cap) return 0;
+    const size_t c = std::max(need, 2 * cap);
+    CK(cudaStreamSynchronize(s));
+    release();
+    CK(cudaMalloc(&d, c));
+    cap = c;
+    return 0;
+  }
+  void release() {
+    if (d) cudaFree(d);
+    d = nullptr; cap = 0;
+  }
+  ~DevBuf() { release(); }
+};
+
+inline bool finite(const double* v, size_t k) {
+  for (size_t i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false;
+  return true;
+}
+
+// the outcome of an aided or landmark update whose first member with a non-finite delta-x or covariance entry is `member` (-1: none)
+int numeric_error(const char* what, int member) {
+  if (member < 0) return 0;
+  return fail(MSCKF_B200_ERR_NUMERIC, std::string(what) + ": non-finite delta-x or covariance entry (member " + std::to_string(member) + "); the update was applied");
+}
 
 // tail kernel choice (engine option 3 / window size)
 inline size_t tail_legacy_smem(int n, int NB) {
@@ -294,17 +326,13 @@ template <class S>
 struct Ctx : CtxBase {
   std::vector<Engine<S>*> eng;
   std::vector<Plan<S>> plan;
+  // The update's inputs and reports: a staged or launched update lives in them across calls (and the class packs its tracks
+  // into `in` through msckf_b200_input_buffer before stage), so no other call may use them.
   Arena in, rep;
-  Arena poses_out;  // clone poses of a batched get_state (pinned: all members' copies are asynchronous)
-  Arena nees_io;    // NEES: every member's truth (one host-to-device copy), then every member's result (one copy back)
-  double* nees_ws = nullptr;  // NEES: the members' fp64 Cholesky workspaces, (n + 1) x n each
-  size_t nees_ws_cap = 0;
-  Arena aid_io;               // aided updates: every member's inputs (one host-to-device copy), then the results (one copy back)
-  double* aid_ws = nullptr;   // aided updates: W^T and dx of the members whose share does not fit in shared memory
-  size_t aid_ws_cap = 0;
-  Arena lmk_io;               // landmark updates: every member's observations (one host-to-device copy), then results, gamma, flags (one copy back)
-  double* lmk_ws = nullptr;   // landmark updates: the members' per-clone slots, [S ; (T P)^T ; rho] factors, dx and control words
-  size_t lmk_ws_cap = 0;
+  // The side calls (get_state, nees, aid, landmarks) copy in, launch, copy back and synchronise before they return, so no two
+  // are ever live at once: they share one pinned block for their inputs and results, and one device workspace.
+  Arena io;
+  DevBuf ws;
   size_t in_used = 0, rep_used = 0;
   int device = 0;
   bool owns_stream = false;
@@ -323,12 +351,10 @@ struct Ctx : CtxBase {
   cudaEvent_t ev[kMaxEv] = {};
   const char* ev_name[kMaxEv] = {};
   int n_ev = 0;
-  int n_sm = 0;
 
   int init(int dev) {
     device = dev;
     CK(cudaSetDevice(device));
-    CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     CK(cudaStreamCreateWithFlags(&stream2, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&stream3, cudaStreamNonBlocking));
     CK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
@@ -340,10 +366,6 @@ struct Ctx : CtxBase {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
     drop_graphs();
-    in.release(); rep.release(); poses_out.release(); nees_io.release(); aid_io.release(); lmk_io.release();
-    if (nees_ws) cudaFree(nees_ws);
-    if (aid_ws) cudaFree(aid_ws);
-    if (lmk_ws) cudaFree(lmk_ws);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
@@ -380,6 +402,33 @@ struct Ctx : CtxBase {
   int launch_timed(float* ms) override;
   int fetch(msckf_b200_report* reports) override;
   int members_ready(const char* what) const;
+  // the launching halves of the state calls, for a batch and for the single filter's own calls (each checks its arguments first)
+  int enqueue_propagate_n(const void* const* readings, const int* k);
+  int enqueue_augment(const std::vector<int>& idx);
+  int enqueue_prune(const std::vector<int>& idx, const int* const* keep, const int* n_keep);
+  int read_state(void* const* imu, void* const* poses);
+  // The one launch path of the per-member kernels.  args(i) gives member i's arguments; launch(a, nm) launches once for an
+  // mb::Members<Args, NM> a filled with nm members.  NM = 1 when the context has one member (a single filter, or a batch of
+  // one), else mb::kBatchMembers with one launch per chunk of that many.  counted: every launch counts on the context and on
+  // the engine of each member it runs (the state calls).
+  template <class ArgsOf, class Launch>
+  void per_member(const std::vector<int>& idx, bool counted, ArgsOf&& args, Launch&& launch) {
+    if (eng.size() == 1) chunks<1>(idx, counted, args, launch);
+    else chunks<mb::kBatchMembers>(idx, counted, args, launch);
+  }
+  template <int NM, class ArgsOf, class Launch>
+  void chunks(const std::vector<int>& idx, bool counted, ArgsOf& args, Launch& launch) {
+    for (size_t c = 0; c < idx.size(); c += NM) {
+      const int nm = (int)std::min<size_t>(NM, idx.size() - c);
+      mb::Members<decltype(args(0)), NM> a;
+      for (int j = 0; j < nm; ++j) {
+        a.m[j] = args(idx[c + j]);
+        if (counted) eng[idx[c + j]]->launches++;
+      }
+      launch(a, nm);
+      if (counted) launches++;
+    }
+  }
   int propagate_n(const void* const* readings, const int* k) override;
   int augment(const int* which) override;
   int prune(const int* const* keep, const int* n_keep) override;
@@ -534,9 +583,11 @@ struct Engine : EngineBase {
     CK(cudaMemsetAsync(d_prof, 0, sizeof(unsigned long long) * 80, stream));
     RC(alloc_window());
     RC(alloc_batchws());
-    // the private context's packed arenas, sized for a full batch (no pinned allocation inside the first update)
+    // the private context's packed arenas, sized for a full batch and a full window (no pinned allocation inside the first
+    // update or get_state)
     RC(solo.in.ensure(solo.args_bytes() + up256(Plan<S>::in_bytes(Tmax, Omax)), nullptr));
     RC(solo.rep.ensure(up256(Plan<S>::rep_bytes(Tmax)), nullptr));
+    RC(solo.io.ensure(up16(sizeof(S) * mb::kPoseStride * Mmax), nullptr));
     CK(cudaMallocHost(&h_st, sizeof(mb::DevState<S>)));
     memset(h_st, 0, sizeof(mb::DevState<S>));
     RC(set_func_attrs(device));
@@ -630,37 +681,22 @@ struct Engine : EngineBase {
   int propagate_n(const void* r_, int k) override {
     if (!initialized) return fail(MSCKF_B200_ERR_STATE, "propagate before initialize");
     if (k < 0 || (k > 0 && !r_)) return fail(MSCKF_B200_ERR_ARG, "propagate_n: bad arguments");
-    const S* r = (const S*)r_;
-    CK(cudaSetDevice(device));
-    for (int k0 = 0; k0 < k; k0 += mb::kPropMax) {
-      mb::Members<mb::PropBatch<S>, 1> a;
-      prop_args(a.m[0], r, k0, std::min(mb::kPropMax, k - k0));
-      mb::k_propagate<S, 1><<<1, 256, 0, stream>>>(a);
-      launches++;
-    }
-    CK(cudaGetLastError());
-    return 0;
+    return solo.enqueue_propagate_n(&r_, &k);
   }
   // k_propagate's arguments for readings k0 .. k0 + n - 1 of r (n <= kPropMax)
-  void prop_args(mb::PropBatch<S>& pb, const S* r, int k0, int n) const {
+  mb::PropBatch<S> prop_args(const S* r, int k0, int n) const {
+    mb::PropBatch<S> pb;
     pb.st = d_st; pb.P = d_P; pb.ldp = ldp; pb.M = M; pb.k = n; pb.pad_ = 0;
     pb.prof = profile ? d_prof : nullptr;
     for (int i = 0; i < n; ++i)
       for (int j = 0; j < 7; ++j) pb.r[i][j] = r[7 * (size_t)(k0 + i) + j];
+    return pb;
   }
 
   int augment() override {
     if (!initialized) return fail(MSCKF_B200_ERR_STATE, "augment before initialize");
     if (busy) return fail(MSCKF_B200_ERR_STATE, "augment with an un-fetched update pending");
-    RC(ensure_clones(M + 1));
-    CK(cudaSetDevice(device));
-    mb::Members<mb::AugArgs<S>, 1> a;
-    a.m[0] = aug_args();
-    mb::k_augment<S, 1><<<1, 256, 0, stream>>>(a);
-    launches++;
-    CK(cudaGetLastError());
-    M += 1;
-    return 0;
+    return solo.enqueue_augment({0});
   }
   mb::AugArgs<S> aug_args() const { return {d_st, d_P, d_poses, ldp, M}; }
   // k_nees's arguments; truth / W / out are device addresses in the calling context's buffers
@@ -722,14 +758,7 @@ struct Engine : EngineBase {
   int prune(const int* keep, int n_keep) override {
     RC(prune_check(keep, n_keep));
     if (n_keep == M) return 0;
-    CK(cudaSetDevice(device));
-    mb::Members<mb::GatherArgs<S>, 1> g;
-    gather_args(g.m[0], keep, n_keep);
-    mb::k_gather<S, 1><<<gather_grid(n_keep), 256, 0, stream>>>(g);
-    launches++;
-    CK(cudaGetLastError());
-    prune_swap(n_keep);
-    return 0;
+    return solo.enqueue_prune({0}, &keep, &n_keep);
   }
   int prune_check(const int* keep, int n_keep) const {
     if (n_keep < 0 || n_keep > M) return fail(MSCKF_B200_ERR_ARG, "prune: bad keep count");
@@ -739,15 +768,13 @@ struct Engine : EngineBase {
       if (keep[i] < 0 || keep[i] >= M || (i && keep[i] <= keep[i - 1])) return fail(MSCKF_B200_ERR_ARG, "prune: keep[] must be ascending positions");
     return 0;
   }
-  int gather_grid(int n_keep) const {
-    const int n_new = 15 + 6 * n_keep;
-    return std::min(2 * num_sms(device), (n_new * n_new + 255) / 256);
-  }
-  void gather_args(mb::GatherArgs<S>& g, const int* keep, int n_keep) const {
+  mb::GatherArgs<S> gather_args(const int* keep, int n_keep) const {
+    mb::GatherArgs<S> g;
     g.Pold = d_P; g.Pnew = d_P2; g.poses_old = d_poses; g.poses_new = d_poses2;
     g.n_new = 15 + 6 * n_keep; g.ldp = ldp;
     g.kl.n = n_keep;
     for (int i = 0; i < n_keep; ++i) g.kl.idx[i] = keep[i];
+    return g;
   }
   void prune_swap(int n_keep) {
     std::swap(d_P, d_P2);      // (buffer addresses ride in UpdArgs, not in captured kernel arguments:
@@ -755,15 +782,7 @@ struct Engine : EngineBase {
     M = n_keep;
   }
 
-  int get_state(void* imu_, void* poses_) override {
-    CK(cudaSetDevice(device));
-    std::vector<S> tmp;
-    if (poses_ && M > 0) tmp.resize((size_t)mb::kPoseStride * M);
-    RC(state_copy(imu_ != nullptr, tmp.empty() ? nullptr : tmp.data()));
-    CK(cudaStreamSynchronize(stream));  // one synchronisation for both copies
-    state_unpack(imu_, poses_, tmp.data());
-    return 0;
-  }
+  int get_state(void* imu_, void* poses_) override { return solo.read_state(&imu_, &poses_); }
   // get_state in two halves: enqueue the copies (IMU state into h_st, kPoseStride * M clone-pose scalars into raw_poses),
   // and, once the stream has been synchronised, convert them into the C-ABI's layouts
   int state_copy(bool imu, S* raw_poses) {
@@ -1235,9 +1254,9 @@ int Ctx<S>::fetch(msckf_b200_report* reports) {
   return 0;
 }
 
-// ---- batched state calls.  Every member is validated before anything is launched, so a bad argument changes no member.
-// Members' arguments travel by value, mb::kBatchMembers per launch (one launch per chunk past that): no staging buffer, no
-// host synchronisation.  A member runs exactly the kernel body and arguments of its single-filter call.
+// ---- state calls.  A batch validates every member before anything is launched, so a bad argument changes no member; then it
+// and the single filter's calls launch through the same enqueue_* and per_member, so a member runs exactly the kernel body and
+// arguments of its single-filter call.  Arguments travel by value: no staging buffer, no host synchronisation.
 template <class S>
 int Ctx<S>::members_ready(const char* what) const {
   for (auto* e : eng) {
@@ -1251,30 +1270,25 @@ int Ctx<S>::members_ready(const char* what) const {
 template <class S>
 int Ctx<S>::propagate_n(const void* const* readings, const int* k) {
   RC(members_ready("batch_propagate_n"));
-  const int nf = (int)eng.size();
-  int kmax = 0;
-  for (int i = 0; i < nf; ++i) {
+  for (int i = 0; i < (int)eng.size(); ++i) {
     const int ki = k ? k[i] : 0;
     if (ki < 0 || (ki > 0 && (!readings || !readings[i]))) return fail(MSCKF_B200_ERR_ARG, "batch_propagate_n: bad arguments");
-    kmax = std::max(kmax, ki);
   }
+  return enqueue_propagate_n(readings, k);
+}
+template <class S>
+int Ctx<S>::enqueue_propagate_n(const void* const* readings, const int* k) {
+  const int nf = (int)eng.size();
+  int kmax = 0;
+  for (int i = 0; i < nf; ++i) kmax = std::max(kmax, k ? k[i] : 0);
   CK(cudaSetDevice(device));
   std::vector<int> idx;
-  // the same split into kPropMax readings per launch as propagate_n: step k0 runs every member with more than k0 readings
+  // kPropMax readings per launch: step k0 runs every member with more than k0 readings
   for (int k0 = 0; k0 < kmax; k0 += mb::kPropMax) {
     idx.clear();
     for (int i = 0; i < nf; ++i) if (k[i] > k0) idx.push_back(i);
-    for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
-      const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
-      mb::Members<mb::PropBatch<S>, mb::kBatchMembers> a;
-      for (int j = 0; j < nm; ++j) {
-        const int i = idx[c + j];
-        eng[i]->prop_args(a.m[j], (const S*)readings[i], k0, std::min(mb::kPropMax, k[i] - k0));
-        eng[i]->launches++;
-      }
-      mb::k_propagate<S, mb::kBatchMembers><<<nm, 256, 0, stream>>>(a);
-      launches++;
-    }
+    per_member(idx, true, [&](int i) { return eng[i]->prop_args((const S*)readings[i], k0, std::min(mb::kPropMax, k[i] - k0)); },
+               [&](const auto& a, int nm) { mb::k_propagate<<<nm, 256, 0, stream>>>(a); });
   }
   CK(cudaGetLastError());
   return 0;
@@ -1289,15 +1303,14 @@ int Ctx<S>::augment(const int* which) {
     if (eng[i]->M + 1 > kMaxClonesHard) return fail(MSCKF_B200_ERR_CAPACITY, "sliding window exceeds the engine's hard limit of " + std::to_string(kMaxClonesHard) + " clones");
     idx.push_back(i);
   }
+  return enqueue_augment(idx);
+}
+template <class S>
+int Ctx<S>::enqueue_augment(const std::vector<int>& idx) {
   for (int i : idx) RC(eng[i]->ensure_clones(eng[i]->M + 1));
   CK(cudaSetDevice(device));
-  for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
-    const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
-    mb::Members<mb::AugArgs<S>, mb::kBatchMembers> a;
-    for (int j = 0; j < nm; ++j) { a.m[j] = eng[idx[c + j]]->aug_args(); eng[idx[c + j]]->launches++; }
-    mb::k_augment<S, mb::kBatchMembers><<<nm, 256, 0, stream>>>(a);
-    launches++;
-  }
+  per_member(idx, true, [&](int i) { return eng[i]->aug_args(); },
+             [&](const auto& a, int nm) { mb::k_augment<<<nm, 256, 0, stream>>>(a); });
   CK(cudaGetLastError());
   for (int i : idx) eng[i]->M += 1;
   return 0;
@@ -1313,20 +1326,17 @@ int Ctx<S>::prune(const int* const* keep, const int* n_keep) {
     RC(eng[i]->prune_check(keep ? keep[i] : nullptr, n_keep[i]));
     idx.push_back(i);
   }
+  return enqueue_prune(idx, keep, n_keep);
+}
+template <class S>
+int Ctx<S>::enqueue_prune(const std::vector<int>& idx, const int* const* keep, const int* n_keep) {
   CK(cudaSetDevice(device));
-  for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
-    const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
-    mb::Members<mb::GatherArgs<S>, mb::kBatchMembers> g;
-    int gx = 1;  // the largest member's grid; smaller members' CTAs past their own grid-stride range exit at once
-    for (int j = 0; j < nm; ++j) {
-      const int i = idx[c + j];
-      eng[i]->gather_args(g.m[j], keep[i], n_keep[i]);
-      gx = std::max(gx, eng[i]->gather_grid(n_keep[i]));
-      eng[i]->launches++;
-    }
-    mb::k_gather<S, mb::kBatchMembers><<<dim3(gx, nm), 256, 0, stream>>>(g);
-    launches++;
-  }
+  per_member(idx, true, [&](int i) { return eng[i]->gather_args(keep ? keep[i] : nullptr, n_keep[i]); },
+             [&](const auto& a, int nm) {
+               int gx = 1;  // the largest member's grid; smaller members' CTAs past their own grid-stride range exit at once
+               for (int j = 0; j < nm; ++j) gx = std::max(gx, std::min(2 * num_sms(device), (a.m[j].n_new * a.m[j].n_new + 255) / 256));
+               mb::k_gather<<<dim3(gx, nm), 256, 0, stream>>>(a);
+             });
   CK(cudaGetLastError());
   for (int i : idx) eng[i]->prune_swap(n_keep[i]);
   return 0;
@@ -1335,21 +1345,27 @@ int Ctx<S>::prune(const int* const* keep, const int* n_keep) {
 template <class S>
 int Ctx<S>::get_state(void* const* imu, void* const* poses) {
   RC(members_ready("batch_get_state"));
+  return read_state(imu, poses);
+}
+// every member's copies into the pinned I/O block, one synchronisation, then the C-ABI's layouts
+template <class S>
+int Ctx<S>::read_state(void* const* imu, void* const* poses) {
   const int nf = (int)eng.size();
   std::vector<size_t> off(nf + 1, 0);
   for (int i = 0; i < nf; ++i) off[i + 1] = off[i] + (poses && poses[i] ? up16(sizeof(S) * mb::kPoseStride * eng[i]->M) : 0);
-  RC(poses_out.ensure(off[nf], stream));
   CK(cudaSetDevice(device));
+  RC(io.ensure(off[nf], stream));
   for (int i = 0; i < nf; ++i)
-    RC(eng[i]->state_copy(imu && imu[i], off[i + 1] > off[i] ? reinterpret_cast<S*>(poses_out.h + off[i]) : nullptr));
+    RC(eng[i]->state_copy(imu && imu[i], off[i + 1] > off[i] ? reinterpret_cast<S*>(io.h + off[i]) : nullptr));
   CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
   for (int i = 0; i < nf; ++i)
-    eng[i]->state_unpack(imu ? imu[i] : nullptr, off[i + 1] > off[i] ? poses[i] : nullptr, reinterpret_cast<S*>(poses_out.h + off[i]));
+    eng[i]->state_unpack(imu ? imu[i] : nullptr, off[i + 1] > off[i] ? poses[i] : nullptr, reinterpret_cast<S*>(io.h + off[i]));
   return 0;
 }
 
-// Truth travels in one pinned block ([19] IMU + [M][7] poses per member) with one host-to-device copy; the results come back
-// with one copy and one synchronisation.  Nothing of the filters is written (P, state, poses, graphs, launch counts).
+// Truth travels in the I/O block ([19] IMU + [M][7] poses per member) with one host-to-device copy; k_nees runs through
+// per_member (NM = 1 with one member in the context); the results come back with one copy and one synchronisation.  Nothing of
+// the filters is written (P, state, poses, graphs, launch counts).
 static_assert(sizeof(mb::NeesOut) == sizeof(msckf_b200_nees_result) && offsetof(msckf_b200_nees_result, first_bad_pivot) == 44,
               "mb::NeesOut must have the layout of msckf_b200_nees_result");
 template <class S>
@@ -1357,9 +1373,9 @@ int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_pose
   if (!truth_imu || !out) return fail(MSCKF_B200_ERR_ARG, "nees: null argument");
   RC(members_ready("nees"));
   const int nf = (int)eng.size();
-  auto finite = [](const double* v, int k) { for (int i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false; return true; };
   auto unit_ok = [](const double* q) { return q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0; };
   std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
+  std::vector<int> idx;
   for (int i = 0; i < nf; ++i) {
     const double* ti = truth_imu[i];
     const double* tp = truth_poses ? truth_poses[i] : nullptr;
@@ -1373,51 +1389,35 @@ int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_pose
     const int n = tp ? 15 + 6 * M : 15;
     off[i + 1] = off[i] + up16(sizeof(double) * (mb::kNeesTruthImu + (tp ? 7 * (size_t)M : 0)));
     woff[i + 1] = woff[i] + up256(sizeof(double) * (size_t)(n + 1) * n);
+    idx.push_back(i);
   }
   const size_t res_off = up256(off[nf]);
   CK(cudaSetDevice(device));
-  RC(nees_io.ensure(res_off + sizeof(mb::NeesOut) * nf, stream));
-  if (woff[nf] > nees_ws_cap) {
-    const size_t c = std::max(woff[nf], 2 * nees_ws_cap);
-    CK(cudaStreamSynchronize(stream));
-    if (nees_ws) cudaFree(nees_ws);
-    nees_ws = nullptr; nees_ws_cap = 0;
-    CK(cudaMalloc(&nees_ws, c));
-    nees_ws_cap = c;
-  }
+  RC(io.ensure(res_off + sizeof(mb::NeesOut) * nf, stream));
+  RC(ws.ensure(woff[nf], stream));
   for (int i = 0; i < nf; ++i) {
-    double* h = reinterpret_cast<double*>(nees_io.h + off[i]);
+    double* h = reinterpret_cast<double*>(io.h + off[i]);
     memcpy(h, truth_imu[i], sizeof(double) * mb::kNeesTruthImu);
     if (truth_poses && truth_poses[i] && eng[i]->M > 0) memcpy(h + mb::kNeesTruthImu, truth_poses[i], sizeof(double) * 7 * eng[i]->M);
   }
-  CK(cudaMemcpyAsync(nees_io.d, nees_io.h, off[nf], cudaMemcpyHostToDevice, stream));
-  auto args = [&](int i) {
-    return eng[i]->nees_args(reinterpret_cast<const double*>(nees_io.d + off[i]), truth_poses && truth_poses[i],
-                             reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(nees_ws) + woff[i]),
-                             reinterpret_cast<mb::NeesOut*>(nees_io.d + res_off) + i);
-  };
-  if (nf == 1) {
-    mb::Members<mb::NeesArgs<S>, 1> a;
-    a.m[0] = args(0);
-    mb::k_nees<S, 1><<<1, 256, 0, stream>>>(a);
-  } else {
-    for (int c = 0; c < nf; c += mb::kBatchMembers) {
-      const int nm = std::min(mb::kBatchMembers, nf - c);
-      mb::Members<mb::NeesArgs<S>, mb::kBatchMembers> a;
-      for (int j = 0; j < nm; ++j) a.m[j] = args(c + j);
-      mb::k_nees<S, mb::kBatchMembers><<<nm, 256, 0, stream>>>(a);
-    }
-  }
+  CK(cudaMemcpyAsync(io.d, io.h, off[nf], cudaMemcpyHostToDevice, stream));
+  per_member(idx, false,
+             [&](int i) {
+               return eng[i]->nees_args(reinterpret_cast<const double*>(io.d + off[i]), truth_poses && truth_poses[i],
+                                        reinterpret_cast<double*>(ws.d + woff[i]), reinterpret_cast<mb::NeesOut*>(io.d + res_off) + i);
+             },
+             [&](const auto& a, int nm) { mb::k_nees<<<nm, 256, 0, stream>>>(a); });
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(nees_io.h + res_off, nees_io.d + res_off, sizeof(mb::NeesOut) * nf, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(io.h + res_off, io.d + res_off, sizeof(mb::NeesOut) * nf, cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
-  memcpy(out, nees_io.h + res_off, sizeof(mb::NeesOut) * nf);
+  memcpy(out, io.h + res_off, sizeof(mb::NeesOut) * nf);
   return 0;
 }
 
-// Aided updates: every updated member's inputs travel in one pinned block ([32] z, R [m][m], H [m][n] for LINEAR), the results
-// come back with one copy and one synchronisation.  W^T and dx (n (m + 1) doubles) sit in dynamic shared memory up to
-// kAidSmemMax bytes, else in a global workspace.  Nothing is launched unless every member is valid.
+// Aided updates: every updated member's inputs travel in the I/O block ([32] z, R [m][m], H [m][n] for LINEAR), k_aid runs
+// through per_member (NM = 1 with one member in the context), the results come back with one copy and one synchronisation.
+// W^T and dx (n (m + 1) doubles) sit in dynamic shared memory up to kAidSmemMax bytes, else in the workspace.  Nothing is
+// launched unless every member is valid.
 static_assert(offsetof(mb::AidOut, status) == offsetof(msckf_b200_aid_result, status), "mb::AidOut must start like msckf_b200_aid_result");
 constexpr size_t kAidSmemMax = 32 * 1024;
 template <class S>
@@ -1425,7 +1425,6 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "aid_update: null argument");
   RC(members_ready("aid_update"));
   const int nf = (int)eng.size();
-  auto finite = [](const double* v, size_t k) { for (size_t i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false; return true; };
   std::vector<int> idx, rows(nf, 0);
   std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
   for (int i = 0; i < nf; ++i) {
@@ -1458,66 +1457,49 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
   if (idx.empty()) return 0;
   const size_t res_off = up256(off[nf]);
   CK(cudaSetDevice(device));
-  RC(aid_io.ensure(res_off + sizeof(mb::AidOut) * nf, stream));
-  if (woff[nf] > aid_ws_cap) {
-    const size_t c = std::max(woff[nf], 2 * aid_ws_cap);
-    CK(cudaStreamSynchronize(stream));
-    if (aid_ws) cudaFree(aid_ws);
-    aid_ws = nullptr; aid_ws_cap = 0;
-    CK(cudaMalloc(&aid_ws, c));
-    aid_ws_cap = c;
-  }
+  RC(io.ensure(res_off + sizeof(mb::AidOut) * nf, stream));
+  RC(ws.ensure(woff[nf], stream));
   for (int i : idx) {
     const msckf_b200_aid& q = in[i];
     const int m = rows[i], n = 15 + 6 * eng[i]->M;
-    double* h = reinterpret_cast<double*>(aid_io.h + off[i]);
+    double* h = reinterpret_cast<double*>(io.h + off[i]);
     memset(h, 0, sizeof(double) * mb::kAidZ);
     memcpy(h, q.z, sizeof(double) * (q.model == MSCKF_B200_AID_LINEAR ? m : q.model <= MSCKF_B200_AID_POSITION ? 3 : 7));
     memcpy(h + mb::kAidZ, q.R, sizeof(double) * m * m);
     if (q.model == MSCKF_B200_AID_LINEAR) memcpy(h + mb::kAidZ + m * m, q.H, sizeof(double) * m * n);
   }
-  CK(cudaMemcpyAsync(aid_io.d, aid_io.h, off[nf], cudaMemcpyHostToDevice, stream));
-  mb::AidOut* d_out = reinterpret_cast<mb::AidOut*>(aid_io.d + res_off);
-  // a member's arguments, and the dynamic shared memory it needs (0: its W^T and dx are in the global workspace)
-  auto args = [&](int i, size_t& smem) {
-    const int m = rows[i], n = 15 + 6 * eng[i]->M;
-    const bool global = woff[i + 1] > woff[i];
-    if (!global) smem = std::max(smem, mb::aid_ws_bytes(n, m));
-    return eng[i]->aid_args(in[i], m, reinterpret_cast<const double*>(aid_io.d + off[i]),
-                            global ? reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(aid_ws) + woff[i]) : nullptr, d_out + i);
-  };
-  if (nf == 1) {
-    mb::Members<mb::AidArgs<S>, 1> a;
-    size_t smem = 0;
-    a.m[0] = args(0, smem);
-    mb::k_aid<S, 1><<<1, mb::kAidThreads, smem, stream>>>(a);
-  } else {
-    for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
-      const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
-      mb::Members<mb::AidArgs<S>, mb::kBatchMembers> a;
-      size_t smem = 0;
-      for (int j = 0; j < nm; ++j) a.m[j] = args(idx[c + j], smem);
-      mb::k_aid<S, mb::kBatchMembers><<<nm, mb::kAidThreads, smem, stream>>>(a);
-    }
-  }
+  CK(cudaMemcpyAsync(io.d, io.h, off[nf], cudaMemcpyHostToDevice, stream));
+  mb::AidOut* d_out = reinterpret_cast<mb::AidOut*>(io.d + res_off);
+  per_member(idx, false,
+             [&](int i) {
+               const bool global = woff[i + 1] > woff[i];
+               return eng[i]->aid_args(in[i], rows[i], reinterpret_cast<const double*>(io.d + off[i]),
+                                       global ? reinterpret_cast<double*>(ws.d + woff[i]) : nullptr, d_out + i);
+             },
+             [&](const auto& a, int nm) {
+               size_t smem = 0;  // the largest need of the members whose W^T and dx are in shared memory
+               for (int j = 0; j < nm; ++j)
+                 if (!a.m[j].ws) smem = std::max(smem, mb::aid_ws_bytes(15 + 6 * a.m[j].M, a.m[j].m));
+               mb::k_aid<<<nm, mb::kAidThreads, smem, stream>>>(a);
+             });
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(aid_io.h + res_off, aid_io.d + res_off, sizeof(mb::AidOut) * nf, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(io.h + res_off, io.d + res_off, sizeof(mb::AidOut) * nf, cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
-  const mb::AidOut* h_out = reinterpret_cast<const mb::AidOut*>(aid_io.h + res_off);
+  const mb::AidOut* h_out = reinterpret_cast<const mb::AidOut*>(io.h + res_off);
   int numeric = -1;
   for (int i : idx) {
     const mb::AidOut& o = h_out[i];
     out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].applied = o.applied; out[i].status = o.status;
     if (o.numeric && numeric < 0) numeric = i;
   }
-  if (numeric >= 0) return fail(MSCKF_B200_ERR_NUMERIC, "aid_update: non-finite delta-x or covariance entry (member " + std::to_string(numeric) + "); the update was applied");
-  return 0;
+  return numeric_error("aid_update", numeric);
 }
 
 // Mapped-landmark updates: every member with observations sends its observations (grouped by clone in window order, input
-// order kept inside a clone) and its clone table in one pinned block with one host-to-device copy; results, gamma and flags come
-// back with one copy and one synchronisation.  Three launches per chunk of 32 such members (k_lmk_clone, k_lmk_gain,
-// k_lmk_downdate), whatever the observations turn out to be.  Nothing is launched unless every member is valid.
+// order kept inside a clone) and its clone table in the I/O block with one host-to-device copy; results, gamma and flags come
+// back with one copy and one synchronisation.  Three launches per per_member chunk of such members (k_lmk_clone, k_lmk_gain,
+// k_lmk_downdate; NM = 1 with one member in the context), whatever the observations turn out to be.  Nothing is launched
+// unless every member is valid.
 static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_result, status),
               "mb::LmkOut must start like msckf_b200_landmark_result");
 template <class S>
@@ -1525,7 +1507,6 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "landmark_update: null argument");
   RC(members_ready("landmark_update"));
   const int nf = (int)eng.size();
-  auto finite = [](const double* v, size_t k) { for (size_t i = 0; i < k; ++i) if (!std::isfinite(v[i])) return false; return true; };
   struct LmkPlan { std::vector<int> perm, grp; int G = 0, ld = 0; size_t in_off = 0, res_off = 0, ws_off = 0; };
   std::vector<LmkPlan> pl(nf);
   std::vector<int> idx;
@@ -1566,72 +1547,55 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
   if (idx.empty()) return 0;
   const size_t res_base = up256(in_bytes);
   CK(cudaSetDevice(device));
-  RC(lmk_io.ensure(res_base + res_bytes, stream));
-  if (ws_bytes > lmk_ws_cap) {
-    const size_t c = std::max(ws_bytes, 2 * lmk_ws_cap);
-    CK(cudaStreamSynchronize(stream));
-    if (lmk_ws) cudaFree(lmk_ws);
-    lmk_ws = nullptr; lmk_ws_cap = 0;
-    CK(cudaMalloc(&lmk_ws, c));
-    lmk_ws_cap = c;
-  }
+  RC(io.ensure(res_base + res_bytes, stream));
+  RC(ws.ensure(ws_bytes, stream));
   std::vector<mb::LmkArgs<S>> args(nf);
   for (int i : idx) {
     const msckf_b200_landmarks& q = in[i];
     const LmkPlan& p = pl[i];
     const int no = q.n_obs, n = 15 + 6 * eng[i]->M;
-    double* ho = reinterpret_cast<double*>(lmk_io.h + p.in_off);
+    double* ho = reinterpret_cast<double*>(io.h + p.in_off);
     for (int j = 0; j < no; ++j) {
       const int s = p.perm[j];
       ho[5 * j] = q.z[2 * s]; ho[5 * j + 1] = q.z[2 * s + 1];
       ho[5 * j + 2] = q.p_L_G[3 * s]; ho[5 * j + 3] = q.p_L_G[3 * s + 1]; ho[5 * j + 4] = q.p_L_G[3 * s + 2];
     }
     const size_t goff = p.in_off + up16(sizeof(double) * 5 * (size_t)no);
-    memcpy(lmk_io.h + goff, p.grp.data(), sizeof(int) * p.grp.size());
+    memcpy(io.h + goff, p.grp.data(), sizeof(int) * p.grp.size());
     mb::LmkArgs<S> a = eng[i]->lmk_args(q, p.G, p.ld);
-    a.obs = reinterpret_cast<const double*>(lmk_io.d + p.in_off);
-    a.grp = reinterpret_cast<const int*>(lmk_io.d + goff);
-    unsigned char* r = lmk_io.d + res_base + p.res_off;
+    a.obs = reinterpret_cast<const double*>(io.d + p.in_off);
+    a.grp = reinterpret_cast<const int*>(io.d + goff);
+    unsigned char* r = io.d + res_base + p.res_off;
     a.out = reinterpret_cast<mb::LmkOut*>(r);
     a.gamma = reinterpret_cast<double*>(r + up16(sizeof(mb::LmkOut)));
     a.flag = reinterpret_cast<int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no));
-    double* w = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(lmk_ws) + p.ws_off);
+    double* w = reinterpret_cast<double*>(ws.d + p.ws_off);
     a.slot = w;
     a.A = w + (size_t)mb::kLmkSlot * p.G;
     a.dx = a.A + (size_t)(p.ld + n + 1) * p.ld;
     a.ctl = reinterpret_cast<mb::LmkCtl*>(a.dx + n);
     args[i] = a;
   }
-  CK(cudaMemcpyAsync(lmk_io.d, lmk_io.h, in_bytes, cudaMemcpyHostToDevice, stream));
-  if (nf == 1) {
-    mb::Members<mb::LmkArgs<S>, 1> a;
-    a.m[0] = args[0];
-    mb::k_lmk_clone<S, 1><<<dim3(a.m[0].G, 1), mb::kLmkThreads, 0, stream>>>(a);
-    mb::k_lmk_gain<S, 1><<<1, mb::kLmkThreads, 0, stream>>>(a);
-    mb::k_lmk_downdate<S, 1><<<dim3(a.m[0].ntiles, 1), mb::kLmkThreads, 0, stream>>>(a);
-  } else {
-    for (size_t c = 0; c < idx.size(); c += mb::kBatchMembers) {
-      const int nm = (int)std::min<size_t>(mb::kBatchMembers, idx.size() - c);
-      mb::Members<mb::LmkArgs<S>, mb::kBatchMembers> a;
-      int gx = 1, tx = 1;  // the largest member's grid; other members' CTAs past their own range exit at once
-      for (int j = 0; j < nm; ++j) {
-        a.m[j] = args[idx[c + j]];
-        gx = std::max(gx, a.m[j].G);
-        tx = std::max(tx, a.m[j].ntiles);
-      }
-      mb::k_lmk_clone<S, mb::kBatchMembers><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
-      mb::k_lmk_gain<S, mb::kBatchMembers><<<nm, mb::kLmkThreads, 0, stream>>>(a);
-      mb::k_lmk_downdate<S, mb::kBatchMembers><<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(a);
-    }
-  }
+  CK(cudaMemcpyAsync(io.d, io.h, in_bytes, cudaMemcpyHostToDevice, stream));
+  per_member(idx, false, [&](int i) { return args[i]; },
+             [&](const auto& a, int nm) {
+               int gx = 1, tx = 1;  // the largest member's grid; other members' CTAs past their own range exit at once
+               for (int j = 0; j < nm; ++j) {
+                 gx = std::max(gx, a.m[j].G);
+                 tx = std::max(tx, a.m[j].ntiles);
+               }
+               mb::k_lmk_clone<<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
+               mb::k_lmk_gain<<<nm, mb::kLmkThreads, 0, stream>>>(a);
+               mb::k_lmk_downdate<<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(a);
+             });
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(lmk_io.h + res_base, lmk_io.d + res_base, res_bytes, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(io.h + res_base, io.d + res_base, res_bytes, cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
   int numeric = -1;
   for (int i : idx) {
     const msckf_b200_landmarks& q = in[i];
     const LmkPlan& p = pl[i];
-    const unsigned char* r = lmk_io.h + res_base + p.res_off;
+    const unsigned char* r = io.h + res_base + p.res_off;
     const mb::LmkOut& o = *reinterpret_cast<const mb::LmkOut*>(r);
     const double* g = reinterpret_cast<const double*>(r + up16(sizeof(mb::LmkOut)));
     const int* fl = reinterpret_cast<const int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)q.n_obs));
@@ -1643,8 +1607,7 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
     }
     if (o.numeric && numeric < 0) numeric = i;
   }
-  if (numeric >= 0) return fail(MSCKF_B200_ERR_NUMERIC, "landmark_update: non-finite delta-x or covariance entry (member " + std::to_string(numeric) + "); the update was applied");
-  return 0;
+  return numeric_error("landmark_update", numeric);
 }
 }  // namespace
 
@@ -1670,6 +1633,20 @@ int make_batch(msckf_b200_engine** engines, int n, msckf_b200_batch** out) {
   c->plan.resize(n);
   *out = new msckf_b200_batch{c, first->dtype};
   return 0;
+}
+
+// stage and launch an update of a filter's or a batch's context; update() also fetches
+int update_async(CtxBase* c, int mode, const msckf_b200_tracks* tracks, int threads) {
+  if (!tracks) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  RC(c->stage(mode, tracks, threads));
+  return c->launch();
+}
+int update(CtxBase* c, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports, int threads) {
+  const int rc = update_async(c, mode, tracks, threads);
+  if (rc == 0) return c->fetch(reports);
+  // keep the real cause: clean up a half-started update without touching the error message
+  if (c->pending) { const std::string keep = g_err; c->fetch(nullptr); g_err = keep; }
+  return rc;
 }
 }  // namespace
 
@@ -1720,19 +1697,11 @@ int msckf_b200_stage(msckf_b200_engine* e, int mode, const msckf_b200_tracks* tr
 int msckf_b200_launch(msckf_b200_engine* e) { return e->impl->solo_ctx()->launch(); }
 int msckf_b200_launch_timed(msckf_b200_engine* e, float* ms) { return e->impl->solo_ctx()->launch_timed(ms); }
 int msckf_b200_update_async(msckf_b200_engine* e, int mode, const msckf_b200_tracks* tracks) {
-  int rc = msckf_b200_stage(e, mode, tracks);
-  if (rc != 0) return rc;
-  return e->impl->solo_ctx()->launch();
+  return update_async(e->impl->solo_ctx(), mode, tracks, 1);
 }
 int msckf_b200_fetch(msckf_b200_engine* e, msckf_b200_report* report) { return e->impl->solo_ctx()->fetch(report); }
 int msckf_b200_update(msckf_b200_engine* e, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* report) {
-  int rc = msckf_b200_update_async(e, mode, tracks);
-  if (rc != 0) {  // keep the real cause: clean up a half-started update without touching the error message
-    CtxBase* c = e->impl->solo_ctx();
-    if (c->pending) { const std::string keep = g_err; c->fetch(nullptr); g_err = keep; }
-    return rc;
-  }
-  return e->impl->solo_ctx()->fetch(report);
+  return update(e->impl->solo_ctx(), mode, tracks, report, 1);
 }
 
 int msckf_b200_batch_create(msckf_b200_engine** engines, int n, msckf_b200_batch** out) {
@@ -1765,18 +1734,11 @@ int msckf_b200_batch_stage(msckf_b200_batch* b, int mode, const msckf_b200_track
 int msckf_b200_batch_launch(msckf_b200_batch* b) { return b->ctx->launch(); }
 int msckf_b200_batch_launch_timed(msckf_b200_batch* b, float* ms) { return b->ctx->launch_timed(ms); }
 int msckf_b200_batch_update_async(msckf_b200_batch* b, int mode, const msckf_b200_tracks* tracks, int threads) {
-  int rc = msckf_b200_batch_stage(b, mode, tracks, threads);
-  if (rc != 0) return rc;
-  return b->ctx->launch();
+  return b ? update_async(b->ctx, mode, tracks, threads) : fail(MSCKF_B200_ERR_ARG, "null argument");
 }
 int msckf_b200_batch_fetch(msckf_b200_batch* b, msckf_b200_report* reports) { return b->ctx->fetch(reports); }
 int msckf_b200_batch_update(msckf_b200_batch* b, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports, int threads) {
-  int rc = msckf_b200_batch_update_async(b, mode, tracks, threads);
-  if (rc != 0) {
-    if (b->ctx->pending) { const std::string keep = g_err; b->ctx->fetch(nullptr); g_err = keep; }
-    return rc;
-  }
-  return b->ctx->fetch(reports);
+  return b ? update(b->ctx, mode, tracks, reports, threads) : fail(MSCKF_B200_ERR_ARG, "null argument");
 }
 int msckf_b200_batch_kernel_times(msckf_b200_batch* b, float* ms, const char** names, int cap) { return b->ctx->kernel_times(ms, names, cap); }
 long long msckf_b200_batch_launch_count(const msckf_b200_batch* b) { return b->ctx->launches; }

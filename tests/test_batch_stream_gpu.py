@@ -55,27 +55,28 @@ def assert_same(a, b):
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_batched_propagate_is_bit_identical(dtype):
     """windows 0, 5, 30 and 90 clones (90: past the 85 clones whose P_IC columns k_propagate keeps in registers), per-member
-    reading counts 0, 1, 16, 17 and 40 (one, two and three steps of 16 readings)"""
-    Ms = [0, 5, 30, 90]
-    mem = [Member(dtype, M, seed=i) for i, M in enumerate(Ms)]
-    twins = [m.twin(dtype) for m in mem]
-    for a, b in zip(mem, twins):
-        assert_same(a, b)
-    batch = capi.Batch([m.e for m in mem])
-    rng = np.random.default_rng(7)
-    for ks in ([1, 16, 17, 40], [40, 0, 1, 16], [17, 40, 0, 1], [0, 0, 0, 0]):
-        rs = [readings(rng, k) for k in ks]
-        batch.propagate_n(rs)
-        for t, r in zip(twins, rs):
-            if len(r):
-                t.e.propagate_n(r)
+    reading counts 0, 1, 16, 17 and 40 (one, two and three steps of 16 readings); then a batch of one member, which takes the
+    NM = 1 form of the kernels"""
+    for Ms in ([0, 5, 30, 90], [30]):
+        mem = [Member(dtype, M, seed=i) for i, M in enumerate(Ms)]
+        twins = [m.twin(dtype) for m in mem]
         for a, b in zip(mem, twins):
             assert_same(a, b)
-    # the batched getter returns what the single-engine getter returns
-    for (imu, poses), m in zip(batch.state(), mem):
-        imu1, poses1 = m.e.state()
-        assert np.array_equal(imu, imu1) and np.array_equal(poses, poses1)
-    batch.close()
+        batch = capi.Batch([m.e for m in mem])
+        rng = np.random.default_rng(7)
+        for ks in ([1, 16, 17, 40], [40, 0, 1, 16], [17, 40, 0, 1], [0, 0, 0, 0]):
+            rs = [readings(rng, k) for k in ks[:len(Ms)]]
+            batch.propagate_n(rs)
+            for t, r in zip(twins, rs):
+                if len(r):
+                    t.e.propagate_n(r)
+            for a, b in zip(mem, twins):
+                assert_same(a, b)
+        # the batched getter returns what the single-engine getter returns
+        for (imu, poses), m in zip(batch.state(), mem):
+            imu1, poses1 = m.e.state()
+            assert np.array_equal(imu, imu1) and np.array_equal(poses, poses1)
+        batch.close()
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
