@@ -212,7 +212,9 @@ enum msckf_b200_aid_model {
   MSCKF_B200_AID_POSITION = 1,
   MSCKF_B200_AID_POSE = 2,
   MSCKF_B200_AID_CLONE_POSE = 3,
-  MSCKF_B200_AID_LINEAR = 4
+  MSCKF_B200_AID_LINEAR = 4,
+  MSCKF_B200_AID_BODY_VELOCITY = 5, /* stacks only (msckf_b200_aid_stack_update) */
+  MSCKF_B200_AID_RELATIVE_POSE = 6  /* stacks only */
 };
 typedef struct {
   int model;          /* msckf_b200_aid_model; in a batch, < 0 leaves that member untouched */
@@ -237,6 +239,36 @@ int msckf_b200_aid_update(msckf_b200_engine* e, const msckf_b200_aid* aid, msckf
 /* the same for every member of a batch (aid[i], out[i]; out[i] is not written for a member with aid[i].model < 0); every
  * member is validated before anything is launched.  One launch per 32 updated members. */
 int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
+/* ---- stacked aided updates: odometry (wheel speed, non-holonomic constraints, relative motion) with other aids --------------
+ * One EKF update of up to 8 items whose rows are stacked (sum of rows m <= 32) with R block-diagonal across items: the update,
+ * outcomes and costs of msckf_b200_aid_update, with one NIS and one dof = m for the whole stack and one chi2_max gate.  Every
+ * item forms its residual and its Jacobian on the device from the resident state, in fp64 for both dtypes; each row of H has at
+ * most 12 non-zeros.  Allowed models: VELOCITY, POSITION, POSE, CLONE_POSE (a = the clone) as in msckf_b200_aid, and
+ *   BODY_VELOCITY  z = v_I (3), the IMU velocity in the IMU frame; v^ = C(q_IG) v_I_G, r = z - v^ over the rows selected by the
+ *                  mask a (bits 0..2; 0b110 with z = 0: the non-holonomic constraint v_y = v_z = 0; 0b111: full wheel velocity).
+ *                  H is non-zero over dtheta (0..2) and dv (6..8) only.
+ *   RELATIVE_POSE  clones a != b (window positions): z = p (3), q xyzw (4) of b relative to a in camera frames; predicted
+ *                  C^ = C_b C_a^T (q^ = q_b * q_a^-1) and p^ = C_a (p_C_G,b - p_C_G,a); r = [dtheta(q_z, q^); z_p - p^] with the
+ *                  dtheta of POSE.  H is non-zero over the two clones' [dtheta, dp].  (Odometry between the IMU state and a
+ *                  clone is not a model: convert it to camera frames with q_CI and p_C_I.)
+ * C(q) is Eigen's toRotationMatrix (C(q_CG) maps G to the camera frame).  LINEAR is not allowed in a stack.  R of an item is its
+ * own rows x rows block (3, 3, 6, 6, popcount(mask), 6 rows), row-major, lower triangle read. */
+typedef struct {
+  int model;          /* msckf_b200_aid_model except LINEAR */
+  int a;              /* CLONE_POSE, RELATIVE_POSE: clone position; BODY_VELOCITY: row mask (1..7); else ignored */
+  int b;              /* RELATIVE_POSE: the second clone; else ignored */
+  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components) or 7 doubles */
+  const double* R;    /* [rows][rows] */
+} msckf_b200_aid_item;
+/* A bad model, a clone outside the window, a == b, an empty mask, more than 8 items or 32 rows, a NULL or non-finite z / R, a zero
+ * quaternion or a NaN chi2_max returns MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
+ * A non-finite dx or P entry returns MSCKF_B200_ERR_NUMERIC with the result filled and the update applied.  n_items >= 1. */
+int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,
+                                msckf_b200_aid_result* out);
+/* the same for every member of a batch (items[i] [n_items[i]], out[i]; n_items[i] = 0 leaves member i untouched and out[i] not
+ * written); every member is validated before anything is launched.  One launch per 32 updated members. */
+int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                      double chi2_max, msckf_b200_aid_result* out);
 /* ---- mapped landmarks: image observations of landmarks whose position is known (prior map, surveyed marker, relocalisation) --
  * Observation i is (clone[i], z[i] normalised image coordinates, p_L_G[i] landmark position in G).  With C = C(q_CG) and p_C_G of
  * that clone: p_C = C (p_L - p_C_G), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), Jacobian the 2 x 6

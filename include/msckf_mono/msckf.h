@@ -370,6 +370,37 @@ class MSCKF {
     a.H = h.data();
     return aidedUpdate(a);
   }
+  // stacked aided updates (not in the reference; msckf_b200_aid_stack_update): up to 8 items -- odometry (BODY_VELOCITY,
+  // RELATIVE_POSE) and the fixes above -- fused as ONE update with R block-diagonal across items, one NIS over all rows and one
+  // chi2_max gate.  Items name clones by window position.  Bookkeeping as aidedUpdate(const msckf_b200_aid&).
+  msckf_b200_aid_result aidedUpdate(const std::vector<msckf_b200_aid_item>& items, double chi2_max = 0) {
+    msckf_b200_aid_result r = {};
+    checkNumeric(msckf_b200_aid_stack_update(eng(), items.data(), (int)items.size(), chi2_max, &r), "msckf_b200_aid_stack_update");
+    aidAbsorb(r);
+    return r;
+  }
+  // v_I: the IMU's velocity in its own frame (wheel or leg odometry); mask bits 0..2 select the rows used, R is popcount(mask)
+  // square over them.  mask 0b110 with v_I = 0 is the non-holonomic constraint v_y = v_z = 0.
+  msckf_b200_aid_result bodyVelocityUpdate(const Vector3<double>& v_I, const MatrixX<double>& R, int mask = 7, double chi2_max = 0) {
+    if (mask < 1 || mask > 7) throw std::invalid_argument("MSCKF::bodyVelocityUpdate: the mask must select rows 0..2");
+    const double z[3] = {v_I(0), v_I(1), v_I(2)};
+    const int m = (mask & 1) + ((mask >> 1) & 1) + ((mask >> 2) & 1);
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_BODY_VELOCITY, mask, 0, m, z, R)}, chi2_max);
+  }
+  // the pose of image state_id_b relative to image state_id_a in camera frames: p = C_a (p_C_G,b - p_C_G,a), q of C_b C_a^T;
+  // R 6 x 6 over [dtheta, dp].  An id that is not in the window throws std::invalid_argument before any device call.
+  msckf_b200_aid_result relativePoseUpdate(int state_id_a, int state_id_b, const Vector3<double>& p, const Quaternion<double>& q,
+                                           const FixedMatrix<double, 6, 6>& R, double chi2_max = 0) {
+    const int a = windowPosition(state_id_a, "MSCKF::relativePoseUpdate"), b = windowPosition(state_id_b, "MSCKF::relativePoseUpdate");
+    const double z[7] = {p(0), p(1), p(2), q.x(), q.y(), q.z(), q.w()};
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_RELATIVE_POSE, a, b, 6, z, R)}, chi2_max);
+  }
+  // the window position of the clone of image state_id (std::invalid_argument when it is not in the window)
+  int windowPosition(int state_id, const char* what) const {
+    for (size_t pos = 0; pos < cam_states_.size(); ++pos)
+      if (cam_states_[pos].state_id == state_id) return (int)pos;
+    throw std::invalid_argument(std::string(what) + ": state_id " + std::to_string(state_id) + " is not in the window");
+  }
   // host bookkeeping after an aided update: the mirror is stale, and an applied update moves the state the queued tracks saw
   void aidAbsorb(const msckf_b200_aid_result& r) {
     state_dirty_ = true;
@@ -651,6 +682,14 @@ class MSCKF {
     a.z = z; a.H = nullptr; a.R = aid_R_.data(); a.chi2_max = chi2_max;
     return a;
   }
+  // a msckf_b200_aid_item of one of the single-item forms (z must outlive the call; R is copied into aid_R_ as by aidModel)
+  template <class Mat>
+  msckf_b200_aid_item aidItem(int model, int a, int b, int m, const double* z, const Mat& R) {
+    const msckf_b200_aid q = aidModel(model, 0, m, z, R, 0.0);
+    msckf_b200_aid_item it = {};
+    it.model = model; it.a = a; it.b = b; it.z = z; it.R = q.R;
+    return it;
+  }
 
   static void check(int rc, const char* what) {
     if (rc != 0) throw std::runtime_error(std::string(what) + " failed (" + std::to_string(rc) + "): " + msckf_b200_last_error());
@@ -927,6 +966,26 @@ class MSCKFBatch {
     else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_update");
     for (size_t i = 0; i < size(); ++i)
       if (aid[i].model >= 0) filters_[i]->aidAbsorb(r[i]);
+    return r;
+  }
+  // MSCKF::aidedUpdate(items) of every filter (items[i] empty: filter i is left alone) as one msckf_b200_batch_aid_stack_update:
+  // one launch per 32 updated filters and one synchronisation.  result[i] of a filter left alone is value-initialised.
+  std::vector<msckf_b200_aid_result> aidedUpdate(const std::vector<std::vector<msckf_b200_aid_item>>& items, double chi2_max = 0) {
+    const size_t n = size();
+    if (items.size() != n) throw std::invalid_argument("MSCKFBatch::aidedUpdate: one item list per filter");
+    std::vector<const msckf_b200_aid_item*> p(n, nullptr);
+    std::vector<int> k(n, 0);
+    for (size_t i = 0; i < n; ++i) {
+      p[i] = items[i].empty() ? nullptr : items[i].data();
+      k[i] = (int)items[i].size();
+    }
+    flushImu();
+    std::vector<msckf_b200_aid_result> r(n, msckf_b200_aid_result());
+    const int rc = msckf_b200_batch_aid_stack_update(batch_, p.data(), k.data(), chi2_max, r.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch stacked aided update: " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_stack_update");
+    for (size_t i = 0; i < n; ++i)
+      if (!items[i].empty()) filters_[i]->aidAbsorb(r[i]);
     return r;
   }
   // MSCKF::landmarkUpdate of every filter (obs[i] empty: filter i is left alone) as one msckf_b200_batch_landmark_update: three

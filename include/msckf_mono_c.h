@@ -77,6 +77,17 @@ int msckf_mono_batch_nees(void* batch, const double* const* truth_imu, const dou
  * alone), one device call for the batch. */
 int msckf_mono_aid_update(void* h, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
 int msckf_mono_batch_aid_update(void* batch, const msckf_b200_aid* aid, msckf_b200_aid_result* out);
+/* stacked aided update (MSCKF::aidedUpdate(items), msckf_b200_aid_stack_update: models, layouts and errors there): n_items
+ * items with clones by window position, one chi2_max.  _batch_aid_stack_update: n_items[i] per filter (0: filter i is left alone
+ * and out[i] is not written), the items concatenated in filter order, one device call.  _body_velocity_update: v3 in the IMU
+ * frame, mask bits 0..2, R [m][m] over the selected rows.  _relative_pose_update: the pose of image state_id_b relative to
+ * image state_id_a (p3, q4 xyzw, R36 [6][6]); an id not in the window fails before any device call. */
+int msckf_mono_aid_stack_update(void* h, const msckf_b200_aid_item* items, int n_items, double chi2_max, msckf_b200_aid_result* out);
+int msckf_mono_batch_aid_stack_update(void* batch, const int* n_items, const msckf_b200_aid_item* items, double chi2_max,
+                                      msckf_b200_aid_result* out);
+int msckf_mono_body_velocity_update(void* h, const double* v3, int mask, const double* R, double chi2_max, msckf_b200_aid_result* out);
+int msckf_mono_relative_pose_update(void* h, int state_id_a, int state_id_b, const double* p3, const double* q4, const double* R36,
+                                    double chi2_max, msckf_b200_aid_result* out);
 /* mapped-landmark update (MSCKF::landmarkUpdate, msckf_b200_landmark_update: model, gate and errors there): n_obs observations,
  * state_ids [n] (the image's state id; an id not in the window fails before any device call), z [n][2], p_L_G [n][3];
  * R3 = uu, uv, vv or NULL (the filter's pixel noise); gamma [n] / flag [n] out, or NULL.  _batch_landmark_update: n_obs[i] per

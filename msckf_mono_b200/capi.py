@@ -41,7 +41,7 @@ def _truth(truth_imu, truth_poses):
     return imu, poses
 
 
-AID_VELOCITY, AID_POSITION, AID_POSE, AID_CLONE_POSE, AID_LINEAR = range(5)
+AID_VELOCITY, AID_POSITION, AID_POSE, AID_CLONE_POSE, AID_LINEAR, AID_BODY_VELOCITY, AID_RELATIVE_POSE = range(7)
 
 
 class Aid(C.Structure):
@@ -68,6 +68,24 @@ def aid_struct(spec):
     a = Aid(int(spec["model"]), int(spec.get("clone", 0)), m, n, z.ctypes.data, None if H is None else H.ctypes.data,
             R.ctypes.data, float(spec.get("chi2_max", 0.0)))
     return a, (z, R, H)
+
+
+class AidItem(C.Structure):
+    _fields_ = [("model", C.c_int), ("a", C.c_int), ("b", C.c_int), ("z", C.c_void_p), ("R", C.c_void_p)]
+
+
+def aid_items(items):
+    """(AidItem array, the float64 arrays it points into) of one stack: items = list of dicts model, z, R [rows, rows],
+    a (CLONE_POSE and RELATIVE_POSE: a clone's window position, BODY_VELOCITY: the row mask; "clone" is read when "a" is
+    missing), b (RELATIVE_POSE: the second clone)"""
+    arr = (AidItem * max(len(items), 1))()
+    keep = []
+    for k, it in enumerate(items):
+        z = np.ascontiguousarray(it["z"], dtype=np.float64).ravel()
+        R = np.ascontiguousarray(it["R"], dtype=np.float64)
+        keep += [z, R]
+        arr[k] = AidItem(int(it["model"]), int(it.get("a", it.get("clone", 0))), int(it.get("b", 0)), z.ctypes.data, R.ctypes.data)
+    return arr, keep
 
 
 class Landmarks(C.Structure):
@@ -283,6 +301,18 @@ class Batch:
         check(lib().msckf_b200_batch_aid_update(self.h, (Aid * n)(*[a for a, _ in st]), out), "msckf_b200_batch_aid_update")
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
+    def aid_stack_update(self, stacks, chi2_max=0.0):
+        """msckf_b200_batch_aid_stack_update: stacks[i] = list of item dicts for engine i (see aid_items; None or [] leaves
+        engine i alone); a list of result dicts (None for an engine left alone)"""
+        n = len(self.engines)
+        assert len(stacks) == n
+        st = [aid_items(s or []) for s in stacks]
+        ptrs = (C.POINTER(AidItem) * n)(*[C.cast(a, C.POINTER(AidItem)) for a, _ in st])
+        cnt = (C.c_int * n)(*[len(s or []) for s in stacks])
+        out = (AidResult * n)()
+        check(lib().msckf_b200_batch_aid_stack_update(self.h, ptrs, cnt, C.c_double(chi2_max), out), "msckf_b200_batch_aid_stack_update")
+        return [o.as_dict() if s else None for s, o in zip(stacks, out)]
+
     def landmark_update(self, specs):
         """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
         i alone); a list of result dicts with "gamma" and "flag" arrays (None for an engine left alone)"""
@@ -427,6 +457,14 @@ class Engine:
         a, keep = aid_struct({"model": model, "z": z, "R": R, "H": H, "clone": clone, "chi2_max": chi2_max})
         out = AidResult()
         check(lib().msckf_b200_aid_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_aid_update")
+        return out.as_dict()
+
+    def aid_stack_update(self, items, chi2_max=0.0):
+        """msckf_b200_aid_stack_update: one stacked update of items (see aid_items); the result as a dict"""
+        arr, keep = aid_items(items)
+        out = AidResult()
+        check(lib().msckf_b200_aid_stack_update(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)),
+              "msckf_b200_aid_stack_update")
         return out.as_dict()
 
     def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0):

@@ -1,9 +1,11 @@
 // msckf_mono_b200/csrc/aid_kernels.cuh
-// Aided measurements fused into the device-resident filter (msckf_b200_aid_update / _batch_aid_update):
-//   k_aid : residual r (from the resident state, or the caller's), H P (rows of P for the selection models, a product for a
-//           caller-linearised H), S = H P H^T + R = L L^T with r as an extra row (y = L^-1 r), W = L^-1 H P, NIS = y^T y,
-//           the optional chi-square gate, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to
-//           the filter precision once) and the state injection of k_syrk (inject_state).  All arithmetic in fp64.
+// Aided measurements fused into the device-resident filter (msckf_b200_aid_update / _batch_aid_update and the stacked
+// msckf_b200_aid_stack_update / _batch_aid_stack_update):
+//   k_aid : residual r and H (a stack of up to 8 model items, each row at most 12 (state index, coefficient) pairs formed from
+//           the resident state; or the caller's r and dense H), H P (sparse gathers over rows of P, or a product for a dense H),
+//           S = H P H^T + R = L L^T with r as an extra row (y = L^-1 r), W = L^-1 H P, NIS = y^T y, the optional chi-square
+//           gate, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to the filter precision
+//           once) and the state injection of k_syrk (inject_state).  All arithmetic in fp64.
 // One CTA per member, one launch for everything; one body for a single filter (NM = 1) and a device batch (NM =
 // kBatchMembers), like k_nees.  W^T and dx live in dynamic shared memory where they fit, else in a per-member global workspace.
 #pragma once
@@ -14,9 +16,14 @@
 namespace mb {
 
 // the models of msckf_b200_aid_model (include/msckf_b200.h)
-enum AidModel { kAidVelocity = 0, kAidPosition = 1, kAidPose = 2, kAidClonePose = 3, kAidLinear = 4 };
+enum AidModel {
+  kAidVelocity = 0, kAidPosition = 1, kAidPose = 2, kAidClonePose = 3, kAidLinear = 4, kAidBodyVelocity = 5, kAidRelativePose = 6
+};
 constexpr int kAidMaxRows = 32;      // m <= 32: S is factored by one warp
-constexpr int kAidZ = kAidMaxRows;   // input block: [32] z (or r of LINEAR), then R [m][m], then H [m][n] (LINEAR)
+constexpr int kAidMaxItems = 8;      // model items of one stack
+constexpr int kAidItemZ = 8;         // doubles reserved for one item's z
+constexpr int kAidNnz = 12;          // (state index, coefficient) pairs of one row of a model's H
+constexpr int kAidZ = kAidMaxItems * kAidItemZ;  // input block: [8][8] z of the items (LINEAR: r [m]), R [m][m], H [m][n] (LINEAR)
 constexpr int kAidThreads = 256;
 
 // per-member result; the first five fields are msckf_b200_aid_result's
@@ -24,6 +31,12 @@ struct AidOut {
   double nis, dx_norm;
   int dof, applied, status;
   int numeric;  // a non-finite dx or P entry was written
+};
+
+// one item of a stack: its model, a (CLONE_POSE and RELATIVE_POSE: a clone's window position; BODY_VELOCITY: the row mask),
+// b (RELATIVE_POSE: the second clone) and its first row in the stack
+struct AidItem {
+  short model, a, b, row;
 };
 
 template <class S>
@@ -35,16 +48,95 @@ struct AidArgs {
   double* ws;        // W^T [n][m] then dx [n] in global memory, or nullptr: in dynamic shared memory
   AidOut* out;
   double chi2_max;   // > 0: gate on NIS
-  int ldp, M, model, clone, m, pad_;
+  int ldp, M, m, n_items;  // LINEAR: one item of model kAidLinear
+  AidItem item[kAidMaxItems];
 };
 static_assert(sizeof(Members<AidArgs<double>, kBatchMembers>) <= 32764, "k_aid's batched arguments exceed the parameter limit");
 
 // bytes of W^T and dx of one member (in shared or global memory)
 __host__ __device__ constexpr size_t aid_ws_bytes(int n, int m) { return sizeof(double) * (size_t)n * (m + 1); }
 
-// state index of row i of a selection model: VELOCITY 6..8, POSITION 12..14, POSE [0..2, 12..14], CLONE_POSE 15+6k .. 20+6k
-__device__ __forceinline__ int aid_index(int model, int clone, int i) {
-  return model == kAidVelocity ? 6 + i : model == kAidPosition ? 12 + i : model == kAidPose ? (i < 3 ? i : 9 + i) : 15 + 6 * clone + i;
+// The rows of one model item: residual r[row + i] (fp64) and row row + i of H as nnz (state index, coefficient) pairs.
+// Perturbations follow the state injection, C(q+) = (I - [dtheta]x) C(q) (q+ = buildUpdateQuat(dtheta) * q), and the
+// rotation residual is dtheta(q_z, q^) of msckf_b200_nees, so that r ~ H dx to first order:
+//   VELOCITY, POSITION, POSE, CLONE_POSE  one coefficient 1 per row (the state index the model selects)
+//   BODY_VELOCITY  v^ = C(q_IG) v_I_G; row j of the mask: r = z_j - v^_j, H over dtheta [v^]x (row j), over dv C (row j)
+//   RELATIVE_POSE  C^ = C_b C_a^T, q^ = q_b * q_a^-1, p^ = C_a (p_b - p_a) of clones a, b:
+//                  rotation rows  H over dtheta_a -C^, over dtheta_b I, over dp_a and dp_b 0
+//                  position rows  H over dtheta_a [p^]x, over dp_a -C_a, over dtheta_b 0, over dp_b C_a
+// (Out of line, with the item by value: inlined into k_aid<double, 1>, this code made ptxas spill.)
+template <class S>
+__device__ __noinline__ void aid_item_rows(const AidItem it, const double* z, const DevState<S>* st, const S* poses,
+                                              double* r, int (*col)[kAidNnz], double (*coef)[kAidNnz], int* nnz) {
+  const int r0 = it.row;
+  if (it.model == kAidVelocity || it.model == kAidPosition) {
+    const S* x = it.model == kAidVelocity ? st->v_I_G : st->p_I_G;
+    for (int i = 0; i < 3; ++i) {
+      r[r0 + i] = z[i] - (double)x[i];
+      col[r0 + i][0] = (it.model == kAidVelocity ? 6 : 12) + i; coef[r0 + i][0] = 1.0; nnz[r0 + i] = 1;
+    }
+  } else if (it.model == kAidPose || it.model == kAidClonePose) {  // [dtheta(q_z, q_est); z_p - p_est]
+    const bool imu = it.model == kAidPose;
+    const S* q = imu ? st->q_IG : poses + kPoseStride * it.a;
+    const S* p = imu ? st->p_I_G : poses + kPoseStride * it.a + 4;
+    nees_quat_error(z + 3, q, r + r0);
+    for (int i = 0; i < 3; ++i) r[r0 + 3 + i] = z[i] - (double)p[i];
+    for (int i = 0; i < 6; ++i) {
+      col[r0 + i][0] = imu ? (i < 3 ? i : 9 + i) : 15 + 6 * it.a + i; coef[r0 + i][0] = 1.0; nnz[r0 + i] = 1;
+    }
+  } else if (it.model == kAidBodyVelocity) {
+    const double q[4] = {(double)st->q_IG[0], (double)st->q_IG[1], (double)st->q_IG[2], (double)st->q_IG[3]};
+    double C[9], v[3];
+    quat_to_rot(q, C);
+    for (int j = 0; j < 3; ++j) v[j] = C[3 * j] * (double)st->v_I_G[0] + C[3 * j + 1] * (double)st->v_I_G[1] + C[3 * j + 2] * (double)st->v_I_G[2];
+    const double sk[9] = {0.0, -v[2], v[1], v[2], 0.0, -v[0], -v[1], v[0], 0.0};  // [v^]x
+    int row = r0;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      if ((it.a >> j) & 1) {
+        r[row] = z[j] - v[j];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          col[row][k] = k; coef[row][k] = sk[3 * j + k];
+          col[row][3 + k] = 6 + k; coef[row][3 + k] = C[3 * j + k];
+        }
+        nnz[row++] = 6;
+      }
+    }
+  } else {  // kAidRelativePose
+    const S* A = poses + kPoseStride * it.a;
+    const S* B = poses + kPoseStride * it.b;
+    const double qa[4] = {(double)A[0], (double)A[1], (double)A[2], (double)A[3]};
+    const double qb[4] = {(double)B[0], (double)B[1], (double)B[2], (double)B[3]};
+    const double na = qa[0] * qa[0] + qa[1] * qa[1] + qa[2] * qa[2] + qa[3] * qa[3];
+    const double qai[4] = {-qa[0] / na, -qa[1] / na, -qa[2] / na, qa[3] / na};
+    double Ca[9], Cb[9], Ch[9], qh[4], ph[3];
+    quat_to_rot(qa, Ca);
+    quat_to_rot(qb, Cb);
+    quat_mul(qb, qai, qh);
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) Ch[3 * i + j] = Cb[3 * i] * Ca[3 * j] + Cb[3 * i + 1] * Ca[3 * j + 1] + Cb[3 * i + 2] * Ca[3 * j + 2];
+    const double d[3] = {(double)B[4] - (double)A[4], (double)B[5] - (double)A[5], (double)B[6] - (double)A[6]};
+    for (int i = 0; i < 3; ++i) ph[i] = Ca[3 * i] * d[0] + Ca[3 * i + 1] * d[1] + Ca[3 * i + 2] * d[2];
+    nees_quat_error(z + 3, qh, r + r0);
+    for (int i = 0; i < 3; ++i) r[r0 + 3 + i] = z[i] - ph[i];
+    const double sk[9] = {0.0, -ph[2], ph[1], ph[2], 0.0, -ph[0], -ph[1], ph[0], 0.0};  // [p^]x
+    const int ca = 15 + 6 * it.a, cb = 15 + 6 * it.b;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        col[r0 + i][k] = ca + k; col[r0 + i][3 + k] = ca + 3 + k; col[r0 + i][6 + k] = cb + k; col[r0 + i][9 + k] = cb + 3 + k;
+        if (i < 3) {
+          coef[r0 + i][k] = -Ch[3 * i + k]; coef[r0 + i][3 + k] = 0.0; coef[r0 + i][6 + k] = i == k ? 1.0 : 0.0; coef[r0 + i][9 + k] = 0.0;
+        } else {
+          coef[r0 + i][k] = sk[3 * (i - 3) + k]; coef[r0 + i][3 + k] = -Ca[3 * (i - 3) + k];
+          coef[r0 + i][6 + k] = 0.0; coef[r0 + i][9 + k] = Ca[3 * (i - 3) + k];
+        }
+      }
+      nnz[r0 + i] = kAidNnz;
+    }
+  }
 }
 
 template <class S, int NM>
@@ -56,7 +148,8 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
   S* const poses = a.m[f].poses;
   const double* __restrict__ const in = a.m[f].in;
   AidOut* const out = a.m[f].out;
-  const int ldp = a.m[f].ldp, M = a.m[f].M, model = a.m[f].model, clone = a.m[f].clone, m = a.m[f].m, n = 15 + 6 * M;
+  const int ldp = a.m[f].ldp, M = a.m[f].M, m = a.m[f].m, n = 15 + 6 * M;
+  const bool lin = a.m[f].item[0].model == kAidLinear;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   double* const Wt = a.m[f].ws ? a.m[f].ws : aid_dyn;  // [n][m]: column c of H P, then of W = L^-1 H P
   double* const dx = Wt + (size_t)n * m;
@@ -65,31 +158,20 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
   __shared__ double L[kAidMaxRows + 1][kAidMaxRows + 1];  // S = L L^T (lower); row m: r, then y = L^-1 r
   __shared__ double idg[kAidMaxRows];
   __shared__ double part[kAidThreads / 32];
-  __shared__ int s_idx[kAidMaxRows];
+  __shared__ int s_col[kAidMaxRows][kAidNnz];             // the model rows of H: (state index, coefficient) pairs
+  __shared__ double s_coef[kAidMaxRows][kAidNnz];
+  __shared__ int s_nnz[kAidMaxRows];
   __shared__ int s_nv, s_apply, s_bad;
 
-  // ---- residual (fp64) and the selected state indices
-  if (model == kAidLinear) {
+  // ---- residual (fp64) and the rows of H, one thread per item
+  if (lin) {
     if (t < m) L[m][t] = in[t];
-  } else {
-    if (t < m) s_idx[t] = aid_index(model, clone, t);
-    if (t == 0) {
-      const double* z = in;
-      if (model == kAidVelocity) {
-        for (int i = 0; i < 3; ++i) L[3][i] = z[i] - (double)st->v_I_G[i];
-      } else if (model == kAidPosition) {
-        for (int i = 0; i < 3; ++i) L[3][i] = z[i] - (double)st->p_I_G[i];
-      } else {  // [dtheta(q_z, q_est); z_p - p_est], dtheta in the convention of the NEES error state
-        const S* q = model == kAidPose ? st->q_IG : poses + kPoseStride * clone;
-        const S* p = model == kAidPose ? st->p_I_G : poses + kPoseStride * clone + 4;
-        nees_quat_error(z + 3, q, &L[6][0]);
-        for (int i = 0; i < 3; ++i) L[6][3 + i] = z[i] - (double)p[i];
-      }
-    }
+  } else if (t < a.m[f].n_items) {
+    aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, &L[m][0], s_col, s_coef, s_nnz);
   }
   __syncthreads();
   // ---- H P, stored transposed: Wt[c][i] = (H P)[i][c]
-  if (model == kAidLinear) {
+  if (lin) {
     for (int idx = t; idx < m * n; idx += kAidThreads) {
       const int i = idx / n, c = idx - i * n;
       const double* h = H + (size_t)i * n;
@@ -100,7 +182,9 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
   } else {
     for (int idx = t; idx < m * n; idx += kAidThreads) {
       const int i = idx / n, c = idx - i * n;
-      Wt[(size_t)c * m + i] = (double)P[(size_t)s_idx[i] * ldp + c];
+      double s = s_coef[i][0] * (double)P[(size_t)s_col[i][0] * ldp + c];  // (exact for the one-coefficient rows)
+      for (int k = 1; k < s_nnz[i]; ++k) s += s_coef[i][k] * (double)P[(size_t)s_col[i][k] * ldp + c];
+      Wt[(size_t)c * m + i] = s;
     }
   }
   __syncthreads();
@@ -109,12 +193,13 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
     const int i = idx / m, j = idx - i * m;
     if (j > i) continue;
     double s;
-    if (model == kAidLinear) {
+    if (lin) {
       const double* h = H + (size_t)j * n;
       s = 0.0;
       for (int k = 0; k < n; ++k) s += Wt[(size_t)k * m + i] * h[k];
     } else {
-      s = Wt[(size_t)s_idx[j] * m + i];
+      s = s_coef[j][0] * Wt[(size_t)s_col[j][0] * m + i];
+      for (int k = 1; k < s_nnz[j]; ++k) s += s_coef[j][k] * Wt[(size_t)s_col[j][k] * m + i];
     }
     L[i][j] = s + R[i * m + j];
   }

@@ -122,6 +122,18 @@ int numeric_error(const char* what, int member) {
   return fail(MSCKF_B200_ERR_NUMERIC, std::string(what) + ": non-finite delta-x or covariance entry (member " + std::to_string(member) + "); the update was applied");
 }
 
+// One member's aided update as k_aid takes it: up to 8 model items stacked into m rows (a single-model call or a LINEAR
+// update is one item), each with its z and its own block of the block-diagonal R.  n_items = 0: the member is left alone.
+struct AidJob {
+  int m = 0, n_items = 0;
+  mb::AidItem item[mb::kAidMaxItems] = {};
+  const double* z[mb::kAidMaxItems] = {};  // (LINEAR: the residual r)
+  int nz[mb::kAidMaxItems] = {};
+  const double* R[mb::kAidMaxItems] = {};  // [rows][rows] of the item, row-major, lower triangle read
+  const double* H = nullptr;               // LINEAR: [m][n]
+  double chi2_max = 0.0;
+};
+
 // tail kernel choice (engine option 3 / window size)
 inline size_t tail_legacy_smem(int n, int NB) {
   const int ldt = (n + 3) & ~3;
@@ -163,8 +175,10 @@ struct CtxBase {
   virtual int get_state(void* const* imu, void* const* poses) = 0;
   // NEES of every member against caller-given truth (msckf_b200_nees / _batch_nees): read-only, one synchronisation
   virtual int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) = 0;
-  // aided measurement updates of the members (msckf_b200_aid_update / _batch_aid_update): one launch per 32, one synchronisation
+  // aided measurement updates of the members (msckf_b200_aid_update / _batch_aid_update, and the stacked
+  // msckf_b200_aid_stack_update / _batch_aid_stack_update): one launch per 32, one synchronisation
   virtual int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) = 0;
+  virtual int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) = 0;
   // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
   virtual int landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) = 0;
   cudaStream_t stream = nullptr;
@@ -435,6 +449,8 @@ struct Ctx : CtxBase {
   int get_state(void* const* imu, void* const* poses) override;
   int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) override;
   int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) override;
+  int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) override;
+  int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what);
   int landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
@@ -704,8 +720,10 @@ struct Engine : EngineBase {
     return {d_st, d_P, d_poses, truth, W, out, ldp, M, full ? 15 + 6 * M : 15, full ? 1 : 0};
   }
   // k_aid's arguments; in / ws / out are device addresses in the calling context's buffers (ws = nullptr: shared memory)
-  mb::AidArgs<S> aid_args(const msckf_b200_aid& q, int m, const double* in, double* ws, mb::AidOut* out) const {
-    return {d_st, d_P, d_poses, in, ws, out, q.chi2_max, ldp, M, q.model, q.model == MSCKF_B200_AID_CLONE_POSE ? q.clone : 0, m, 0};
+  mb::AidArgs<S> aid_args(const AidJob& q, const double* in, double* ws, mb::AidOut* out) const {
+    mb::AidArgs<S> a = {d_st, d_P, d_poses, in, ws, out, q.chi2_max, ldp, M, q.m, q.n_items, {}};
+    for (int k = 0; k < q.n_items; ++k) a.item[k] = q.item[k];
+    return a;
   }
   // the landmark kernels' arguments except the device addresses, which the calling context fills in
   mb::LmkArgs<S> lmk_args(const msckf_b200_landmarks& q, int G, int ld) const {
@@ -1414,22 +1432,22 @@ int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_pose
   return 0;
 }
 
-// Aided updates: every updated member's inputs travel in the I/O block ([32] z, R [m][m], H [m][n] for LINEAR), k_aid runs
-// through per_member (NM = 1 with one member in the context), the results come back with one copy and one synchronisation.
-// W^T and dx (n (m + 1) doubles) sit in dynamic shared memory up to kAidSmemMax bytes, else in the workspace.  Nothing is
-// launched unless every member is valid.
+// Aided updates: every updated member's inputs travel in the I/O block ([8][8] z of its items (LINEAR: r), the block-diagonal
+// R [m][m], H [m][n] for LINEAR), k_aid runs through per_member (NM = 1 with one member in the context), the results come back
+// with one copy and one synchronisation.  W^T and dx (n (m + 1) doubles) sit in dynamic shared memory up to kAidSmemMax bytes,
+// else in the workspace.  Nothing is launched unless every member is valid: aid and aid_stack check their arguments and
+// build one AidJob per member, aid_run launches them.
 static_assert(offsetof(mb::AidOut, status) == offsetof(msckf_b200_aid_result, status), "mb::AidOut must start like msckf_b200_aid_result");
+static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && (int)MSCKF_B200_AID_RELATIVE_POSE == (int)mb::kAidRelativePose,
+              "msckf_b200_aid_model and mb::AidModel differ");
 constexpr size_t kAidSmemMax = 32 * 1024;
 template <class S>
 int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "aid_update: null argument");
   RC(members_ready("aid_update"));
   const int nf = (int)eng.size();
-  std::vector<int> idx, rows(nf, 0);
-  std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
+  std::vector<AidJob> job(nf);
   for (int i = 0; i < nf; ++i) {
-    off[i + 1] = off[i];
-    woff[i + 1] = woff[i];
     const msckf_b200_aid& q = in[i];
     if (q.model < 0) continue;
     const std::string who = " (member " + std::to_string(i) + ")";
@@ -1449,9 +1467,81 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
     if (!lin && nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
       return fail(MSCKF_B200_ERR_ARG, "aid_update: zero quaternion" + who);
     if (std::isnan(q.chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_update: chi2_max is NaN" + who);
-    rows[i] = m;
+    AidJob& j = job[i];
+    j.m = m; j.n_items = 1; j.chi2_max = q.chi2_max;
+    j.item[0] = {(short)q.model, (short)(q.model == MSCKF_B200_AID_CLONE_POSE ? q.clone : 0), 0, 0};
+    j.z[0] = q.z; j.nz[0] = nz; j.R[0] = q.R; j.H = lin ? q.H : nullptr;
+  }
+  return aid_run(job, out, "aid_update");
+}
+
+template <class S>
+int Ctx<S>::aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) {
+  if (!items || !n_items || !out) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: null argument");
+  RC(members_ready("aid_stack_update"));
+  if (std::isnan(chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: chi2_max is NaN");
+  const int nf = (int)eng.size();
+  std::vector<AidJob> job(nf);
+  for (int i = 0; i < nf; ++i) {
+    if (n_items[i] == 0) continue;
+    const std::string who = " (member " + std::to_string(i) + ")";
+    if (n_items[i] < 0 || n_items[i] > mb::kAidMaxItems) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: 1 to 8 items per stack" + who);
+    if (!items[i]) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: null item list" + who);
+    const int M = eng[i]->M;
+    AidJob& j = job[i];
+    for (int k = 0; k < n_items[i]; ++k) {
+      const msckf_b200_aid_item& q = items[i][k];
+      const std::string wk = " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")";
+      int m = 0, nz = 3;
+      switch (q.model) {
+        case MSCKF_B200_AID_VELOCITY: case MSCKF_B200_AID_POSITION: m = 3; break;
+        case MSCKF_B200_AID_POSE: m = 6; nz = 7; break;
+        case MSCKF_B200_AID_CLONE_POSE:
+          if (q.a < 0 || q.a >= M) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: clone outside the window" + wk);
+          m = 6; nz = 7;
+          break;
+        case MSCKF_B200_AID_BODY_VELOCITY:
+          if (q.a < 1 || q.a > 7) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: the row mask must select rows 0..2" + wk);
+          m = (q.a & 1) + ((q.a >> 1) & 1) + ((q.a >> 2) & 1);
+          break;
+        case MSCKF_B200_AID_RELATIVE_POSE:
+          if (q.a < 0 || q.a >= M || q.b < 0 || q.b >= M) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: clone outside the window" + wk);
+          if (q.a == q.b) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: a relative pose needs two different clones" + wk);
+          m = 6; nz = 7;
+          break;
+        default: return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: model not allowed in a stack" + wk);
+      }
+      if (j.m + m > mb::kAidMaxRows) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: more than 32 rows" + who);
+      if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: missing or non-finite z" + wk);
+      if (nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
+        return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: zero quaternion" + wk);
+      if (!q.R) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: missing R" + wk);
+      for (int r = 0; r < m; ++r)
+        if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: non-finite R" + wk);
+      j.item[k] = {(short)q.model, (short)(q.model == MSCKF_B200_AID_VELOCITY || q.model == MSCKF_B200_AID_POSITION ||
+                                           q.model == MSCKF_B200_AID_POSE ? 0 : q.a),
+                   (short)(q.model == MSCKF_B200_AID_RELATIVE_POSE ? q.b : 0), (short)j.m};
+      j.z[k] = q.z; j.nz[k] = nz; j.R[k] = q.R;
+      j.m += m;
+    }
+    j.n_items = n_items[i];
+    j.chi2_max = chi2_max;
+  }
+  return aid_run(job, out, "aid_stack_update");
+}
+
+template <class S>
+int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what) {
+  const int nf = (int)eng.size();
+  std::vector<int> idx;
+  std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
+  for (int i = 0; i < nf; ++i) {
+    const int m = job[i].m, n = 15 + 6 * eng[i]->M;
+    off[i + 1] = off[i];
+    woff[i + 1] = woff[i];
+    if (job[i].n_items == 0) continue;
     idx.push_back(i);
-    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (lin ? (size_t)m * n : 0)));
+    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (job[i].H ? (size_t)m * n : 0)));
     if (mb::aid_ws_bytes(n, m) > kAidSmemMax) woff[i + 1] = woff[i] + up256(mb::aid_ws_bytes(n, m));
   }
   if (idx.empty()) return 0;
@@ -1460,20 +1550,24 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
   RC(io.ensure(res_off + sizeof(mb::AidOut) * nf, stream));
   RC(ws.ensure(woff[nf], stream));
   for (int i : idx) {
-    const msckf_b200_aid& q = in[i];
-    const int m = rows[i], n = 15 + 6 * eng[i]->M;
+    const AidJob& q = job[i];
+    const int m = q.m, n = 15 + 6 * eng[i]->M;
     double* h = reinterpret_cast<double*>(io.h + off[i]);
-    memset(h, 0, sizeof(double) * mb::kAidZ);
-    memcpy(h, q.z, sizeof(double) * (q.model == MSCKF_B200_AID_LINEAR ? m : q.model <= MSCKF_B200_AID_POSITION ? 3 : 7));
-    memcpy(h + mb::kAidZ, q.R, sizeof(double) * m * m);
-    if (q.model == MSCKF_B200_AID_LINEAR) memcpy(h + mb::kAidZ + m * m, q.H, sizeof(double) * m * n);
+    memset(h, 0, sizeof(double) * (mb::kAidZ + (size_t)m * m));
+    double* R = h + mb::kAidZ;
+    for (int k = 0; k < q.n_items; ++k) {
+      memcpy(h + mb::kAidItemZ * k, q.z[k], sizeof(double) * q.nz[k]);
+      const int r0 = q.item[k].row, mk = (k + 1 < q.n_items ? q.item[k + 1].row : m) - r0;
+      for (int r = 0; r < mk; ++r) memcpy(R + (size_t)(r0 + r) * m + r0, q.R[k] + (size_t)r * mk, sizeof(double) * mk);
+    }
+    if (q.H) memcpy(h + mb::kAidZ + m * m, q.H, sizeof(double) * m * n);
   }
   CK(cudaMemcpyAsync(io.d, io.h, off[nf], cudaMemcpyHostToDevice, stream));
   mb::AidOut* d_out = reinterpret_cast<mb::AidOut*>(io.d + res_off);
   per_member(idx, false,
              [&](int i) {
                const bool global = woff[i + 1] > woff[i];
-               return eng[i]->aid_args(in[i], rows[i], reinterpret_cast<const double*>(io.d + off[i]),
+               return eng[i]->aid_args(job[i], reinterpret_cast<const double*>(io.d + off[i]),
                                        global ? reinterpret_cast<double*>(ws.d + woff[i]) : nullptr, d_out + i);
              },
              [&](const auto& a, int nm) {
@@ -1492,7 +1586,7 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
     out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].applied = o.applied; out[i].status = o.status;
     if (o.numeric && numeric < 0) numeric = i;
   }
-  return numeric_error("aid_update", numeric);
+  return numeric_error(what, numeric);
 }
 
 // Mapped-landmark updates: every member with observations sends its observations (grouped by clone in window order, input
@@ -1772,6 +1866,11 @@ int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, 
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->aid(aid, out);
 }
+int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                      double chi2_max, msckf_b200_aid_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->aid_stack(items, n_items, chi2_max, out);
+}
 int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->landmarks(lm, out);
@@ -1810,6 +1909,12 @@ int msckf_b200_aid_update(msckf_b200_engine* e, const msckf_b200_aid* aid, msckf
   if (!e || !aid) return fail(MSCKF_B200_ERR_ARG, "null argument");
   if (aid->model < 0) return fail(MSCKF_B200_ERR_ARG, "aid_update: unknown model");
   return e->impl->solo_ctx()->aid(aid, out);
+}
+int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,
+                                msckf_b200_aid_result* out) {
+  if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: 1 to 8 items per stack");
+  return e->impl->solo_ctx()->aid_stack(&items, &n_items, chi2_max, out);
 }
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");

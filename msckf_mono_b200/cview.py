@@ -133,6 +133,19 @@ class FilterBatch:
         self._call("aid_update", (Aid * n)(*[a for a, _ in st]), out)
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
+    def aid_stack_update(self, stacks, chi2_max=0.0):
+        """MSCKFBatch::aidedUpdate(items): stacks[i] = list of item dicts for filter i (as for capi.aid_items; None or []:
+        filter i left alone); one device call for the batch.  A list of result dicts (None for a filter left alone)."""
+        from .capi import AidResult, aid_items
+        n = len(self.filters)
+        assert len(stacks) == n
+        flat = [it for s in stacks for it in (s or [])]
+        arr, keep = aid_items(flat)
+        cnt = np.array([len(s or []) for s in stacks], dtype=np.int32)
+        out = (AidResult * n)()
+        self._call("aid_stack_update", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), out)
+        return [o.as_dict() if s else None for s, o in zip(stacks, out)]
+
     def landmark_update(self, obs, R=None, chi2_obs=0.0):
         """MSCKFBatch::landmarkUpdate: obs[i] = (state_ids [n], z [n, 2], p_L [n, 3]) for filter i, or None (filter i left
         alone); R None (each filter's pixel noise) or 2 x 2; one device call for the batch.  A list of result dicts with
@@ -329,6 +342,36 @@ class CFilter:
         a, keep = aid_struct({"model": model, "z": z, "R": R, "H": H, "clone": clone, "chi2_max": chi2_max})
         out = AidResult()
         self._chk(self._f("aid_update")(self.h, C.byref(a), C.byref(out)), "aid_update")
+        return out.as_dict()
+
+    def aid_stack_update(self, items, chi2_max=0.0):
+        """MSCKF::aidedUpdate(items) (include/msckf_b200.h: msckf_b200_aid_stack_update): items as for capi.aid_items, one
+        chi2_max for the stack.  A dict nis, dx_norm, dof, applied, status."""
+        from .capi import AidResult, aid_items
+        arr, keep = aid_items(items)
+        out = AidResult()
+        self._chk(self._f("aid_stack_update")(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)), "aid_stack_update")
+        return out.as_dict()
+
+    def body_velocity_update(self, v_I, R, mask=7, chi2_max=0.0):
+        """MSCKF::bodyVelocityUpdate: the IMU's velocity v_I in its own frame, rows selected by mask (bits 0..2), R over them"""
+        from .capi import AidResult
+        v, pv = _d(np.asarray(v_I, float).ravel())
+        Rm, pR = _d(np.asarray(R, float))
+        out = AidResult()
+        self._chk(self._f("body_velocity_update")(self.h, pv, C.c_int(int(mask)), pR, C.c_double(chi2_max), C.byref(out)),
+                  "body_velocity_update")
+        return out.as_dict()
+
+    def relative_pose_update(self, state_id_a, state_id_b, p, q, R, chi2_max=0.0):
+        """MSCKF::relativePoseUpdate: the pose (p, q xyzw) of image state_id_b relative to image state_id_a, R 6 x 6"""
+        from .capi import AidResult
+        pa, pp = _d(np.asarray(p, float).ravel())
+        qa, pq = _d(np.asarray(q, float).ravel())
+        Rm, pR = _d(np.asarray(R, float))
+        out = AidResult()
+        self._chk(self._f("relative_pose_update")(self.h, C.c_int(int(state_id_a)), C.c_int(int(state_id_b)), pp, pq, pR,
+                                                  C.c_double(chi2_max), C.byref(out)), "relative_pose_update")
         return out.as_dict()
 
     def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0):

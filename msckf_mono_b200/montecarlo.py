@@ -24,6 +24,15 @@ are drawn independently of the tracked-feature pixels of the same landmark in th
 would see one pixel noise in both), which leaves the two measurements uncorrelated.  The NIS of the map updates gives another
 truth-free consistency figure (ANIS against chi^2 with 2 dof per used observation).
 
+Optional odometry (wheel or leg odometry, or another tracker's relative motion): every `odo_every` frames, after the prune (and
+after a position fix when both are on), each trial fuses ONE stacked update (MSCKFBatch::aidedUpdate(items), one batched call):
+the truth body velocity C(q_IG) v_I_G plus N(0, odo_sigma_v^2) per row (rows y, z only with nhc: the rows a non-holonomic
+constraint uses; on this trajectory they are not zero, so z is the truth plus noise, not 0), and, once the window holds two
+clones, the truth pose of its newest clone relative to the one before plus noise: position N(0, odo_sigma_rel^2 I) in metres,
+rotation buildUpdateQuat-style N(0, odo_sigma_rel^2 I) in radians.  The noise of trial k comes from its own stream
+np.random.default_rng([seed, k, 3]), 9 standard normals per odometry frame, so the trial's other inputs are the same with
+odometry on or off.  The NIS of the stacks gives another truth-free consistency figure (ANIS against chi^2 with the stack's rows).
+
 Error-state convention (the inverse of the filter's state injection q+ = buildUpdateQuat(dtheta) * q): dq = q_true * q_est^-1
 with the Hamilton product, dq negated when dq.w < 0, dtheta = -2 vec(dq); every other component is truth - estimate.  Host
 vectors here are in the filter's covariance order [dtheta, db_g, dv, db_a, dp, clones (dtheta_C, dp_C)...].
@@ -34,6 +43,7 @@ import numpy as np
 from scipy import stats
 
 from . import synth
+from .capi import AID_BODY_VELOCITY, AID_RELATIVE_POSE
 
 COMPONENTS = ("orientation", "position", "pose", "imu", "full")
 DOF = {"orientation": 3, "position": 3, "pose": 6, "imu": 15}
@@ -64,6 +74,76 @@ def quat_of_error(dth):
     """the quaternion dq of dtheta (w >= 0): buildUpdateQuat without its renormalisation"""
     v = -0.5 * np.asarray(dth, dtype=np.float64)
     return np.array([v[0], v[1], v[2], np.sqrt(max(0.0, 1.0 - v @ v))])
+
+
+def quat_to_rot(q):
+    """C(q): Eigen's toRotationMatrix, as the filter's quat_to_rot (C(q_CG) maps G to the camera frame)"""
+    x, y, z, w = np.asarray(q, dtype=np.float64)
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+# ---- odometry models (msckf_b200_aid_stack_update's BODY_VELOCITY and RELATIVE_POSE) ---------------------------------------
+def body_velocity(imu):
+    """v_I = C(q_IG) v_I_G of a 19-double IMU state (p, v, b_g, b_a, g, q_IG)"""
+    imu = np.asarray(imu, dtype=np.float64)
+    return quat_to_rot(imu[15:19]) @ imu[3:6]
+
+
+def relative_pose(pose_a, pose_b):
+    """(p, q xyzw) of camera pose b relative to camera pose a (each p_C_G (3), q_CG (4)): p = C_a (p_b - p_a), q = q_b * q_a^-1"""
+    a, b = np.asarray(pose_a, dtype=np.float64), np.asarray(pose_b, dtype=np.float64)
+    return quat_to_rot(a[3:7]) @ (b[0:3] - a[0:3]), quat_mul(b[3:7], quat_inv(a[3:7]))
+
+
+def odometry_residual(item, imu, poses):
+    """r of one BODY_VELOCITY or RELATIVE_POSE item (a dict as for capi.aid_items) at the state (imu 19+, poses [M, 7]), in fp64"""
+    z = np.asarray(item["z"], dtype=np.float64)
+    if item["model"] == AID_BODY_VELOCITY:  # the rows of the mask
+        return (z - body_velocity(imu))[[j for j in range(3) if (item["a"] >> j) & 1]]
+    p, q = relative_pose(poses[item["a"]], poses[item["b"]])
+    return np.concatenate([quat_error(z[3:7], q), z[0:3] - p])
+
+
+def odometry_jacobian(item, imu, poses, n):
+    """H [m, n] of one BODY_VELOCITY or RELATIVE_POSE item in the filter's injection convention, C(q+) = (I - [dtheta]x) C(q):
+    the host linearisation of the models msckf_b200_aid_stack_update forms on the device"""
+    def skew(v):
+        return np.array([[0.0, -v[2], v[1]], [v[2], 0.0, -v[0]], [-v[1], v[0], 0.0]])
+    imu, poses = np.asarray(imu, dtype=np.float64), np.asarray(poses, dtype=np.float64)
+    if item["model"] == AID_BODY_VELOCITY:
+        C = quat_to_rot(imu[15:19])
+        rows = [j for j in range(3) if (item["a"] >> j) & 1]
+        H = np.zeros((len(rows), n))
+        H[:, 0:3] = skew(C @ imu[3:6])[rows]
+        H[:, 6:9] = C[rows]
+        return H
+    a, b = item["a"], item["b"]
+    Ca, Cb = quat_to_rot(poses[a, 3:7]), quat_to_rot(poses[b, 3:7])
+    ia, ib = 15 + 6 * a, 15 + 6 * b
+    H = np.zeros((6, n))
+    H[0:3, ia:ia + 3] = -Cb @ Ca.T
+    H[0:3, ib:ib + 3] = np.eye(3)
+    H[3:6, ia:ia + 3] = skew(Ca @ (poses[b, 0:3] - poses[a, 0:3]))
+    H[3:6, ia + 3:ia + 6] = -Ca
+    H[3:6, ib + 3:ib + 6] = Ca
+    return H
+
+
+def odometry_items(truth_imu, pose_a, pose_b, noise, sigma_v, sigma_rel, nhc=False):
+    """one odometry stack as aid item dicts: the body velocity of truth_imu plus sigma_v noise[0:3] (mask 0b110 with nhc, else
+    0b111) and, when pose_a is not None, the pose of pose_b relative to pose_a with position noise sigma_rel noise[3:6] and
+    rotation noise sigma_rel noise[6:9]; clones a, b are the window's last two positions (a = -2, b = -1: set by the caller)"""
+    mask = 0b110 if nhc else 0b111
+    rows = [j for j in range(3) if (mask >> j) & 1]
+    items = [{"model": AID_BODY_VELOCITY, "a": mask, "z": body_velocity(truth_imu) + sigma_v * noise[0:3], "R": sigma_v ** 2 * np.eye(len(rows))}]
+    if pose_a is not None:
+        p, q = relative_pose(pose_a, pose_b)
+        q = quat_mul(quat_of_error(sigma_rel * noise[6:9]), q)
+        items.append({"model": AID_RELATIVE_POSE, "z": np.concatenate([p + sigma_rel * noise[3:6], q / np.linalg.norm(q)]),
+                      "R": sigma_rel ** 2 * np.eye(6)})
+    return items
 
 
 # ---- states: {"imu": 19 doubles (p, v, b_g, b_a, g, q_IG), "poses": [M, 7] (p_C_G, q_CG) or None} ----------------------
@@ -141,10 +221,11 @@ def map_observations(truth, frame, stride):
     return idx, np.stack([xn[idx], yn[idx]], axis=1)
 
 
-def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20):
+def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
     fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
-    map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks."""
+    map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks.  With
+    odo_every > 0, "odometry" holds per frame None or the 9 standard normals of that frame's odometry noise (odometry_items)."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -188,6 +269,9 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
                 continue
             idx, z = map_observations(truth, f, map_stride)
             out["maps"].append((idx, truth["landmarks"][::map_stride][idx], z + mrng.standard_normal(z.shape) * np.array([su, sv])))
+    if odo_every > 0:
+        orng = np.random.default_rng([seed, k, 3])
+        out["odometry"] = [orng.standard_normal(9) if (f + 1) % odo_every == 0 else None for f in range(len(truth["frames"]))]
     return out
 
 
@@ -199,15 +283,17 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=()):
-    """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes and of its
-    map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n), as plain lists"""
+def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=()):
+    """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes, of its
+    map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n) and of its odometry
+    stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists"""
     return {"nees": {c: [float(r[c]) for r in nees_rows] for c in COMPONENTS},
             "dim": {c: [int(r["dim_full"]) if c == "full" else DOF[c] for r in nees_rows] for c in COMPONENTS},
             "first_bad_pivot": [int(r["first_bad_pivot"]) for r in nees_rows],
             "pos_err2": [float(x) for x in pos_err2],
             "fix_nis": [float(x) for x in fix_nis],
-            "map": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in map_rows] for key in ("nis", "dof", "used", "applied", "n")}}
+            "map": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in map_rows] for key in ("nis", "dof", "used", "applied", "n")},
+            "odometry": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in odo_rows] for key in ("nis", "dof", "applied")}}
 
 
 def chi2_bounds(total_dof, n, lo=0.025, hi=0.975):
@@ -262,23 +348,36 @@ def summarize(records):
                       "run_bounds": list(tot), "updates_inside": float(np.mean(inside)),
                       "applied": float(np.mean([a for m in mp for a in m["applied"]])),
                       "observations": int(n_obs), "gated": float(1.0 - sum(sum(m["used"]) for m in mp) / max(n_obs, 1))}
+    od = [records[k].get("odometry") for k in keys]
+    if all(o is not None and len(o["nis"]) for o in od):  # ANIS of the odometry stacks: the stack's rows per trial and update
+        V = np.array([o["nis"] for o in od]); D = np.array([o["dof"] for o in od])
+        anis, dof = V.sum(axis=0) / N, D.sum(axis=0)
+        lo, hi = zip(*[chi2_bounds(int(d), N) for d in dof])
+        out["odometry"] = {"anis": [float(a) for a in anis], "lower": list(lo), "upper": list(hi), "dof": [int(d) for d in dof],
+                           "mean_anis": float(V.sum() / V.size), "mean_dof": float(D.sum() / D.size),
+                           "run_bounds": list(chi2_bounds(int(D.sum()), V.size)),
+                           "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])),
+                           "applied": float(np.mean([a for o in od for a in o["applied"]]))}
     return out
 
 
 # ---- the batched run ---------------------------------------------------------------------------------------------------------
-def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0):
+def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0,
+        odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
+    [every odo_every frames one batched odometry stack (odometry_items)],
     [every map_every frames one batched mapped-landmark update from the newest clone, gated per observation at map_chi2 > 0],
     refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.
     Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
     from . import engine_filter
     from .capi import AID_POSITION
     from .cview import FilterBatch
-    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride) for k in trials]
+    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every) for k in trials]
     R_fix = (fix_sigma ** 2) * np.eye(3)
     nis = [[] for _ in trs]
     maps = [[] for _ in trs]
+    odo = [[] for _ in trs]
     fs = [engine_filter(dtype) for _ in trs]
     for f, tr in zip(fs, trs):
         f.initialize(truth["camera"], truth["noise"], truth["params"], tr["imu_state"])
@@ -300,6 +399,17 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             res = fb.aid_update([{"model": AID_POSITION, "z": tr["fixes"][fi], "R": R_fix} for tr in trs])
             for i, r in enumerate(res):
                 nis[i].append(r["nis"])
+        if odo_every > 0 and trs[0]["odometry"][fi] is not None:
+            stacks = []
+            for f, tr in zip(fs, trs):
+                ids = f.getCamStates()["state_id"]
+                pa, pb = (truth["truth_pose"][ids[-2]], truth["truth_pose"][ids[-1]]) if len(ids) >= 2 else (None, None)
+                items = odometry_items(truth["truth_imu"][fi], pa, pb, tr["odometry"][fi], odo_sigma_v, odo_sigma_rel, nhc)
+                if len(items) > 1:
+                    items[1].update(a=len(ids) - 2, b=len(ids) - 1)
+                stacks.append(items)
+            for i, r in enumerate(fb.aid_stack_update(stacks)):
+                odo[i].append(r)
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [(np.full(len(tr["maps"][fi][0]), fr["state_id"]), tr["maps"][fi][2], tr["maps"][fi][1]) if len(tr["maps"][fi][0]) else None
                    for tr, fr in zip(trs, frs)]
@@ -319,7 +429,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         if on_frame is not None:
             on_frame(fi, fs, res)
     fb.close()
-    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i]) for i, tr in enumerate(trs)}
+    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i]) for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):
         s = f.getImuState()

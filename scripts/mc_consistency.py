@@ -14,6 +14,10 @@ With --map-every K, every K frames each trial also observes the map (every --map
 its newest clone and fuses the observations as mapped landmarks (after the prune and after a position fix), and the summary adds
 the map updates' ANIS against its 95 % chi^2 bounds and the fraction of observations gated out.
 
+With --odometry-every K, every K frames each trial also fuses one stacked odometry update (the truth body velocity, and the
+truth relative pose of its two newest clones, each plus noise of --odometry-sigma-v m/s and --odometry-sigma-rel m / rad;
+--nhc keeps only the body velocity's y and z rows), and the summary adds the stacks' ANIS against its 95 % chi^2 bounds.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -126,6 +130,10 @@ def main():
     ap.add_argument("--position-fix-sigma", type=float, default=0.1)
     ap.add_argument("--map-every", type=int, default=0)
     ap.add_argument("--map-stride", type=int, default=20)
+    ap.add_argument("--odometry-every", type=int, default=0)
+    ap.add_argument("--odometry-sigma-v", type=float, default=0.05)
+    ap.add_argument("--odometry-sigma-rel", type=float, default=0.01)
+    ap.add_argument("--nhc", action="store_true")
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -141,7 +149,8 @@ def main():
     t0 = time.perf_counter()
     records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed,
                         fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma, map_every=args.map_every,
-                        map_stride=args.map_stride)
+                        map_stride=args.map_stride, odo_every=args.odometry_every, odo_sigma_v=args.odometry_sigma_v,
+                        odo_sigma_rel=args.odometry_sigma_rel, nhc=args.nhc)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -154,6 +163,9 @@ def main():
     if "map" in s:
         res["map"] = {"every": args.map_every, "stride": args.map_stride,
                       **{k: s["map"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "observations", "gated")}}
+    if "odometry" in s:
+        res["odometry"] = {"every": args.odometry_every, "sigma_v": args.odometry_sigma_v, "sigma_rel": args.odometry_sigma_rel,
+                           "nhc": args.nhc, **{k: s["odometry"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied")}}
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
