@@ -282,7 +282,17 @@ int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_
  * both halves written, in place) and the state injection of msckf_b200_aid_update.  All arithmetic is fp64 for both dtypes.
  * Three launches per 32 members with observations, one host-to-device copy, one device-to-host copy, one synchronisation.
  * Caps: 256 observations per clone and 4096 per member and call.  The vision update's bookkeeping and the launch count are
- * not changed. */
+ * not changed.
+ * Iterated update (max_iter >= 2, an iterated EKF for relocalisation after drift, where one linearisation is far off): with
+ * delta_0 = 0 and the iterate x_i = x^ [+] delta_i on the clone poses (q <- normalise(buildUpdateQuat(dtheta) * q), p <- p + dp,
+ * fp64), linearisation i evaluates r_i, H_i at x_i, compresses [X~ | r~ + X~ e_k] per clone as above (e_k: delta_i of clone k)
+ * and factors S against the prior P; delta_{i+1} = W^T y = K_i (r_i + H_i delta_i).  It stops when max |delta_{i+1} - delta_i|
+ * <= tol (converged) or after max_iter linearisations; then P <- P - W^T W and one injection of W^T y, both of the last
+ * linearisation.  The flags, gamma, NIS and dof are linearisation 0's.  A used observation that is behind the camera or not
+ * finite at an iterate stops the iteration, and the previous linearisation is applied.  The Jacobian of [+] is not applied
+ * (the iterate's error-state Jacobian is taken as I).  The launches per 32 members become clone, gain, (step, clone, gain) x
+ * (K - 1), downdate, with K the largest max_iter among them; still one copy each way and one synchronisation.
+ * max_iter 0 or 1 is the single linearisation above, bit for bit. */
 typedef struct {
   int n_obs;             /* observations; in a batch, 0 leaves the member untouched */
   const int* clone;      /* [n_obs] positions in the window */
@@ -292,6 +302,8 @@ typedef struct {
   double chi2_obs;       /* > 0: per-observation gate on gamma */
   double* gamma;         /* [n_obs] out, or NULL */
   int* flag;             /* [n_obs] out (0 used, 1 gated out, 2 behind the camera / not finite), or NULL */
+  int max_iter;          /* linearisations, 0 .. 16 (0 or 1: one) */
+  double tol;            /* finite, >= 0: the iteration has converged when max |delta_{i+1} - delta_i| <= tol */
 } msckf_b200_landmarks;
 typedef struct {
   double nis;            /* NIS of the used observations (NaN when S is not positive definite) */
@@ -300,10 +312,13 @@ typedef struct {
   int rows;              /* rows of the compressed system (sum over clones of min(2 a_k, 6)) */
   int used;              /* observations with flag 0 */
   int applied;           /* 1: P and the state were updated */
-  int status;            /* 0: applied, or nothing used; 1: S not positive definite, nothing written */
+  int status;            /* 0: applied, or nothing used; 1: S not positive definite (at any linearisation), nothing written */
+  int iterations;        /* linearisations applied (1 for the single linearisation; 0 when nothing was applied) */
+  int converged;         /* 1: the last step was <= tol (always 0 for max_iter <= 1) */
+  double step;           /* the last max |delta_{i+1} - delta_i| (0 for max_iter <= 1) */
 } msckf_b200_landmark_result;
 /* A clone outside the window, n_obs < 0 or beyond the caps, a NULL or non-finite z / p_L_G / R, an R that is not positive
- * definite or a NaN chi2_obs returns MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
+ * definite, a NaN chi2_obs, max_iter outside 0 .. 16 or a tol that is not finite and >= 0 returns MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
  * A non-finite dx or P entry returns MSCKF_B200_ERR_NUMERIC with the result filled and the update applied.  n_obs = 0 on a single
  * engine fills out with zeros and launches nothing. */
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out);

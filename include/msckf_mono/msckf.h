@@ -411,11 +411,15 @@ class MSCKF {
   // coordinates (NULL: diag(u_var', v_var')); chi2_obs > 0 gates every observation on its own.  gamma / flag (optional) receive
   // one entry per observation.  An observation of an image that is not in the window throws std::invalid_argument before any
   // device call.  Queued IMU readings are applied first, the host mirror is refreshed on the next getter, and an applied update
-  // between update() and marginalize() makes marginalize() refuse the queued tracks, as after aidedUpdate().
+  // between update() and marginalize() makes marginalize() refuse the queued tracks, as after aidedUpdate().  max_iter >= 2
+  // iterates the update (an iterated EKF: relinearise at the updated clone poses until max |delta_{i+1} - delta_i| <= tol, at
+  // most max_iter linearisations), for relocalisation after drift; the default is the single linearisation.
   msckf_b200_landmark_result landmarkUpdate(const std::vector<landmarkObservation>& obs, const FixedMatrix<double, 2, 2>* R = nullptr,
-                                            double chi2_obs = 0, std::vector<double>* gamma = nullptr, std::vector<int>* flag = nullptr) {
-    msckf_b200_landmarks lm;
+                                            double chi2_obs = 0, std::vector<double>* gamma = nullptr, std::vector<int>* flag = nullptr,
+                                            int max_iter = 1, double tol = 1e-10) {
+    msckf_b200_landmarks lm{};
     landmarkPack(obs, R, chi2_obs, gamma, flag, lm);
+    lm.max_iter = max_iter; lm.tol = tol;
     msckf_b200_landmark_result r = {};
     checkNumeric(msckf_b200_landmark_update(eng(), &lm, &r), "msckf_b200_landmark_update");
     landmarkAbsorb(r);
@@ -990,11 +994,13 @@ class MSCKFBatch {
   }
   // MSCKF::landmarkUpdate of every filter (obs[i] empty: filter i is left alone) as one msckf_b200_batch_landmark_update: three
   // launches per 32 updated filters and one synchronisation.  gamma / flag (optional) receive one list per filter.  An unknown
-  // state_id throws before any device call.  result[i] of a filter left alone is value-initialised.
+  // state_id throws before any device call.  result[i] of a filter left alone is value-initialised.  max_iter / tol: the
+  // iterated update of MSCKF::landmarkUpdate for every updated filter (still one synchronisation).
   std::vector<msckf_b200_landmark_result> landmarkUpdate(const std::vector<std::vector<landmarkObservation>>& obs,
                                                          const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
                                                          std::vector<std::vector<double>>* gamma = nullptr,
-                                                         std::vector<std::vector<int>>* flag = nullptr) {
+                                                         std::vector<std::vector<int>>* flag = nullptr, int max_iter = 1,
+                                                         double tol = 1e-10) {
     const size_t n = size();
     if (obs.size() != n) throw std::invalid_argument("MSCKFBatch::landmarkUpdate: one observation list per filter");
     if (gamma) gamma->assign(n, std::vector<double>());
@@ -1003,6 +1009,7 @@ class MSCKFBatch {
     for (size_t i = 0; i < n; ++i)
       if (!obs[i].empty())
         filters_[i]->landmarkPack(obs[i], R, chi2_obs, gamma ? &(*gamma)[i] : nullptr, flag ? &(*flag)[i] : nullptr, lm[i]);
+    for (size_t i = 0; i < n; ++i) { lm[i].max_iter = max_iter; lm[i].tol = tol; }
     flushImu();
     std::vector<msckf_b200_landmark_result> r(n, msckf_b200_landmark_result());
     const int rc = msckf_b200_batch_landmark_update(batch_, lm.data(), r.data());

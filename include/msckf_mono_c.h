@@ -96,6 +96,13 @@ int msckf_mono_landmark_update(void* h, int n_obs, const int* state_ids, const d
                                double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out);
 int msckf_mono_batch_landmark_update(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
                                      const double* R3, double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out);
+/* the same, iterated: at most max_iter (0 .. 16) linearisations, converged when max |delta_{i+1} - delta_i| <= tol
+ * (MSCKF::landmarkUpdate's max_iter / tol; max_iter 0 or 1 is the calls above) */
+int msckf_mono_landmark_update_iter(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
+                                    double chi2_obs, int max_iter, double tol, double* gamma, int* flag, msckf_b200_landmark_result* out);
+int msckf_mono_batch_landmark_update_iter(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
+                                          const double* R3, double chi2_obs, int max_iter, double tol, double* gamma, int* flag,
+                                          msckf_b200_landmark_result* out);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

@@ -90,12 +90,12 @@ def aid_items(items):
 
 class Landmarks(C.Structure):
     _fields_ = [("n_obs", C.c_int), ("clone", C.c_void_p), ("z", C.c_void_p), ("p_L_G", C.c_void_p), ("R", C.c_void_p),
-                ("chi2_obs", C.c_double), ("gamma", C.c_void_p), ("flag", C.c_void_p)]
+                ("chi2_obs", C.c_double), ("gamma", C.c_void_p), ("flag", C.c_void_p), ("max_iter", C.c_int), ("tol", C.c_double)]
 
 
 class LandmarkResult(C.Structure):
     _fields_ = [("nis", C.c_double), ("dx_norm", C.c_double), ("dof", C.c_int), ("rows", C.c_int), ("used", C.c_int),
-                ("applied", C.c_int), ("status", C.c_int)]
+                ("applied", C.c_int), ("status", C.c_int), ("iterations", C.c_int), ("converged", C.c_int), ("step", C.c_double)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -104,7 +104,8 @@ class LandmarkResult(C.Structure):
 def landmark_struct(spec):
     """(Landmarks, the arrays it points into) of one call's mapped-landmark observations: spec = None (a batch member left
     alone) or a dict clone [n] (window positions), z [n, 2], p_L [n, 3], R (None: the filter's pixel noise, else 2 x 2 or
-    (uu, uv, vv)), chi2_obs.  The arrays are (clone, z, p_L, R, gamma [n] out, flag [n] out)."""
+    (uu, uv, vv)), chi2_obs, and optionally max_iter (0 or 1: one linearisation; up to 16: the iterated update) and tol.  The
+    arrays are (clone, z, p_L, R, gamma [n] out, flag [n] out)."""
     if spec is None or len(spec["clone"]) == 0:
         return Landmarks(0, None, None, None, None, 0.0, None, None), ()
     clone = np.ascontiguousarray(spec["clone"], dtype=np.int32).ravel()
@@ -117,7 +118,8 @@ def landmark_struct(spec):
     n = len(clone)
     gamma, flag = np.zeros(n), np.zeros(n, dtype=np.int32)
     a = Landmarks(n, clone.ctypes.data, z.ctypes.data, p.ctypes.data, None if R is None else R.ctypes.data,
-                  float(spec.get("chi2_obs", 0.0)), gamma.ctypes.data, flag.ctypes.data)
+                  float(spec.get("chi2_obs", 0.0)), gamma.ctypes.data, flag.ctypes.data, int(spec.get("max_iter", 0)),
+                  float(spec.get("tol", 0.0)))
     return a, (clone, z, p, R, gamma, flag)
 
 
@@ -313,12 +315,14 @@ class Batch:
         check(lib().msckf_b200_batch_aid_stack_update(self.h, ptrs, cnt, C.c_double(chi2_max), out), "msckf_b200_batch_aid_stack_update")
         return [o.as_dict() if s else None for s, o in zip(stacks, out)]
 
-    def landmark_update(self, specs):
+    def landmark_update(self, specs, max_iter=None, tol=None):
         """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
-        i alone); a list of result dicts with "gamma" and "flag" arrays (None for an engine left alone)"""
+        i alone); max_iter / tol, when given, apply to every spec that does not set its own.  A list of result dicts with
+        "gamma" and "flag" arrays (None for an engine left alone)"""
         n = len(self.engines)
         assert len(specs) == n
-        st = [landmark_struct(s) for s in specs]
+        extra = {k: v for k, v in (("max_iter", max_iter), ("tol", tol)) if v is not None}
+        st = [landmark_struct(s if s is None else dict(extra, **s)) for s in specs]
         out = (LandmarkResult * n)()
         check(lib().msckf_b200_batch_landmark_update(self.h, (Landmarks * n)(*[a for a, _ in st]), out),
               "msckf_b200_batch_landmark_update")
@@ -467,10 +471,11 @@ class Engine:
               "msckf_b200_aid_stack_update")
         return out.as_dict()
 
-    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0):
+    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0):
         """msckf_b200_landmark_update: observations of known landmarks p_L [n, 3] at z [n, 2] from window positions clone [n];
-        the result as a dict with the per-observation "gamma" and "flag" arrays"""
-        a, keep = landmark_struct({"clone": clone, "z": z, "p_L": p_L, "R": R, "chi2_obs": chi2_obs})
+        max_iter >= 2 iterates the update (at most max_iter linearisations, converged at max |delta_{i+1} - delta_i| <= tol).
+        The result as a dict with the per-observation "gamma" and "flag" arrays"""
+        a, keep = landmark_struct({"clone": clone, "z": z, "p_L": p_L, "R": R, "chi2_obs": chi2_obs, "max_iter": max_iter, "tol": tol})
         out = LandmarkResult()
         check(lib().msckf_b200_landmark_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_landmark_update")
         return dict(out.as_dict(), gamma=keep[4] if keep else np.zeros(0), flag=keep[5] if keep else np.zeros(0, np.int32))

@@ -1592,16 +1592,20 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
 // Mapped-landmark updates: every member with observations sends its observations (grouped by clone in window order, input
 // order kept inside a clone) and its clone table in the I/O block with one host-to-device copy; results, gamma and flags come
 // back with one copy and one synchronisation.  Three launches per per_member chunk of such members (k_lmk_clone, k_lmk_gain,
-// k_lmk_downdate; NM = 1 with one member in the context), whatever the observations turn out to be.  Nothing is launched
-// unless every member is valid.
-static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_result, status),
-              "mb::LmkOut must start like msckf_b200_landmark_result");
+// k_lmk_downdate; NM = 1 with one member in the context), whatever the observations turn out to be; a chunk whose largest
+// max_iter K is >= 2 launches (k_lmk_step, k_lmk_clone<..., true>, k_lmk_gain<..., true>) K - 1 times between the gain and the
+// downdate, with no host synchronisation in between.  Nothing is launched unless every member is valid.
+static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_result, status) &&
+                  offsetof(mb::LmkOut, iterations) == offsetof(msckf_b200_landmark_result, iterations) &&
+                  offsetof(mb::LmkOut, converged) == offsetof(msckf_b200_landmark_result, converged) &&
+                  offsetof(mb::LmkOut, step) == offsetof(msckf_b200_landmark_result, step),
+              "mb::LmkOut must have msckf_b200_landmark_result's fields at their offsets");
 template <class S>
 int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "landmark_update: null argument");
   RC(members_ready("landmark_update"));
   const int nf = (int)eng.size();
-  struct LmkPlan { std::vector<int> perm, grp; int G = 0, ld = 0; size_t in_off = 0, res_off = 0, ws_off = 0; };
+  struct LmkPlan { std::vector<int> perm, grp; int G = 0, ld = 0; size_t in_off = 0, res_off = 0, ws_off = 0, it_off = 0; };
   std::vector<LmkPlan> pl(nf);
   std::vector<int> idx;
   size_t in_bytes = 0, res_bytes = 0, ws_bytes = 0;
@@ -1609,6 +1613,8 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
     const msckf_b200_landmarks& q = in[i];
     const std::string who = " (member " + std::to_string(i) + ")";
     if (q.n_obs < 0 || q.n_obs > mb::kLmkMaxObs) return fail(MSCKF_B200_ERR_ARG, "landmark_update: n_obs outside 0 .. 4096" + who);
+    if (q.max_iter < 0 || q.max_iter > mb::kLmkMaxIter) return fail(MSCKF_B200_ERR_ARG, "landmark_update: max_iter outside 0 .. 16" + who);
+    if (!std::isfinite(q.tol) || q.tol < 0.0) return fail(MSCKF_B200_ERR_ARG, "landmark_update: tol is not finite and >= 0" + who);
     if (q.n_obs == 0) continue;
     const int M = eng[i]->M, n = 15 + 6 * M, no = q.n_obs;
     if (!q.clone || !q.z || !q.p_L_G) return fail(MSCKF_B200_ERR_ARG, "landmark_update: missing clone, z or p_L_G" + who);
@@ -1636,6 +1642,10 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
     res_bytes += up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no) + up16(sizeof(int) * (size_t)no);
     p.ws_off = ws_bytes;
     ws_bytes += up256(sizeof(double) * ((size_t)mb::kLmkSlot * p.G + (size_t)(p.ld + n + 1) * p.ld + n) + sizeof(mb::LmkCtl));
+    if (q.max_iter > 1) {  // the iterate table, delta_i and the iteration's control words
+      p.it_off = ws_bytes;
+      ws_bytes += up256(sizeof(double) * (7 * (size_t)M + n) + sizeof(mb::LmkIt));
+    }
     idx.push_back(i);
   }
   if (idx.empty()) return 0;
@@ -1643,7 +1653,7 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
   CK(cudaSetDevice(device));
   RC(io.ensure(res_base + res_bytes, stream));
   RC(ws.ensure(ws_bytes, stream));
-  std::vector<mb::LmkArgs<S>> args(nf);
+  std::vector<mb::LmkItArgs<S>> args(nf);
   for (int i : idx) {
     const msckf_b200_landmarks& q = in[i];
     const LmkPlan& p = pl[i];
@@ -1656,7 +1666,15 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
     }
     const size_t goff = p.in_off + up16(sizeof(double) * 5 * (size_t)no);
     memcpy(io.h + goff, p.grp.data(), sizeof(int) * p.grp.size());
-    mb::LmkArgs<S> a = eng[i]->lmk_args(q, p.G, p.ld);
+    mb::LmkItArgs<S> a;
+    static_cast<mb::LmkArgs<S>&>(a) = eng[i]->lmk_args(q, p.G, p.ld);
+    a.max_iter = q.max_iter; a.tol = q.tol;
+    a.xi = nullptr; a.d = nullptr; a.it = nullptr;
+    if (q.max_iter > 1) {
+      a.xi = reinterpret_cast<double*>(ws.d + p.it_off);
+      a.d = a.xi + 7 * (size_t)eng[i]->M;
+      a.it = reinterpret_cast<mb::LmkIt*>(a.d + n);
+    }
     a.obs = reinterpret_cast<const double*>(io.d + p.in_off);
     a.grp = reinterpret_cast<const int*>(io.d + goff);
     unsigned char* r = io.d + res_base + p.res_off;
@@ -1673,14 +1691,23 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
   CK(cudaMemcpyAsync(io.d, io.h, in_bytes, cudaMemcpyHostToDevice, stream));
   per_member(idx, false, [&](int i) { return args[i]; },
              [&](const auto& a, int nm) {
-               int gx = 1, tx = 1;  // the largest member's grid; other members' CTAs past their own range exit at once
+               constexpr int NM = (int)std::extent<decltype(std::decay_t<decltype(a)>::m)>::value;
+               mb::Members<mb::LmkArgs<S>, NM> b;  // the single linearisation's arguments, as they always were
+               int gx = 1, tx = 1, K = 1;  // the largest member's grid; other members' CTAs past their own range exit at once
                for (int j = 0; j < nm; ++j) {
+                 b.m[j] = a.m[j];
                  gx = std::max(gx, a.m[j].G);
                  tx = std::max(tx, a.m[j].ntiles);
+                 K = std::max(K, a.m[j].max_iter);
                }
-               mb::k_lmk_clone<<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
-               mb::k_lmk_gain<<<nm, mb::kLmkThreads, 0, stream>>>(a);
-               mb::k_lmk_downdate<<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(a);
+               mb::k_lmk_clone<S, NM><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(b);
+               mb::k_lmk_gain<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(b);
+               for (int it = 0; it + 1 < K; ++it) {
+                 mb::k_lmk_step<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(a, it);
+                 mb::k_lmk_clone<S, NM, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
+                 mb::k_lmk_gain<S, NM, true><<<nm, mb::kLmkThreads, 0, stream>>>(a);
+               }
+               mb::k_lmk_downdate<S, NM><<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(b);
              });
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(io.h + res_base, io.d + res_base, res_bytes, cudaMemcpyDeviceToHost, stream));
@@ -1695,6 +1722,11 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
     const int* fl = reinterpret_cast<const int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)q.n_obs));
     out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].rows = o.rows; out[i].used = o.used;
     out[i].applied = o.applied; out[i].status = o.status;
+    if (q.max_iter > 1) {
+      out[i].iterations = o.iterations; out[i].converged = o.converged; out[i].step = o.step;
+    } else {
+      out[i].iterations = o.applied; out[i].converged = 0; out[i].step = 0.0;
+    }
     for (int j = 0; j < q.n_obs; ++j) {
       if (q.gamma) q.gamma[p.perm[j]] = g[j];
       if (q.flag) q.flag[p.perm[j]] = fl[j];
@@ -1918,7 +1950,8 @@ int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item*
 }
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
-  if (lm->n_obs == 0) { memset(out, 0, sizeof(*out)); return 0; }
+  const bool it_ok = lm->max_iter >= 0 && lm->max_iter <= mb::kLmkMaxIter && std::isfinite(lm->tol) && lm->tol >= 0.0;
+  if (lm->n_obs == 0 && it_ok) { memset(out, 0, sizeof(*out)); return 0; }
   return e->impl->solo_ctx()->landmarks(lm, out);
 }
 int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->impl->set_covariance(in); }

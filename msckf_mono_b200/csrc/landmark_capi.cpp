@@ -1,5 +1,5 @@
 // msckf_mono_b200/csrc/landmark_capi.cpp -- mapped-landmark updates in the C view (include/msckf_mono_c.h,
-// msckf_mono_landmark_update / msckf_mono_batch_landmark_update): MSCKF<_S>::landmarkUpdate and MSCKFBatch<_S>::landmarkUpdate
+// msckf_mono_landmark_update / msckf_mono_batch_landmark_update and their _iter forms): MSCKF<_S>::landmarkUpdate and MSCKFBatch<_S>::landmarkUpdate
 // over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own translation unit, so that the other view
 // files link against a C-ABI without msckf_b200_landmark_update / msckf_b200_batch_landmark_update.
 #include <stdexcept>
@@ -29,7 +29,8 @@ FixedMatrix<double, 2, 2> noise(const double* R3) {
 }
 template <class S>
 void batch_landmarks(MSCKFBatch<S>& b, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
-                     const double* R3, double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out) {
+                     const double* R3, double chi2_obs, int max_iter, double tol, double* gamma, int* flag,
+                     msckf_b200_landmark_result* out) {
   const size_t nf = b.size();
   std::vector<std::vector<landmarkObservation>> obs(nf);
   size_t o = 0;
@@ -40,7 +41,7 @@ void batch_landmarks(MSCKFBatch<S>& b, const int* n_obs, const int* state_ids, c
   const FixedMatrix<double, 2, 2> R = R3 ? noise(R3) : FixedMatrix<double, 2, 2>();
   std::vector<std::vector<double>> g;
   std::vector<std::vector<int>> fl;
-  const std::vector<msckf_b200_landmark_result> r = b.landmarkUpdate(obs, R3 ? &R : nullptr, chi2_obs, &g, &fl);
+  const std::vector<msckf_b200_landmark_result> r = b.landmarkUpdate(obs, R3 ? &R : nullptr, chi2_obs, &g, &fl, max_iter, tol);
   o = 0;
   for (size_t i = 0; i < nf; ++i) {
     if (n_obs[i] > 0) {
@@ -53,11 +54,8 @@ void batch_landmarks(MSCKFBatch<S>& b, const int* n_obs, const int* state_ids, c
     o += n_obs[i];
   }
 }
-}  // namespace
-
-extern "C" {
-int msckf_mono_landmark_update(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
-                               double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out) {
+int single_landmarks(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
+                     double chi2_obs, int max_iter, double tol, double* gamma, int* flag, msckf_b200_landmark_result* out) {
   return guard([&] {
     if (!h || !out) throw std::invalid_argument("landmark_update: null argument");
     const std::vector<landmarkObservation> obs = observations(n_obs, state_ids, z, p_L_G);
@@ -65,8 +63,10 @@ int msckf_mono_landmark_update(void* h, int n_obs, const int* state_ids, const d
     std::vector<double> g;
     std::vector<int> fl;
     Base* b = static_cast<Base*>(h);
-    if (b->dtype == 0) *out = static_cast<MSCKF<float>*>(b->filter_ptr())->landmarkUpdate(obs, R3 ? &R : nullptr, chi2_obs, &g, &fl);
-    else *out = static_cast<MSCKF<double>*>(b->filter_ptr())->landmarkUpdate(obs, R3 ? &R : nullptr, chi2_obs, &g, &fl);
+    if (b->dtype == 0)
+      *out = static_cast<MSCKF<float>*>(b->filter_ptr())->landmarkUpdate(obs, R3 ? &R : nullptr, chi2_obs, &g, &fl, max_iter, tol);
+    else
+      *out = static_cast<MSCKF<double>*>(b->filter_ptr())->landmarkUpdate(obs, R3 ? &R : nullptr, chi2_obs, &g, &fl, max_iter, tol);
     for (int i = 0; i < n_obs; ++i) {
       if (gamma) gamma[i] = g[i];
       if (flag) flag[i] = fl[i];
@@ -74,14 +74,34 @@ int msckf_mono_landmark_update(void* h, int n_obs, const int* state_ids, const d
     return 0;
   });
 }
-int msckf_mono_batch_landmark_update(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
-                                     const double* R3, double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out) {
+int many_landmarks(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
+                   double chi2_obs, int max_iter, double tol, double* gamma, int* flag, msckf_b200_landmark_result* out) {
   return guard([&] {
     if (!batch || !n_obs || !out) throw std::invalid_argument("batch_landmark_update: null argument");
     auto* vb = static_cast<ViewBatch*>(batch);
-    if (vb->bf) batch_landmarks(*vb->bf, n_obs, state_ids, z, p_L_G, R3, chi2_obs, gamma, flag, out);
-    else batch_landmarks(*vb->bd, n_obs, state_ids, z, p_L_G, R3, chi2_obs, gamma, flag, out);
+    if (vb->bf) batch_landmarks(*vb->bf, n_obs, state_ids, z, p_L_G, R3, chi2_obs, max_iter, tol, gamma, flag, out);
+    else batch_landmarks(*vb->bd, n_obs, state_ids, z, p_L_G, R3, chi2_obs, max_iter, tol, gamma, flag, out);
     return 0;
   });
+}
+}  // namespace
+
+extern "C" {
+int msckf_mono_landmark_update(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
+                               double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out) {
+  return single_landmarks(h, n_obs, state_ids, z, p_L_G, R3, chi2_obs, 1, 1e-10, gamma, flag, out);
+}
+int msckf_mono_batch_landmark_update(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
+                                     const double* R3, double chi2_obs, double* gamma, int* flag, msckf_b200_landmark_result* out) {
+  return many_landmarks(batch, n_obs, state_ids, z, p_L_G, R3, chi2_obs, 1, 1e-10, gamma, flag, out);
+}
+int msckf_mono_landmark_update_iter(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G, const double* R3,
+                                    double chi2_obs, int max_iter, double tol, double* gamma, int* flag, msckf_b200_landmark_result* out) {
+  return single_landmarks(h, n_obs, state_ids, z, p_L_G, R3, chi2_obs, max_iter, tol, gamma, flag, out);
+}
+int msckf_mono_batch_landmark_update_iter(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
+                                          const double* R3, double chi2_obs, int max_iter, double tol, double* gamma, int* flag,
+                                          msckf_b200_landmark_result* out) {
+  return many_landmarks(batch, n_obs, state_ids, z, p_L_G, R3, chi2_obs, max_iter, tol, gamma, flag, out);
 }
 }

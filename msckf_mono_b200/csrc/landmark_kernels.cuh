@@ -12,25 +12,34 @@
 //                    NIS = |y|^2 + sum_k e_k^2 (the NIS of the dense stacked system).
 //   k_lmk_downdate : 32 x 32 tiles of the lower triangle of P - W^T W (fp64, rounded once, both halves written, in place) and
 //                    dx = W^T y on the diagonal tiles; the last tile of a member (ticket counter) runs the state injection.
+// Iterated form (max_iter >= 2, an IEKF): after k_lmk_gain, k_lmk_step forms delta_{i+1} = W^T y and the iterate clone poses
+// x^ [+] delta_{i+1} (fp64); k_lmk_clone<..., true> relinearises there with linearisation 0's flags, adding X~ e_k (e_k: delta_i of
+// clone k) to the whitened residual, and k_lmk_gain<..., true> refactors against the same prior P without touching the NIS.
+// k_lmk_downdate then applies the last W, y.  P and the resident state are not written before the downdate.
 // One body for a single filter (NM = 1) and a device batch (NM = kBatchMembers), like k_aid.  Each member's arithmetic depends
 // only on its own inputs: a batch equals single calls bit for bit.
 #pragma once
 #include "common.cuh"
 #include "state_kernels.cuh"
 
+#include <type_traits>
+
 namespace mb {
 
 constexpr int kLmkMaxPerClone = 256;  // observations of one clone in one call (2 x 256 rows of 7 doubles in shared memory)
 constexpr int kLmkMaxObs = 4096;      // observations of one member in one call
+constexpr int kLmkMaxIter = 16;       // linearisations of the iterated form
 constexpr int kLmkThreads = 256;
 constexpr int kLmkSlot = 48;          // doubles per touched clone: T [6][6], rho [6], e^2, used, q
 constexpr int kLmkNB = 32;            // panel width of the blocked Cholesky and tile size of the downdate
 
-// per-member result; the first seven fields are msckf_b200_landmark_result's
+// per-member result; every field but numeric is msckf_b200_landmark_result's, at its offset
 struct LmkOut {
   double nis, dx_norm;
   int dof, rows, used, applied, status;
-  int numeric;  // a non-finite dx or P entry was written
+  int iterations, converged;  // written by the iterated form only (the host fills them for max_iter <= 1)
+  int numeric;                // a non-finite dx or P entry was written
+  double step;
 };
 // per-member control words in the workspace (k_lmk_gain -> k_lmk_downdate)
 struct LmkCtl {
@@ -57,6 +66,28 @@ struct LmkArgs {
   int ldp, M, G, ld, ntiles, use_R;
 };
 static_assert(sizeof(Members<LmkArgs<double>, kBatchMembers>) <= 32764, "the landmark kernels' batched arguments exceed the parameter limit");
+
+// the iterated form's per-member control words (k_lmk_step writes them at its first launch of a call)
+struct alignas(8) LmkIt {
+  int done;  // converged, stopped or out of iterations: every later iteration kernel returns at once
+  int stop;  // a used observation is behind the camera or not finite at the iterate (k_lmk_clone<..., true>)
+};
+// done or stop, in one load (two loads of the words cost k_lmk_gain<..., 32, true> an 8-byte spill)
+__device__ __forceinline__ bool lmk_it_ended(const LmkIt* ic) {
+  const int2 w = __ldcg(reinterpret_cast<const int2*>(ic));
+  return (w.x | w.y) != 0;
+}
+template <class S>
+struct LmkItArgs : LmkArgs<S> {
+  double* xi;    // [M][7] iterate clone poses x^ [+] delta_i: q (x, y, z, w), p_C_G
+  double* d;     // [n] delta_i
+  LmkIt* it;
+  double tol;    // stop when max |delta_{i+1} - delta_i| <= tol
+  int max_iter;  // linearisations; <= 1: the member does not iterate and every iteration kernel returns at once
+};
+static_assert(sizeof(Members<LmkItArgs<double>, kBatchMembers>) <= 32764, "the iterated landmark kernels' arguments exceed the parameter limit");
+template <class S, bool IT>
+using LmkArgsT = std::conditional_t<IT, LmkItArgs<S>, LmkArgs<S>>;
 
 __host__ __device__ constexpr int lmk_tiles(int n) { return ((n + kLmkNB - 1) / kLmkNB) * ((n + kLmkNB - 1) / kLmkNB + 1) / 2; }
 
@@ -94,9 +125,14 @@ __device__ __forceinline__ double lmk_obs(const double* o, const double* Cr, con
   return gam;
 }
 
-template <class S, int NM>
-__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs<S>, NM> a) {
+// IT: the iterate form.  The clone pose comes from the iterate table, the flags are linearisation 0's (gamma and flag are not
+// written), X~ e_k is added to the whitened residual, and a used observation that fails at the iterate raises the stop word.
+template <class S, int NM, bool IT = false>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgsT<S, IT>, NM> a) {
   const int f = NM == 1 ? 0 : blockIdx.y, g = blockIdx.x;
+  if constexpr (IT) {
+    if (a.m[f].max_iter <= 1 || lmk_it_ended(a.m[f].it)) return;
+  }
   if (g >= a.m[f].G) return;
   const S* __restrict__ const P = a.m[f].P;
   const int ldp = a.m[f].ldp, t = threadIdx.x, lane = t & 31;
@@ -106,13 +142,23 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   __shared__ double Q[2 * kLmkMaxPerClone][7];  // used rows [X~ | r~], input order, then R and the Householder vectors
   __shared__ double Pk[6][6], Cr[9], pc[3], LR[3], Rm[3];
   __shared__ int fl[kLmkMaxPerClone], pos[kLmkMaxPerClone], s_used;
+  __shared__ double ek[IT ? 6 : 1];
 
   if (t < 36) Pk[t / 6][t % 6] = (double)P[(size_t)(15 + 6 * k + t / 6) * ldp + 15 + 6 * k + t % 6];
+  if constexpr (IT) {
+    if (t >= 64 && t < 70) ek[t - 64] = a.m[f].d[15 + 6 * k + t - 64];
+  }
   if (t == 0) {
-    const S* ps = a.m[f].poses + kPoseStride * k;
-    const double q[4] = {(double)ps[0], (double)ps[1], (double)ps[2], (double)ps[3]};
-    quat_to_rot(q, Cr);
-    pc[0] = (double)ps[4]; pc[1] = (double)ps[5]; pc[2] = (double)ps[6];
+    if constexpr (IT) {
+      const double* x = a.m[f].xi + 7 * k;
+      quat_to_rot(x, Cr);
+      pc[0] = x[4]; pc[1] = x[5]; pc[2] = x[6];
+    } else {
+      const S* ps = a.m[f].poses + kPoseStride * k;
+      const double q[4] = {(double)ps[0], (double)ps[1], (double)ps[2], (double)ps[3]};
+      quat_to_rot(q, Cr);
+      pc[0] = (double)ps[4]; pc[1] = (double)ps[5]; pc[2] = (double)ps[6];
+    }
     if (a.m[f].use_R) {
       Rm[0] = a.m[f].R[0]; Rm[1] = a.m[f].R[1]; Rm[2] = a.m[f].R[2];
     } else {
@@ -129,8 +175,14 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   int fg = 2;
   if (t < cnt) {
     const double gam = lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
-    a.m[f].gamma[i0 + t] = gam;
-    a.m[f].flag[i0 + t] = fg;
+    if constexpr (IT) {
+      const int f0 = a.m[f].flag[i0 + t];  // linearisation 0's
+      if (f0 == 0 && fg == 2) a.m[f].it->stop = 1;
+      fg = f0;
+    } else {
+      a.m[f].gamma[i0 + t] = gam;
+      a.m[f].flag[i0 + t] = fg;
+    }
     fl[t] = fg;
   }
   __syncthreads();
@@ -142,10 +194,19 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   __syncthreads();
   if (t < cnt && fg == 0) {
     lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
-    for (int c = 0; c < 7; ++c) {  // whiten: L_R^-1 [X | r]
-      const double y0 = row[0][c] / LR[0];
-      Q[2 * pos[t]][c] = y0;
-      Q[2 * pos[t] + 1][c] = (row[1][c] - LR[1] * y0) / LR[2];
+    if constexpr (IT) {  // whiten in place, then r~ + X~ e_k
+      for (int c = 0; c < 7; ++c) {
+        row[0][c] /= LR[0];
+        row[1][c] = (row[1][c] - LR[1] * row[0][c]) / LR[2];
+      }
+      for (int c = 0; c < 6; ++c) { row[0][6] += row[0][c] * ek[c]; row[1][6] += row[1][c] * ek[c]; }
+      for (int c = 0; c < 7; ++c) { Q[2 * pos[t]][c] = row[0][c]; Q[2 * pos[t] + 1][c] = row[1][c]; }
+    } else {
+      for (int c = 0; c < 7; ++c) {  // whiten: L_R^-1 [X | r]
+        const double y0 = row[0][c] / LR[0];
+        Q[2 * pos[t]][c] = y0;
+        Q[2 * pos[t] + 1][c] = (row[1][c] - LR[1] * y0) / LR[2];
+      }
     }
   }
   __syncthreads();
@@ -188,9 +249,14 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   }
 }
 
-template <class S, int NM>
-__global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgs<S>, NM> a) {
+// IT: the iterate form.  A raised stop word ends the iteration with nothing written (the previous W, y stay); otherwise the
+// factorisation is today's, and only apply, iterations and (S not positive definite) the status are written.
+template <class S, int NM, bool IT = false>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT<S, IT>, NM> a) {
   const int f = NM == 1 ? 0 : blockIdx.x;
+  if constexpr (IT) {
+    if (a.m[f].max_iter <= 1 || lmk_it_ended(a.m[f].it)) return;
+  }
   const S* __restrict__ const P = a.m[f].P;
   double* __restrict__ const A = a.m[f].A;
   const double* __restrict__ const slot = a.m[f].slot;
@@ -217,8 +283,8 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgs<
   for (int g = t; g < G; g += kLmkThreads) ck[g] = a.m[f].grp[3 * g];
   __syncthreads();
   const int m = off[G], Rt = m + n + 1;
-  if (s_used == 0) {  // no observation used: nothing is written
-    if (t == 0) {
+  if (s_used == 0) {  // no observation used: nothing is written (the iterate form never gets here: k_lmk_step stops it)
+    if (!IT && t == 0) {
       ctl->apply = 0;
       out->nis = 0.0; out->dx_norm = 0.0; out->dof = 0; out->rows = 0; out->used = 0; out->applied = 0; out->status = 0;
       out->numeric = 0;
@@ -306,6 +372,10 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgs<
       ctl->apply = 0;
       out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
       out->status = 1; out->applied = 0;
+      if constexpr (IT) out->iterations = 0;  // (k_lmk_step sees apply = 0 and ends the iteration)
+    } else if constexpr (IT) {  // linearisation 0's NIS, dof and counts stay
+      ctl->apply = 1;
+      out->iterations += 1;
     } else {
       const double* y = A + (size_t)(m + n) * ld;
       double g = s_e2;
@@ -313,7 +383,78 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgs<
       ctl->apply = 1;
       out->nis = g; out->status = 0; out->applied = 1;
     }
-    out->dof = 2 * s_used; out->rows = m; out->used = s_used; out->numeric = 0;
+    if constexpr (!IT) { out->dof = 2 * s_used; out->rows = m; out->used = s_used; out->numeric = 0; }
+  }
+}
+
+// One CTA per member, after linearisation `it` (0-based): delta_{i+1} = W^T y (the rows of dx in k_lmk_downdate, same order),
+// step = max |delta_{i+1} - delta_i| (NaN counts as infinite), then either the member is done (step <= tol: converged; or
+// max_iter linearisations made) or the iterate table x^ [+] delta_{i+1} is written for the next linearisation: q <-
+// normalise(buildUpdateQuat(dtheta_k) * q^), p <- p^ + dp_k in fp64 (inject_state's clone arithmetic on the widened poses).
+template <class S, int NM>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_step(const Members<LmkItArgs<S>, NM> a, int it) {
+  const int f = NM == 1 ? 0 : blockIdx.x;
+  if (a.m[f].max_iter <= 1) return;
+  LmkIt* const ic = a.m[f].it;
+  if (it > 0 && ic->done) return;
+  if (it + 1 >= a.m[f].max_iter) {  // the member's max_iter linearisations are made (a chunk with a larger max_iter goes on)
+    if (threadIdx.x == 0) ic->done = 1;
+    return;
+  }
+  const LmkCtl* const ctl = a.m[f].ctl;
+  LmkOut* const out = a.m[f].out;
+  const int t = threadIdx.x, lane = t & 31, ld = a.m[f].ld, M = a.m[f].M, n = 15 + 6 * M;
+  __shared__ double red[kLmkThreads / 32];
+  __shared__ int s_go;
+  if (it > 0 && (ic->stop || !ctl->apply)) {  // stopped at the last iterate, or S was not positive definite there
+    if (t == 0) ic->done = 1;
+    return;
+  }
+  if (it == 0) {  // the call's first step: reset the control words
+    const int ap = ctl->apply;
+    if (t == 0) {
+      ic->stop = 0; ic->done = !ap;
+      out->iterations = ap; out->converged = 0; out->step = 0.0;
+    }
+    if (!ap) return;
+  }
+  const int m = ctl->m;
+  const double* __restrict__ const Wt = a.m[f].A + (size_t)m * ld;
+  const double* __restrict__ const y = a.m[f].A + (size_t)(m + n) * ld;
+  double* const d = a.m[f].d;
+  double c = 0.0;
+  for (int r = t; r < n; r += kLmkThreads) {
+    const double* w = Wt + (size_t)r * ld;
+    double v = 0.0;
+    for (int p = 0; p < m; ++p) v += w[p] * y[p];
+    const double dc = fabs(v - (it == 0 ? 0.0 : d[r]));
+    c = fmax(c, isnan(dc) ? __longlong_as_double(0x7ff0000000000000ll) : dc);
+    d[r] = v;
+  }
+  for (int o = 16; o > 0; o >>= 1) c = fmax(c, __shfl_xor_sync(0xffffffffu, c, o));
+  if (lane == 0) red[t >> 5] = c;
+  __syncthreads();
+  if (t == 0) {
+    double s = red[0];
+    for (int w = 1; w < kLmkThreads / 32; ++w) s = fmax(s, red[w]);
+    const int conv = s <= a.m[f].tol, go = !conv && it + 2 <= a.m[f].max_iter;
+    out->step = s; out->converged = conv;
+    if (!go) ic->done = 1;
+    s_go = go;
+  }
+  __syncthreads();
+  if (!s_go) return;
+  for (int k = t; k < M; k += kLmkThreads) {
+    const S* ps = a.m[f].poses + kPoseStride * k;
+    const double q[4] = {(double)ps[0], (double)ps[1], (double)ps[2], (double)ps[3]};
+    const double dth[3] = {d[15 + 6 * k], d[16 + 6 * k], d[17 + 6 * k]};
+    double uq[4], qn[4];
+    build_update_quat(dth, uq);
+    quat_mul(uq, q, qn);
+    quat_normalize(qn);
+    double* x = a.m[f].xi + 7 * k;
+    x[0] = qn[0]; x[1] = qn[1]; x[2] = qn[2]; x[3] = qn[3];
+    x[4] = (double)ps[4] + d[18 + 6 * k]; x[5] = (double)ps[5] + d[19 + 6 * k]; x[6] = (double)ps[6] + d[20 + 6 * k];
   }
 }
 

@@ -146,9 +146,10 @@ class FilterBatch:
         self._call("aid_stack_update", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), out)
         return [o.as_dict() if s else None for s, o in zip(stacks, out)]
 
-    def landmark_update(self, obs, R=None, chi2_obs=0.0):
+    def landmark_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
         """MSCKFBatch::landmarkUpdate: obs[i] = (state_ids [n], z [n, 2], p_L [n, 3]) for filter i, or None (filter i left
-        alone); R None (each filter's pixel noise) or 2 x 2; one device call for the batch.  A list of result dicts with
+        alone); R None (each filter's pixel noise) or 2 x 2; one device call for the batch; max_iter >= 2: the iterated update
+        (at most max_iter linearisations, converged at max |delta_{i+1} - delta_i| <= tol).  A list of result dicts with
         "gamma" and "flag" (None for a filter left alone)."""
         from .capi import LandmarkResult
         n = len(self.filters)
@@ -162,9 +163,10 @@ class FilterBatch:
         tot = max(int(cnt.sum()), 1)
         gamma, flag = np.zeros(tot), np.zeros(tot, dtype=np.int32)
         out = (LandmarkResult * n)()
-        self._call("landmark_update", cnt.ctypes.data_as(_ip), ids.ctypes.data_as(_ip), z.ctypes.data_as(_dp), p.ctypes.data_as(_dp),
-                   None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs), gamma.ctypes.data_as(_dp),
-                   flag.ctypes.data_as(_ip), out)
+        it = () if max_iter == 1 else (C.c_int(int(max_iter)), C.c_double(tol))
+        self._call("landmark_update" + ("_iter" if it else ""), cnt.ctypes.data_as(_ip), ids.ctypes.data_as(_ip),
+                   z.ctypes.data_as(_dp), p.ctypes.data_as(_dp), None if r3 is None else r3.ctypes.data_as(_dp),
+                   C.c_double(chi2_obs), *it, gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip), out)
         res, o0 = [], 0
         for i in range(n):
             c = int(cnt[i])
@@ -374,10 +376,11 @@ class CFilter:
                                                   C.c_double(chi2_max), C.byref(out)), "relative_pose_update")
         return out.as_dict()
 
-    def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0):
+    def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
         """MSCKF::landmarkUpdate (include/msckf_b200.h: msckf_b200_landmark_update): observations of known landmarks p_L [n, 3]
         at z [n, 2] from the images state_ids [n]; R None (the filter's pixel noise) or 2 x 2; chi2_obs > 0: per-observation
-        gate.  A dict nis, dx_norm, dof, rows, used, applied, status, gamma [n], flag [n]."""
+        gate; max_iter >= 2: the iterated update.  A dict nis, dx_norm, dof, rows, used, applied, status, iterations,
+        converged, step, gamma [n], flag [n]."""
         from .capi import LandmarkResult
         ids = np.ascontiguousarray(state_ids, dtype=np.int32).ravel()
         n = len(ids)
@@ -386,9 +389,11 @@ class CFilter:
         r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
         gamma, flag = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int32)
         out = LandmarkResult()
-        self._chk(self._f("landmark_update")(self.h, C.c_int(n), ids.ctypes.data_as(_ip), pz, pp,
-                                             None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs),
-                                             gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip), C.byref(out)), "landmark_update")
+        it = () if max_iter == 1 else (C.c_int(int(max_iter)), C.c_double(tol))
+        name = "landmark_update" + ("_iter" if it else "")
+        self._chk(self._f(name)(self.h, C.c_int(n), ids.ctypes.data_as(_ip), pz, pp,
+                                None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs), *it,
+                                gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip), C.byref(out)), name)
         return dict(out.as_dict(), gamma=gamma[:n].copy(), flag=flag[:n].copy())
 
     # ---- test hooks --------------------------------------------------------------------

@@ -221,10 +221,11 @@ def map_observations(truth, frame, stride):
     return idx, np.stack([xn[idx], yn[idx]], axis=1)
 
 
-def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0):
+def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0, map_start=0):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
     fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
-    map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks.  With
+    map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks, None
+    before frame map_start (the map noise of those frames is still drawn, so a frame's map is the same for every map_start).  With
     odo_every > 0, "odometry" holds per frame None or the 9 standard normals of that frame's odometry noise (odometry_items)."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
@@ -268,7 +269,8 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
                 out["maps"].append(None)
                 continue
             idx, z = map_observations(truth, f, map_stride)
-            out["maps"].append((idx, truth["landmarks"][::map_stride][idx], z + mrng.standard_normal(z.shape) * np.array([su, sv])))
+            z = z + mrng.standard_normal(z.shape) * np.array([su, sv])
+            out["maps"].append((idx, truth["landmarks"][::map_stride][idx], z) if f >= map_start else None)
     if odo_every > 0:
         orng = np.random.default_rng([seed, k, 3])
         out["odometry"] = [orng.standard_normal(9) if (f + 1) % odo_every == 0 else None for f in range(len(truth["frames"]))]
@@ -283,10 +285,18 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=()):
+def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None):
     """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes, of its
     map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n) and of its odometry
-    stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists"""
+    stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists; map_first (a dict of plain numbers: frame,
+    squared position error before and after, nis, dof, iterations, converged) describes the first map update"""
+    rec = _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows)
+    if map_first is not None:
+        rec["map_first"] = dict(map_first)
+    return rec
+
+
+def _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows):
     return {"nees": {c: [float(r[c]) for r in nees_rows] for c in COMPONENTS},
             "dim": {c: [int(r["dim_full"]) if c == "full" else DOF[c] for r in nees_rows] for c in COMPONENTS},
             "first_bad_pivot": [int(r["first_bad_pivot"]) for r in nees_rows],
@@ -348,6 +358,18 @@ def summarize(records):
                       "run_bounds": list(tot), "updates_inside": float(np.mean(inside)),
                       "applied": float(np.mean([a for m in mp for a in m["applied"]])),
                       "observations": int(n_obs), "gated": float(1.0 - sum(sum(m["used"]) for m in mp) / max(n_obs, 1))}
+    mf = [records[k].get("map_first") for k in keys]
+    if all(m is not None for m in mf):  # the first map update: position error before / after, its ANIS, the IMU-state ANEES after
+        f0 = mf[0]["frame"]
+        d = int(sum(m["dof"] for m in mf))
+        imu = out["components"]["imu"]
+        out["map_first"] = {"frame": int(f0), "pos_rmse_before": float(np.sqrt(np.mean([m["pos_err2_before"] for m in mf]))),
+                            "pos_rmse_after": float(np.sqrt(np.mean([m["pos_err2_after"] for m in mf]))),
+                            "anis": float(sum(m["nis"] for m in mf) / N), "mean_dof": d / N,
+                            "bounds": list(chi2_bounds(d, N)) if d > 0 else [float("nan")] * 2,
+                            "imu_anees": imu["anees"][f0], "imu_bounds": [imu["lower"][f0], imu["upper"][f0]],
+                            "iterations": float(np.mean([m["iterations"] for m in mf])),
+                            "converged": float(np.mean([m["converged"] for m in mf]))}
     od = [records[k].get("odometry") for k in keys]
     if all(o is not None and len(o["nis"]) for o in od):  # ANIS of the odometry stacks: the stack's rows per trial and update
         V = np.array([o["nis"] for o in od]); D = np.array([o["dof"] for o in od])
@@ -363,17 +385,20 @@ def summarize(records):
 
 # ---- the batched run ---------------------------------------------------------------------------------------------------------
 def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0,
-        odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False):
+        odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False, map_start=0, map_iterations=1):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
-    [every map_every frames one batched mapped-landmark update from the newest clone, gated per observation at map_chi2 > 0],
-    refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.
+    [every map_every frames from frame map_start on, one batched mapped-landmark update from the newest clone, gated per
+    observation at map_chi2 > 0, iterated up to map_iterations linearisations],
+    refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.  The first
+    map update is also recorded on its own (trial_record's map_first; the state is read just before it).
     Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
     from . import engine_filter
     from .capi import AID_POSITION
     from .cview import FilterBatch
-    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every) for k in trials]
+    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start) for k in trials]
+    first = [None for _ in trs]
     R_fix = (fix_sigma ** 2) * np.eye(3)
     nis = [[] for _ in trs]
     maps = [[] for _ in trs]
@@ -413,9 +438,15 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [(np.full(len(tr["maps"][fi][0]), fr["state_id"]), tr["maps"][fi][2], tr["maps"][fi][1]) if len(tr["maps"][fi][0]) else None
                    for tr, fr in zip(trs, frs)]
-            res = fb.landmark_update(obs, chi2_obs=map_chi2)
+            if first[0] is None:
+                fb.refreshState()
+                for i, (f, tr) in enumerate(zip(fs, trs)):
+                    first[i] = {"frame": fi, "pos_err2_before": float(np.sum((truth_imu_of(truth, tr, fi)[0:3] - f.getImuState()["p_I_G"]) ** 2))}
+            res = fb.landmark_update(obs, chi2_obs=map_chi2, max_iter=map_iterations)
             for i, r in enumerate(res):
                 maps[i].append({"nis": 0.0, "dof": 0, "used": 0, "applied": 0, "n": 0} if r is None else dict(r, n=len(r["flag"])))
+                if first[i]["frame"] == fi:
+                    first[i].update({k: (float if k == "nis" else int)(r[k]) if r is not None else 0 for k in ("nis", "dof", "iterations", "converged")})
         fb.refreshState()
         timu, tposes = [], []
         for i, (f, tr) in enumerate(zip(fs, trs)):
@@ -423,13 +454,15 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             timu.append(truth_imu_of(truth, tr, fi))
             tposes.append(truth["truth_pose"][ids])
             err2[i].append(float(np.sum((timu[-1][0:3] - f.getImuState()["p_I_G"]) ** 2)))
+            if first[i] is not None and first[i]["frame"] == fi:
+                first[i]["pos_err2_after"] = err2[i][-1]
         res = fb.nees(timu, tposes)
         for i, r in enumerate(res):
             rows[i].append(r)
         if on_frame is not None:
             on_frame(fi, fs, res)
     fb.close()
-    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i]) for i, tr in enumerate(trs)}
+    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i]) for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):
         s = f.getImuState()

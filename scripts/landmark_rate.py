@@ -3,8 +3,12 @@
 fp64 at 30 clones, for 1 / 8 / 32 filters and 25 / 100 / 400 observations spread over the newest 1 / 5 / 30 clones: host wall
 clock around the synchronising call, median of 20 after a warm-up.  For <= 16 observations on one filter it also times the path
 available without it: get_state, the projection linearised in numpy, then one aid_update(LINEAR).  Per-kernel device times
-(k_lmk_clone, k_lmk_gain, k_lmk_downdate) come from torch.profiler over repeated calls.  Reads the card's name and power limit
-in the same process.  Prints one JSON line."""
+(k_lmk_clone, k_lmk_gain, k_lmk_downdate) come from torch.profiler over repeated calls.  With --iterations K ..., it times the
+iterated update instead: 25 observations over the newest clone and 100 over the newest 5, seen from poses 0.3 m away, at each
+max_iter K with tol 0 (so every call makes its K linearisations unless a step is exactly zero), for 1 / 8 / 32 filters, with the
+linearisations the calls reported and the per-kernel split (k_lmk_step too) for 100 over 5.  Reads the card's name and power
+limit in the same process.  Prints one JSON line."""
+import argparse
 import json
 import subprocess
 import sys
@@ -53,10 +57,13 @@ def filters(n):
     return fs, es
 
 
-def observations(rng, e, n_obs, n_clones):
-    """n_obs observations spread evenly over the newest n_clones clones, landmarks 2 .. 8 m in front, measured exactly"""
+def observations(rng, e, n_obs, n_clones, offset=None):
+    """n_obs observations spread evenly over the newest n_clones clones, landmarks 2 .. 8 m in front, measured exactly (from
+    clone positions moved by `offset`, when given)"""
     _, poses = e.state()
     poses = poses.astype(np.float64)
+    if offset is not None:
+        poses[:, 0:3] += offset
     clone = np.array([M - 1 - (i % n_clones) for i in range(n_obs)], dtype=np.int32)
     d = rng.uniform(2.0, 8.0, n_obs)
     pc = np.stack([rng.uniform(-0.4, 0.4, n_obs) * d, rng.uniform(-0.3, 0.3, n_obs) * d, d], axis=1)
@@ -103,13 +110,49 @@ def kernel_times(fn, reps=50):
         torch.cuda.synchronize()
     out = {}
     for ev in prof.key_averages():
-        for name in ("k_lmk_clone", "k_lmk_gain", "k_lmk_downdate"):
+        for name in ("k_lmk_clone", "k_lmk_gain", "k_lmk_step", "k_lmk_downdate"):
             if name in ev.key:
                 out[name] = out.get(name, 0.0) + ev.device_time_total / 1e3 / reps  # ms per call
     return out
 
 
+def iterated(ks):
+    rng = np.random.default_rng(5)
+    res = {"gpu": gpu_line(), "dtype": "f64", "clones": M, "offset_m": 0.3, "tol": 0.0, "call_ms": {}, "iterations": {},
+           "kernel_ms": {}}
+    for nf in (1, 8, 32):
+        fs, es = filters(nf)
+        b = capi.Batch(es) if nf > 1 else None
+        for n_obs, nc in ((25, 1), (100, 5)):
+            specs = [observations(rng, e, n_obs, nc, offset=np.array([0.3, 0.0, 0.0])) for e in es]
+            for k in ks:
+                key = f"{nf}x{n_obs}obs/{nc}clones/max_iter{k}"
+                its = []
+                sp = [dict(s, max_iter=k, tol=0.0) for s in specs]
+
+                def fn():
+                    out = b.landmark_update(sp) if b else [es[0].landmark_update(**sp[0])]
+                    its.append(np.mean([o["iterations"] for o in out]))
+                res["call_ms"][key] = timed(fn)
+                res["iterations"][key] = float(np.mean(its))
+                if nf in (1, 32) and n_obs == 100:
+                    try:
+                        res["kernel_ms"][key] = kernel_times(fn)
+                    except Exception as ex:  # (the profiler is an extra; the call times above stand on their own)
+                        res["kernel_ms"][key] = f"not measured: {ex}"
+        if b:
+            b.close()
+        for f in fs:
+            f.close()
+    print(json.dumps(res), flush=True)
+
+
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iterations", type=int, nargs="*", default=None)
+    args = ap.parse_args()
+    if args.iterations:
+        return iterated(args.iterations)
     rng = np.random.default_rng(3)
     res = {"gpu": gpu_line(), "dtype": "f64", "clones": M, "call_ms": {}, "host_linear_ms": {}, "kernel_ms": {}}
     for nf in (1, 8, 32):

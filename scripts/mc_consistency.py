@@ -12,7 +12,9 @@ With --position-fix-every K, every K frames each trial also fuses a noisy positi
 
 With --map-every K, every K frames each trial also observes the map (every --map-stride-th landmark of the truth stream) from
 its newest clone and fuses the observations as mapped landmarks (after the prune and after a position fix), and the summary adds
-the map updates' ANIS against its 95 % chi^2 bounds and the fraction of observations gated out.
+the map updates' ANIS against its 95 % chi^2 bounds and the fraction of observations gated out.  --map-start F observes the map
+only from frame F on (relocalisation after drift), --map-iterations K iterates each map update (at most K linearisations), and
+the summary then adds the first map update: the position RMSE before and after it, its ANIS and the IMU-state ANEES after it.
 
 With --odometry-every K, every K frames each trial also fuses one stacked odometry update (the truth body velocity, and the
 truth relative pose of its two newest clones, each plus noise of --odometry-sigma-v m/s and --odometry-sigma-rel m / rad;
@@ -130,6 +132,8 @@ def main():
     ap.add_argument("--position-fix-sigma", type=float, default=0.1)
     ap.add_argument("--map-every", type=int, default=0)
     ap.add_argument("--map-stride", type=int, default=20)
+    ap.add_argument("--map-start", type=int, default=0)
+    ap.add_argument("--map-iterations", type=int, default=1)
     ap.add_argument("--odometry-every", type=int, default=0)
     ap.add_argument("--odometry-sigma-v", type=float, default=0.05)
     ap.add_argument("--odometry-sigma-rel", type=float, default=0.01)
@@ -150,7 +154,8 @@ def main():
     records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed,
                         fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma, map_every=args.map_every,
                         map_stride=args.map_stride, odo_every=args.odometry_every, odo_sigma_v=args.odometry_sigma_v,
-                        odo_sigma_rel=args.odometry_sigma_rel, nhc=args.nhc)
+                        odo_sigma_rel=args.odometry_sigma_rel, nhc=args.nhc, map_start=args.map_start,
+                        map_iterations=args.map_iterations)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -163,6 +168,8 @@ def main():
     if "map" in s:
         res["map"] = {"every": args.map_every, "stride": args.map_stride,
                       **{k: s["map"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "observations", "gated")}}
+        if args.map_start or args.map_iterations != 1:
+            res["map"].update(start=args.map_start, iterations=args.map_iterations, first_update=s["map_first"])
     if "odometry" in s:
         res["odometry"] = {"every": args.odometry_every, "sigma_v": args.odometry_sigma_v, "sigma_rel": args.odometry_sigma_rel,
                            "nhc": args.nhc, **{k: s["odometry"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied")}}
