@@ -225,7 +225,8 @@ __device__ __forceinline__ void inject_state(DevState<S>* st, S* poses, int M, i
 }
 
 // One warp (lane = row) factors the leading nb x nb block (nb <= 32) of the lower triangle of D in place, D = L L^T.  Returns
-// the number of leading pivots that were positive (nb: positive definite); idg[i] = 1 / L[i][i] for those.  (k_nees, k_aid)
+// the number of leading pivots that were positive (nb: positive definite); idg[i] = 1 / L[i][i] for those.  (cta_bordered_chol,
+// k_aid)
 template <int LD>
 __device__ __forceinline__ int warp_chol(double (*D)[LD], int nb, double* idg, int lane) {
   int nv = nb;
@@ -255,6 +256,87 @@ __device__ __forceinline__ double warp_row_solve(double x, const double (*D)[LD]
     else if (lane > c) x -= xc * D[lane][c];
   }
   return x;
+}
+
+// One 32 x 32 tile product over shared tiles, four outputs per thread of 256 (i = t >> 3):
+// s[u] += D[i][p] B[(t & 7) + 8 u][p], p = 0 .. 31 in order.  (cta_bordered_chol's trailing update, k_lmk_downdate)
+__device__ __forceinline__ void tile_dot32(const double (*D)[33], const double (*B)[33], int t, double (&s)[4]) {
+  const int i = t >> 3;
+#pragma unroll 8
+  for (int p = 0; p < 32; ++p) {
+    const double di = D[i][p];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) s[u] += di * B[(t & 7) + 8 * u][p];
+  }
+}
+
+// Blocked right-looking Cholesky (panels of 32, all 256 threads of the CTA) of the leading ncols x ncols block of the row-major
+// A (leading dimension ld, lower triangle read), A = L L^T in place, with the rows ncols .. Rt - 1 beneath it solved alongside:
+// each ends as x L^-T, x the row as given.  Returns -1, or the first pivot that is not positive (or NaN): at that panel only row
+// Rt - 1 is solved, over the good columns before the pivot, and the factor stops.  Ends with the CTA synchronised.  (k_nees,
+// k_lmk_gain)
+__device__ __forceinline__ int cta_bordered_chol(double* __restrict__ A, int ld, int ncols, int Rt, int t) {
+  __shared__ double D[32][33];  // diagonal block, then the row panel of a trailing tile
+  __shared__ double B[32][33];  // column panel of a trailing tile
+  __shared__ double idg[32];    // 1 / diagonal of the factored block
+  __shared__ int s_nv;
+  const int lane = t & 31;
+  for (int k0 = 0; k0 < ncols; k0 += 32) {
+    const int nb = min(32, ncols - k0);
+    for (int idx = t; idx < 32 * 32; idx += 256) {
+      const int i = idx / 32, j = idx - i * 32;
+      if (j <= i) D[i][j] = (i < nb) ? A[(size_t)(k0 + i) * ld + k0 + j] : 0.0;
+    }
+    __syncthreads();
+    if (t < 32) {  // unblocked factor of the diagonal block: lane = row
+      const int nv = warp_chol(D, nb, idg, t);
+      if (t == 0) s_nv = nv;
+    }
+    __syncthreads();
+    const int nv = s_nv;
+    // rows below the block: x = A[r, k0 : k0 + nb] L_kk^-T, one warp per row, lane = column
+    if (nv < nb) {  // a bad pivot: only row Rt - 1, over the nv good columns
+      if (t < 32) {
+        double* row = A + (size_t)(Rt - 1) * ld + k0;
+        const double x = warp_row_solve(lane < nv ? row[lane] : 0.0, D, idg, nv, lane);
+        if (lane < nv) row[lane] = x;
+      }
+      __syncthreads();
+      return k0 + nv;
+    }
+    for (int r = k0 + nb + (t >> 5); r < Rt; r += 8) {
+      double* row = A + (size_t)r * ld + k0;
+      const double x = warp_row_solve(lane < nb ? row[lane] : 0.0, D, idg, nb, lane);
+      if (lane < nb) row[lane] = x;
+    }
+    __syncthreads();
+    // trailing update A[r, c] -= L[r, k0:k1] . L[c, k0:k1] for k1 <= c <= r, c < ncols, r < Rt (nb = 32 here): 32 x 32 tiles of
+    // the lower triangle, both panels staged through shared memory
+    const int k1 = k0 + nb;
+    if (k1 < ncols) {
+      const int nti = (Rt - k1 + 31) / 32, ntj = (ncols - k1 + 31) / 32;
+      for (int ti = 0; ti < nti; ++ti)
+        for (int tj = 0; tj <= ti && tj < ntj; ++tj) {
+          const int rb = k1 + 32 * ti, cb = k1 + 32 * tj;
+          for (int idx = t; idx < 32 * 32; idx += 256) {
+            const int i = idx / 32, p = idx - i * 32;
+            D[i][p] = (rb + i < Rt) ? A[(size_t)(rb + i) * ld + k0 + p] : 0.0;
+            B[i][p] = (cb + i < ncols) ? A[(size_t)(cb + i) * ld + k0 + p] : 0.0;
+          }
+          __syncthreads();
+          double s[4] = {0.0, 0.0, 0.0, 0.0};
+          tile_dot32(D, B, t, s);
+          const int r = rb + (t >> 3);
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const int c = cb + (t & 7) + 8 * u;
+            if (r < Rt && c < ncols && c <= r) A[(size_t)r * ld + c] -= s[u];
+          }
+          __syncthreads();
+        }
+    }
+  }
+  return -1;
 }
 
 // ---- TMA (bulk async copy) staging of a small contiguous table into shared memory -----------------

@@ -134,6 +134,42 @@ struct AidJob {
   double chi2_max = 0.0;
 };
 
+// Checks one item of a stacked aided update against a window of M clones and appends it to j, its rows after j's: the check
+// of every stack item and of msckf_b200_aid_update's four item models.  0, or MSCKF_B200_ERR_ARG.
+int aid_append(AidJob& j, const msckf_b200_aid_item& q, int M, const std::string& w, const std::string& who) {
+  int m = 0, nz = 3;
+  switch (q.model) {
+    case MSCKF_B200_AID_VELOCITY: case MSCKF_B200_AID_POSITION: m = 3; break;
+    case MSCKF_B200_AID_POSE: m = 6; nz = 7; break;
+    case MSCKF_B200_AID_CLONE_POSE:
+      if (q.a < 0 || q.a >= M) return fail(MSCKF_B200_ERR_ARG, w + ": clone outside the window" + who);
+      m = 6; nz = 7;
+      break;
+    case MSCKF_B200_AID_BODY_VELOCITY:
+      if (q.a < 1 || q.a > 7) return fail(MSCKF_B200_ERR_ARG, w + ": the row mask must select rows 0..2" + who);
+      m = (q.a & 1) + ((q.a >> 1) & 1) + ((q.a >> 2) & 1);
+      break;
+    case MSCKF_B200_AID_RELATIVE_POSE:
+      if (q.a < 0 || q.a >= M || q.b < 0 || q.b >= M) return fail(MSCKF_B200_ERR_ARG, w + ": clone outside the window" + who);
+      if (q.a == q.b) return fail(MSCKF_B200_ERR_ARG, w + ": a relative pose needs two different clones" + who);
+      m = 6; nz = 7;
+      break;
+    default: return fail(MSCKF_B200_ERR_ARG, w + ": model not allowed in a stack" + who);
+  }
+  if (j.m + m > mb::kAidMaxRows) return fail(MSCKF_B200_ERR_ARG, w + ": more than 32 rows" + who);
+  if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, w + ": missing or non-finite z" + who);
+  if (nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
+    return fail(MSCKF_B200_ERR_ARG, w + ": zero quaternion" + who);
+  if (!q.R) return fail(MSCKF_B200_ERR_ARG, w + ": missing R" + who);
+  for (int r = 0; r < m; ++r)
+    if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, w + ": non-finite R" + who);
+  const int k = j.n_items++;
+  j.item[k] = {(short)q.model, (short)(q.model >= MSCKF_B200_AID_CLONE_POSE ? q.a : 0),  // (LINEAR is not an item model)
+               (short)(q.model == MSCKF_B200_AID_RELATIVE_POSE ? q.b : 0), (short)j.m};
+  j.z[k] = q.z; j.nz[k] = nz; j.R[k] = q.R; j.m += m;
+  return 0;
+}
+
 // tail kernel choice (engine option 3 / window size)
 inline size_t tail_legacy_smem(int n, int NB) {
   const int ldt = (n + 3) & ~3;
@@ -1453,24 +1489,23 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
     const std::string who = " (member " + std::to_string(i) + ")";
     const int M = eng[i]->M, n = 15 + 6 * M;
     if (q.model > MSCKF_B200_AID_LINEAR) return fail(MSCKF_B200_ERR_ARG, "aid_update: unknown model" + who);
-    const bool lin = q.model == MSCKF_B200_AID_LINEAR;
-    const int m = lin ? q.m : (q.model <= MSCKF_B200_AID_POSITION ? 3 : 6);
-    if (lin ? (m < 1 || m > mb::kAidMaxRows || q.n != n) : ((q.m != 0 && q.m != m) || (q.n != 0 && q.n != n)))
-      return fail(MSCKF_B200_ERR_ARG, "aid_update: m / n do not match the model and the window" + who);
-    if (q.model == MSCKF_B200_AID_CLONE_POSE && (q.clone < 0 || q.clone >= M)) return fail(MSCKF_B200_ERR_ARG, "aid_update: clone outside the window" + who);
-    const int nz = lin ? m : (q.model <= MSCKF_B200_AID_POSITION ? 3 : 7);
-    if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing or non-finite z" + who);
+    if (std::isnan(q.chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_update: chi2_max is NaN" + who);
+    AidJob& j = job[i];
+    j.chi2_max = q.chi2_max;
+    if (q.model != MSCKF_B200_AID_LINEAR) {  // one item of the stacked form (a = the clone of CLONE_POSE; ignored otherwise)
+      RC(aid_append(j, msckf_b200_aid_item{q.model, q.clone, 0, q.z, q.R}, M, "aid_update", who));
+      if ((q.m != 0 && q.m != j.m) || (q.n != 0 && q.n != n)) return fail(MSCKF_B200_ERR_ARG, "aid_update: m / n do not match the model and the window" + who);
+      continue;
+    }
+    const int m = q.m;  // LINEAR: the caller's r and H
+    if (m < 1 || m > mb::kAidMaxRows || q.n != n) return fail(MSCKF_B200_ERR_ARG, "aid_update: m / n do not match the model and the window" + who);
+    if (!q.z || !finite(q.z, m)) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing or non-finite z" + who);
     if (!q.R) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing R" + who);
     for (int r = 0; r < m; ++r)
       if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, "aid_update: non-finite R" + who);
-    if (lin && (!q.H || !finite(q.H, (size_t)m * n))) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing or non-finite H" + who);
-    if (!lin && nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
-      return fail(MSCKF_B200_ERR_ARG, "aid_update: zero quaternion" + who);
-    if (std::isnan(q.chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_update: chi2_max is NaN" + who);
-    AidJob& j = job[i];
-    j.m = m; j.n_items = 1; j.chi2_max = q.chi2_max;
-    j.item[0] = {(short)q.model, (short)(q.model == MSCKF_B200_AID_CLONE_POSE ? q.clone : 0), 0, 0};
-    j.z[0] = q.z; j.nz[0] = nz; j.R[0] = q.R; j.H = lin ? q.H : nullptr;
+    if (!q.H || !finite(q.H, (size_t)m * n)) return fail(MSCKF_B200_ERR_ARG, "aid_update: missing or non-finite H" + who);
+    j.m = m; j.n_items = 1; j.item[0] = {(short)q.model, 0, 0, 0};
+    j.z[0] = q.z; j.nz[0] = m; j.R[0] = q.R; j.H = q.H;
   }
   return aid_run(job, out, "aid_update");
 }
@@ -1487,45 +1522,9 @@ int Ctx<S>::aid_stack(const msckf_b200_aid_item* const* items, const int* n_item
     const std::string who = " (member " + std::to_string(i) + ")";
     if (n_items[i] < 0 || n_items[i] > mb::kAidMaxItems) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: 1 to 8 items per stack" + who);
     if (!items[i]) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: null item list" + who);
-    const int M = eng[i]->M;
-    AidJob& j = job[i];
-    for (int k = 0; k < n_items[i]; ++k) {
-      const msckf_b200_aid_item& q = items[i][k];
-      const std::string wk = " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")";
-      int m = 0, nz = 3;
-      switch (q.model) {
-        case MSCKF_B200_AID_VELOCITY: case MSCKF_B200_AID_POSITION: m = 3; break;
-        case MSCKF_B200_AID_POSE: m = 6; nz = 7; break;
-        case MSCKF_B200_AID_CLONE_POSE:
-          if (q.a < 0 || q.a >= M) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: clone outside the window" + wk);
-          m = 6; nz = 7;
-          break;
-        case MSCKF_B200_AID_BODY_VELOCITY:
-          if (q.a < 1 || q.a > 7) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: the row mask must select rows 0..2" + wk);
-          m = (q.a & 1) + ((q.a >> 1) & 1) + ((q.a >> 2) & 1);
-          break;
-        case MSCKF_B200_AID_RELATIVE_POSE:
-          if (q.a < 0 || q.a >= M || q.b < 0 || q.b >= M) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: clone outside the window" + wk);
-          if (q.a == q.b) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: a relative pose needs two different clones" + wk);
-          m = 6; nz = 7;
-          break;
-        default: return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: model not allowed in a stack" + wk);
-      }
-      if (j.m + m > mb::kAidMaxRows) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: more than 32 rows" + who);
-      if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: missing or non-finite z" + wk);
-      if (nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
-        return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: zero quaternion" + wk);
-      if (!q.R) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: missing R" + wk);
-      for (int r = 0; r < m; ++r)
-        if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: non-finite R" + wk);
-      j.item[k] = {(short)q.model, (short)(q.model == MSCKF_B200_AID_VELOCITY || q.model == MSCKF_B200_AID_POSITION ||
-                                           q.model == MSCKF_B200_AID_POSE ? 0 : q.a),
-                   (short)(q.model == MSCKF_B200_AID_RELATIVE_POSE ? q.b : 0), (short)j.m};
-      j.z[k] = q.z; j.nz[k] = nz; j.R[k] = q.R;
-      j.m += m;
-    }
-    j.n_items = n_items[i];
-    j.chi2_max = chi2_max;
+    for (int k = 0; k < n_items[i]; ++k)
+      RC(aid_append(job[i], items[i][k], eng[i]->M, "aid_stack_update", " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")"));
+    job[i].chi2_max = chi2_max;
   }
   return aid_run(job, out, "aid_stack_update");
 }

@@ -7,8 +7,8 @@
 //   k_lmk_clone    : one CTA per (touched clone, member).  Residual, per-observation gate gamma_i = r^T (X P_kk X^T + R)^-1 r
 //                    and flag, rows whitened by R = L_R L_R^T, then a Householder QR (one warp) of the clone's used rows
 //                    [X~ | r~] (2a x 7): q = min(2a, 6) rows [T_k | rho_k] and the leftover e_k^2 go to the member's workspace.
-//   k_lmk_gain     : one CTA per member.  T P (rows of T in window order), S = T P T^T + I, and one blocked right-looking
-//                    Cholesky of [S ; (T P)^T ; rho^T]: the extra rows end as W^T = (L^-1 T P)^T and y = L^-1 rho.
+//   k_lmk_gain     : one CTA per member.  T P (rows of T in window order), S = T P T^T + I, and one blocked Cholesky
+//                    (cta_bordered_chol) of [S ; (T P)^T ; rho^T]: the extra rows end as W^T = (L^-1 T P)^T and y = L^-1 rho.
 //                    NIS = |y|^2 + sum_k e_k^2 (the NIS of the dense stacked system).
 //   k_lmk_downdate : 32 x 32 tiles of the lower triangle of P - W^T W (fp64, rounded once, both halves written, in place) and
 //                    dx = W^T y on the diagonal tiles; the last tile of a member (ticket counter) runs the state injection.
@@ -31,7 +31,7 @@ constexpr int kLmkMaxObs = 4096;      // observations of one member in one call
 constexpr int kLmkMaxIter = 16;       // linearisations of the iterated form
 constexpr int kLmkThreads = 256;
 constexpr int kLmkSlot = 48;          // doubles per touched clone: T [6][6], rho [6], e^2, used, q
-constexpr int kLmkNB = 32;            // panel width of the blocked Cholesky and tile size of the downdate
+constexpr int kLmkNB = 32;            // tile size of the downdate (tile_dot32's)
 
 // per-member result; every field but numeric is msckf_b200_landmark_result's, at its offset
 struct LmkOut {
@@ -262,11 +262,10 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
   const double* __restrict__ const slot = a.m[f].slot;
   LmkCtl* const ctl = a.m[f].ctl;
   LmkOut* const out = a.m[f].out;
-  const int ldp = a.m[f].ldp, G = a.m[f].G, ld = a.m[f].ld, n = 15 + 6 * a.m[f].M, t = threadIdx.x, lane = t & 31;
+  const int ldp = a.m[f].ldp, G = a.m[f].G, ld = a.m[f].ld, n = 15 + 6 * a.m[f].M, t = threadIdx.x;
   __shared__ int off[kMaxKeep + 1], ck[kMaxKeep], rg[6 * kMaxKeep];
-  __shared__ double D[kLmkNB][kLmkNB + 1], B[kLmkNB][kLmkNB + 1], idg[kLmkNB];
   __shared__ double s_e2;
-  __shared__ int s_used, s_nv;
+  __shared__ int s_used;
 
   if (t == 0) {
     int o = 0, u = 0;
@@ -282,7 +281,7 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
   }
   for (int g = t; g < G; g += kLmkThreads) ck[g] = a.m[f].grp[3 * g];
   __syncthreads();
-  const int m = off[G], Rt = m + n + 1;
+  const int m = off[G];
   if (s_used == 0) {  // no observation used: nothing is written (the iterate form never gets here: k_lmk_step stops it)
     if (!IT && t == 0) {
       ctl->apply = 0;
@@ -317,58 +316,10 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
     A[(size_t)r * ld + s_] = v;
   }
   __syncthreads();
-  // ---- blocked right-looking Cholesky of [S ; (T P)^T ; rho^T] (Rt x m): the extra rows end as W^T and y
-  int bad = 0;
-  for (int k0 = 0; k0 < m; k0 += kLmkNB) {
-    const int nb = min(kLmkNB, m - k0);
-    for (int idx = t; idx < kLmkNB * kLmkNB; idx += kLmkThreads) {
-      const int i = idx / kLmkNB, j = idx - i * kLmkNB;
-      if (j <= i) D[i][j] = (i < nb) ? A[(size_t)(k0 + i) * ld + k0 + j] : 0.0;
-    }
-    __syncthreads();
-    if (t < 32) {
-      const int nv = warp_chol(D, nb, idg, t);
-      if (t == 0) s_nv = nv;
-    }
-    __syncthreads();
-    if (s_nv < nb) { bad = 1; break; }
-    for (int r = k0 + nb + (t >> 5); r < Rt; r += kLmkThreads / 32) {
-      double* row = A + (size_t)r * ld + k0;
-      const double x = warp_row_solve(lane < nb ? row[lane] : 0.0, D, idg, nb, lane);
-      if (lane < nb) row[lane] = x;
-    }
-    __syncthreads();
-    const int k1 = k0 + nb;
-    if (k1 < m) {  // A[r, c] -= L[r, k0:k1] . L[c, k0:k1] for k1 <= c <= r, c < m, r < Rt
-      const int nti = (Rt - k1 + kLmkNB - 1) / kLmkNB, ntj = (m - k1 + kLmkNB - 1) / kLmkNB;
-      for (int ti = 0; ti < nti; ++ti)
-        for (int tj = 0; tj <= ti && tj < ntj; ++tj) {
-          const int rb = k1 + kLmkNB * ti, cb = k1 + kLmkNB * tj;
-          for (int idx = t; idx < kLmkNB * kLmkNB; idx += kLmkThreads) {
-            const int i = idx / kLmkNB, p = idx - i * kLmkNB;
-            D[i][p] = (rb + i < Rt && p < nb) ? A[(size_t)(rb + i) * ld + k0 + p] : 0.0;
-            B[i][p] = (cb + i < m && p < nb) ? A[(size_t)(cb + i) * ld + k0 + p] : 0.0;
-          }
-          __syncthreads();
-          const int i = t >> 3, r = rb + i;
-          double s[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll 8
-          for (int p = 0; p < kLmkNB; ++p) {
-            const double di = D[i][p];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) s[u] += di * B[(t & 7) + 8 * u][p];
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int c = cb + (t & 7) + 8 * u;
-            if (r < Rt && c < m && c <= r) A[(size_t)r * ld + c] -= s[u];
-          }
-          __syncthreads();
-        }
-    }
-  }
+  // ---- Cholesky of [S ; (T P)^T ; rho^T] (m + n + 1 rows): the extra rows end as W^T and y
+  const int bad = cta_bordered_chol(A, ld, m, m + n + 1, t);
   if (t == 0) {
-    if (bad) {  // S not positive definite: nothing is written
+    if (bad >= 0) {  // S not positive definite: nothing is written
       ctl->apply = 0;
       out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
       out->status = 1; out->applied = 0;
@@ -482,12 +433,7 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_downdate(const Members<LmkA
       B[ii][p] = (cb + ii < n && p0 + p < m) ? Wt[(size_t)(cb + ii) * ld + p0 + p] : 0.0;
     }
     __syncthreads();
-#pragma unroll 8
-    for (int p = 0; p < kLmkNB; ++p) {
-      const double di = D[i][p];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) s[u] += di * B[(t & 7) + 8 * u][p];
-    }
+    tile_dot32(D, B, t, s);
     __syncthreads();
   }
   int bad = 0;

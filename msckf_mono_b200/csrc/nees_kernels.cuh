@@ -17,7 +17,6 @@ struct NeesOut {
   int dim_full, first_bad_pivot;
 };
 constexpr int kNeesTruthImu = 19;  // p, v, b_g, b_a, g, q_IG (the layout of msckf_b200_initialize's imu_state)
-constexpr int kNeesNB = 32;        // panel width of the blocked Cholesky
 
 template <class S>
 struct NeesArgs {
@@ -63,10 +62,6 @@ __global__ void __launch_bounds__(256) k_nees(const Members<NeesArgs<S>, NM> a) 
   const int ldp = a.m[f].ldp, n = a.m[f].n, t = threadIdx.x;
   const bool full = a.m[f].full != 0;
   double* __restrict__ const e = W + (size_t)n * n;  // row n
-  __shared__ double D[kNeesNB][kNeesNB + 1];         // diagonal block, then the row panel of a trailing tile
-  __shared__ double B[kNeesNB][kNeesNB + 1];         // column panel of a trailing tile
-  __shared__ double idg[kNeesNB];                    // 1 / diagonal of the factored block
-  __shared__ int s_nv, s_bad;
 
   // ---- error state (fp64), in the NEES order
   if (t == 0) {
@@ -77,7 +72,6 @@ __global__ void __launch_bounds__(256) k_nees(const Members<NeesArgs<S>, NM> a) 
       e[9 + i] = truth[6 + i] - (double)st->b_g[i];
       e[12 + i] = truth[9 + i] - (double)st->b_a[i];
     }
-    s_bad = -1;
   }
   for (int k = t; k < (n - 15) / 6; k += 256) {  // clone k: pose table q(4) p(3) pad, truth p(3) q(4)
     const S* ps = poses + kPoseStride * k;
@@ -92,72 +86,13 @@ __global__ void __launch_bounds__(256) k_nees(const Members<NeesArgs<S>, NM> a) 
   }
   __syncthreads();
 
-  // ---- blocked right-looking Cholesky of [P_SS ; e^T] ((n + 1) x n): row n ends as y = L^-1 e.  The factor stays in W.
-  for (int k0 = 0; k0 < n; k0 += kNeesNB) {
-    const int nb = min(kNeesNB, n - k0);
-    for (int idx = t; idx < kNeesNB * kNeesNB; idx += 256) {
-      const int i = idx / kNeesNB, j = idx - i * kNeesNB;
-      if (j <= i) D[i][j] = (i < nb) ? W[(size_t)(k0 + i) * n + k0 + j] : 0.0;
-    }
-    __syncthreads();
-    if (t < 32) {  // unblocked factor of the diagonal block: lane = row
-      const int nv = warp_chol(D, nb, idg, t);
-      if (t == 0) s_nv = nv;
-    }
-    __syncthreads();
-    const int nv = s_nv;
-    // rows below the block (and the error row): x = A[r, k0 : k0 + nv] L_kk^-T, one warp per row, lane = column.  After a bad
-    // pivot only the error row is still wanted.
-    const int r0 = nv < nb ? n : k0 + nb, lane = t & 31;
-    for (int r = r0 + (t >> 5); r <= n; r += 8) {
-      double* row = W + (size_t)r * n + k0;
-      const double x = warp_row_solve(lane < nv ? row[lane] : 0.0, D, idg, nv, lane);
-      if (lane < nv) row[lane] = x;
-    }
-    if (nv < nb) {
-      if (t == 0) s_bad = k0 + nv;
-      __syncthreads();
-      break;
-    }
-    __syncthreads();
-    // trailing update A[r, c] -= L[r, k0:k0+nb] . L[c, k0:k0+nb] for k1 <= c <= r, c < n, r <= n: 32 x 32 tiles of the lower
-    // triangle, both panels staged through shared memory, four outputs per thread
-    const int k1 = k0 + nb;
-    if (k1 < n) {
-      const int nti = (n + 1 - k1 + kNeesNB - 1) / kNeesNB, ntj = (n - k1 + kNeesNB - 1) / kNeesNB;
-      for (int tl = 0; tl < nti * (nti + 1) / 2; ++tl) {
-        int ti, tj;
-        tri_tile_index(tl, ti, tj);
-        if (tj >= ntj) continue;
-        const int rb = k1 + kNeesNB * ti, cb = k1 + kNeesNB * tj;
-        for (int idx = t; idx < kNeesNB * kNeesNB; idx += 256) {
-          const int i = idx / kNeesNB, p = idx - i * kNeesNB;
-          D[i][p] = (rb + i <= n) ? W[(size_t)(rb + i) * n + k0 + p] : 0.0;
-          B[i][p] = (cb + i < n) ? W[(size_t)(cb + i) * n + k0 + p] : 0.0;
-        }
-        __syncthreads();
-        const int i = t >> 3, r = rb + i;
-        double s[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll 8
-        for (int p = 0; p < kNeesNB; ++p) {
-          const double di = D[i][p];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) s[u] += di * B[(t & 7) + 8 * u][p];
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int c = cb + (t & 7) + 8 * u;
-          if (r <= n && c < n && c <= r) W[(size_t)r * n + c] -= s[u];
-        }
-        __syncthreads();
-      }
-    }
-  }
+  // ---- Cholesky of [P_SS ; e^T] ((n + 1) x n): row n ends as y = L^-1 e (over the good pivots).  The factor stays in W.
+  const int bad = cta_bordered_chol(W, n, n, n + 1, t);
 
   // ---- prefix sums of y^2; the position block by its own 3 x 3 solve
   if (t == 0) {
     const double nan = __longlong_as_double(0x7ff8000000000000ll);
-    const int lim = s_bad < 0 ? n : s_bad;
+    const int lim = bad < 0 ? n : bad;
     double acc = 0.0, v3 = nan, v6 = nan, v15 = nan, vall = nan;
     for (int i = 0; i < lim; ++i) {
       acc += e[i] * e[i];
@@ -188,7 +123,7 @@ __global__ void __launch_bounds__(256) k_nees(const Members<NeesArgs<S>, NM> a) 
     }
     out->orientation = v3; out->position = vp; out->pose = v6; out->imu = v15; out->full = vall;
     out->dim_full = full ? n : 0;
-    out->first_bad_pivot = s_bad;
+    out->first_bad_pivot = bad;
   }
 }
 
