@@ -274,7 +274,7 @@ int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_
  * that clone: p_C = C (p_L - p_C_G), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), Jacobian the 2 x 6
  * block [J [p_C]x, -J C] over the clone's [dtheta, dp] (msckf.h:929-936) WITHOUT the observability projection (a known landmark
  * observes global position and yaw) and without a feature null space (the landmark is not estimated; its position is taken as
- * exact -- inflate R to account for map uncertainty).  Noise R (2 x 2, same for every observation; NULL: diag(u_var', v_var')).
+ * exact -- msckf_b200_map_landmark_update below takes each landmark's map covariance).  Noise R (2 x 2, same for every observation; NULL: diag(u_var', v_var')).
  * Per observation: flag 2 (not used) when p_C[2] <= 0 or z^ is not finite (gamma NaN); else gamma = r^T (X P_kk X^T + R)^-1 r,
  * flag 1 (gated out) when chi2_obs > 0 and gamma > chi2_obs, else flag 0 (used).  The used rows are whitened and compressed per
  * clone by a Householder QR (exact: each row touches one clone), then S = T P T^T + I = L L^T, W = L^-1 T P, y = L^-1 rho,
@@ -325,6 +325,38 @@ int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks*
 /* the same for every member of a batch (lm[i], out[i]; out[i] is not written for a member with lm[i].n_obs = 0); every member is
  * validated before anything is launched. */
 int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out);
+/* ---- mapped landmarks with map uncertainty: the same update with each landmark's position error marginalised -----------
+ * Observation i is of landmark landmark[i], whose true position is p_L_G[i] + dp, dp ~ N(0, Sigma_L[landmark[i]]) (p_L_G must be
+ * identical for observations of one landmark).  With F_i = J C, the observation's block over dp (= -X_i[:, 3:6]), the gate is
+ * gamma_i = r^T (X P_kk X^T + F Sigma F^T + R)^-1 r, and the used observations are fused with the noise R (x) I + F Sigma F^T,
+ * which couples the rows of one landmark across the clones that see it: the landmark's error is common to them.  On the device
+ * a landmark seen from one clone is whitened by R + F Sigma F^T before its clone's QR; the used rows of a landmark seen from
+ * 2 .. 8 clones are stacked under the prior rows [0 | L^-1 | 0] (Sigma = L L^T) and three Householder reflectors on the F
+ * columns eliminate dp exactly; the landmarks with one clone set are then compressed together by one Householder QR over their
+ * 6c clone columns to min(2 used, 6c) rows.  rows reports the sum of those and of the clones' min(2 a_k, 6); dof = 2 x used and
+ * NIS are those of the dense marginal system.  The gain, downdate and injection are the exact-map update's.  Iterated
+ * (max_iter >= 2): each linearisation relinearises at the iterate clone poses (F too) with the landmarks kept at p_L_G, so it is
+ * an IEKF over the clone poses with the map marginalised, not a joint estimate of the landmarks.  Each call treats the map
+ * error as fresh: fusing the same landmarks call after call counts their error more than once (DESIGN.md 4.12).
+ * Launches per 32 members when any of them has Sigma_L: clone, set, gain, (step, clone, set, gain) x (K - 1), downdate; still
+ * one copy each way and one synchronisation.
+ * Caps, each MSCKF_B200_ERR_ARG before anything is launched (nothing written): 8 clones per landmark, 256 observations per
+ * clone set, 256 clone sets per member and 1152 rows (6 x 192 clones, the gain's row table) in the worst-case compressed system
+ * (the sum over clones of min(2 a_k, 6) and over clone sets of min(2 observations, 6c)).  Also ERR_ARG: landmark NULL or
+ * outside 0 .. n_landmarks - 1, a Sigma_L that is not finite or not positive definite, p_L_G differing within a landmark, and one
+ * landmark observed twice from one clone. */
+typedef struct {
+  const int* landmark;   /* [n_obs] landmark of each observation, 0 .. n_landmarks - 1 */
+  const double* Sigma_L; /* [n_landmarks][6] lower triangle xx, yx, yy, zx, zy, zz (positive definite), or NULL: the map is exact
+                            and the call is msckf_b200_landmark_update's, with its kernels and launches */
+  int n_landmarks;
+} msckf_b200_landmark_map;
+/* map NULL: msckf_b200_landmark_update */
+int msckf_b200_map_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                   msckf_b200_landmark_result* out);
+/* the same for every member of a batch (lm[i], map[i], out[i]; map NULL: every member exact) */
+int msckf_b200_batch_map_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                         msckf_b200_landmark_result* out);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

@@ -39,6 +39,18 @@ struct landmarkObservation {
   double z[2];
   double p_L_G[3];
 };
+// A map landmark with position uncertainty (not in the reference): its map position p_L_G and the lower triangle xx, yx, yy,
+// zx, zy, zz of its 3 x 3 covariance.  mapObservation: normalised image coordinates z of landmark `landmark` (an index into
+// the landmark list of the call) seen from the image whose clone has id state_id.
+struct mapLandmark {
+  double p_L_G[3];
+  double Sigma[6];
+};
+struct mapObservation {
+  int state_id;
+  int landmark;
+  double z[2];
+};
 
 template <typename _S>
 class MSCKF {
@@ -425,6 +437,43 @@ class MSCKF {
     landmarkAbsorb(r);
     return r;
   }
+  // mapped landmarks with map uncertainty (not in the reference; msckf_b200_map_landmark_update: model, gate, caps there): each
+  // landmark's position error, N(0, Sigma), is marginalised over all its observations in the call.  An observation of an
+  // image that is not in the window, or of a landmark outside `landmarks`, throws std::invalid_argument before any device
+  // call; otherwise as the landmarkUpdate above.
+  msckf_b200_landmark_result landmarkUpdate(const std::vector<mapObservation>& obs, const std::vector<mapLandmark>& landmarks,
+                                            const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
+                                            std::vector<double>* gamma = nullptr, std::vector<int>* flag = nullptr, int max_iter = 1,
+                                            double tol = 1e-10) {
+    msckf_b200_landmarks lm{};
+    msckf_b200_landmark_map map{};
+    mapPack(obs, landmarks, R, chi2_obs, gamma, flag, lm, map);
+    lm.max_iter = max_iter; lm.tol = tol;
+    msckf_b200_landmark_result r = {};
+    checkNumeric(msckf_b200_map_landmark_update(eng(), &lm, &map, &r), "msckf_b200_map_landmark_update");
+    landmarkAbsorb(r);
+    return r;
+  }
+  // landmarkPack of the observations' map positions, and the map (landmark ids, Sigma) in this object's buffers
+  void mapPack(const std::vector<mapObservation>& obs, const std::vector<mapLandmark>& landmarks, const FixedMatrix<double, 2, 2>* R,
+               double chi2_obs, std::vector<double>* gamma, std::vector<int>* flag, msckf_b200_landmarks& lm,
+               msckf_b200_landmark_map& map) {
+    std::vector<landmarkObservation> o(obs.size());
+    lmk_id_.resize(obs.size());
+    for (size_t i = 0; i < obs.size(); ++i) {
+      if (obs[i].landmark < 0 || obs[i].landmark >= (int)landmarks.size())
+        throw std::invalid_argument("MSCKF::landmarkUpdate: landmark " + std::to_string(obs[i].landmark) + " is not in the map");
+      o[i].state_id = obs[i].state_id;
+      o[i].z[0] = obs[i].z[0]; o[i].z[1] = obs[i].z[1];
+      for (int c = 0; c < 3; ++c) o[i].p_L_G[c] = landmarks[obs[i].landmark].p_L_G[c];
+      lmk_id_[i] = obs[i].landmark;
+    }
+    landmarkPack(o, R, chi2_obs, gamma, flag, lm);
+    lmk_sig_.resize(6 * landmarks.size());
+    for (size_t l = 0; l < landmarks.size(); ++l)
+      for (int c = 0; c < 6; ++c) lmk_sig_[6 * l + c] = landmarks[l].Sigma[c];
+    map.landmark = lmk_id_.data(); map.Sigma_L = lmk_sig_.data(); map.n_landmarks = (int)landmarks.size();
+  }
   // a msckf_b200_landmarks of obs with window positions from the clone list (pointers into this object's buffers)
   void landmarkPack(const std::vector<landmarkObservation>& obs, const FixedMatrix<double, 2, 2>* R, double chi2_obs,
                     std::vector<double>* gamma, std::vector<int>* flag, msckf_b200_landmarks& lm) {
@@ -671,6 +720,8 @@ class MSCKF {
   std::vector<featureTrackToResidualize<_S>> tri_batch_, res_batch_;
   std::vector<double> aid_R_;  // R of the last convenience-form aided update, row-major
   std::vector<int> lmk_clone_;  // the last landmark update's observations in the C-ABI's layout (landmarkPack)
+  std::vector<int> lmk_id_;       // ... and the landmark of each, with every landmark's Sigma (mapPack)
+  std::vector<double> lmk_sig_;
   std::vector<double> lmk_z_, lmk_p_;
   double lmk_R_[3] = {0.0, 0.0, 0.0};
 
@@ -1015,6 +1066,35 @@ class MSCKFBatch {
     const int rc = msckf_b200_batch_landmark_update(batch_, lm.data(), r.data());
     if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch landmark update: " << msckf_b200_last_error() << std::endl;
     else MSCKF<_S>::check(rc, "msckf_b200_batch_landmark_update");
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty()) filters_[i]->landmarkAbsorb(r[i]);
+    return r;
+  }
+  // MSCKF::landmarkUpdate with map uncertainty for every filter (obs[i] empty: filter i is left alone; landmarks[i] is filter
+  // i's landmark list) as one msckf_b200_batch_map_landmark_update.  Bad ids throw before any device call.
+  std::vector<msckf_b200_landmark_result> landmarkUpdate(const std::vector<std::vector<mapObservation>>& obs,
+                                                         const std::vector<std::vector<mapLandmark>>& landmarks,
+                                                         const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
+                                                         std::vector<std::vector<double>>* gamma = nullptr,
+                                                         std::vector<std::vector<int>>* flag = nullptr, int max_iter = 1,
+                                                         double tol = 1e-10) {
+    const size_t n = size();
+    if (obs.size() != n || landmarks.size() != n)
+      throw std::invalid_argument("MSCKFBatch::landmarkUpdate: one observation list and one landmark list per filter");
+    if (gamma) gamma->assign(n, std::vector<double>());
+    if (flag) flag->assign(n, std::vector<int>());
+    std::vector<msckf_b200_landmarks> lm(n, msckf_b200_landmarks());
+    std::vector<msckf_b200_landmark_map> map(n, msckf_b200_landmark_map());
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty())
+        filters_[i]->mapPack(obs[i], landmarks[i], R, chi2_obs, gamma ? &(*gamma)[i] : nullptr, flag ? &(*flag)[i] : nullptr, lm[i],
+                             map[i]);
+    for (size_t i = 0; i < n; ++i) { lm[i].max_iter = max_iter; lm[i].tol = tol; }
+    flushImu();
+    std::vector<msckf_b200_landmark_result> r(n, msckf_b200_landmark_result());
+    const int rc = msckf_b200_batch_map_landmark_update(batch_, lm.data(), map.data(), r.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch map landmark update: " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_map_landmark_update");
     for (size_t i = 0; i < n; ++i)
       if (!obs[i].empty()) filters_[i]->landmarkAbsorb(r[i]);
     return r;

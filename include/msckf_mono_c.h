@@ -103,6 +103,18 @@ int msckf_mono_landmark_update_iter(void* h, int n_obs, const int* state_ids, co
 int msckf_mono_batch_landmark_update_iter(void* batch, const int* n_obs, const int* state_ids, const double* z, const double* p_L_G,
                                           const double* R3, double chi2_obs, int max_iter, double tol, double* gamma, int* flag,
                                           msckf_b200_landmark_result* out);
+/* mapped-landmark update with map uncertainty (MSCKF::landmarkUpdate over mapObservation / mapLandmark,
+ * msckf_b200_map_landmark_update: model, gate, caps and errors there): n_obs observations (state_ids [n], landmark [n] indices
+ * into this call's landmarks, z [n][2]) of n_landmarks landmarks (p_L_G [L][3], Sigma [L][6] lower triangle xx, yx, yy, zx, zy,
+ * zz); R3, chi2_obs, max_iter, tol, gamma, flag as in msckf_mono_landmark_update_iter.  _batch_map_update: n_obs[i] and
+ * n_landmarks[i] per filter, every array concatenated over the filters in order; out[i] of a filter with n_obs[i] = 0 is not
+ * written. */
+int msckf_mono_map_update(void* h, int n_obs, const int* state_ids, const int* landmark, const double* z, int n_landmarks,
+                          const double* p_L_G, const double* Sigma, const double* R3, double chi2_obs, int max_iter, double tol,
+                          double* gamma, int* flag, msckf_b200_landmark_result* out);
+int msckf_mono_batch_map_update(void* batch, const int* n_obs, const int* state_ids, const int* landmark, const double* z,
+                                const int* n_landmarks, const double* p_L_G, const double* Sigma, const double* R3, double chi2_obs,
+                                int max_iter, double tol, double* gamma, int* flag, msckf_b200_landmark_result* out);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

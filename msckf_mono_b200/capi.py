@@ -93,6 +93,10 @@ class Landmarks(C.Structure):
                 ("chi2_obs", C.c_double), ("gamma", C.c_void_p), ("flag", C.c_void_p), ("max_iter", C.c_int), ("tol", C.c_double)]
 
 
+class LandmarkMap(C.Structure):
+    _fields_ = [("landmark", C.c_void_p), ("Sigma_L", C.c_void_p), ("n_landmarks", C.c_int)]
+
+
 class LandmarkResult(C.Structure):
     _fields_ = [("nis", C.c_double), ("dx_norm", C.c_double), ("dof", C.c_int), ("rows", C.c_int), ("used", C.c_int),
                 ("applied", C.c_int), ("status", C.c_int), ("iterations", C.c_int), ("converged", C.c_int), ("step", C.c_double)]
@@ -121,6 +125,22 @@ def landmark_struct(spec):
                   float(spec.get("chi2_obs", 0.0)), gamma.ctypes.data, flag.ctypes.data, int(spec.get("max_iter", 0)),
                   float(spec.get("tol", 0.0)))
     return a, (clone, z, p, R, gamma, flag)
+
+
+def landmark_map_struct(spec):
+    """(LandmarkMap, the arrays it points into) of a spec's map uncertainty: landmark [n] (the landmark of each observation)
+    with Sigma_L [n_landmarks, 3, 3] or [n_landmarks, 6] (lower triangle xx, yx, yy, zx, zy, zz).  No Sigma_L (or spec None):
+    an exact map, all fields zero."""
+    S = None if spec is None else spec.get("Sigma_L")
+    if S is None:
+        return LandmarkMap(None, None, 0), ()
+    lm = spec.get("landmark")
+    lm = None if lm is None else np.ascontiguousarray(lm, dtype=np.int32).ravel()
+    S = np.asarray(S, dtype=np.float64)
+    if S.ndim == 3:
+        S = S[:, [0, 1, 1, 2, 2, 2], [0, 0, 1, 0, 1, 2]]
+    S = np.ascontiguousarray(S.reshape(-1, 6))
+    return LandmarkMap(None if lm is None else lm.ctypes.data, S.ctypes.data, len(S)), (lm, S)
 
 
 _lib = None
@@ -317,15 +337,21 @@ class Batch:
 
     def landmark_update(self, specs, max_iter=None, tol=None):
         """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
-        i alone); max_iter / tol, when given, apply to every spec that does not set its own.  A list of result dicts with
-        "gamma" and "flag" arrays (None for an engine left alone)"""
+        i alone); max_iter / tol, when given, apply to every spec that does not set its own.  When a spec has Sigma_L (see
+        landmark_map_struct) the call is msckf_b200_batch_map_landmark_update.  A list of result dicts with "gamma" and "flag"
+        arrays (None for an engine left alone)"""
         n = len(self.engines)
         assert len(specs) == n
         extra = {k: v for k, v in (("max_iter", max_iter), ("tol", tol)) if v is not None}
         st = [landmark_struct(s if s is None else dict(extra, **s)) for s in specs]
         out = (LandmarkResult * n)()
-        check(lib().msckf_b200_batch_landmark_update(self.h, (Landmarks * n)(*[a for a, _ in st]), out),
-              "msckf_b200_batch_landmark_update")
+        arr = (Landmarks * n)(*[a for a, _ in st])
+        if any(s is not None and s.get("Sigma_L") is not None for s in specs):
+            maps = [landmark_map_struct(s) for s in specs]
+            check(lib().msckf_b200_batch_map_landmark_update(self.h, arr, (LandmarkMap * n)(*[m for m, _ in maps]), out),
+                  "msckf_b200_batch_map_landmark_update")
+        else:
+            check(lib().msckf_b200_batch_landmark_update(self.h, arr, out), "msckf_b200_batch_landmark_update")
         return [None if not k else dict(o.as_dict(), gamma=k[4], flag=k[5]) for (a, k), o in zip(st, out)]
 
     def jac_occupancy(self):
@@ -471,13 +497,19 @@ class Engine:
               "msckf_b200_aid_stack_update")
         return out.as_dict()
 
-    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0):
+    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0, landmark=None, Sigma_L=None):
         """msckf_b200_landmark_update: observations of known landmarks p_L [n, 3] at z [n, 2] from window positions clone [n];
         max_iter >= 2 iterates the update (at most max_iter linearisations, converged at max |delta_{i+1} - delta_i| <= tol).
+        landmark [n] with Sigma_L (see landmark_map_struct): msckf_b200_map_landmark_update, each landmark's map error
+        marginalised over its observations.
         The result as a dict with the per-observation "gamma" and "flag" arrays"""
         a, keep = landmark_struct({"clone": clone, "z": z, "p_L": p_L, "R": R, "chi2_obs": chi2_obs, "max_iter": max_iter, "tol": tol})
         out = LandmarkResult()
-        check(lib().msckf_b200_landmark_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_landmark_update")
+        if Sigma_L is None:
+            check(lib().msckf_b200_landmark_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_landmark_update")
+        else:
+            m, mk = landmark_map_struct({"landmark": landmark, "Sigma_L": Sigma_L})
+            check(lib().msckf_b200_map_landmark_update(self.h, C.byref(a), C.byref(m), C.byref(out)), "msckf_b200_map_landmark_update")
         return dict(out.as_dict(), gamma=keep[4] if keep else np.zeros(0), flag=keep[5] if keep else np.zeros(0, np.int32))
 
     def covariance(self):

@@ -12,6 +12,7 @@
 #include <condition_variable>
 #include <cstring>
 #include <functional>
+#include <map>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -216,7 +217,7 @@ struct CtxBase {
   virtual int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) = 0;
   virtual int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) = 0;
   // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
-  virtual int landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) = 0;
+  virtual int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) = 0;
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
@@ -487,7 +488,7 @@ struct Ctx : CtxBase {
   int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) override;
   int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) override;
   int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what);
-  int landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) override;
+  int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
@@ -1600,14 +1601,79 @@ static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_resul
                   offsetof(mb::LmkOut, step) == offsetof(msckf_b200_landmark_result, step),
               "mb::LmkOut must have msckf_b200_landmark_result's fields at their offsets");
 template <class S>
-int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result* out) {
+int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "landmark_update: null argument");
   RC(members_ready("landmark_update"));
   const int nf = (int)eng.size();
-  struct LmkPlan { std::vector<int> perm, grp; int G = 0, ld = 0; size_t in_off = 0, res_off = 0, ws_off = 0, it_off = 0; };
+  struct LmkPlan {
+    std::vector<int> perm, grp;
+    int G = 0, ld = 0;
+    size_t in_off = 0, res_off = 0, ws_off = 0, it_off = 0;
+    // map uncertainty: the clone-set groups, each observation's pair (-1: a one-clone landmark), the groups' landmarks
+    std::vector<int> sdesc, pair_of, lms;
+    int H = 0, pairs = 0;
+    size_t map_in = 0, map_ws = 0, E_len = 0, B_len = 0;
+  };
   std::vector<LmkPlan> pl(nf);
   std::vector<int> idx;
   size_t in_bytes = 0, res_bytes = 0, ws_bytes = 0;
+  // Sigma_L given: check the landmark ids and covariances, count the one-clone landmarks' observations per clone (single),
+  // and group the landmarks seen from 2 .. 8 clones by their exact clone set (sets in ascending order, landmarks ascending)
+  auto lmk_map_plan = [&](const msckf_b200_landmarks& q, const msckf_b200_landmark_map& mq, const std::string& who, LmkPlan& p, std::vector<int>& single) {
+    const int nl = mq.n_landmarks, no = q.n_obs;
+    if (!mq.landmark || nl < 1) return fail(MSCKF_B200_ERR_ARG, "landmark_update: Sigma_L without landmark ids" + who);
+    if (!finite(mq.Sigma_L, 6 * (size_t)nl)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: non-finite Sigma_L" + who);
+    // positive definite with room to spare: every squared pivot of the Cholesky factor >= 1e-30 m^2 and >= 1e-12 x the largest
+    // diagonal entry, so that k_lmk_set's L^-1 (entries up to 1e15 / m) is finite and meaningful
+    for (int l = 0; l < nl; ++l) {
+      const double* s = mq.Sigma_L + 6 * (size_t)l;
+      const double a = s[0], b = s[2] - s[1] * s[1] / a;
+      const double c = s[4] - s[3] * s[1] / a;
+      const double d = s[5] - s[3] * s[3] / a - c * c / b, floor = std::max(1e-30, 1e-12 * std::max(s[0], std::max(s[2], s[5])));
+      if (!(a >= floor) || !(b >= floor) || !(d >= floor))
+        return fail(MSCKF_B200_ERR_ARG, "landmark_update: Sigma_L of landmark " + std::to_string(l) +
+                                            " is not positive definite (pivots >= 1e-30 and >= 1e-12 x its largest variance)" + who);
+    }
+    std::vector<std::vector<int>> of(nl);  // observations of each landmark, in input order
+    for (int j = 0; j < no; ++j) {
+      if (mq.landmark[j] < 0 || mq.landmark[j] >= nl) return fail(MSCKF_B200_ERR_ARG, "landmark_update: landmark id outside 0 .. n_landmarks - 1" + who);
+      of[mq.landmark[j]].push_back(j);
+    }
+    std::map<std::vector<int>, std::vector<int>> sets;
+    for (int l = 0; l < nl; ++l) {
+      if (of[l].empty()) continue;
+      std::vector<int> cs;
+      for (int j : of[l]) {
+        if (memcmp(q.p_L_G + 3 * (size_t)j, q.p_L_G + 3 * (size_t)of[l][0], sizeof(double) * 3) != 0)
+          return fail(MSCKF_B200_ERR_ARG, "landmark_update: p_L_G differs within landmark " + std::to_string(l) + who);
+        cs.push_back(q.clone[j]);
+      }
+      std::sort(cs.begin(), cs.end());
+      if (std::adjacent_find(cs.begin(), cs.end()) != cs.end())
+        return fail(MSCKF_B200_ERR_ARG, "landmark_update: landmark " + std::to_string(l) + " observed twice from one clone" + who);
+      if ((int)cs.size() > mb::kLmkMapClones) return fail(MSCKF_B200_ERR_ARG, "landmark_update: a landmark seen from more than 8 clones" + who);
+      if (cs.size() == 1) ++single[cs[0]];
+      else sets[cs].push_back(l);
+    }
+    if ((int)sets.size() > mb::kLmkMaxSets) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 clone sets" + who);
+    p.pair_of.assign(no, -1);
+    for (const auto& [cs, ls] : sets) {
+      const int c = (int)cs.size(), nlg = (int)ls.size();
+      if (c * nlg > mb::kLmkMaxPerSet) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 observations in one clone set" + who);
+      std::vector<int> d(mb::kLmkSetDesc, 0);
+      d[0] = c; d[1] = nlg; d[2] = p.pairs; d[3] = (int)p.lms.size(); d[4] = (int)p.E_len; d[5] = (int)p.B_len;
+      std::copy(cs.begin(), cs.end(), d.begin() + 8);
+      p.sdesc.insert(p.sdesc.end(), d.begin(), d.end());
+      for (int jl = 0; jl < nlg; ++jl)
+        for (int j : of[ls[jl]]) p.pair_of[j] = p.pairs + jl * c + (int)(std::lower_bound(cs.begin(), cs.end(), q.clone[j]) - cs.begin());
+      p.lms.insert(p.lms.end(), ls.begin(), ls.end());
+      p.pairs += c * nlg;
+      p.E_len += (size_t)nlg * (3 + 2 * c) * (6 * c + 4);
+      p.B_len += (size_t)2 * c * nlg * (6 * c + 1);
+      ++p.H;
+    }
+    return 0;
+  };
   for (int i = 0; i < nf; ++i) {
     const msckf_b200_landmarks& q = in[i];
     const std::string who = " (member " + std::to_string(i) + ")";
@@ -1627,16 +1693,31 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
       return fail(MSCKF_B200_ERR_ARG, "landmark_update: R is not finite and positive definite" + who);
     if (std::isnan(q.chi2_obs)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: chi2_obs is NaN" + who);
     LmkPlan& p = pl[i];
+    const msckf_b200_landmark_map* mq = map && map[i].Sigma_L ? &map[i] : nullptr;
+    std::vector<int> single(M, 0);  // observations of one-clone landmarks per clone (all of them without Sigma_L)
+    if (mq) RC(lmk_map_plan(q, *mq, who, p, single));
+    else single = cnt;
     p.perm.resize(no);
     std::vector<int> first(M + 1, 0);
     for (int k = 0; k < M; ++k) first[k + 1] = first[k] + cnt[k];
     std::vector<int> fill(first.begin(), first.end() - 1);
     for (int j = 0; j < no; ++j) p.perm[fill[q.clone[j]]++] = j;  // stable: input order inside a clone
     for (int k = 0; k < M; ++k)
-      if (cnt[k]) { p.grp.insert(p.grp.end(), {k, first[k], cnt[k]}); p.ld += std::min(2 * cnt[k], 6); }
+      if (cnt[k]) { p.grp.insert(p.grp.end(), {k, first[k], cnt[k]}); p.ld += std::min(2 * single[k], 6); }
     p.G = (int)p.grp.size() / 3;
+    for (int h = 0; h < p.H; ++h) {
+      const int* D = &p.sdesc[mb::kLmkSetDesc * h];
+      p.ld += std::min(2 * D[0] * D[1], 6 * D[0]);
+    }
+    if (p.ld > mb::kLmkMaxRows)
+      return fail(MSCKF_B200_ERR_ARG, "landmark_update: the compressed system may exceed " + std::to_string(mb::kLmkMaxRows) + " rows" + who);
     p.in_off = in_bytes;
     in_bytes += up16(sizeof(double) * 5 * (size_t)no) + up16(sizeof(int) * p.grp.size());
+    if (mq) {  // Sigma of each observation's landmark, its pair, the group table, Sigma of the groups' landmarks
+      p.map_in = in_bytes;
+      in_bytes += up16(sizeof(double) * 6 * (size_t)no) + up16(sizeof(int) * (size_t)no) + up16(sizeof(int) * p.sdesc.size()) +
+                  up16(sizeof(double) * 6 * p.lms.size());
+    }
     p.res_off = res_bytes;
     res_bytes += up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no) + up16(sizeof(int) * (size_t)no);
     p.ws_off = ws_bytes;
@@ -1645,6 +1726,10 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
       p.it_off = ws_bytes;
       ws_bytes += up256(sizeof(double) * (7 * (size_t)M + n) + sizeof(mb::LmkIt));
     }
+    if (mq) {  // the pairs, the elimination and group rows, the groups' slots
+      p.map_ws = ws_bytes;
+      ws_bytes += up256(sizeof(double) * ((size_t)mb::kLmkPair * p.pairs + p.E_len + p.B_len + (size_t)mb::kLmkSetSlot * p.H));
+    }
     idx.push_back(i);
   }
   if (idx.empty()) return 0;
@@ -1652,7 +1737,7 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
   CK(cudaSetDevice(device));
   RC(io.ensure(res_base + res_bytes, stream));
   RC(ws.ensure(ws_bytes, stream));
-  std::vector<mb::LmkItArgs<S>> args(nf);
+  std::vector<mb::LmkMapArgs<S>> args(nf);
   for (int i : idx) {
     const msckf_b200_landmarks& q = in[i];
     const LmkPlan& p = pl[i];
@@ -1665,8 +1750,33 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
     }
     const size_t goff = p.in_off + up16(sizeof(double) * 5 * (size_t)no);
     memcpy(io.h + goff, p.grp.data(), sizeof(int) * p.grp.size());
-    mb::LmkItArgs<S> a;
+    mb::LmkMapArgs<S> a;
+    memset(&a, 0, sizeof(a));
     static_cast<mb::LmkArgs<S>&>(a) = eng[i]->lmk_args(q, p.G, p.ld);
+    if (map && map[i].Sigma_L) {
+      const msckf_b200_landmark_map& mq = map[i];
+      const size_t o_sig = p.map_in, o_wr = o_sig + up16(sizeof(double) * 6 * (size_t)no), o_sd = o_wr + up16(sizeof(int) * (size_t)no),
+                   o_ls = o_sd + up16(sizeof(int) * p.sdesc.size());
+      double* hs = reinterpret_cast<double*>(io.h + o_sig);
+      int* hw = reinterpret_cast<int*>(io.h + o_wr);
+      for (int j = 0; j < no; ++j) {
+        const int s = p.perm[j];
+        memcpy(hs + 6 * j, mq.Sigma_L + 6 * (size_t)mq.landmark[s], sizeof(double) * 6);
+        hw[j] = p.pair_of[s];
+      }
+      memcpy(io.h + o_sd, p.sdesc.data(), sizeof(int) * p.sdesc.size());
+      double* hl = reinterpret_cast<double*>(io.h + o_ls);
+      for (size_t l = 0; l < p.lms.size(); ++l) memcpy(hl + 6 * l, mq.Sigma_L + 6 * (size_t)p.lms[l], sizeof(double) * 6);
+      a.sig = reinterpret_cast<const double*>(io.d + o_sig);
+      a.wrow = reinterpret_cast<const int*>(io.d + o_wr);
+      a.sdesc = reinterpret_cast<const int*>(io.d + o_sd);
+      a.lsig = reinterpret_cast<const double*>(io.d + o_ls);
+      a.pair = reinterpret_cast<double*>(ws.d + p.map_ws);
+      a.E = a.pair + (size_t)mb::kLmkPair * p.pairs;
+      a.B = a.E + p.E_len;
+      a.sslot = a.B + p.B_len;
+      a.H = p.H;
+    }
     a.max_iter = q.max_iter; a.tol = q.tol;
     a.xi = nullptr; a.d = nullptr; a.it = nullptr;
     if (q.max_iter > 1) {
@@ -1692,19 +1802,34 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, msckf_b200_landmark_result
              [&](const auto& a, int nm) {
                constexpr int NM = (int)std::extent<decltype(std::decay_t<decltype(a)>::m)>::value;
                mb::Members<mb::LmkArgs<S>, NM> b;  // the single linearisation's arguments, as they always were
-               int gx = 1, tx = 1, K = 1;  // the largest member's grid; other members' CTAs past their own range exit at once
+               mb::Members<mb::LmkItArgs<S>, NM> c;  // the iterated form's
+               int gx = 1, tx = 1, K = 1, hx = 0;  // the largest member's grid; other members' CTAs past their own range exit at once
                for (int j = 0; j < nm; ++j) {
                  b.m[j] = a.m[j];
+                 c.m[j] = a.m[j];
                  gx = std::max(gx, a.m[j].G);
                  tx = std::max(tx, a.m[j].ntiles);
                  K = std::max(K, a.m[j].max_iter);
+                 if (a.m[j].sig) hx = std::max(hx, std::max(1, a.m[j].H));
                }
-               mb::k_lmk_clone<S, NM><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(b);
-               mb::k_lmk_gain<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(b);
-               for (int it = 0; it + 1 < K; ++it) {
-                 mb::k_lmk_step<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(a, it);
-                 mb::k_lmk_clone<S, NM, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
-                 mb::k_lmk_gain<S, NM, true><<<nm, mb::kLmkThreads, 0, stream>>>(a);
+               if (hx == 0) {  // no member has Sigma_L: the exact-map launches
+                 mb::k_lmk_clone<S, NM><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(b);
+                 mb::k_lmk_gain<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(b);
+                 for (int it = 0; it + 1 < K; ++it) {
+                   mb::k_lmk_step<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(c, it);
+                   mb::k_lmk_clone<S, NM, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(c);
+                   mb::k_lmk_gain<S, NM, true><<<nm, mb::kLmkThreads, 0, stream>>>(c);
+                 }
+               } else {
+                 mb::k_lmk_clone<S, NM, false, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
+                 mb::k_lmk_set<S, NM><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(a);
+                 mb::k_lmk_gain<S, NM, false, true><<<nm, mb::kLmkThreads, 0, stream>>>(a);
+                 for (int it = 0; it + 1 < K; ++it) {
+                   mb::k_lmk_step<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(c, it);
+                   mb::k_lmk_clone<S, NM, true, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
+                   mb::k_lmk_set<S, NM, true><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(a);
+                   mb::k_lmk_gain<S, NM, true, true><<<nm, mb::kLmkThreads, 0, stream>>>(a);
+                 }
                }
                mb::k_lmk_downdate<S, NM><<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(b);
              });
@@ -1904,7 +2029,12 @@ int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_
 }
 int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
-  return b->ctx->landmarks(lm, out);
+  return b->ctx->landmarks(lm, nullptr, out);
+}
+int msckf_b200_batch_map_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                         msckf_b200_landmark_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->landmarks(lm, map, out);
 }
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,
@@ -1951,7 +2081,14 @@ int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks*
   if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
   const bool it_ok = lm->max_iter >= 0 && lm->max_iter <= mb::kLmkMaxIter && std::isfinite(lm->tol) && lm->tol >= 0.0;
   if (lm->n_obs == 0 && it_ok) { memset(out, 0, sizeof(*out)); return 0; }
-  return e->impl->solo_ctx()->landmarks(lm, out);
+  return e->impl->solo_ctx()->landmarks(lm, nullptr, out);
+}
+int msckf_b200_map_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                   msckf_b200_landmark_result* out) {
+  if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  const bool it_ok = lm->max_iter >= 0 && lm->max_iter <= mb::kLmkMaxIter && std::isfinite(lm->tol) && lm->tol >= 0.0;
+  if (lm->n_obs == 0 && it_ok) { memset(out, 0, sizeof(*out)); return 0; }
+  return e->impl->solo_ctx()->landmarks(lm, map, out);
 }
 int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->impl->set_covariance(in); }
 int msckf_b200_get_counters(msckf_b200_engine* e, long long* counters) { return e->impl->get_counters(counters); }

@@ -16,6 +16,11 @@
 // x^ [+] delta_{i+1} (fp64); k_lmk_clone<..., true> relinearises there with linearisation 0's flags, adding X~ e_k (e_k: delta_i of
 // clone k) to the whitened residual, and k_lmk_gain<..., true> refactors against the same prior P without touching the NIS.
 // k_lmk_downdate then applies the last W, y.  P and the resident state are not written before the downdate.
+// Map uncertainty (MAP: Sigma_L given, DESIGN.md 4.12): each landmark's position error dp_l ~ N(0, Sigma_l) is marginalised
+// over its observations in the call.  k_lmk_clone<..., MAP> gates with X P_kk X^T + F Sigma F^T + R (F = J C) and whitens a
+// one-clone landmark by R + F Sigma F^T before the clone's QR; k_lmk_set eliminates the landmarks seen from 2 .. 8 clones and
+// compresses each group of one clone set; k_lmk_gain<..., MAP> gathers a row over its group's clone blocks.  A chunk with a
+// Sigma_L member launches clone, set, gain (and step, clone, set, gain per extra linearisation), then the same downdate.
 // One body for a single filter (NM = 1) and a device batch (NM = kBatchMembers), like k_aid.  Each member's arithmetic depends
 // only on its own inputs: a batch equals single calls bit for bit.
 #pragma once
@@ -86,8 +91,33 @@ struct LmkItArgs : LmkArgs<S> {
   int max_iter;  // linearisations; <= 1: the member does not iterate and every iteration kernel returns at once
 };
 static_assert(sizeof(Members<LmkItArgs<double>, kBatchMembers>) <= 32764, "the iterated landmark kernels' arguments exceed the parameter limit");
-template <class S, bool IT>
-using LmkArgsT = std::conditional_t<IT, LmkItArgs<S>, LmkArgs<S>>;
+// Map uncertainty (MAP, Sigma_L given): a landmark seen from one clone (so by one observation) is whitened with
+// R + F Sigma F^T inside k_lmk_clone; the observations of a landmark seen from c >= 2 clones leave k_lmk_clone as row pairs,
+// whitened by L_R, and k_lmk_set marginalises each landmark and compresses each group of landmarks with one clone set.
+constexpr int kLmkMapClones = 8;                       // clones that see one landmark
+constexpr int kLmkMaxPerSet = 256;                     // observations of one clone-set group
+constexpr int kLmkMaxSets = 256;                       // clone-set groups of one member
+constexpr int kLmkMaxRows = 6 * kMaxKeep;              // rows of the compressed system (k_lmk_gain's row table)
+constexpr int kLmkSetLd = 6 * kLmkMapClones;           // T_g row stride
+constexpr int kLmkSetSlot = kLmkSetLd * (kLmkSetLd + 1) + 8;  // doubles per group: T [48][48], rho [48], e^2, used, q
+constexpr int kLmkPair = 16;                           // doubles per row pair: [X~ | r~] (2 x 7), flag
+constexpr int kLmkSetDesc = 16;                        // ints per group: c, landmarks, first pair, first landmark,
+                                                       // E offset, B offset, 2 spare, clones [8] (window order)
+template <class S>
+struct LmkMapArgs : LmkItArgs<S> {
+  const double* sig;   // [n_obs][6] Sigma of each observation's landmark (packed order), or NULL: an exact-map member
+  const int* wrow;     // [n_obs] the observation's pair (a landmark seen from >= 2 clones), or -1
+  const int* sdesc;    // [H][kLmkSetDesc]
+  const double* lsig;  // [landmarks of the groups][6] Sigma, group by group
+  double* pair;        // [pairs][kLmkPair] (k_lmk_clone -> k_lmk_set)
+  double* E;           // per landmark [3 + 2c][6c + 4]: prior rows, then its used rows [X~ | r~ | F~]
+  double* B;           // per group [2 obs][6c + 1]: the marginalised rows [X~' | r~']
+  double* sslot;       // [H][kLmkSetSlot]
+  int H;
+};
+static_assert(sizeof(Members<LmkMapArgs<double>, kBatchMembers>) <= 32764, "the map landmark kernels' arguments exceed the parameter limit");
+template <class S, bool IT, bool MAP = false>
+using LmkArgsT = std::conditional_t<MAP, LmkMapArgs<S>, std::conditional_t<IT, LmkItArgs<S>, LmkArgs<S>>>;
 
 __host__ __device__ constexpr int lmk_tiles(int n) { return ((n + kLmkNB - 1) / kLmkNB) * ((n + kLmkNB - 1) / kLmkNB + 1) / 2; }
 
@@ -125,10 +155,33 @@ __device__ __forceinline__ double lmk_obs(const double* o, const double* Cr, con
   return gam;
 }
 
+// Ri += F Sigma F^T with F = J C, the observation's block over the landmark position (= -X[:, 3:6]); Ri unchanged behind the
+// camera (lmk_obs flags that).  sg: Sigma's lower triangle xx, yx, yy, zx, zy, zz.
+__device__ __forceinline__ void lmk_map_R(const double* o, const double* Cr, const double* pc, const double* sg, double (&Ri)[3]) {
+  const double d[3] = {o[2] - pc[0], o[3] - pc[1], o[4] - pc[2]};
+  double p[3];
+  for (int i = 0; i < 3; ++i) p[i] = Cr[3 * i] * d[0] + Cr[3 * i + 1] * d[1] + Cr[3 * i + 2] * d[2];
+  if (!(p[2] > 0.0)) return;
+  const double iz = 1.0 / p[2];
+  const double J[2][3] = {{iz, 0.0, -p[0] / p[2] * iz}, {0.0, iz, -p[1] / p[2] * iz}};
+  const double Sm[3][3] = {{sg[0], sg[1], sg[3]}, {sg[1], sg[2], sg[4]}, {sg[3], sg[4], sg[5]}};
+  double F[2][3], FS[2][3];
+  for (int r = 0; r < 2; ++r)
+    for (int c = 0; c < 3; ++c) F[r][c] = J[r][0] * Cr[c] + J[r][1] * Cr[3 + c] + J[r][2] * Cr[6 + c];
+  for (int r = 0; r < 2; ++r)
+    for (int c = 0; c < 3; ++c) FS[r][c] = F[r][0] * Sm[0][c] + F[r][1] * Sm[1][c] + F[r][2] * Sm[2][c];
+  Ri[0] += FS[0][0] * F[0][0] + FS[0][1] * F[0][1] + FS[0][2] * F[0][2];
+  Ri[1] += FS[1][0] * F[0][0] + FS[1][1] * F[0][1] + FS[1][2] * F[0][2];
+  Ri[2] += FS[1][0] * F[1][0] + FS[1][1] * F[1][1] + FS[1][2] * F[1][2];
+}
+
 // IT: the iterate form.  The clone pose comes from the iterate table, the flags are linearisation 0's (gamma and flag are not
 // written), X~ e_k is added to the whitened residual, and a used observation that fails at the iterate raises the stop word.
-template <class S, int NM, bool IT = false>
-__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgsT<S, IT>, NM> a) {
+// MAP: gamma includes F Sigma F^T; a one-clone landmark's rows are whitened by the Cholesky factor of R + F Sigma F^T (exact
+// marginalisation of its position), and the rows of a landmark seen from several clones go to its pair (whitened by L_R, with
+// the flag) instead of the clone's QR.  A member without Sigma runs the exact-map arithmetic.
+template <class S, int NM, bool IT = false, bool MAP = false>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgsT<S, IT, MAP>, NM> a) {
   const int f = NM == 1 ? 0 : blockIdx.y, g = blockIdx.x;
   if constexpr (IT) {
     if (a.m[f].max_iter <= 1 || lmk_it_ended(a.m[f].it)) return;
@@ -173,6 +226,50 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   // kept in registers across the compaction)
   double row[2][7];
   int fg = 2;
+  if constexpr (MAP) {
+    double Ri[3] = {Rm[0], Rm[1], Rm[2]};
+    const double* sg = a.m[f].sig;
+    const int wr = sg && t < cnt ? a.m[f].wrow[i0 + t] : -1;
+    if (t < cnt) {
+      if (sg) lmk_map_R(obs, Cr, pc, sg + 6 * (size_t)(i0 + t), Ri);
+      const double gam = lmk_obs(obs, Cr, pc, Pk, Ri, chi2, row, fg);
+      if constexpr (IT) {
+        const int f0 = a.m[f].flag[i0 + t];
+        if (f0 == 0 && fg == 2) a.m[f].it->stop = 1;
+        fg = f0;
+      } else {
+        a.m[f].gamma[i0 + t] = gam;
+        a.m[f].flag[i0 + t] = fg;
+      }
+      if (wr >= 0) a.m[f].pair[(size_t)kLmkPair * wr + 14] = (double)fg;
+      fl[t] = wr >= 0 && fg == 0 ? 3 : fg;  // 3: used, in a pair
+    }
+    __syncthreads();
+    if (t == 0) {
+      int u = 0;
+      for (int i = 0; i < cnt; ++i) { pos[i] = u; u += fl[i] == 0; }
+      s_used = u;
+    }
+    __syncthreads();
+    if (t < cnt && fg == 0) {
+      lmk_obs(obs, Cr, pc, Pk, Ri, chi2, row, fg);
+      double l0 = LR[0], l1 = LR[1], l2 = LR[2];
+      if (sg && wr < 0) { l0 = sqrt(Ri[0]); l1 = Ri[1] / l0; l2 = sqrt(Ri[2] - l1 * l1); }
+      for (int c = 0; c < 7; ++c) {
+        row[0][c] /= l0;
+        row[1][c] = (row[1][c] - l1 * row[0][c]) / l2;
+      }
+      if constexpr (IT) {
+        for (int c = 0; c < 6; ++c) { row[0][6] += row[0][c] * ek[c]; row[1][6] += row[1][c] * ek[c]; }
+      }
+      if (wr >= 0) {
+        double* pr = a.m[f].pair + (size_t)kLmkPair * wr;
+        for (int c = 0; c < 7; ++c) { pr[c] = row[0][c]; pr[7 + c] = row[1][c]; }
+      } else {
+        for (int c = 0; c < 7; ++c) { Q[2 * pos[t]][c] = row[0][c]; Q[2 * pos[t] + 1][c] = row[1][c]; }
+      }
+    }
+  } else {
   if (t < cnt) {
     const double gam = lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
     if constexpr (IT) {
@@ -208,6 +305,7 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
         Q[2 * pos[t] + 1][c] = (row[1][c] - LR[1] * y0) / LR[2];
       }
     }
+  }
   }
   __syncthreads();
   // ---- Householder QR of the used rows (one warp): R's first q rows are [T_k | rho_k], rows q.. of column 6 give e_k^2
@@ -249,10 +347,141 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   }
 }
 
+// One CTA per (clone-set group h, member): for each landmark of the group (one warp each), the 3 prior rows [0 | L_S^-1 | 0]
+// (Sigma = L_S L_S^T) over its used rows [X~ | r~ | F~] (F~ = -X~[:, 3:6]) and three Householder reflectors on the F columns;
+// its rows below the prior rows are then [X~' | r~'] with noise I, the exact marginalisation of its position.  Then one
+// Householder QR of the group's rows over its 6c clone columns: q = min(2 used, 6c) rows [T_g | rho_g] and e_g^2 to the slot.
+template <class S, int NM, bool IT = false>
+__global__ void __launch_bounds__(kLmkThreads, 1) k_lmk_set(const Members<LmkMapArgs<S>, NM> a) {
+  const int f = NM == 1 ? 0 : blockIdx.y, h = blockIdx.x;
+  if constexpr (IT) {
+    if (a.m[f].max_iter <= 1 || lmk_it_ended(a.m[f].it)) return;
+  }
+  if (h >= a.m[f].H) return;
+  const int* const D = a.m[f].sdesc + kLmkSetDesc * h;
+  const int c = D[0], nl = D[1], p0 = D[2], l0 = D[3], w = 6 * c, ne = w + 4, nb = w + 1, er = 3 + 2 * c;
+  const double* __restrict__ const pair = a.m[f].pair;
+  double* const E = a.m[f].E + D[4];
+  double* const B = a.m[f].B + D[5];
+  const int t = threadIdx.x, lane = t & 31, wp = t >> 5;
+  __shared__ int uo[kLmkMaxPerSet / 2 + 1];  // used observations before each landmark
+  __shared__ double s_al, s_tau;
+  __shared__ int s_ok;
+  if (t == 0) {
+    int u = 0;
+    for (int j = 0; j < nl; ++j) {
+      uo[j] = u;
+      for (int b = 0; b < c; ++b) u += pair[(size_t)kLmkPair * (p0 + j * c + b) + 14] == 0.0;
+    }
+    uo[nl] = u;
+  }
+  __syncthreads();
+  // ---- per landmark: each lane owns one row of E_j
+  for (int j = wp; j < nl; j += kLmkThreads / 32) {
+    const int nr = 3 + 2 * (uo[j + 1] - uo[j]);
+    if (nr == 3) continue;
+    double* const Ej = E + (size_t)j * er * ne;
+    double* const er_ = Ej + (size_t)lane * ne;
+    if (lane < 3) {  // row lane of L_S^-1
+      const double* sg = a.m[f].lsig + 6 * (size_t)(l0 + j);
+      const double L00 = sqrt(sg[0]), L10 = sg[1] / L00, L20 = sg[3] / L00;
+      const double L11 = sqrt(sg[2] - L10 * L10), L21 = (sg[4] - L20 * L10) / L11;
+      const double L22 = sqrt(sg[5] - L20 * L20 - L21 * L21);
+      const double I00 = 1.0 / L00, I11 = 1.0 / L11, I22 = 1.0 / L22, I10 = -L10 * I00 / L11, I21 = -L21 * I11 / L22;
+      const double I20 = -(L20 * I00 + L21 * I10) / L22;
+      for (int col = 0; col <= w; ++col) er_[col] = 0.0;
+      er_[w + 1] = lane == 0 ? I00 : lane == 1 ? I10 : I20;
+      er_[w + 2] = lane == 0 ? 0.0 : lane == 1 ? I11 : I21;
+      er_[w + 3] = lane == 2 ? I22 : 0.0;
+    } else if (lane < nr) {  // half (lane - 3) & 1 of the ((lane - 3) >> 1)-th used observation
+      int k = (lane - 3) >> 1, b = 0;
+      for (;; ++b)
+        if (pair[(size_t)kLmkPair * (p0 + j * c + b) + 14] == 0.0 && k-- == 0) break;
+      const double* src = pair + (size_t)kLmkPair * (p0 + j * c + b) + 7 * ((lane - 3) & 1);
+      for (int col = 0; col < w; ++col) er_[col] = (col / 6 == b) ? src[col - 6 * b] : 0.0;
+      er_[w] = src[6];
+      er_[w + 1] = -src[3]; er_[w + 2] = -src[4]; er_[w + 3] = -src[5];
+    }
+    __syncwarp();
+    for (int jj = 0; jj < 3; ++jj) {
+      const int cj = w + 1 + jj;
+      double v = (lane >= jj && lane < nr) ? er_[cj] : 0.0;
+      const double s = warp_sum(v * v), x0 = __shfl_sync(0xffffffffu, v, jj);
+      if (!(s > 0.0)) continue;
+      const double al = x0 >= 0.0 ? -sqrt(s) : sqrt(s), tau = 1.0 / (s - al * x0);
+      if (lane == jj) v = x0 - al;
+      for (int col = 0; col < ne; ++col) {
+        if (col > w && col <= cj) continue;
+        const double dd = tau * warp_sum((lane >= jj && lane < nr) ? v * er_[col] : 0.0);
+        if (lane >= jj && lane < nr) er_[col] -= dd * v;
+      }
+    }
+    if (lane >= 3 && lane < nr)
+      for (int col = 0; col <= w; ++col) B[(size_t)(2 * uo[j] + lane - 3) * nb + col] = er_[col];
+  }
+  __syncthreads();
+  // ---- Householder QR of the group's 2 used rows over 6c + 1 columns (warp 0 forms each reflector, all warps apply it)
+  const int nr = 2 * uo[nl], q = min(nr, w);
+  for (int j = 0; j < q; ++j) {
+    if (wp == 0) {
+      double s = 0.0;
+      for (int r = j + lane; r < nr; r += 32) s += B[(size_t)r * nb + j] * B[(size_t)r * nb + j];
+      s = warp_sum(s);
+      if (lane == 0) {
+        const double x0 = B[(size_t)j * nb + j];
+        s_ok = s > 0.0;
+        if (s > 0.0) {
+          s_al = x0 >= 0.0 ? -sqrt(s) : sqrt(s);
+          s_tau = 1.0 / (s - s_al * x0);
+          B[(size_t)j * nb + j] = x0 - s_al;
+        }
+      }
+    }
+    __syncthreads();
+    if (s_ok) {
+      for (int col = j + 1 + wp; col < nb; col += kLmkThreads / 32) {
+        double dd = 0.0;
+        for (int r = j + lane; r < nr; r += 32) dd += B[(size_t)r * nb + j] * B[(size_t)r * nb + col];
+        dd = s_tau * warp_sum(dd);
+        for (int r = j + lane; r < nr; r += 32) B[(size_t)r * nb + col] -= dd * B[(size_t)r * nb + j];
+      }
+    }
+    __syncthreads();
+    if (t == 0 && s_ok) B[(size_t)j * nb + j] = s_al;
+    __syncthreads();
+  }
+  double* const sl = a.m[f].sslot + (size_t)kLmkSetSlot * h;
+  for (int i = t; i < q * w; i += kLmkThreads) {
+    const int r = i / w, col = i - r * w;
+    sl[kLmkSetLd * r + col] = col >= r ? B[(size_t)r * nb + col] : 0.0;
+  }
+  for (int r = t; r < q; r += kLmkThreads) sl[kLmkSetLd * kLmkSetLd + r] = B[(size_t)r * nb + w];
+  if (wp == 0) {
+    double e2 = 0.0;
+    for (int r = q + lane; r < nr; r += 32) e2 += B[(size_t)r * nb + w] * B[(size_t)r * nb + w];
+    e2 = warp_sum(e2);
+    if (lane == 0) {
+      double* tl = sl + kLmkSetLd * (kLmkSetLd + 1);
+      tl[0] = e2; tl[1] = (double)uo[nl]; tl[2] = (double)q;
+    }
+  }
+}
+
+// the T row lr of group g of a MAP member (g < G: clone slot g, else clone-set slot g - G): its first entry, width and clones
+template <class A>
+__device__ __forceinline__ const double* lmk_map_row(const A& m0, const double* slot, const int* grp, int G, int g, int lr, int& w,
+                                                    const int*& cl) {
+  if (g < G) { w = 6; cl = grp + 3 * g; return slot + (size_t)kLmkSlot * g + 6 * lr; }
+  const int* D = m0.sdesc + kLmkSetDesc * (g - G);
+  w = 6 * D[0]; cl = D + 8;
+  return m0.sslot + (size_t)kLmkSetSlot * (g - G) + kLmkSetLd * lr;
+}
+
 // IT: the iterate form.  A raised stop word ends the iteration with nothing written (the previous W, y stay); otherwise the
 // factorisation is today's, and only apply, iterations and (S not positive definite) the status are written.
-template <class S, int NM, bool IT = false>
-__global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT<S, IT>, NM> a) {
+// MAP: the rows of the clone-set groups follow the clones' rows, and a T row spans its group's 6c clone columns.
+template <class S, int NM, bool IT = false, bool MAP = false>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT<S, IT, MAP>, NM> a) {
   const int f = NM == 1 ? 0 : blockIdx.x;
   if constexpr (IT) {
     if (a.m[f].max_iter <= 1 || lmk_it_ended(a.m[f].it)) return;
@@ -263,10 +492,28 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
   LmkCtl* const ctl = a.m[f].ctl;
   LmkOut* const out = a.m[f].out;
   const int ldp = a.m[f].ldp, G = a.m[f].G, ld = a.m[f].ld, n = 15 + 6 * a.m[f].M, t = threadIdx.x;
-  __shared__ int off[kMaxKeep + 1], ck[kMaxKeep], rg[6 * kMaxKeep];
+  __shared__ int off[(MAP ? kMaxKeep + kLmkMaxSets : kMaxKeep) + 1], ck[MAP ? 1 : kMaxKeep], rg[kLmkMaxRows];
   __shared__ double s_e2;
   __shared__ int s_used;
+  int Gt = G;  // groups: the clones, then (MAP) the clone sets
 
+  if constexpr (MAP) {
+    Gt = G + a.m[f].H;
+    if (t == 0) {
+      int o = 0, u = 0;
+      double e2 = 0.0;
+      for (int g = 0; g < Gt; ++g) {  // e^2, used, q of each slot
+        const double* tl = g < G ? slot + (size_t)kLmkSlot * g + 42
+                                 : a.m[f].sslot + (size_t)kLmkSetSlot * (g - G) + kLmkSetLd * (kLmkSetLd + 1);
+        off[g] = o;
+        o += (int)tl[2];
+        u += (int)tl[1];
+        e2 += tl[0];
+      }
+      off[Gt] = o; s_used = u; s_e2 = e2;
+      ctl->ticket = 0u; ctl->bad = 0; ctl->m = o;
+    }
+  } else {
   if (t == 0) {
     int o = 0, u = 0;
     double e2 = 0.0;
@@ -280,8 +527,9 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
     ctl->ticket = 0u; ctl->bad = 0; ctl->m = o;
   }
   for (int g = t; g < G; g += kLmkThreads) ck[g] = a.m[f].grp[3 * g];
+  }
   __syncthreads();
-  const int m = off[G];
+  const int m = off[Gt];
   if (s_used == 0) {  // no observation used: nothing is written (the iterate form never gets here: k_lmk_step stops it)
     if (!IT && t == 0) {
       ctl->apply = 0;
@@ -290,9 +538,40 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
     }
     return;
   }
-  for (int g = t; g < G; g += kLmkThreads)
+  for (int g = t; g < Gt; g += kLmkThreads)
     for (int r = off[g]; r < off[g + 1]; ++r) rg[r] = g;
   __syncthreads();
+  if constexpr (MAP) {  // the same products over each row's clone columns
+    const int* const grp = a.m[f].grp;
+    for (int idx = t; idx < m * n; idx += kLmkThreads) {
+      const int r = idx / n, c = idx - r * n, g = rg[r], lr = r - off[g];
+      int w;
+      const int* cl;
+      const double* T = lmk_map_row(a.m[f], slot, grp, G, g, lr, w, cl);
+      double s = 0.0;
+      for (int j = lr; j < w; ++j) s += T[j] * (double)P[(size_t)(15 + 6 * cl[j / 6] + j % 6) * ldp + c];
+      A[(size_t)(m + c) * ld + r] = s;
+    }
+    for (int r = t; r < m; r += kLmkThreads) {
+      int w;
+      const int* cl;
+      const double* T = lmk_map_row(a.m[f], slot, grp, G, rg[r], 0, w, cl);
+      A[(size_t)(m + n) * ld + r] = T[(rg[r] < G ? 36 : kLmkSetLd * kLmkSetLd) + r - off[rg[r]]];
+    }
+    __syncthreads();
+    for (int idx = t; idx < m * m; idx += kLmkThreads) {
+      const int r = idx / m, s_ = idx - r * m;
+      if (s_ > r) continue;
+      const int h = rg[s_], ls = s_ - off[h];
+      int w;
+      const int* cl;
+      const double* T = lmk_map_row(a.m[f], slot, grp, G, h, ls, w, cl);
+      const double* tp = A + (size_t)(m + 15) * ld + r;
+      double v = r == s_ ? 1.0 : 0.0;
+      for (int j = ls; j < w; ++j) v += tp[(size_t)(6 * cl[j / 6] + j % 6) * ld] * T[j];
+      A[(size_t)r * ld + s_] = v;
+    }
+  } else {
   // ---- (T P)^T into rows m .. m + n - 1, rho into row m + n
   for (int idx = t; idx < m * n; idx += kLmkThreads) {
     const int r = idx / n, c = idx - r * n, g = rg[r], lr = r - off[g];
@@ -314,6 +593,7 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
     double v = r == s_ ? 1.0 : 0.0;
     for (int j = ls; j < 6; ++j) v += tp[(size_t)j * ld] * T[j];
     A[(size_t)r * ld + s_] = v;
+  }
   }
   __syncthreads();
   // ---- Cholesky of [S ; (T P)^T ; rho^T] (m + n + 1 rows): the extra rows end as W^T and y

@@ -68,6 +68,14 @@ def marginalize_batch(filters, threads=8):
     f0._chk(f0._f("marginalize_batch")(arr, C.c_int(len(filters)), C.c_int(int(threads))), "marginalize_batch")
 
 
+
+def _tri6(Sigma):
+    """covariances [L, 3, 3] or [L, 6] as contiguous lower triangles xx, yx, yy, zx, zy, zz [L, 6]"""
+    S = np.asarray(Sigma, dtype=np.float64)
+    if S.ndim == 3:
+        S = S[:, [0, 1, 1, 2, 2, 2], [0, 0, 1, 0, 1, 2]]
+    return np.ascontiguousarray(S.reshape(-1, 6))
+
 class FilterBatch:
     """msckf_mono::MSCKFBatch<_S> through the C view: a persistent device batch over engine filters of one dtype."""
 
@@ -145,6 +153,37 @@ class FilterBatch:
         out = (AidResult * n)()
         self._call("aid_stack_update", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), out)
         return [o.as_dict() if s else None for s, o in zip(stacks, out)]
+
+    def map_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
+        """MSCKFBatch::landmarkUpdate over mapObservation / mapLandmark: obs[i] = (state_ids [n], landmark [n], z [n, 2],
+        p_L [L, 3], Sigma [L, 6] or [L, 3, 3]) for filter i, or None (left alone); one device call for the batch.  A list of
+        result dicts with "gamma" and "flag" (None for a filter left alone)."""
+        from .capi import LandmarkResult
+        n = len(self.filters)
+        assert len(obs) == n
+        cnt = np.array([0 if o is None else len(o[0]) for o in obs], dtype=np.int32)
+        nl = np.array([0 if o is None or not len(o[0]) else len(np.asarray(o[3]).reshape(-1, 3)) for o in obs], dtype=np.int32)
+        parts = [o for o in obs if o is not None and len(o[0])]
+
+        def cat(i, w, dt):
+            return np.ascontiguousarray(np.concatenate([np.asarray(o[i], dt).reshape(-1, w) for o in parts]) if parts
+                                        else np.zeros((1, w)), dtype=dt)
+        ids, lm, z, p = cat(0, 1, np.int32), cat(1, 1, np.int32), cat(2, 2, float), cat(3, 3, float)
+        S = np.ascontiguousarray(np.concatenate([_tri6(o[4]) for o in parts]) if parts else np.zeros((1, 6)))
+        r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
+        tot = max(int(cnt.sum()), 1)
+        gamma, flag = np.zeros(tot), np.zeros(tot, dtype=np.int32)
+        out = (LandmarkResult * n)()
+        self._call("map_update", cnt.ctypes.data_as(_ip), ids.ctypes.data_as(_ip), lm.ctypes.data_as(_ip), z.ctypes.data_as(_dp),
+                   nl.ctypes.data_as(_ip), p.ctypes.data_as(_dp), S.ctypes.data_as(_dp), None if r3 is None else r3.ctypes.data_as(_dp),
+                   C.c_double(chi2_obs), C.c_int(int(max_iter)), C.c_double(tol), gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip),
+                   out)
+        res, o0 = [], 0
+        for i in range(n):
+            c = int(cnt[i])
+            res.append(None if c == 0 else dict(out[i].as_dict(), gamma=gamma[o0:o0 + c].copy(), flag=flag[o0:o0 + c].copy()))
+            o0 += c
+        return res
 
     def landmark_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
         """MSCKFBatch::landmarkUpdate: obs[i] = (state_ids [n], z [n, 2], p_L [n, 3]) for filter i, or None (filter i left
@@ -375,6 +414,26 @@ class CFilter:
         self._chk(self._f("relative_pose_update")(self.h, C.c_int(int(state_id_a)), C.c_int(int(state_id_b)), pp, pq, pR,
                                                   C.c_double(chi2_max), C.byref(out)), "relative_pose_update")
         return out.as_dict()
+
+    def map_update(self, state_ids, landmark, z, p_L, Sigma, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
+        """MSCKF::landmarkUpdate over mapObservation / mapLandmark (msckf_b200_map_landmark_update): observations z [n, 2] from
+        the images state_ids [n] of the landmarks landmark [n] (indices into p_L [L, 3] and Sigma [L, 6] lower triangles or
+        [L, 3, 3]); each landmark's map error is marginalised over its observations.  The result dict of landmark_update."""
+        from .capi import LandmarkResult
+        ids = np.ascontiguousarray(state_ids, dtype=np.int32).ravel()
+        lm = np.ascontiguousarray(landmark, dtype=np.int32).ravel()
+        n = len(ids)
+        z, pz = _d(np.asarray(z, float).reshape(-1, 2) if n else np.zeros((1, 2)))
+        p, pp = _d(np.asarray(p_L, float).reshape(-1, 3))
+        S, ps = _d(_tri6(Sigma))
+        r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
+        gamma, flag = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int32)
+        out = LandmarkResult()
+        self._chk(self._f("map_update")(self.h, C.c_int(n), ids.ctypes.data_as(_ip), lm.ctypes.data_as(_ip), pz, C.c_int(len(p)), pp,
+                                        ps, None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs),
+                                        C.c_int(int(max_iter)), C.c_double(tol), gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip),
+                                        C.byref(out)), "map_update")
+        return dict(out.as_dict(), gamma=gamma[:n].copy(), flag=flag[:n].copy())
 
     def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
         """MSCKF::landmarkUpdate (include/msckf_b200.h: msckf_b200_landmark_update): observations of known landmarks p_L [n, 3]

@@ -221,12 +221,17 @@ def map_observations(truth, frame, stride):
     return idx, np.stack([xn[idx], yn[idx]], axis=1)
 
 
-def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0, map_start=0):
+def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0, map_start=0, map_sigma=0.0,
+               map_clones=1):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
     fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
     map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks, None
     before frame map_start (the map noise of those frames is still drawn, so a frame's map is the same for every map_start).  With
-    odo_every > 0, "odometry" holds per frame None or the 9 standard normals of that frame's odometry noise (odometry_items)."""
+    odo_every > 0, "odometry" holds per frame None or the 9 standard normals of that frame's odometry noise (odometry_items).
+    map_sigma > 0: the trial's map ("map_points", and the p_L of "maps") is the truth map plus N(0, map_sigma^2 I), drawn once
+    from np.random.default_rng([seed, k, 4]).  map_clones K > 1 (K <= map_every): a map frame also observes the map from the
+    K - 1 frames before it, and its entry gets a fourth array, how many frames back each observation is (0: the newest); their
+    pixel noise comes from np.random.default_rng([seed, k, 5]), so the newest frame's noise is the same for every K."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -261,8 +266,14 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
         out["fixes"] = [truth["truth_imu"][f][0:3] + fix_sigma * frng.standard_normal(3) if (f + 1) % fix_every == 0 else None
                         for f in range(len(truth["frames"]))]
     if map_every > 0:
+        assert 1 <= map_clones <= map_every, "map_clones must be 1 .. map_every (no clone is observed twice)"
         mrng = np.random.default_rng([seed, k, 2])
+        crng = np.random.default_rng([seed, k, 5])  # pixel noise of the older clones' map observations (map_clones > 1)
         su, sv = np.sqrt(nz["u_var_prime"]), np.sqrt(nz["v_var_prime"])
+        pts = truth["landmarks"][::map_stride]
+        if map_sigma > 0:
+            pts = pts + map_sigma * np.random.default_rng([seed, k, 4]).standard_normal(pts.shape)
+            out["map_points"] = pts
         out["maps"] = []
         for f in range(len(truth["frames"])):
             if (f + 1) % map_every:
@@ -270,7 +281,15 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
                 continue
             idx, z = map_observations(truth, f, map_stride)
             z = z + mrng.standard_normal(z.shape) * np.array([su, sv])
-            out["maps"].append((idx, truth["landmarks"][::map_stride][idx], z) if f >= map_start else None)
+            if map_clones > 1:
+                parts = [(idx, z, np.zeros(len(idx), dtype=int))]
+                for j in range(1, min(map_clones, f + 1)):
+                    ij, zj = map_observations(truth, f - j, map_stride)
+                    parts.append((ij, zj + crng.standard_normal(zj.shape) * np.array([su, sv]), np.full(len(ij), j)))
+                idx, z, ago = (np.concatenate([q[i] for q in parts]) for i in range(3))
+                out["maps"].append((idx, pts[idx], z.reshape(-1, 2), ago) if f >= map_start else None)
+            else:
+                out["maps"].append((idx, pts[idx], z) if f >= map_start else None)
     if odo_every > 0:
         orng = np.random.default_rng([seed, k, 3])
         out["odometry"] = [orng.standard_normal(9) if (f + 1) % odo_every == 0 else None for f in range(len(truth["frames"]))]
@@ -384,20 +403,45 @@ def summarize(records):
 
 
 # ---- the batched run ---------------------------------------------------------------------------------------------------------
+def map_call(tr, f, fi, uncertain, S):
+    """one filter's map observations at frame fi: (state_ids, z, p_L) for landmark_update or, uncertain, (state_ids, landmark,
+    z, p_L, Sigma) for map_update with each distinct landmark once and Sigma = S; only clones still in the window; None when
+    nothing is left"""
+    m = tr["maps"][fi]
+    idx, p, z = m[0], m[1], m[2]
+    ago = m[3] if len(m) > 3 else np.zeros(len(idx), dtype=int)
+    ids = np.array([tr["frames"][fi - a]["state_id"] for a in ago], dtype=np.int64)
+    keep = np.isin(ids, f.getCamStates()["state_id"]) if len(m) > 3 else np.ones(len(idx), dtype=bool)
+    if not keep.any():
+        return None
+    ids, idx, p, z = ids[keep], idx[keep], p[keep], z[keep]
+    if not uncertain:
+        return ids, z, p
+    u, first, inv = np.unique(idx, return_index=True, return_inverse=True)
+    return ids, inv, z, p[first], np.repeat(S, len(u), axis=0)
+
+
 def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0,
-        odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False, map_start=0, map_iterations=1):
+        odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False, map_start=0, map_iterations=1, map_sigma=0.0,
+        map_uncertain=False, map_clones=1):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
     [every map_every frames from frame map_start on, one batched mapped-landmark update from the newest clone, gated per
-    observation at map_chi2 > 0, iterated up to map_iterations linearisations],
+    observation at map_chi2 > 0, iterated up to map_iterations linearisations; the map carries N(0, map_sigma^2 I) errors and
+    is observed from the map_clones newest clones that are still in the window (make_trial); map_uncertain passes
+    Sigma = map_sigma^2 I per landmark (MSCKFBatch::landmarkUpdate over mapObservation / mapLandmark), else the map is taken as
+    exact],
     refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.  The first
     map update is also recorded on its own (trial_record's map_first; the state is read just before it).
     Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
     from . import engine_filter
     from .capi import AID_POSITION
     from .cview import FilterBatch
-    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start) for k in trials]
+    assert not map_uncertain or map_sigma > 0, "map_uncertain needs map_sigma > 0"
+    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start, map_sigma, map_clones)
+           for k in trials]
+    S_map = np.tile([map_sigma ** 2, 0.0, map_sigma ** 2, 0.0, 0.0, map_sigma ** 2], (1, 1))
     first = [None for _ in trs]
     R_fix = (fix_sigma ** 2) * np.eye(3)
     nis = [[] for _ in trs]
@@ -436,13 +480,15 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             for i, r in enumerate(fb.aid_stack_update(stacks)):
                 odo[i].append(r)
         if map_every > 0 and trs[0]["maps"][fi] is not None:
-            obs = [(np.full(len(tr["maps"][fi][0]), fr["state_id"]), tr["maps"][fi][2], tr["maps"][fi][1]) if len(tr["maps"][fi][0]) else None
-                   for tr, fr in zip(trs, frs)]
+            obs = [map_call(tr, f, fi, map_uncertain, S_map) for tr, f in zip(trs, fs)]
             if first[0] is None:
                 fb.refreshState()
                 for i, (f, tr) in enumerate(zip(fs, trs)):
                     first[i] = {"frame": fi, "pos_err2_before": float(np.sum((truth_imu_of(truth, tr, fi)[0:3] - f.getImuState()["p_I_G"]) ** 2))}
-            res = fb.landmark_update(obs, chi2_obs=map_chi2, max_iter=map_iterations)
+            if map_uncertain:
+                res = fb.map_update(obs, chi2_obs=map_chi2, max_iter=map_iterations)
+            else:
+                res = fb.landmark_update(obs, chi2_obs=map_chi2, max_iter=map_iterations)
             for i, r in enumerate(res):
                 maps[i].append({"nis": 0.0, "dof": 0, "used": 0, "applied": 0, "n": 0} if r is None else dict(r, n=len(r["flag"])))
                 if first[i]["frame"] == fi:

@@ -7,7 +7,9 @@ available without it: get_state, the projection linearised in numpy, then one ai
 iterated update instead: 25 observations over the newest clone and 100 over the newest 5, seen from poses 0.3 m away, at each
 max_iter K with tol 0 (so every call makes its K linearisations unless a step is exactly zero), for 1 / 8 / 32 filters, with the
 linearisations the calls reported and the per-kernel split (k_lmk_step too) for 100 over 5.  Reads the card's name and power
-limit in the same process.  Prints one JSON line."""
+limit in the same process.  With --map-sigma S, it times the update with map uncertainty instead: 25 and 100 landmarks, each
+seen from the newest 1 and 5 clones, with Sigma = S^2 I (msckf_b200_map_landmark_update) against the same observations with
+Sigma NULL, for 1 / 8 / 32 filters.  Prints one JSON line."""
 import argparse
 import json
 import subprocess
@@ -110,7 +112,7 @@ def kernel_times(fn, reps=50):
         torch.cuda.synchronize()
     out = {}
     for ev in prof.key_averages():
-        for name in ("k_lmk_clone", "k_lmk_gain", "k_lmk_step", "k_lmk_downdate"):
+        for name in ("k_lmk_clone", "k_lmk_set", "k_lmk_gain", "k_lmk_step", "k_lmk_downdate"):
             if name in ev.key:
                 out[name] = out.get(name, 0.0) + ev.device_time_total / 1e3 / reps  # ms per call
     return out
@@ -147,12 +149,58 @@ def iterated(ks):
     print(json.dumps(res), flush=True)
 
 
+def map_spec(rng, e, n_lm, n_clones, sigma):
+    """n_lm landmarks in front of the newest clone, each observed exactly from n_clones consecutive clones (the newest ones, or
+    for odd landmarks with n_clones > 1 the ones before the newest, so no clone set holds more than 256 observations), with
+    Sigma = sigma^2 I (the exact-map call when sigma is None)"""
+    _, poses = e.state()
+    poses = poses.astype(np.float64)
+    p = observations(rng, e, n_lm, 1)["p_L"]
+    clone, z, p_L, lm = [], [], [], []
+    for l in range(n_lm):
+        last = M - (l % 2 if n_clones > 1 else 0)
+        for k in range(last - n_clones, last):
+            pc = rot(poses[k, 3:7]) @ (p[l] - poses[k, 0:3])
+            clone.append(k); z.append(pc[0:2] / pc[2]); p_L.append(p[l]); lm.append(l)
+    spec = {"clone": np.array(clone, np.int32), "z": np.array(z), "p_L": np.array(p_L), "R": R_PIX}
+    if sigma is not None:
+        spec.update(landmark=np.array(lm, np.int32), Sigma_L=np.tile([sigma ** 2, 0, sigma ** 2, 0, 0, sigma ** 2], (n_lm, 1)))
+    return spec
+
+
+def uncertain(sigma):
+    res = {"gpu": gpu_line(), "dtype": "f64", "clones": M, "map_sigma_m": sigma, "call_ms": {}, "kernel_ms": {}}
+    for nf in (1, 8, 32):
+        fs, es = filters(nf)
+        b = capi.Batch(es) if nf > 1 else None
+        for n_lm in (25, 100):
+            for nc in (1, 5):
+                for tag, s in (("NULL", None), ("Sigma", sigma)):
+                    specs = [map_spec(np.random.default_rng([n_lm, nc, i]), e, n_lm, nc, s) for i, e in enumerate(es)]
+                    fn = (lambda: b.landmark_update(specs)) if b else (lambda: es[0].landmark_update(**specs[0]))
+                    key = f"{nf}x{n_lm}landmarks/{nc}clones/{tag}"
+                    res["call_ms"][key] = timed(fn)
+                    if nf in (1, 32) and n_lm == 100 and nc == 5:
+                        try:
+                            res["kernel_ms"][key] = kernel_times(fn)
+                        except Exception as ex:  # (the profiler is an extra; the call times above stand on their own)
+                            res["kernel_ms"][key] = f"not measured: {ex}"
+        if b:
+            b.close()
+        for f in fs:
+            f.close()
+    print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iterations", type=int, nargs="*", default=None)
+    ap.add_argument("--map-sigma", type=float, default=None, help="time Sigma = s^2 I against Sigma NULL")
     args = ap.parse_args()
     if args.iterations:
         return iterated(args.iterations)
+    if args.map_sigma is not None:
+        return uncertain(args.map_sigma)
     rng = np.random.default_rng(3)
     res = {"gpu": gpu_line(), "dtype": "f64", "clones": M, "call_ms": {}, "host_linear_ms": {}, "kernel_ms": {}}
     for nf in (1, 8, 32):

@@ -15,6 +15,8 @@ its newest clone and fuses the observations as mapped landmarks (after the prune
 the map updates' ANIS against its 95 % chi^2 bounds and the fraction of observations gated out.  --map-start F observes the map
 only from frame F on (relocalisation after drift), --map-iterations K iterates each map update (at most K linearisations), and
 the summary then adds the first map update: the position RMSE before and after it, its ANIS and the IMU-state ANEES after it.
+--map-sigma S gives each trial a map with N(0, S^2 I) errors per landmark, --map-uncertain fuses it with Sigma = S^2 I (map
+error marginalised per landmark) instead of as exact, and --map-clones K observes the map from the K newest clones.
 
 With --odometry-every K, every K frames each trial also fuses one stacked odometry update (the truth body velocity, and the
 truth relative pose of its two newest clones, each plus noise of --odometry-sigma-v m/s and --odometry-sigma-rel m / rad;
@@ -134,6 +136,9 @@ def main():
     ap.add_argument("--map-stride", type=int, default=20)
     ap.add_argument("--map-start", type=int, default=0)
     ap.add_argument("--map-iterations", type=int, default=1)
+    ap.add_argument("--map-sigma", type=float, default=0.0, help="each trial's map = the truth map + N(0, s^2 I) per landmark")
+    ap.add_argument("--map-uncertain", action="store_true", help="fuse the map with Sigma = s^2 I (else it is taken as exact)")
+    ap.add_argument("--map-clones", type=int, default=1, help="observe the map from the K newest clones (K <= --map-every)")
     ap.add_argument("--odometry-every", type=int, default=0)
     ap.add_argument("--odometry-sigma-v", type=float, default=0.05)
     ap.add_argument("--odometry-sigma-rel", type=float, default=0.01)
@@ -155,7 +160,8 @@ def main():
                         fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma, map_every=args.map_every,
                         map_stride=args.map_stride, odo_every=args.odometry_every, odo_sigma_v=args.odometry_sigma_v,
                         odo_sigma_rel=args.odometry_sigma_rel, nhc=args.nhc, map_start=args.map_start,
-                        map_iterations=args.map_iterations)
+                        map_iterations=args.map_iterations, map_sigma=args.map_sigma, map_uncertain=args.map_uncertain,
+                        map_clones=args.map_clones)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -168,6 +174,7 @@ def main():
     if "map" in s:
         res["map"] = {"every": args.map_every, "stride": args.map_stride,
                       **{k: s["map"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "observations", "gated")}}
+        res["map"].update(sigma_m=args.map_sigma, uncertain=args.map_uncertain, clones=args.map_clones)
         if args.map_start or args.map_iterations != 1:
             res["map"].update(start=args.map_start, iterations=args.map_iterations, first_update=s["map_first"])
     if "odometry" in s:
