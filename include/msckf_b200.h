@@ -214,7 +214,11 @@ enum msckf_b200_aid_model {
   MSCKF_B200_AID_CLONE_POSE = 3,
   MSCKF_B200_AID_LINEAR = 4,
   MSCKF_B200_AID_BODY_VELOCITY = 5, /* stacks only (msckf_b200_aid_stack_update) */
-  MSCKF_B200_AID_RELATIVE_POSE = 6  /* stacks only */
+  MSCKF_B200_AID_RELATIVE_POSE = 6, /* stacks only */
+  MSCKF_B200_AID_ANTENNA_POSITION = 7,       /* stacks only: GNSS */
+  MSCKF_B200_AID_CLONE_ANTENNA_POSITION = 8, /* stacks only */
+  MSCKF_B200_AID_HEADING = 9,                /* stacks only */
+  MSCKF_B200_AID_CLONE_HEADING = 10          /* stacks only */
 };
 typedef struct {
   int model;          /* msckf_b200_aid_model; in a batch, < 0 leaves that member untouched */
@@ -230,7 +234,8 @@ typedef struct {
   double dx_norm;     /* |dx| of the applied update (0 when not applied) */
   int dof;            /* m */
   int applied;        /* 1: P and the state were updated */
-  int status;         /* 0: applied or gated out (see applied); 1: S not positive definite, nothing written */
+  int status;         /* 0: applied or gated out (see applied); 1: S not positive definite, nothing written; 2 (stacks
+                         only): a HEADING / CLONE_HEADING axis within ~1e-3 rad of vertical (yaw undefined), nothing written */
 } msckf_b200_aid_result;
 /* A bad model, an out-of-window clone, an m / n mismatch, a NULL or non-finite z / H / R or a zero quaternion returns
  * MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.  A non-finite dx or P entry returns
@@ -251,17 +256,35 @@ int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, 
  *                  C^ = C_b C_a^T (q^ = q_b * q_a^-1) and p^ = C_a (p_C_G,b - p_C_G,a); r = [dtheta(q_z, q^); z_p - p^] with the
  *                  dtheta of POSE.  H is non-zero over the two clones' [dtheta, dp].  (Odometry between the IMU state and a
  *                  clone is not a model: convert it to camera frames with q_CI and p_C_I.)
+ * GNSS and heading models (satellite navigation, a second antenna, a magnetometer or a compass), with C = C(q_IG) and p = p_I_G,
+ * or C = C(q_CG) and p = p_C_G of clone k for the CLONE_ forms -- a fix whose epoch lies behind the IMU's time is fused exactly at
+ * the clone of that epoch's image:
+ *   ANTENNA_POSITION        a = row mask (1..7), z = p_A_G (3), lever arm l (3) in the IMU frame; p^ = p + C^T l and
+ *                           r = z - p^ over the rows of the mask (0b100 with l = 0: an altitude; 0b011: a horizontal fix).
+ *                           H is non-zero over dtheta (-C^T [l]x) and dp (12..14).
+ *   CLONE_ANTENNA_POSITION  a = clone k, b = row mask; z as above with l in that clone's camera frame; H over its [dtheta, dp].
+ *   HEADING                 z = psi (1), axis f (3) in the IMU frame: d = C^T f, psi^ = atan2(d_y, d_x) (yaw of f in G),
+ *                           r = z - psi^ wrapped into (-pi, pi]; one row over dtheta.  When d_x^2 + d_y^2 <= 1e-6 |f|^2 (f within
+ *                           ~1e-3 rad of vertical) yaw is undefined: the stack writes nothing and reports status 2, NIS NaN.
+ *   CLONE_HEADING           a = clone k; z as HEADING with f in that clone's camera frame; one row over its dtheta.
+ *   A and b that a model does not use must be 0.  (A lever arm or an axis given in the IMU frame, l_I or f_I, is converted to
+ *   camera frames with the engine's q_CI and p_C_I (the camera's position in the IMU frame: p_C_G = p_I_G + C(q_IG)^T p_C_I,
+ *   C(q_CG) = C(q_CI) C(q_IG)): l_C = C(q_CI) (l_I - p_C_I), f_C = C(q_CI) f_I.)
  * C(q) is Eigen's toRotationMatrix (C(q_CG) maps G to the camera frame).  LINEAR is not allowed in a stack.  R of an item is its
- * own rows x rows block (3, 3, 6, 6, popcount(mask), 6 rows), row-major, lower triangle read. */
+ * own rows x rows block (3, 3, 6, 6, popcount(mask), 6, popcount(mask), popcount(mask), 1, 1 rows), row-major, lower triangle
+ * read; the struct carries no size, so a caller that passes another size is not caught here (the class forms check it). */
 typedef struct {
   int model;          /* msckf_b200_aid_model except LINEAR */
-  int a;              /* CLONE_POSE, RELATIVE_POSE: clone position; BODY_VELOCITY: row mask (1..7); else ignored */
-  int b;              /* RELATIVE_POSE: the second clone; else ignored */
-  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components) or 7 doubles */
+  int a;              /* CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING: clone position; BODY_VELOCITY,
+                         ANTENNA_POSITION: row mask (1..7); else ignored (0 for the GNSS and heading models) */
+  int b;              /* RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: row mask (1..7); else ignored (0 for the
+                         GNSS and heading models) */
+  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components), 7, 6 (antenna) or 4 (heading) doubles */
   const double* R;    /* [rows][rows] */
 } msckf_b200_aid_item;
 /* A bad model, a clone outside the window, a == b, an empty mask, more than 8 items or 32 rows, a NULL or non-finite z / R, a zero
- * quaternion or a NaN chi2_max returns MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
+ * quaternion, a zero heading axis, a non-zero unused a / b of a GNSS or heading model or a NaN chi2_max returns
+ * MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
  * A non-finite dx or P entry returns MSCKF_B200_ERR_NUMERIC with the result filled and the update applied.  n_items >= 1. */
 int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,
                                 msckf_b200_aid_result* out);

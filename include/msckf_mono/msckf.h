@@ -383,7 +383,7 @@ class MSCKF {
     return aidedUpdate(a);
   }
   // stacked aided updates (not in the reference; msckf_b200_aid_stack_update): up to 8 items -- odometry (BODY_VELOCITY,
-  // RELATIVE_POSE) and the fixes above -- fused as ONE update with R block-diagonal across items, one NIS over all rows and one
+  // RELATIVE_POSE), GNSS antenna positions and headings (at the IMU or at a clone) and the fixes above -- fused as ONE update with R block-diagonal across items, one NIS over all rows and one
   // chi2_max gate.  Items name clones by window position.  Bookkeeping as aidedUpdate(const msckf_b200_aid&).
   msckf_b200_aid_result aidedUpdate(const std::vector<msckf_b200_aid_item>& items, double chi2_max = 0) {
     msckf_b200_aid_result r = {};
@@ -406,6 +406,41 @@ class MSCKF {
     const int a = windowPosition(state_id_a, "MSCKF::relativePoseUpdate"), b = windowPosition(state_id_b, "MSCKF::relativePoseUpdate");
     const double z[7] = {p(0), p(1), p(2), q.x(), q.y(), q.z(), q.w()};
     return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_RELATIVE_POSE, a, b, 6, z, R)}, chi2_max);
+  }
+  // a GNSS antenna position p_A_G = p_I_G + C(q_IG)^T lever, the lever arm in the IMU frame; mask bits 0..2 select the rows
+  // used (0b100 with a zero lever: an altitude, 0b011: a horizontal fix), R is popcount(mask) square over them
+  msckf_b200_aid_result antennaPositionUpdate(const Vector3<double>& p_A_G, const Vector3<double>& lever, const MatrixX<double>& R,
+                                              int mask = 7, double chi2_max = 0) {
+    if (mask < 1 || mask > 7) throw std::invalid_argument("MSCKF::antennaPositionUpdate: the mask must select rows 0..2");
+    const double z[6] = {p_A_G(0), p_A_G(1), p_A_G(2), lever(0), lever(1), lever(2)};
+    const int m = (mask & 1) + ((mask >> 1) & 1) + ((mask >> 2) & 1);
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_ANTENNA_POSITION, mask, 0, m, z, R)}, chi2_max);
+  }
+  // the same at the clone of image state_id (a delayed fix: the image of the fix's epoch), the lever arm in that clone's camera
+  // frame (l_C = C(q_CI) (l_I - p_C_I)).  An id that is not in the window throws std::invalid_argument before any device call.
+  msckf_b200_aid_result cloneAntennaPositionUpdate(int state_id, const Vector3<double>& p_A_G, const Vector3<double>& lever,
+                                                   const MatrixX<double>& R, int mask = 7, double chi2_max = 0) {
+    const int k = windowPosition(state_id, "MSCKF::cloneAntennaPositionUpdate");
+    if (mask < 1 || mask > 7) throw std::invalid_argument("MSCKF::cloneAntennaPositionUpdate: the mask must select rows 0..2");
+    const double z[6] = {p_A_G(0), p_A_G(1), p_A_G(2), lever(0), lever(1), lever(2)};
+    const int m = (mask & 1) + ((mask >> 1) & 1) + ((mask >> 2) & 1);
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_CLONE_ANTENNA_POSITION, k, mask, m, z, R)}, chi2_max);
+  }
+  // a heading psi (rad): the yaw atan2(d_y, d_x) in G of d = C(q_IG)^T axis, the axis in the IMU frame (a dual-antenna baseline,
+  // a compass's forward axis); var is its variance.  An axis within ~1e-3 rad of vertical gives status 2 and changes nothing.
+  msckf_b200_aid_result headingUpdate(double psi, const Vector3<double>& axis, double var, double chi2_max = 0) {
+    const double z[4] = {psi, axis(0), axis(1), axis(2)};
+    MatrixX<double> R(1, 1);
+    R(0, 0) = var;
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_HEADING, 0, 0, 1, z, R)}, chi2_max);
+  }
+  // the same at the clone of image state_id, the axis in that clone's camera frame (f_C = C(q_CI) f_I)
+  msckf_b200_aid_result cloneHeadingUpdate(int state_id, double psi, const Vector3<double>& axis, double var, double chi2_max = 0) {
+    const int k = windowPosition(state_id, "MSCKF::cloneHeadingUpdate");
+    const double z[4] = {psi, axis(0), axis(1), axis(2)};
+    MatrixX<double> R(1, 1);
+    R(0, 0) = var;
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_CLONE_HEADING, k, 0, 1, z, R)}, chi2_max);
   }
   // the window position of the clone of image state_id (std::invalid_argument when it is not in the window)
   int windowPosition(int state_id, const char* what) const {

@@ -2,7 +2,7 @@
 // Aided measurements fused into the device-resident filter (msckf_b200_aid_update / _batch_aid_update and the stacked
 // msckf_b200_aid_stack_update / _batch_aid_stack_update):
 //   k_aid : residual r and H (a stack of up to 8 model items, each row at most 12 (state index, coefficient) pairs formed from
-//           the resident state; or the caller's r and dense H), H P (sparse gathers over rows of P, or a product for a dense H),
+//           the resident state; or the caller's r and dense H; a degenerate heading item ends the member: status 2), H P (sparse gathers over rows of P, or a product for a dense H),
 //           S = H P H^T + R = L L^T with r as an extra row (y = L^-1 r), W = L^-1 H P, NIS = y^T y, the optional chi-square
 //           gate, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to the filter precision
 //           once) and the state injection of k_syrk (inject_state).  All arithmetic in fp64.
@@ -17,8 +17,10 @@ namespace mb {
 
 // the models of msckf_b200_aid_model (include/msckf_b200.h)
 enum AidModel {
-  kAidVelocity = 0, kAidPosition = 1, kAidPose = 2, kAidClonePose = 3, kAidLinear = 4, kAidBodyVelocity = 5, kAidRelativePose = 6
+  kAidVelocity = 0, kAidPosition = 1, kAidPose = 2, kAidClonePose = 3, kAidLinear = 4, kAidBodyVelocity = 5, kAidRelativePose = 6,
+  kAidAntennaPosition = 7, kAidCloneAntennaPosition = 8, kAidHeading = 9, kAidCloneHeading = 10
 };
+constexpr double kAidHeadingMinHoriz = 1e-6;  // HEADING: d_x^2 + d_y^2 <= this |f|^2 (f within ~1e-3 rad of vertical) is degenerate
 constexpr int kAidMaxRows = 32;      // m <= 32: S is factored by one warp
 constexpr int kAidMaxItems = 8;      // model items of one stack
 constexpr int kAidItemZ = 8;         // doubles reserved for one item's z
@@ -33,8 +35,9 @@ struct AidOut {
   int numeric;  // a non-finite dx or P entry was written
 };
 
-// one item of a stack: its model, a (CLONE_POSE and RELATIVE_POSE: a clone's window position; BODY_VELOCITY: the row mask),
-// b (RELATIVE_POSE: the second clone) and its first row in the stack
+// one item of a stack: its model, a (CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING: a clone's window
+// position; BODY_VELOCITY, ANTENNA_POSITION: the row mask), b (RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: the row
+// mask) and its first row in the stack
 struct AidItem {
   short model, a, b, row;
 };
@@ -64,10 +67,17 @@ __host__ __device__ constexpr size_t aid_ws_bytes(int n, int m) { return sizeof(
 //   RELATIVE_POSE  C^ = C_b C_a^T, q^ = q_b * q_a^-1, p^ = C_a (p_b - p_a) of clones a, b:
 //                  rotation rows  H over dtheta_a -C^, over dtheta_b I, over dp_a and dp_b 0
 //                  position rows  H over dtheta_a [p^]x, over dp_a -C_a, over dtheta_b 0, over dp_b C_a
+//   ANTENNA_POSITION, CLONE_ANTENNA_POSITION  z = p_A_G (3), lever l (3) in the body frame of the IMU or of clone k; with
+//                  C = C(q), d = C^T l: p^ = p + d; row j of the mask: r = z_j - p^_j, H over dtheta -C^T [l]x = -[d]x C^T (row j),
+//                  over dp the unit row j
+//   HEADING, CLONE_HEADING  z = psi (1), axis f (3) in the body frame; d = C^T f, psi^ = atan2(d_y, d_x), r = wrap(z - psi^)
+//                  into (-pi, pi]; H over dtheta [-d_y, d_x, 0] / (d_x^2 + d_y^2) (-[d]x C^T).  d_x^2 + d_y^2 <=
+//                  kAidHeadingMinHoriz |f|^2 (yaw undefined) forms no row and returns 1: k_aid writes nothing (status 2).
+// Returns 0 when the rows are formed.
 // (Out of line, with the item by value: inlined into k_aid<double, 1>, this code made ptxas spill.)
 template <class S>
-__device__ __noinline__ void aid_item_rows(const AidItem it, const double* z, const DevState<S>* st, const S* poses,
-                                              double* r, int (*col)[kAidNnz], double (*coef)[kAidNnz], int* nnz) {
+__device__ __noinline__ int aid_item_rows(const AidItem it, const double* z, const DevState<S>* st, const S* poses,
+                                             double* r, int (*col)[kAidNnz], double (*coef)[kAidNnz], int* nnz) {
   const int r0 = it.row;
   if (it.model == kAidVelocity || it.model == kAidPosition) {
     const S* x = it.model == kAidVelocity ? st->v_I_G : st->p_I_G;
@@ -103,6 +113,50 @@ __device__ __noinline__ void aid_item_rows(const AidItem it, const double* z, co
         nnz[row++] = 6;
       }
     }
+  } else if (it.model >= kAidAntennaPosition) {  // the antenna positions and headings, of the IMU or of clone a
+    const bool clone = it.model == kAidCloneAntennaPosition || it.model == kAidCloneHeading;
+    const bool heading = it.model >= kAidHeading;
+    const S* Q = clone ? poses + kPoseStride * it.a : st->q_IG;
+    const double q[4] = {(double)Q[0], (double)Q[1], (double)Q[2], (double)Q[3]};
+    const double* l = heading ? z + 1 : z + 3;  // the lever arm or the axis, in the body frame
+    const int c0 = clone ? 15 + 6 * it.a : 0;   // the pose's dtheta
+    double C[9], d[3], J[9];
+    quat_to_rot(q, C);
+    for (int i = 0; i < 3; ++i) d[i] = C[i] * l[0] + C[3 + i] * l[1] + C[6 + i] * l[2];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {  // J = -[d]x C^T: column k is (row k of C) x d
+      J[k] = C[3 * k + 1] * d[2] - C[3 * k + 2] * d[1];
+      J[3 + k] = C[3 * k + 2] * d[0] - C[3 * k] * d[2];
+      J[6 + k] = C[3 * k] * d[1] - C[3 * k + 1] * d[0];
+    }
+    if (!heading) {
+      const S* p = clone ? poses + kPoseStride * it.a + 4 : st->p_I_G;
+      const int cp = clone ? c0 + 3 : 12, mask = clone ? it.b : it.a;
+      int row = r0;
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        if ((mask >> j) & 1) {
+          r[row] = z[j] - ((double)p[j] + d[j]);
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            col[row][k] = c0 + k; coef[row][k] = J[3 * j + k];
+            col[row][3 + k] = cp + k; coef[row][3 + k] = j == k ? 1.0 : 0.0;
+          }
+          nnz[row++] = 6;
+        }
+      }
+    } else {
+      const double h = d[0] * d[0] + d[1] * d[1];
+      if (!(h > kAidHeadingMinHoriz * (l[0] * l[0] + l[1] * l[1] + l[2] * l[2]))) return 1;
+      constexpr double kPi = 3.141592653589793, k2Pi = 6.283185307179586;
+      double e = remainder(z[0] - atan2(d[1], d[0]), k2Pi);
+      if (e <= -kPi) e += k2Pi;
+      r[r0] = e;
+      const double gx = -d[1] / h, gy = d[0] / h;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { col[r0][k] = c0 + k; coef[r0][k] = gx * J[k] + gy * J[3 + k]; }
+      nnz[r0] = 3;
+    }
   } else {  // kAidRelativePose
     const S* A = poses + kPoseStride * it.a;
     const S* B = poses + kPoseStride * it.b;
@@ -137,6 +191,7 @@ __device__ __noinline__ void aid_item_rows(const AidItem it, const double* z, co
       nnz[r0 + i] = kAidNnz;
     }
   }
+  return 0;
 }
 
 template <class S, int NM>
@@ -164,12 +219,19 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
   __shared__ int s_nv, s_apply, s_bad;
 
   // ---- residual (fp64) and the rows of H, one thread per item
+  int degenerate = 0;
   if (lin) {
     if (t < m) L[m][t] = in[t];
   } else if (t < a.m[f].n_items) {
-    aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, &L[m][0], s_col, s_coef, s_nnz);
+    degenerate = aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, &L[m][0], s_col, s_coef, s_nnz);
   }
-  __syncthreads();
+  if (__syncthreads_or(degenerate)) {  // a heading whose yaw is undefined: nothing is written
+    if (t == 0) {
+      out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
+      out->dof = m; out->applied = 0; out->status = 2; out->numeric = 0;
+    }
+    return;
+  }
   // ---- H P, stored transposed: Wt[c][i] = (H P)[i][c]
   if (lin) {
     for (int idx = t; idx < m * n; idx += kAidThreads) {

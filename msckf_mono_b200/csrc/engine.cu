@@ -155,18 +155,32 @@ int aid_append(AidJob& j, const msckf_b200_aid_item& q, int M, const std::string
       if (q.a == q.b) return fail(MSCKF_B200_ERR_ARG, w + ": a relative pose needs two different clones" + who);
       m = 6; nz = 7;
       break;
+    case MSCKF_B200_AID_ANTENNA_POSITION: case MSCKF_B200_AID_CLONE_ANTENNA_POSITION:
+    case MSCKF_B200_AID_HEADING: case MSCKF_B200_AID_CLONE_HEADING: {  // (the a / b they do not use must be 0)
+      const bool clone = q.model == MSCKF_B200_AID_CLONE_ANTENNA_POSITION || q.model == MSCKF_B200_AID_CLONE_HEADING;
+      const bool heading = q.model == MSCKF_B200_AID_HEADING || q.model == MSCKF_B200_AID_CLONE_HEADING;
+      if (clone && (q.a < 0 || q.a >= M)) return fail(MSCKF_B200_ERR_ARG, w + ": clone outside the window" + who);
+      const int mask = heading ? 1 : clone ? q.b : q.a;
+      if (mask < 1 || mask > 7) return fail(MSCKF_B200_ERR_ARG, w + ": the row mask must select rows 0..2" + who);
+      if ((!clone && heading && q.a != 0) || (q.model != MSCKF_B200_AID_CLONE_ANTENNA_POSITION && q.b != 0))
+        return fail(MSCKF_B200_ERR_ARG, w + ": a / b the model does not use must be 0" + who);
+      m = (mask & 1) + ((mask >> 1) & 1) + ((mask >> 2) & 1);
+      nz = heading ? 4 : 6;
+      break;
+    }
     default: return fail(MSCKF_B200_ERR_ARG, w + ": model not allowed in a stack" + who);
   }
   if (j.m + m > mb::kAidMaxRows) return fail(MSCKF_B200_ERR_ARG, w + ": more than 32 rows" + who);
   if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, w + ": missing or non-finite z" + who);
   if (nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
     return fail(MSCKF_B200_ERR_ARG, w + ": zero quaternion" + who);
+  if (nz == 4 && !(q.z[1] * q.z[1] + q.z[2] * q.z[2] + q.z[3] * q.z[3] > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": zero heading axis" + who);
   if (!q.R) return fail(MSCKF_B200_ERR_ARG, w + ": missing R" + who);
   for (int r = 0; r < m; ++r)
     if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, w + ": non-finite R" + who);
   const int k = j.n_items++;
   j.item[k] = {(short)q.model, (short)(q.model >= MSCKF_B200_AID_CLONE_POSE ? q.a : 0),  // (LINEAR is not an item model)
-               (short)(q.model == MSCKF_B200_AID_RELATIVE_POSE ? q.b : 0), (short)j.m};
+               (short)(q.model == MSCKF_B200_AID_RELATIVE_POSE || q.model == MSCKF_B200_AID_CLONE_ANTENNA_POSITION ? q.b : 0), (short)j.m};
   j.z[k] = q.z; j.nz[k] = nz; j.R[k] = q.R; j.m += m;
   return 0;
 }
@@ -1475,7 +1489,10 @@ int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_pose
 // else in the workspace.  Nothing is launched unless every member is valid: aid and aid_stack check their arguments and
 // build one AidJob per member, aid_run launches them.
 static_assert(offsetof(mb::AidOut, status) == offsetof(msckf_b200_aid_result, status), "mb::AidOut must start like msckf_b200_aid_result");
-static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && (int)MSCKF_B200_AID_RELATIVE_POSE == (int)mb::kAidRelativePose,
+static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && (int)MSCKF_B200_AID_RELATIVE_POSE == (int)mb::kAidRelativePose &&
+                  (int)MSCKF_B200_AID_ANTENNA_POSITION == (int)mb::kAidAntennaPosition &&
+                  (int)MSCKF_B200_AID_CLONE_ANTENNA_POSITION == (int)mb::kAidCloneAntennaPosition &&
+                  (int)MSCKF_B200_AID_HEADING == (int)mb::kAidHeading && (int)MSCKF_B200_AID_CLONE_HEADING == (int)mb::kAidCloneHeading,
               "msckf_b200_aid_model and mb::AidModel differ");
 constexpr size_t kAidSmemMax = 32 * 1024;
 template <class S>

@@ -33,17 +33,30 @@ rotation buildUpdateQuat-style N(0, odo_sigma_rel^2 I) in radians.  The noise of
 np.random.default_rng([seed, k, 3]), 9 standard normals per odometry frame, so the trial's other inputs are the same with
 odometry on or off.  The NIS of the stacks gives another truth-free consistency figure (ANIS against chi^2 with the stack's rows).
 
+Optional GNSS (satellite navigation with its antenna off the IMU, and a heading): every `gnss_every` frames, after the odometry,
+each trial fuses the truth antenna position p_I_G + C(q_IG)^T lever plus N(0, gnss_sigma^2 I) as ANTENNA_POSITION; every
+`heading_every` frames the truth yaw of the IMU axis `heading_axis` plus N(0, heading_sigma^2) as HEADING; both in ONE stacked
+update per frame (MSCKFBatch::aidedUpdate(items)).  gnss_delay d > 0 fuses, at frame f, the fix and heading of frame f - d at that
+frame's clone (CLONE_ANTENNA_POSITION, CLONE_HEADING, the lever and the axis converted to its camera frame), as a receiver whose
+output arrives d images late; an epoch whose clone has left the window is dropped.  gnss_as_position fuses the antenna position
+as a plain POSITION fix of the IMU, which shows the lever-arm bias.  The noise of trial k comes from its own streams
+np.random.default_rng([seed, k, 6]) (3 standard normals per fix) and [seed, k, 7] (1 per heading), so the trial's other inputs
+are the same with GNSS on or off.  The NIS of the stacks gives another truth-free consistency figure.
+
 Error-state convention (the inverse of the filter's state injection q+ = buildUpdateQuat(dtheta) * q): dq = q_true * q_est^-1
 with the Hamilton product, dq negated when dq.w < 0, dtheta = -2 vec(dq); every other component is truth - estimate.  Host
 vectors here are in the filter's covariance order [dtheta, db_g, dv, db_a, dp, clones (dtheta_C, dp_C)...].
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 from scipy import stats
 
 from . import synth
-from .capi import AID_BODY_VELOCITY, AID_RELATIVE_POSE
+from .capi import (AID_ANTENNA_POSITION, AID_BODY_VELOCITY, AID_CLONE_ANTENNA_POSITION, AID_CLONE_HEADING, AID_HEADING,
+                   AID_POSITION, AID_RELATIVE_POSE)
 
 COMPONENTS = ("orientation", "position", "pose", "imu", "full")
 DOF = {"orientation": 3, "position": 3, "pose": 6, "imu": 15}
@@ -98,8 +111,14 @@ def relative_pose(pose_a, pose_b):
 
 
 def odometry_residual(item, imu, poses):
-    """r of one BODY_VELOCITY or RELATIVE_POSE item (a dict as for capi.aid_items) at the state (imu 19+, poses [M, 7]), in fp64"""
+    """r of one BODY_VELOCITY, RELATIVE_POSE or GNSS item (a dict as for capi.aid_items) at the state (imu 19+, poses [M, 7]),
+    in fp64"""
     z = np.asarray(item["z"], dtype=np.float64)
+    if item["model"] in GNSS_MODELS:
+        q, p, _, rows = _gnss_frame(item, imu, poses)
+        if item["model"] in (AID_HEADING, AID_CLONE_HEADING):
+            return np.array([wrap_angle(z[0] - heading_of(q, z[1:4]))])
+        return (z[0:3] - antenna_position(p, q, z[3:6]))[rows]
     if item["model"] == AID_BODY_VELOCITY:  # the rows of the mask
         return (z - body_velocity(imu))[[j for j in range(3) if (item["a"] >> j) & 1]]
     p, q = relative_pose(poses[item["a"]], poses[item["b"]])
@@ -107,11 +126,24 @@ def odometry_residual(item, imu, poses):
 
 
 def odometry_jacobian(item, imu, poses, n):
-    """H [m, n] of one BODY_VELOCITY or RELATIVE_POSE item in the filter's injection convention, C(q+) = (I - [dtheta]x) C(q):
-    the host linearisation of the models msckf_b200_aid_stack_update forms on the device"""
-    def skew(v):
-        return np.array([[0.0, -v[2], v[1]], [v[2], 0.0, -v[0]], [-v[1], v[0], 0.0]])
+    """H [m, n] of one BODY_VELOCITY, RELATIVE_POSE or GNSS item in the filter's injection convention, C(q+) = (I - [dtheta]x)
+    C(q): the host linearisation of the models msckf_b200_aid_stack_update forms on the device"""
+    skew = _skew
     imu, poses = np.asarray(imu, dtype=np.float64), np.asarray(poses, dtype=np.float64)
+    if item["model"] in GNSS_MODELS:  # d(C^T l) / dtheta = -C^T [l]x
+        q, _, c0, rows = _gnss_frame(item, imu, poses)
+        C = quat_to_rot(q)
+        z = np.asarray(item["z"], dtype=np.float64)
+        if item["model"] in (AID_HEADING, AID_CLONE_HEADING):
+            d = C.T @ z[1:4]
+            H = np.zeros((1, n))
+            H[0, c0:c0 + 3] = np.array([-d[1], d[0], 0.0]) / (d[0] ** 2 + d[1] ** 2) @ (-C.T @ skew(z[1:4]))
+            return H
+        H = np.zeros((len(rows), n))
+        H[:, c0:c0 + 3] = (-C.T @ skew(z[3:6]))[rows]
+        cp = c0 + 3 if item["model"] == AID_CLONE_ANTENNA_POSITION else 12
+        H[:, cp:cp + 3] = np.eye(3)[rows]
+        return H
     if item["model"] == AID_BODY_VELOCITY:
         C = quat_to_rot(imu[15:19])
         rows = [j for j in range(3) if (item["a"] >> j) & 1]
@@ -143,6 +175,78 @@ def odometry_items(truth_imu, pose_a, pose_b, noise, sigma_v, sigma_rel, nhc=Fal
         q = quat_mul(quat_of_error(sigma_rel * noise[6:9]), q)
         items.append({"model": AID_RELATIVE_POSE, "z": np.concatenate([p + sigma_rel * noise[3:6], q / np.linalg.norm(q)]),
                       "R": sigma_rel ** 2 * np.eye(6)})
+    return items
+
+
+# ---- GNSS models (ANTENNA_POSITION, CLONE_ANTENNA_POSITION, HEADING, CLONE_HEADING) ------------------------------------------
+GNSS_MODELS = (AID_ANTENNA_POSITION, AID_CLONE_ANTENNA_POSITION, AID_HEADING, AID_CLONE_HEADING)
+
+
+def _skew(v):
+    return np.array([[0.0, -v[2], v[1]], [v[2], 0.0, -v[0]], [-v[1], v[0], 0.0]])
+
+
+def wrap_angle(x):
+    """x wrapped into (-pi, pi]"""
+    y = math.remainder(float(x), 2.0 * math.pi)
+    return y + 2.0 * math.pi if y <= -math.pi else y
+
+
+def antenna_position(p, q, lever):
+    """p_A_G = p + C(q)^T lever of a body (IMU or camera) at p with orientation q, the lever arm in its frame"""
+    return np.asarray(p, dtype=np.float64) + quat_to_rot(q).T @ np.asarray(lever, dtype=np.float64)
+
+
+def heading_of(q, axis):
+    """the yaw in G, atan2(d_y, d_x), of d = C(q)^T axis, the axis in the body frame"""
+    d = quat_to_rot(q).T @ np.asarray(axis, dtype=np.float64)
+    return math.atan2(d[1], d[0])
+
+
+def _gnss_frame(item, imu, poses):
+    """(q, p, first error-state index of the pose's dtheta, the rows of the mask) of a GNSS item's body"""
+    m = item["model"]
+    if m in (AID_CLONE_ANTENNA_POSITION, AID_CLONE_HEADING):
+        k = item["a"]
+        q, p, c0 = poses[k, 3:7], poses[k, 0:3], 15 + 6 * k
+    else:
+        q, p, c0 = imu[15:19], imu[0:3], 0
+    mask = item["b"] if m == AID_CLONE_ANTENNA_POSITION else item.get("a", 0) if m == AID_ANTENNA_POSITION else 1
+    return np.asarray(q, dtype=np.float64), np.asarray(p, dtype=np.float64), c0, [j for j in range(3) if (mask >> j) & 1]
+
+
+def camera_frame(camera, lever=None, axis=None):
+    """an IMU-frame lever arm (l_C = C(q_CI) (l_I - p_C_I)) or axis (f_C = C(q_CI) f_I) in the camera frame"""
+    C = quat_to_rot(camera["q_CI"])
+    if lever is not None:
+        return C @ (np.asarray(lever, dtype=np.float64) - np.asarray(camera["p_C_I"], dtype=np.float64))
+    return C @ np.asarray(axis, dtype=np.float64)
+
+
+def gnss_items(truth_imu, camera, noise_p, noise_psi, sigma, lever, sigma_psi, axis, clone=None, as_position=False):
+    """the GNSS stack of one epoch as aid item dicts, from the truth IMU state of that epoch: with noise_p (3 standard normals)
+    the antenna position p_I_G + C(q_IG)^T lever plus sigma noise_p, with noise_psi (1) the yaw of the IMU axis `axis` plus
+    sigma_psi noise_psi.  clone = k fuses both at clone k (the lever and the axis in its camera frame); as_position fuses the
+    antenna position as a plain POSITION fix (the lever ignored: the bias it leaves is the point)"""
+    imu = np.asarray(truth_imu, dtype=np.float64)
+    items = []
+    if noise_p is not None:
+        z = antenna_position(imu[0:3], imu[15:19], lever) + sigma * np.asarray(noise_p)
+        R = sigma ** 2 * np.eye(3)
+        if as_position:
+            items.append({"model": AID_POSITION, "z": z, "R": R})
+        elif clone is None:
+            items.append({"model": AID_ANTENNA_POSITION, "a": 0b111, "z": np.r_[z, lever], "R": R})
+        else:
+            items.append({"model": AID_CLONE_ANTENNA_POSITION, "a": clone, "b": 0b111,
+                          "z": np.r_[z, camera_frame(camera, lever=lever)], "R": R})
+    if noise_psi is not None:
+        psi = wrap_angle(heading_of(imu[15:19], axis) + sigma_psi * float(np.asarray(noise_psi).ravel()[0]))
+        R = np.array([[sigma_psi ** 2]])
+        if clone is None:
+            items.append({"model": AID_HEADING, "z": np.r_[psi, axis], "R": R})
+        else:
+            items.append({"model": AID_CLONE_HEADING, "a": clone, "z": np.r_[psi, camera_frame(camera, axis=axis)], "R": R})
     return items
 
 
@@ -222,7 +326,7 @@ def map_observations(truth, frame, stride):
 
 
 def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0, map_start=0, map_sigma=0.0,
-               map_clones=1):
+               map_clones=1, gnss_every=0, heading_every=0):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
     fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
     map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks, None
@@ -231,7 +335,10 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
     map_sigma > 0: the trial's map ("map_points", and the p_L of "maps") is the truth map plus N(0, map_sigma^2 I), drawn once
     from np.random.default_rng([seed, k, 4]).  map_clones K > 1 (K <= map_every): a map frame also observes the map from the
     K - 1 frames before it, and its entry gets a fourth array, how many frames back each observation is (0: the newest); their
-    pixel noise comes from np.random.default_rng([seed, k, 5]), so the newest frame's noise is the same for every K."""
+    pixel noise comes from np.random.default_rng([seed, k, 5]), so the newest frame's noise is the same for every K.  With
+    gnss_every > 0, "gnss" holds per frame (the epoch of that frame) None or the 3 standard normals of its antenna-position noise,
+    from np.random.default_rng([seed, k, 6]); with heading_every > 0, "heading" holds None or 1 standard normal, from
+    np.random.default_rng([seed, k, 7]) (gnss_items)."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -293,6 +400,12 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
     if odo_every > 0:
         orng = np.random.default_rng([seed, k, 3])
         out["odometry"] = [orng.standard_normal(9) if (f + 1) % odo_every == 0 else None for f in range(len(truth["frames"]))]
+    if gnss_every > 0:
+        grng = np.random.default_rng([seed, k, 6])
+        out["gnss"] = [grng.standard_normal(3) if (f + 1) % gnss_every == 0 else None for f in range(len(truth["frames"]))]
+    if heading_every > 0:
+        hrng = np.random.default_rng([seed, k, 7])
+        out["heading"] = [hrng.standard_normal(1) if (f + 1) % heading_every == 0 else None for f in range(len(truth["frames"]))]
     return out
 
 
@@ -304,14 +417,17 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None):
+def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None, gnss_rows=None):
     """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes, of its
     map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n) and of its odometry
     stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists; map_first (a dict of plain numbers: frame,
-    squared position error before and after, nis, dof, iterations, converged) describes the first map update"""
+    squared position error before and after, nis, dof, iterations, converged) describes the first map update; gnss_rows
+    (result dicts of aid_stack_update, dof 0 for an epoch whose clone had left the window) the GNSS stacks"""
     rec = _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows)
     if map_first is not None:
         rec["map_first"] = dict(map_first)
+    if gnss_rows is not None:
+        rec["gnss"] = {key: [float(r[key]) if key == "nis" else int(r[key]) for r in gnss_rows] for key in ("nis", "dof", "applied", "status")}
     return rec
 
 
@@ -399,6 +515,21 @@ def summarize(records):
                            "run_bounds": list(chi2_bounds(int(D.sum()), V.size)),
                            "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])),
                            "applied": float(np.mean([a for o in od for a in o["applied"]]))}
+    gn = [records[k].get("gnss") for k in keys]
+    if all(g is not None and len(g["nis"]) for g in gn):  # ANIS of the GNSS stacks: the stack's rows per trial and epoch fused
+        V = np.array([g["nis"] for g in gn]); D = np.array([g["dof"] for g in gn])
+        used = (D > 0) & np.isfinite(V)  # (a dropped epoch, or status 1 / 2: no NIS)
+        V, D = np.where(used, V, 0.0), np.where(used, D, 0)
+        n_used, dof = used.sum(axis=0), D.sum(axis=0)
+        keep = n_used > 0
+        anis = V.sum(axis=0)[keep] / n_used[keep]
+        lo, hi = zip(*[chi2_bounds(int(d), int(c)) for d, c in zip(dof[keep], n_used[keep])]) if keep.any() else ((), ())
+        out["gnss"] = {"anis": [float(a) for a in anis], "lower": list(lo), "upper": list(hi), "dof": [int(d) for d in dof[keep]],
+                       "mean_anis": float(V.sum() / max(used.sum(), 1)), "mean_dof": float(D.sum() / max(used.sum(), 1)),
+                       "run_bounds": list(chi2_bounds(int(D.sum()), int(used.sum()))) if used.any() else [float("nan")] * 2,
+                       "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])) if keep.any() else float("nan"),
+                       "applied": float(np.mean([a for g, u in zip(gn, used) for a, x in zip(g["applied"], u) if x])) if used.any() else 0.0,
+                       "degenerate": int(sum(s == 2 for g in gn for s in g["status"]))}
     return out
 
 
@@ -423,10 +554,14 @@ def map_call(tr, f, fi, uncertain, S):
 
 def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0,
         odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False, map_start=0, map_iterations=1, map_sigma=0.0,
-        map_uncertain=False, map_clones=1):
+        map_uncertain=False, map_clones=1, gnss_every=0, gnss_sigma=0.1, gnss_lever=(0.0, 0.0, 0.0), gnss_delay=0,
+        gnss_as_position=False, heading_every=0, heading_sigma=0.01, heading_axis=(1.0, 0.0, 0.0)):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
+    [one batched GNSS stack (gnss_items) in a frame whose epoch f - gnss_delay has an antenna fix (every gnss_every frames,
+    lever arm gnss_lever in the IMU frame) or a heading (every heading_every frames, of heading_axis); at the IMU when
+    gnss_delay = 0, else at that epoch's clone while it is in the window],
     [every map_every frames from frame map_start on, one batched mapped-landmark update from the newest clone, gated per
     observation at map_chi2 > 0, iterated up to map_iterations linearisations; the map carries N(0, map_sigma^2 I) errors and
     is observed from the map_clones newest clones that are still in the window (make_trial); map_uncertain passes
@@ -439,8 +574,11 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     from .capi import AID_POSITION
     from .cview import FilterBatch
     assert not map_uncertain or map_sigma > 0, "map_uncertain needs map_sigma > 0"
-    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start, map_sigma, map_clones)
-           for k in trials]
+    assert not (gnss_as_position and gnss_delay), "gnss_as_position fuses at the IMU: no delay"
+    trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start, map_sigma, map_clones,
+                      gnss_every, heading_every) for k in trials]
+    gnss = [[] for _ in trs] if gnss_every > 0 or heading_every > 0 else None
+    lever, axis = np.asarray(gnss_lever, dtype=np.float64), np.asarray(heading_axis, dtype=np.float64)
     S_map = np.tile([map_sigma ** 2, 0.0, map_sigma ** 2, 0.0, 0.0, map_sigma ** 2], (1, 1))
     first = [None for _ in trs]
     R_fix = (fix_sigma ** 2) * np.eye(3)
@@ -479,6 +617,22 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
                 stacks.append(items)
             for i, r in enumerate(fb.aid_stack_update(stacks)):
                 odo[i].append(r)
+        g = fi - gnss_delay  # the epoch whose GNSS output arrives at this frame
+        noise = [(tr["gnss"][g] if "gnss" in tr else None, tr["heading"][g] if "heading" in tr else None) for tr in trs] if g >= 0 else []
+        if gnss is not None and g >= 0 and any(x is not None for x in noise[0]):
+            stacks = []
+            for f, tr, (n_p, n_psi) in zip(fs, trs, noise):
+                clone = None
+                if gnss_delay:
+                    ids = list(f.getCamStates()["state_id"])
+                    if tr["frames"][g]["state_id"] not in ids:  # the epoch's clone has left the window
+                        stacks.append(None)
+                        continue
+                    clone = ids.index(tr["frames"][g]["state_id"])
+                stacks.append(gnss_items(truth["truth_imu"][g], truth["camera"], n_p, n_psi, gnss_sigma, lever, heading_sigma, axis,
+                                         clone, gnss_as_position))
+            for i, r in enumerate(fb.aid_stack_update(stacks)):
+                gnss[i].append({"nis": 0.0, "dof": 0, "applied": 0, "status": 0} if r is None else r)
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [map_call(tr, f, fi, map_uncertain, S_map) for tr, f in zip(trs, fs)]
             if first[0] is None:
@@ -508,7 +662,8 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         if on_frame is not None:
             on_frame(fi, fs, res)
     fb.close()
-    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i]) for i, tr in enumerate(trs)}
+    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i], None if gnss is None else gnss[i])
+               for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):
         s = f.getImuState()

@@ -22,6 +22,12 @@ With --odometry-every K, every K frames each trial also fuses one stacked odomet
 truth relative pose of its two newest clones, each plus noise of --odometry-sigma-v m/s and --odometry-sigma-rel m / rad;
 --nhc keeps only the body velocity's y and z rows), and the summary adds the stacks' ANIS against its 95 % chi^2 bounds.
 
+With --gnss-every K, every K frames each trial also fuses the truth GNSS antenna position (lever arm --gnss-lever X Y Z in the
+IMU frame) plus noise of --gnss-sigma m as ANTENNA_POSITION; --heading-every K adds the truth heading of the IMU's x axis plus
+noise of --heading-sigma rad.  --gnss-delay D fuses the epoch of frame f - D at frame f, at that epoch's clone;
+--gnss-as-position fuses the antenna position as a plain POSITION fix (the lever-arm bias).  The summary adds the GNSS stacks'
+ANIS against its 95 % chi^2 bounds.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -143,6 +149,13 @@ def main():
     ap.add_argument("--odometry-sigma-v", type=float, default=0.05)
     ap.add_argument("--odometry-sigma-rel", type=float, default=0.01)
     ap.add_argument("--nhc", action="store_true")
+    ap.add_argument("--gnss-every", type=int, default=0)
+    ap.add_argument("--gnss-sigma", type=float, default=0.1)
+    ap.add_argument("--gnss-lever", type=float, nargs=3, default=[0.0, 0.0, 0.0], metavar=("X", "Y", "Z"))
+    ap.add_argument("--gnss-delay", type=int, default=0, help="fuse the epoch of frame f - d at its clone (frames)")
+    ap.add_argument("--gnss-as-position", action="store_true", help="fuse the antenna position as a plain POSITION fix")
+    ap.add_argument("--heading-every", type=int, default=0)
+    ap.add_argument("--heading-sigma", type=float, default=0.01)
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -161,7 +174,9 @@ def main():
                         map_stride=args.map_stride, odo_every=args.odometry_every, odo_sigma_v=args.odometry_sigma_v,
                         odo_sigma_rel=args.odometry_sigma_rel, nhc=args.nhc, map_start=args.map_start,
                         map_iterations=args.map_iterations, map_sigma=args.map_sigma, map_uncertain=args.map_uncertain,
-                        map_clones=args.map_clones)
+                        map_clones=args.map_clones, gnss_every=args.gnss_every, gnss_sigma=args.gnss_sigma,
+                        gnss_lever=args.gnss_lever, gnss_delay=args.gnss_delay, gnss_as_position=args.gnss_as_position,
+                        heading_every=args.heading_every, heading_sigma=args.heading_sigma)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -180,6 +195,10 @@ def main():
     if "odometry" in s:
         res["odometry"] = {"every": args.odometry_every, "sigma_v": args.odometry_sigma_v, "sigma_rel": args.odometry_sigma_rel,
                            "nhc": args.nhc, **{k: s["odometry"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied")}}
+    if "gnss" in s:
+        res["gnss"] = {"every": args.gnss_every, "sigma_m": args.gnss_sigma, "lever_m": args.gnss_lever, "delay": args.gnss_delay,
+                       "as_position": args.gnss_as_position, "heading_every": args.heading_every, "heading_sigma": args.heading_sigma,
+                       **{k: s["gnss"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate")}}
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
