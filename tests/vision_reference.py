@@ -2,13 +2,20 @@
 for it.
 
 The update is the one of the engine's RESIDUALIZE mode (pruneRedundantStates, msckf.h:545-614): per track the residual and the
-observability-projected Jacobian of oracle/msckf_numpy.py projected on an orthonormal basis of the left null space of H_f, the
-chi-square gate, then the stacked update.  With isotropic pixel noise (u_var = v_var = sigma^2) every projected noise block is
-sigma^2 I whatever basis is used, so the reference is exact rather than one more implementation:
-  * gamma_j = r~^T (H_o,j P H_o,j^T + sigma^2 I)^-1 r~, accepted when gamma_j < chi2_table[L_j] (msckf.h:1103-1124);
-  * the accepted rows H_o, r_o are compressed by an economic QR H_o = Q_1 T (any such Q_1 gives the same update, R_n = sigma^2 I)
-    and the update uses the innovation S = T P T^T + sigma^2 I >= sigma^2 I: no P^-1, so the filter's own ill-conditioned P works;
-  * P+ in Joseph form, dx = K Q_1^T r_o, and the state injection of msckf_numpy (IMU quaternion not renormalised, clones' are);
+observability-projected Jacobian of oracle/msckf_numpy.py projected on an orthonormal basis A_j of the left null space of H_f,
+the chi-square gate, then the stacked update.  The pixel noise is D_j = diag(u_var, v_var, u_var, ...) per track, projected to
+R_o,j = A_j^T D_j A_j:
+  * gamma_j = r~^T (H_o,j P H_o,j^T + u_var I)^-1 r~, accepted when gamma_j < chi2_table[L_j] (msckf.h:1103-1124: u_var only,
+    whatever v_var is);
+  * isotropic noise (u_var = v_var = sigma^2): every R_o,j is sigma^2 I whatever basis is used, so the accepted rows H_o, r_o are
+    compressed by an economic QR H_o = Q_1 T (any such Q_1 gives the same update, R_n = sigma^2 I) and the update uses the
+    innovation S = T P T^T + sigma^2 I >= sigma^2 I: no P^-1, so the filter's own ill-conditioned P works;
+  * anisotropic noise, m <= n: the plain update in the full measurement space, R_o = blkdiag(R_o,j);
+  * anisotropic noise, m > n: the exact-subspace update (DESIGN.md 3, 4.4): Q_1 an orthonormal basis of span(E_15) + range(H_o),
+    taken from the singular vectors of [E_15 | H_c] above the rank gap (rank_of), T = Q_1^T H_o, r = Q_1^T r_o,
+    R = Q_1^T R_o Q_1 summed track by track (R_o itself is never formed).  A Householder Q_1 would add basis vectors outside
+    that span at a clone no track sees, and under anisotropic noise they move the update;
+  * P+ in Joseph form, dx = K r, and the state injection of msckf_numpy (IMU quaternion not renormalised, clones' are);
   * the rank of the compressed system: m when m <= n (the reference's Q is square), else the numerical rank of
     [E_15 | H_o(:, 15:)] (DESIGN.md 4.4), split in the gap of its singular values (null directions ~1e-14, or ~1e-8 at poses rounded to fp32;
     real ones ~1e-2, ~1e-4 when only a few tracks make m just above n).
@@ -33,12 +40,44 @@ T0, DT, READINGS_PER_CLONE = 1.0, 0.01, 10
 # singular values of the column-normalised [E_15 | H_c] relative to the largest: the null directions lie below NULL_SV, the
 # real ones above REAL_SV (asserted); the rank counts those above their geometric mean
 NULL_SV, REAL_SV = 1e-7, 1e-5
+# ceilings that separate rounding from a wrong result in the engine's agreement with this reference, whatever was measured
+# (tests/test_update_shapes_gpu.py, tests/test_update_noise_gpu.py); dx, P, state, gamma, p_f_G as measured there
+CONTRACT = {"float64": {"dx": 1e-4, "P": 1e-5, "state": 1e-4, "gamma": 1e-6, "p_f_G": 1e-6},
+            "float32": {"dx": 5e-2, "P": 1e-3, "state": 5e-2, "gamma": 1e-2, "p_f_G": 1e-2}}
 
 
-def setup():
-    """(camera, noise, params, imu_state) of a filter for the builder: EuRoC camera, isotropic pixel noise"""
+def pixel_noise(ratio, dtype=np.float64):
+    """(u_var, v_var) as a filter of `dtype` holds them: u_var = SIGMA2 and v_var = ratio * SIGMA2, or EuRoC's own pair
+    (v_var 0.6 % above u_var: f_u > f_v) for ratio "euroc"; rounded to dtype, in fp64"""
+    if ratio == "euroc":
+        nz = synth.euroc_noise(tuned=True)
+        u, v = nz["u_var_prime"], nz["v_var_prime"]
+    else:
+        u, v = SIGMA2, ratio * SIGMA2
+    return float(np.dtype(dtype).type(u)), float(np.dtype(dtype).type(v))
+
+
+def setup(noise=None):
+    """(camera, noise, params, imu_state) of a filter for the builder: EuRoC camera, pixel noise (u_var, v_var) (default
+    isotropic, SIGMA2)"""
     params = synth.euroc_params(max_track_length=98, min_track_length=2, max_cam_states=192)
-    return synth.euroc_camera(), NOISE, params, synth.true_imu_state(TRAJ, T0)
+    nz = NOISE if noise is None else dict(NOISE, u_var_prime=noise[0], v_var_prime=noise[1])
+    return synth.euroc_camera(), nz, params, synth.true_imu_state(TRAJ, T0)
+
+
+def head_lengths(case, M):
+    """(track lengths, outlier tracks) that place the first 15 stacked rows (the ones the engine keeps explicit when m > n)
+    across track edges in a given way, followed by long tracks so that m > n:
+      "edge": five 3-observation tracks (3 rows each), row 15 on a track edge;
+      "straddle": 5-observation tracks (7 rows each), the third track holds rows 14 .. 20;
+      "whole": a 12-observation track (21 rows) holds the whole head;
+      "pairs": fifteen 2-observation tracks (one row each);
+      "gated": the second of three 5-observation tracks gated out (an outlier), the fourth track reaches row 15"""
+    head = {"edge": [3] * 5, "straddle": [5] * 3, "whole": [12], "pairs": [2] * 15, "gated": [5] * 3}[case]
+    return head + [M, M - 1, M // 2, M] * 2, ((1,) if case == "gated" else ())
+
+
+HEAD_CASES = ["edge", "straddle", "whole", "pairs", "gated"]
 
 
 def readings(k):
@@ -47,10 +86,10 @@ def readings(k):
     return np.array([np.concatenate([w, a, [dt]]) for w, a, dt in rs])
 
 
-def numpy_filter(M, dtype=np.float64, drop_null_rows=True):
+def numpy_filter(M, dtype=np.float64, drop_null_rows=True, noise=None):
     """msckf_numpy's filter driven through the builder's M clones"""
     f = NumpyMSCKF(dtype, drop_null_rows=drop_null_rows)
-    f.initialize(*setup())
+    f.initialize(*setup(noise))
     for k in range(M):
         if k:
             for r in readings(k):
@@ -137,8 +176,9 @@ def _view(imu, poses):
 
 
 def project_tracks(imu, poses, tracks):
-    """per track (H_o,j [2L-3, n], r_o,j [2L-3]) on msckf_numpy's null-space basis (any orthonormal one would do), or None for
-    a track of one observation (no row left after the projection)"""
+    """per track (H_o,j [2L-3, n], r_o,j [2L-3], A_j [2L, 2L-3]) on msckf_numpy's null-space basis A_j (any orthonormal one
+    would do, with R_o,j = A_j^T D_j A_j formed on the same basis), or None for a track of one observation (no row left after
+    the projection)"""
     f = _view(imu, poses)
     out = []
     for t in tracks:
@@ -148,17 +188,23 @@ def project_tracks(imu, poses, tracks):
             continue
         r = f._calc_residual(np.asarray(t["pfg"], np.float64), [f.cam_states[k] for k in idx], list(t["obs"]))
         H_o, A = f._calc_meas_jacobian(np.asarray(t["pfg"], np.float64), idx)
-        out.append((H_o, A.T @ r))
+        out.append((H_o, A.T @ r, A))
     return out
 
 
+def noise_block(A, u_var, v_var):
+    """R_o,j = A_j^T D_j A_j, D_j = diag(u_var, v_var, u_var, ...)"""
+    d = np.tile([u_var, v_var], A.shape[0] // 2)
+    return A.T @ (d[:, None] * A)
+
+
 def gate(P, blocks, tracks, sigma2=SIGMA2):
-    """(gamma [N] (NaN for a track of one observation), accepted [N] bool)"""
+    """(gamma [N] (NaN for a track of one observation), accepted [N] bool); sigma2 is u_var, whatever v_var is"""
     gam = np.full(len(blocks), np.nan)
     for j, (b, t) in enumerate(zip(blocks, tracks)):
         if b is None:
             continue
-        H, r = b
+        H, r = b[0], b[1]
         cols = np.concatenate([np.arange(15 + 6 * k, 21 + 6 * k) for k in np.unique(t["idx"])])
         Hc = H[:, cols]
         gam[j] = float(r @ np.linalg.solve(Hc @ P[np.ix_(cols, cols)] @ Hc.T + sigma2 * np.eye(len(r)), r))
@@ -180,13 +226,27 @@ def compressed_update(P, H_o, r_o, sigma2=SIGMA2):
 
 
 def dense_update(P, H_o, r_o, sigma2=SIGMA2):
-    """(dx, P+) of the uncompressed m x m innovation form (Joseph form): the cross-check of compressed_update"""
+    """(dx, P+) of the uncompressed m x m innovation form (Joseph form): the cross-check of compressed_update.  sigma2 is the
+    measurement noise: a scalar (sigma2 I) or the m x m matrix"""
     n, m = P.shape[0], H_o.shape[0]
-    S = H_o @ P @ H_o.T + sigma2 * np.eye(m)
+    iso = np.ndim(sigma2) == 0
+    S = H_o @ P @ H_o.T + (sigma2 * np.eye(m) if iso else sigma2)
     K = sla.solve(S, H_o @ P, assume_a="pos").T
     A = np.eye(n) - K @ H_o
-    Pn = A @ P @ A.T + sigma2 * (K @ K.T)
+    Pn = A @ P @ A.T + (sigma2 * (K @ K.T) if iso else K @ sigma2 @ K.T)
     return K @ r_o, (Pn + Pn.T) / 2
+
+
+def subspace_update(P, H_o, r_o, Ro_blocks, Q1):
+    """(dx, P+) of the exact-subspace update (Joseph form): the stacked system projected on the orthonormal basis Q1 [m, rank]
+    (rank_of), its noise Q1^T R_o Q1 formed from each track's rows of Q1 and its R_o,j (Ro_blocks, in stacking order)"""
+    R = np.zeros((Q1.shape[1], Q1.shape[1]))
+    off = 0
+    for Rb in Ro_blocks:
+        Qb = Q1[off:off + Rb.shape[0]]
+        R += Qb.T @ Rb @ Qb
+        off += Rb.shape[0]
+    return dense_update(P, Q1.T @ H_o, Q1.T @ r_o, (R + R.T) / 2)
 
 
 def inject(imu, poses, dx):
@@ -201,34 +261,47 @@ def inject(imu, poses, dx):
     return imu, poses
 
 
-def rank_of(H_o):
-    """(rank, relative singular values of the column-normalised [E_15 | H_c] or None when m <= n)"""
+def rank_of(H_o, basis=False):
+    """(rank, relative singular values of the column-normalised [E_15 | H_c] or None when m <= n); with basis, also an
+    orthonormal basis [m, rank] of span(E_15) + range(H_o): its leading left singular vectors (None when m <= n)"""
     m, n = H_o.shape
     if m <= n:
-        return m, None
+        return (m, None, None) if basis else (m, None)
     B = np.hstack([np.eye(m)[:, :15], H_o[:, 15:]])
     nrm = np.linalg.norm(B, axis=0)
     B = B[:, nrm > 0] / nrm[nrm > 0]  # the columns of a clone no track sees are zero (Gamma's diagonal is exactly 0 there)
-    s = np.linalg.svd(sla.qr(B, mode="r")[0][: B.shape[1]], compute_uv=False)
+    Q, R = sla.qr(B, mode="economic")
+    W, s, _ = np.linalg.svd(R)
     s = s / s[0]
-    return min(int(np.sum(s > np.sqrt(NULL_SV * REAL_SV))), m, n), s
+    rank = min(int(np.sum(s > np.sqrt(NULL_SV * REAL_SV))), m, n)
+    return (rank, s, Q @ W[:, :rank]) if basis else (rank, s)
 
 
-def reference(P, imu, poses, tracks, sigma2=SIGMA2, blocks=None):
-    """the whole update on fp64 inputs: dict gamma, accepted, rows [N], m, rank, sv (see rank_of), H_o, r_o and, when a track is
+def reference(P, imu, poses, tracks, noise=None, blocks=None):
+    """the whole update on fp64 inputs at pixel noise (u_var, v_var) (default isotropic, SIGMA2; pass the values the filter
+    holds, see pixel_noise): dict gamma, accepted, rows [N], m, rank, sv (see rank_of), H_o, r_o and, when a track is
     accepted, dx, P, imu, poses after the update (else P, imu, poses unchanged and dx None)"""
+    u_var, v_var = (SIGMA2, SIGMA2) if noise is None else noise
     P = np.asarray(P, np.float64)
     blocks = project_tracks(imu, poses, tracks) if blocks is None else blocks
-    gam, acc = gate(P, blocks, tracks, sigma2)
+    gam, acc = gate(P, blocks, tracks, u_var)
     rows = np.array([0 if b is None or not a else b[0].shape[0] for b, a in zip(blocks, acc)], dtype=int)
     n = P.shape[0]
     H_o = np.vstack([b[0] for b, a in zip(blocks, acc) if a]) if acc.any() else np.zeros((0, n))
     r_o = np.concatenate([b[1] for b, a in zip(blocks, acc) if a]) if acc.any() else np.zeros(0)
     out = {"gamma": gam, "accepted": acc, "rows": rows, "m": int(rows.sum()), "H_o": H_o, "r_o": r_o,
            "dx": None, "P": P, "imu": np.asarray(imu, np.float64), "poses": np.asarray(poses, np.float64), "rank": 0, "sv": None}
-    if out["m"]:
+    if out["m"] and u_var == v_var:
         out["rank"], out["sv"] = rank_of(H_o)
-        out["dx"], out["P"] = compressed_update(P, H_o, r_o, sigma2)
+        out["dx"], out["P"] = compressed_update(P, H_o, r_o, u_var)
+    elif out["m"]:
+        out["rank"], out["sv"], Q1 = rank_of(H_o, basis=True)
+        Ro = [noise_block(b[2], u_var, v_var) for b, a in zip(blocks, acc) if a]
+        if Q1 is None:
+            out["dx"], out["P"] = dense_update(P, H_o, r_o, sla.block_diag(*Ro))
+        else:
+            out["dx"], out["P"] = subspace_update(P, H_o, r_o, Ro, Q1)
+    if out["m"]:
         out["imu"], out["poses"] = inject(np.asarray(imu, np.float64), np.asarray(poses, np.float64), out["dx"])
     return out
 
