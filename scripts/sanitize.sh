@@ -8,9 +8,14 @@ OUT=${1:?usage: scripts/sanitize.sh OUT_DIR}
 timeout 1500 compute-sanitizer --tool memcheck --leak-check no --error-exitcode 9 --log-file $OUT/r02_memcheck.log \
   python -m pytest tests/test_engine_gpu.py tests/test_asl_gpu.py -m gpu -q -x > $OUT/r02_memcheck_pytest.log 2>&1
 echo "memcheck exit $?" >> $OUT/r02_memcheck_pytest.log
+# the side updates (k_aid on both storage paths, k_nees to 37 panels, k_lmk_* and k_lmk_set at their row, observation and
+# group caps, device batches of 33 members)
+timeout 1500 compute-sanitizer --tool memcheck --leak-check no --error-exitcode 9 --log-file $OUT/r02_memcheck_side.log \
+  python -m pytest tests/test_side_shapes_gpu.py -m gpu -q -x > $OUT/r02_memcheck_side_pytest.log 2>&1
+echo "memcheck exit $?" >> $OUT/r02_memcheck_side_pytest.log
 SELR='window_fp64_vs_clean_oracle and not 300 or persistent_batch'
 timeout 1500 compute-sanitizer --tool racecheck --racecheck-report all --error-exitcode 9 --log-file $OUT/r02_racecheck.log \
   python -m pytest tests/test_engine_gpu.py -m gpu -q -x -k "$SELR" > $OUT/r02_racecheck_pytest.log 2>&1
 echo "racecheck exit $?" >> $OUT/r02_racecheck_pytest.log
-tail -n 3 $OUT/r02_memcheck_pytest.log $OUT/r02_racecheck_pytest.log
-tail -n 5 $OUT/r02_memcheck.log $OUT/r02_racecheck.log
+tail -n 3 $OUT/r02_memcheck_pytest.log $OUT/r02_memcheck_side_pytest.log $OUT/r02_racecheck_pytest.log
+tail -n 5 $OUT/r02_memcheck.log $OUT/r02_memcheck_side.log $OUT/r02_racecheck.log

@@ -1,0 +1,175 @@
+"""The shapes the side-update kernels (k_aid, k_nees, k_lmk_*) dispatch on, as the host decides them, the grid of
+tests/test_side_shapes_gpu.py that reaches both sides of each decision and every cap, and the information-form update for
+stacked systems too large for the dense Joseph form.
+
+The constants are read from the CUDA sources (`parse_constants`) and checked against `MIRROR` by
+tests/test_side_shapes_cpu.py: a threshold moved in the code fails there instead of leaving the grid on one side of it."""
+import re
+from pathlib import Path
+
+import numpy as np
+
+CSRC = Path(__file__).resolve().parent.parent / "msckf_mono_b200" / "csrc"
+# name -> (source that defines it, the value the grid below is built for); a name is defined before the names that use it
+MIRROR = {"kAidSmemMax": ("engine.cu", 32 * 1024), "kAidMaxRows": ("aid_kernels.cuh", 32), "kAidMaxItems": ("aid_kernels.cuh", 8),
+          "kMaxKeep": ("state_kernels.cuh", 192), "kBatchMembers": ("state_kernels.cuh", 32),
+          "kLmkMaxPerClone": ("landmark_kernels.cuh", 256), "kLmkMaxObs": ("landmark_kernels.cuh", 4096),
+          "kLmkMaxRows": ("landmark_kernels.cuh", 1152), "kLmkMaxPerSet": ("landmark_kernels.cuh", 256),
+          "kLmkMaxSets": ("landmark_kernels.cuh", 256), "kLmkMapClones": ("landmark_kernels.cuh", 8),
+          "kLmkNB": ("landmark_kernels.cuh", 32)}
+K = {k: v for k, (_, v) in MIRROR.items()}
+
+
+def parse_constants():
+    """the MIRROR names as the sources define them: `constexpr int|size_t kName = <integers, * + - ( ) and earlier names>;`"""
+    out = {}
+    for name, (fn, _) in MIRROR.items():
+        found = re.findall(r"constexpr\s+(?:int|size_t)\s+" + name + r"\s*=\s*([^;]+);", (CSRC / fn).read_text())
+        assert len(found) == 1, (name, fn, found)
+        expr = re.sub(r"\bmb::", "", found[0])
+        assert re.fullmatch(r"[\w\s*+()-]+", expr), (name, expr)
+        out[name] = int(eval(expr, {"__builtins__": {}}, dict(out)))  # noqa: S307 (integers and names parsed above)
+    return out
+
+
+def n_of(M):
+    return 15 + 6 * M
+
+
+def chunks(count, size=32):
+    """ceil(count / size): panels of a factor over `count` columns, p0 steps of the downdate, launch chunks of members"""
+    return -(-count // size)
+
+
+# ---- k_aid: W^T and dx (n (m + 1) doubles) in dynamic shared memory up to kAidSmemMax bytes, else in the global workspace
+def aid_ws_bytes(n, m):
+    return 8 * n * (m + 1)
+
+
+def aid_global(M, m):
+    return aid_ws_bytes(n_of(M), m) > K["kAidSmemMax"]
+
+
+def aid_dynamic_smem(M, m):
+    """the dynamic shared memory of a k_aid launch of one member"""
+    return 0 if aid_global(M, m) else aid_ws_bytes(n_of(M), m)
+
+
+# row count -> (last window on the shared side, first window on the global side; None: shared at every window)
+AID_EDGES = {1: (192, None), 3: (168, 169), 6: (95, 96), 9: (65, 66), 16: (37, 38), 31: (18, 19), 32: (18, 19)}
+AID_END_WINDOWS = (0, 1, 191, 192)  # with m = 1 and 32: the first and last rows and columns of P
+AID_END_ROWS = (1, 32)
+# stacks of model items with exactly m rows, every clone item at the window's last clone (M - 1) unless it says 0:
+# (model, rows, clone); RELATIVE_POSE is between clones 0 and M - 1.  The models of windows of < 2 clones stand apart.
+AID_STACKS = {
+    1: [("CLONE_HEADING", 1, -1)],
+    3: [("CLONE_ANTENNA_POSITION", 3, -1)],
+    6: [("RELATIVE_POSE", 6, None)],
+    9: [("RELATIVE_POSE", 6, None), ("CLONE_ANTENNA_POSITION", 3, -1)],
+    16: [("CLONE_POSE", 6, -1), ("RELATIVE_POSE", 6, None), ("BODY_VELOCITY", 3, None), ("CLONE_HEADING", 1, -1)],
+    31: [("CLONE_POSE", 6, -1), ("RELATIVE_POSE", 6, None), ("POSE", 6, None), ("CLONE_ANTENNA_POSITION", 3, -1),
+         ("ANTENNA_POSITION", 3, None), ("BODY_VELOCITY", 3, None), ("VELOCITY", 3, None), ("CLONE_HEADING", 1, -1)],
+    32: [("CLONE_POSE", 6, -1), ("RELATIVE_POSE", 6, None), ("POSE", 6, None), ("CLONE_POSE", 6, 0),
+         ("CLONE_ANTENNA_POSITION", 3, -1), ("BODY_VELOCITY", 3, None), ("CLONE_HEADING", 1, -1), ("HEADING", 1, None)],
+}
+AID_STACKS_SMALL = {  # windows of 0 and 1 clones (M = 1: the clone items at clone 0)
+    (0, 1): [("HEADING", 1, None)],
+    (0, 32): [("POSE", 6, None)] * 5 + [("HEADING", 1, None)] * 2,
+    (1, 1): [("CLONE_HEADING", 1, -1)],
+    (1, 32): [("CLONE_POSE", 6, -1), ("POSE", 6, None), ("CLONE_POSE", 6, -1), ("POSE", 6, None),
+              ("CLONE_ANTENNA_POSITION", 3, -1), ("ANTENNA_POSITION", 3, None), ("HEADING", 1, None), ("CLONE_HEADING", 1, -1)],
+}
+
+
+def aid_stack(M, m):
+    return AID_STACKS_SMALL[(M, m)] if M < 2 else AID_STACKS[m]
+
+
+def aid_cases():
+    """(M, m) of every single-call case: each row count at its last shared and first global window, and the end windows"""
+    out = []
+    for m, (a, b) in AID_EDGES.items():
+        out += [(a, m)] + ([(b, m)] if b is not None else [])
+    return out + [(M, m) for M in AID_END_WINDOWS for m in AID_END_ROWS if (M, m) not in out]
+
+
+# a device batch of 33 LINEAR members (two launch chunks), chunk 0 mixing shared and global members of different m
+AID_BATCH = [((18, 19, 37, 38, 65, 66, 95, 96, 168, 169, 0)[i % 11], (31, 32, 16, 9, 6, 3, 1)[i % 7]) for i in range(33)]
+
+# ---- k_nees: one CTA factors the (n + 1) x n bordered matrix in panels of 32
+NEES_WINDOWS = (19, 24, 41, 95, 136, 191, 192)  # n mod 32 = 1, 31, 5, 9, 31, 9, 15
+NEES_BREAK = (192, 150)  # window, clone whose block is made negative: first bad pivot 15 + 6 * 150 = 915, panel 28
+
+
+# ---- mapped landmarks: the planned rows (ld, the workspace stride, from every observation) and the used rows m'
+def lmk_rows(per_clone, groups=()):
+    """sum over clones of min(2 a_k, 6) (a_k: observations of one-clone landmarks) plus over clone-set groups (c clones, o
+    observations) min(2 o, 6 c).  With every observation: the host's ld; with the used ones: k_lmk_gain's m'."""
+    return int(sum(min(2 * a, 6) for a in per_clone.values()) + sum(min(2 * o, 6 * c) for c, o in groups))
+
+
+def spread(M, k):
+    """k distinct clones of a window of M spread from 0 to M - 1"""
+    return sorted({int(round(x)) for x in np.linspace(0, M - 1, k)}) if k > 1 else [M - 1]
+
+
+def sweep_counts(M, rows):
+    """clone -> observations with `rows` used rows: rows // 6 clones with 3 observations, one clone with 1 or 2 for the rest"""
+    full, rest = divmod(rows, 6)
+    clones = spread(M, full + (rest > 0))
+    counts = {k: 3 for k in clones[:full]}
+    if rest:
+        counts[clones[full]] = rest // 2
+    return counts
+
+
+LMK_WINDOW = 192
+LMK_SWEEP_ROWS = (30, 32, 34, 64, 66, 180, 1152)
+LMK_WINDOWS = (91, 136, 191, 192)  # with clones 0, M // 2 and M - 1 observed
+LMK_PER_CLONE = (255, 256)  # on clone 191 of a 192-clone window
+LMK_FULL = {k: 256 for k in spread(192, 16)}  # 4096 observations: 16 clones x 256
+# gating: (observations per clone, the clone whose every observation is gated): ld 36 -> m' 30 and ld 66 -> m' 60
+LMK_GATE = ({k: 3 for k in spread(192, 6)}, {k: 3 for k in spread(192, 11)})
+LMK_ITER_ROWS = (180, 1152)
+# map uncertainty: (clone sets, landmarks per set); one-clone sets count per clone, the others per group
+MAP_END = ([list(range(184, 192))] * 3 + [[191], [191], [0]])
+MAP_FULL_SET = [list(range(184, 192))] * 32  # one group of 32 landmarks x 8 clones = 256 observations
+MAP_SETS = [[k, k + 1] for k in range(191)] + [[k, k + 2] for k in range(65)]  # 256 clone-set groups of 2 clones
+MAP_ROWS = [list(range(8 * g, 8 * g + 8)) for g in range(24) for _ in range(4)]  # 24 groups x 4 landmarks: 48 rows each
+MAP_PAST = MAP_ROWS + [[0]]  # 2 rows more than kLmkMaxRows (planned rows are even: one row past cannot be asked for)
+
+
+def map_rows(sets):
+    """lmk_rows of landmarks with the given clone sets (one landmark per entry, every observation used)"""
+    single, groups = {}, {}
+    for cs in sets:
+        if len(cs) == 1:
+            single[cs[0]] = single.get(cs[0], 0) + 1
+        else:
+            groups[tuple(cs)] = groups.get(tuple(cs), 0) + len(cs)
+    return lmk_rows(single, [(len(cs), o) for cs, o in groups.items()])
+
+
+def lmk_tiles(n):
+    """k_lmk_downdate's CTAs per member: the 32 x 32 tiles of P's lower triangle"""
+    t = chunks(n, K["kLmkNB"])
+    return t * (t + 1) // 2
+
+
+# ---- the information form of the EKF update
+def information_update(P, imu, poses, H, r, R_blocks):
+    """the update of test_aid_gpu.numpy_update in information form, for a block-diagonal R = blkdiag(R_blocks [k, b, b]):
+    b = H^T R^-1 r, P+ = (P^-1 + H^T R^-1 H)^-1, dx = P+ b, NIS = r^T R^-1 r - b^T P+ b; injection as numpy_update's.
+    Costs n^3 and k b^2 n^2 instead of the Joseph form's (k b)^3."""
+    from tests.landmark_map_reference import inject
+    Rb = np.asarray(R_blocks, dtype=np.float64)
+    k, bs = Rb.shape[0], Rb.shape[1]
+    Ri = np.linalg.inv(Rb)
+    RiH = np.einsum("kij,kjn->kin", Ri, H.reshape(k, bs, -1)).reshape(k * bs, -1)
+    Rir = np.einsum("kij,kj->ki", Ri, r.reshape(k, bs)).ravel()
+    b = H.T @ Rir
+    Pn = np.linalg.inv(np.linalg.inv(P) + H.T @ RiH)
+    Pn = 0.5 * (Pn + Pn.T)
+    dx = Pn @ b
+    imu, poses = inject(imu, poses, dx)
+    return Pn, imu, poses, float(r @ Rir - b @ dx), float(np.linalg.norm(dx))
