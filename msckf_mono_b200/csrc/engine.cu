@@ -1607,214 +1607,225 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
 }
 
 // Mapped-landmark updates: every member with observations sends its observations (grouped by clone in window order, input
-// order kept inside a clone) and its clone table in the I/O block with one host-to-device copy; results, gamma and flags come
-// back with one copy and one synchronisation.  Three launches per per_member chunk of such members (k_lmk_clone, k_lmk_gain,
-// k_lmk_downdate; NM = 1 with one member in the context), whatever the observations turn out to be; a chunk whose largest
-// max_iter K is >= 2 launches (k_lmk_step, k_lmk_clone<..., true>, k_lmk_gain<..., true>) K - 1 times between the gain and the
-// downdate, with no host synchronisation in between.  Nothing is launched unless every member is valid.
+// order kept inside a clone), its clone table and (Sigma_L given) its map in the I/O block with one host-to-device copy;
+// results, gamma and flags come back with one copy and one synchronisation.  Each per_member chunk (NM = 1 with one member in
+// the context) launches clone, [set], gain, (step, clone, [set], gain) x (K - 1), downdate, K its largest max_iter and set only
+// with a Sigma_L member, whatever the observations turn out to be.  Nothing is launched unless every member is valid.
 static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_result, status) &&
                   offsetof(mb::LmkOut, iterations) == offsetof(msckf_b200_landmark_result, iterations) &&
                   offsetof(mb::LmkOut, converged) == offsetof(msckf_b200_landmark_result, converged) &&
                   offsetof(mb::LmkOut, step) == offsetof(msckf_b200_landmark_result, step),
               "mb::LmkOut must have msckf_b200_landmark_result's fields at their offsets");
+// one member's call, planned on the host
+struct LmkPlan {
+  std::vector<int> perm, grp;  // packed observation j is input observation perm[j]; [G][3] clone, first observation, count
+  int M = 0, G = 0, ld = 0;    // clones in the window; touched clones; rows of the compressed system, at most
+  // Sigma_L given: the map, the clone-set groups, each observation's pair (-1: a one-clone landmark), the groups' landmarks
+  const msckf_b200_landmark_map* map = nullptr;
+  std::vector<int> sdesc, pair_of, lms;
+  int H = 0, pairs = 0;
+  size_t E_len = 0, B_len = 0;
+};
+
+// Sigma_L given: check the landmark ids and covariances, count the one-clone landmarks' observations per clone (single),
+// and group the landmarks seen from 2 .. 8 clones by their exact clone set (sets in ascending order, landmarks ascending)
+int lmk_map_plan(const msckf_b200_landmarks& q, const msckf_b200_landmark_map& mq, const std::string& who, LmkPlan& p,
+                 std::vector<int>& single) {
+  const int nl = mq.n_landmarks, no = q.n_obs;
+  if (!mq.landmark || nl < 1) return fail(MSCKF_B200_ERR_ARG, "landmark_update: Sigma_L without landmark ids" + who);
+  if (!finite(mq.Sigma_L, 6 * (size_t)nl)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: non-finite Sigma_L" + who);
+  // positive definite with room to spare: every squared pivot of the Cholesky factor >= 1e-30 m^2 and >= 1e-12 x the largest
+  // diagonal entry, so that k_lmk_set's L^-1 (entries up to 1e15 / m) is finite and meaningful
+  for (int l = 0; l < nl; ++l) {
+    const double* s = mq.Sigma_L + 6 * (size_t)l;
+    const double a = s[0], b = s[2] - s[1] * s[1] / a;
+    const double c = s[4] - s[3] * s[1] / a;
+    const double d = s[5] - s[3] * s[3] / a - c * c / b, floor = std::max(1e-30, 1e-12 * std::max(s[0], std::max(s[2], s[5])));
+    if (!(a >= floor) || !(b >= floor) || !(d >= floor))
+      return fail(MSCKF_B200_ERR_ARG, "landmark_update: Sigma_L of landmark " + std::to_string(l) +
+                                          " is not positive definite (pivots >= 1e-30 and >= 1e-12 x its largest variance)" + who);
+  }
+  std::vector<std::vector<int>> of(nl);  // observations of each landmark, in input order
+  for (int j = 0; j < no; ++j) {
+    if (mq.landmark[j] < 0 || mq.landmark[j] >= nl) return fail(MSCKF_B200_ERR_ARG, "landmark_update: landmark id outside 0 .. n_landmarks - 1" + who);
+    of[mq.landmark[j]].push_back(j);
+  }
+  std::map<std::vector<int>, std::vector<int>> sets;
+  for (int l = 0; l < nl; ++l) {
+    if (of[l].empty()) continue;
+    std::vector<int> cs;
+    for (int j : of[l]) {
+      if (memcmp(q.p_L_G + 3 * (size_t)j, q.p_L_G + 3 * (size_t)of[l][0], sizeof(double) * 3) != 0)
+        return fail(MSCKF_B200_ERR_ARG, "landmark_update: p_L_G differs within landmark " + std::to_string(l) + who);
+      cs.push_back(q.clone[j]);
+    }
+    std::sort(cs.begin(), cs.end());
+    if (std::adjacent_find(cs.begin(), cs.end()) != cs.end())
+      return fail(MSCKF_B200_ERR_ARG, "landmark_update: landmark " + std::to_string(l) + " observed twice from one clone" + who);
+    if ((int)cs.size() > mb::kLmkMapClones) return fail(MSCKF_B200_ERR_ARG, "landmark_update: a landmark seen from more than 8 clones" + who);
+    if (cs.size() == 1) ++single[cs[0]];
+    else sets[cs].push_back(l);
+  }
+  if ((int)sets.size() > mb::kLmkMaxSets) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 clone sets" + who);
+  p.pair_of.assign(no, -1);
+  for (const auto& [cs, ls] : sets) {
+    const int c = (int)cs.size(), nlg = (int)ls.size();
+    if (c * nlg > mb::kLmkMaxPerSet) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 observations in one clone set" + who);
+    std::vector<int> d(mb::kLmkSetDesc, 0);
+    d[0] = c; d[1] = nlg; d[2] = p.pairs; d[3] = (int)p.lms.size(); d[4] = (int)p.E_len; d[5] = (int)p.B_len;
+    std::copy(cs.begin(), cs.end(), d.begin() + 8);
+    p.sdesc.insert(p.sdesc.end(), d.begin(), d.end());
+    for (int jl = 0; jl < nlg; ++jl)
+      for (int j : of[ls[jl]]) p.pair_of[j] = p.pairs + jl * c + (int)(std::lower_bound(cs.begin(), cs.end(), q.clone[j]) - cs.begin());
+    p.lms.insert(p.lms.end(), ls.begin(), ls.end());
+    p.ld += std::min(2 * c * nlg, 6 * c);  // the group's rows, at most
+    p.pairs += c * nlg;
+    p.E_len += (size_t)nlg * (3 + 2 * c) * (6 * c + 4);
+    p.B_len += (size_t)2 * c * nlg * (6 * c + 1);
+    ++p.H;
+  }
+  return 0;
+}
+
+// Checks one member's call (mq: its map, or NULL) against a window of M clones and plans it.  A member without observations
+// is only checked.
+int lmk_plan(const msckf_b200_landmarks& q, const msckf_b200_landmark_map* mq, int M, const std::string& who, LmkPlan& p) {
+  if (q.n_obs < 0 || q.n_obs > mb::kLmkMaxObs) return fail(MSCKF_B200_ERR_ARG, "landmark_update: n_obs outside 0 .. 4096" + who);
+  if (q.max_iter < 0 || q.max_iter > mb::kLmkMaxIter) return fail(MSCKF_B200_ERR_ARG, "landmark_update: max_iter outside 0 .. 16" + who);
+  if (!std::isfinite(q.tol) || q.tol < 0.0) return fail(MSCKF_B200_ERR_ARG, "landmark_update: tol is not finite and >= 0" + who);
+  if (q.n_obs == 0) return 0;
+  const int no = q.n_obs;
+  if (!q.clone || !q.z || !q.p_L_G) return fail(MSCKF_B200_ERR_ARG, "landmark_update: missing clone, z or p_L_G" + who);
+  std::vector<int> cnt(M, 0);
+  for (int j = 0; j < no; ++j) {
+    if (q.clone[j] < 0 || q.clone[j] >= M) return fail(MSCKF_B200_ERR_ARG, "landmark_update: clone outside the window" + who);
+    if (++cnt[q.clone[j]] > mb::kLmkMaxPerClone) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 observations of one clone" + who);
+  }
+  if (!finite(q.z, 2 * (size_t)no) || !finite(q.p_L_G, 3 * (size_t)no)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: non-finite z or p_L_G" + who);
+  if (q.R && (!finite(q.R, 3) || !(q.R[0] > 0.0) || !(q.R[0] * q.R[2] - q.R[1] * q.R[1] > 0.0)))
+    return fail(MSCKF_B200_ERR_ARG, "landmark_update: R is not finite and positive definite" + who);
+  if (std::isnan(q.chi2_obs)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: chi2_obs is NaN" + who);
+  p.M = M; p.map = mq;
+  std::vector<int> single(M, 0);  // observations of one-clone landmarks per clone (all of them without Sigma_L)
+  if (mq) RC(lmk_map_plan(q, *mq, who, p, single));
+  else single = cnt;
+  p.perm.resize(no);
+  std::vector<int> first(M + 1, 0);
+  for (int k = 0; k < M; ++k) first[k + 1] = first[k] + cnt[k];
+  std::vector<int> fill(first.begin(), first.end() - 1);
+  for (int j = 0; j < no; ++j) p.perm[fill[q.clone[j]]++] = j;  // stable: input order inside a clone
+  for (int k = 0; k < M; ++k)
+    if (cnt[k]) { p.grp.insert(p.grp.end(), {k, first[k], cnt[k]}); p.ld += std::min(2 * single[k], 6); }
+  p.G = (int)p.grp.size() / 3;
+  if (p.ld > mb::kLmkMaxRows)
+    return fail(MSCKF_B200_ERR_ARG, "landmark_update: the compressed system may exceed " + std::to_string(mb::kLmkMaxRows) + " rows" + who);
+  return 0;
+}
+
+// one member's host addresses in the I/O block: the inputs the host packs and the results it reads back
+struct LmkHost {
+  double *obs, *sig, *lsig, *gamma;
+  int *grp, *wrow, *sdesc, *flag;
+  mb::LmkOut* out;
+};
+struct LmkSizes { size_t in = 0, res = 0, io = 0, ws = 0; };  // bytes of inputs; offset of the results; I/O block; workspace
+
+// The landmark call's buffers.  The I/O block holds every member's inputs, then (from a 256-byte boundary) every member's
+// results; the workspace holds each member's slots, [S ; (T P)^T ; rho], dx and control words, then its iterated form's and
+// its map's regions, each region 256-byte aligned.  With null bases this only sizes the blocks; with the allocated bases it
+// also gives each member's host addresses (h) and its arguments' device addresses (a).
+template <class S>
+LmkSizes lmk_layout(const std::vector<int>& idx, const msckf_b200_landmarks* in, const std::vector<LmkPlan>& pl, unsigned char* ioh,
+                    unsigned char* iod, unsigned char* wsd, std::vector<LmkHost>& h, std::vector<mb::LmkMapArgs<S>>& a) {
+  LmkSizes z;
+  size_t o = 0, w = 0;  // the cursors in the I/O block and in the workspace
+  const auto io = [&](auto& hp, auto& dp, size_t bytes) {  // the next `bytes` of the I/O block, then 16-byte aligned
+    if (ioh) {
+      hp = reinterpret_cast<std::remove_reference_t<decltype(hp)>>(ioh + o);
+      dp = reinterpret_cast<std::remove_reference_t<decltype(dp)>>(iod + o);
+    }
+    o += up16(bytes);
+  };
+  const auto take = [&](auto& dp, size_t bytes) { if (wsd) dp = reinterpret_cast<std::remove_reference_t<decltype(dp)>>(wsd + w); w += bytes; };
+  for (int i : idx) {
+    const LmkPlan& p = pl[i];
+    const size_t no = p.perm.size(), n = 15 + 6 * (size_t)p.M;
+    io(h[i].obs, a[i].obs, sizeof(double) * 5 * no);
+    io(h[i].grp, a[i].grp, sizeof(int) * p.grp.size());
+    if (p.map) {  // Sigma of each observation's landmark, its pair, the group table, Sigma of the groups' landmarks
+      io(h[i].sig, a[i].sig, sizeof(double) * 6 * no);
+      io(h[i].wrow, a[i].wrow, sizeof(int) * no);
+      io(h[i].sdesc, a[i].sdesc, sizeof(int) * p.sdesc.size());
+      io(h[i].lsig, a[i].lsig, sizeof(double) * 6 * p.lms.size());
+    }
+    take(a[i].slot, sizeof(double) * mb::kLmkSlot * p.G);
+    take(a[i].A, sizeof(double) * (p.ld + n + 1) * p.ld);
+    take(a[i].dx, sizeof(double) * n);
+    take(a[i].ctl, sizeof(mb::LmkCtl));
+    w = up256(w);
+    if (in[i].max_iter > 1) {  // the iterate table, delta_i and the iteration's control words
+      take(a[i].xi, sizeof(double) * 7 * p.M); take(a[i].d, sizeof(double) * n); take(a[i].it, sizeof(mb::LmkIt));
+      w = up256(w);
+    }
+    if (p.map) {  // the pairs, the elimination and group rows, the groups' slots
+      take(a[i].pair, sizeof(double) * mb::kLmkPair * p.pairs); take(a[i].E, sizeof(double) * p.E_len);
+      take(a[i].B, sizeof(double) * p.B_len); take(a[i].sslot, sizeof(double) * mb::kLmkSetSlot * p.H);
+      w = up256(w);
+    }
+  }
+  z.in = o;
+  o = z.res = up256(o);
+  for (int i : idx) {
+    const size_t no = pl[i].perm.size();
+    io(h[i].out, a[i].out, sizeof(mb::LmkOut));
+    io(h[i].gamma, a[i].gamma, sizeof(double) * no);
+    io(h[i].flag, a[i].flag, sizeof(int) * no);
+  }
+  z.io = o; z.ws = w;
+  return z;
+}
+
 template <class S>
 int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "landmark_update: null argument");
   RC(members_ready("landmark_update"));
   const int nf = (int)eng.size();
-  struct LmkPlan {
-    std::vector<int> perm, grp;
-    int G = 0, ld = 0;
-    size_t in_off = 0, res_off = 0, ws_off = 0, it_off = 0;
-    // map uncertainty: the clone-set groups, each observation's pair (-1: a one-clone landmark), the groups' landmarks
-    std::vector<int> sdesc, pair_of, lms;
-    int H = 0, pairs = 0;
-    size_t map_in = 0, map_ws = 0, E_len = 0, B_len = 0;
-  };
   std::vector<LmkPlan> pl(nf);
+  std::vector<LmkHost> h(nf);
+  std::vector<mb::LmkMapArgs<S>> args(nf);  // zeroed; the layout fills in the addresses
   std::vector<int> idx;
-  size_t in_bytes = 0, res_bytes = 0, ws_bytes = 0;
-  // Sigma_L given: check the landmark ids and covariances, count the one-clone landmarks' observations per clone (single),
-  // and group the landmarks seen from 2 .. 8 clones by their exact clone set (sets in ascending order, landmarks ascending)
-  auto lmk_map_plan = [&](const msckf_b200_landmarks& q, const msckf_b200_landmark_map& mq, const std::string& who, LmkPlan& p, std::vector<int>& single) {
-    const int nl = mq.n_landmarks, no = q.n_obs;
-    if (!mq.landmark || nl < 1) return fail(MSCKF_B200_ERR_ARG, "landmark_update: Sigma_L without landmark ids" + who);
-    if (!finite(mq.Sigma_L, 6 * (size_t)nl)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: non-finite Sigma_L" + who);
-    // positive definite with room to spare: every squared pivot of the Cholesky factor >= 1e-30 m^2 and >= 1e-12 x the largest
-    // diagonal entry, so that k_lmk_set's L^-1 (entries up to 1e15 / m) is finite and meaningful
-    for (int l = 0; l < nl; ++l) {
-      const double* s = mq.Sigma_L + 6 * (size_t)l;
-      const double a = s[0], b = s[2] - s[1] * s[1] / a;
-      const double c = s[4] - s[3] * s[1] / a;
-      const double d = s[5] - s[3] * s[3] / a - c * c / b, floor = std::max(1e-30, 1e-12 * std::max(s[0], std::max(s[2], s[5])));
-      if (!(a >= floor) || !(b >= floor) || !(d >= floor))
-        return fail(MSCKF_B200_ERR_ARG, "landmark_update: Sigma_L of landmark " + std::to_string(l) +
-                                            " is not positive definite (pivots >= 1e-30 and >= 1e-12 x its largest variance)" + who);
-    }
-    std::vector<std::vector<int>> of(nl);  // observations of each landmark, in input order
-    for (int j = 0; j < no; ++j) {
-      if (mq.landmark[j] < 0 || mq.landmark[j] >= nl) return fail(MSCKF_B200_ERR_ARG, "landmark_update: landmark id outside 0 .. n_landmarks - 1" + who);
-      of[mq.landmark[j]].push_back(j);
-    }
-    std::map<std::vector<int>, std::vector<int>> sets;
-    for (int l = 0; l < nl; ++l) {
-      if (of[l].empty()) continue;
-      std::vector<int> cs;
-      for (int j : of[l]) {
-        if (memcmp(q.p_L_G + 3 * (size_t)j, q.p_L_G + 3 * (size_t)of[l][0], sizeof(double) * 3) != 0)
-          return fail(MSCKF_B200_ERR_ARG, "landmark_update: p_L_G differs within landmark " + std::to_string(l) + who);
-        cs.push_back(q.clone[j]);
-      }
-      std::sort(cs.begin(), cs.end());
-      if (std::adjacent_find(cs.begin(), cs.end()) != cs.end())
-        return fail(MSCKF_B200_ERR_ARG, "landmark_update: landmark " + std::to_string(l) + " observed twice from one clone" + who);
-      if ((int)cs.size() > mb::kLmkMapClones) return fail(MSCKF_B200_ERR_ARG, "landmark_update: a landmark seen from more than 8 clones" + who);
-      if (cs.size() == 1) ++single[cs[0]];
-      else sets[cs].push_back(l);
-    }
-    if ((int)sets.size() > mb::kLmkMaxSets) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 clone sets" + who);
-    p.pair_of.assign(no, -1);
-    for (const auto& [cs, ls] : sets) {
-      const int c = (int)cs.size(), nlg = (int)ls.size();
-      if (c * nlg > mb::kLmkMaxPerSet) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 observations in one clone set" + who);
-      std::vector<int> d(mb::kLmkSetDesc, 0);
-      d[0] = c; d[1] = nlg; d[2] = p.pairs; d[3] = (int)p.lms.size(); d[4] = (int)p.E_len; d[5] = (int)p.B_len;
-      std::copy(cs.begin(), cs.end(), d.begin() + 8);
-      p.sdesc.insert(p.sdesc.end(), d.begin(), d.end());
-      for (int jl = 0; jl < nlg; ++jl)
-        for (int j : of[ls[jl]]) p.pair_of[j] = p.pairs + jl * c + (int)(std::lower_bound(cs.begin(), cs.end(), q.clone[j]) - cs.begin());
-      p.lms.insert(p.lms.end(), ls.begin(), ls.end());
-      p.pairs += c * nlg;
-      p.E_len += (size_t)nlg * (3 + 2 * c) * (6 * c + 4);
-      p.B_len += (size_t)2 * c * nlg * (6 * c + 1);
-      ++p.H;
-    }
-    return 0;
-  };
   for (int i = 0; i < nf; ++i) {
-    const msckf_b200_landmarks& q = in[i];
-    const std::string who = " (member " + std::to_string(i) + ")";
-    if (q.n_obs < 0 || q.n_obs > mb::kLmkMaxObs) return fail(MSCKF_B200_ERR_ARG, "landmark_update: n_obs outside 0 .. 4096" + who);
-    if (q.max_iter < 0 || q.max_iter > mb::kLmkMaxIter) return fail(MSCKF_B200_ERR_ARG, "landmark_update: max_iter outside 0 .. 16" + who);
-    if (!std::isfinite(q.tol) || q.tol < 0.0) return fail(MSCKF_B200_ERR_ARG, "landmark_update: tol is not finite and >= 0" + who);
-    if (q.n_obs == 0) continue;
-    const int M = eng[i]->M, n = 15 + 6 * M, no = q.n_obs;
-    if (!q.clone || !q.z || !q.p_L_G) return fail(MSCKF_B200_ERR_ARG, "landmark_update: missing clone, z or p_L_G" + who);
-    std::vector<int> cnt(M, 0);
-    for (int j = 0; j < no; ++j) {
-      if (q.clone[j] < 0 || q.clone[j] >= M) return fail(MSCKF_B200_ERR_ARG, "landmark_update: clone outside the window" + who);
-      if (++cnt[q.clone[j]] > mb::kLmkMaxPerClone) return fail(MSCKF_B200_ERR_ARG, "landmark_update: more than 256 observations of one clone" + who);
-    }
-    if (!finite(q.z, 2 * (size_t)no) || !finite(q.p_L_G, 3 * (size_t)no)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: non-finite z or p_L_G" + who);
-    if (q.R && (!finite(q.R, 3) || !(q.R[0] > 0.0) || !(q.R[0] * q.R[2] - q.R[1] * q.R[1] > 0.0)))
-      return fail(MSCKF_B200_ERR_ARG, "landmark_update: R is not finite and positive definite" + who);
-    if (std::isnan(q.chi2_obs)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: chi2_obs is NaN" + who);
-    LmkPlan& p = pl[i];
-    const msckf_b200_landmark_map* mq = map && map[i].Sigma_L ? &map[i] : nullptr;
-    std::vector<int> single(M, 0);  // observations of one-clone landmarks per clone (all of them without Sigma_L)
-    if (mq) RC(lmk_map_plan(q, *mq, who, p, single));
-    else single = cnt;
-    p.perm.resize(no);
-    std::vector<int> first(M + 1, 0);
-    for (int k = 0; k < M; ++k) first[k + 1] = first[k] + cnt[k];
-    std::vector<int> fill(first.begin(), first.end() - 1);
-    for (int j = 0; j < no; ++j) p.perm[fill[q.clone[j]]++] = j;  // stable: input order inside a clone
-    for (int k = 0; k < M; ++k)
-      if (cnt[k]) { p.grp.insert(p.grp.end(), {k, first[k], cnt[k]}); p.ld += std::min(2 * single[k], 6); }
-    p.G = (int)p.grp.size() / 3;
-    for (int h = 0; h < p.H; ++h) {
-      const int* D = &p.sdesc[mb::kLmkSetDesc * h];
-      p.ld += std::min(2 * D[0] * D[1], 6 * D[0]);
-    }
-    if (p.ld > mb::kLmkMaxRows)
-      return fail(MSCKF_B200_ERR_ARG, "landmark_update: the compressed system may exceed " + std::to_string(mb::kLmkMaxRows) + " rows" + who);
-    p.in_off = in_bytes;
-    in_bytes += up16(sizeof(double) * 5 * (size_t)no) + up16(sizeof(int) * p.grp.size());
-    if (mq) {  // Sigma of each observation's landmark, its pair, the group table, Sigma of the groups' landmarks
-      p.map_in = in_bytes;
-      in_bytes += up16(sizeof(double) * 6 * (size_t)no) + up16(sizeof(int) * (size_t)no) + up16(sizeof(int) * p.sdesc.size()) +
-                  up16(sizeof(double) * 6 * p.lms.size());
-    }
-    p.res_off = res_bytes;
-    res_bytes += up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no) + up16(sizeof(int) * (size_t)no);
-    p.ws_off = ws_bytes;
-    ws_bytes += up256(sizeof(double) * ((size_t)mb::kLmkSlot * p.G + (size_t)(p.ld + n + 1) * p.ld + n) + sizeof(mb::LmkCtl));
-    if (q.max_iter > 1) {  // the iterate table, delta_i and the iteration's control words
-      p.it_off = ws_bytes;
-      ws_bytes += up256(sizeof(double) * (7 * (size_t)M + n) + sizeof(mb::LmkIt));
-    }
-    if (mq) {  // the pairs, the elimination and group rows, the groups' slots
-      p.map_ws = ws_bytes;
-      ws_bytes += up256(sizeof(double) * ((size_t)mb::kLmkPair * p.pairs + p.E_len + p.B_len + (size_t)mb::kLmkSetSlot * p.H));
-    }
+    RC(lmk_plan(in[i], map && map[i].Sigma_L ? &map[i] : nullptr, eng[i]->M, " (member " + std::to_string(i) + ")", pl[i]));
+    if (!in[i].n_obs) continue;
     idx.push_back(i);
+    static_cast<mb::LmkArgs<S>&>(args[i]) = eng[i]->lmk_args(in[i], pl[i].G, pl[i].ld);
+    args[i].H = pl[i].H; args[i].max_iter = in[i].max_iter; args[i].tol = in[i].tol;
   }
   if (idx.empty()) return 0;
-  const size_t res_base = up256(in_bytes);
+  const LmkSizes z = lmk_layout<S>(idx, in, pl, nullptr, nullptr, nullptr, h, args);
   CK(cudaSetDevice(device));
-  RC(io.ensure(res_base + res_bytes, stream));
-  RC(ws.ensure(ws_bytes, stream));
-  std::vector<mb::LmkMapArgs<S>> args(nf);
+  RC(io.ensure(z.io, stream));
+  RC(ws.ensure(z.ws, stream));
+  lmk_layout<S>(idx, in, pl, io.h, io.d, ws.d, h, args);
   for (int i : idx) {
     const msckf_b200_landmarks& q = in[i];
     const LmkPlan& p = pl[i];
-    const int no = q.n_obs, n = 15 + 6 * eng[i]->M;
-    double* ho = reinterpret_cast<double*>(io.h + p.in_off);
-    for (int j = 0; j < no; ++j) {
+    const LmkHost& hm = h[i];
+    const msckf_b200_landmark_map* mq = p.map;
+    for (int j = 0; j < q.n_obs; ++j) {
       const int s = p.perm[j];
-      ho[5 * j] = q.z[2 * s]; ho[5 * j + 1] = q.z[2 * s + 1];
-      ho[5 * j + 2] = q.p_L_G[3 * s]; ho[5 * j + 3] = q.p_L_G[3 * s + 1]; ho[5 * j + 4] = q.p_L_G[3 * s + 2];
+      double* o = hm.obs + 5 * j;
+      o[0] = q.z[2 * s]; o[1] = q.z[2 * s + 1];
+      o[2] = q.p_L_G[3 * s]; o[3] = q.p_L_G[3 * s + 1]; o[4] = q.p_L_G[3 * s + 2];
+      if (mq) { memcpy(hm.sig + 6 * j, mq->Sigma_L + 6 * (size_t)mq->landmark[s], sizeof(double) * 6); hm.wrow[j] = p.pair_of[s]; }
     }
-    const size_t goff = p.in_off + up16(sizeof(double) * 5 * (size_t)no);
-    memcpy(io.h + goff, p.grp.data(), sizeof(int) * p.grp.size());
-    mb::LmkMapArgs<S> a;
-    memset(&a, 0, sizeof(a));
-    static_cast<mb::LmkArgs<S>&>(a) = eng[i]->lmk_args(q, p.G, p.ld);
-    if (map && map[i].Sigma_L) {
-      const msckf_b200_landmark_map& mq = map[i];
-      const size_t o_sig = p.map_in, o_wr = o_sig + up16(sizeof(double) * 6 * (size_t)no), o_sd = o_wr + up16(sizeof(int) * (size_t)no),
-                   o_ls = o_sd + up16(sizeof(int) * p.sdesc.size());
-      double* hs = reinterpret_cast<double*>(io.h + o_sig);
-      int* hw = reinterpret_cast<int*>(io.h + o_wr);
-      for (int j = 0; j < no; ++j) {
-        const int s = p.perm[j];
-        memcpy(hs + 6 * j, mq.Sigma_L + 6 * (size_t)mq.landmark[s], sizeof(double) * 6);
-        hw[j] = p.pair_of[s];
-      }
-      memcpy(io.h + o_sd, p.sdesc.data(), sizeof(int) * p.sdesc.size());
-      double* hl = reinterpret_cast<double*>(io.h + o_ls);
-      for (size_t l = 0; l < p.lms.size(); ++l) memcpy(hl + 6 * l, mq.Sigma_L + 6 * (size_t)p.lms[l], sizeof(double) * 6);
-      a.sig = reinterpret_cast<const double*>(io.d + o_sig);
-      a.wrow = reinterpret_cast<const int*>(io.d + o_wr);
-      a.sdesc = reinterpret_cast<const int*>(io.d + o_sd);
-      a.lsig = reinterpret_cast<const double*>(io.d + o_ls);
-      a.pair = reinterpret_cast<double*>(ws.d + p.map_ws);
-      a.E = a.pair + (size_t)mb::kLmkPair * p.pairs;
-      a.B = a.E + p.E_len;
-      a.sslot = a.B + p.B_len;
-      a.H = p.H;
+    memcpy(hm.grp, p.grp.data(), sizeof(int) * p.grp.size());
+    if (mq) {
+      memcpy(hm.sdesc, p.sdesc.data(), sizeof(int) * p.sdesc.size());
+      for (size_t l = 0; l < p.lms.size(); ++l) memcpy(hm.lsig + 6 * l, mq->Sigma_L + 6 * (size_t)p.lms[l], sizeof(double) * 6);
     }
-    a.max_iter = q.max_iter; a.tol = q.tol;
-    a.xi = nullptr; a.d = nullptr; a.it = nullptr;
-    if (q.max_iter > 1) {
-      a.xi = reinterpret_cast<double*>(ws.d + p.it_off);
-      a.d = a.xi + 7 * (size_t)eng[i]->M;
-      a.it = reinterpret_cast<mb::LmkIt*>(a.d + n);
-    }
-    a.obs = reinterpret_cast<const double*>(io.d + p.in_off);
-    a.grp = reinterpret_cast<const int*>(io.d + goff);
-    unsigned char* r = io.d + res_base + p.res_off;
-    a.out = reinterpret_cast<mb::LmkOut*>(r);
-    a.gamma = reinterpret_cast<double*>(r + up16(sizeof(mb::LmkOut)));
-    a.flag = reinterpret_cast<int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)no));
-    double* w = reinterpret_cast<double*>(ws.d + p.ws_off);
-    a.slot = w;
-    a.A = w + (size_t)mb::kLmkSlot * p.G;
-    a.dx = a.A + (size_t)(p.ld + n + 1) * p.ld;
-    a.ctl = reinterpret_cast<mb::LmkCtl*>(a.dx + n);
-    args[i] = a;
   }
-  CK(cudaMemcpyAsync(io.d, io.h, in_bytes, cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(io.d, io.h, z.in, cudaMemcpyHostToDevice, stream));
   per_member(idx, false, [&](int i) { return args[i]; },
              [&](const auto& a, int nm) {
                constexpr int NM = (int)std::extent<decltype(std::decay_t<decltype(a)>::m)>::value;
@@ -1822,55 +1833,43 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_
                mb::Members<mb::LmkItArgs<S>, NM> c;  // the iterated form's
                int gx = 1, tx = 1, K = 1, hx = 0;  // the largest member's grid; other members' CTAs past their own range exit at once
                for (int j = 0; j < nm; ++j) {
-                 b.m[j] = a.m[j];
-                 c.m[j] = a.m[j];
+                 b.m[j] = a.m[j]; c.m[j] = a.m[j];
                  gx = std::max(gx, a.m[j].G);
                  tx = std::max(tx, a.m[j].ntiles);
                  K = std::max(K, a.m[j].max_iter);
                  if (a.m[j].sig) hx = std::max(hx, std::max(1, a.m[j].H));
                }
-               if (hx == 0) {  // no member has Sigma_L: the exact-map launches
-                 mb::k_lmk_clone<S, NM><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(b);
-                 mb::k_lmk_gain<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(b);
+               // MAP (a member has Sigma_L): clone, set and gain take the map arguments; else b (linearisation 0) and c
+               const auto lin = [&](auto map, const auto& x0, const auto& x1) {
+                 constexpr bool MAP = decltype(map)::value;
+                 mb::k_lmk_clone<S, NM, false, MAP><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(x0);
+                 if constexpr (MAP) mb::k_lmk_set<S, NM><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(x0);
+                 mb::k_lmk_gain<S, NM, false, MAP><<<nm, mb::kLmkThreads, 0, stream>>>(x0);
                  for (int it = 0; it + 1 < K; ++it) {
                    mb::k_lmk_step<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(c, it);
-                   mb::k_lmk_clone<S, NM, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(c);
-                   mb::k_lmk_gain<S, NM, true><<<nm, mb::kLmkThreads, 0, stream>>>(c);
+                   mb::k_lmk_clone<S, NM, true, MAP><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(x1);
+                   if constexpr (MAP) mb::k_lmk_set<S, NM, true><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(x1);
+                   mb::k_lmk_gain<S, NM, true, MAP><<<nm, mb::kLmkThreads, 0, stream>>>(x1);
                  }
-               } else {
-                 mb::k_lmk_clone<S, NM, false, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
-                 mb::k_lmk_set<S, NM><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(a);
-                 mb::k_lmk_gain<S, NM, false, true><<<nm, mb::kLmkThreads, 0, stream>>>(a);
-                 for (int it = 0; it + 1 < K; ++it) {
-                   mb::k_lmk_step<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(c, it);
-                   mb::k_lmk_clone<S, NM, true, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
-                   mb::k_lmk_set<S, NM, true><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(a);
-                   mb::k_lmk_gain<S, NM, true, true><<<nm, mb::kLmkThreads, 0, stream>>>(a);
-                 }
-               }
+               };
+               if (hx == 0) lin(std::false_type(), b, c);
+               else lin(std::true_type(), a, a);
                mb::k_lmk_downdate<S, NM><<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(b);
              });
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(io.h + res_base, io.d + res_base, res_bytes, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(io.h + z.res, io.d + z.res, z.io - z.res, cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
   int numeric = -1;
   for (int i : idx) {
     const msckf_b200_landmarks& q = in[i];
-    const LmkPlan& p = pl[i];
-    const unsigned char* r = io.h + res_base + p.res_off;
-    const mb::LmkOut& o = *reinterpret_cast<const mb::LmkOut*>(r);
-    const double* g = reinterpret_cast<const double*>(r + up16(sizeof(mb::LmkOut)));
-    const int* fl = reinterpret_cast<const int*>(r + up16(sizeof(mb::LmkOut)) + up16(sizeof(double) * (size_t)q.n_obs));
+    const mb::LmkOut& o = *h[i].out;
     out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].rows = o.rows; out[i].used = o.used;
     out[i].applied = o.applied; out[i].status = o.status;
-    if (q.max_iter > 1) {
-      out[i].iterations = o.iterations; out[i].converged = o.converged; out[i].step = o.step;
-    } else {
-      out[i].iterations = o.applied; out[i].converged = 0; out[i].step = 0.0;
-    }
+    const bool it = q.max_iter > 1;  // (the single linearisation leaves these to the host)
+    out[i].iterations = it ? o.iterations : o.applied; out[i].converged = it ? o.converged : 0; out[i].step = it ? o.step : 0.0;
     for (int j = 0; j < q.n_obs; ++j) {
-      if (q.gamma) q.gamma[p.perm[j]] = g[j];
-      if (q.flag) q.flag[p.perm[j]] = fl[j];
+      if (q.gamma) q.gamma[pl[i].perm[j]] = h[i].gamma[j];
+      if (q.flag) q.flag[pl[i].perm[j]] = h[i].flag[j];
     }
     if (o.numeric && numeric < 0) numeric = i;
   }
@@ -2095,11 +2094,9 @@ int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item*
   return e->impl->solo_ctx()->aid_stack(&items, &n_items, chi2_max, out);
 }
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
-  if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
-  const bool it_ok = lm->max_iter >= 0 && lm->max_iter <= mb::kLmkMaxIter && std::isfinite(lm->tol) && lm->tol >= 0.0;
-  if (lm->n_obs == 0 && it_ok) { memset(out, 0, sizeof(*out)); return 0; }
-  return e->impl->solo_ctx()->landmarks(lm, nullptr, out);
+  return msckf_b200_map_landmark_update(e, lm, nullptr, out);
 }
+// (an empty call with valid iteration settings only zeroes the result)
 int msckf_b200_map_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
                                    msckf_b200_landmark_result* out) {
   if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");

@@ -226,52 +226,21 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   // kept in registers across the compaction)
   double row[2][7];
   int fg = 2;
+  // MAP: R + F Sigma F^T of a member with Sigma (sg), and the observation's pair (wr >= 0: a landmark seen from >= 2 clones)
+  [[maybe_unused]] double Ri[3];
+  [[maybe_unused]] const double* sg = nullptr;
+  int wr = -1;
   if constexpr (MAP) {
-    double Ri[3] = {Rm[0], Rm[1], Rm[2]};
-    const double* sg = a.m[f].sig;
-    const int wr = sg && t < cnt ? a.m[f].wrow[i0 + t] : -1;
-    if (t < cnt) {
-      if (sg) lmk_map_R(obs, Cr, pc, sg + 6 * (size_t)(i0 + t), Ri);
-      const double gam = lmk_obs(obs, Cr, pc, Pk, Ri, chi2, row, fg);
-      if constexpr (IT) {
-        const int f0 = a.m[f].flag[i0 + t];
-        if (f0 == 0 && fg == 2) a.m[f].it->stop = 1;
-        fg = f0;
-      } else {
-        a.m[f].gamma[i0 + t] = gam;
-        a.m[f].flag[i0 + t] = fg;
-      }
-      if (wr >= 0) a.m[f].pair[(size_t)kLmkPair * wr + 14] = (double)fg;
-      fl[t] = wr >= 0 && fg == 0 ? 3 : fg;  // 3: used, in a pair
-    }
-    __syncthreads();
-    if (t == 0) {
-      int u = 0;
-      for (int i = 0; i < cnt; ++i) { pos[i] = u; u += fl[i] == 0; }
-      s_used = u;
-    }
-    __syncthreads();
-    if (t < cnt && fg == 0) {
-      lmk_obs(obs, Cr, pc, Pk, Ri, chi2, row, fg);
-      double l0 = LR[0], l1 = LR[1], l2 = LR[2];
-      if (sg && wr < 0) { l0 = sqrt(Ri[0]); l1 = Ri[1] / l0; l2 = sqrt(Ri[2] - l1 * l1); }
-      for (int c = 0; c < 7; ++c) {
-        row[0][c] /= l0;
-        row[1][c] = (row[1][c] - l1 * row[0][c]) / l2;
-      }
-      if constexpr (IT) {
-        for (int c = 0; c < 6; ++c) { row[0][6] += row[0][c] * ek[c]; row[1][6] += row[1][c] * ek[c]; }
-      }
-      if (wr >= 0) {
-        double* pr = a.m[f].pair + (size_t)kLmkPair * wr;
-        for (int c = 0; c < 7; ++c) { pr[c] = row[0][c]; pr[7 + c] = row[1][c]; }
-      } else {
-        for (int c = 0; c < 7; ++c) { Q[2 * pos[t]][c] = row[0][c]; Q[2 * pos[t] + 1][c] = row[1][c]; }
-      }
-    }
-  } else {
+    Ri[0] = Rm[0]; Ri[1] = Rm[1]; Ri[2] = Rm[2];
+    sg = a.m[f].sig;
+    wr = sg && t < cnt ? a.m[f].wrow[i0 + t] : -1;
+  }
+  const double* const Ro = MAP ? Ri : Rm;  // the gate's observation noise
   if (t < cnt) {
-    const double gam = lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
+    if constexpr (MAP) {
+      if (sg) lmk_map_R(obs, Cr, pc, sg + 6 * (size_t)(i0 + t), Ri);
+    }
+    const double gam = lmk_obs(obs, Cr, pc, Pk, Ro, chi2, row, fg);
     if constexpr (IT) {
       const int f0 = a.m[f].flag[i0 + t];  // linearisation 0's
       if (f0 == 0 && fg == 2) a.m[f].it->stop = 1;
@@ -280,7 +249,10 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
       a.m[f].gamma[i0 + t] = gam;
       a.m[f].flag[i0 + t] = fg;
     }
-    fl[t] = fg;
+    if constexpr (MAP) {
+      if (wr >= 0) a.m[f].pair[(size_t)kLmkPair * wr + 14] = (double)fg;
+    }
+    fl[t] = wr >= 0 && fg == 0 ? 3 : fg;  // 3: used, in a pair
   }
   __syncthreads();
   if (t == 0) {
@@ -290,22 +262,32 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   }
   __syncthreads();
   if (t < cnt && fg == 0) {
-    lmk_obs(obs, Cr, pc, Pk, Rm, chi2, row, fg);
-    if constexpr (IT) {  // whiten in place, then r~ + X~ e_k
-      for (int c = 0; c < 7; ++c) {
-        row[0][c] /= LR[0];
-        row[1][c] = (row[1][c] - LR[1] * row[0][c]) / LR[2];
-      }
-      for (int c = 0; c < 6; ++c) { row[0][6] += row[0][c] * ek[c]; row[1][6] += row[1][c] * ek[c]; }
-      for (int c = 0; c < 7; ++c) { Q[2 * pos[t]][c] = row[0][c]; Q[2 * pos[t] + 1][c] = row[1][c]; }
-    } else {
-      for (int c = 0; c < 7; ++c) {  // whiten: L_R^-1 [X | r]
-        const double y0 = row[0][c] / LR[0];
-        Q[2 * pos[t]][c] = y0;
-        Q[2 * pos[t] + 1][c] = (row[1][c] - LR[1] * y0) / LR[2];
-      }
+    lmk_obs(obs, Cr, pc, Pk, Ro, chi2, row, fg);
+    [[maybe_unused]] double Li[3];  // MAP: L_R, or the Cholesky factor of Ri for a one-clone landmark
+    if constexpr (MAP) {
+      Li[0] = LR[0]; Li[1] = LR[1]; Li[2] = LR[2];
+      if (sg && wr < 0) { Li[0] = sqrt(Ri[0]); Li[1] = Ri[1] / Li[0]; Li[2] = sqrt(Ri[2] - Li[1] * Li[1]); }
     }
-  }
+    const double* const L = MAP ? Li : LR;
+    // whiten in place: L^-1 [X | r].  The exact map's single linearisation changes the rows no further and stores each
+    // column as it is whitened (storing after the loop costs its schedule a few instructions); the other forms store below.
+    for (int c = 0; c < 7; ++c) {
+      row[0][c] /= L[0];
+      if constexpr (!IT && !MAP) Q[2 * pos[t]][c] = row[0][c];
+      row[1][c] = (row[1][c] - row[0][c] * L[1]) / L[2];
+      if constexpr (!IT && !MAP) Q[2 * pos[t] + 1][c] = row[1][c];
+    }
+    if constexpr (IT) {  // r~ + X~ e_k
+      for (int c = 0; c < 6; ++c) { row[0][6] += row[0][c] * ek[c]; row[1][6] += row[1][c] * ek[c]; }
+    }
+    if (wr >= 0) {
+      if constexpr (MAP) {
+        double* pr = a.m[f].pair + (size_t)kLmkPair * wr;
+        for (int c = 0; c < 7; ++c) { pr[c] = row[0][c]; pr[7 + c] = row[1][c]; }
+      }
+    } else if constexpr (IT || MAP) {
+      for (int c = 0; c < 7; ++c) { Q[2 * pos[t]][c] = row[0][c]; Q[2 * pos[t] + 1][c] = row[1][c]; }
+    }
   }
   __syncthreads();
   // ---- Householder QR of the used rows (one warp): R's first q rows are [T_k | rho_k], rows q.. of column 6 give e_k^2
@@ -496,37 +478,26 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
   __shared__ double s_e2;
   __shared__ int s_used;
   int Gt = G;  // groups: the clones, then (MAP) the clone sets
+  if constexpr (MAP) Gt = G + a.m[f].H;
 
-  if constexpr (MAP) {
-    Gt = G + a.m[f].H;
-    if (t == 0) {
-      int o = 0, u = 0;
-      double e2 = 0.0;
-      for (int g = 0; g < Gt; ++g) {  // e^2, used, q of each slot
-        const double* tl = g < G ? slot + (size_t)kLmkSlot * g + 42
-                                 : a.m[f].sslot + (size_t)kLmkSetSlot * (g - G) + kLmkSetLd * (kLmkSetLd + 1);
-        off[g] = o;
-        o += (int)tl[2];
-        u += (int)tl[1];
-        e2 += tl[0];
-      }
-      off[Gt] = o; s_used = u; s_e2 = e2;
-      ctl->ticket = 0u; ctl->bad = 0; ctl->m = o;
-    }
-  } else {
   if (t == 0) {
     int o = 0, u = 0;
     double e2 = 0.0;
-    for (int g = 0; g < G; ++g) {
+    for (int g = 0; g < Gt; ++g) {  // e^2, used, q of each slot
+      const double* tl = slot + (size_t)kLmkSlot * g + 42;
+      if constexpr (MAP) {
+        if (g >= G) tl = a.m[f].sslot + (size_t)kLmkSetSlot * (g - G) + kLmkSetLd * (kLmkSetLd + 1);
+      }
       off[g] = o;
-      o += (int)slot[(size_t)kLmkSlot * g + 44];
-      u += (int)slot[(size_t)kLmkSlot * g + 43];
-      e2 += slot[(size_t)kLmkSlot * g + 42];
+      o += (int)tl[2];
+      u += (int)tl[1];
+      e2 += tl[0];
     }
-    off[G] = o; s_used = u; s_e2 = e2;
+    off[Gt] = o; s_used = u; s_e2 = e2;
     ctl->ticket = 0u; ctl->bad = 0; ctl->m = o;
   }
-  for (int g = t; g < G; g += kLmkThreads) ck[g] = a.m[f].grp[3 * g];
+  if constexpr (!MAP) {
+    for (int g = t; g < G; g += kLmkThreads) ck[g] = a.m[f].grp[3 * g];
   }
   __syncthreads();
   const int m = off[Gt];
@@ -541,59 +512,56 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_gain(const Members<LmkArgsT
   for (int g = t; g < Gt; g += kLmkThreads)
     for (int r = off[g]; r < off[g + 1]; ++r) rg[r] = g;
   __syncthreads();
-  if constexpr (MAP) {  // the same products over each row's clone columns
-    const int* const grp = a.m[f].grp;
-    for (int idx = t; idx < m * n; idx += kLmkThreads) {
-      const int r = idx / n, c = idx - r * n, g = rg[r], lr = r - off[g];
-      int w;
-      const int* cl;
-      const double* T = lmk_map_row(a.m[f], slot, grp, G, g, lr, w, cl);
-      double s = 0.0;
-      for (int j = lr; j < w; ++j) s += T[j] * (double)P[(size_t)(15 + 6 * cl[j / 6] + j % 6) * ldp + c];
-      A[(size_t)(m + c) * ld + r] = s;
+  // ---- (T P)^T into rows m .. m + n - 1, rho into row m + n.  A row's T entries and clone columns: its clone's 6 (the
+  // clone table ck), or (MAP) its group's 6c (lmk_map_row)
+  [[maybe_unused]] const int* const grp = a.m[f].grp;
+  for (int idx = t; idx < m * n; idx += kLmkThreads) {
+    const int r = idx / n, c = idx - r * n, g = rg[r], lr = r - off[g];
+    const double* T;
+    const S* pc;
+    int w = 6;
+    [[maybe_unused]] const int* cl;
+    if constexpr (MAP) {
+      T = lmk_map_row(a.m[f], slot, grp, G, g, lr, w, cl);
+      pc = P + c;
+    } else {
+      T = slot + (size_t)kLmkSlot * g + 6 * lr;
+      pc = P + (size_t)(15 + 6 * ck[g]) * ldp + c;
     }
-    for (int r = t; r < m; r += kLmkThreads) {
+    double s = 0.0;
+    for (int j = lr; j < w; ++j) s += T[j] * (double)pc[(size_t)(MAP ? 15 + 6 * cl[j / 6] + j % 6 : j) * ldp];
+    A[(size_t)(m + c) * ld + r] = s;
+  }
+  for (int r = t; r < m; r += kLmkThreads) {
+    if constexpr (MAP) {
       int w;
       const int* cl;
       const double* T = lmk_map_row(a.m[f], slot, grp, G, rg[r], 0, w, cl);
       A[(size_t)(m + n) * ld + r] = T[(rg[r] < G ? 36 : kLmkSetLd * kLmkSetLd) + r - off[rg[r]]];
+    } else {
+      A[(size_t)(m + n) * ld + r] = slot[(size_t)kLmkSlot * rg[r] + 36 + r - off[rg[r]]];
     }
-    __syncthreads();
-    for (int idx = t; idx < m * m; idx += kLmkThreads) {
-      const int r = idx / m, s_ = idx - r * m;
-      if (s_ > r) continue;
-      const int h = rg[s_], ls = s_ - off[h];
-      int w;
-      const int* cl;
-      const double* T = lmk_map_row(a.m[f], slot, grp, G, h, ls, w, cl);
-      const double* tp = A + (size_t)(m + 15) * ld + r;
-      double v = r == s_ ? 1.0 : 0.0;
-      for (int j = ls; j < w; ++j) v += tp[(size_t)(6 * cl[j / 6] + j % 6) * ld] * T[j];
-      A[(size_t)r * ld + s_] = v;
-    }
-  } else {
-  // ---- (T P)^T into rows m .. m + n - 1, rho into row m + n
-  for (int idx = t; idx < m * n; idx += kLmkThreads) {
-    const int r = idx / n, c = idx - r * n, g = rg[r], lr = r - off[g];
-    const double* T = slot + (size_t)kLmkSlot * g + 6 * lr;
-    const S* pc = P + (size_t)(15 + 6 * ck[g]) * ldp + c;
-    double s = 0.0;
-    for (int j = lr; j < 6; ++j) s += T[j] * (double)pc[(size_t)j * ldp];
-    A[(size_t)(m + c) * ld + r] = s;
   }
-  for (int r = t; r < m; r += kLmkThreads) A[(size_t)(m + n) * ld + r] = slot[(size_t)kLmkSlot * rg[r] + 36 + r - off[rg[r]]];
   __syncthreads();
   // ---- S = T P T^T + I, lower triangle
   for (int idx = t; idx < m * m; idx += kLmkThreads) {
     const int r = idx / m, s_ = idx - r * m;
     if (s_ > r) continue;
     const int h = rg[s_], ls = s_ - off[h];
-    const double* T = slot + (size_t)kLmkSlot * h + 6 * ls;
-    const double* tp = A + (size_t)(m + 15 + 6 * ck[h]) * ld + r;
+    const double* T;
+    const double* tp;
+    int w = 6;
+    [[maybe_unused]] const int* cl;
+    if constexpr (MAP) {
+      T = lmk_map_row(a.m[f], slot, grp, G, h, ls, w, cl);
+      tp = A + (size_t)(m + 15) * ld + r;
+    } else {
+      T = slot + (size_t)kLmkSlot * h + 6 * ls;
+      tp = A + (size_t)(m + 15 + 6 * ck[h]) * ld + r;
+    }
     double v = r == s_ ? 1.0 : 0.0;
-    for (int j = ls; j < 6; ++j) v += tp[(size_t)j * ld] * T[j];
+    for (int j = ls; j < w; ++j) v += tp[(size_t)(MAP ? 6 * cl[j / 6] + j % 6 : j) * ld] * T[j];
     A[(size_t)r * ld + s_] = v;
-  }
   }
   __syncthreads();
   // ---- Cholesky of [S ; (T P)^T ; rho^T] (m + n + 1 rows): the extra rows end as W^T and y
