@@ -341,24 +341,26 @@ __device__ __forceinline__ void ld6_odd(const S* p, S (&v)[6]) {
 }
 
 // ---- gate Cholesky, blocked by panels of 8 columns, all G threads of the track's group.
-// The matrix is the trailing block [3:, 3:] of the packed-lower 2L x 2L array Y (rho = 2L - 3 rows); the right-hand side
-// r[3:] rides along as row rho.  Only y = L^-1 r is wanted (gamma = |y|^2), so the factor itself is never written back.
+// The matrix is the packed-lower n x n array Y (n = 2L pivots from row 0); the kJRhs right-hand sides ride along as rows
+// n .. n + 3 of the augmented matrix, stored as contiguous rows of n at rhs (row q at rhs + q n).  Only L^-1 rhs is wanted (the
+// gate's quadratic forms), so the factor itself is never written back: each right-hand side row ends as L^-1 of itself.
 // Per panel:  (1) every thread that owns a row loads the 8 x 8 diagonal micro-block and factorises it redundantly in registers (static
 // indices, right-looking: the dependent chain of a pivot is rsqrt -> multiply -> one FMA) -- no shuffles, no barriers, no
-// pivot broadcast;  (2) every thread solves its own rows of the panel against that micro-block in registers (row rho = the
-// right-hand side: its 8 entries are final components of y);  (3) the solved panel goes to shared memory TRANSPOSED
-// ([8][Rp]: neighbouring threads touch neighbouring words), one barrier;  (4) trailing update in 4 x 4 register tiles over
-// the lower triangle, one barrier.  57 pivots cost 8 panels x 2 barriers instead of 57 dependent warp-wide steps
-// (round 1: one warp, shuffle + shared-memory round trip per pivot: over a third of k_jac).
+// pivot broadcast;  (2) every thread solves its own rows of the panel against that micro-block in registers (rows >= n = the
+// right-hand sides: their 8 entries are final);  (3) the solved panel goes to shared memory TRANSPOSED ([8][Rp]: neighbouring
+// threads touch neighbouring words), one barrier;  (4) trailing update in 4 x 4 register tiles over the lower triangle, one
+// barrier.  60 pivots cost 8 panels x 2 barriers instead of 60 dependent warp-wide steps (round 1: one warp, shuffle +
+// shared-memory round trip per pivot: over a third of k_jac).
 constexpr int kPW = 8;
+constexpr int kJRhs = 4;  // z, U(:,0), U(:,1), U(:,2)
 template <class S, int G>
-__device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restrict__ r, int L2, S* __restrict__ PnT, int Rp, int* s_fail, int grp) {
-  const int rho = L2 - 3, R = rho + 1, tid = threadIdx.x % G;
+__device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restrict__ rhs, int n, S* __restrict__ PnT, int Rp, int* s_fail, int grp) {
+  const int R = n + kJRhs, tid = threadIdx.x % G;
   if (tid == 0) *s_fail = 0;
   for (int e = tid; e < kPW * Rp; e += G) PnT[e] = S(0);  // (rows R..Rp-1 of a partial tile must read as zero)
   JGrp<G>::sync(grp);
-  for (int p0 = 0; p0 < rho; p0 += kPW) {
-    const int w = min(kPW, rho - p0);
+  for (int p0 = 0; p0 < n; p0 += kPW) {
+    const int w = min(kPW, n - p0);
     // (1) diagonal micro-block: lower triangle in registers, identity padding beyond w -- only in the threads that own a row
     // of this panel (the others would spend a fifth of the kernel's instructions on a result they never use)
     const int q0 = p0 + w;
@@ -367,7 +369,7 @@ __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restri
 #pragma unroll
       for (int a = 0; a < kPW; ++a)
 #pragma unroll
-        for (int b = 0; b <= a; ++b) Lm[a][b] = (a < w) ? Y[pk(3 + p0 + a, 3 + p0 + b)] : ((a == b) ? S(1) : S(0));
+        for (int b = 0; b <= a; ++b) Lm[a][b] = (a < w) ? Y[pk(p0 + a, p0 + b)] : ((a == b) ? S(1) : S(0));
       bool ok = true;
 #pragma unroll
       for (int j = 0; j < kPW; ++j) {
@@ -382,18 +384,13 @@ __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restri
 #pragma unroll
           for (int a = b; a < kPW; ++a) Lm[a][b] -= Lm[a][j] * Lm[b][j];
       }
-      if (!ok && tid == 0) *s_fail = 1;  // (thread 0 always owns a row: the right-hand side is row rho >= q0)
-      // (2) rows below the micro-block, and the right-hand side
+      if (!ok && tid == 0) *s_fail = 1;  // (thread 0 always owns a row: the right-hand sides are rows >= n >= q0)
+      // (2) rows below the micro-block, and the right-hand sides
       for (int i = q0 + tid; i < R; i += G) {
+        S* row = (i < n) ? Y + pk(i, p0) : rhs + (size_t)(i - n) * n + p0;
         S x[kPW];
-        if (i < rho) {
-          const S* row = Y + pk(3 + i, 3 + p0);
 #pragma unroll
-          for (int j = 0; j < kPW; ++j) x[j] = (j < w) ? row[j] : S(0);
-        } else {
-#pragma unroll
-          for (int j = 0; j < kPW; ++j) x[j] = (j < w) ? r[3 + p0 + j] : S(0);
-        }
+        for (int j = 0; j < kPW; ++j) x[j] = (j < w) ? row[j] : S(0);
 #pragma unroll
         for (int j = 0; j < kPW; ++j) {
           x[j] *= inv[j];
@@ -402,22 +399,23 @@ __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restri
         }
 #pragma unroll
         for (int j = 0; j < kPW; ++j) PnT[j * Rp + i] = x[j];
-        if (i == rho) {
+        if (i >= n) {
 #pragma unroll
-          for (int j = 0; j < kPW; ++j) if (j < w) r[3 + p0 + j] = x[j];  // final components of y
+          for (int j = 0; j < kPW; ++j) if (j < w) row[j] = x[j];  // final components of L^-1 rhs
         }
       }
     }
     JGrp<G>::sync(grp);
     if (*s_fail) return false;  // a non-positive pivot (uniform: read after the barrier)
-    // (4) trailing update: rows q0..R-1, columns q0..rho-1, lower triangle, 4 x 4 tiles (q0 is a multiple of 8 here)
-    const int nrows = R - q0;
-    if (nrows > 1) {
-      const int nt = (nrows + 3) >> 2, ntile = nt * (nt + 1) / 2;
+    // (4) trailing update: rows q0..R-1, columns q0..n-1, lower triangle, 4 x 4 tiles (q0 < n: a full panel, q0 a multiple
+    // of 8; after the last panel only right-hand-side rows are left, and they have no columns to update)
+    if (q0 < n) {
+      const int nt = (R - q0 + 3) >> 2, ntile = nt * (nt + 1) / 2;
       for (int q = tid; q < ntile; q += G) {
         int ti, tj;
         tri_tile_index(q, ti, tj);
         const int r0 = q0 + 4 * ti, c0 = q0 + 4 * tj;
+        if (c0 >= n) continue;  // (the tile of the right-hand sides against themselves)
         S acc[4][4];
 #pragma unroll
         for (int a = 0; a < 4; ++a)
@@ -440,8 +438,8 @@ __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restri
 #pragma unroll
           for (int b = 0; b < 4; ++b) {
             const int col = c0 + b;
-            if (col < rho && col <= row) {
-              if (row < rho) Y[pk(3 + row, 3 + col)] -= acc[a][b]; else r[3 + col] -= acc[a][b];
+            if (col < n && col <= row) {
+              if (row < n) Y[pk(row, col)] -= acc[a][b]; else rhs[(size_t)(row - n) * n + col] -= acc[a][b];
             }
           }
         }
@@ -454,12 +452,17 @@ __device__ __forceinline__ bool gate_chol_blocked(S* __restrict__ Y, S* __restri
 
 // shared memory of one track's group (rounded to 16 bytes), in units of S:
 //   r 2L | X 12L | V 6L (+ slack) | Ypacked L(2L+1)
-// with two aliases: W | F of the two-sided transform ([2L][3] each) take X's place once the compact outputs are written,
-// and the gate Cholesky's transposed panel PnT (8 x Rp, Rp = (2L + 1) & ~3, 16-byte aligned) lives on X | V once the
-// transform is done.  U (the first 3 columns of the feature's Q, fp64) is never stored: its rows are rebuilt from V where
-// they are needed (u_row).
+// Once the compact outputs are written X is dead: the gate's right-hand sides U^T ([3][2L], U rounded to S) take its first
+// 6L, right after r (which becomes z), so that the four right-hand-side rows are contiguous; and once they are built V is dead
+// too: the gate Cholesky's transposed panel PnT (8 x Rp, Rp = (2L + 7) & ~3 >= 2L + 4 rows, 16-byte aligned) follows U^T, over
+// the rest of X, V and the slack.  U (the first 3 columns of the feature's Q, fp64) is otherwise never stored: its rows are
+// rebuilt from V where they are needed (u_row).
+__host__ __device__ inline int jac_panel_rows(int L) { return (2 * L + 7) & ~3; }
 template <class S>
-__host__ __device__ inline size_t jac_xv_elems(int L) { return (size_t)(18 * L > 16 * L + 12 ? 18 * L : 16 * L + 12); }
+__host__ __device__ inline size_t jac_xv_elems(int L) {
+  const size_t gate = (size_t)6 * L + (16 / sizeof(S) - 1) + (size_t)kPW * jac_panel_rows(L);  // U^T | alignment | PnT
+  return (size_t)18 * L > gate ? (size_t)18 * L : gate;
+}
 template <class S>
 __host__ __device__ inline size_t jac_group_bytes(int L) {
   const size_t b = sizeof(S) * ((size_t)2 * L + jac_xv_elems<S>(L) + (size_t)L * (2 * L + 1));
@@ -603,11 +606,10 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   S* r = reinterpret_cast<S*>(gmem_sm);
   S* X = r + L2;
   S* V = X + 12 * L;
-  S* wv = X;            // [2L][3]  W = Y V     (X is dead by then)
-  S* Fv = wv + 3 * L2;  // [2L][3]  F of the two-sided transform
+  S* Ut = X;  // [3][2L]  U^T rounded to S, the gate's right-hand sides after z = r (X is dead by then)
   S* Y = X + jac_xv_elems<S>(L);
-  S* PnT = reinterpret_cast<S*>((reinterpret_cast<uintptr_t>(X) + 15) & ~uintptr_t(15));  // [8][Rp]; W, F, V are dead by then
-  const int Rp = (L2 + 1) & ~3;  // >= rho + 1 = 2L - 2, multiple of 4
+  S* PnT = reinterpret_cast<S*>((reinterpret_cast<uintptr_t>(Ut + 6 * L) + 15) & ~uintptr_t(15));  // [8][Rp]; V is dead by then
+  const int Rp = jac_panel_rows(L);  // >= 2L + 4 rows, multiple of 4
   const int* idx = a.clone_idx + o0;
   const S* z = a.obs + 2 * (size_t)o0;
   const DevState<S>* st = a.st;
@@ -665,14 +667,10 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
   Gp::sync(grp);
   stamp();  // X, r
   // ---- warp 0: column-pivoted Householder QR of H_f (2L x 3) -- the trailing 2L-3 columns of Q are A_j
-  // (msckf.h:954-955) -- then U, U^T r, r~ and the compact-WY factor, all warp-synchronous (shuffle reductions, no CTA
-  // barriers).  Warps 1..3 meanwhile: Y = X P_sub X^T.
-  __shared__ S s_tau_[Gp::TPC][3];
-  __shared__ S s_T_[Gp::TPC][9];
+  // (msckf.h:954-955) -- then U and U^T r, all warp-synchronous (shuffle reductions, no CTA barriers).  Warps 1..3
+  // meanwhile: Y = X P_sub X^T + u_var I.
   __shared__ double s_urv_[Gp::TPC][3];
   __shared__ double s_sd_[Gp::TPC][9];
-  S* s_tau = s_tau_[grp];
-  S* s_T = s_T_[grp];
   double* s_urv = s_urv_[grp];
   double* s_sd = s_sd_[grp];
   const int warp = tid >> 5;
@@ -741,17 +739,14 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
     // that Q = H_0 H_1 H_2 is orthogonal to 1e-16 whatever the filter precision: G_j = I - U_j U_j^T is an exact
     // projector and the body Gram terms and the explicit rows (k_rows) describe the same H_o.
     double tau64[3];
-    S vtv01 = 0, vtv02 = 0, vtv12 = 0;  // v_a^T v_b for the compact-WY factor
     {
       double vv3[3] = {0.0, 0.0, 0.0};
       _Pragma("unroll 1") for (int row = lane; row < L2; row += 32) {  // v_k is zero above row k
         const S v0 = V[3 * row], v1 = V[3 * row + 1], v2 = V[3 * row + 2];
         vv3[0] += (double)v0 * (double)v0; vv3[1] += (double)v1 * (double)v1; vv3[2] += (double)v2 * (double)v2;
-        vtv01 += v0 * v1; vtv02 += v0 * v2; vtv12 += v1 * v2;
       }
 #pragma unroll
       for (int k = 0; k < 3; ++k) { vv3[k] = warp_sum_call(vv3[k]); tau64[k] = (tau[k] != S(0)) ? 2.0 / vv3[k] : 0.0; }
-      vtv01 = warp_sum_call(vtv01); vtv02 = warp_sum_call(vtv02); vtv12 = warp_sum_call(vtv12);
     }
     // ---- U = Q(:,0:3) = H0 H1 H2 [I3; 0]  (fp64), kept as the nine coefficients sd_k of u_row
     double sd[9];
@@ -784,34 +779,15 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
       for (int q = 0; q < 3; ++q) urv[q] = warp_sum_call(urv[q]);
       if (lane == 0) { s_urv[0] = urv[0]; s_urv[1] = urv[1]; s_urv[2] = urv[2]; }
     }
-    // ---- r~ = H2 H1 H0 r in the filter precision (r_o = r~[3:], used by the gate only)
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      S sacc = 0;
-      _Pragma("unroll 1") for (int row = k + lane; row < L2; row += 32) sacc += V[3 * row + k] * r[row];
-      const S sdot = tau[k] * warp_sum_call(sacc);
-      _Pragma("unroll 1") for (int row = k + lane; row < L2; row += 32) r[row] -= sdot * V[3 * row + k];
-      __syncwarp();
-    }
-    // ---- compact WY: H0 H1 H2 = I - V T V^T, T upper triangular (forward accumulation)
-    if (lane == 0) {
-      const S t00 = tau[0], t11 = tau[1], t22 = tau[2];
-      const S t01 = -t11 * (t00 * vtv01);
-      const S t02 = -t22 * (t00 * vtv02 + t01 * vtv12);
-      const S t12 = -t22 * (t11 * vtv12);
-      s_T[0] = t00; s_T[1] = t01; s_T[2] = t02;
-      s_T[3] = S(0); s_T[4] = t11; s_T[5] = t12;
-      s_T[6] = S(0); s_T[7] = S(0); s_T[8] = t22;
-      s_tau[0] = t00; s_tau[1] = t11; s_tau[2] = t22;
-    }
   }
   if (G == 32 || warp != 0) {  // (a single-warp group does both, one after the other)
     // ---- gating (msckf.h:1103-1124): gamma = r_o^T (H_o P H_o^T + u_var I)^-1 r_o with H_o = (Q^T X)[3:]
-    // Y = X P_sub X^T, symmetric 2L x 2L, packed lower, by 2 x 2 blocks (i, k), k <= i.  Block rows i and L-1-i share a pass
+    // Y = X P_sub X^T + u_var I, symmetric 2L x 2L, packed lower, by 2 x 2 blocks (i, k), k <= i.  Block rows i and L-1-i share a pass
     // of L + 1 blocks (lane e takes (i, e) for e <= i, else (L-1-i, e-i-1)): no pair decode, and the lanes of a pass read P
     // along the same two block rows.  Each block's sums run in the same order whichever thread computes it.
     const S* P = a.P;
     const int ldp = a.ldp;
+    const S uvar = st->u_var;
     constexpr int YW = (G == 32) ? 1 : G / 32 - 1;  // warps on the pairs
     for (int ps = (G == 32) ? 0 : warp - 1; ps < (L + 1) / 2; ps += YW) {
       const int ilo = ps, ihi = L - 1 - ps, ne = (ilo == ihi) ? ilo + 1 : L + 1;
@@ -844,17 +820,16 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
         }
         S* y0 = Y + pk(2 * i, 2 * k);
         S* y1 = y0 + 2 * i + 1;  // pk(2i + 1, 2k)
-        y0[0] = y00;
+        y0[0] = (i == k) ? y00 + uvar : y00;
         y1[0] = y10;
-        y1[1] = y11;
+        y1[1] = (i == k) ? y11 + uvar : y11;
         if (i != k) y0[1] = y01;
       }
     }
   }
   Gp::sync(grp);
-  stamp();  // QR, U, r~ (warp 0) | Y pairs (warps 1..3)
-  const double urv[3] = {s_urv[0], s_urv[1], s_urv[2]};
-  // ---- compact outputs for the Gram stage, written as if accepted (X's shared memory is about to become W | F); a rejected
+  stamp();  // QR, U (warp 0) | Y pairs (warps 1..3)
+  // ---- compact outputs for the Gram stage, written as if accepted (X's shared memory is about to become U^T); a rejected
   // track zeroes them again after the gate
   for (int k = tid; k < 3 * c; k += G) { Zr[k] = 0.0; Yr[k] = 0.0; }
   double Mm[6];  // M = U^T D U (3x3 symmetric), D = diag(u_var, v_var, u_var, ...)
@@ -893,81 +868,39 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
       }
     }
   }
-  Gp::sync(grp);  // X is dead: W, F take its place
-  // ---- two-sided transform in one pass: Q^T Y Q = Y - (V F^T + F V^T),  F = W T - V (T^T B T) / 2,  W = Y V,  B = V^T W
-  S* Wv = wv;  // [L2][3]
-  {
-    // W = Y V: a thread per row, L2 steps each (the row part b <= ar and the column part b > ar of the packed symmetric
-    // storage are summed apart, then added)
-    for (int ar = tid; ar < L2; ar += G) {
-      S w0 = 0, w1 = 0, w2 = 0, c0 = 0, c1 = 0, c2 = 0;
-      const S* y = Y + pk(ar, 0);
-      for (int b = 0; b <= ar; ++b) { const S yv = y[b]; w0 += yv * V[3 * b]; w1 += yv * V[3 * b + 1]; w2 += yv * V[3 * b + 2]; }
-      y = Y + pk(ar + 1, ar);
-      for (int b = ar + 1; b < L2; y += ++b) { const S yv = *y; c0 += yv * V[3 * b]; c1 += yv * V[3 * b + 1]; c2 += yv * V[3 * b + 2]; }
-      Wv[3 * ar] = w0 + c0; Wv[3 * ar + 1] = w1 + c1; Wv[3 * ar + 2] = w2 + c2;
-    }
+  Gp::sync(grp);  // X is dead: U^T takes its place
+  // ---- gate (msckf.h:1103-1124) without forming S = A^T Y A + u_var I: with M = Y + u_var I (SPD) and [U A] orthogonal,
+  // the Schur complement of (Q^T M Q)^-1 = Q^T M^-1 Q gives
+  //   gamma = r_o^T S^-1 r_o = z^T M^-1 z - (U^T M^-1 z)^T (U^T M^-1 U)^-1 (U^T M^-1 z),  z = A r_o = r - U (U^T r),
+  // so with M = L L^T, a = L^-1 z, B = L^-1 U and c = B^T a:  gamma = a^T a - c^T (B^T B)^-1 c.  The right-hand sides of the
+  // Cholesky of M are z (in r's place) and the three columns of U (rows of U^T).
+  for (int row = tid; row < L2; row += G) {
+    double u[3];
+    u_row(V, s_sd, row, 0, u);
+    r[row] = (S)((double)r[row] - (u[0] * s_urv[0] + u[1] * s_urv[1] + u[2] * s_urv[2]));
+    Ut[row] = (S)u[0]; Ut[L2 + row] = (S)u[1]; Ut[2 * L2 + row] = (S)u[2];
   }
-  Gp::sync(grp);
-  if (warp == 0) {
-    S Bm[6] = {0, 0, 0, 0, 0, 0};  // B = V^T W (symmetric): 00 01 02 11 12 22
-    for (int row = lane; row < L2; row += 32) {
-      const S v0 = V[3 * row], v1 = V[3 * row + 1], v2 = V[3 * row + 2];
-      const S w0 = Wv[3 * row], w1 = Wv[3 * row + 1], w2 = Wv[3 * row + 2];
-      Bm[0] += v0 * w0; Bm[1] += v0 * w1; Bm[2] += v0 * w2; Bm[3] += v1 * w1; Bm[4] += v1 * w2; Bm[5] += v2 * w2;
-    }
-#pragma unroll
-    for (int q = 0; q < 6; ++q) Bm[q] = warp_sum_call(Bm[q]);
-    const S Bf[3][3] = {{Bm[0], Bm[1], Bm[2]}, {Bm[1], Bm[3], Bm[4]}, {Bm[2], Bm[4], Bm[5]}};
-    S Tm[3][3], BT[3][3], G3[3][3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) Tm[i][j] = s_T[3 * i + j];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) BT[i][j] = Bf[i][0] * Tm[0][j] + Bf[i][1] * Tm[1][j] + Bf[i][2] * Tm[2][j];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) G3[i][j] = S(0.5) * (Tm[0][i] * BT[0][j] + Tm[1][i] * BT[1][j] + Tm[2][i] * BT[2][j]);
-    __syncwarp();
-    for (int row = lane; row < L2; row += 32) {
-      const S v0 = V[3 * row], v1 = V[3 * row + 1], v2 = V[3 * row + 2];
-      const S w0 = Wv[3 * row], w1 = Wv[3 * row + 1], w2 = Wv[3 * row + 2];
-#pragma unroll
-      for (int j = 0; j < 3; ++j)
-        Fv[3 * row + j] = (w0 * Tm[0][j] + w1 * Tm[1][j] + w2 * Tm[2][j]) - (v0 * G3[0][j] + v1 * G3[1][j] + v2 * G3[2][j]);
-    }
-  }
-  Gp::sync(grp);
-  // only the trailing block [3:, 3:] is used below: S = (Q^T Y Q)[3:,3:] + u_var I, in place in the packed array
-  const S uvar = st->u_var;
-  const int rho = L2 - 3;
-  // rows 3 + f and L2 - 1 - f share a warp pass of rho + 1 entries, lanes along the two rows
-  for (int f = warp; f < (rho + 1) / 2; f += G / 32) {
-    const int rlo = 3 + f, rhi = L2 - 1 - f, ne = (rlo == rhi) ? f + 1 : rho + 1;
-    for (int e = lane; e < ne; e += 32) {
-      const int ar = (e <= f) ? rlo : rhi, b = 3 + ((e <= f) ? e : e - f - 1);
-      const S va0 = V[3 * ar], va1 = V[3 * ar + 1], va2 = V[3 * ar + 2];
-      const S fa0 = Fv[3 * ar], fa1 = Fv[3 * ar + 1], fa2 = Fv[3 * ar + 2];
-      const S val = Y[pk(ar, b)] - ((va0 * Fv[3 * b] + va1 * Fv[3 * b + 1] + va2 * Fv[3 * b + 2]) + (fa0 * V[3 * b] + fa1 * V[3 * b + 1] + fa2 * V[3 * b + 2]));
-      Y[pk(ar, b)] = (b == ar) ? val + uvar : val;
-    }
-  }
-  Gp::sync(grp);
-  stamp();  // two-sided transform
-  // Cholesky with the right-hand side r~[3:] riding along as an extra row: y = L^-1 r~, gamma = |y|^2
+  Gp::sync(grp);  // V is dead: PnT takes its place
+  stamp();  // compact outputs, right-hand sides
   __shared__ int s_chol_fail[Gp::TPC];
-  const bool chol_ok = gate_chol_blocked<S, G>(Y, r, L2, PnT, Rp, &s_chol_fail[grp], grp);
-  (void)rho;
-  S gam1[1];
-  group_vsum<G, 1>(gam1, [&](int v, S (&p)[1]) {
-    p[0] = S(0);
-    for (int j = 3 + v; j < L2; j += 128) p[0] += r[j] * r[j];
+  bool chol_ok = gate_chol_blocked<S, G>(Y, r, L2, PnT, Rp, &s_chol_fail[grp], grp);
+  // a^T a, c = B^T a, B^T B (00 01 02 11 12 22): r holds a, Ut holds B^T
+  S qf[10];
+  group_vsum<G, 10>(qf, [&](int v, S (&p)[10]) {
+    for (int k = 0; k < 10; ++k) p[k] = S(0);
+    for (int j = v; j < L2; j += 128) {
+      const S aj = r[j], b0 = Ut[j], b1 = Ut[L2 + j], b2 = Ut[2 * L2 + j];
+      p[0] += aj * aj; p[1] += b0 * aj; p[2] += b1 * aj; p[3] += b2 * aj;
+      p[4] += b0 * b0; p[5] += b0 * b1; p[6] += b0 * b2; p[7] += b1 * b1; p[8] += b1 * b2; p[9] += b2 * b2;
+    }
   }, reds, grp);
-  S gam = gam1[0];
+  // c^T (B^T B)^-1 c = |l^-1 c|^2 with B^T B = l l^T (3 x 3, in registers)
+  const S l00 = tsqrt<S>(qf[4]), l10 = qf[5] / l00, l20 = qf[6] / l00;
+  const S d11 = qf[7] - l10 * l10, l11 = tsqrt<S>(d11), l21 = (qf[8] - l20 * l10) / l11;
+  const S d22 = qf[9] - (l20 * l20 + l21 * l21), l22 = tsqrt<S>(d22);
+  const S w0 = qf[1] / l00, w1 = (qf[2] - l10 * w0) / l11, w2 = (qf[3] - (l20 * w0 + l21 * w1)) / l22;
+  if (!(qf[4] > S(0) && d11 > S(0) && d22 > S(0))) chol_ok = false;
+  S gam = qf[0] - ((w0 * w0 + w1 * w1) + w2 * w2);
   const int acc = chol_ok && (gam < st->chi2[L]);  // table[dof+1], dof = L-1 (msckf.h:433,:1117)
   if (!chol_ok) gam = S(1e30);
   stamp();  // Cholesky + gamma
@@ -982,14 +915,14 @@ __device__ __forceinline__ void jac_track(const UpdArgs<S>& a, const int t, cons
     a.accept[t] = acc;
     a.gamma[t] = gam;
     a.rows[t] = acc ? (L2 - 3) : 0;
-    for (int q = 0; q < 3; ++q) a.ur[3 * t + q] = acc ? urv[q] : 0.0;
+    for (int q = 0; q < 3; ++q) a.ur[3 * t + q] = acc ? s_urv[q] : 0.0;
   }
   stamp();  // outputs
   if (a.prof && blockIdx.x == 0 && threadIdx.x == 0) a.prof[40 + prof_i] = 0ull;
 }
 
 // (G = 32, fp32: 10 CTAs = 20 tracks per SM, the 2 640 resident tracks a batch of 8 config-B filters needs to run in one
-// wave -- 96 registers and 10 x (2 x 9.7 KB) of shared memory at L = 30)
+// wave -- 96 registers and 10 x (2 x 10.3 KB) of shared memory at L = 30)
 template <class S, int G>
 __global__ void __launch_bounds__(JGrp<G>::CT, (G == 32) ? (sizeof(S) == 4 ? 10 : 5) : (sizeof(S) == 4 ? 5 : 3)) k_jac(const UpdArgs<S>* __restrict__ args) {
   pdl_wait();
@@ -1008,8 +941,11 @@ __global__ void __launch_bounds__(JGrp<G>::CT, (G == 32) ? (sizeof(S) == 4 ? 10 
     wp += 16 + sizeof(S) * kPoseStride * (size_t)a.M;
     wp = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(wp) + 15) & ~uintptr_t(15));
   }
-  __shared__ double redd[TPC * 4 * 6];
-  __shared__ S reds[TPC * 4];
+  // group_vsum's slots, one array per element type so that every group of the CTA owns its own bytes in both (the groups of
+  // a CTA synchronise only among themselves): 6 doubles (M = U^T D U) and 10 S (the gate's quadratic forms) per virtual warp;
+  // a single-warp group reduces by shuffles alone
+  __shared__ double redd[(G == 32) ? 1 : TPC * 4 * 6];
+  __shared__ S reds[(G == 32) ? 1 : TPC * 4 * 10];
   __shared__ int redi[CT / 32];
   const int grp = threadIdx.x / G, t = blockIdx.x * TPC + grp;
   if (t < N) jac_track<S, G>(a, t, grp, wp + (size_t)grp * jac_group_bytes<S>(a.Lmax), poses, redd, reds, redi);

@@ -13,7 +13,7 @@ ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from msckf_mono_b200 import capi, engine_filter, synth  # noqa: E402
 
-PHASES = ["bookkeeping", "X/r", "QR|Y pairs", "two-sided transform", "gate Cholesky", "outputs"]
+PHASES = ["bookkeeping", "X/r", "QR|Y pairs", "Z/Yq, right-hand sides", "gate Cholesky", "outputs"]
 
 
 def run(nf, nfeat=300, nclones=30, dtype=np.float32, reps=6):
