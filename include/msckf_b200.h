@@ -53,7 +53,9 @@ typedef struct {
  * engine grows its device buffers on demand (x2, contents preserved).  Hard limits that remain: 98 observations per track
  * (the reference's chi-square table has 99 entries, msckf.h:91 -- longer tracks index past it there) and the window the
  * tail kernel's shared-memory panels can hold (136 clones; an update of a larger window fails at staging and writes nothing):
- * they fail with MSCKF_B200_ERR_ARG / _CAPACITY. */
+ * they fail with MSCKF_B200_ERR_ARG / _CAPACITY.  A track names each clone at most once (MSCKF sees a feature once per
+ * image); a track that names one clone twice fails with MSCKF_B200_ERR_ARG.  Such failures come before anything is launched:
+ * nothing is written, and in a device batch no member is. */
 
 /* One batch of feature tracks, flat SoA (types.h:102-113 featureTrackToResidualize without the clone copies:
  * the clone poses are device resident and addressed by POSITION in the sliding window, msckf.h:1481). */
@@ -61,7 +63,8 @@ typedef struct {
   int n_tracks;
   const int* obs_offset;  /* [n_tracks+1] prefix offsets into obs / clone_index */
   const void* obs;        /* [2*obs_offset[n_tracks]] normalised image coordinates (u,v), dtype scalars */
-  const int* clone_index; /* [obs_offset[n_tracks]] positional index of the observing clone */
+  const int* clone_index; /* [obs_offset[n_tracks]] positional index of the observing clone, each at most once per track, in
+                             any order */
   const void* p_f_G;      /* MSCKF_B200_RESIDUALIZE only: [3*n_tracks] feature positions; else NULL */
 } msckf_b200_tracks;
 

@@ -1027,8 +1027,16 @@ int Ctx<S>::stage(int mode, const msckf_b200_tracks* tracks, int threads) {
       lm = std::max(lm, L);
     }
     const int Mi = e->M;
-    for (int o = 0; o < O; ++o)
-      if ((unsigned)tr.clone_index[o] >= (unsigned)Mi) return fail(MSCKF_B200_ERR_ARG, "clone_index out of range");
+    // one observation per clone and track: MSCKF sees a feature once per image, and k_jac writes a track's compact Gram
+    // outputs one clone column per observation, so a clone named twice would keep only one of its observations' terms
+    std::vector<int> seen(Mi, -1);
+    for (int t = 0; t < N; ++t)
+      for (int o = tr.obs_offset[t]; o < tr.obs_offset[t + 1]; ++o) {
+        const int k = tr.clone_index[o];
+        if ((unsigned)k >= (unsigned)Mi) return fail(MSCKF_B200_ERR_ARG, "clone_index out of range");
+        if (seen[k] == t) return fail(MSCKF_B200_ERR_ARG, "a track names one clone twice");
+        seen[k] = t;
+      }
     if (mode == MSCKF_B200_RESIDUALIZE && !tr.p_f_G) return fail(MSCKF_B200_ERR_ARG, "RESIDUALIZE needs p_f_G");
     NO[i] = {N, O};
     Lmax[i] = lm;

@@ -62,8 +62,11 @@ int msckf_b200_stage(msckf_b200_engine* e, int mode, const msckf_b200_tracks* tr
   for (int t = 0; t < tr->n_tracks; ++t) {
     const int L = tr->obs_offset[t + 1] - tr->obs_offset[t];
     if (L < 1 || L > 98) return fail(MSCKF_B200_ERR_ARG, "stub: bad track length");
-    for (int o = tr->obs_offset[t]; o < tr->obs_offset[t + 1]; ++o)
+    for (int o = tr->obs_offset[t]; o < tr->obs_offset[t + 1]; ++o) {
       if (tr->clone_index[o] < 0 || tr->clone_index[o] >= e->M) return fail(MSCKF_B200_ERR_ARG, "stub: clone_index out of range");
+      for (int q = tr->obs_offset[t]; q < o; ++q)
+        if (tr->clone_index[q] == tr->clone_index[o]) return fail(MSCKF_B200_ERR_ARG, "stub: a track names one clone twice");
+    }
     e->last_len.push_back(L);
   }
   e->mode = mode;

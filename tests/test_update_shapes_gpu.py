@@ -97,10 +97,13 @@ def expect(e, tracks, dtype, noise=None):
     return ref
 
 
-def compare(e, rep, ref, tracks, dtype, label, bounds=None):
+def compare(e, rep, ref, tracks, dtype, label, bounds=None, noise_floor=0.0):
     """the update's report and the engine's state after it against the reference: flags, m and rank exactly (and the rank
     pivots' gap), the numbers against CONTRACT and 10 x MEASURED (or against the (contract, measured) pair of one dtype that
-    bounds(dtype name, rank above the reference's) gives); returns the numbers"""
+    bounds(dtype name, rank above the reference's) gives); returns the numbers.  noise_floor: the rank decision's largest
+    noise pivot in a plain fp64 evaluation of the same Gram form (vision_reference.gram_noise), where the model below
+    underestimates it; the engine's is held to 10 x that there, and a noise pivot that lands above the threshold inside
+    that band may be kept or dropped, as in fp32"""
     name = np.dtype(dtype).name
     lengths = np.array([len(t["idx"]) for t in tracks])
     assert np.array_equal(rep["accepted"].astype(bool), ref["accepted"]), (label, rep["accepted"], ref["accepted"])
@@ -130,11 +133,11 @@ def compare(e, rep, ref, tracks, dtype, label, bounds=None):
     # leaves a null direction a pivot of about eps * n * cond(Gamma), cond(Gamma) ~ 1 / (smallest real pivot).  A kernel that
     # made it larger than that model allows would otherwise hide in the count of noise pivots kept below
     eps = np.finfo(np.float64 if name == "float64" else np.float32).eps  # the Jacobians are formed in the filter's type
-    assert noise <= 100 * eps * n / real.min(), (label, noise, real.min())
+    assert noise <= max(100 * eps * n / real.min(), 10 * noise_floor), (label, noise, real.min(), noise_floor)
     extra = int(np.sum(null > 1e-9))
-    if name == "float64":
+    if name == "float64" and not noise_floor:
         assert rep["rank"] == ref["rank"] + extra, (label, rep["rank"], ref["rank"], noise)
-    else:  # a Gamma direction kept on noise may still be dropped by its S'' pivot
+    else:  # a Gamma direction kept on noise may still be dropped by its S'' pivot (fp64: within the Gram form's noise floor)
         assert ref["rank"] <= rep["rank"] <= ref["rank"] + extra, (label, rep["rank"], ref["rank"], noise)
     contract, measured = (CONTRACT[name], MEASURED[name]) if bounds is None else bounds(name, rep["rank"] - ref["rank"])
     fin = lengths >= 2

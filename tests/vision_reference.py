@@ -28,7 +28,7 @@ import numpy as np
 import scipy.linalg as sla
 
 from msckf_mono_b200 import synth
-from oracle.msckf_numpy import MSCKF as NumpyMSCKF, CamState, chi2_table, quat_mul, quat_normalized, quat_to_rot
+from oracle.msckf_numpy import MSCKF as NumpyMSCKF, CamState, chi2_table, quat_mul, quat_normalized, quat_to_rot, skew
 
 CHI2 = chi2_table(np.float64)  # CHI2[L]: the gate of a track of L observations (table[dof + 1], dof = L - 1)
 NOISE = synth.euroc_noise(isotropic=True, tuned=True)
@@ -150,6 +150,52 @@ def make_tracks(rng, poses, lengths, unseen=(), outliers=(), noise=np.sqrt(SIGMA
             obs[1::3] += 0.1 * rng.choice([-1.0, 1.0], size=obs[1::3].shape)
         out.append({"idx": idx.astype(np.int32), "obs": obs, "pfg": p + offset * rng.normal(size=3) / np.sqrt(3)})
     return out
+
+
+def gate_delta(L, dtype):
+    """how far threshold_tracks places a track of L observations from its threshold, relative to CHI2[L]: fp64 1e-9 (over
+    100 x the engine's measured gamma error); fp32 0.4 x the relative distance from CHI2[L] to the nearer neighbouring entry
+    (CHI2[L - 1], or CHI2[L + 1] below L = 98), so that a gate reading a neighbouring entry flips one track of each pair"""
+    if np.dtype(dtype) == np.float64:
+        return 1e-9
+    near = [CHI2[L - 1]] + ([CHI2[L + 1]] if L + 1 < len(CHI2) else [])
+    return 0.4 * min(abs(x / CHI2[L] - 1) for x in near)
+
+
+def threshold_tracks(rng, P, imu, poses, lengths, sides, dtype, delta):
+    """(tracks, gamma): tracks of the given lengths (make_tracks' clone subsets and landmarks, p_f_G the landmark itself) whose
+    reference gamma is CHI2[L] (1 + side delta), side -1 (accepted) or +1 (rejected) per track, delta a scalar or one per
+    track; as an engine of `dtype` receives them (observations and p_f_G rounded to dtype, in fp64), at the covariance P and
+    state (imu, poses) the update will see.  The observations are the exact projections of p_f_G plus s d, d a random
+    pixel-noise direction: H_o and A_j do not depend on z, so gamma(s) = s^2 gamma(1).  s is rescaled to the target and the
+    gamma of the rounded track recomputed, four times (rounding to fp32 moves gamma by ~1e-5 of itself)"""
+    tracks = rounded(make_tracks(rng, poses, lengths, noise=0.0, offset=0.0), dtype)
+    delta = np.broadcast_to(np.asarray(delta, dtype=np.float64), (len(tracks),))
+    target = np.array([CHI2[len(t["idx"])] * (1 + s * d) for t, s, d in zip(tracks, sides, delta)])
+    exact = [np.array([project(poses[k], t["pfg"])[1] for k in t["idx"]]) for t in tracks]
+    dirs = [np.sqrt(SIGMA2) * rng.normal(size=x.shape) for x in exact]
+    scale = np.ones(len(tracks))
+    for it in range(5):
+        cur = [dict(t, obs=(x + s * d).astype(dtype).astype(np.float64)) for t, x, d, s in zip(tracks, exact, dirs, scale)]
+        gam, _ = gate(P, project_tracks(imu, poses, cur), cur)
+        scale = scale * np.sqrt(target / gam)
+    return cur, gam
+
+
+def threshold_sides(lengths):
+    """a pair of tracks per length: -1 (just below the threshold: accepted) / +1 (just above: rejected), the pair in the order
+    (-1, +1) at even lengths and (+1, -1) at odd ones, so that accepted and rejected tracks alternate and a CTA of two tracks
+    holds one of each, in both orders; (track lengths, sides)"""
+    return [L for L in lengths for _ in (0, 1)], [s if L % 2 == 0 else -s for L in lengths for s in (-1, 1)]
+
+
+def threshold_pairs(rng, P, imu, poses, lengths, dtype):
+    """(tracks, gamma, target, sides) of threshold_sides' pairs of the given lengths at gate_delta's distance from CHI2[L]"""
+    ls, sides = threshold_sides(lengths)
+    delta = np.array([gate_delta(L, dtype) for L in ls])
+    tracks, gam = threshold_tracks(rng, P, imu, poses, ls, sides, dtype, delta)
+    target = np.array([CHI2[L] * (1 + s * d) for L, s, d in zip(ls, sides, delta)])
+    return tracks, gam, target, np.array(sides)
 
 
 def pack(tracks, dtype):
@@ -304,6 +350,66 @@ def reference(P, imu, poses, tracks, noise=None, blocks=None):
     if out["m"]:
         out["imu"], out["poses"] = inject(np.asarray(imu, np.float64), np.asarray(poses, np.float64), out["dx"])
     return out
+
+
+def _unprojected(imu, poses, t):
+    """(X_j [2L, n], U_j [2L, 3]) of a track: its measurement Jacobian with the observability projection, before the left
+    null-space projection (as msckf_numpy's _calc_meas_jacobian forms it), and an orthonormal basis of range(H_f)"""
+    g = np.asarray(imu[12:15], np.float64)
+    n, L = 15 + 6 * len(poses), len(t["idx"])
+    X, Hf = np.zeros((2 * L, n)), np.zeros((2 * L, 3))
+    for i, k in enumerate(t["idx"]):
+        C = quat_to_rot(poses[k, 3:7])
+        d = t["pfg"] - poses[k, 0:3]
+        pc = C @ d
+        J = np.array([[1.0, 0.0, -pc[0] / pc[2]], [0.0, 1.0, -pc[1] / pc[2]]]) / pc[2]
+        A = np.hstack([J @ skew(pc), -J @ C])
+        u = np.concatenate([C @ g, skew(d) @ g])
+        H = A - np.outer(A @ u, u) / (u @ u)
+        Hf[2 * i:2 * i + 2] = -H[:, 3:6]
+        X[2 * i:2 * i + 2, 15 + 6 * k:21 + 6 * k] = H
+    return X, np.linalg.qr(Hf, mode="complete")[0][:, :3]
+
+
+def skip_cholesky_pivots(G, thr=1e-9):
+    """the relative pivots (pivot / original diagonal) of a Cholesky of G that skips a column whose pivot is not above thr
+    times its original diagonal, in column order: the engine's rank decision (DESIGN.md 4.4)"""
+    G = np.array(G, dtype=np.float64)
+    d0 = np.diag(G).copy()
+    piv = np.zeros(len(G))
+    for k in range(len(G)):
+        p = G[k, k]
+        piv[k] = p / d0[k] if d0[k] > 0 else 0.0
+        if not (d0[k] > 0 and p > thr * d0[k]):
+            G[k, :] = 0.0
+            G[:, k] = 0.0
+            continue
+        col = G[k:, k] / np.sqrt(p)
+        G[k:, k:] -= np.outer(col, col)
+    return piv
+
+
+def gram_noise(imu, poses, tracks, ref):
+    """the largest rounding-noise pivot of the rank decision evaluated in fp64 in the engine's own Gram form: Gamma =
+    [[I, H_h], [H_h^T, Lambda]], Lambda = sum_j X_j^T X_j - Z_j^T Z_j, Z_j = U_j^T X_j over the accepted tracks (DESIGN.md
+    4.4), factorised by skip_cholesky_pivots, the pivots beyond the reference's rank; 0 when m <= n (no decision).  The
+    Gram form's noise is a property of the formula, not of the kernel that evaluates it: on 130 threshold tracks over 70
+    clones it reaches 3e-9 where the reference's own H_o^T H_o gives 5e-10 (tests/test_gate_threshold_cpu.py)"""
+    if ref["sv"] is None:
+        return 0.0
+    n = ref["H_o"].shape[1]
+    G = np.zeros((n, n))
+    for t, a in zip(tracks, ref["accepted"]):
+        if a:
+            X, U = _unprojected(imu, poses, t)
+            Z = U.T @ X
+            G += X.T @ X - Z.T @ Z
+    Hh = ref["H_o"][:15, 15:]
+    G[:15, :15] = np.eye(15)
+    G[:15, 15:] = Hh
+    G[15:, :15] = Hh.T
+    pv = np.sort(skip_cholesky_pivots(G))[::-1]
+    return float(np.abs(pv[ref["rank"]:]).max()) if n > ref["rank"] else 0.0
 
 
 def gate_margin(ref, tracks):
