@@ -221,7 +221,11 @@ enum msckf_b200_aid_model {
   MSCKF_B200_AID_ANTENNA_POSITION = 7,       /* stacks only: GNSS */
   MSCKF_B200_AID_CLONE_ANTENNA_POSITION = 8, /* stacks only */
   MSCKF_B200_AID_HEADING = 9,                /* stacks only */
-  MSCKF_B200_AID_CLONE_HEADING = 10          /* stacks only */
+  MSCKF_B200_AID_CLONE_HEADING = 10,         /* stacks only */
+  MSCKF_B200_AID_RANGE = 11,                 /* stacks only: radio ranging to a surveyed anchor */
+  MSCKF_B200_AID_CLONE_RANGE = 12,           /* stacks only */
+  MSCKF_B200_AID_PLANE_RANGE = 13,           /* stacks only: a rangefinder over a level plane */
+  MSCKF_B200_AID_CLONE_PLANE_RANGE = 14      /* stacks only */
 };
 typedef struct {
   int model;          /* msckf_b200_aid_model; in a batch, < 0 leaves that member untouched */
@@ -238,7 +242,9 @@ typedef struct {
   int dof;            /* m */
   int applied;        /* 1: P and the state were updated */
   int status;         /* 0: applied or gated out (see applied); 1: S not positive definite, nothing written; 2 (stacks
-                         only): a HEADING / CLONE_HEADING axis within ~1e-3 rad of vertical (yaw undefined), nothing written */
+                         only): a HEADING / CLONE_HEADING axis within ~1e-3 rad of vertical (yaw undefined), a RANGE /
+                         CLONE_RANGE antenna within 1e-6 m of its anchor, or a PLANE_RANGE / CLONE_PLANE_RANGE beam within
+                         ~1e-3 rad of the plane or with the plane behind it; nothing written */
 } msckf_b200_aid_result;
 /* A bad model, an out-of-window clone, an m / n mismatch, a NULL or non-finite z / H / R or a zero quaternion returns
  * MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.  A non-finite dx or P entry returns
@@ -270,23 +276,38 @@ int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, 
  *                           r = z - psi^ wrapped into (-pi, pi]; one row over dtheta.  When d_x^2 + d_y^2 <= 1e-6 |f|^2 (f within
  *                           ~1e-3 rad of vertical) yaw is undefined: the stack writes nothing and reports status 2, NIS NaN.
  *   CLONE_HEADING           a = clone k; z as HEADING with f in that clone's camera frame; one row over its dtheta.
+ * Range models (UWB or other radio ranging to surveyed anchors; a laser or sonar rangefinder over the ground or a ceiling), with
+ * the same C, p and clone forms; one row each:
+ *   RANGE                   z = rho (1), anchor a_G (3), lever arm l (3) in the IMU frame: e = p + C^T l - a_G, rho^ = |e|,
+ *                           r = rho - rho^; H over dtheta and dp (12..14).  When rho^ <= 1e-6 m the direction is undefined:
+ *                           status 2, NIS NaN, nothing written.
+ *   CLONE_RANGE             a = clone k; z as RANGE with l in that clone's camera frame; H over its [dtheta, dp].
+ *   PLANE_RANGE             z = rho (1), plane height h (1), lever l (3), beam axis f (3, any non-zero length) in the IMU frame;
+ *                           the plane {x : x_z = h} is level in G.  b = C^T f / |f|, rho^ = (h - (p + C^T l)_z) / b_z,
+ *                           r = rho - rho^; H over dtheta and dp_z (14).  When b_z^2 <= 1e-6 (the beam within ~1e-3 rad of
+ *                           parallel to the plane) or rho^ <= 0 (the plane behind the sensor): status 2, NIS NaN, nothing written.
+ *   CLONE_PLANE_RANGE       a = clone k; z as PLANE_RANGE with l and f in that clone's camera frame; H over its [dtheta, dp_z].
+ *   A degenerate item ends its member's whole stack (in a batch the other members are applied).  An anchor's position is taken
+ *   as exact, and a range as unbiased; a caller with more than 8 anchors in one epoch makes two calls.
  *   A and b that a model does not use must be 0.  (A lever arm or an axis given in the IMU frame, l_I or f_I, is converted to
  *   camera frames with the engine's q_CI and p_C_I (the camera's position in the IMU frame: p_C_G = p_I_G + C(q_IG)^T p_C_I,
  *   C(q_CG) = C(q_CI) C(q_IG)): l_C = C(q_CI) (l_I - p_C_I), f_C = C(q_CI) f_I.)
  * C(q) is Eigen's toRotationMatrix (C(q_CG) maps G to the camera frame).  LINEAR is not allowed in a stack.  R of an item is its
- * own rows x rows block (3, 3, 6, 6, popcount(mask), 6, popcount(mask), popcount(mask), 1, 1 rows), row-major, lower triangle
+ * own rows x rows block (3, 3, 6, 6, popcount(mask), 6, popcount(mask), popcount(mask), 1, 1, 1, 1, 1, 1 rows), row-major, lower triangle
  * read; the struct carries no size, so a caller that passes another size is not caught here (the class forms check it). */
 typedef struct {
   int model;          /* msckf_b200_aid_model except LINEAR */
-  int a;              /* CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING: clone position; BODY_VELOCITY,
-                         ANTENNA_POSITION: row mask (1..7); else ignored (0 for the GNSS and heading models) */
+  int a;              /* CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING, CLONE_RANGE, CLONE_PLANE_RANGE: clone
+                         position; BODY_VELOCITY, ANTENNA_POSITION: row mask (1..7); else ignored (0 for the GNSS, heading
+                         and range models) */
   int b;              /* RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: row mask (1..7); else ignored (0 for the
-                         GNSS and heading models) */
-  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components), 7, 6 (antenna) or 4 (heading) doubles */
+                         GNSS, heading and range models) */
+  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components), 7, 6 (antenna), 4 (heading), 7 (range)
+                         or 8 (plane range) doubles */
   const double* R;    /* [rows][rows] */
 } msckf_b200_aid_item;
 /* A bad model, a clone outside the window, a == b, an empty mask, more than 8 items or 32 rows, a NULL or non-finite z / R, a zero
- * quaternion, a zero heading axis, a non-zero unused a / b of a GNSS or heading model or a NaN chi2_max returns
+ * quaternion, a zero heading or beam axis, a non-zero unused a / b of a GNSS, heading or range model or a NaN chi2_max returns
  * MSCKF_B200_ERR_ARG, an un-fetched update MSCKF_B200_ERR_STATE; then nothing is written.
  * A non-finite dx or P entry returns MSCKF_B200_ERR_NUMERIC with the result filled and the update applied.  n_items >= 1. */
 int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,

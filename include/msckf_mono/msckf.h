@@ -383,7 +383,7 @@ class MSCKF {
     return aidedUpdate(a);
   }
   // stacked aided updates (not in the reference; msckf_b200_aid_stack_update): up to 8 items -- odometry (BODY_VELOCITY,
-  // RELATIVE_POSE), GNSS antenna positions and headings (at the IMU or at a clone) and the fixes above -- fused as ONE update with R block-diagonal across items, one NIS over all rows and one
+  // RELATIVE_POSE), GNSS antenna positions and headings, radio ranges and rangefinder distances (at the IMU or at a clone) and the fixes above -- fused as ONE update with R block-diagonal across items, one NIS over all rows and one
   // chi2_max gate.  Items name clones by window position.  Bookkeeping as aidedUpdate(const msckf_b200_aid&).
   msckf_b200_aid_result aidedUpdate(const std::vector<msckf_b200_aid_item>& items, double chi2_max = 0) {
     msckf_b200_aid_result r = {};
@@ -441,6 +441,44 @@ class MSCKF {
     MatrixX<double> R(1, 1);
     R(0, 0) = var;
     return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_CLONE_HEADING, k, 0, 1, z, R)}, chi2_max);
+  }
+  // a radio range (UWB two-way ranging, an acoustic or radio beacon) |p_I_G + C(q_IG)^T lever - anchor| from an antenna on the
+  // body, the lever arm in the IMU frame, to an anchor at a surveyed position in G; var is its variance.  An antenna within 1e-6 m
+  // of its anchor gives status 2 and changes nothing.
+  msckf_b200_aid_result rangeUpdate(double range, const Vector3<double>& anchor, const Vector3<double>& lever, double var,
+                                    double chi2_max = 0) {
+    const double z[7] = {range, anchor(0), anchor(1), anchor(2), lever(0), lever(1), lever(2)};
+    MatrixX<double> R(1, 1);
+    R(0, 0) = var;
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_RANGE, 0, 0, 1, z, R)}, chi2_max);
+  }
+  // the same at the clone of image state_id (a delayed range: the image of its epoch), the lever arm in that clone's camera frame
+  msckf_b200_aid_result cloneRangeUpdate(int state_id, double range, const Vector3<double>& anchor, const Vector3<double>& lever,
+                                         double var, double chi2_max = 0) {
+    const int k = windowPosition(state_id, "MSCKF::cloneRangeUpdate");
+    const double z[7] = {range, anchor(0), anchor(1), anchor(2), lever(0), lever(1), lever(2)};
+    MatrixX<double> R(1, 1);
+    R(0, 0) = var;
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_CLONE_RANGE, k, 0, 1, z, R)}, chi2_max);
+  }
+  // a rangefinder (laser, sonar) distance along the beam axis, from a sensor at lever (both in the IMU frame), to the level plane
+  // {x : x_z = h} in G (the ground below, a ceiling above); var is its variance.  A beam within ~1e-3 rad of parallel to the
+  // plane, or a plane behind the sensor, gives status 2 and changes nothing.
+  msckf_b200_aid_result planeRangeUpdate(double range, double h, const Vector3<double>& lever, const Vector3<double>& axis, double var,
+                                         double chi2_max = 0) {
+    const double z[8] = {range, h, lever(0), lever(1), lever(2), axis(0), axis(1), axis(2)};
+    MatrixX<double> R(1, 1);
+    R(0, 0) = var;
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_PLANE_RANGE, 0, 0, 1, z, R)}, chi2_max);
+  }
+  // the same at the clone of image state_id, the lever arm and the axis in that clone's camera frame
+  msckf_b200_aid_result clonePlaneRangeUpdate(int state_id, double range, double h, const Vector3<double>& lever,
+                                              const Vector3<double>& axis, double var, double chi2_max = 0) {
+    const int k = windowPosition(state_id, "MSCKF::clonePlaneRangeUpdate");
+    const double z[8] = {range, h, lever(0), lever(1), lever(2), axis(0), axis(1), axis(2)};
+    MatrixX<double> R(1, 1);
+    R(0, 0) = var;
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_CLONE_PLANE_RANGE, k, 0, 1, z, R)}, chi2_max);
   }
   // the window position of the clone of image state_id (std::invalid_argument when it is not in the window)
   int windowPosition(int state_id, const char* what) const {

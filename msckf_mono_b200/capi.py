@@ -43,6 +43,7 @@ def _truth(truth_imu, truth_poses):
 
 AID_VELOCITY, AID_POSITION, AID_POSE, AID_CLONE_POSE, AID_LINEAR, AID_BODY_VELOCITY, AID_RELATIVE_POSE = range(7)
 AID_ANTENNA_POSITION, AID_CLONE_ANTENNA_POSITION, AID_HEADING, AID_CLONE_HEADING = range(7, 11)
+AID_RANGE, AID_CLONE_RANGE, AID_PLANE_RANGE, AID_CLONE_PLANE_RANGE = range(11, 15)
 
 
 class Aid(C.Structure):
@@ -80,8 +81,10 @@ def aid_items(items):
     a (CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION and CLONE_HEADING: a clone's window position, BODY_VELOCITY and
     ANTENNA_POSITION: the row mask; "clone" is read when "a" is missing), b (RELATIVE_POSE: the second clone,
     CLONE_ANTENNA_POSITION: the row mask).  z: ANTENNA_POSITION and CLONE_ANTENNA_POSITION p_A_G (3) and the lever arm (3) in
-    the body frame, HEADING and CLONE_HEADING psi (1) and the axis (3) in the body frame (include/msckf_b200.h); R of a heading
-    is 1 x 1"""
+    the body frame, HEADING and CLONE_HEADING psi (1) and the axis (3) in the body frame, RANGE and CLONE_RANGE rho (1), the
+    anchor (3) in G and the lever arm (3) in the body frame, PLANE_RANGE and CLONE_PLANE_RANGE rho (1), the plane height h (1),
+    the lever arm (3) and the beam axis (3) in the body frame (include/msckf_b200.h); "a" of CLONE_RANGE and CLONE_PLANE_RANGE
+    is the clone; R of a heading or a range is 1 x 1"""
     arr = (AidItem * max(len(items), 1))()
     keep = []
     for k, it in enumerate(items):

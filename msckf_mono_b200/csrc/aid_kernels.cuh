@@ -2,7 +2,7 @@
 // Aided measurements fused into the device-resident filter (msckf_b200_aid_update / _batch_aid_update and the stacked
 // msckf_b200_aid_stack_update / _batch_aid_stack_update):
 //   k_aid : residual r and H (a stack of up to 8 model items, each row at most 12 (state index, coefficient) pairs formed from
-//           the resident state; or the caller's r and dense H; a degenerate heading item ends the member: status 2), H P (sparse gathers over rows of P, or a product for a dense H),
+//           the resident state; or the caller's r and dense H; a degenerate heading or range item ends the member: status 2), H P (sparse gathers over rows of P, or a product for a dense H),
 //           S = H P H^T + R = L L^T with r as an extra row (y = L^-1 r), W = L^-1 H P, NIS = y^T y, the optional chi-square
 //           gate, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to the filter precision
 //           once) and the state injection of k_syrk (inject_state).  All arithmetic in fp64.
@@ -18,9 +18,12 @@ namespace mb {
 // the models of msckf_b200_aid_model (include/msckf_b200.h)
 enum AidModel {
   kAidVelocity = 0, kAidPosition = 1, kAidPose = 2, kAidClonePose = 3, kAidLinear = 4, kAidBodyVelocity = 5, kAidRelativePose = 6,
-  kAidAntennaPosition = 7, kAidCloneAntennaPosition = 8, kAidHeading = 9, kAidCloneHeading = 10
+  kAidAntennaPosition = 7, kAidCloneAntennaPosition = 8, kAidHeading = 9, kAidCloneHeading = 10,
+  kAidRange = 11, kAidCloneRange = 12, kAidPlaneRange = 13, kAidClonePlaneRange = 14
 };
 constexpr double kAidHeadingMinHoriz = 1e-6;  // HEADING: d_x^2 + d_y^2 <= this |f|^2 (f within ~1e-3 rad of vertical) is degenerate
+constexpr double kAidRangeMin = 1e-6;         // RANGE: a predicted range at or below this (m) leaves its direction undefined
+constexpr double kAidPlaneMinBeamZ = 1e-6;    // PLANE_RANGE: b_z^2 <= this (the beam within ~1e-3 rad of the plane) is degenerate
 constexpr int kAidMaxRows = 32;      // m <= 32: S is factored by one warp
 constexpr int kAidMaxItems = 8;      // model items of one stack
 constexpr int kAidItemZ = 8;         // doubles reserved for one item's z
@@ -35,8 +38,8 @@ struct AidOut {
   int numeric;  // a non-finite dx or P entry was written
 };
 
-// one item of a stack: its model, a (CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING: a clone's window
-// position; BODY_VELOCITY, ANTENNA_POSITION: the row mask), b (RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: the row
+// one item of a stack: its model, a (CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING, CLONE_RANGE,
+// CLONE_PLANE_RANGE: a clone's window position; BODY_VELOCITY, ANTENNA_POSITION: the row mask), b (RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: the row
 // mask) and its first row in the stack
 struct AidItem {
   short model, a, b, row;
@@ -73,6 +76,12 @@ __host__ __device__ constexpr size_t aid_ws_bytes(int n, int m) { return sizeof(
 //   HEADING, CLONE_HEADING  z = psi (1), axis f (3) in the body frame; d = C^T f, psi^ = atan2(d_y, d_x), r = wrap(z - psi^)
 //                  into (-pi, pi]; H over dtheta [-d_y, d_x, 0] / (d_x^2 + d_y^2) (-[d]x C^T).  d_x^2 + d_y^2 <=
 //                  kAidHeadingMinHoriz |f|^2 (yaw undefined) forms no row and returns 1: k_aid writes nothing (status 2).
+//   RANGE, CLONE_RANGE  z = rho, anchor a_G (3), lever l (3) in the body frame; e = p + d - a, rho^ = |e|, u = e / rho^,
+//                  r = rho - rho^; H over dtheta u^T J, over dp u^T.  rho^ <= kAidRangeMin returns 1 (status 2).
+//   PLANE_RANGE, CLONE_PLANE_RANGE  z = rho, plane height h, lever l (3), beam axis f (3) in the body frame; the plane is
+//                  {x : x_z = h} in G.  b = C^T f / |f|, rho^ = (h - (p + d)_z) / b_z, r = rho - rho^; with d' = C^T (l + rho^ f/|f|)
+//                  (the hit point from the body) and J' = -[d']x C^T: H over dtheta -J'_z / b_z (= e_z^T C^T [l + rho^ f/|f|]x / b_z),
+//                  over dp_z -1 / b_z.  b_z^2 <= kAidPlaneMinBeamZ or rho^ <= 0 (the plane behind the sensor) returns 1 (status 2).
 // Returns 0 when the rows are formed.
 // (Out of line, with the item by value: inlined into k_aid<double, 1>, this code made ptxas spill.)
 template <class S>
@@ -113,25 +122,57 @@ __device__ __noinline__ int aid_item_rows(const AidItem it, const double* z, con
         nnz[row++] = 6;
       }
     }
-  } else if (it.model >= kAidAntennaPosition) {  // the antenna positions and headings, of the IMU or of clone a
-    const bool clone = it.model == kAidCloneAntennaPosition || it.model == kAidCloneHeading;
-    const bool heading = it.model >= kAidHeading;
+  } else if (it.model >= kAidAntennaPosition) {  // the antenna positions, headings and ranges, of the IMU or of clone a
+    const bool clone = it.model == kAidCloneAntennaPosition || it.model == kAidCloneHeading || it.model == kAidCloneRange ||
+                       it.model == kAidClonePlaneRange;
+    const bool heading = it.model == kAidHeading || it.model == kAidCloneHeading;
+    const bool range = it.model == kAidRange || it.model == kAidCloneRange;
+    const bool plane = it.model == kAidPlaneRange || it.model == kAidClonePlaneRange;
     const S* Q = clone ? poses + kPoseStride * it.a : st->q_IG;
     const double q[4] = {(double)Q[0], (double)Q[1], (double)Q[2], (double)Q[3]};
-    const double* l = heading ? z + 1 : z + 3;  // the lever arm or the axis, in the body frame
+    const double* l = heading ? z + 1 : range ? z + 4 : plane ? z + 2 : z + 3;  // the lever arm or the axis, in the body frame
     const int c0 = clone ? 15 + 6 * it.a : 0;   // the pose's dtheta
+    const S* p = clone ? poses + kPoseStride * it.a + 4 : st->p_I_G;
+    const int cp = clone ? c0 + 3 : 12;         // the pose's dp
     double C[9], d[3], J[9];
     quat_to_rot(q, C);
     for (int i = 0; i < 3; ++i) d[i] = C[i] * l[0] + C[3 + i] * l[1] + C[6 + i] * l[2];
+    double rho = 0.0, bz = 0.0;  // PLANE_RANGE: rho^ and b_z
+    if (plane) {  // d becomes C^T (l + rho^ f/|f|), the hit point from the body, so that J below is J'
+      const double* f = z + 5;
+      const double nf = sqrt(f[0] * f[0] + f[1] * f[1] + f[2] * f[2]);
+      double b[3];
+      for (int i = 0; i < 3; ++i) b[i] = (C[i] * f[0] + C[3 + i] * f[1] + C[6 + i] * f[2]) / nf;
+      bz = b[2];
+      rho = (z[1] - ((double)p[2] + d[2])) / bz;
+      if (!(bz * bz > kAidPlaneMinBeamZ) || !(rho > 0.0)) return 1;
+      for (int i = 0; i < 3; ++i) d[i] += rho * b[i];
+    }
 #pragma unroll
     for (int k = 0; k < 3; ++k) {  // J = -[d]x C^T: column k is (row k of C) x d
       J[k] = C[3 * k + 1] * d[2] - C[3 * k + 2] * d[1];
       J[3 + k] = C[3 * k + 2] * d[0] - C[3 * k] * d[2];
       J[6 + k] = C[3 * k] * d[1] - C[3 * k + 1] * d[0];
     }
-    if (!heading) {
-      const S* p = clone ? poses + kPoseStride * it.a + 4 : st->p_I_G;
-      const int cp = clone ? c0 + 3 : 12, mask = clone ? it.b : it.a;
+    if (range) {
+      const double e[3] = {(double)p[0] + d[0] - z[1], (double)p[1] + d[1] - z[2], (double)p[2] + d[2] - z[3]};
+      const double rh = sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+      if (!(rh > kAidRangeMin)) return 1;
+      r[r0] = z[0] - rh;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        col[r0][k] = c0 + k; coef[r0][k] = (e[0] * J[k] + e[1] * J[3 + k] + e[2] * J[6 + k]) / rh;
+        col[r0][3 + k] = cp + k; coef[r0][3 + k] = e[k] / rh;
+      }
+      nnz[r0] = 6;
+    } else if (plane) {
+      r[r0] = z[0] - rho;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { col[r0][k] = c0 + k; coef[r0][k] = -J[6 + k] / bz; }
+      col[r0][3] = cp + 2; coef[r0][3] = -1.0 / bz;
+      nnz[r0] = 4;
+    } else if (!heading) {
+      const int mask = clone ? it.b : it.a;
       int row = r0;
 #pragma unroll
       for (int j = 0; j < 3; ++j) {
@@ -225,7 +266,7 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
   } else if (t < a.m[f].n_items) {
     degenerate = aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, &L[m][0], s_col, s_coef, s_nnz);
   }
-  if (__syncthreads_or(degenerate)) {  // a heading whose yaw is undefined: nothing is written
+  if (__syncthreads_or(degenerate)) {  // a heading whose yaw or a range whose prediction is undefined: nothing is written
     if (t == 0) {
       out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
       out->dof = m; out->applied = 0; out->status = 2; out->numeric = 0;

@@ -168,13 +168,26 @@ int aid_append(AidJob& j, const msckf_b200_aid_item& q, int M, const std::string
       nz = heading ? 4 : 6;
       break;
     }
+    case MSCKF_B200_AID_RANGE: case MSCKF_B200_AID_CLONE_RANGE:
+    case MSCKF_B200_AID_PLANE_RANGE: case MSCKF_B200_AID_CLONE_PLANE_RANGE: {  // one row each (b and the IMU forms' a must be 0)
+      const bool clone = q.model == MSCKF_B200_AID_CLONE_RANGE || q.model == MSCKF_B200_AID_CLONE_PLANE_RANGE;
+      if (clone && (q.a < 0 || q.a >= M)) return fail(MSCKF_B200_ERR_ARG, w + ": clone outside the window" + who);
+      if ((!clone && q.a != 0) || q.b != 0) return fail(MSCKF_B200_ERR_ARG, w + ": a / b the model does not use must be 0" + who);
+      m = 1;
+      nz = q.model == MSCKF_B200_AID_RANGE || q.model == MSCKF_B200_AID_CLONE_RANGE ? 7 : 8;
+      break;
+    }
     default: return fail(MSCKF_B200_ERR_ARG, w + ": model not allowed in a stack" + who);
   }
   if (j.m + m > mb::kAidMaxRows) return fail(MSCKF_B200_ERR_ARG, w + ": more than 32 rows" + who);
   if (!q.z || !finite(q.z, nz)) return fail(MSCKF_B200_ERR_ARG, w + ": missing or non-finite z" + who);
-  if (nz == 7 && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
+  const bool pose = q.model == MSCKF_B200_AID_POSE || q.model == MSCKF_B200_AID_CLONE_POSE || q.model == MSCKF_B200_AID_RELATIVE_POSE;
+  const bool heading = q.model == MSCKF_B200_AID_HEADING || q.model == MSCKF_B200_AID_CLONE_HEADING;
+  const bool plane = q.model == MSCKF_B200_AID_PLANE_RANGE || q.model == MSCKF_B200_AID_CLONE_PLANE_RANGE;
+  if (pose && !(q.z[3] * q.z[3] + q.z[4] * q.z[4] + q.z[5] * q.z[5] + q.z[6] * q.z[6] > 0.0))
     return fail(MSCKF_B200_ERR_ARG, w + ": zero quaternion" + who);
-  if (nz == 4 && !(q.z[1] * q.z[1] + q.z[2] * q.z[2] + q.z[3] * q.z[3] > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": zero heading axis" + who);
+  if (heading && !(q.z[1] * q.z[1] + q.z[2] * q.z[2] + q.z[3] * q.z[3] > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": zero heading axis" + who);
+  if (plane && !(q.z[5] * q.z[5] + q.z[6] * q.z[6] + q.z[7] * q.z[7] > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": zero beam axis" + who);
   if (!q.R) return fail(MSCKF_B200_ERR_ARG, w + ": missing R" + who);
   for (int r = 0; r < m; ++r)
     if (!finite(q.R + (size_t)r * m, r + 1)) return fail(MSCKF_B200_ERR_ARG, w + ": non-finite R" + who);
@@ -1500,7 +1513,10 @@ static_assert(offsetof(mb::AidOut, status) == offsetof(msckf_b200_aid_result, st
 static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && (int)MSCKF_B200_AID_RELATIVE_POSE == (int)mb::kAidRelativePose &&
                   (int)MSCKF_B200_AID_ANTENNA_POSITION == (int)mb::kAidAntennaPosition &&
                   (int)MSCKF_B200_AID_CLONE_ANTENNA_POSITION == (int)mb::kAidCloneAntennaPosition &&
-                  (int)MSCKF_B200_AID_HEADING == (int)mb::kAidHeading && (int)MSCKF_B200_AID_CLONE_HEADING == (int)mb::kAidCloneHeading,
+                  (int)MSCKF_B200_AID_HEADING == (int)mb::kAidHeading && (int)MSCKF_B200_AID_CLONE_HEADING == (int)mb::kAidCloneHeading &&
+                  (int)MSCKF_B200_AID_RANGE == (int)mb::kAidRange && (int)MSCKF_B200_AID_CLONE_RANGE == (int)mb::kAidCloneRange &&
+                  (int)MSCKF_B200_AID_PLANE_RANGE == (int)mb::kAidPlaneRange &&
+                  (int)MSCKF_B200_AID_CLONE_PLANE_RANGE == (int)mb::kAidClonePlaneRange,
               "msckf_b200_aid_model and mb::AidModel differ");
 constexpr size_t kAidSmemMax = 32 * 1024;
 template <class S>

@@ -43,6 +43,15 @@ as a plain POSITION fix of the IMU, which shows the lever-arm bias.  The noise o
 np.random.default_rng([seed, k, 6]) (3 standard normals per fix) and [seed, k, 7] (1 per heading), so the trial's other inputs
 are the same with GNSS on or off.  The NIS of the stacks gives another truth-free consistency figure.
 
+Optional ranging (UWB-style radio ranges to the surveyed anchors ANCHORS, and a downward rangefinder over the level ground plane
+z = plane_height): every `range_every` frames the truth range |p_I_G + C(q_IG)^T range_lever - a| to each anchor plus
+N(0, range_sigma^2) as RANGE, and every `plane_every` frames the truth distance along the IMU axis `plane_axis` from
+`plane_lever` to the plane plus N(0, plane_sigma^2) as PLANE_RANGE; a frame's ranges and plane range in ONE stacked update.
+range_delay d > 0 fuses, at frame f, both of frame f - d at that frame's clone (CLONE_RANGE, CLONE_PLANE_RANGE, the levers and
+the axis converted to its camera frame), like gnss_delay.  The noise of trial k comes from its own streams
+np.random.default_rng([seed, k, 8]) (one standard normal per anchor) and [seed, k, 9] (1 per plane range), so the trial's other
+inputs are the same with ranging on or off.  The NIS of the stacks is recorded and summarised as the GNSS stacks' are.
+
 Error-state convention (the inverse of the filter's state injection q+ = buildUpdateQuat(dtheta) * q): dq = q_true * q_est^-1
 with the Hamilton product, dq negated when dq.w < 0, dtheta = -2 vec(dq); every other component is truth - estimate.  Host
 vectors here are in the filter's covariance order [dtheta, db_g, dv, db_a, dp, clones (dtheta_C, dp_C)...].
@@ -55,8 +64,9 @@ import numpy as np
 from scipy import stats
 
 from . import synth
-from .capi import (AID_ANTENNA_POSITION, AID_BODY_VELOCITY, AID_CLONE_ANTENNA_POSITION, AID_CLONE_HEADING, AID_HEADING,
-                   AID_POSITION, AID_RELATIVE_POSE)
+from .capi import (AID_ANTENNA_POSITION, AID_BODY_VELOCITY, AID_CLONE_ANTENNA_POSITION, AID_CLONE_HEADING,
+                   AID_CLONE_PLANE_RANGE, AID_CLONE_RANGE, AID_HEADING, AID_PLANE_RANGE, AID_POSITION, AID_RANGE,
+                   AID_RELATIVE_POSE)
 
 COMPONENTS = ("orientation", "position", "pose", "imu", "full")
 DOF = {"orientation": 3, "position": 3, "pose": 6, "imu": 15}
@@ -111,9 +121,14 @@ def relative_pose(pose_a, pose_b):
 
 
 def odometry_residual(item, imu, poses):
-    """r of one BODY_VELOCITY, RELATIVE_POSE or GNSS item (a dict as for capi.aid_items) at the state (imu 19+, poses [M, 7]),
-    in fp64"""
+    """r of one BODY_VELOCITY, RELATIVE_POSE, GNSS or range item (a dict as for capi.aid_items) at the state (imu 19+, poses
+    [M, 7]), in fp64"""
     z = np.asarray(item["z"], dtype=np.float64)
+    if item["model"] in RANGE_MODELS:
+        q, p, _ = _range_frame(item, imu, poses)
+        if item["model"] in (AID_RANGE, AID_CLONE_RANGE):
+            return np.array([z[0] - range_of(p, q, z[4:7], z[1:4])])
+        return np.array([z[0] - plane_range_of(p, q, z[1], z[2:5], z[5:8])])
     if item["model"] in GNSS_MODELS:
         q, p, _, rows = _gnss_frame(item, imu, poses)
         if item["model"] in (AID_HEADING, AID_CLONE_HEADING):
@@ -126,10 +141,28 @@ def odometry_residual(item, imu, poses):
 
 
 def odometry_jacobian(item, imu, poses, n):
-    """H [m, n] of one BODY_VELOCITY, RELATIVE_POSE or GNSS item in the filter's injection convention, C(q+) = (I - [dtheta]x)
-    C(q): the host linearisation of the models msckf_b200_aid_stack_update forms on the device"""
+    """H [m, n] of one BODY_VELOCITY, RELATIVE_POSE, GNSS or range item in the filter's injection convention, C(q+) = (I -
+    [dtheta]x) C(q): the host linearisation of the models msckf_b200_aid_stack_update forms on the device"""
     skew = _skew
     imu, poses = np.asarray(imu, dtype=np.float64), np.asarray(poses, dtype=np.float64)
+    if item["model"] in RANGE_MODELS:  # d(C^T v) / dtheta = -C^T [v]x
+        q, p, c0 = _range_frame(item, imu, poses)
+        C = quat_to_rot(q)
+        z = np.asarray(item["z"], dtype=np.float64)
+        cp = c0 + 3 if c0 else 12
+        H = np.zeros((1, n))
+        if item["model"] in (AID_RANGE, AID_CLONE_RANGE):  # u^T d(p + C^T l) with u the unit vector from the anchor
+            e = p + C.T @ z[4:7] - z[1:4]
+            u = e / np.linalg.norm(e)
+            H[0, c0:c0 + 3] = u @ (-C.T @ skew(z[4:7]))
+            H[0, cp:cp + 3] = u
+            return H
+        f = z[5:8] / np.linalg.norm(z[5:8])
+        bz = (C.T @ f)[2]
+        rho = plane_range_of(p, q, z[1], z[2:5], z[5:8])
+        H[0, c0:c0 + 3] = (C.T @ skew(z[2:5] + rho * f))[2] / bz  # through the hit point l + rho f in the body frame
+        H[0, cp + 2] = -1.0 / bz
+        return H
     if item["model"] in GNSS_MODELS:  # d(C^T l) / dtheta = -C^T [l]x
         q, _, c0, rows = _gnss_frame(item, imu, poses)
         C = quat_to_rot(q)
@@ -250,6 +283,63 @@ def gnss_items(truth_imu, camera, noise_p, noise_psi, sigma, lever, sigma_psi, a
     return items
 
 
+# ---- range models (RANGE, CLONE_RANGE, PLANE_RANGE, CLONE_PLANE_RANGE) --------------------------------------------------------
+RANGE_MODELS = (AID_RANGE, AID_CLONE_RANGE, AID_PLANE_RANGE, AID_CLONE_PLANE_RANGE)
+# the ranging scene around the synthetic circle (radius 2 m about the origin, heights within +-0.2 m): four surveyed anchors, not
+# coplanar, and a level ground plane below the trajectory.  The synthetic IMU's x axis points up: a downward beam is -x.
+ANCHORS = np.array([[5.0, 5.0, -1.0], [-5.0, 5.0, 2.0], [-5.0, -5.0, -1.0], [5.0, -5.0, 2.0]])
+PLANE_HEIGHT = -1.5
+PLANE_AXIS = (-1.0, 0.0, 0.0)
+
+
+def range_of(p, q, lever, anchor):
+    """|p + C(q)^T lever - anchor|: the range from an antenna at lever in the frame of a body at p with orientation q"""
+    return float(np.linalg.norm(antenna_position(p, q, lever) - np.asarray(anchor, dtype=np.float64)))
+
+
+def plane_range_of(p, q, h, lever, axis):
+    """the distance along axis (body frame, any length) from a sensor at lever in the body frame to the plane {x : x_z = h}:
+    (h - (p + C^T lever)_z) / b_z with b = C^T axis / |axis| (negative when the plane is behind the sensor)"""
+    axis = np.asarray(axis, dtype=np.float64)
+    b = quat_to_rot(q).T @ (axis / np.linalg.norm(axis))
+    return float((h - antenna_position(p, q, lever)[2]) / b[2])
+
+
+def _range_frame(item, imu, poses):
+    """(q, p, first error-state index of the pose's dtheta) of a range item's body"""
+    if item["model"] in (AID_CLONE_RANGE, AID_CLONE_PLANE_RANGE):
+        k = item["a"]
+        return np.asarray(poses[k, 3:7], dtype=np.float64), np.asarray(poses[k, 0:3], dtype=np.float64), 15 + 6 * k
+    return np.asarray(imu[15:19], dtype=np.float64), np.asarray(imu[0:3], dtype=np.float64), 0
+
+
+def range_items(truth_imu, camera, noise_r, noise_h, sigma, lever, sigma_h, h, plane_lever, axis, clone=None, anchors=ANCHORS):
+    """the ranging stack of one epoch as aid item dicts, from the truth IMU state of that epoch: with noise_r (one standard
+    normal per anchor) the range from the antenna at lever (IMU frame) to each anchor plus sigma noise_r, with noise_h (1) the
+    distance along axis from plane_lever (IMU frame) to the plane z = h plus sigma_h noise_h.  clone = k fuses them at clone k
+    (the levers and the axis in its camera frame)"""
+    imu = np.asarray(truth_imu, dtype=np.float64)
+    p, q = imu[0:3], imu[15:19]
+    items = []
+    if noise_r is not None:
+        lv = lever if clone is None else camera_frame(camera, lever=lever)
+        for a, nr in zip(np.asarray(anchors, dtype=np.float64), np.asarray(noise_r).ravel()):
+            z = np.r_[range_of(p, q, lever, a) + sigma * nr, a, lv]
+            if clone is None:
+                items.append({"model": AID_RANGE, "z": z, "R": np.array([[sigma ** 2]])})
+            else:
+                items.append({"model": AID_CLONE_RANGE, "a": clone, "z": z, "R": np.array([[sigma ** 2]])})
+    if noise_h is not None:
+        rho = plane_range_of(p, q, h, plane_lever, axis) + sigma_h * float(np.asarray(noise_h).ravel()[0])
+        R = np.array([[sigma_h ** 2]])
+        if clone is None:
+            items.append({"model": AID_PLANE_RANGE, "z": np.r_[rho, h, plane_lever, axis], "R": R})
+        else:
+            items.append({"model": AID_CLONE_PLANE_RANGE, "a": clone,
+                          "z": np.r_[rho, h, camera_frame(camera, lever=plane_lever), camera_frame(camera, axis=axis)], "R": R})
+    return items
+
+
 # ---- states: {"imu": 19 doubles (p, v, b_g, b_a, g, q_IG), "poses": [M, 7] (p_C_G, q_CG) or None} ----------------------
 def error_state(truth, est):
     """truth - estimate in the filter's covariance order (15, or 15 + 6M when both carry poses)"""
@@ -326,7 +416,7 @@ def map_observations(truth, frame, stride):
 
 
 def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0, map_start=0, map_sigma=0.0,
-               map_clones=1, gnss_every=0, heading_every=0):
+               map_clones=1, gnss_every=0, heading_every=0, range_every=0, plane_every=0):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
     fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
     map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks, None
@@ -338,7 +428,9 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
     pixel noise comes from np.random.default_rng([seed, k, 5]), so the newest frame's noise is the same for every K.  With
     gnss_every > 0, "gnss" holds per frame (the epoch of that frame) None or the 3 standard normals of its antenna-position noise,
     from np.random.default_rng([seed, k, 6]); with heading_every > 0, "heading" holds None or 1 standard normal, from
-    np.random.default_rng([seed, k, 7]) (gnss_items)."""
+    np.random.default_rng([seed, k, 7]) (gnss_items).  With range_every > 0, "range" holds per frame None or one standard normal
+    per anchor of ANCHORS, from np.random.default_rng([seed, k, 8]); with plane_every > 0, "plane" holds None or 1 standard
+    normal, from np.random.default_rng([seed, k, 9]) (range_items)."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -406,6 +498,12 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
     if heading_every > 0:
         hrng = np.random.default_rng([seed, k, 7])
         out["heading"] = [hrng.standard_normal(1) if (f + 1) % heading_every == 0 else None for f in range(len(truth["frames"]))]
+    if range_every > 0:
+        rrng = np.random.default_rng([seed, k, 8])
+        out["range"] = [rrng.standard_normal(len(ANCHORS)) if (f + 1) % range_every == 0 else None for f in range(len(truth["frames"]))]
+    if plane_every > 0:
+        prng = np.random.default_rng([seed, k, 9])
+        out["plane"] = [prng.standard_normal(1) if (f + 1) % plane_every == 0 else None for f in range(len(truth["frames"]))]
     return out
 
 
@@ -417,17 +515,19 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None, gnss_rows=None):
+def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None, gnss_rows=None, range_rows=None):
     """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes, of its
     map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n) and of its odometry
     stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists; map_first (a dict of plain numbers: frame,
     squared position error before and after, nis, dof, iterations, converged) describes the first map update; gnss_rows
-    (result dicts of aid_stack_update, dof 0 for an epoch whose clone had left the window) the GNSS stacks"""
+    (result dicts of aid_stack_update, dof 0 for an epoch whose clone had left the window) the GNSS stacks, range_rows (the
+    same) the ranging stacks"""
     rec = _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows)
     if map_first is not None:
         rec["map_first"] = dict(map_first)
-    if gnss_rows is not None:
-        rec["gnss"] = {key: [float(r[key]) if key == "nis" else int(r[key]) for r in gnss_rows] for key in ("nis", "dof", "applied", "status")}
+    for key, rows in (("gnss", gnss_rows), ("range", range_rows)):
+        if rows is not None:
+            rec[key] = {k: [float(r[k]) if k == "nis" else int(r[k]) for r in rows] for k in ("nis", "dof", "applied", "status")}
     return rec
 
 
@@ -515,8 +615,10 @@ def summarize(records):
                            "run_bounds": list(chi2_bounds(int(D.sum()), V.size)),
                            "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])),
                            "applied": float(np.mean([a for o in od for a in o["applied"]]))}
-    gn = [records[k].get("gnss") for k in keys]
-    if all(g is not None and len(g["nis"]) for g in gn):  # ANIS of the GNSS stacks: the stack's rows per trial and epoch fused
+    for key in ("gnss", "range"):  # ANIS of the GNSS and of the ranging stacks: the stack's rows per trial and epoch fused
+        gn = [records[k].get(key) for k in keys]
+        if not all(g is not None and len(g["nis"]) for g in gn):
+            continue
         V = np.array([g["nis"] for g in gn]); D = np.array([g["dof"] for g in gn])
         used = (D > 0) & np.isfinite(V)  # (a dropped epoch, or status 1 / 2: no NIS)
         V, D = np.where(used, V, 0.0), np.where(used, D, 0)
@@ -524,12 +626,12 @@ def summarize(records):
         keep = n_used > 0
         anis = V.sum(axis=0)[keep] / n_used[keep]
         lo, hi = zip(*[chi2_bounds(int(d), int(c)) for d, c in zip(dof[keep], n_used[keep])]) if keep.any() else ((), ())
-        out["gnss"] = {"anis": [float(a) for a in anis], "lower": list(lo), "upper": list(hi), "dof": [int(d) for d in dof[keep]],
-                       "mean_anis": float(V.sum() / max(used.sum(), 1)), "mean_dof": float(D.sum() / max(used.sum(), 1)),
-                       "run_bounds": list(chi2_bounds(int(D.sum()), int(used.sum()))) if used.any() else [float("nan")] * 2,
-                       "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])) if keep.any() else float("nan"),
-                       "applied": float(np.mean([a for g, u in zip(gn, used) for a, x in zip(g["applied"], u) if x])) if used.any() else 0.0,
-                       "degenerate": int(sum(s == 2 for g in gn for s in g["status"]))}
+        out[key] = {"anis": [float(a) for a in anis], "lower": list(lo), "upper": list(hi), "dof": [int(d) for d in dof[keep]],
+                    "mean_anis": float(V.sum() / max(used.sum(), 1)), "mean_dof": float(D.sum() / max(used.sum(), 1)),
+                    "run_bounds": list(chi2_bounds(int(D.sum()), int(used.sum()))) if used.any() else [float("nan")] * 2,
+                    "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])) if keep.any() else float("nan"),
+                    "applied": float(np.mean([a for g, u in zip(gn, used) for a, x in zip(g["applied"], u) if x])) if used.any() else 0.0,
+                    "degenerate": int(sum(s == 2 for g in gn for s in g["status"]))}
     return out
 
 
@@ -552,16 +654,44 @@ def map_call(tr, f, fi, uncertain, S):
     return ids, inv, z, p[first], np.repeat(S, len(u), axis=0)
 
 
+def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items):
+    """one batched stack per filter of the epoch g = f - delay when a trial input of `keys` (two noise lists of make_trial) has
+    noise there: items(g, noise of keys[0], noise of keys[1], clone) with clone None at delay 0, else the window position of
+    the epoch's clone; a filter whose epoch clone has left the window sends nothing and records dof 0.  Appends each filter's
+    result to out[i]."""
+    noise = [tuple(tr[key][g] if key in tr else None for key in keys) for tr in trs] if g >= 0 else []
+    if g < 0 or not any(x is not None for x in noise[0]):
+        return
+    stacks = []
+    for f, tr, (n_a, n_b) in zip(fs, trs, noise):
+        clone = None
+        if delay:
+            ids = list(f.getCamStates()["state_id"])
+            if tr["frames"][g]["state_id"] not in ids:  # the epoch's clone has left the window
+                stacks.append(None)
+                continue
+            clone = ids.index(tr["frames"][g]["state_id"])
+        stacks.append(items(g, n_a, n_b, clone))
+    for i, r in enumerate(fb.aid_stack_update(stacks)):
+        out[i].append({"nis": 0.0, "dof": 0, "applied": 0, "status": 0} if r is None else r)
+
+
 def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0,
         odo_every=0, odo_sigma_v=0.05, odo_sigma_rel=0.01, nhc=False, map_start=0, map_iterations=1, map_sigma=0.0,
         map_uncertain=False, map_clones=1, gnss_every=0, gnss_sigma=0.1, gnss_lever=(0.0, 0.0, 0.0), gnss_delay=0,
-        gnss_as_position=False, heading_every=0, heading_sigma=0.01, heading_axis=(1.0, 0.0, 0.0)):
+        gnss_as_position=False, heading_every=0, heading_sigma=0.01, heading_axis=(1.0, 0.0, 0.0), range_every=0, range_sigma=0.1,
+        range_lever=(0.0, 0.0, 0.0), range_delay=0, plane_every=0, plane_sigma=0.02, plane_height=PLANE_HEIGHT, plane_axis=PLANE_AXIS,
+        plane_lever=(0.0, 0.0, 0.0)):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
     [one batched GNSS stack (gnss_items) in a frame whose epoch f - gnss_delay has an antenna fix (every gnss_every frames,
     lever arm gnss_lever in the IMU frame) or a heading (every heading_every frames, of heading_axis); at the IMU when
     gnss_delay = 0, else at that epoch's clone while it is in the window],
+    [one batched ranging stack (range_items) in a frame whose epoch f - range_delay has anchor ranges (every range_every frames,
+    antenna at range_lever in the IMU frame, standard deviation range_sigma) or a plane range (every plane_every frames, along
+    plane_axis from plane_lever to the plane z = plane_height, standard deviation plane_sigma); at the IMU or the epoch's clone
+    as for GNSS],
     [every map_every frames from frame map_start on, one batched mapped-landmark update from the newest clone, gated per
     observation at map_chi2 > 0, iterated up to map_iterations linearisations; the map carries N(0, map_sigma^2 I) errors and
     is observed from the map_clones newest clones that are still in the window (make_trial); map_uncertain passes
@@ -576,9 +706,11 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     assert not map_uncertain or map_sigma > 0, "map_uncertain needs map_sigma > 0"
     assert not (gnss_as_position and gnss_delay), "gnss_as_position fuses at the IMU: no delay"
     trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start, map_sigma, map_clones,
-                      gnss_every, heading_every) for k in trials]
+                      gnss_every, heading_every, range_every, plane_every) for k in trials]
     gnss = [[] for _ in trs] if gnss_every > 0 or heading_every > 0 else None
+    ranging = [[] for _ in trs] if range_every > 0 or plane_every > 0 else None
     lever, axis = np.asarray(gnss_lever, dtype=np.float64), np.asarray(heading_axis, dtype=np.float64)
+    r_lever, p_lever, p_axis = (np.asarray(v, dtype=np.float64) for v in (range_lever, plane_lever, plane_axis))
     S_map = np.tile([map_sigma ** 2, 0.0, map_sigma ** 2, 0.0, 0.0, map_sigma ** 2], (1, 1))
     first = [None for _ in trs]
     R_fix = (fix_sigma ** 2) * np.eye(3)
@@ -617,22 +749,14 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
                 stacks.append(items)
             for i, r in enumerate(fb.aid_stack_update(stacks)):
                 odo[i].append(r)
-        g = fi - gnss_delay  # the epoch whose GNSS output arrives at this frame
-        noise = [(tr["gnss"][g] if "gnss" in tr else None, tr["heading"][g] if "heading" in tr else None) for tr in trs] if g >= 0 else []
-        if gnss is not None and g >= 0 and any(x is not None for x in noise[0]):
-            stacks = []
-            for f, tr, (n_p, n_psi) in zip(fs, trs, noise):
-                clone = None
-                if gnss_delay:
-                    ids = list(f.getCamStates()["state_id"])
-                    if tr["frames"][g]["state_id"] not in ids:  # the epoch's clone has left the window
-                        stacks.append(None)
-                        continue
-                    clone = ids.index(tr["frames"][g]["state_id"])
-                stacks.append(gnss_items(truth["truth_imu"][g], truth["camera"], n_p, n_psi, gnss_sigma, lever, heading_sigma, axis,
-                                         clone, gnss_as_position))
-            for i, r in enumerate(fb.aid_stack_update(stacks)):
-                gnss[i].append({"nis": 0.0, "dof": 0, "applied": 0, "status": 0} if r is None else r)
+        if gnss is not None:  # the epoch whose GNSS output arrives at this frame
+            _epoch_stacks(fb, fs, trs, fi - gnss_delay, gnss_delay, ("gnss", "heading"), gnss,
+                          lambda g, n_p, n_psi, clone: gnss_items(truth["truth_imu"][g], truth["camera"], n_p, n_psi, gnss_sigma, lever,
+                                                                  heading_sigma, axis, clone, gnss_as_position))
+        if ranging is not None:  # the epoch whose ranges arrive at this frame
+            _epoch_stacks(fb, fs, trs, fi - range_delay, range_delay, ("range", "plane"), ranging,
+                          lambda g, n_r, n_h, clone: range_items(truth["truth_imu"][g], truth["camera"], n_r, n_h, range_sigma, r_lever,
+                                                                 plane_sigma, plane_height, p_lever, p_axis, clone))
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [map_call(tr, f, fi, map_uncertain, S_map) for tr, f in zip(trs, fs)]
             if first[0] is None:
@@ -662,7 +786,8 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         if on_frame is not None:
             on_frame(fi, fs, res)
     fb.close()
-    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i], None if gnss is None else gnss[i])
+    records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i], None if gnss is None else gnss[i],
+                                     None if ranging is None else ranging[i])
                for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):

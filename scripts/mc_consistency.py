@@ -28,6 +28,12 @@ noise of --heading-sigma rad.  --gnss-delay D fuses the epoch of frame f - D at 
 --gnss-as-position fuses the antenna position as a plain POSITION fix (the lever-arm bias).  The summary adds the GNSS stacks'
 ANIS against its 95 % chi^2 bounds.
 
+With --range-every K, every K frames each trial also fuses the truth ranges from an antenna at --range-lever X Y Z (IMU frame) to
+the four surveyed anchors of montecarlo.ANCHORS plus noise of --range-sigma m as RANGE; --plane-every K adds the truth distance
+along --plane-axis X Y Z from --plane-lever X Y Z (both in the IMU frame) to the level plane z = --plane-height plus noise of
+--plane-sigma m as PLANE_RANGE; a frame's ranges and plane range go in one stacked update.  --range-delay D fuses the epoch of
+frame f - D at frame f, at that epoch's clone.  The summary adds the ranging stacks' ANIS against its 95 % chi^2 bounds.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -156,6 +162,15 @@ def main():
     ap.add_argument("--gnss-as-position", action="store_true", help="fuse the antenna position as a plain POSITION fix")
     ap.add_argument("--heading-every", type=int, default=0)
     ap.add_argument("--heading-sigma", type=float, default=0.01)
+    ap.add_argument("--range-every", type=int, default=0)
+    ap.add_argument("--range-sigma", type=float, default=0.1)
+    ap.add_argument("--range-lever", type=float, nargs=3, default=[0.0, 0.0, 0.0], metavar=("X", "Y", "Z"))
+    ap.add_argument("--range-delay", type=int, default=0, help="fuse the ranges of frame f - d at its clone (frames)")
+    ap.add_argument("--plane-every", type=int, default=0)
+    ap.add_argument("--plane-sigma", type=float, default=0.02)
+    ap.add_argument("--plane-height", type=float, default=mc.PLANE_HEIGHT)
+    ap.add_argument("--plane-axis", type=float, nargs=3, default=list(mc.PLANE_AXIS), metavar=("X", "Y", "Z"))
+    ap.add_argument("--plane-lever", type=float, nargs=3, default=[0.0, 0.0, 0.0], metavar=("X", "Y", "Z"))
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -176,7 +191,10 @@ def main():
                         map_iterations=args.map_iterations, map_sigma=args.map_sigma, map_uncertain=args.map_uncertain,
                         map_clones=args.map_clones, gnss_every=args.gnss_every, gnss_sigma=args.gnss_sigma,
                         gnss_lever=args.gnss_lever, gnss_delay=args.gnss_delay, gnss_as_position=args.gnss_as_position,
-                        heading_every=args.heading_every, heading_sigma=args.heading_sigma)
+                        heading_every=args.heading_every, heading_sigma=args.heading_sigma, range_every=args.range_every,
+                        range_sigma=args.range_sigma, range_lever=args.range_lever, range_delay=args.range_delay,
+                        plane_every=args.plane_every, plane_sigma=args.plane_sigma, plane_height=args.plane_height,
+                        plane_axis=args.plane_axis, plane_lever=args.plane_lever)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -199,6 +217,11 @@ def main():
         res["gnss"] = {"every": args.gnss_every, "sigma_m": args.gnss_sigma, "lever_m": args.gnss_lever, "delay": args.gnss_delay,
                        "as_position": args.gnss_as_position, "heading_every": args.heading_every, "heading_sigma": args.heading_sigma,
                        **{k: s["gnss"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate")}}
+    if "range" in s:
+        res["range"] = {"every": args.range_every, "sigma_m": args.range_sigma, "lever_m": args.range_lever, "delay": args.range_delay,
+                        "plane_every": args.plane_every, "plane_sigma_m": args.plane_sigma, "plane_height_m": args.plane_height,
+                        "plane_axis": args.plane_axis, "plane_lever_m": args.plane_lever,
+                        **{k: s["range"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate")}}
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
