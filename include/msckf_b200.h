@@ -316,6 +316,47 @@ int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item*
  * written); every member is validated before anything is launched.  One launch per 32 updated members. */
 int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
                                       double chi2_max, msckf_b200_aid_result* out);
+/* ---- fault detection and exclusion (FDE) over a stack's items --------------------------------------------------------------
+ * The stacked update with one faulty item (an NLOS range, a GNSS multipath jump, a rangefinder on a table) removed on the device
+ * instead of the whole epoch.  A starts as the items that can be linearised; a degenerate item (what ends a plain stack with
+ * status 2) is dropped: its state is 2 and it does not count toward max_exclude.  Then, in rounds over the d_A rows of A
+ * (S_AA is the principal submatrix of S = H P H^T + R: R is block-diagonal across items):
+ *   1. NIS_A = r_A^T S_AA^-1 r_A <= chi2[d_A - 1]: the update is applied with the rows of A; stop.
+ *   2. max_exclude items already excluded: rejected (outcome 2).  |A| = 1: rejected (outcome 3).
+ *   3. for each j in A, t_j = NIS_A - NIS_{A\j} = y_j^T B_j^-1 y_j with y = S_AA^-1 r_A and B_j = (S_AA^-1)_jj (the block
+ *      w-test: chi-square with d_j dof when j is not faulty).
+ *   4. j* maximises t_j / chi2[d_j - 1], the lowest item index on a tie; a ratio <= 1 rejects the stack (outcome 3: no single
+ *      item explains the failure), else j* leaves A and the next round starts at 1.
+ * An applied update is msckf_b200_aid_stack_update on the items of A alone, in their order, without a gate, bit for bit (P,
+ * state, NIS, dx_norm); max_exclude = 0 is msckf_b200_aid_stack_update with chi2_max = chi2[m - 1].  S_AA not positive
+ * definite in any round: stack.status 1 (outcome -1), nothing written.  No item left: stack.status 2 (outcome -1, dof 0), nothing
+ * written.  A rejection writes nothing.  The thresholds come from the caller, e.g. the chi-square quantile 1 - alpha of d dof. */
+typedef struct {
+  double chi2[32];   /* chi2[d-1], d = 1..32: gate on the NIS of a set of d rows and on an item's t_j of d rows; finite, > 0 */
+  int max_exclude;   /* 0 .. 7 */
+} msckf_b200_aid_fde;
+typedef struct {
+  double nis;        /* r_j^T S_jj^-1 r_j: the item alone against the prior P (NaN: degenerate) */
+  double test;       /* t_j of the last round the item took part in (NaN: no exclusion round ran) */
+  int state;         /* 0 used, 1 excluded, 2 degenerate (dropped), 3 not applied (stack rejected) */
+  int round;         /* 0-based round in which it was excluded, else -1 */
+} msckf_b200_aid_item_result;
+typedef struct {
+  msckf_b200_aid_result stack;  /* nis / dof of the last set gated, dx_norm, applied, status 0 / 1 / 2 as above */
+  int outcome;                  /* 0 passed, 1 passed after exclusions, 2 rejected at max_exclude, 3 rejected: not identifiable;
+                                   -1 with status 1 or 2 */
+  int n_excluded;
+  msckf_b200_aid_item_result item[8];  /* item[k] for k < n_items; the others have state -1 */
+} msckf_b200_aid_fde_result;
+/* Refusals (MSCKF_B200_ERR_ARG, nothing written): everything msckf_b200_aid_stack_update refuses, fde NULL, a chi2 entry that
+ * is not finite or not > 0, max_exclude outside 0..7; an un-fetched update returns MSCKF_B200_ERR_STATE.  A non-finite dx or P
+ * entry returns MSCKF_B200_ERR_NUMERIC with the update applied.  One launch, one copy each way, one synchronisation. */
+int msckf_b200_aid_stack_update_fde(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items,
+                                    const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out);
+/* the same for every member of a batch with one fde (n_items[i] = 0 leaves member i untouched and out[i] not written); every
+ * member is validated before anything is launched.  One launch per 32 updated members. */
+int msckf_b200_batch_aid_stack_update_fde(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                          const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out);
 /* ---- mapped landmarks: image observations of landmarks whose position is known (prior map, surveyed marker, relocalisation) --
  * Observation i is (clone[i], z[i] normalised image coordinates, p_L_G[i] landmark position in G).  With C = C(q_CG) and p_C_G of
  * that clone: p_C = C (p_L - p_C_G), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), Jacobian the 2 x 6

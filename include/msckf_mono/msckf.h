@@ -391,6 +391,21 @@ class MSCKF {
     aidAbsorb(r);
     return r;
   }
+  // the same stack with fault detection and exclusion over its items (msckf_b200_aid_stack_update_fde): degenerate items are
+  // dropped, and up to fde.max_exclude items failing the block w-test are excluded before the rest is applied.  A thresholds
+  // table or max_exclude the C-ABI would refuse throws std::invalid_argument.  Bookkeeping as aidedUpdate(items).
+  msckf_b200_aid_fde_result aidedUpdate(const std::vector<msckf_b200_aid_item>& items, const msckf_b200_aid_fde& fde) {
+    checkFde(fde);
+    msckf_b200_aid_fde_result r = {};
+    checkNumeric(msckf_b200_aid_stack_update_fde(eng(), items.data(), (int)items.size(), &fde, &r), "msckf_b200_aid_stack_update_fde");
+    aidAbsorb(r.stack);
+    return r;
+  }
+  static void checkFde(const msckf_b200_aid_fde& fde) {
+    for (int d = 0; d < 32; ++d)
+      if (!(std::isfinite(fde.chi2[d]) && fde.chi2[d] > 0.0)) throw std::invalid_argument("MSCKF::aidedUpdate: fde.chi2 must be finite and > 0");
+    if (fde.max_exclude < 0 || fde.max_exclude > 7) throw std::invalid_argument("MSCKF::aidedUpdate: fde.max_exclude outside 0..7");
+  }
   // v_I: the IMU's velocity in its own frame (wheel or leg odometry); mask bits 0..2 select the rows used, R is popcount(mask)
   // square over them.  mask 0b110 with v_I = 0 is the non-holonomic constraint v_y = v_z = 0.
   msckf_b200_aid_result bodyVelocityUpdate(const Vector3<double>& v_I, const MatrixX<double>& R, int mask = 7, double chi2_max = 0) {
@@ -1114,6 +1129,27 @@ class MSCKFBatch {
     else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_stack_update");
     for (size_t i = 0; i < n; ++i)
       if (!items[i].empty()) filters_[i]->aidAbsorb(r[i]);
+    return r;
+  }
+  // MSCKF::aidedUpdate(items, fde) of every filter (items[i] empty: filter i is left alone) as one
+  // msckf_b200_batch_aid_stack_update_fde with one fde: one launch per 32 updated filters and one synchronisation.
+  std::vector<msckf_b200_aid_fde_result> aidedUpdate(const std::vector<std::vector<msckf_b200_aid_item>>& items, const msckf_b200_aid_fde& fde) {
+    const size_t n = size();
+    if (items.size() != n) throw std::invalid_argument("MSCKFBatch::aidedUpdate: one item list per filter");
+    MSCKF<_S>::checkFde(fde);
+    std::vector<const msckf_b200_aid_item*> p(n, nullptr);
+    std::vector<int> k(n, 0);
+    for (size_t i = 0; i < n; ++i) {
+      p[i] = items[i].empty() ? nullptr : items[i].data();
+      k[i] = (int)items[i].size();
+    }
+    flushImu();
+    std::vector<msckf_b200_aid_fde_result> r(n, msckf_b200_aid_fde_result());
+    const int rc = msckf_b200_batch_aid_stack_update_fde(batch_, p.data(), k.data(), &fde, r.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch stacked aided update (FDE): " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_stack_update_fde");
+    for (size_t i = 0; i < n; ++i)
+      if (!items[i].empty()) filters_[i]->aidAbsorb(r[i].stack);
     return r;
   }
   // MSCKF::landmarkUpdate of every filter (obs[i] empty: filter i is left alone) as one msckf_b200_batch_landmark_update: three

@@ -85,6 +85,13 @@ int msckf_mono_batch_aid_update(void* batch, const msckf_b200_aid* aid, msckf_b2
 int msckf_mono_aid_stack_update(void* h, const msckf_b200_aid_item* items, int n_items, double chi2_max, msckf_b200_aid_result* out);
 int msckf_mono_batch_aid_stack_update(void* batch, const int* n_items, const msckf_b200_aid_item* items, double chi2_max,
                                       msckf_b200_aid_result* out);
+/* the same stacks with fault detection and exclusion over their items (MSCKF::aidedUpdate(items, fde),
+ * msckf_b200_aid_stack_update_fde: rounds, outcomes and errors there); one fde for the batch.  A NULL fde, a chi2 entry that is
+ * not finite or not > 0, or max_exclude outside 0..7 fails before any device call. */
+int msckf_mono_aid_stack_update_fde(void* h, const msckf_b200_aid_item* items, int n_items, const msckf_b200_aid_fde* fde,
+                                    msckf_b200_aid_fde_result* out);
+int msckf_mono_batch_aid_stack_update_fde(void* batch, const int* n_items, const msckf_b200_aid_item* items,
+                                          const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out);
 int msckf_mono_body_velocity_update(void* h, const double* v3, int mask, const double* R, double chi2_max, msckf_b200_aid_result* out);
 int msckf_mono_relative_pose_update(void* h, int state_id_a, int state_id_b, const double* p3, const double* q4, const double* R36,
                                     double chi2_max, msckf_b200_aid_result* out);

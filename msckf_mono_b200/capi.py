@@ -95,6 +95,37 @@ def aid_items(items):
     return arr, keep
 
 
+class AidFde(C.Structure):
+    _fields_ = [("chi2", C.c_double * 32), ("max_exclude", C.c_int)]
+
+
+class AidItemResult(C.Structure):
+    _fields_ = [("nis", C.c_double), ("test", C.c_double), ("state", C.c_int), ("round", C.c_int)]
+
+
+class AidFdeResult(C.Structure):
+    _fields_ = [("stack", AidResult), ("outcome", C.c_int), ("n_excluded", C.c_int), ("item", AidItemResult * 8)]
+
+    def as_dict(self, n_items):
+        d = self.stack.as_dict()
+        d.update(outcome=self.outcome, n_excluded=self.n_excluded,
+                 items=[{k: getattr(self.item[j], k) for k, _ in AidItemResult._fields_} for j in range(n_items)])
+        return d
+
+
+def fde_thresholds(alpha):
+    """chi2[d - 1] = the chi-square quantile 1 - alpha of d dof, d = 1..32 (the thresholds of msckf_b200_aid_fde)"""
+    from scipy.stats import chi2
+    return [float(chi2.ppf(1.0 - alpha, d)) for d in range(1, 33)]
+
+
+def fde_struct(fde):
+    """msckf_b200_aid_fde of fde = dict chi2 (32 thresholds, chi2[d - 1] for d rows; see fde_thresholds), max_exclude (0..7)"""
+    chi2 = np.asarray(fde["chi2"], dtype=np.float64).ravel()
+    assert chi2.size == 32, chi2.size
+    return AidFde((C.c_double * 32)(*chi2.tolist()), int(fde["max_exclude"]))
+
+
 class Landmarks(C.Structure):
     _fields_ = [("n_obs", C.c_int), ("clone", C.c_void_p), ("z", C.c_void_p), ("p_L_G", C.c_void_p), ("R", C.c_void_p),
                 ("chi2_obs", C.c_double), ("gamma", C.c_void_p), ("flag", C.c_void_p), ("max_iter", C.c_int), ("tol", C.c_double)]
@@ -330,14 +361,19 @@ class Batch:
         check(lib().msckf_b200_batch_aid_update(self.h, (Aid * n)(*[a for a, _ in st]), out), "msckf_b200_batch_aid_update")
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
-    def aid_stack_update(self, stacks, chi2_max=0.0):
+    def aid_stack_update(self, stacks, chi2_max=0.0, fde=None):
         """msckf_b200_batch_aid_stack_update: stacks[i] = list of item dicts for engine i (see aid_items; None or [] leaves
-        engine i alone); a list of result dicts (None for an engine left alone)"""
+        engine i alone); a list of result dicts (None for an engine left alone).  fde (see fde_struct):
+        msckf_b200_batch_aid_stack_update_fde instead (chi2_max unused); each dict then has outcome, n_excluded and items"""
         n = len(self.engines)
         assert len(stacks) == n
         st = [aid_items(s or []) for s in stacks]
         ptrs = (C.POINTER(AidItem) * n)(*[C.cast(a, C.POINTER(AidItem)) for a, _ in st])
         cnt = (C.c_int * n)(*[len(s or []) for s in stacks])
+        if fde is not None:
+            f, out = fde_struct(fde), (AidFdeResult * n)()
+            check(lib().msckf_b200_batch_aid_stack_update_fde(self.h, ptrs, cnt, C.byref(f), out), "msckf_b200_batch_aid_stack_update_fde")
+            return [o.as_dict(len(s)) if s else None for s, o in zip(stacks, out)]
         out = (AidResult * n)()
         check(lib().msckf_b200_batch_aid_stack_update(self.h, ptrs, cnt, C.c_double(chi2_max), out), "msckf_b200_batch_aid_stack_update")
         return [o.as_dict() if s else None for s, o in zip(stacks, out)]
@@ -496,9 +532,15 @@ class Engine:
         check(lib().msckf_b200_aid_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_aid_update")
         return out.as_dict()
 
-    def aid_stack_update(self, items, chi2_max=0.0):
-        """msckf_b200_aid_stack_update: one stacked update of items (see aid_items); the result as a dict"""
+    def aid_stack_update(self, items, chi2_max=0.0, fde=None):
+        """msckf_b200_aid_stack_update: one stacked update of items (see aid_items); the result as a dict.  fde (see
+        fde_struct): msckf_b200_aid_stack_update_fde instead (chi2_max unused); the dict then has outcome, n_excluded and items"""
         arr, keep = aid_items(items)
+        if fde is not None:
+            f, out = fde_struct(fde), AidFdeResult()
+            check(lib().msckf_b200_aid_stack_update_fde(self.h, arr, C.c_int(len(items)), C.byref(f), C.byref(out)),
+                  "msckf_b200_aid_stack_update_fde")
+            return out.as_dict(len(items))
         out = AidResult()
         check(lib().msckf_b200_aid_stack_update(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)),
               "msckf_b200_aid_stack_update")

@@ -6,6 +6,11 @@
 //           S = H P H^T + R = L L^T with r as an extra row (y = L^-1 r), W = L^-1 H P, NIS = y^T y, the optional chi-square
 //           gate, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to the filter precision
 //           once) and the state injection of k_syrk (inject_state).  All arithmetic in fp64.
+//   k_aid<S, NM, true> (msckf_b200_aid_stack_update_fde): the same kernel with fault detection and exclusion over the stack's
+//           items.  A degenerate item is dropped instead of ending the member; rounds over the kept set A rebuild S_AA from
+//           H P (kept in Wt until the update) and R, factor it, gate NIS_A on chi2[d_A - 1] and, while it fails, exclude the
+//           item with the largest t_j / chi2[d_j - 1] (t_j = y_j^T B_j^-1 y_j, y = S_AA^-1 r, B_j = (S_AA^-1)_jj; one warp per
+//           item).  The update of the final A runs the arithmetic of the plain kernel on those rows, in their order.
 // One CTA per member, one launch for everything; one body for a single filter (NM = 1) and a device batch (NM =
 // kBatchMembers), like k_nees.  W^T and dx live in dynamic shared memory where they fit, else in a per-member global workspace.
 #pragma once
@@ -37,6 +42,40 @@ struct AidOut {
   int dof, applied, status;
   int numeric;  // a non-finite dx or P entry was written
 };
+// per-member result of the FDE form: the plain result, then msckf_b200_aid_fde_result's outcome, count and item block
+struct AidItemOut {
+  double nis, test;
+  int state, round;
+};
+struct AidFdeOut {
+  AidOut stack;
+  int outcome, n_excluded;
+  AidItemOut item[kAidMaxItems];
+};
+constexpr int kAidFdeIn = kAidMaxRows + 1;  // FDE: chi2[32] then max_exclude (as a double) follow R in the input block
+
+// lane 0: v^T A^-1 v of a d x d symmetric A (row-major, lower triangle read, overwritten by its Cholesky factor; v by
+// L^-1 v); NaN when A is not positive definite.  (k_aid<S, NM, true>: an item's NIS and its exclusion statistic)
+__device__ __noinline__ double aid_small_quad(double* A, double* v, int d) {
+  double q = 0.0;
+  for (int j = 0; j < d; ++j) {
+    double s = A[j * d + j];
+    for (int k = 0; k < j; ++k) s -= A[j * d + k] * A[j * d + k];
+    if (!(s > 0.0)) return __longlong_as_double(0x7ff8000000000000ll);
+    const double l = sqrt(s);
+    A[j * d + j] = l;
+    for (int i = j + 1; i < d; ++i) {
+      double t = A[i * d + j];
+      for (int k = 0; k < j; ++k) t -= A[i * d + k] * A[j * d + k];
+      A[i * d + j] = t / l;
+    }
+    double x = v[j];
+    for (int k = 0; k < j; ++k) x -= A[j * d + k] * v[k];
+    v[j] = x / l;
+    q += v[j] * v[j];
+  }
+  return q;
+}
 
 // one item of a stack: its model, a (CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING, CLONE_RANGE,
 // CLONE_PLANE_RANGE: a clone's window position; BODY_VELOCITY, ANTENNA_POSITION: the row mask), b (RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: the row
@@ -235,7 +274,7 @@ __device__ __noinline__ int aid_item_rows(const AidItem it, const double* z, con
   return 0;
 }
 
-template <class S, int NM>
+template <class S, int NM, bool FDE = false>
 __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, NM> a) {
   extern __shared__ double aid_dyn[];
   const int f = NM == 1 ? 0 : blockIdx.x;
@@ -261,6 +300,177 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
 
   // ---- residual (fp64) and the rows of H, one thread per item
   int degenerate = 0;
+  int mA = m;  // the rows of the update (FDE: of the kept items, the first mA entries of each Wt row; y in row mA of L)
+  if constexpr (FDE) {  // r stays in s_r for every round; a degenerate item is dropped from A (its rows are never read)
+    __shared__ double s_r[kAidMaxRows];
+    __shared__ int s_ri[kAidMaxRows], s_c0[kAidMaxItems];  // row k of S_AA is stack row s_ri[k]; item w's first row in S_AA
+    __shared__ double s_t[kAidMaxItems], s_blk[kAidMaxItems][42];  // t_j of the round; a warp's d x d block and vector
+    __shared__ unsigned s_A;  // the items of A (bits)
+    __shared__ int s_mA, s_done;
+    AidFdeOut* const fo = reinterpret_cast<AidFdeOut*>(out);
+    const double* __restrict__ const chi2 = R + m * m;
+    const int n_items = a.m[f].n_items;
+    const auto rows_of = [&](int k) { return (k + 1 < n_items ? a.m[f].item[k + 1].row : m) - a.m[f].item[k].row; };
+    if (t < n_items) {
+      degenerate = aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, s_r, s_col, s_coef, s_nnz);
+      fo->item[t] = {__longlong_as_double(0x7ff8000000000000ll), __longlong_as_double(0x7ff8000000000000ll), degenerate ? 2 : 3, -1};
+    }
+    const unsigned keep = __ballot_sync(0xffffffffu, t < n_items && !degenerate);
+    if (t == 0) { s_A = keep; s_mA = 0; }
+    __syncthreads();
+    if (s_A == 0u) {  // every item degenerate: nothing is written
+      if (t == 0) {
+        out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
+        out->dof = 0; out->applied = 0; out->status = 2; out->numeric = 0;
+        fo->outcome = -1; fo->n_excluded = 0;
+      }
+      return;
+    }
+    // H P of the kept rows, stored transposed (stride m): kept until the update, S_AA of every round is formed from it
+    for (int idx = t; idx < m * n; idx += kAidThreads) {
+      const int i = idx / n, c = idx - i * n;
+      int k = 0;
+      while (k + 1 < n_items && a.m[f].item[k + 1].row <= i) ++k;
+      if (!((s_A >> k) & 1u)) continue;
+      double s = s_coef[i][0] * (double)P[(size_t)s_col[i][0] * ldp + c];
+      for (int q = 1; q < s_nnz[i]; ++q) s += s_coef[i][q] * (double)P[(size_t)s_col[i][q] * ldp + c];
+      Wt[(size_t)c * m + i] = s;
+    }
+    __syncthreads();
+    // each kept item alone against the prior: r_j^T S_jj^-1 r_j (warp j, lane 0)
+    if (warp < n_items && lane == 0 && ((s_A >> warp) & 1u)) {
+      const int r0 = a.m[f].item[warp].row, d = rows_of(warp);
+      double* B = s_blk[warp];
+      for (int i = 0; i < d; ++i) {
+        for (int j = 0; j <= i; ++j) {
+          const int ri = r0 + i, rj = r0 + j;
+          double s = s_coef[rj][0] * Wt[(size_t)s_col[rj][0] * m + ri];
+          for (int q = 1; q < s_nnz[rj]; ++q) s += s_coef[rj][q] * Wt[(size_t)s_col[rj][q] * m + ri];
+          B[i * d + j] = s + R[ri * m + rj];
+        }
+        B[36 + i] = s_r[r0 + i];
+      }
+      fo->item[warp].nis = aid_small_quad(B, B + 36, d);
+    }
+    const int max_exclude = (int)R[m * m + kAidMaxRows];
+    int outcome = -1, n_exc = 0;
+    for (int round = 0;; ++round) {
+      // ---- S_AA (lower) from H P and R with the expression of the plain kernel, r_A as row m_A
+      if (t == 0) {
+        int k = 0;
+        for (int w = 0; w < n_items; ++w) {
+          if (!((s_A >> w) & 1u)) continue;
+          s_c0[w] = k;
+          for (int i = 0, r0 = a.m[f].item[w].row, d = rows_of(w); i < d; ++i) s_ri[k++] = r0 + i;
+        }
+        s_mA = k;
+      }
+      __syncthreads();
+      const int ma = s_mA;
+      for (int idx = t; idx < ma * ma; idx += kAidThreads) {
+        const int i = idx / ma, j = idx - i * ma;
+        if (j > i) continue;
+        const int ri = s_ri[i], rj = s_ri[j];
+        double s = s_coef[rj][0] * Wt[(size_t)s_col[rj][0] * m + ri];
+        for (int q = 1; q < s_nnz[rj]; ++q) s += s_coef[rj][q] * Wt[(size_t)s_col[rj][q] * m + ri];
+        L[i][j] = s + R[ri * m + rj];
+      }
+      if (t < ma) L[ma][t] = s_r[s_ri[t]];
+      __syncthreads();
+      if (warp == 0) {
+        const int nv = warp_chol(L, ma, idg, lane);
+        if (lane == 0) s_nv = nv;
+        if (nv == ma) {
+          const double x = warp_row_solve(lane < ma ? L[ma][lane] : 0.0, L, idg, ma, lane);
+          if (lane < ma) L[ma][lane] = x;
+        }
+      }
+      __syncthreads();
+      if (s_nv < ma) {  // S_AA not positive definite: nothing is written
+        if (t == 0) {
+          out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
+          out->dof = ma; out->applied = 0; out->status = 1; out->numeric = 0;
+          fo->outcome = -1; fo->n_excluded = n_exc;
+        }
+        return;
+      }
+      if (t == 0) {
+        double g = 0.0;
+        for (int i = 0; i < ma; ++i) g += L[ma][i] * L[ma][i];
+        out->nis = g; out->dof = ma; out->status = 0;
+        s_done = !(g > chi2[ma - 1]) ? (n_exc ? 1 : 0) : n_exc >= max_exclude ? 2 : __popc(s_A) == 1 ? 3 : -1;
+      }
+      __syncthreads();
+      if (s_done >= 0) { outcome = s_done; break; }
+      // ---- exclusion round: warp w of A forms g_a = L^-1 e_a over its rows, y_w = G^T (L^-1 r_A), B_w = G^T G, t_w
+      if (warp < n_items && ((s_A >> warp) & 1u)) {
+        const int d = rows_of(warp), c0 = s_c0[warp];
+        const double u = lane < ma ? L[ma][lane] : 0.0;
+        double g[6];
+#pragma unroll
+        for (int p = 0; p < 6; ++p) {  // (lanes >= m_A hold whatever rows past the factor give: kept out of the sums)
+          if (p < d) g[p] = warp_row_solve(lane == c0 + p ? 1.0 : 0.0, L, idg, ma, lane);
+          if (lane >= ma) g[p] = 0.0;
+        }
+        double* B = s_blk[warp];
+#pragma unroll
+        for (int p = 0; p < 6; ++p) {
+          if (p >= d) break;
+          const double yp = warp_sum(g[p] * u);
+          if (lane == 0) B[36 + p] = yp;
+#pragma unroll
+          for (int q = 0; q <= p; ++q) {
+            const double bpq = warp_sum(g[p] * g[q]);
+            if (lane == 0) B[p * d + q] = bpq;
+          }
+        }
+        if (lane == 0) {
+          s_t[warp] = aid_small_quad(B, B + 36, d);
+          fo->item[warp].test = s_t[warp];
+        }
+      }
+      __syncthreads();
+      if (t == 0) {  // j* = argmax t_j / chi2[d_j - 1], the lowest item on a tie; not above 1: no single item explains it
+        int best = -1;
+        double rb = 1.0;
+        for (int w = 0; w < n_items; ++w) {
+          if (!((s_A >> w) & 1u)) continue;
+          const double rw = s_t[w] / chi2[rows_of(w) - 1];
+          if (rw > rb) { rb = rw; best = w; }
+        }
+        if (best < 0) {
+          s_done = 3;
+        } else {
+          s_A &= ~(1u << best);
+          fo->item[best].state = 1; fo->item[best].round = round;
+        }
+      }
+      __syncthreads();
+      if (s_done >= 0) { outcome = s_done; break; }
+      ++n_exc;
+    }
+    if (t == 0) {
+      fo->outcome = outcome; fo->n_excluded = n_exc;
+      for (int w = 0; w < n_items; ++w)
+        if ((s_A >> w) & 1u) fo->item[w].state = outcome <= 1 ? 0 : 3;
+      out->applied = outcome <= 1;
+      s_apply = outcome <= 1;
+      s_bad = 0;
+      if (!s_apply) { out->dx_norm = 0.0; out->numeric = 0; }
+    }
+    __syncthreads();
+    if (!s_apply) return;
+    // ---- W = L^-1 H P over the rows of A, gathered in order into the first m_A entries of each Wt row
+    mA = s_mA;
+    for (int r = warp; r < n; r += kAidThreads / 32) {
+      double* row = Wt + (size_t)r * m;
+      const double x0 = lane < mA ? row[s_ri[lane]] : 0.0;
+      __syncwarp();
+      const double x = warp_row_solve(x0, L, idg, mA, lane);
+      if (lane < mA) row[lane] = x;
+    }
+    __syncthreads();
+  } else {  // the plain single-model, LINEAR and stacked update (left at its original indentation)
   if (lin) {
     if (t < m) L[m][t] = in[t];
   } else if (t < a.m[f].n_items) {
@@ -339,12 +549,13 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
     if (t == 0) { out->dx_norm = 0.0; out->numeric = 0; }
     return;
   }
+  }  // (FDE)
   // ---- dx = W^T y, and P <- P - W^T W (lower triangle in fp64, written to both halves: exactly symmetric)
   double nn = 0.0;
   for (int c = t; c < n; c += kAidThreads) {
     const double* w = Wt + (size_t)c * m;
     double s = 0.0;
-    for (int i = 0; i < m; ++i) s += w[i] * L[m][i];
+    for (int i = 0; i < mA; ++i) s += w[i] * L[mA][i];
     dx[c] = s;
     nn += s * s;
   }
@@ -355,7 +566,7 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
     const double* wr = Wt + (size_t)r * m;
     const double* wc = Wt + (size_t)c * m;
     double v = 0.0;
-    for (int i = 0; i < m; ++i) v += wr[i] * wc[i];
+    for (int i = 0; i < mA; ++i) v += wr[i] * wc[i];
     const S x = (S)((double)P[(size_t)r * ldp + c] - v);
     if (!isfinite((double)x)) bad = 1;
     P[(size_t)r * ldp + c] = x;

@@ -243,6 +243,9 @@ struct CtxBase {
   // msckf_b200_aid_stack_update / _batch_aid_stack_update): one launch per 32, one synchronisation
   virtual int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) = 0;
   virtual int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) = 0;
+  // the stacked form with fault detection and exclusion over the items (msckf_b200_aid_stack_update_fde / _batch_..._fde)
+  virtual int aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
+                            msckf_b200_aid_fde_result* out) = 0;
   // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
   virtual int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) = 0;
   cudaStream_t stream = nullptr;
@@ -514,7 +517,11 @@ struct Ctx : CtxBase {
   int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) override;
   int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) override;
   int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) override;
-  int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what);
+  int aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
+                    msckf_b200_aid_fde_result* out) override;
+  int aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job);
+  int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what, const msckf_b200_aid_fde* fde = nullptr,
+              msckf_b200_aid_fde_result* fout = nullptr);
   int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
@@ -1510,6 +1517,7 @@ int Ctx<S>::nees(const double* const* truth_imu, const double* const* truth_pose
 // else in the workspace.  Nothing is launched unless every member is valid: aid and aid_stack check their arguments and
 // build one AidJob per member, aid_run launches them.
 static_assert(offsetof(mb::AidOut, status) == offsetof(msckf_b200_aid_result, status), "mb::AidOut must start like msckf_b200_aid_result");
+static_assert(offsetof(mb::AidFdeOut, stack) == 0 && sizeof(mb::AidFdeOut) % alignof(double) == 0, "mb::AidFdeOut must start with mb::AidOut");
 static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && (int)MSCKF_B200_AID_RELATIVE_POSE == (int)mb::kAidRelativePose &&
                   (int)MSCKF_B200_AID_ANTENNA_POSITION == (int)mb::kAidAntennaPosition &&
                   (int)MSCKF_B200_AID_CLONE_ANTENNA_POSITION == (int)mb::kAidCloneAntennaPosition &&
@@ -1557,23 +1565,47 @@ int Ctx<S>::aid_stack(const msckf_b200_aid_item* const* items, const int* n_item
   if (!items || !n_items || !out) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: null argument");
   RC(members_ready("aid_stack_update"));
   if (std::isnan(chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: chi2_max is NaN");
-  const int nf = (int)eng.size();
-  std::vector<AidJob> job(nf);
-  for (int i = 0; i < nf; ++i) {
-    if (n_items[i] == 0) continue;
-    const std::string who = " (member " + std::to_string(i) + ")";
-    if (n_items[i] < 0 || n_items[i] > mb::kAidMaxItems) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: 1 to 8 items per stack" + who);
-    if (!items[i]) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: null item list" + who);
-    for (int k = 0; k < n_items[i]; ++k)
-      RC(aid_append(job[i], items[i][k], eng[i]->M, "aid_stack_update", " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")"));
-    job[i].chi2_max = chi2_max;
-  }
+  std::vector<AidJob> job;
+  RC(aid_stack_jobs(items, n_items, "aid_stack_update", job));
+  for (AidJob& j : job) j.chi2_max = chi2_max;
   return aid_run(job, out, "aid_stack_update");
 }
 
 template <class S>
-int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what) {
+int Ctx<S>::aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
+                          msckf_b200_aid_fde_result* out) {
+  if (!items || !n_items || !fde || !out) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: null argument");
+  RC(members_ready("aid_stack_update_fde"));
+  for (int d = 0; d < mb::kAidMaxRows; ++d)
+    if (!(std::isfinite(fde->chi2[d]) && fde->chi2[d] > 0.0))
+      return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: chi2[" + std::to_string(d) + "] is not finite and > 0");
+  if (fde->max_exclude < 0 || fde->max_exclude > mb::kAidMaxItems - 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: max_exclude outside 0..7");
+  std::vector<AidJob> job;
+  RC(aid_stack_jobs(items, n_items, "aid_stack_update_fde", job));
+  return aid_run(job, nullptr, "aid_stack_update_fde", fde, out);
+}
+
+// one AidJob per member of a stacked call (n_items[i] = 0: member i is left alone); 0, or MSCKF_B200_ERR_ARG
+template <class S>
+int Ctx<S>::aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job) {
   const int nf = (int)eng.size();
+  job.assign(nf, AidJob{});
+  for (int i = 0; i < nf; ++i) {
+    if (n_items[i] == 0) continue;
+    const std::string who = " (member " + std::to_string(i) + ")";
+    if (n_items[i] < 0 || n_items[i] > mb::kAidMaxItems) return fail(MSCKF_B200_ERR_ARG, w + ": 1 to 8 items per stack" + who);
+    if (!items[i]) return fail(MSCKF_B200_ERR_ARG, w + ": null item list" + who);
+    for (int k = 0; k < n_items[i]; ++k)
+      RC(aid_append(job[i], items[i][k], eng[i]->M, w, " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")"));
+  }
+  return 0;
+}
+
+template <class S>
+int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what, const msckf_b200_aid_fde* fde,
+                    msckf_b200_aid_fde_result* fout) {
+  const int nf = (int)eng.size();
+  const size_t osz = fde ? sizeof(mb::AidFdeOut) : sizeof(mb::AidOut);  // FDE: the item block follows the plain result
   std::vector<int> idx;
   std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
   for (int i = 0; i < nf; ++i) {
@@ -1582,13 +1614,13 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
     woff[i + 1] = woff[i];
     if (job[i].n_items == 0) continue;
     idx.push_back(i);
-    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (job[i].H ? (size_t)m * n : 0)));
+    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (job[i].H ? (size_t)m * n : 0) + (fde ? mb::kAidFdeIn : 0)));
     if (mb::aid_ws_bytes(n, m) > kAidSmemMax) woff[i + 1] = woff[i] + up256(mb::aid_ws_bytes(n, m));
   }
   if (idx.empty()) return 0;
   const size_t res_off = up256(off[nf]);
   CK(cudaSetDevice(device));
-  RC(io.ensure(res_off + sizeof(mb::AidOut) * nf, stream));
+  RC(io.ensure(res_off + osz * nf, stream));
   RC(ws.ensure(woff[nf], stream));
   for (int i : idx) {
     const AidJob& q = job[i];
@@ -1602,29 +1634,42 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
       for (int r = 0; r < mk; ++r) memcpy(R + (size_t)(r0 + r) * m + r0, q.R[k] + (size_t)r * mk, sizeof(double) * mk);
     }
     if (q.H) memcpy(h + mb::kAidZ + m * m, q.H, sizeof(double) * m * n);
+    if (fde) {
+      memcpy(R + m * m, fde->chi2, sizeof(double) * mb::kAidMaxRows);
+      R[m * m + mb::kAidMaxRows] = fde->max_exclude;
+    }
   }
   CK(cudaMemcpyAsync(io.d, io.h, off[nf], cudaMemcpyHostToDevice, stream));
-  mb::AidOut* d_out = reinterpret_cast<mb::AidOut*>(io.d + res_off);
   per_member(idx, false,
              [&](int i) {
                const bool global = woff[i + 1] > woff[i];
                return eng[i]->aid_args(job[i], reinterpret_cast<const double*>(io.d + off[i]),
-                                       global ? reinterpret_cast<double*>(ws.d + woff[i]) : nullptr, d_out + i);
+                                       global ? reinterpret_cast<double*>(ws.d + woff[i]) : nullptr,
+                                       reinterpret_cast<mb::AidOut*>(io.d + res_off + osz * i));
              },
              [&](const auto& a, int nm) {
+               constexpr int NM = (int)std::extent<decltype(std::decay_t<decltype(a)>::m)>::value;
                size_t smem = 0;  // the largest need of the members whose W^T and dx are in shared memory
                for (int j = 0; j < nm; ++j)
                  if (!a.m[j].ws) smem = std::max(smem, mb::aid_ws_bytes(15 + 6 * a.m[j].M, a.m[j].m));
-               mb::k_aid<<<nm, mb::kAidThreads, smem, stream>>>(a);
+               if (fde) mb::k_aid<S, NM, true><<<nm, mb::kAidThreads, smem, stream>>>(a);
+               else mb::k_aid<<<nm, mb::kAidThreads, smem, stream>>>(a);
              });
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(io.h + res_off, io.d + res_off, sizeof(mb::AidOut) * nf, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(io.h + res_off, io.d + res_off, osz * nf, cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));  // one synchronisation for the whole batch
-  const mb::AidOut* h_out = reinterpret_cast<const mb::AidOut*>(io.h + res_off);
   int numeric = -1;
   for (int i : idx) {
-    const mb::AidOut& o = h_out[i];
-    out[i].nis = o.nis; out[i].dx_norm = o.dx_norm; out[i].dof = o.dof; out[i].applied = o.applied; out[i].status = o.status;
+    const mb::AidOut& o = *reinterpret_cast<const mb::AidOut*>(io.h + res_off + osz * i);
+    msckf_b200_aid_result& r = fde ? fout[i].stack : out[i];
+    r.nis = o.nis; r.dx_norm = o.dx_norm; r.dof = o.dof; r.applied = o.applied; r.status = o.status;
+    if (fde) {
+      const mb::AidFdeOut& g = *reinterpret_cast<const mb::AidFdeOut*>(&o);
+      fout[i].outcome = g.outcome; fout[i].n_excluded = g.n_excluded;
+      for (int k = 0; k < mb::kAidMaxItems; ++k)
+        fout[i].item[k] = k < job[i].n_items ? msckf_b200_aid_item_result{g.item[k].nis, g.item[k].test, g.item[k].state, g.item[k].round}
+                                             : msckf_b200_aid_item_result{std::nan(""), std::nan(""), -1, -1};
+    }
     if (o.numeric && numeric < 0) numeric = i;
   }
   return numeric_error(what, numeric);
@@ -2067,6 +2112,11 @@ int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->aid_stack(items, n_items, chi2_max, out);
 }
+int msckf_b200_batch_aid_stack_update_fde(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                          const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->aid_stack_fde(items, n_items, fde, out);
+}
 int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->landmarks(lm, nullptr, out);
@@ -2116,6 +2166,12 @@ int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item*
   if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
   if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: 1 to 8 items per stack");
   return e->impl->solo_ctx()->aid_stack(&items, &n_items, chi2_max, out);
+}
+int msckf_b200_aid_stack_update_fde(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, const msckf_b200_aid_fde* fde,
+                                    msckf_b200_aid_fde_result* out) {
+  if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: 1 to 8 items per stack");
+  return e->impl->solo_ctx()->aid_stack_fde(&items, &n_items, fde, out);
 }
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   return msckf_b200_map_landmark_update(e, lm, nullptr, out);

@@ -141,15 +141,20 @@ class FilterBatch:
         self._call("aid_update", (Aid * n)(*[a for a, _ in st]), out)
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
-    def aid_stack_update(self, stacks, chi2_max=0.0):
+    def aid_stack_update(self, stacks, chi2_max=0.0, fde=None):
         """MSCKFBatch::aidedUpdate(items): stacks[i] = list of item dicts for filter i (as for capi.aid_items; None or []:
-        filter i left alone); one device call for the batch.  A list of result dicts (None for a filter left alone)."""
-        from .capi import AidResult, aid_items
+        filter i left alone); one device call for the batch.  A list of result dicts (None for a filter left alone).  fde (as for
+        capi.fde_struct): MSCKFBatch::aidedUpdate(items, fde) instead; each dict then has outcome, n_excluded and items."""
+        from .capi import AidFdeResult, AidResult, aid_items, fde_struct
         n = len(self.filters)
         assert len(stacks) == n
         flat = [it for s in stacks for it in (s or [])]
         arr, keep = aid_items(flat)
         cnt = np.array([len(s or []) for s in stacks], dtype=np.int32)
+        if fde is not None:
+            f, out = fde_struct(fde), (AidFdeResult * n)()
+            self._call("aid_stack_update_fde", cnt.ctypes.data_as(_ip), arr, C.byref(f), out)
+            return [o.as_dict(len(s)) if s else None for s, o in zip(stacks, out)]
         out = (AidResult * n)()
         self._call("aid_stack_update", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), out)
         return [o.as_dict() if s else None for s, o in zip(stacks, out)]
@@ -385,11 +390,16 @@ class CFilter:
         self._chk(self._f("aid_update")(self.h, C.byref(a), C.byref(out)), "aid_update")
         return out.as_dict()
 
-    def aid_stack_update(self, items, chi2_max=0.0):
+    def aid_stack_update(self, items, chi2_max=0.0, fde=None):
         """MSCKF::aidedUpdate(items) (include/msckf_b200.h: msckf_b200_aid_stack_update): items as for capi.aid_items, one
-        chi2_max for the stack.  A dict nis, dx_norm, dof, applied, status."""
-        from .capi import AidResult, aid_items
+        chi2_max for the stack.  A dict nis, dx_norm, dof, applied, status.  fde (as for capi.fde_struct):
+        MSCKF::aidedUpdate(items, fde) (msckf_b200_aid_stack_update_fde) instead; the dict then has outcome, n_excluded, items."""
+        from .capi import AidFdeResult, AidResult, aid_items, fde_struct
         arr, keep = aid_items(items)
+        if fde is not None:
+            f, out = fde_struct(fde), AidFdeResult()
+            self._chk(self._f("aid_stack_update_fde")(self.h, arr, C.c_int(len(items)), C.byref(f), C.byref(out)), "aid_stack_update_fde")
+            return out.as_dict(len(items))
         out = AidResult()
         self._chk(self._f("aid_stack_update")(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)), "aid_stack_update")
         return out.as_dict()

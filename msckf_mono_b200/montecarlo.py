@@ -528,7 +528,27 @@ def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_
     for key, rows in (("gnss", gnss_rows), ("range", range_rows)):
         if rows is not None:
             rec[key] = {k: [float(r[k]) if k == "nis" else int(r[k]) for r in rows] for k in ("nis", "dof", "applied", "status")}
+            rec[key].update(_fault_counts(rows))
     return rec
+
+
+def _fault_counts(rows):
+    """the injected faults of a trial's stacks (each row's "faults": the item indices made faulty) and what became of them: with
+    FDE item states (row "items"), faults excluded, clean items excluded, faults missed (used in an applied stack), stacks
+    rejected (outcome 2 or 3); without, a fault in an applied stack is missed and a stack not applied is rejected"""
+    c = {"injected": 0, "faults_excluded": 0, "clean_excluded": 0, "faults_missed": 0, "stacks_rejected": 0}
+    for r in rows:
+        faults = set(r.get("faults", ()))
+        c["injected"] += len(faults)
+        if "items" in r:
+            for j, it in enumerate(r["items"]):
+                c["faults_excluded" if j in faults else "clean_excluded"] += it["state"] == 1
+                c["faults_missed"] += j in faults and it["state"] == 0
+            c["stacks_rejected"] += r["outcome"] in (2, 3)
+        elif r["dof"] > 0:
+            c["faults_missed"] += len(faults) if r["applied"] else 0
+            c["stacks_rejected"] += r["status"] == 0 and not r["applied"]
+    return c
 
 
 def _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows):
@@ -620,7 +640,9 @@ def summarize(records):
         if not all(g is not None and len(g["nis"]) for g in gn):
             continue
         V = np.array([g["nis"] for g in gn]); D = np.array([g["dof"] for g in gn])
-        used = (D > 0) & np.isfinite(V)  # (a dropped epoch, or status 1 / 2: no NIS)
+        A = np.array([g["applied"] for g in gn])
+        fused = (D > 0) & np.isfinite(V)  # (a dropped epoch, or status 1 / 2: no NIS)
+        used = fused & (A > 0)  # (a stack the gate or FDE rejected is not in the ANIS)
         V, D = np.where(used, V, 0.0), np.where(used, D, 0)
         n_used, dof = used.sum(axis=0), D.sum(axis=0)
         keep = n_used > 0
@@ -630,8 +652,10 @@ def summarize(records):
                     "mean_anis": float(V.sum() / max(used.sum(), 1)), "mean_dof": float(D.sum() / max(used.sum(), 1)),
                     "run_bounds": list(chi2_bounds(int(D.sum()), int(used.sum()))) if used.any() else [float("nan")] * 2,
                     "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])) if keep.any() else float("nan"),
-                    "applied": float(np.mean([a for g, u in zip(gn, used) for a, x in zip(g["applied"], u) if x])) if used.any() else 0.0,
-                    "degenerate": int(sum(s == 2 for g in gn for s in g["status"]))}
+                    "applied": float(A[fused].mean()) if fused.any() else 0.0,
+                    "degenerate": int(sum(s == 2 for g in gn for s in g["status"])),
+                    **{c: int(sum(g.get(c, 0) for g in gn)) for c in ("injected", "faults_excluded", "clean_excluded", "faults_missed",
+                                                                      "stacks_rejected")}}
     return out
 
 
@@ -654,11 +678,12 @@ def map_call(tr, f, fi, uncertain, S):
     return ids, inv, z, p[first], np.repeat(S, len(u), axis=0)
 
 
-def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items):
+def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items, faults=None, fde=None):
     """one batched stack per filter of the epoch g = f - delay when a trial input of `keys` (two noise lists of make_trial) has
     noise there: items(g, noise of keys[0], noise of keys[1], clone) with clone None at delay 0, else the window position of
-    the epoch's clone; a filter whose epoch clone has left the window sends nothing and records dof 0.  Appends each filter's
-    result to out[i]."""
+    the epoch's clone; a filter whose epoch clone has left the window sends nothing and records dof 0.  faults(i, g, items), when
+    given, makes some of filter i's items faulty in place and returns their indices (kept as the row's "faults"); fde, when
+    given, sends the stacks through fault detection and exclusion.  Appends each filter's result to out[i]."""
     noise = [tuple(tr[key][g] if key in tr else None for key in keys) for tr in trs] if g >= 0 else []
     if g < 0 or not any(x is not None for x in noise[0]):
         return
@@ -672,8 +697,9 @@ def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items):
                 continue
             clone = ids.index(tr["frames"][g]["state_id"])
         stacks.append(items(g, n_a, n_b, clone))
-    for i, r in enumerate(fb.aid_stack_update(stacks)):
-        out[i].append({"nis": 0.0, "dof": 0, "applied": 0, "status": 0} if r is None else r)
+    bad = [faults(i, g, s) if faults is not None and s is not None else [] for i, s in enumerate(stacks)]
+    for i, r in enumerate(fb.aid_stack_update(stacks) if fde is None else fb.aid_stack_update(stacks, fde=fde)):
+        out[i].append({"nis": 0.0, "dof": 0, "applied": 0, "status": 0} if r is None else dict(r, faults=bad[i]))
 
 
 def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, map_chi2=0.0,
@@ -681,7 +707,8 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         map_uncertain=False, map_clones=1, gnss_every=0, gnss_sigma=0.1, gnss_lever=(0.0, 0.0, 0.0), gnss_delay=0,
         gnss_as_position=False, heading_every=0, heading_sigma=0.01, heading_axis=(1.0, 0.0, 0.0), range_every=0, range_sigma=0.1,
         range_lever=(0.0, 0.0, 0.0), range_delay=0, plane_every=0, plane_sigma=0.02, plane_height=PLANE_HEIGHT, plane_axis=PLANE_AXIS,
-        plane_lever=(0.0, 0.0, 0.0)):
+        plane_lever=(0.0, 0.0, 0.0), range_outlier_rate=0.0, range_outlier_bias=1.0, gnss_outlier_rate=0.0, gnss_outlier_jump=5.0,
+        fde_alpha=0.0, fde_max_exclude=2):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
@@ -691,7 +718,11 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     [one batched ranging stack (range_items) in a frame whose epoch f - range_delay has anchor ranges (every range_every frames,
     antenna at range_lever in the IMU frame, standard deviation range_sigma) or a plane range (every plane_every frames, along
     plane_axis from plane_lever to the plane z = plane_height, standard deviation plane_sigma); at the IMU or the epoch's clone
-    as for GNSS],
+    as for GNSS; each anchor range made range_outlier_bias m long (NLOS) with probability range_outlier_rate, drawn from the
+    stream default_rng([seed, k, 10]) per frame, and each antenna fix moved gnss_outlier_jump m horizontally in a random
+    direction with probability gnss_outlier_rate, from [seed, k, 11]; fde_alpha > 0 sends the GNSS and ranging stacks through
+    fault detection and exclusion with thresholds capi.fde_thresholds(fde_alpha) and fde_max_exclude (0: the stack gate only),
+    fde_alpha = 0 fuses them ungated],
     [every map_every frames from frame map_start on, one batched mapped-landmark update from the newest clone, gated per
     observation at map_chi2 > 0, iterated up to map_iterations linearisations; the map carries N(0, map_sigma^2 I) errors and
     is observed from the map_clones newest clones that are still in the window (make_trial); map_uncertain passes
@@ -711,6 +742,41 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     ranging = [[] for _ in trs] if range_every > 0 or plane_every > 0 else None
     lever, axis = np.asarray(gnss_lever, dtype=np.float64), np.asarray(heading_axis, dtype=np.float64)
     r_lever, p_lever, p_axis = (np.asarray(v, dtype=np.float64) for v in (range_lever, plane_lever, plane_axis))
+    n_fr = len(truth["frames"])
+    # NLOS ranges (flags per frame and anchor) and GNSS jumps (flag and direction per frame) of each trial; no draws when off
+    r_out = [np.random.default_rng([seed, tr["k"], 10]).random((n_fr, len(ANCHORS))) < range_outlier_rate if range_outlier_rate > 0
+             else None for tr in trs]
+    g_out = []
+    for tr in trs:
+        if gnss_outlier_rate > 0:
+            rg = np.random.default_rng([seed, tr["k"], 11])
+            g_out.append((rg.random(n_fr) < gnss_outlier_rate, rg.uniform(0.0, 2.0 * np.pi, n_fr)))
+        else:
+            g_out.append(None)
+
+    def range_faults(i, g, items):
+        if r_out[i] is None or not items or items[0]["model"] not in (AID_RANGE, AID_CLONE_RANGE):
+            return []
+        bad = [j for j in range(len(ANCHORS)) if r_out[i][g, j]]
+        for j in bad:
+            items[j]["z"] = np.r_[items[j]["z"][0] + range_outlier_bias, items[j]["z"][1:]]
+        return bad
+
+    def gnss_faults(i, g, items):
+        if g_out[i] is None or not items or items[0]["model"] not in (AID_ANTENNA_POSITION, AID_CLONE_ANTENNA_POSITION, AID_POSITION):
+            return []
+        flag, ang = g_out[i]
+        if not flag[g]:
+            return []
+        z = np.array(items[0]["z"], dtype=np.float64)
+        z[0:2] += gnss_outlier_jump * np.array([np.cos(ang[g]), np.sin(ang[g])])
+        items[0]["z"] = z
+        return [0]
+
+    fde = None
+    if fde_alpha > 0:
+        from .capi import fde_thresholds
+        fde = {"chi2": fde_thresholds(fde_alpha), "max_exclude": int(fde_max_exclude)}
     S_map = np.tile([map_sigma ** 2, 0.0, map_sigma ** 2, 0.0, 0.0, map_sigma ** 2], (1, 1))
     first = [None for _ in trs]
     R_fix = (fix_sigma ** 2) * np.eye(3)
@@ -752,11 +818,13 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         if gnss is not None:  # the epoch whose GNSS output arrives at this frame
             _epoch_stacks(fb, fs, trs, fi - gnss_delay, gnss_delay, ("gnss", "heading"), gnss,
                           lambda g, n_p, n_psi, clone: gnss_items(truth["truth_imu"][g], truth["camera"], n_p, n_psi, gnss_sigma, lever,
-                                                                  heading_sigma, axis, clone, gnss_as_position))
+                                                                  heading_sigma, axis, clone, gnss_as_position),
+                          gnss_faults if gnss_outlier_rate > 0 else None, fde)
         if ranging is not None:  # the epoch whose ranges arrive at this frame
             _epoch_stacks(fb, fs, trs, fi - range_delay, range_delay, ("range", "plane"), ranging,
                           lambda g, n_r, n_h, clone: range_items(truth["truth_imu"][g], truth["camera"], n_r, n_h, range_sigma, r_lever,
-                                                                 plane_sigma, plane_height, p_lever, p_axis, clone))
+                                                                 plane_sigma, plane_height, p_lever, p_axis, clone),
+                          range_faults if range_outlier_rate > 0 else None, fde)
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [map_call(tr, f, fi, map_uncertain, S_map) for tr, f in zip(trs, fs)]
             if first[0] is None:

@@ -34,6 +34,13 @@ along --plane-axis X Y Z from --plane-lever X Y Z (both in the IMU frame) to the
 --plane-sigma m as PLANE_RANGE; a frame's ranges and plane range go in one stacked update.  --range-delay D fuses the epoch of
 frame f - D at frame f, at that epoch's clone.  The summary adds the ranging stacks' ANIS against its 95 % chi^2 bounds.
 
+--range-outlier-rate P --range-outlier-bias B makes each anchor range B m long (NLOS) with probability P; --gnss-outlier-rate P
+--gnss-outlier-jump D moves each antenna fix D m horizontally in a random direction with probability P.  --fde-alpha A > 0 sends
+the GNSS and ranging stacks through fault detection and exclusion (thresholds: the chi^2 quantiles 1 - A) with at most
+--fde-max-exclude K items excluded (K = 0: the stack gate only); A = 0 fuses them ungated.  The GNSS and ranging summaries add
+the injected faults, faults excluded, clean items excluded, faults missed and stacks rejected; their ANIS is over the stacks
+applied.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -49,6 +56,8 @@ import numpy as np
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from msckf_mono_b200 import capi, montecarlo as mc, shard, synth  # noqa: E402
+
+FAULTS = ("injected", "faults_excluded", "clean_excluded", "faults_missed", "stacks_rejected")
 
 
 def gpu_line():
@@ -171,6 +180,12 @@ def main():
     ap.add_argument("--plane-height", type=float, default=mc.PLANE_HEIGHT)
     ap.add_argument("--plane-axis", type=float, nargs=3, default=list(mc.PLANE_AXIS), metavar=("X", "Y", "Z"))
     ap.add_argument("--plane-lever", type=float, nargs=3, default=[0.0, 0.0, 0.0], metavar=("X", "Y", "Z"))
+    ap.add_argument("--range-outlier-rate", type=float, default=0.0)
+    ap.add_argument("--range-outlier-bias", type=float, default=1.0)
+    ap.add_argument("--gnss-outlier-rate", type=float, default=0.0)
+    ap.add_argument("--gnss-outlier-jump", type=float, default=5.0)
+    ap.add_argument("--fde-alpha", type=float, default=0.0, help="> 0: fault detection and exclusion in the GNSS and ranging stacks")
+    ap.add_argument("--fde-max-exclude", type=int, default=2)
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -194,7 +209,9 @@ def main():
                         heading_every=args.heading_every, heading_sigma=args.heading_sigma, range_every=args.range_every,
                         range_sigma=args.range_sigma, range_lever=args.range_lever, range_delay=args.range_delay,
                         plane_every=args.plane_every, plane_sigma=args.plane_sigma, plane_height=args.plane_height,
-                        plane_axis=args.plane_axis, plane_lever=args.plane_lever)
+                        plane_axis=args.plane_axis, plane_lever=args.plane_lever, range_outlier_rate=args.range_outlier_rate,
+                        range_outlier_bias=args.range_outlier_bias, gnss_outlier_rate=args.gnss_outlier_rate,
+                        gnss_outlier_jump=args.gnss_outlier_jump, fde_alpha=args.fde_alpha, fde_max_exclude=args.fde_max_exclude)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -216,12 +233,16 @@ def main():
     if "gnss" in s:
         res["gnss"] = {"every": args.gnss_every, "sigma_m": args.gnss_sigma, "lever_m": args.gnss_lever, "delay": args.gnss_delay,
                        "as_position": args.gnss_as_position, "heading_every": args.heading_every, "heading_sigma": args.heading_sigma,
-                       **{k: s["gnss"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate")}}
+                       **{k: s["gnss"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate") + FAULTS}}
     if "range" in s:
         res["range"] = {"every": args.range_every, "sigma_m": args.range_sigma, "lever_m": args.range_lever, "delay": args.range_delay,
                         "plane_every": args.plane_every, "plane_sigma_m": args.plane_sigma, "plane_height_m": args.plane_height,
                         "plane_axis": args.plane_axis, "plane_lever_m": args.plane_lever,
-                        **{k: s["range"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate")}}
+                        **{k: s["range"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate") + FAULTS}}
+    if args.fde_alpha > 0 or args.range_outlier_rate > 0 or args.gnss_outlier_rate > 0:
+        res["faults"] = {"range_outlier_rate": args.range_outlier_rate, "range_outlier_bias_m": args.range_outlier_bias,
+                         "gnss_outlier_rate": args.gnss_outlier_rate, "gnss_outlier_jump_m": args.gnss_outlier_jump,
+                         "fde_alpha": args.fde_alpha, "fde_max_exclude": args.fde_max_exclude}
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
