@@ -45,6 +45,9 @@ constexpr int kMaxSplit = 16;
 constexpr int kJacBatchGroup = 32;  // k_jac threads per track in a device batch (DESIGN.md 4.2)
 constexpr int kTailCluster = 8;  // portable cluster size: the serial EKF tail runs on 8 SMs of one GPC
 constexpr size_t kSmemBudget = 220 * 1024;  // dynamic shared memory per CTA, under H100's 227 KB opt-in limit
+// k_aid: W^T and dx in dynamic shared memory up to this many bytes, else in the global workspace (both forms of the kernel;
+// with the FDE form's static shared memory this passes the default 48 KB per CTA, so set_func_attrs raises the limit)
+constexpr size_t kAidSmemMax = 32 * 1024;
 constexpr int kMaxClonesHard = mb::kMaxKeep;  // the keep list of prune() travels as a kernel argument
 constexpr int kMaxGraphs = 8;
 
@@ -594,6 +597,10 @@ struct Engine : EngineBase {
     cudaGetLastError();
     CK(cudaFuncSetAttribute(mb::k_tail<S, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     CK(cudaFuncSetAttribute(mb::k_tail<S, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+    CK(cudaFuncSetAttribute(mb::k_aid<S, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid<S, mb::kBatchMembers>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid<S, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid<S, mb::kBatchMembers, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
     done[dev] = true;
     return 0;
   }
@@ -1526,7 +1533,6 @@ static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && 
                   (int)MSCKF_B200_AID_PLANE_RANGE == (int)mb::kAidPlaneRange &&
                   (int)MSCKF_B200_AID_CLONE_PLANE_RANGE == (int)mb::kAidClonePlaneRange,
               "msckf_b200_aid_model and mb::AidModel differ");
-constexpr size_t kAidSmemMax = 32 * 1024;
 template <class S>
 int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "aid_update: null argument");

@@ -1,6 +1,7 @@
 """Dense numpy fault detection and exclusion over the items of a stacked aided update (the rounds of
 msckf_b200_aid_stack_update_fde, include/msckf_b200.h), in fp64, built on montecarlo.odometry_residual / odometry_jacobian,
-with the Joseph-form update of the kept items."""
+with the Joseph-form update of the kept items, and the scenes the tests draw: stacks of side_shapes recipes with faults of a
+chosen size."""
 import numpy as np
 from scipy.linalg import block_diag
 
@@ -8,8 +9,10 @@ from msckf_mono_b200 import montecarlo as mc
 
 
 def linearise(items, imu, poses, n):
-    """[(H_j [d_j, n], r_j [d_j])] of the items at the state"""
-    return [(mc.odometry_jacobian(it, imu, poses, n), mc.odometry_residual(it, imu, poses)) for it in items]
+    """[(H_j [d_j, n], r_j [d_j])] of the items at the state (the models of montecarlo; VELOCITY, POSITION, POSE and CLONE_POSE
+    as test_odometry_gpu.H_r)"""
+    from tests.test_range_gpu import H_r
+    return [H_r(it, imu, poses, n) for it in items]
 
 
 def set_nis(S, r, rows):
@@ -120,3 +123,63 @@ def range_scene(rng, imu, poses, n_ranges=4, sigma=0.1, faults=(), bias=2.0, gns
         items.append({"model": mc.AID_CLONE_RANGE, "a": clone, "b": 0,
                       "z": np.r_[mc.range_of(pc, qc, lever, anchor) + sigma * rng.normal(), anchor, lever], "R": np.array([[sigma ** 2]])})
     return items
+
+
+def recipe_items(rng, recipe, imu, poses, M):
+    """the items of a recipe of tests/side_shapes.py ((model, rows, clone), clone -1: M - 1) near their predictions"""
+    from msckf_mono_b200 import capi
+    from tests.side_shapes import FDE_MASK
+    from tests.test_aid_gpu import make_spec
+    from tests.test_gnss_gpu import antenna_item
+    from tests.test_odometry_gpu import body_item, rel_item
+    from tests.test_range_gpu import plane_item, range_item
+    items = []
+    for model, rows, clone in recipe:
+        k = None if clone is None else (M - 1 if clone == -1 else clone)
+        if model in ("RANGE", "CLONE_RANGE"):
+            it = range_item(rng, imu, poses, clone=k)
+        elif model in ("PLANE_RANGE", "CLONE_PLANE_RANGE"):
+            it = plane_item(rng, imu, poses, clone=k)
+        elif model in ("ANTENNA_POSITION", "CLONE_ANTENNA_POSITION"):
+            it = antenna_item(rng, imu, poses, FDE_MASK[rows], clone=k)
+        elif model == "BODY_VELOCITY":
+            it = body_item(rng, imu, FDE_MASK[rows])
+        elif model == "RELATIVE_POSE":
+            it = rel_item(rng, poses, 0, M - 1)
+        else:  # POSE, CLONE_POSE
+            it = dict(make_spec(rng, getattr(capi, "AID_" + model), imu, poses, 15 + 6 * M, k or 0)[0])
+            it["a"] = it.pop("clone")
+        assert len(it["R"]) == rows and it["model"] == getattr(capi, "AID_" + model), (model, rows)
+        items.append(it)
+    return items
+
+
+def fault_rows(item):
+    """(indices into z, rows of r) that a fault moves (r = z - h(x) on them): a range, an antenna fix's or a body velocity's
+    masked coordinates, a pose's or a relative pose's position"""
+    m = item["model"]
+    if m in mc.RANGE_MODELS:
+        return [0], [0]
+    mask = {mc.AID_ANTENNA_POSITION: item.get("a"), mc.AID_CLONE_ANTENNA_POSITION: item.get("b"), mc.AID_BODY_VELOCITY: item.get("a")}
+    if m in mask:
+        rows = [j for j in range(3) if (mask[m] >> j) & 1]
+        return rows, list(range(len(rows)))
+    assert len(item["R"]) == 6, m  # POSE, CLONE_POSE, RELATIVE_POSE: r = [dtheta, z_p - p]
+    return [0, 1, 2], [3, 4, 5]
+
+
+def with_faults(rng, items, faults, ratios, imu, poses, P, chi2):
+    """copies of the items with item faults[i] moved along a random direction of its fault rows by b, where b^2 e^T S_jj^-1 e =
+    ratios[i] chi2[d_j - 1] (e the unit move in r, S_jj = H_j P H_j^T + R_j): the fault alone is that many thresholds"""
+    out = [dict(it, z=np.array(it["z"], dtype=np.float64)) for it in items]
+    for j, ratio in zip(faults, ratios):
+        H, _ = linearise([out[j]], imu, poses, P.shape[0])[0]
+        S = H @ P @ H.T + out[j]["R"]
+        zi, ri = fault_rows(out[j])
+        u = rng.normal(size=len(zi))
+        u /= np.linalg.norm(u)
+        e = np.zeros(len(S))
+        e[ri] = u
+        b = np.sqrt(ratio * chi2[len(S) - 1] / (e @ np.linalg.solve(S, e)))
+        out[j]["z"][zi] += b * u
+    return out

@@ -1,6 +1,6 @@
-"""The shapes the side-update kernels (k_aid, k_nees, k_lmk_*) dispatch on, as the host decides them, the grid of
-tests/test_side_shapes_gpu.py that reaches both sides of each decision and every cap, and the information-form update for
-stacked systems too large for the dense Joseph form.
+"""The shapes the side-update kernels (k_aid, k_nees, k_lmk_*) dispatch on, as the host decides them, the grids of
+tests/test_side_shapes_gpu.py and tests/test_aid_fde_shapes_gpu.py that reach both sides of each decision and every cap, and
+the information-form update for stacked systems too large for the dense Joseph form.
 
 The constants are read from the CUDA sources (`parse_constants`) and checked against `MIRROR` by
 tests/test_side_shapes_cpu.py: a threshold moved in the code fails there instead of leaving the grid on one side of it."""
@@ -95,6 +95,105 @@ def aid_cases():
 
 # a device batch of 33 LINEAR members (two launch chunks), chunk 0 mixing shared and global members of different m
 AID_BATCH = [((18, 19, 37, 38, 65, 66, 95, 96, 168, 169, 0)[i % 11], (31, 32, 16, 9, 6, 3, 1)[i % 7]) for i in range(33)]
+
+# ---- k_aid's launch: its static shared memory per form (-Xptxas -v, sm_90a, both dtypes, NM = 1 and 32; cuobjdump's SHARED is
+# 1 KB more, sm_90's reservation) plus the dynamic bytes above.  A launch past the default 48 KB per CTA needs the kernel's
+# raised dynamic limit: AID_OPT_IN lists those shapes (today FDE launches only, the plain form's 13 792 B leave 35 360 B)
+AID_STATIC_SMEM = {"plain": 13792, "fde": 16976}
+AID_DEFAULT_SMEM = 48 * 1024
+
+
+def aid_launch_smem(M, m, fde):
+    return AID_STATIC_SMEM["fde" if fde else "plain"] + aid_dynamic_smem(M, m)
+
+
+AID_OPT_IN = [(18, 32), (20, 29), (21, 28), (27, 22), (28, 21), (30, 20), (33, 18), (35, 17), (37, 16), (40, 15), (43, 14),
+              (46, 13), (50, 12), (54, 11), (59, 10), (65, 9), (72, 8), (73, 8), (82, 7), (94, 6), (95, 6), (110, 5), (111, 5),
+              (132, 4), (133, 4), (134, 4), (166, 3), (167, 3), (168, 3)]
+
+
+def aid_opt_in():
+    """(M, m) of every window and row count whose k_aid launch, in either form, takes more than the default 48 KB"""
+    return [(M, m) for M in range(K["kMaxKeep"] + 1) for m in range(1, K["kAidMaxRows"] + 1)
+            if max(aid_launch_smem(M, m, f) for f in (False, True)) > AID_DEFAULT_SMEM]
+
+
+# ---- k_aid<S, NM, true>: fault detection and exclusion over the items of a stack.  Recipes as AID_STACKS, (model, rows, clone),
+# with exactly m rows in at most 8 items; ANTENNA_POSITION and BODY_VELOCITY take the mask of their rows (FDE_MASK).  The four
+# range models sit on both storage sides, their clone forms at clone M - 1 and at clone 0; window 192's stacks put both at clone
+# 191.  m = 32 fills all 8 warps of an exclusion round, with 6-row items (s_blk: 36 + 6 doubles per warp).  Items of equal
+# rows observe different parts of the state where they can (a clone >= 0 is that clone): a fault that two such items explain
+# alike is a tie of the exclusion test, not a check of it.
+FDE_MASK = {1: 0b100, 2: 0b101, 3: 0b111}
+_FDE_32 = [("CLONE_POSE", 6, -1), ("CLONE_POSE", 6, 5), ("POSE", 6, None), ("CLONE_POSE", 6, 0),
+           ("CLONE_ANTENNA_POSITION", 3, 9), ("BODY_VELOCITY", 3, None)]
+FDE_STACKS = {
+    1: [("CLONE_RANGE", 1, -1)],
+    3: [("RANGE", 1, None), ("PLANE_RANGE", 1, None), ("CLONE_RANGE", 1, 0)],
+    6: [("CLONE_PLANE_RANGE", 1, -1), ("PLANE_RANGE", 1, None), ("CLONE_RANGE", 1, 0), ("RANGE", 1, None), ("BODY_VELOCITY", 2, None)],
+    9: [("CLONE_RANGE", 1, -1), ("RELATIVE_POSE", 6, None), ("ANTENNA_POSITION", 2, None)],
+    16: [("CLONE_POSE", 6, -1), ("RANGE", 1, None), ("RELATIVE_POSE", 6, None), ("CLONE_PLANE_RANGE", 1, 0), ("BODY_VELOCITY", 2, None)],
+    31: [("POSE", 6, None), ("CLONE_POSE", 6, 5), ("CLONE_POSE", 6, 0), ("CLONE_POSE", 6, -1), ("CLONE_ANTENNA_POSITION", 3, 9),
+         ("ANTENNA_POSITION", 2, None), ("PLANE_RANGE", 1, None), ("CLONE_RANGE", 1, -1)],
+    32: _FDE_32 + [("RANGE", 1, None), ("CLONE_PLANE_RANGE", 1, 0)],
+}
+FDE_STACKS_AT = {  # the end windows' stacks where they differ from FDE_STACKS, and windows of 0 and 1 clones
+    (191, 1): [("CLONE_PLANE_RANGE", 1, -1)],
+    (191, 32): _FDE_32 + [("CLONE_RANGE", 1, -1), ("CLONE_PLANE_RANGE", 1, -1)],
+    (192, 32): _FDE_32 + [("CLONE_RANGE", 1, -1), ("CLONE_PLANE_RANGE", 1, -1)],
+    (0, 1): [("RANGE", 1, None)],
+    (0, 32): [("POSE", 6, None)] * 4 + [("ANTENNA_POSITION", 3, None), ("PLANE_RANGE", 1, None), ("BODY_VELOCITY", 3, None),
+                                        ("RANGE", 1, None)],
+    (1, 1): [("CLONE_PLANE_RANGE", 1, -1)],
+    (1, 32): [("CLONE_POSE", 6, -1), ("POSE", 6, None), ("CLONE_POSE", 6, -1), ("POSE", 6, None), ("CLONE_ANTENNA_POSITION", 3, -1),
+              ("BODY_VELOCITY", 3, None), ("CLONE_RANGE", 1, -1), ("PLANE_RANGE", 1, None)],
+}
+FDE_DEPTH_WINDOWS = AID_EDGES[32]  # the exclusion depth at m = 32, one window on each storage side
+# 8 items on separate parts of the state (a fault in one moves no other item's test much): faults of strictly decreasing size
+# in the first k leave in that order, and at k = 7 one item is left
+FDE_DEPTH = [("CLONE_POSE", 6, 0), ("CLONE_POSE", 6, -1), ("POSE", 6, None), ("CLONE_POSE", 6, 9), ("CLONE_ANTENNA_POSITION", 3, 5),
+             ("CLONE_ANTENNA_POSITION", 3, 14), ("CLONE_RANGE", 1, 12), ("CLONE_PLANE_RANGE", 1, 3)]
+FDE_DEPTH_RATIOS = [300.0 / 2 ** i for i in range(8)]  # each fault alone, in thresholds chi2[d_j - 1] of its item
+FDE_SPREAD_RATIO = 0.75  # every item this far off: the stack fails, no single item explains it (outcome 3, all 8 in A)
+FDE_BATCH_OPT_IN = [(e[0], m) for m, e in AID_EDGES.items() if (e[0], m) in AID_OPT_IN]  # AID_EDGES' last shared windows among them
+# the shapes of a 33-member FDE batch, in turn: chunk 0 mixes them with other shapes of both storage paths
+FDE_BATCH = FDE_BATCH_OPT_IN + [(20, 29), (133, 4), (0, 32), (1, 32), (192, 1), (18, 31), (19, 32), (38, 16), (96, 6), (169, 3)]
+
+
+def fde_fill(M, m):
+    """m rows in at most 8 items at a window of M >= 11 clones: a range at the IMU and one at the last clone, clone poses at
+    clones 0, 2, .. 8, then a masked antenna fix and body velocity for the rest"""
+    out = [("RANGE", 1, None), ("CLONE_RANGE", 1, -1)][:m]
+    left = m - len(out)
+    while left >= 6:
+        out.append(("CLONE_POSE", 6, 2 * (len(out) - 2)))
+        left -= 6
+    if left > 3:
+        out.append(("ANTENNA_POSITION", 3, None))
+        left -= 3
+    if left:
+        out.append(("BODY_VELOCITY", left, None))
+    return out
+
+
+def fde_stack(M, m):
+    if (M, m) in FDE_STACKS_AT:
+        return FDE_STACKS_AT[(M, m)]
+    return FDE_STACKS[m] if m in FDE_STACKS and M >= 2 else fde_fill(M, m)
+
+
+def fde_faults(recipe):
+    """[(name, faulty items, max_exclude)] of a recipe: none; the last item (warp 7 at 8 items); the first 6-row item; two items
+    apart (the kept rows gathered around a hole) with max_exclude 2 and 1"""
+    k = len(recipe)
+    out = [("none", (), 2), ("last", (k - 1,), 1)]
+    six = [i for i, (_, rows, _) in enumerate(recipe) if rows == 6 and i != k - 1]
+    if six:
+        out.append(("six", (six[0],), 1))
+    if k >= 3:
+        pair = (1, k - 1) if k >= 4 else (0, 2)
+        out += [("pair", pair, 2), ("pair", pair, 1)]
+    return out
 
 # ---- k_nees: one CTA factors the (n + 1) x n bordered matrix in panels of 32
 NEES_WINDOWS = (19, 24, 41, 95, 136, 191, 192)  # n mod 32 = 1, 31, 5, 9, 31, 9, 15

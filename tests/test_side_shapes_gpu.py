@@ -2,7 +2,8 @@
 and fp32, against dense fp64 references on the engine's fetched state:
   * k_aid: each row count 1 .. 32 at its last window with W^T and dx in shared memory and its first with them in the global
     workspace, as one LINEAR call and one stack of model items; windows 0, 1, 191, 192; the chi2 gate 1e-6 either side of the
-    NIS on both paths; a 33-member device batch whose first launch chunk mixes both paths;
+    NIS on both paths; a 33-member device batch whose first launch chunk mixes both paths; the shared memory of each path's
+    launch in a profiler trace, plain and FDE (its launch past the default 48 KB);
   * k_nees: windows of 19 .. 192 clones (1 .. 37 panels of the factor), with and without truth poses, a 33-member batch, and a
     first bad pivot past the first panel;
   * k_lmk_*: exact-map rows 30 .. 1152 across the panel edges of k_lmk_gain's factor and k_lmk_downdate's loop, windows 91 ..
@@ -20,7 +21,7 @@ import numpy as np
 import pytest
 
 from msckf_mono_b200 import capi, montecarlo as mc
-from tests import landmark_map_reference as mref, side_shapes as ss
+from tests import aid_fde_reference as fde_ref, landmark_map_reference as mref, side_shapes as ss
 from tests.landmark_iter_reference import iekf
 from tests.test_aid_gpu import assert_unchanged, call, make_spec, numpy_update, snapshot, state_of
 from tests.test_batch_stream_gpu import Member
@@ -199,6 +200,39 @@ def test_aid_launch_shared_memory_follows_the_storage_path():
             smem.append(int(ev[0]["args"]["shared memory"]))
     assert ss.aid_global(M1, 3) and not ss.aid_global(M0, 3)
     assert smem[0] - smem[1] == ss.aid_dynamic_smem(M0, 3) == ss.aid_ws_bytes(ss.n_of(M0), 3), smem
+
+
+def test_aid_fde_launch_shared_memory_past_the_default_limit():
+    """the same for k_aid<S, 1, true> at the same two windows (m = 3 at window 168 is one of ss.AID_OPT_IN): the shared-side
+    launch carries aid_ws_bytes(n, 3) more, and where the trace counts static shared memory, it is over the default 48 KB"""
+    torch = pytest.importorskip("torch")
+    from torch.profiler import ProfilerActivity, profile
+    M0, M1 = ss.AID_EDGES[3]
+    assert (M0, 3) in ss.AID_OPT_IN
+    rng = np.random.default_rng(76)
+    chi2 = capi.fde_thresholds(0.01)
+    torch.cuda.init()
+    smem = []
+    with tempfile.TemporaryDirectory() as tmp:
+        for M in (M0, M1):
+            b = fresh(np.float64, M)
+            imu, poses = state_of(b.e)
+            items = fde_ref.recipe_items(rng, ss.fde_stack(M, 3), imu, poses, M)
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                got = b.e.aid_stack_update(items, fde={"chi2": chi2, "max_exclude": 1})
+            assert got["applied"] == 1
+            path = os.path.join(tmp, "trace.json")
+            prof.export_chrome_trace(path)
+            with open(path) as fh:
+                ev = [e for e in json.load(fh).get("traceEvents", []) if "k_aid" in str(e.get("name", ""))]
+            if not ev or "shared memory" not in ev[0].get("args", {}):
+                pytest.skip("the profiler trace carries no k_aid launch with its shared memory")
+            smem.append(int(ev[0]["args"]["shared memory"]))
+    print(f"k_aid FDE launch shared memory: window {M0} {smem[0]} B, window {M1} {smem[1]} B")
+    assert ss.aid_global(M1, 3) and not ss.aid_global(M0, 3)
+    assert smem[0] - smem[1] == ss.aid_ws_bytes(ss.n_of(M0), 3), smem
+    if smem[1] >= ss.AID_STATIC_SMEM["fde"]:
+        assert smem[0] > ss.AID_DEFAULT_SMEM, smem
 
 
 # ---- k_nees ------------------------------------------------------------------------------------------------------------
