@@ -1,16 +1,18 @@
 // msckf_mono_b200/csrc/aid_kernels.cuh
-// Aided measurements fused into the device-resident filter (msckf_b200_aid_update / _batch_aid_update and the stacked
-// msckf_b200_aid_stack_update / _batch_aid_stack_update):
-//   k_aid : residual r and H (a stack of up to 8 model items, each row at most 12 (state index, coefficient) pairs formed from
-//           the resident state; or the caller's r and dense H; a degenerate heading or range item ends the member: status 2), H P (sparse gathers over rows of P, or a product for a dense H),
-//           S = H P H^T + R = L L^T with r as an extra row (y = L^-1 r), W = L^-1 H P, NIS = y^T y, the optional chi-square
-//           gate, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to the filter precision
-//           once) and the state injection of k_syrk (inject_state).  All arithmetic in fp64.
-//   k_aid<S, NM, true> (msckf_b200_aid_stack_update_fde): the same kernel with fault detection and exclusion over the stack's
-//           items.  A degenerate item is dropped instead of ending the member; rounds over the kept set A rebuild S_AA from
-//           H P (kept in Wt until the update) and R, factor it, gate NIS_A on chi2[d_A - 1] and, while it fails, exclude the
-//           item with the largest t_j / chi2[d_j - 1] (t_j = y_j^T B_j^-1 y_j, y = S_AA^-1 r, B_j = (S_AA^-1)_jj; one warp per
-//           item).  The update of the final A runs the arithmetic of the plain kernel on those rows, in their order.
+// Aided measurements fused into the device-resident filter (msckf_b200_aid_update / _batch_aid_update, the stacked
+// msckf_b200_aid_stack_update / _batch_aid_stack_update and their fault detection and exclusion, _fde).  k_aid<S, NM, FDE>,
+// one body for both forms:
+//   rows   residual r and H (a stack of up to 8 model items, each row at most 12 (state index, coefficient) pairs formed from
+//          the resident state; or the caller's r and dense H).  A degenerate heading or range item ends a plain member
+//          (status 2); the FDE form drops it from the kept set A.
+//   H P    sparse gathers over rows of P, or a product for a dense H; kept in Wt until the update.
+//   rounds S_AA = (H P H^T + R)_AA = L L^T with r_A as an extra row (y = L^-1 r_A), NIS = y^T y and the gate.  Plain: one
+//          round over every row, gated on the optional chi2_max.  FDE: gated on chi2[d_A - 1]; while it fails, an exclusion
+//          round removes the item with the largest t_j / chi2[d_j - 1] (t_j = y_j^T B_j^-1 y_j, y = S_AA^-1 r,
+//          B_j = (S_AA^-1)_jj; one warp per item), and the next round rebuilds S_AA.
+//   update W = L^-1 H P over A's rows, dx = W^T y, P <- P - W^T W (lower triangle in fp64, both halves written, rounded to the
+//          filter precision once) and the state injection of k_syrk (inject_state).
+// All arithmetic in fp64; the FDE form's update of the final A is the plain arithmetic on those rows, in their order.
 // One CTA per member, one launch for everything; one body for a single filter (NM = 1) and a device batch (NM =
 // kBatchMembers), like k_nees.  W^T and dx live in dynamic shared memory where they fit, else in a per-member global workspace.
 #pragma once
@@ -274,6 +276,12 @@ __device__ __noinline__ int aid_item_rows(const AidItem it, const double* z, con
   return 0;
 }
 
+// The member's result when nothing is written: NIS NaN, no step, not applied
+__device__ __forceinline__ void aid_nothing(AidOut* out, int dof, int status) {
+  out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
+  out->dof = dof; out->applied = 0; out->status = status; out->numeric = 0;
+}
+
 template <class S, int NM, bool FDE = false>
 __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, NM> a) {
   extern __shared__ double aid_dyn[];
@@ -284,60 +292,80 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
   const double* __restrict__ const in = a.m[f].in;
   AidOut* const out = a.m[f].out;
   const int ldp = a.m[f].ldp, M = a.m[f].M, m = a.m[f].m, n = 15 + 6 * M;
-  const bool lin = a.m[f].item[0].model == kAidLinear;
+  const int& n_items = a.m[f].n_items;  // (read where used: a copy held in a register cost the batched forms 8 registers)
+  const bool lin = !FDE && a.m[f].item[0].model == kAidLinear;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   double* const Wt = a.m[f].ws ? a.m[f].ws : aid_dyn;  // [n][m]: column c of H P, then of W = L^-1 H P
   double* const dx = Wt + (size_t)n * m;
   const double* __restrict__ const R = in + kAidZ;
   const double* __restrict__ const H = R + m * m;      // LINEAR only
-  __shared__ double L[kAidMaxRows + 1][kAidMaxRows + 1];  // S = L L^T (lower); row m: r, then y = L^-1 r
+  __shared__ double L[kAidMaxRows + 1][kAidMaxRows + 1];  // S_AA = L L^T (lower); row m_A: r_A, then y = L^-1 r_A
   __shared__ double idg[kAidMaxRows];
   __shared__ double part[kAidThreads / 32];
   __shared__ int s_col[kAidMaxRows][kAidNnz];             // the model rows of H: (state index, coefficient) pairs
   __shared__ double s_coef[kAidMaxRows][kAidNnz];
   __shared__ int s_nnz[kAidMaxRows];
   __shared__ int s_nv, s_apply, s_bad;
+  // FDE only: the plain form never touches these, so it allocates none of them
+  __shared__ double s_r[kAidMaxRows];                    // r, for every round
+  __shared__ int s_ri[kAidMaxRows], s_c0[kAidMaxItems];  // row k of S_AA is stack row s_ri[k]; item w's first row in S_AA
+  __shared__ double s_t[kAidMaxItems], s_blk[kAidMaxItems][42];  // t_j of the round; a warp's d x d block and vector
+  __shared__ unsigned s_A;  // the items of A (bits)
+  __shared__ int s_mA, s_done;  // s_done: the outcome once it is decided, else -1
+  AidFdeOut* const fo = reinterpret_cast<AidFdeOut*>(out);
+  const double* __restrict__ const chi2 = R + m * m;     // FDE: chi2[32], then max_exclude
+  const auto rows_of = [&](int k) { return (k + 1 < n_items ? a.m[f].item[k + 1].row : m) - a.m[f].item[k].row; };
 
-  // ---- residual (fp64) and the rows of H, one thread per item
+  // ---- residual (fp64) and the rows of H, one thread per item.  A degenerate item (a heading whose yaw or a range whose
+  // prediction is undefined) ends a plain member; the FDE form drops it from A and never reads its rows.
   int degenerate = 0;
-  int mA = m;  // the rows of the update (FDE: of the kept items, the first mA entries of each Wt row; y in row mA of L)
-  if constexpr (FDE) {  // r stays in s_r for every round; a degenerate item is dropped from A (its rows are never read)
-    __shared__ double s_r[kAidMaxRows];
-    __shared__ int s_ri[kAidMaxRows], s_c0[kAidMaxItems];  // row k of S_AA is stack row s_ri[k]; item w's first row in S_AA
-    __shared__ double s_t[kAidMaxItems], s_blk[kAidMaxItems][42];  // t_j of the round; a warp's d x d block and vector
-    __shared__ unsigned s_A;  // the items of A (bits)
-    __shared__ int s_mA, s_done;
-    AidFdeOut* const fo = reinterpret_cast<AidFdeOut*>(out);
-    const double* __restrict__ const chi2 = R + m * m;
-    const int n_items = a.m[f].n_items;
-    const auto rows_of = [&](int k) { return (k + 1 < n_items ? a.m[f].item[k + 1].row : m) - a.m[f].item[k].row; };
-    if (t < n_items) {
-      degenerate = aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, s_r, s_col, s_coef, s_nnz);
+  if (lin) {
+    if (t < m) L[m][t] = in[t];
+  } else if (t < n_items) {
+    degenerate = aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, FDE ? s_r : &L[m][0], s_col, s_coef, s_nnz);
+    if constexpr (FDE)
       fo->item[t] = {__longlong_as_double(0x7ff8000000000000ll), __longlong_as_double(0x7ff8000000000000ll), degenerate ? 2 : 3, -1};
-    }
+  }
+  bool stop;
+  if constexpr (FDE) {
     const unsigned keep = __ballot_sync(0xffffffffu, t < n_items && !degenerate);
-    if (t == 0) { s_A = keep; s_mA = 0; }
+    if (t == 0) s_A = keep;
     __syncthreads();
-    if (s_A == 0u) {  // every item degenerate: nothing is written
-      if (t == 0) {
-        out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
-        out->dof = 0; out->applied = 0; out->status = 2; out->numeric = 0;
-        fo->outcome = -1; fo->n_excluded = 0;
-      }
-      return;
+    stop = s_A == 0u;  // every item degenerate
+  } else {
+    stop = __syncthreads_or(degenerate);
+  }
+  if (stop) {  // nothing is written
+    if (t == 0) {
+      aid_nothing(out, FDE ? 0 : m, 2);
+      if constexpr (FDE) { fo->outcome = -1; fo->n_excluded = 0; }
     }
-    // H P of the kept rows, stored transposed (stride m): kept until the update, S_AA of every round is formed from it
+    return;
+  }
+  // ---- H P, stored transposed: Wt[c][i] = (H P)[i][c] (FDE: of the kept rows); every round forms S_AA from it
+  if (lin) {
     for (int idx = t; idx < m * n; idx += kAidThreads) {
       const int i = idx / n, c = idx - i * n;
-      int k = 0;
-      while (k + 1 < n_items && a.m[f].item[k + 1].row <= i) ++k;
-      if (!((s_A >> k) & 1u)) continue;
-      double s = s_coef[i][0] * (double)P[(size_t)s_col[i][0] * ldp + c];
-      for (int q = 1; q < s_nnz[i]; ++q) s += s_coef[i][q] * (double)P[(size_t)s_col[i][q] * ldp + c];
+      const double* h = H + (size_t)i * n;
+      double s = 0.0;
+      for (int k = 0; k < n; ++k) s += h[k] * (double)P[(size_t)k * ldp + c];
       Wt[(size_t)c * m + i] = s;
     }
-    __syncthreads();
-    // each kept item alone against the prior: r_j^T S_jj^-1 r_j (warp j, lane 0)
+  } else {
+    for (int idx = t; idx < m * n; idx += kAidThreads) {
+      const int i = idx / n, c = idx - i * n;
+      if constexpr (FDE) {
+        int k = 0;
+        while (k + 1 < n_items && a.m[f].item[k + 1].row <= i) ++k;
+        if (!((s_A >> k) & 1u)) continue;
+      }
+      double s = s_coef[i][0] * (double)P[(size_t)s_col[i][0] * ldp + c];  // (exact for the one-coefficient rows)
+      for (int k = 1; k < s_nnz[i]; ++k) s += s_coef[i][k] * (double)P[(size_t)s_col[i][k] * ldp + c];
+      Wt[(size_t)c * m + i] = s;
+    }
+  }
+  __syncthreads();
+  if constexpr (FDE) {  // each kept item alone against the prior: r_j^T S_jj^-1 r_j (warp j, lane 0)
     if (warp < n_items && lane == 0 && ((s_A >> warp) & 1u)) {
       const int r0 = a.m[f].item[warp].row, d = rows_of(warp);
       double* B = s_blk[warp];
@@ -352,10 +380,12 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
       }
       fo->item[warp].nis = aid_small_quad(B, B + 36, d);
     }
-    const int max_exclude = (int)R[m * m + kAidMaxRows];
-    int outcome = -1, n_exc = 0;
-    for (int round = 0;; ++round) {
-      // ---- S_AA (lower) from H P and R with the expression of the plain kernel, r_A as row m_A
+  }
+  // ---- rounds over the kept set A (plain: one round, A every row): S_AA, its factor, y = L^-1 r_A, NIS and the gate.
+  // FDE outcome 0: applied; 1: applied after exclusions; 2: rejected (at max_exclude); 3: no identifiable fault.
+  int ma = m, n_exc = 0;
+  for (int round = 0;; ++round) {
+    if constexpr (FDE) {
       if (t == 0) {
         int k = 0;
         for (int w = 0; w < n_items; ++w) {
@@ -366,42 +396,62 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
         s_mA = k;
       }
       __syncthreads();
-      const int ma = s_mA;
-      for (int idx = t; idx < ma * ma; idx += kAidThreads) {
-        const int i = idx / ma, j = idx - i * ma;
-        if (j > i) continue;
-        const int ri = s_ri[i], rj = s_ri[j];
-        double s = s_coef[rj][0] * Wt[(size_t)s_col[rj][0] * m + ri];
-        for (int q = 1; q < s_nnz[rj]; ++q) s += s_coef[rj][q] * Wt[(size_t)s_col[rj][q] * m + ri];
-        L[i][j] = s + R[ri * m + rj];
+      ma = s_mA;
+    }
+    // S_AA = (H P H^T + R)_AA, lower triangle (only R's lower triangle is read); R is block-diagonal across items, so S_AA is
+    // a principal submatrix of S
+    for (int idx = t; idx < ma * ma; idx += kAidThreads) {
+      const int i = idx / ma, j = idx - i * ma;
+      if (j > i) continue;
+      const int ri = FDE ? s_ri[i] : i, rj = FDE ? s_ri[j] : j;
+      double s;
+      if (lin) {
+        const double* h = H + (size_t)j * n;
+        s = 0.0;
+        for (int k = 0; k < n; ++k) s += Wt[(size_t)k * m + i] * h[k];
+      } else {
+        s = s_coef[rj][0] * Wt[(size_t)s_col[rj][0] * m + ri];
+        for (int k = 1; k < s_nnz[rj]; ++k) s += s_coef[rj][k] * Wt[(size_t)s_col[rj][k] * m + ri];
       }
+      L[i][j] = s + R[ri * m + rj];
+    }
+    if constexpr (FDE) {
       if (t < ma) L[ma][t] = s_r[s_ri[t]];
-      __syncthreads();
-      if (warp == 0) {
-        const int nv = warp_chol(L, ma, idg, lane);
-        if (lane == 0) s_nv = nv;
-        if (nv == ma) {
-          const double x = warp_row_solve(lane < ma ? L[ma][lane] : 0.0, L, idg, ma, lane);
-          if (lane < ma) L[ma][lane] = x;
-        }
+    }
+    __syncthreads();
+    if (warp == 0) {
+      const int nv = warp_chol(L, ma, idg, lane);
+      if (lane == 0) s_nv = nv;
+      if (nv == ma) {
+        const double x = warp_row_solve(lane < ma ? L[ma][lane] : 0.0, L, idg, ma, lane);
+        if (lane < ma) L[ma][lane] = x;
       }
-      __syncthreads();
-      if (s_nv < ma) {  // S_AA not positive definite: nothing is written
-        if (t == 0) {
-          out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
-          out->dof = ma; out->applied = 0; out->status = 1; out->numeric = 0;
-          fo->outcome = -1; fo->n_excluded = n_exc;
-        }
-        return;
-      }
+    }
+    __syncthreads();
+    if (s_nv < ma) {  // S_AA not positive definite: nothing is written
       if (t == 0) {
-        double g = 0.0;
-        for (int i = 0; i < ma; ++i) g += L[ma][i] * L[ma][i];
-        out->nis = g; out->dof = ma; out->status = 0;
-        s_done = !(g > chi2[ma - 1]) ? (n_exc ? 1 : 0) : n_exc >= max_exclude ? 2 : __popc(s_A) == 1 ? 3 : -1;
+        aid_nothing(out, ma, 1);
+        if constexpr (FDE) { fo->outcome = -1; fo->n_excluded = n_exc; }
       }
-      __syncthreads();
-      if (s_done >= 0) { outcome = s_done; break; }
+      return;
+    }
+    if (t == 0) {
+      double g = 0.0;
+      for (int i = 0; i < ma; ++i) g += L[ma][i] * L[ma][i];
+      out->nis = g; out->dof = ma; out->status = 0;
+      if constexpr (FDE) {
+        const int max_exclude = (int)chi2[kAidMaxRows];
+        s_done = !(g > chi2[ma - 1]) ? (n_exc ? 1 : 0) : n_exc >= max_exclude ? 2 : __popc(s_A) == 1 ? 3 : -1;
+      } else {
+        const double chi2_max = a.m[f].chi2_max;
+        s_apply = !(chi2_max > 0.0 && g > chi2_max);
+      }
+    }
+    __syncthreads();
+    if constexpr (!FDE) {
+      break;
+    } else {
+      if (s_done >= 0) break;
       // ---- exclusion round: warp w of A forms g_a = L^-1 e_a over its rows, y_w = G^T (L^-1 r_A), B_w = G^T G, t_w
       if (warp < n_items && ((s_A >> warp) & 1u)) {
         const int d = rows_of(warp), c0 = s_c0[warp];
@@ -446,116 +496,38 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
         }
       }
       __syncthreads();
-      if (s_done >= 0) { outcome = s_done; break; }
+      if (s_done >= 0) break;
       ++n_exc;
     }
-    if (t == 0) {
-      fo->outcome = outcome; fo->n_excluded = n_exc;
-      for (int w = 0; w < n_items; ++w)
-        if ((s_A >> w) & 1u) fo->item[w].state = outcome <= 1 ? 0 : 3;
-      out->applied = outcome <= 1;
-      s_apply = outcome <= 1;
-      s_bad = 0;
-      if (!s_apply) { out->dx_norm = 0.0; out->numeric = 0; }
-    }
-    __syncthreads();
-    if (!s_apply) return;
-    // ---- W = L^-1 H P over the rows of A, gathered in order into the first m_A entries of each Wt row
-    mA = s_mA;
-    for (int r = warp; r < n; r += kAidThreads / 32) {
-      double* row = Wt + (size_t)r * m;
-      const double x0 = lane < mA ? row[s_ri[lane]] : 0.0;
-      __syncwarp();
-      const double x = warp_row_solve(x0, L, idg, mA, lane);
-      if (lane < mA) row[lane] = x;
-    }
-    __syncthreads();
-  } else {  // the plain single-model, LINEAR and stacked update (left at its original indentation)
-  if (lin) {
-    if (t < m) L[m][t] = in[t];
-  } else if (t < a.m[f].n_items) {
-    degenerate = aid_item_rows(a.m[f].item[t], in + kAidItemZ * t, st, poses, &L[m][0], s_col, s_coef, s_nnz);
   }
-  if (__syncthreads_or(degenerate)) {  // a heading whose yaw or a range whose prediction is undefined: nothing is written
-    if (t == 0) {
-      out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
-      out->dof = m; out->applied = 0; out->status = 2; out->numeric = 0;
-    }
-    return;
-  }
-  // ---- H P, stored transposed: Wt[c][i] = (H P)[i][c]
-  if (lin) {
-    for (int idx = t; idx < m * n; idx += kAidThreads) {
-      const int i = idx / n, c = idx - i * n;
-      const double* h = H + (size_t)i * n;
-      double s = 0.0;
-      for (int k = 0; k < n; ++k) s += h[k] * (double)P[(size_t)k * ldp + c];
-      Wt[(size_t)c * m + i] = s;
-    }
-  } else {
-    for (int idx = t; idx < m * n; idx += kAidThreads) {
-      const int i = idx / n, c = idx - i * n;
-      double s = s_coef[i][0] * (double)P[(size_t)s_col[i][0] * ldp + c];  // (exact for the one-coefficient rows)
-      for (int k = 1; k < s_nnz[i]; ++k) s += s_coef[i][k] * (double)P[(size_t)s_col[i][k] * ldp + c];
-      Wt[(size_t)c * m + i] = s;
-    }
-  }
-  __syncthreads();
-  // ---- S = H P H^T + R, lower triangle (only R's lower triangle is read)
-  for (int idx = t; idx < m * m; idx += kAidThreads) {
-    const int i = idx / m, j = idx - i * m;
-    if (j > i) continue;
-    double s;
-    if (lin) {
-      const double* h = H + (size_t)j * n;
-      s = 0.0;
-      for (int k = 0; k < n; ++k) s += Wt[(size_t)k * m + i] * h[k];
-    } else {
-      s = s_coef[j][0] * Wt[(size_t)s_col[j][0] * m + i];
-      for (int k = 1; k < s_nnz[j]; ++k) s += s_coef[j][k] * Wt[(size_t)s_col[j][k] * m + i];
-    }
-    L[i][j] = s + R[i * m + j];
-  }
-  __syncthreads();
-  // ---- S = L L^T (one warp), then y = L^-1 r and W = L^-1 H P: rows of [W^T ; y^T] against L^T, one warp per row
-  if (warp == 0) {
-    const int nv = warp_chol(L, m, idg, lane);
-    if (lane == 0) s_nv = nv;
-  }
-  __syncthreads();
-  if (s_nv < m) {  // S not positive definite: nothing is written
-    if (t == 0) {
-      out->nis = __longlong_as_double(0x7ff8000000000000ll); out->dx_norm = 0.0;
-      out->dof = m; out->applied = 0; out->status = 1; out->numeric = 0;
-    }
-    return;
-  }
-  for (int r = warp; r <= n; r += kAidThreads / 32) {
-    double* row = r < n ? Wt + (size_t)r * m : &L[m][0];
-    const double x = warp_row_solve(lane < m ? row[lane] : 0.0, L, idg, m, lane);
-    if (lane < m) row[lane] = x;
-  }
-  __syncthreads();
   if (t == 0) {
-    double g = 0.0;
-    for (int i = 0; i < m; ++i) g += L[m][i] * L[m][i];
-    const double chi2_max = a.m[f].chi2_max;
-    s_apply = !(chi2_max > 0.0 && g > chi2_max);
+    if constexpr (FDE) {
+      fo->outcome = s_done; fo->n_excluded = n_exc;
+      for (int w = 0; w < n_items; ++w)
+        if ((s_A >> w) & 1u) fo->item[w].state = s_done <= 1 ? 0 : 3;
+      s_apply = s_done <= 1;
+    }
+    out->applied = s_apply;
     s_bad = 0;
-    out->nis = g; out->dof = m; out->status = 0; out->applied = s_apply;
+    if (!s_apply) { out->dx_norm = 0.0; out->numeric = 0; }
   }
   __syncthreads();
-  if (!s_apply) {
-    if (t == 0) { out->dx_norm = 0.0; out->numeric = 0; }
-    return;
+  if (!s_apply) return;
+  // ---- W = L^-1 H P over the rows of A (FDE: gathered in order into the first m_A entries of each Wt row), one warp per row
+  for (int r = warp; r < n; r += kAidThreads / 32) {
+    double* row = Wt + (size_t)r * m;
+    const double x0 = lane < ma ? row[FDE ? s_ri[lane] : lane] : 0.0;
+    __syncwarp();
+    const double x = warp_row_solve(x0, L, idg, ma, lane);
+    if (lane < ma) row[lane] = x;
   }
-  }  // (FDE)
+  __syncthreads();
   // ---- dx = W^T y, and P <- P - W^T W (lower triangle in fp64, written to both halves: exactly symmetric)
   double nn = 0.0;
   for (int c = t; c < n; c += kAidThreads) {
     const double* w = Wt + (size_t)c * m;
     double s = 0.0;
-    for (int i = 0; i < mA; ++i) s += w[i] * L[mA][i];
+    for (int i = 0; i < ma; ++i) s += w[i] * L[ma][i];
     dx[c] = s;
     nn += s * s;
   }
@@ -566,7 +538,7 @@ __global__ void __launch_bounds__(kAidThreads) k_aid(const Members<AidArgs<S>, N
     const double* wr = Wt + (size_t)r * m;
     const double* wc = Wt + (size_t)c * m;
     double v = 0.0;
-    for (int i = 0; i < mA; ++i) v += wr[i] * wc[i];
+    for (int i = 0; i < ma; ++i) v += wr[i] * wc[i];
     const S x = (S)((double)P[(size_t)r * ldp + c] - v);
     if (!isfinite((double)x)) bad = 1;
     P[(size_t)r * ldp + c] = x;

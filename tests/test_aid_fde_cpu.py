@@ -1,9 +1,8 @@
 """The numpy FDE over a stack's items (tests/aid_fde_reference.py), without a device: the block w-test against the NIS
 difference, and the outcomes the rounds of msckf_b200_aid_stack_update_fde reach on range stacks with and without NLOS faults;
-capi.fde_thresholds / fde_struct; and what the class and C view forms send to the C-ABI, through the recording fake
-tests/stub/stub_aid_fde.cpp."""
+capi.fde_thresholds / fde_struct; and what the class and C view forms send to the C-ABI, through the recording fake of
+tests/aid_stack_stub.py."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
@@ -11,7 +10,7 @@ import pytest
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
 from tests import aid_fde_reference as ref
-from tests.common import ROOT
+from tests.aid_stack_stub import recorded, stub_view  # noqa: F401 (stub_view: the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 CHI2 = capi.fde_thresholds(0.01)
@@ -106,33 +105,6 @@ def test_scene_is_consistent_at_the_state():
 
 
 # ---- the class and C view forms over the recording fake of the C-ABI --------------------------------------------------------
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_fde_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / n for n in ("stub_engine.cpp", "stub_batch_state.cpp", "stub_aid.cpp", "stub_range_stack.cpp",
-                                                 "stub_aid_fde.cpp")]
-    src += [csrc / n for n in ("filter_capi.cpp", "batch_capi.cpp", "aid_capi.cpp", "aid_stack_capi.cpp", "fde_capi.cpp")]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", f"-I{csrc}", *map(str, src),
-                               "-o", str(so)])
-    return so
-
-
-def _recorded(f):
-    """([single calls, batched calls] naming f, the last call's fde as (chi2 [32], max_exclude), its items as dicts)"""
-    out, fde, rec = (C.c_longlong * 2)(), (C.c_double * 33)(), (C.c_double * (20 * 8))()
-    n = f.lib.msckf_b200_stub_fde_calls(C.c_void_p(f.engineHandle()), out, fde, rec, 8)
-    items = []
-    for k in range(n):
-        r = np.array(rec[20 * k:20 * k + 20])
-        z, R = r[3:11], r[11:20]
-        items.append({"model": int(r[0]), "a": int(r[1]), "b": int(r[2]), "z": z[np.isfinite(z)], "R": R[np.isfinite(R)]})
-    return [out[0], out[1]], (list(fde[:32]), int(fde[32])), items
-
-
 def _filters(lib, n, dtype, frames=4):
     wl = synth.make_stream_workload(n_frames=frames + 1, seq=2, max_features=10)
     fs = [shim_filter(lib, dtype) for _ in range(n)]
@@ -158,7 +130,7 @@ def test_views_pass_fde_and_items_through_unchanged(stub_view, dtype):
     fde = {"chi2": [float(x) for x in 1.0 + rng.random(32)], "max_exclude": 3}
 
     def check(f, items, fde):
-        _, (chi2, K), got = _recorded(f)
+        _, _, (chi2, K), got = recorded(f)
         assert chi2 == fde["chi2"] and K == fde["max_exclude"]
         assert len(got) == len(items)
         for g, it in zip(got, items):
@@ -166,22 +138,22 @@ def test_views_pass_fde_and_items_through_unchanged(stub_view, dtype):
             assert np.array_equal(g["z"], np.asarray(it["z"], dtype=np.float64))
             assert np.array_equal(g["R"], np.asarray(it["R"], dtype=np.float64).ravel())
 
-    base = [_recorded(f)[0] for f in fs]
+    base = [recorded(f)[0] for f in fs]
     r = fs[0].aid_stack_update(stack, fde=fde)
     assert r["dof"] == 1 + 1 + 2 + 3 + 3 and r["outcome"] == 0 and [it["state"] for it in r["items"]] == [0] * 5
-    assert _recorded(fs[0])[0] == [base[0][0] + 1, base[0][1]]
+    assert recorded(fs[0])[0] == [base[0][0] + 1, base[0][1]]
     check(fs[0], stack, fde)
     fb = FilterBatch(fs)
     fde2 = dict(fde, max_exclude=0)
     res = fb.aid_stack_update([stack[3:], None, stack[:2]], fde=fde2)
     assert res[1] is None and res[0]["dof"] == 6 and res[2]["dof"] == 2 and len(res[0]["items"]) == 2
-    assert [[c[0] - b[0], c[1] - b[1]] for c, b in zip([_recorded(f)[0] for f in fs], base)] == [[1, 1], [0, 0], [0, 1]]
+    assert [[c[0] - b[0], c[1] - b[1]] for c, b in zip([recorded(f)[0] for f in fs], base)] == [[1, 1], [0, 0], [0, 1]]
     check(fs[0], stack[3:], fde2)
     check(fs[2], stack[:2], fde2)
     # refused in the class: nothing reaches the C-ABI
     err = fs[0].lib.msckf_mono_last_error
     err.restype = C.c_char_p
-    n_calls = [_recorded(f)[0] for f in fs]
+    n_calls = [recorded(f)[0] for f in fs]
     bad = [dict(fde, max_exclude=8), dict(fde, max_exclude=-1), dict(fde, chi2=[np.nan] + fde["chi2"][1:]),
            dict(fde, chi2=fde["chi2"][:31] + [0.0]), dict(fde, chi2=fde["chi2"][:5] + [np.inf] + fde["chi2"][6:])]
     for b in bad:
@@ -191,7 +163,7 @@ def test_views_pass_fde_and_items_through_unchanged(stub_view, dtype):
         with pytest.raises(RuntimeError):
             fb.aid_stack_update([stack, stack[:1], None], fde=b)
         assert "fde" in err().decode()
-    assert [_recorded(f)[0] for f in fs] == n_calls
+    assert [recorded(f)[0] for f in fs] == n_calls
     fb.close()
     for f in fs:
         f.close()

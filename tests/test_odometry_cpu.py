@@ -3,40 +3,22 @@ bodyVelocityUpdate, relativePoseUpdate and MSCKFBatch::aidedUpdate(items) (one C
 handed over first, the host mirror refreshed afterwards, state ids mapped to window positions), and the Monte-Carlo runner's
 odometry (the trials' other inputs do not change; the truth odometry agrees with the truth trajectory).
 
-The C view is linked against the recording fake of the C-ABI (tests/stub/stub_engine.cpp, stub_batch_state.cpp, stub_aid.cpp)
-plus tests/stub/stub_aid_stack.cpp, whose VELOCITY / POSITION items copy z into the fake's IMU state."""
-import ctypes as C
-import subprocess
-
+The C view is linked against the recording fake of the C-ABI (tests/aid_stack_stub.py), whose VELOCITY / POSITION items
+copy z into the fake's IMU state."""
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.common import ROOT
+from tests.aid_stack_stub import batch_calls, recorded, stub_view  # noqa: F401 (stub_view: the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
-
-
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_odometry_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / n for n in ("stub_engine.cpp", "stub_batch_state.cpp", "stub_aid.cpp", "stub_aid_stack.cpp")]
-    src += [csrc / n for n in ("filter_capi.cpp", "batch_capi.cpp", "aid_capi.cpp", "aid_stack_capi.cpp")]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", *map(str, src), "-o", str(so)])
-    return so
 
 
 def _calls(f, base=(0, 0)):
     """[single calls, batched calls naming f] since `base`, the readings handed over before the last one, and that call's
     items as (model, a, b) triples"""
-    out = (C.c_longlong * 3)()
-    items = (C.c_int * 24)()
-    n = f.lib.msckf_b200_stub_aid_stack_calls(C.c_void_p(f.engineHandle()), out, items, 8)
-    return [out[0] - base[0], out[1] - base[1], out[2]], [tuple(items[3 * k:3 * k + 3]) for k in range(n)]
+    calls, readings, _, items = recorded(f)
+    return [calls[0] - base[0], calls[1] - base[1], readings], [(it["model"], it["a"], it["b"]) for it in items]
 
 
 def _filters(lib, n, dtype, frames=3):
@@ -94,6 +76,7 @@ def test_batch_makes_one_call_and_leaves_unnamed_members_alone(stub_view, dtype)
     fb = FilterBatch(fs)
     p0 = [f.getImuState()["p_I_G"].copy() for f in fs]
     c0 = [_calls(f)[0] for f in fs]
+    nb = batch_calls(fb)  # (the fake keys its counters by handle address, which a later batch may reuse)
     for (w, a, dT) in wl["frames"][3]["imu"][:3]:
         fb.propagate(1, w, a, dT)
     zs = [p + 10.0 * (i + 1) for i, p in enumerate(p0)]
@@ -101,7 +84,7 @@ def test_batch_makes_one_call_and_leaves_unnamed_members_alone(stub_view, dtype)
     res = fb.aid_stack_update([[bv, {"model": capi.AID_POSITION, "z": zs[0], "R": np.eye(3)}], None,
                                [{"model": capi.AID_POSITION, "z": zs[2], "R": np.eye(3)}]])
     assert res[1] is None and res[0]["dof"] == 6 and res[2]["dof"] == 3
-    assert fs[0].lib.msckf_b200_stub_batch_aid_stack_calls(C.c_void_p(fb.handle())) == 1
+    assert batch_calls(fb) == nb + 1
     assert [_calls(f, c)[0][:2] for f, c in zip(fs, c0)] == [[0, 1], [0, 0], [0, 1]]
     assert np.array_equal(fs[0].getImuState()["p_I_G"], zs[0].astype(dtype))
     assert np.array_equal(fs[1].getImuState()["p_I_G"], p0[1])

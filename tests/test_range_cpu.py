@@ -3,51 +3,23 @@ PLANE_RANGE, CLONE_PLANE_RANGE) against the truth stream and against central dif
 (MSCKF::rangeUpdate, cloneRangeUpdate, planeRangeUpdate, clonePlaneRangeUpdate) and MSCKFBatch::aidedUpdate(items) send to the
 C-ABI, and the Monte-Carlo runner's ranging inputs and summary.
 
-The C view is linked against the recording fake of the C-ABI (tests/stub/stub_engine.cpp, stub_batch_state.cpp, stub_aid.cpp)
-plus tests/stub/stub_range_stack.cpp, which records every stacked item in full and calls the class forms on a view handle."""
+The C view is linked against the recording fake of the C-ABI (tests/aid_stack_stub.py), which records every stacked item in
+full and calls the class forms on a view handle."""
 import ctypes as C
 import math
-import subprocess
 
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.common import ROOT
+from tests.aid_stack_stub import batch_calls, recorded, stub_view  # noqa: F401 (stub_view: the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 RANGES = (capi.AID_RANGE, capi.AID_CLONE_RANGE, capi.AID_PLANE_RANGE, capi.AID_CLONE_PLANE_RANGE)
 LEVER = np.array([0.3, -0.2, 0.5])
 PLANE_LEVER = np.array([0.1, 0.2, -0.1])
 TILTED = np.array([-1.0, 0.2, 0.1])  # a beam about 13 degrees off the IMU's downward axis
-
-
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_range_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / n for n in ("stub_engine.cpp", "stub_batch_state.cpp", "stub_aid.cpp", "stub_range_stack.cpp")]
-    src += [csrc / n for n in ("filter_capi.cpp", "batch_capi.cpp", "aid_capi.cpp", "aid_stack_capi.cpp")]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", f"-I{csrc}", *map(str, src),
-                               "-o", str(so)])
-    return so
-
-
-def _recorded(f):
-    """([single calls, batched calls] naming f, the items of its last stacked call as dicts model, a, b, z, R)"""
-    out = (C.c_longlong * 2)()
-    rec = (C.c_double * (20 * 8))()
-    n = f.lib.msckf_b200_stub_range_calls(C.c_void_p(f.engineHandle()), out, rec, 8)
-    items = []
-    for k in range(n):
-        r = np.array(rec[20 * k:20 * k + 20])
-        z, R = r[3:11], r[11:20]
-        items.append({"model": int(r[0]), "a": int(r[1]), "b": int(r[2]), "z": z[np.isfinite(z)], "R": R[np.isfinite(R)]})
-    return [out[0], out[1]], items
 
 
 def _class_call(f, which, state_id=0, rho=1.0, h=0.0, anchor=(0.0, 0.0, 0.0), lever=(0.0, 0.0, 0.0), axis=(-1.0, 0.0, 0.0), var=1.0):
@@ -178,7 +150,7 @@ def test_class_forms_send_the_expected_items(stub_view, dtype):
     ids = [int(x) for x in f.getCamStates()["state_id"]]
     assert len(ids) == 4
     a, lv, ax = np.array([5.0, -5.0, 2.0]), np.array([0.3, -0.2, 0.5]), np.array([-1.0, 0.2, 0.1])
-    base = _recorded(f)[0]
+    base = recorded(f)[0]
     cases = [  # (which, kwargs, expected item)
         (0, dict(rho=7.5, anchor=a, lever=lv, var=0.01), {"model": capi.AID_RANGE, "a": 0, "b": 0, "z": np.r_[7.5, a, lv], "R": [0.01]}),
         (1, dict(state_id=ids[1], rho=6.0, anchor=a, lever=lv, var=0.04),
@@ -191,20 +163,20 @@ def test_class_forms_send_the_expected_items(stub_view, dtype):
     for k, (which, kw, want) in enumerate(cases):
         rc, res = _class_call(f, which, **kw)
         assert rc == 0 and res.applied == 1 and res.dof == 1, (which, rc)
-        calls, got = _recorded(f)
+        calls, _, _, got = recorded(f)
         assert calls == [base[0] + k + 1, base[1]]  # one C-ABI call per class call
         assert len(got) == 1
         for key in ("model", "a", "b"):
             assert got[0][key] == want[key], (which, key)
         assert np.array_equal(got[0]["z"], want["z"]) and np.array_equal(got[0]["R"], np.array(want["R"])), which
-    n_calls = _recorded(f)[0]
+    n_calls = recorded(f)[0]
     # refused before any device call: an id that is not in the window
     err = f.lib.msckf_mono_last_error
     err.restype = C.c_char_p
     for which, sid in ((1, max(ids) + 1), (3, -5), (1, min(ids) - 1)):
         rc, _ = _class_call(f, which, state_id=sid)
         assert rc == -1 and "not in the window" in err().decode(), (which, sid, err())
-    assert _recorded(f)[0] == n_calls
+    assert recorded(f)[0] == n_calls
     f.close()
 
 
@@ -222,23 +194,23 @@ def test_views_pass_items_through_unchanged(stub_view, dtype):
              {"model": capi.AID_PLANE_RANGE, "z": rng.normal(size=8), "R": np.array([[0.02]])}]
 
     def check(f, items):
-        got = _recorded(f)[1]
+        got = recorded(f)[3]
         assert len(got) == len(items)
         for g, it in zip(got, items):
             assert g["model"] == it["model"] and g["a"] == it.get("a", 0) and g["b"] == it.get("b", 0)
             assert np.array_equal(g["z"], np.asarray(it["z"], dtype=np.float64))
             assert np.array_equal(g["R"], np.asarray(it["R"], dtype=np.float64).ravel())
 
-    base = [_recorded(f)[0] for f in fs]  # (the fake keys its counters by handle address, which a later filter may reuse)
+    base = [recorded(f)[0] for f in fs]  # (the fake keys its counters by handle address, which a later filter may reuse)
     r = fs[0].aid_stack_update(stack)
-    assert r["dof"] == 1 + 1 + 2 + 1 + 2 + 1 and _recorded(fs[0])[0] == [base[0][0] + 1, base[0][1]]
+    assert r["dof"] == 1 + 1 + 2 + 1 + 2 + 1 and recorded(fs[0])[0] == [base[0][0] + 1, base[0][1]]
     check(fs[0], stack)
     fb = FilterBatch(fs)
-    nb = fs[0].lib.msckf_b200_stub_range_batch_calls(C.c_void_p(fb.handle()))
+    nb = batch_calls(fb)
     res = fb.aid_stack_update([stack[3:], None, stack[:2]])
     assert res[1] is None and res[0]["dof"] == 4 and res[2]["dof"] == 2
-    assert fs[0].lib.msckf_b200_stub_range_batch_calls(C.c_void_p(fb.handle())) == nb + 1
-    assert [[c[0] - b[0], c[1] - b[1]] for c, b in zip([_recorded(f)[0] for f in fs], base)] == [[1, 1], [0, 0], [0, 1]]
+    assert batch_calls(fb) == nb + 1
+    assert [[c[0] - b[0], c[1] - b[1]] for c, b in zip([recorded(f)[0] for f in fs], base)] == [[1, 1], [0, 0], [0, 1]]
     check(fs[0], stack[3:])
     check(fs[2], stack[:2])
     fb.close()
