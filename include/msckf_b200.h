@@ -357,6 +357,46 @@ int msckf_b200_aid_stack_update_fde(msckf_b200_engine* e, const msckf_b200_aid_i
  * member is validated before anything is launched.  One launch per 32 updated members. */
 int msckf_b200_batch_aid_stack_update_fde(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
                                           const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out);
+/* ---- iterated stacked updates (an iterated EKF for the first range or GNSS epoch after drift) ------------------------------
+ * One linearisation at the prior leaves a far-off filter overconfident: a range's curvature is of order delta^2 / (2 rho), and
+ * the attitude terms of lever arms, BODY_VELOCITY, RELATIVE_POSE, POSE, HEADING and PLANE_RANGE are nonlinear too.  With
+ * delta_0 = 0 and the iterate x_i = x^ [+] delta_i (fp64, the injection above on q_IG, v_I_G, p_I_G and on the poses of the clones
+ * the items name: q_IG <- buildUpdateQuat(dtheta) * q_IG not renormalised, clone q <- normalise(buildUpdateQuat(dtheta_k) * q),
+ * v and p additive), linearisation i forms r_i, H_i of the stack's items at x_i and factors S against the prior P with the
+ * residual r_i + H_i delta_i; delta_{i+1} = W^T y = K_i (r_i + H_i delta_i).  It stops when max |delta_{i+1} - delta_i| <= tol
+ * (converged; NaN counts as infinite) or after max_iter linearisations; then P <- P - W^T W and one injection of W^T y, both of
+ * the last linearisation.  The Jacobian of [+] is not applied.  Linearisation 0 decides the NIS, dof, the chi2_max gate and
+ * (FDE) the kept set, every outcome and each item's record; the iteration runs only on an applied stack, over its kept rows.
+ * An item of the stack that is degenerate at an iterate (status 2's conditions) stops the iteration and the previous
+ * linearisation is applied.  S not positive definite at any linearisation: status 1, nothing written.  max_iter 0 or 1 is the
+ * call without _iter bit for bit (P, the state, the NIS, dx_norm).  Still one launch per 32 members, one copy each way and one
+ * synchronisation; the iteration runs inside the member's CTA. */
+typedef struct {
+  int max_iter;          /* linearisations, 0 .. 16 (0 or 1: one) */
+  double tol;            /* finite, >= 0: converged when max |delta_{i+1} - delta_i| <= tol */
+} msckf_b200_aid_iter;
+typedef struct {
+  int iterations;        /* linearisations applied (0 when nothing was applied) */
+  int converged;         /* 1: the last step was <= tol (always 0 for max_iter <= 1) */
+  double step;           /* the last max |delta_{i+1} - delta_i| (0 for max_iter <= 1) */
+} msckf_b200_aid_iter_result;
+/* Refusals (MSCKF_B200_ERR_ARG, nothing written): everything the call without _iter refuses, iter or iter_out NULL, max_iter
+ * outside 0..16, a tol that is not finite and >= 0; an un-fetched update returns MSCKF_B200_ERR_STATE.  A non-finite dx or P
+ * entry returns MSCKF_B200_ERR_NUMERIC with the update applied. */
+int msckf_b200_aid_stack_update_iter(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,
+                                     const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out, msckf_b200_aid_iter_result* iter_out);
+int msckf_b200_aid_stack_update_fde_iter(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items,
+                                         const msckf_b200_aid_fde* fde, const msckf_b200_aid_iter* iter,
+                                         msckf_b200_aid_fde_result* out, msckf_b200_aid_iter_result* iter_out);
+/* the same for every member of a batch: iter[i] and iter_out[i] per member (n_items[i] = 0 leaves member i untouched and out[i],
+ * iter_out[i] not written, and iter[i] is not read); every member is validated before anything is launched.  One launch per 32
+ * updated members. */
+int msckf_b200_batch_aid_stack_update_iter(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                           double chi2_max, const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out,
+                                           msckf_b200_aid_iter_result* iter_out);
+int msckf_b200_batch_aid_stack_update_fde_iter(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                               const msckf_b200_aid_fde* fde, const msckf_b200_aid_iter* iter,
+                                               msckf_b200_aid_fde_result* out, msckf_b200_aid_iter_result* iter_out);
 /* ---- mapped landmarks: image observations of landmarks whose position is known (prior map, surveyed marker, relocalisation) --
  * Observation i is (clone[i], z[i] normalised image coordinates, p_L_G[i] landmark position in G).  With C = C(q_CG) and p_C_G of
  * that clone: p_C = C (p_L - p_C_G), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), Jacobian the 2 x 6

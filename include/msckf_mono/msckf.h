@@ -406,6 +406,33 @@ class MSCKF {
       if (!(std::isfinite(fde.chi2[d]) && fde.chi2[d] > 0.0)) throw std::invalid_argument("MSCKF::aidedUpdate: fde.chi2 must be finite and > 0");
     if (fde.max_exclude < 0 || fde.max_exclude > 7) throw std::invalid_argument("MSCKF::aidedUpdate: fde.max_exclude outside 0..7");
   }
+  // the iterated stacks (msckf_b200_aid_stack_update_iter / _fde_iter): the stack relinearised about its own update, up to
+  // iter.max_iter linearisations (0 or 1: the call above bit for bit), for the first range or GNSS epoch after drift; iter_out
+  // receives the linearisations applied, whether the step converged to iter.tol, and the last step.  An iter the C-ABI would
+  // refuse throws std::invalid_argument.  Bookkeeping as aidedUpdate(items).
+  msckf_b200_aid_result aidedUpdate(const std::vector<msckf_b200_aid_item>& items, double chi2_max, const msckf_b200_aid_iter& iter,
+                                    msckf_b200_aid_iter_result& iter_out) {
+    checkIter(iter);
+    msckf_b200_aid_result r = {};
+    checkNumeric(msckf_b200_aid_stack_update_iter(eng(), items.data(), (int)items.size(), chi2_max, &iter, &r, &iter_out),
+                 "msckf_b200_aid_stack_update_iter");
+    aidAbsorb(r);
+    return r;
+  }
+  msckf_b200_aid_fde_result aidedUpdate(const std::vector<msckf_b200_aid_item>& items, const msckf_b200_aid_fde& fde,
+                                        const msckf_b200_aid_iter& iter, msckf_b200_aid_iter_result& iter_out) {
+    checkFde(fde);
+    checkIter(iter);
+    msckf_b200_aid_fde_result r = {};
+    checkNumeric(msckf_b200_aid_stack_update_fde_iter(eng(), items.data(), (int)items.size(), &fde, &iter, &r, &iter_out),
+                 "msckf_b200_aid_stack_update_fde_iter");
+    aidAbsorb(r.stack);
+    return r;
+  }
+  static void checkIter(const msckf_b200_aid_iter& iter) {
+    if (iter.max_iter < 0 || iter.max_iter > 16) throw std::invalid_argument("MSCKF::aidedUpdate: iter.max_iter outside 0..16");
+    if (!(std::isfinite(iter.tol) && iter.tol >= 0.0)) throw std::invalid_argument("MSCKF::aidedUpdate: iter.tol must be finite and >= 0");
+  }
   // v_I: the IMU's velocity in its own frame (wheel or leg odometry); mask bits 0..2 select the rows used, R is popcount(mask)
   // square over them.  mask 0b110 with v_I = 0 is the non-holonomic constraint v_y = v_z = 0.
   msckf_b200_aid_result bodyVelocityUpdate(const Vector3<double>& v_I, const MatrixX<double>& R, int mask = 7, double chi2_max = 0) {
@@ -1152,6 +1179,38 @@ class MSCKFBatch {
       if (!items[i].empty()) filters_[i]->aidAbsorb(r[i].stack);
     return r;
   }
+  // MSCKF::aidedUpdate(items, chi2_max, iter[i], iter_out[i]) of every filter (items[i] empty: filter i is left alone, iter[i]
+  // not read) as one msckf_b200_batch_aid_stack_update_iter: one launch per 32 updated filters and one synchronisation.
+  std::vector<msckf_b200_aid_result> aidedUpdate(const std::vector<std::vector<msckf_b200_aid_item>>& items, double chi2_max,
+                                                 const std::vector<msckf_b200_aid_iter>& iter,
+                                                 std::vector<msckf_b200_aid_iter_result>& iter_out) {
+    std::vector<const msckf_b200_aid_item*> p;
+    std::vector<int> k;
+    iterArgs(items, iter, p, k, iter_out);
+    std::vector<msckf_b200_aid_result> r(size(), msckf_b200_aid_result());
+    const int rc = msckf_b200_batch_aid_stack_update_iter(batch_, p.data(), k.data(), chi2_max, iter.data(), r.data(), iter_out.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch stacked aided update (iterated): " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_stack_update_iter");
+    for (size_t i = 0; i < size(); ++i)
+      if (!items[i].empty()) filters_[i]->aidAbsorb(r[i]);
+    return r;
+  }
+  // the same with fault detection and exclusion, one fde for the batch (msckf_b200_batch_aid_stack_update_fde_iter)
+  std::vector<msckf_b200_aid_fde_result> aidedUpdate(const std::vector<std::vector<msckf_b200_aid_item>>& items, const msckf_b200_aid_fde& fde,
+                                                     const std::vector<msckf_b200_aid_iter>& iter,
+                                                     std::vector<msckf_b200_aid_iter_result>& iter_out) {
+    MSCKF<_S>::checkFde(fde);
+    std::vector<const msckf_b200_aid_item*> p;
+    std::vector<int> k;
+    iterArgs(items, iter, p, k, iter_out);
+    std::vector<msckf_b200_aid_fde_result> r(size(), msckf_b200_aid_fde_result());
+    const int rc = msckf_b200_batch_aid_stack_update_fde_iter(batch_, p.data(), k.data(), &fde, iter.data(), r.data(), iter_out.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch stacked aided update (FDE, iterated): " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_aid_stack_update_fde_iter");
+    for (size_t i = 0; i < size(); ++i)
+      if (!items[i].empty()) filters_[i]->aidAbsorb(r[i].stack);
+    return r;
+  }
   // MSCKF::landmarkUpdate of every filter (obs[i] empty: filter i is left alone) as one msckf_b200_batch_landmark_update: three
   // launches per 32 updated filters and one synchronisation.  gamma / flag (optional) receive one list per filter.  An unknown
   // state_id throws before any device call.  result[i] of a filter left alone is value-initialised.  max_iter / tol: the
@@ -1218,6 +1277,23 @@ class MSCKFBatch {
   std::vector<std::vector<int>> keep_;
   msckf_b200_batch* batch_ = nullptr;
   int threads_ = 1;
+
+  // the iterated batch forms' arguments: one item list and one iter per filter (each updated filter's iter checked as
+  // MSCKF::aidedUpdate does), the item pointers and counts, iter_out sized; then the IMU queues are handed over
+  void iterArgs(const std::vector<std::vector<msckf_b200_aid_item>>& items, const std::vector<msckf_b200_aid_iter>& iter,
+                std::vector<const msckf_b200_aid_item*>& p, std::vector<int>& k, std::vector<msckf_b200_aid_iter_result>& iter_out) {
+    const size_t n = size();
+    if (items.size() != n || iter.size() != n) throw std::invalid_argument("MSCKFBatch::aidedUpdate: one item list and one iter per filter");
+    p.assign(n, nullptr);
+    k.assign(n, 0);
+    for (size_t i = 0; i < n; ++i) {
+      if (!items[i].empty()) MSCKF<_S>::checkIter(iter[i]);
+      p[i] = items[i].empty() ? nullptr : items[i].data();
+      k[i] = (int)items[i].size();
+    }
+    iter_out.assign(n, msckf_b200_aid_iter_result());
+    flushImu();
+  }
 
   // the IMU readings queued on every filter, as one msckf_b200_batch_propagate_n
   void flushImu() {

@@ -92,6 +92,21 @@ int msckf_mono_aid_stack_update_fde(void* h, const msckf_b200_aid_item* items, i
                                     msckf_b200_aid_fde_result* out);
 int msckf_mono_batch_aid_stack_update_fde(void* batch, const int* n_items, const msckf_b200_aid_item* items,
                                           const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out);
+/* the same stacks iterated (MSCKF::aidedUpdate(items, chi2_max | fde, iter, iter_out), msckf_b200_aid_stack_update_iter /
+ * _fde_iter: iteration, results and errors there); the batch forms take iter[i] and fill iter_out[i] per filter (not read or
+ * written for a filter left alone).  A NULL iter or iter_out, max_iter outside 0..16 or a tol that is not finite and >= 0
+ * fails before any device call. */
+int msckf_mono_aid_stack_update_iter(void* h, const msckf_b200_aid_item* items, int n_items, double chi2_max,
+                                     const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out, msckf_b200_aid_iter_result* iter_out);
+int msckf_mono_aid_stack_update_fde_iter(void* h, const msckf_b200_aid_item* items, int n_items, const msckf_b200_aid_fde* fde,
+                                         const msckf_b200_aid_iter* iter, msckf_b200_aid_fde_result* out,
+                                         msckf_b200_aid_iter_result* iter_out);
+int msckf_mono_batch_aid_stack_update_iter(void* batch, const int* n_items, const msckf_b200_aid_item* items, double chi2_max,
+                                           const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out,
+                                           msckf_b200_aid_iter_result* iter_out);
+int msckf_mono_batch_aid_stack_update_fde_iter(void* batch, const int* n_items, const msckf_b200_aid_item* items,
+                                               const msckf_b200_aid_fde* fde, const msckf_b200_aid_iter* iter,
+                                               msckf_b200_aid_fde_result* out, msckf_b200_aid_iter_result* iter_out);
 int msckf_mono_body_velocity_update(void* h, const double* v3, int mask, const double* R, double chi2_max, msckf_b200_aid_result* out);
 int msckf_mono_relative_pose_update(void* h, int state_id_a, int state_id_b, const double* p3, const double* q4, const double* R36,
                                     double chi2_max, msckf_b200_aid_result* out);

@@ -113,6 +113,25 @@ class AidFdeResult(C.Structure):
         return d
 
 
+class AidIter(C.Structure):
+    _fields_ = [("max_iter", C.c_int), ("tol", C.c_double)]
+
+
+class AidIterResult(C.Structure):
+    _fields_ = [("iterations", C.c_int), ("converged", C.c_int), ("step", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def aid_iter_structs(n, max_iter, tol):
+    """n msckf_b200_aid_iter of max_iter / tol, each a number or a sequence of n (None: 0)"""
+    per = lambda v: list(v) if isinstance(v, (list, tuple, np.ndarray)) else [v] * n  # noqa: E731
+    mi, tl = per(max_iter), per(tol)
+    assert len(mi) == n and len(tl) == n
+    return (AidIter * n)(*[AidIter(int(a or 0), float(b or 0.0)) for a, b in zip(mi, tl)])
+
+
 def fde_thresholds(alpha):
     """chi2[d - 1] = the chi-square quantile 1 - alpha of d dof, d = 1..32 (the thresholds of msckf_b200_aid_fde)"""
     from scipy.stats import chi2
@@ -361,22 +380,40 @@ class Batch:
         check(lib().msckf_b200_batch_aid_update(self.h, (Aid * n)(*[a for a, _ in st]), out), "msckf_b200_batch_aid_update")
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
-    def aid_stack_update(self, stacks, chi2_max=0.0, fde=None):
+    def aid_stack_update(self, stacks, chi2_max=0.0, fde=None, max_iter=None, tol=None):
         """msckf_b200_batch_aid_stack_update: stacks[i] = list of item dicts for engine i (see aid_items; None or [] leaves
         engine i alone); a list of result dicts (None for an engine left alone).  fde (see fde_struct):
-        msckf_b200_batch_aid_stack_update_fde instead (chi2_max unused); each dict then has outcome, n_excluded and items"""
+        msckf_b200_batch_aid_stack_update_fde instead (chi2_max unused); each dict then has outcome, n_excluded and items.
+        max_iter / tol (a number for every engine or one per engine; see Engine.aid_stack_update): the _iter forms, and each
+        dict also has iterations, converged and step"""
         n = len(self.engines)
         assert len(stacks) == n
         st = [aid_items(s or []) for s in stacks]
         ptrs = (C.POINTER(AidItem) * n)(*[C.cast(a, C.POINTER(AidItem)) for a, _ in st])
         cnt = (C.c_int * n)(*[len(s or []) for s in stacks])
+        it = None if max_iter is None and tol is None else aid_iter_structs(n, max_iter, tol)
+        iout = (AidIterResult * n)()
         if fde is not None:
             f, out = fde_struct(fde), (AidFdeResult * n)()
-            check(lib().msckf_b200_batch_aid_stack_update_fde(self.h, ptrs, cnt, C.byref(f), out), "msckf_b200_batch_aid_stack_update_fde")
-            return [o.as_dict(len(s)) if s else None for s, o in zip(stacks, out)]
-        out = (AidResult * n)()
-        check(lib().msckf_b200_batch_aid_stack_update(self.h, ptrs, cnt, C.c_double(chi2_max), out), "msckf_b200_batch_aid_stack_update")
-        return [o.as_dict() if s else None for s, o in zip(stacks, out)]
+            if it is None:
+                check(lib().msckf_b200_batch_aid_stack_update_fde(self.h, ptrs, cnt, C.byref(f), out), "msckf_b200_batch_aid_stack_update_fde")
+            else:
+                check(lib().msckf_b200_batch_aid_stack_update_fde_iter(self.h, ptrs, cnt, C.byref(f), it, out, iout),
+                      "msckf_b200_batch_aid_stack_update_fde_iter")
+            res = [o.as_dict(len(s)) if s else None for s, o in zip(stacks, out)]
+        else:
+            out = (AidResult * n)()
+            if it is None:
+                check(lib().msckf_b200_batch_aid_stack_update(self.h, ptrs, cnt, C.c_double(chi2_max), out), "msckf_b200_batch_aid_stack_update")
+            else:
+                check(lib().msckf_b200_batch_aid_stack_update_iter(self.h, ptrs, cnt, C.c_double(chi2_max), it, out, iout),
+                      "msckf_b200_batch_aid_stack_update_iter")
+            res = [o.as_dict() if s else None for s, o in zip(stacks, out)]
+        if it is not None:
+            for r, o in zip(res, iout):
+                if r is not None:
+                    r.update(o.as_dict())
+        return res
 
     def landmark_update(self, specs, max_iter=None, tol=None):
         """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
@@ -532,19 +569,36 @@ class Engine:
         check(lib().msckf_b200_aid_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_aid_update")
         return out.as_dict()
 
-    def aid_stack_update(self, items, chi2_max=0.0, fde=None):
+    def aid_stack_update(self, items, chi2_max=0.0, fde=None, max_iter=None, tol=None):
         """msckf_b200_aid_stack_update: one stacked update of items (see aid_items); the result as a dict.  fde (see
-        fde_struct): msckf_b200_aid_stack_update_fde instead (chi2_max unused); the dict then has outcome, n_excluded and items"""
+        fde_struct): msckf_b200_aid_stack_update_fde instead (chi2_max unused); the dict then has outcome, n_excluded and items.
+        max_iter (0..16; 0 or 1: one linearisation) / tol (finite, >= 0; None: 0): the iterated update
+        (msckf_b200_aid_stack_update_iter / _fde_iter); the dict then also has iterations, converged and step.  With neither
+        given the call is the one above."""
         arr, keep = aid_items(items)
+        it = None if max_iter is None and tol is None else aid_iter_structs(1, max_iter, tol)
+        iout = AidIterResult()
         if fde is not None:
             f, out = fde_struct(fde), AidFdeResult()
-            check(lib().msckf_b200_aid_stack_update_fde(self.h, arr, C.c_int(len(items)), C.byref(f), C.byref(out)),
-                  "msckf_b200_aid_stack_update_fde")
-            return out.as_dict(len(items))
-        out = AidResult()
-        check(lib().msckf_b200_aid_stack_update(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)),
-              "msckf_b200_aid_stack_update")
-        return out.as_dict()
+            if it is None:
+                check(lib().msckf_b200_aid_stack_update_fde(self.h, arr, C.c_int(len(items)), C.byref(f), C.byref(out)),
+                      "msckf_b200_aid_stack_update_fde")
+            else:
+                check(lib().msckf_b200_aid_stack_update_fde_iter(self.h, arr, C.c_int(len(items)), C.byref(f), it, C.byref(out),
+                                                                 C.byref(iout)), "msckf_b200_aid_stack_update_fde_iter")
+            res = out.as_dict(len(items))
+        else:
+            out = AidResult()
+            if it is None:
+                check(lib().msckf_b200_aid_stack_update(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)),
+                      "msckf_b200_aid_stack_update")
+            else:
+                check(lib().msckf_b200_aid_stack_update_iter(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), it,
+                                                             C.byref(out), C.byref(iout)), "msckf_b200_aid_stack_update_iter")
+            res = out.as_dict()
+        if it is not None:
+            res.update(iout.as_dict())
+        return res
 
     def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0, landmark=None, Sigma_L=None):
         """msckf_b200_landmark_update: observations of known landmarks p_L [n, 3] at z [n, 2] from window positions clone [n];

@@ -245,10 +245,13 @@ struct CtxBase {
   // aided measurement updates of the members (msckf_b200_aid_update / _batch_aid_update, and the stacked
   // msckf_b200_aid_stack_update / _batch_aid_stack_update): one launch per 32, one synchronisation
   virtual int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) = 0;
-  virtual int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) = 0;
+  // iter: the iterated form (msckf_b200_aid_stack_update_iter / ..._fde_iter and their batch forms), iter[i] and iout[i] per
+  // member; nullptr: one linearisation
+  virtual int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out,
+                        const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) = 0;
   // the stacked form with fault detection and exclusion over the items (msckf_b200_aid_stack_update_fde / _batch_..._fde)
   virtual int aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
-                            msckf_b200_aid_fde_result* out) = 0;
+                            msckf_b200_aid_fde_result* out, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) = 0;
   // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
   virtual int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) = 0;
   cudaStream_t stream = nullptr;
@@ -519,12 +522,15 @@ struct Ctx : CtxBase {
   int get_state(void* const* imu, void* const* poses) override;
   int nees(const double* const* truth_imu, const double* const* truth_poses, msckf_b200_nees_result* out) override;
   int aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) override;
-  int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) override;
+  int aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out,
+                const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) override;
   int aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
-                    msckf_b200_aid_fde_result* out) override;
-  int aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job);
+                    msckf_b200_aid_fde_result* out, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) override;
+  int aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job,
+                     const msckf_b200_aid_iter* iter);
   int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what, const msckf_b200_aid_fde* fde = nullptr,
-              msckf_b200_aid_fde_result* fout = nullptr);
+              msckf_b200_aid_fde_result* fout = nullptr, const msckf_b200_aid_iter* iter = nullptr,
+              msckf_b200_aid_iter_result* iout = nullptr);
   int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
@@ -601,6 +607,10 @@ struct Engine : EngineBase {
     CK(cudaFuncSetAttribute(mb::k_aid<S, mb::kBatchMembers>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
     CK(cudaFuncSetAttribute(mb::k_aid<S, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
     CK(cudaFuncSetAttribute(mb::k_aid<S, mb::kBatchMembers, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid_iter<S, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid_iter<S, mb::kBatchMembers>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid_iter<S, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
+    CK(cudaFuncSetAttribute(mb::k_aid_iter<S, mb::kBatchMembers, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAidSmemMax));
     done[dev] = true;
     return 0;
   }
@@ -1567,33 +1577,38 @@ int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
 }
 
 template <class S>
-int Ctx<S>::aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out) {
-  if (!items || !n_items || !out) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: null argument");
-  RC(members_ready("aid_stack_update"));
-  if (std::isnan(chi2_max)) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: chi2_max is NaN");
+int Ctx<S>::aid_stack(const msckf_b200_aid_item* const* items, const int* n_items, double chi2_max, msckf_b200_aid_result* out,
+                      const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) {
+  const char* w = iter ? "aid_stack_update_iter" : "aid_stack_update";
+  if (!items || !n_items || !out) return fail(MSCKF_B200_ERR_ARG, std::string(w) + ": null argument");
+  RC(members_ready(w));
+  if (std::isnan(chi2_max)) return fail(MSCKF_B200_ERR_ARG, std::string(w) + ": chi2_max is NaN");
   std::vector<AidJob> job;
-  RC(aid_stack_jobs(items, n_items, "aid_stack_update", job));
+  RC(aid_stack_jobs(items, n_items, w, job, iter));
   for (AidJob& j : job) j.chi2_max = chi2_max;
-  return aid_run(job, out, "aid_stack_update");
+  return aid_run(job, out, w, nullptr, nullptr, iter, iout);
 }
 
 template <class S>
 int Ctx<S>::aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
-                          msckf_b200_aid_fde_result* out) {
-  if (!items || !n_items || !fde || !out) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: null argument");
-  RC(members_ready("aid_stack_update_fde"));
+                          msckf_b200_aid_fde_result* out, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) {
+  const std::string w = iter ? "aid_stack_update_fde_iter" : "aid_stack_update_fde";
+  if (!items || !n_items || !fde || !out) return fail(MSCKF_B200_ERR_ARG, w + ": null argument");
+  RC(members_ready(w.c_str()));
   for (int d = 0; d < mb::kAidMaxRows; ++d)
     if (!(std::isfinite(fde->chi2[d]) && fde->chi2[d] > 0.0))
-      return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: chi2[" + std::to_string(d) + "] is not finite and > 0");
-  if (fde->max_exclude < 0 || fde->max_exclude > mb::kAidMaxItems - 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: max_exclude outside 0..7");
+      return fail(MSCKF_B200_ERR_ARG, w + ": chi2[" + std::to_string(d) + "] is not finite and > 0");
+  if (fde->max_exclude < 0 || fde->max_exclude > mb::kAidMaxItems - 1) return fail(MSCKF_B200_ERR_ARG, w + ": max_exclude outside 0..7");
   std::vector<AidJob> job;
-  RC(aid_stack_jobs(items, n_items, "aid_stack_update_fde", job));
-  return aid_run(job, nullptr, "aid_stack_update_fde", fde, out);
+  RC(aid_stack_jobs(items, n_items, w, job, iter));
+  return aid_run(job, nullptr, w.c_str(), fde, out, iter, iout);
 }
 
-// one AidJob per member of a stacked call (n_items[i] = 0: member i is left alone); 0, or MSCKF_B200_ERR_ARG
+// one AidJob per member of a stacked call (n_items[i] = 0: member i is left alone), iter[i] checked for the members updated
+// (iter given); 0, or MSCKF_B200_ERR_ARG
 template <class S>
-int Ctx<S>::aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job) {
+int Ctx<S>::aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job,
+                           const msckf_b200_aid_iter* iter) {
   const int nf = (int)eng.size();
   job.assign(nf, AidJob{});
   for (int i = 0; i < nf; ++i) {
@@ -1601,6 +1616,9 @@ int Ctx<S>::aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n
     const std::string who = " (member " + std::to_string(i) + ")";
     if (n_items[i] < 0 || n_items[i] > mb::kAidMaxItems) return fail(MSCKF_B200_ERR_ARG, w + ": 1 to 8 items per stack" + who);
     if (!items[i]) return fail(MSCKF_B200_ERR_ARG, w + ": null item list" + who);
+    if (iter && (iter[i].max_iter < 0 || iter[i].max_iter > mb::kAidMaxIter))
+      return fail(MSCKF_B200_ERR_ARG, w + ": max_iter outside 0..16" + who);
+    if (iter && !(std::isfinite(iter[i].tol) && iter[i].tol >= 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": tol is not finite and >= 0" + who);
     for (int k = 0; k < n_items[i]; ++k)
       RC(aid_append(job[i], items[i][k], eng[i]->M, w, " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")"));
   }
@@ -1609,9 +1627,11 @@ int Ctx<S>::aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n
 
 template <class S>
 int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what, const msckf_b200_aid_fde* fde,
-                    msckf_b200_aid_fde_result* fout) {
+                    msckf_b200_aid_fde_result* fout, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) {
   const int nf = (int)eng.size();
-  const size_t osz = fde ? sizeof(mb::AidFdeOut) : sizeof(mb::AidOut);  // FDE: the item block follows the plain result
+  // FDE: the item block follows the plain result; iter: then AidIterOut
+  const size_t obase = fde ? sizeof(mb::AidFdeOut) : sizeof(mb::AidOut), osz = obase + (iter ? sizeof(mb::AidIterOut) : 0);
+  const size_t in_tail = (fde ? mb::kAidFdeIn : 0) + (iter ? 2 : 0);  // doubles after R (and H)
   std::vector<int> idx;
   std::vector<size_t> off(nf + 1, 0), woff(nf + 1, 0);
   for (int i = 0; i < nf; ++i) {
@@ -1620,7 +1640,7 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
     woff[i + 1] = woff[i];
     if (job[i].n_items == 0) continue;
     idx.push_back(i);
-    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (job[i].H ? (size_t)m * n : 0) + (fde ? mb::kAidFdeIn : 0)));
+    off[i + 1] = off[i] + up16(sizeof(double) * (mb::kAidZ + (size_t)m * m + (job[i].H ? (size_t)m * n : 0) + in_tail));
     if (mb::aid_ws_bytes(n, m) > kAidSmemMax) woff[i + 1] = woff[i] + up256(mb::aid_ws_bytes(n, m));
   }
   if (idx.empty()) return 0;
@@ -1644,6 +1664,10 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
       memcpy(R + m * m, fde->chi2, sizeof(double) * mb::kAidMaxRows);
       R[m * m + mb::kAidMaxRows] = fde->max_exclude;
     }
+    if (iter) {
+      double* t = R + m * m + (fde ? mb::kAidFdeIn : 0);
+      t[0] = iter[i].max_iter; t[1] = iter[i].tol;
+    }
   }
   CK(cudaMemcpyAsync(io.d, io.h, off[nf], cudaMemcpyHostToDevice, stream));
   per_member(idx, false,
@@ -1658,7 +1682,9 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
                size_t smem = 0;  // the largest need of the members whose W^T and dx are in shared memory
                for (int j = 0; j < nm; ++j)
                  if (!a.m[j].ws) smem = std::max(smem, mb::aid_ws_bytes(15 + 6 * a.m[j].M, a.m[j].m));
-               if (fde) mb::k_aid<S, NM, true><<<nm, mb::kAidThreads, smem, stream>>>(a);
+               if (fde && iter) mb::k_aid_iter<S, NM, true><<<nm, mb::kAidThreads, smem, stream>>>(a);
+               else if (fde) mb::k_aid<S, NM, true><<<nm, mb::kAidThreads, smem, stream>>>(a);
+               else if (iter) mb::k_aid_iter<S, NM><<<nm, mb::kAidThreads, smem, stream>>>(a);
                else mb::k_aid<<<nm, mb::kAidThreads, smem, stream>>>(a);
              });
   CK(cudaGetLastError());
@@ -1675,6 +1701,10 @@ int Ctx<S>::aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, 
       for (int k = 0; k < mb::kAidMaxItems; ++k)
         fout[i].item[k] = k < job[i].n_items ? msckf_b200_aid_item_result{g.item[k].nis, g.item[k].test, g.item[k].state, g.item[k].round}
                                              : msckf_b200_aid_item_result{std::nan(""), std::nan(""), -1, -1};
+    }
+    if (iter) {
+      const mb::AidIterOut& g = *reinterpret_cast<const mb::AidIterOut*>(io.h + res_off + osz * i + obase);
+      iout[i] = msckf_b200_aid_iter_result{g.iterations, g.converged, g.step};
     }
     if (o.numeric && numeric < 0) numeric = i;
   }
@@ -2116,12 +2146,24 @@ int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, 
 int msckf_b200_batch_aid_stack_update(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
                                       double chi2_max, msckf_b200_aid_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
-  return b->ctx->aid_stack(items, n_items, chi2_max, out);
+  return b->ctx->aid_stack(items, n_items, chi2_max, out, nullptr, nullptr);
+}
+int msckf_b200_batch_aid_stack_update_iter(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                           double chi2_max, const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out,
+                                           msckf_b200_aid_iter_result* iter_out) {
+  if (!b || !iter || !iter_out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->aid_stack(items, n_items, chi2_max, out, iter, iter_out);
 }
 int msckf_b200_batch_aid_stack_update_fde(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
                                           const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
-  return b->ctx->aid_stack_fde(items, n_items, fde, out);
+  return b->ctx->aid_stack_fde(items, n_items, fde, out, nullptr, nullptr);
+}
+int msckf_b200_batch_aid_stack_update_fde_iter(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
+                                               const msckf_b200_aid_fde* fde, const msckf_b200_aid_iter* iter,
+                                               msckf_b200_aid_fde_result* out, msckf_b200_aid_iter_result* iter_out) {
+  if (!b || !iter || !iter_out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->aid_stack_fde(items, n_items, fde, out, iter, iter_out);
 }
 int msckf_b200_batch_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
@@ -2171,13 +2213,26 @@ int msckf_b200_aid_stack_update(msckf_b200_engine* e, const msckf_b200_aid_item*
                                 msckf_b200_aid_result* out) {
   if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
   if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update: 1 to 8 items per stack");
-  return e->impl->solo_ctx()->aid_stack(&items, &n_items, chi2_max, out);
+  return e->impl->solo_ctx()->aid_stack(&items, &n_items, chi2_max, out, nullptr, nullptr);
+}
+int msckf_b200_aid_stack_update_iter(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,
+                                     const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out, msckf_b200_aid_iter_result* iter_out) {
+  if (!e || !iter || !iter_out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_iter: 1 to 8 items per stack");
+  return e->impl->solo_ctx()->aid_stack(&items, &n_items, chi2_max, out, iter, iter_out);
 }
 int msckf_b200_aid_stack_update_fde(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, const msckf_b200_aid_fde* fde,
                                     msckf_b200_aid_fde_result* out) {
   if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
   if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde: 1 to 8 items per stack");
-  return e->impl->solo_ctx()->aid_stack_fde(&items, &n_items, fde, out);
+  return e->impl->solo_ctx()->aid_stack_fde(&items, &n_items, fde, out, nullptr, nullptr);
+}
+int msckf_b200_aid_stack_update_fde_iter(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items,
+                                         const msckf_b200_aid_fde* fde, const msckf_b200_aid_iter* iter,
+                                         msckf_b200_aid_fde_result* out, msckf_b200_aid_iter_result* iter_out) {
+  if (!e || !iter || !iter_out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde_iter: 1 to 8 items per stack");
+  return e->impl->solo_ctx()->aid_stack_fde(&items, &n_items, fde, out, iter, iter_out);
 }
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   return msckf_b200_map_landmark_update(e, lm, nullptr, out);

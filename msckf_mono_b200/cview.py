@@ -141,23 +141,39 @@ class FilterBatch:
         self._call("aid_update", (Aid * n)(*[a for a, _ in st]), out)
         return [None if s is None or s["model"] < 0 else o.as_dict() for s, o in zip(specs, out)]
 
-    def aid_stack_update(self, stacks, chi2_max=0.0, fde=None):
+    def aid_stack_update(self, stacks, chi2_max=0.0, fde=None, max_iter=None, tol=None):
         """MSCKFBatch::aidedUpdate(items): stacks[i] = list of item dicts for filter i (as for capi.aid_items; None or []:
         filter i left alone); one device call for the batch.  A list of result dicts (None for a filter left alone).  fde (as for
-        capi.fde_struct): MSCKFBatch::aidedUpdate(items, fde) instead; each dict then has outcome, n_excluded and items."""
-        from .capi import AidFdeResult, AidResult, aid_items, fde_struct
+        capi.fde_struct): MSCKFBatch::aidedUpdate(items, fde) instead; each dict then has outcome, n_excluded and items.
+        max_iter / tol (a number for every filter or one per filter, as for capi.Batch.aid_stack_update): the iterated forms
+        (MSCKFBatch::aidedUpdate(items, chi2_max | fde, iter, iter_out)); each dict then also has iterations, converged, step."""
+        from .capi import AidFdeResult, AidIterResult, AidResult, aid_items, aid_iter_structs, fde_struct
         n = len(self.filters)
         assert len(stacks) == n
         flat = [it for s in stacks for it in (s or [])]
         arr, keep = aid_items(flat)
         cnt = np.array([len(s or []) for s in stacks], dtype=np.int32)
+        it = None if max_iter is None and tol is None else aid_iter_structs(n, max_iter, tol)
+        iout = (AidIterResult * n)()
         if fde is not None:
             f, out = fde_struct(fde), (AidFdeResult * n)()
-            self._call("aid_stack_update_fde", cnt.ctypes.data_as(_ip), arr, C.byref(f), out)
-            return [o.as_dict(len(s)) if s else None for s, o in zip(stacks, out)]
-        out = (AidResult * n)()
-        self._call("aid_stack_update", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), out)
-        return [o.as_dict() if s else None for s, o in zip(stacks, out)]
+            if it is None:
+                self._call("aid_stack_update_fde", cnt.ctypes.data_as(_ip), arr, C.byref(f), out)
+            else:
+                self._call("aid_stack_update_fde_iter", cnt.ctypes.data_as(_ip), arr, C.byref(f), it, out, iout)
+            res = [o.as_dict(len(s)) if s else None for s, o in zip(stacks, out)]
+        else:
+            out = (AidResult * n)()
+            if it is None:
+                self._call("aid_stack_update", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), out)
+            else:
+                self._call("aid_stack_update_iter", cnt.ctypes.data_as(_ip), arr, C.c_double(chi2_max), it, out, iout)
+            res = [o.as_dict() if s else None for s, o in zip(stacks, out)]
+        if it is not None:
+            for r, o in zip(res, iout):
+                if r is not None:
+                    r.update(o.as_dict())
+        return res
 
     def map_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
         """MSCKFBatch::landmarkUpdate over mapObservation / mapLandmark: obs[i] = (state_ids [n], landmark [n], z [n, 2],
@@ -390,19 +406,35 @@ class CFilter:
         self._chk(self._f("aid_update")(self.h, C.byref(a), C.byref(out)), "aid_update")
         return out.as_dict()
 
-    def aid_stack_update(self, items, chi2_max=0.0, fde=None):
+    def aid_stack_update(self, items, chi2_max=0.0, fde=None, max_iter=None, tol=None):
         """MSCKF::aidedUpdate(items) (include/msckf_b200.h: msckf_b200_aid_stack_update): items as for capi.aid_items, one
         chi2_max for the stack.  A dict nis, dx_norm, dof, applied, status.  fde (as for capi.fde_struct):
-        MSCKF::aidedUpdate(items, fde) (msckf_b200_aid_stack_update_fde) instead; the dict then has outcome, n_excluded, items."""
-        from .capi import AidFdeResult, AidResult, aid_items, fde_struct
+        MSCKF::aidedUpdate(items, fde) (msckf_b200_aid_stack_update_fde) instead; the dict then has outcome, n_excluded, items.
+        max_iter / tol (as for capi.Engine.aid_stack_update): MSCKF::aidedUpdate(items, chi2_max | fde, iter, iter_out)
+        (msckf_b200_aid_stack_update_iter / _fde_iter); the dict then also has iterations, converged and step."""
+        from .capi import AidFdeResult, AidIterResult, AidResult, aid_items, aid_iter_structs, fde_struct
         arr, keep = aid_items(items)
+        it = None if max_iter is None and tol is None else aid_iter_structs(1, max_iter, tol)
+        iout = AidIterResult()
         if fde is not None:
             f, out = fde_struct(fde), AidFdeResult()
-            self._chk(self._f("aid_stack_update_fde")(self.h, arr, C.c_int(len(items)), C.byref(f), C.byref(out)), "aid_stack_update_fde")
-            return out.as_dict(len(items))
-        out = AidResult()
-        self._chk(self._f("aid_stack_update")(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)), "aid_stack_update")
-        return out.as_dict()
+            if it is None:
+                self._chk(self._f("aid_stack_update_fde")(self.h, arr, C.c_int(len(items)), C.byref(f), C.byref(out)), "aid_stack_update_fde")
+            else:
+                self._chk(self._f("aid_stack_update_fde_iter")(self.h, arr, C.c_int(len(items)), C.byref(f), it, C.byref(out), C.byref(iout)),
+                          "aid_stack_update_fde_iter")
+            res = out.as_dict(len(items))
+        else:
+            out = AidResult()
+            if it is None:
+                self._chk(self._f("aid_stack_update")(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), C.byref(out)), "aid_stack_update")
+            else:
+                self._chk(self._f("aid_stack_update_iter")(self.h, arr, C.c_int(len(items)), C.c_double(chi2_max), it, C.byref(out),
+                                                            C.byref(iout)), "aid_stack_update_iter")
+            res = out.as_dict()
+        if it is not None:
+            res.update(iout.as_dict())
+        return res
 
     def body_velocity_update(self, v_I, R, mask=7, chi2_max=0.0):
         """MSCKF::bodyVelocityUpdate: the IMU's velocity v_I in its own frame, rows selected by mask (bits 0..2), R over them"""

@@ -416,7 +416,7 @@ def map_observations(truth, frame, stride):
 
 
 def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_stride=20, odo_every=0, map_start=0, map_sigma=0.0,
-               map_clones=1, gnss_every=0, heading_every=0, range_every=0, plane_every=0):
+               map_clones=1, gnss_every=0, heading_every=0, range_every=0, plane_every=0, range_start=0, gnss_start=0):
     """trial k's inputs: the truth stream with noise drawn from the filter's model; records the injected noise.  With
     fix_every > 0, "fixes" holds per frame None or the noisy position fix z = p_true + N(0, fix_sigma^2 I).  With
     map_every > 0, "maps" holds per frame None or (map indices, p_L [n, 3], noisy z [n, 2]) of the visible map landmarks, None
@@ -430,7 +430,9 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
     from np.random.default_rng([seed, k, 6]); with heading_every > 0, "heading" holds None or 1 standard normal, from
     np.random.default_rng([seed, k, 7]) (gnss_items).  With range_every > 0, "range" holds per frame None or one standard normal
     per anchor of ANCHORS, from np.random.default_rng([seed, k, 8]); with plane_every > 0, "plane" holds None or 1 standard
-    normal, from np.random.default_rng([seed, k, 9]) (range_items)."""
+    normal, from np.random.default_rng([seed, k, 9]) (range_items).  range_start / gnss_start > 0: the "range" and "plane" /
+    "gnss" and "heading" entries of the epochs before that frame are None (their noise is still drawn, so an epoch's noise is the
+    same for every start)."""
     rng = np.random.default_rng([seed, k])
     nz = truth["noise"]
     Q = np.asarray(nz["Q_imu"], dtype=np.float64)
@@ -504,6 +506,9 @@ def make_trial(truth, k, seed=0, fix_every=0, fix_sigma=1.0, map_every=0, map_st
     if plane_every > 0:
         prng = np.random.default_rng([seed, k, 9])
         out["plane"] = [prng.standard_normal(1) if (f + 1) % plane_every == 0 else None for f in range(len(truth["frames"]))]
+    for key, start in (("gnss", gnss_start), ("heading", gnss_start), ("range", range_start), ("plane", range_start)):
+        if key in out and start > 0:
+            out[key] = [None if f < start else x for f, x in enumerate(out[key])]
     return out
 
 
@@ -515,16 +520,18 @@ def truth_imu_of(truth, trial, frame):
 
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
-def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None, gnss_rows=None, range_rows=None):
+def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None, gnss_rows=None, range_rows=None,
+                 range_first=None, gnss_first=None):
     """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes, of its
     map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n) and of its odometry
     stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists; map_first (a dict of plain numbers: frame,
     squared position error before and after, nis, dof, iterations, converged) describes the first map update; gnss_rows
     (result dicts of aid_stack_update, dof 0 for an epoch whose clone had left the window) the GNSS stacks, range_rows (the
-    same) the ranging stacks"""
+    same) the ranging stacks; range_first / gnss_first (as map_first) the first ranging / GNSS stack"""
     rec = _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows)
-    if map_first is not None:
-        rec["map_first"] = dict(map_first)
+    for key, first in (("map_first", map_first), ("range_first", range_first), ("gnss_first", gnss_first)):
+        if first is not None:
+            rec[key] = dict(first)
     for key, rows in (("gnss", gnss_rows), ("range", range_rows)):
         if rows is not None:
             rec[key] = {k: [float(r[k]) if k == "nis" else int(r[k]) for r in rows] for k in ("nis", "dof", "applied", "status")}
@@ -613,18 +620,21 @@ def summarize(records):
                       "run_bounds": list(tot), "updates_inside": float(np.mean(inside)),
                       "applied": float(np.mean([a for m in mp for a in m["applied"]])),
                       "observations": int(n_obs), "gated": float(1.0 - sum(sum(m["used"]) for m in mp) / max(n_obs, 1))}
-    mf = [records[k].get("map_first") for k in keys]
-    if all(m is not None for m in mf):  # the first map update: position error before / after, its ANIS, the IMU-state ANEES after
+    for key in ("map_first", "range_first", "gnss_first"):
+        mf = [records[k].get(key) for k in keys]
+        if not all(m is not None for m in mf):
+            continue
+        # the first map update, ranging or GNSS stack: position error before / after, its ANIS, the IMU-state ANEES after
         f0 = mf[0]["frame"]
         d = int(sum(m["dof"] for m in mf))
         imu = out["components"]["imu"]
-        out["map_first"] = {"frame": int(f0), "pos_rmse_before": float(np.sqrt(np.mean([m["pos_err2_before"] for m in mf]))),
-                            "pos_rmse_after": float(np.sqrt(np.mean([m["pos_err2_after"] for m in mf]))),
-                            "anis": float(sum(m["nis"] for m in mf) / N), "mean_dof": d / N,
-                            "bounds": list(chi2_bounds(d, N)) if d > 0 else [float("nan")] * 2,
-                            "imu_anees": imu["anees"][f0], "imu_bounds": [imu["lower"][f0], imu["upper"][f0]],
-                            "iterations": float(np.mean([m["iterations"] for m in mf])),
-                            "converged": float(np.mean([m["converged"] for m in mf]))}
+        out[key] = {"frame": int(f0), "pos_rmse_before": float(np.sqrt(np.mean([m["pos_err2_before"] for m in mf]))),
+                    "pos_rmse_after": float(np.sqrt(np.mean([m["pos_err2_after"] for m in mf]))),
+                    "anis": float(sum(m["nis"] for m in mf) / N), "mean_dof": d / N,
+                    "bounds": list(chi2_bounds(d, N)) if d > 0 else [float("nan")] * 2,
+                    "imu_anees": imu["anees"][f0], "imu_bounds": [imu["lower"][f0], imu["upper"][f0]],
+                    "iterations": float(np.mean([m["iterations"] for m in mf])),
+                    "converged": float(np.mean([m["converged"] for m in mf]))}
     od = [records[k].get("odometry") for k in keys]
     if all(o is not None and len(o["nis"]) for o in od):  # ANIS of the odometry stacks: the stack's rows per trial and update
         V = np.array([o["nis"] for o in od]); D = np.array([o["dof"] for o in od])
@@ -678,12 +688,13 @@ def map_call(tr, f, fi, uncertain, S):
     return ids, inv, z, p[first], np.repeat(S, len(u), axis=0)
 
 
-def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items, faults=None, fde=None):
+def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items, faults=None, fde=None, iterate=None):
     """one batched stack per filter of the epoch g = f - delay when a trial input of `keys` (two noise lists of make_trial) has
     noise there: items(g, noise of keys[0], noise of keys[1], clone) with clone None at delay 0, else the window position of
     the epoch's clone; a filter whose epoch clone has left the window sends nothing and records dof 0.  faults(i, g, items), when
     given, makes some of filter i's items faulty in place and returns their indices (kept as the row's "faults"); fde, when
-    given, sends the stacks through fault detection and exclusion.  Appends each filter's result to out[i]."""
+    given, sends the stacks through fault detection and exclusion; iterate (max_iter, tol), when given, iterates them.  Appends
+    each filter's result to out[i]."""
     noise = [tuple(tr[key][g] if key in tr else None for key in keys) for tr in trs] if g >= 0 else []
     if g < 0 or not any(x is not None for x in noise[0]):
         return
@@ -698,7 +709,8 @@ def _epoch_stacks(fb, fs, trs, g, delay, keys, out, items, faults=None, fde=None
             clone = ids.index(tr["frames"][g]["state_id"])
         stacks.append(items(g, n_a, n_b, clone))
     bad = [faults(i, g, s) if faults is not None and s is not None else [] for i, s in enumerate(stacks)]
-    for i, r in enumerate(fb.aid_stack_update(stacks) if fde is None else fb.aid_stack_update(stacks, fde=fde)):
+    kw = {} if iterate is None else {"max_iter": iterate[0], "tol": iterate[1]}
+    for i, r in enumerate(fb.aid_stack_update(stacks, **kw) if fde is None else fb.aid_stack_update(stacks, fde=fde, **kw)):
         out[i].append({"nis": 0.0, "dof": 0, "applied": 0, "status": 0} if r is None else dict(r, faults=bad[i]))
 
 
@@ -708,7 +720,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         gnss_as_position=False, heading_every=0, heading_sigma=0.01, heading_axis=(1.0, 0.0, 0.0), range_every=0, range_sigma=0.1,
         range_lever=(0.0, 0.0, 0.0), range_delay=0, plane_every=0, plane_sigma=0.02, plane_height=PLANE_HEIGHT, plane_axis=PLANE_AXIS,
         plane_lever=(0.0, 0.0, 0.0), range_outlier_rate=0.0, range_outlier_bias=1.0, gnss_outlier_rate=0.0, gnss_outlier_jump=5.0,
-        fde_alpha=0.0, fde_max_exclude=2):
+        fde_alpha=0.0, fde_max_exclude=2, range_start=0, gnss_start=0, aid_iterations=1, aid_tol=1e-10):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
@@ -722,7 +734,9 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     stream default_rng([seed, k, 10]) per frame, and each antenna fix moved gnss_outlier_jump m horizontally in a random
     direction with probability gnss_outlier_rate, from [seed, k, 11]; fde_alpha > 0 sends the GNSS and ranging stacks through
     fault detection and exclusion with thresholds capi.fde_thresholds(fde_alpha) and fde_max_exclude (0: the stack gate only),
-    fde_alpha = 0 fuses them ungated],
+    fde_alpha = 0 fuses them ungated; range_start / gnss_start > 0 fuse no ranging / GNSS epoch before that frame (the first
+    one after it is also recorded on its own, as range_first / gnss_first in trial_record); aid_iterations K > 1 iterates the
+    GNSS, ranging and odometry stacks (at most K linearisations, converged at a step <= aid_tol)],
     [every map_every frames from frame map_start on, one batched mapped-landmark update from the newest clone, gated per
     observation at map_chi2 > 0, iterated up to map_iterations linearisations; the map carries N(0, map_sigma^2 I) errors and
     is observed from the map_clones newest clones that are still in the window (make_trial); map_uncertain passes
@@ -737,7 +751,10 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     assert not map_uncertain or map_sigma > 0, "map_uncertain needs map_sigma > 0"
     assert not (gnss_as_position and gnss_delay), "gnss_as_position fuses at the IMU: no delay"
     trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start, map_sigma, map_clones,
-                      gnss_every, heading_every, range_every, plane_every) for k in trials]
+                      gnss_every, heading_every, range_every, plane_every, range_start=range_start, gnss_start=gnss_start)
+           for k in trials]
+    iterate = None if aid_iterations == 1 else (int(aid_iterations), float(aid_tol))
+    it_kw = {} if iterate is None else {"max_iter": iterate[0], "tol": iterate[1]}
     gnss = [[] for _ in trs] if gnss_every > 0 or heading_every > 0 else None
     ranging = [[] for _ in trs] if range_every > 0 or plane_every > 0 else None
     lever, axis = np.asarray(gnss_lever, dtype=np.float64), np.asarray(heading_axis, dtype=np.float64)
@@ -779,6 +796,23 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         fde = {"chi2": fde_thresholds(fde_alpha), "max_exclude": int(fde_max_exclude)}
     S_map = np.tile([map_sigma ** 2, 0.0, map_sigma ** 2, 0.0, 0.0, map_sigma ** 2], (1, 1))
     first = [None for _ in trs]
+    first_r = [None for _ in trs] if range_start > 0 else None
+    first_g = [None for _ in trs] if gnss_start > 0 else None
+
+    def first_stack(first_x, rows, fi, g, keys, send):
+        """send an epoch's stacks; the first one sent is also recorded on its own (the state read just before it)"""
+        now = first_x is not None and first_x[0] is None and g >= 0 and any(trs[0][k][g] is not None for k in keys if k in trs[0])
+        if now:
+            fb.refreshState()
+            for i, (f, tr) in enumerate(zip(fs, trs)):
+                first_x[i] = {"frame": fi, "pos_err2_before": float(np.sum((truth_imu_of(truth, tr, fi)[0:3] - f.getImuState()["p_I_G"]) ** 2))}
+        send()
+        if now:
+            for i in range(len(trs)):
+                r = rows[i][-1]
+                first_x[i].update(nis=float(r["nis"]), dof=int(r["dof"]), iterations=int(r.get("iterations", r["applied"])),
+                                  converged=int(r.get("converged", 0)))
+
     R_fix = (fix_sigma ** 2) * np.eye(3)
     nis = [[] for _ in trs]
     maps = [[] for _ in trs]
@@ -813,18 +847,20 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
                 if len(items) > 1:
                     items[1].update(a=len(ids) - 2, b=len(ids) - 1)
                 stacks.append(items)
-            for i, r in enumerate(fb.aid_stack_update(stacks)):
+            for i, r in enumerate(fb.aid_stack_update(stacks, **it_kw)):
                 odo[i].append(r)
         if gnss is not None:  # the epoch whose GNSS output arrives at this frame
-            _epoch_stacks(fb, fs, trs, fi - gnss_delay, gnss_delay, ("gnss", "heading"), gnss,
-                          lambda g, n_p, n_psi, clone: gnss_items(truth["truth_imu"][g], truth["camera"], n_p, n_psi, gnss_sigma, lever,
-                                                                  heading_sigma, axis, clone, gnss_as_position),
-                          gnss_faults if gnss_outlier_rate > 0 else None, fde)
+            first_stack(first_g, gnss, fi, fi - gnss_delay, ("gnss", "heading"), lambda: _epoch_stacks(
+                fb, fs, trs, fi - gnss_delay, gnss_delay, ("gnss", "heading"), gnss,
+                lambda g, n_p, n_psi, clone: gnss_items(truth["truth_imu"][g], truth["camera"], n_p, n_psi, gnss_sigma, lever,
+                                                        heading_sigma, axis, clone, gnss_as_position),
+                gnss_faults if gnss_outlier_rate > 0 else None, fde, iterate))
         if ranging is not None:  # the epoch whose ranges arrive at this frame
-            _epoch_stacks(fb, fs, trs, fi - range_delay, range_delay, ("range", "plane"), ranging,
-                          lambda g, n_r, n_h, clone: range_items(truth["truth_imu"][g], truth["camera"], n_r, n_h, range_sigma, r_lever,
-                                                                 plane_sigma, plane_height, p_lever, p_axis, clone),
-                          range_faults if range_outlier_rate > 0 else None, fde)
+            first_stack(first_r, ranging, fi, fi - range_delay, ("range", "plane"), lambda: _epoch_stacks(
+                fb, fs, trs, fi - range_delay, range_delay, ("range", "plane"), ranging,
+                lambda g, n_r, n_h, clone: range_items(truth["truth_imu"][g], truth["camera"], n_r, n_h, range_sigma, r_lever,
+                                                       plane_sigma, plane_height, p_lever, p_axis, clone),
+                range_faults if range_outlier_rate > 0 else None, fde, iterate))
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [map_call(tr, f, fi, map_uncertain, S_map) for tr, f in zip(trs, fs)]
             if first[0] is None:
@@ -846,8 +882,9 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             timu.append(truth_imu_of(truth, tr, fi))
             tposes.append(truth["truth_pose"][ids])
             err2[i].append(float(np.sum((timu[-1][0:3] - f.getImuState()["p_I_G"]) ** 2)))
-            if first[i] is not None and first[i]["frame"] == fi:
-                first[i]["pos_err2_after"] = err2[i][-1]
+            for fx in (first, first_r, first_g):
+                if fx is not None and fx[i] is not None and fx[i]["frame"] == fi:
+                    fx[i]["pos_err2_after"] = err2[i][-1]
         res = fb.nees(timu, tposes)
         for i, r in enumerate(res):
             rows[i].append(r)
@@ -855,7 +892,8 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             on_frame(fi, fs, res)
     fb.close()
     records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i], None if gnss is None else gnss[i],
-                                     None if ranging is None else ranging[i])
+                                     None if ranging is None else ranging[i], None if first_r is None else first_r[i],
+                                     None if first_g is None else first_g[i])
                for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):

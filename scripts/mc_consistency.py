@@ -41,6 +41,11 @@ the GNSS and ranging stacks through fault detection and exclusion (thresholds: t
 the injected faults, faults excluded, clean items excluded, faults missed and stacks rejected; their ANIS is over the stacks
 applied.
 
+--range-start F / --gnss-start F fuse no ranging / GNSS epoch before frame F (the first stack after an outage, when the filter has
+drifted), and --aid-iterations K iterates the GNSS, ranging and odometry stacks (at most K linearisations, converged at a step
+<= --aid-tol); the summary then adds the first ranging / GNSS stack: the position RMSE before and after it, its ANIS, the
+IMU-state ANEES after it, the mean linearisations and the share converged.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -186,6 +191,10 @@ def main():
     ap.add_argument("--gnss-outlier-jump", type=float, default=5.0)
     ap.add_argument("--fde-alpha", type=float, default=0.0, help="> 0: fault detection and exclusion in the GNSS and ranging stacks")
     ap.add_argument("--fde-max-exclude", type=int, default=2)
+    ap.add_argument("--range-start", type=int, default=0, help="fuse no ranging epoch before this frame")
+    ap.add_argument("--gnss-start", type=int, default=0, help="fuse no GNSS epoch before this frame")
+    ap.add_argument("--aid-iterations", type=int, default=1, help="iterate the GNSS, ranging and odometry stacks (linearisations)")
+    ap.add_argument("--aid-tol", type=float, default=1e-10)
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -211,7 +220,9 @@ def main():
                         plane_every=args.plane_every, plane_sigma=args.plane_sigma, plane_height=args.plane_height,
                         plane_axis=args.plane_axis, plane_lever=args.plane_lever, range_outlier_rate=args.range_outlier_rate,
                         range_outlier_bias=args.range_outlier_bias, gnss_outlier_rate=args.gnss_outlier_rate,
-                        gnss_outlier_jump=args.gnss_outlier_jump, fde_alpha=args.fde_alpha, fde_max_exclude=args.fde_max_exclude)
+                        gnss_outlier_jump=args.gnss_outlier_jump, fde_alpha=args.fde_alpha, fde_max_exclude=args.fde_max_exclude,
+                        range_start=args.range_start, gnss_start=args.gnss_start, aid_iterations=args.aid_iterations,
+                        aid_tol=args.aid_tol)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -239,6 +250,11 @@ def main():
                         "plane_every": args.plane_every, "plane_sigma_m": args.plane_sigma, "plane_height_m": args.plane_height,
                         "plane_axis": args.plane_axis, "plane_lever_m": args.plane_lever,
                         **{k: s["range"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "degenerate") + FAULTS}}
+    for key, start in (("range", args.range_start), ("gnss", args.gnss_start)):
+        if key in res and (start or args.aid_iterations != 1):
+            res[key].update(start=start, iterations=args.aid_iterations, tol=args.aid_tol)
+            if key + "_first" in s:
+                res[key]["first_stack"] = s[key + "_first"]
     if args.fde_alpha > 0 or args.range_outlier_rate > 0 or args.gnss_outlier_rate > 0:
         res["faults"] = {"range_outlier_rate": args.range_outlier_rate, "range_outlier_bias_m": args.range_outlier_bias,
                          "gnss_outlier_rate": args.gnss_outlier_rate, "gnss_outlier_jump_m": args.gnss_outlier_jump,

@@ -6,7 +6,10 @@ _batch_aid_update with LINEAR).  fp64 filters at 30 clones (n = 195); the stack 
 of montecarlo.ANCHORS placed around the filter's position, and one rangefinder distance to a level plane 1.5 m below (5 rows),
 the method of scripts/gnss_rate.py.  Host time around each synchronising call, median of --reps after a warm-up, at 1 / 8 / 32
 members.  --fde instead times the plain stack against msckf_b200_aid_stack_update_fde (alpha = 0.01, max_exclude = 2) on the
-same five items with R = 0.01 m^2, without a fault and with the first range 1 m long (one exclusion round).
+same five items with R = 0.01 m^2, without a fault and with the first range 1 m long (one exclusion round).  --iterations K ...
+instead times msckf_b200_aid_stack_update_iter / _batch_aid_stack_update_iter at each max_iter K on the same five items with
+R = 0.01 m^2, the ranges measured from 0.3 m beside the estimate, tol 0 (every call makes its K linearisations unless a step is
+exactly zero), and reports the mean linearisations made.
 Prints one JSON line with the card's name, power limit and max SM clock."""
 import argparse
 import json
@@ -25,12 +28,14 @@ from odometry_rate import gpu_line, median_ms, members  # noqa: E402
 LEVER = np.array([0.3, -0.2, 0.5])
 
 
-def stack_of(e, sigma=1e3, fault=0.0):
-    """the five range items at the current estimate (large R: P barely moves), the first range `fault` m long"""
+def stack_of(e, sigma=1e3, fault=0.0, offset=0.0):
+    """the five range items at the current estimate (large R: P barely moves), the first range `fault` m long, the anchor
+    ranges measured from `offset` m beside the estimate (along x)"""
     imu, _ = e.state()
     imu = imu.astype(np.float64)
     p, q = imu[0:3], imu[15:19]
-    items = [{"model": capi.AID_RANGE, "z": np.r_[mc.range_of(p, q, LEVER, p + a) + 0.01, p + a, LEVER], "R": np.array([[sigma]])}
+    pm = p + np.array([offset, 0.0, 0.0])
+    items = [{"model": capi.AID_RANGE, "z": np.r_[mc.range_of(pm, q, LEVER, p + a) + 0.01, p + a, LEVER], "R": np.array([[sigma]])}
              for a in mc.ANCHORS]
     axis = mc.quat_to_rot(q) @ np.array([0.0, 0.0, -1.0])  # straight down in G
     h = mc.antenna_position(p, q, LEVER)[2] - 1.5
@@ -59,13 +64,35 @@ def fde_calls(args, res):
         res["calls_ms"][str(nm)] = row
 
 
+def iterated_calls(args, res):
+    for nm in args.members:
+        row = {}
+        for K in args.iterations:
+            fs, es = members(nm)
+            stacks = [stack_of(e, 0.01, offset=0.3) for e in es]
+            b = capi.Batch(es) if nm > 1 else None
+            call = (lambda: b.aid_stack_update(stacks, max_iter=K, tol=0.0)) if b else \
+                (lambda: [es[0].aid_stack_update(stacks[0], max_iter=K, tol=0.0)])
+            row[str(K)] = {"ms": median_ms(call, args.reps), "iterations": float(np.mean([o["iterations"] for o in call()]))}
+            if b:
+                b.close()
+            for f in fs:
+                f.close()
+        res["calls_ms"][str(nm)] = row
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--members", type=int, nargs="+", default=[1, 8, 32])
     ap.add_argument("--fde", action="store_true", help="plain stack against fault detection and exclusion")
+    ap.add_argument("--iterations", type=int, nargs="*", default=None, help="time the iterated stack at these max_iter")
     args = ap.parse_args()
     res = {"gpu": gpu_line(), "clones": 30, "rows": 5, "reps": args.reps, "calls_ms": {}}
+    if args.iterations:
+        iterated_calls(args, res)
+        print(json.dumps(res), flush=True)
+        return
     if args.fde:
         fde_calls(args, res)
         print(json.dumps(res), flush=True)
