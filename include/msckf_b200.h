@@ -429,7 +429,7 @@ typedef struct {
   const double* R;       /* [3]: uu, uv, vv (positive definite), or NULL: diag(u_var', v_var') of the filter */
   double chi2_obs;       /* > 0: per-observation gate on gamma */
   double* gamma;         /* [n_obs] out, or NULL */
-  int* flag;             /* [n_obs] out (0 used, 1 gated out, 2 behind the camera / not finite), or NULL */
+  int* flag;             /* [n_obs] out (0 used, 1 gated out, 2 behind the camera / not finite, 3 excluded by consensus), or NULL */
   int max_iter;          /* linearisations, 0 .. 16 (0 or 1: one) */
   double tol;            /* finite, >= 0: the iteration has converged when max |delta_{i+1} - delta_i| <= tol */
 } msckf_b200_landmarks;
@@ -485,6 +485,49 @@ int msckf_b200_map_landmark_update(msckf_b200_engine* e, const msckf_b200_landma
 /* the same for every member of a batch (lm[i], map[i], out[i]; map NULL: every member exact) */
 int msckf_b200_batch_map_landmark_update(msckf_b200_batch* b, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
                                          msckf_b200_landmark_result* out);
+/* ---- mapped landmarks with consensus: which matches to trust, decided on the device before the update (DESIGN.md 4.17) ----
+ * Relocalisation matches contain wrong ones, and after drift a per-observation gate against the prior cannot tell them from
+ * right ones.  Right matches agree on one common correction of the window; wrong ones do not.  A hypothesis is a 4-dof rigid
+ * correction (psi about G's z axis, t) applied to the map: p_L' = Rz(psi)^T (p_L - c - t) + c, c = pivot = the mean p_C_G of the
+ * clones the observations name, projected with the filter's clone pose.  Observation i is an inlier of (psi, t) when its depth is
+ * > 0 and e_i = (z_i - z^_i)^T R^-1 (z_i - z^_i) <= thresh (R: the call's, or diag(u_var', v_var')).
+ * Hypothesis h is fitted to the observations (i, j) drawn from seed by splitmix64 (DESIGN.md 4.17), i != j in input order, by
+ * Gauss-Newton from (0, 0): at most 8 steps, stopping at max |step| <= 1e-12.  It is valid when every step's 4 x 4 Cholesky has
+ * its pivots > 1e-12 x their diagonal entries, both points stay in front and both are inliers of the result.  The best valid
+ * hypothesis has the most inliers (a tie: the lowest h).  A refit (Gauss-Newton over its inliers, from its (psi, t), at most 8
+ * steps) is rescored once; the final inliers are the refit's if it succeeded and kept at least as many, else the hypothesis's.
+ * Fewer than min_inliers final inliers (no valid hypothesis included): status 1, every observation not flagged 2 gets flag 3
+ * and nothing is written (applied 0).  Otherwise the outliers get flag 3 (excluded by consensus, not used) and the update runs
+ * on the rest, in every form (exact map or Sigma_L, single or iterated): flag 2 comes before 3, and 3 before the chi2_obs gate.
+ * gamma is written as without consensus.  The consensus never seeds the iterate: the update starts from the prior.
+ * Two more launches per 32 members with consensus; still one copy each way and one synchronisation. */
+typedef struct {
+  int hypotheses;             /* 0 .. 1024; 0: no consensus (the plain call, bit for bit) */
+  double thresh;              /* finite, > 0 (when hypotheses > 0) */
+  int min_inliers;            /* >= 2 (when hypotheses > 0) */
+  unsigned long long seed;
+  int* scores;                /* [hypotheses] out: each hypothesis's inliers, or -1 when it is not valid; or NULL */
+} msckf_b200_landmark_consensus;
+typedef struct {
+  int status;                 /* 0: a consensus was found; 1: fewer than min_inliers inliers (nothing was written) */
+  int inliers;                /* final inliers */
+  int best;                   /* the best valid hypothesis, or -1 */
+  int valid;                  /* valid hypotheses (0: none) */
+  int refit;                  /* 1: the final inliers and (yaw, t) are the refit's */
+  double yaw, t[3];           /* the final correction */
+  double pivot[3];            /* c */
+} msckf_b200_landmark_consensus_result;
+/* cons NULL or hypotheses = 0: msckf_b200_map_landmark_update (map NULL: the exact map), bit for bit, and cons_out (if given)
+ * gets best = -1 and zeros; cons_out may be NULL.  MSCKF_B200_ERR_ARG before anything is launched: hypotheses outside 0 .. 1024,
+ * and with hypotheses > 0 a thresh that is not finite and > 0 or min_inliers < 2; and what the plain call refuses. */
+int msckf_b200_landmark_update_consensus(msckf_b200_engine* e, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                         const msckf_b200_landmark_consensus* cons, msckf_b200_landmark_result* out,
+                                         msckf_b200_landmark_consensus_result* cons_out);
+/* the same for every member of a batch: cons[i] and cons_out[i] (cons NULL: no member runs a consensus); a member's arithmetic
+ * depends only on its own inputs, so a batch equals single calls bit for bit */
+int msckf_b200_batch_landmark_update_consensus(msckf_b200_batch* b, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                               const msckf_b200_landmark_consensus* cons, msckf_b200_landmark_result* out,
+                                               msckf_b200_landmark_consensus_result* cons_out);
 /* Convenience: one update on each of n engines through a batch.  If the engines already form a batch (in this order) it is
  * used; otherwise a temporary one is created and destroyed around the call.  Returns the first non-zero status. */
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,

@@ -569,6 +569,45 @@ class MSCKF {
     landmarkAbsorb(r);
     return r;
   }
+  // the same updates with a consensus on the matches (msckf_b200_landmark_update_consensus: model, sampling, selection and flag 3
+  // there): the outliers of the best 4-dof correction are excluded before the update; cons_out receives the consensus result.
+  // An invalid consensus (hypotheses outside 0 .. 1024, or with hypotheses > 0 a thresh that is not finite and > 0 or
+  // min_inliers < 2) throws std::invalid_argument before any device call; otherwise as the landmarkUpdate forms above.
+  msckf_b200_landmark_result landmarkUpdate(const std::vector<landmarkObservation>& obs, const msckf_b200_landmark_consensus& cons,
+                                            msckf_b200_landmark_consensus_result& cons_out, const FixedMatrix<double, 2, 2>* R = nullptr,
+                                            double chi2_obs = 0, std::vector<double>* gamma = nullptr, std::vector<int>* flag = nullptr,
+                                            int max_iter = 1, double tol = 1e-10) {
+    checkConsensus(cons);
+    msckf_b200_landmarks lm{};
+    landmarkPack(obs, R, chi2_obs, gamma, flag, lm);
+    lm.max_iter = max_iter; lm.tol = tol;
+    msckf_b200_landmark_result r = {};
+    checkNumeric(msckf_b200_landmark_update_consensus(eng(), &lm, nullptr, &cons, &r, &cons_out), "msckf_b200_landmark_update_consensus");
+    landmarkAbsorb(r);
+    return r;
+  }
+  msckf_b200_landmark_result landmarkUpdate(const std::vector<mapObservation>& obs, const std::vector<mapLandmark>& landmarks,
+                                            const msckf_b200_landmark_consensus& cons, msckf_b200_landmark_consensus_result& cons_out,
+                                            const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
+                                            std::vector<double>* gamma = nullptr, std::vector<int>* flag = nullptr, int max_iter = 1,
+                                            double tol = 1e-10) {
+    checkConsensus(cons);
+    msckf_b200_landmarks lm{};
+    msckf_b200_landmark_map map{};
+    mapPack(obs, landmarks, R, chi2_obs, gamma, flag, lm, map);
+    lm.max_iter = max_iter; lm.tol = tol;
+    msckf_b200_landmark_result r = {};
+    checkNumeric(msckf_b200_landmark_update_consensus(eng(), &lm, &map, &cons, &r, &cons_out), "msckf_b200_landmark_update_consensus");
+    landmarkAbsorb(r);
+    return r;
+  }
+  // the consensus settings the C-ABI accepts
+  static void checkConsensus(const msckf_b200_landmark_consensus& c) {
+    if (c.hypotheses < 0 || c.hypotheses > 1024) throw std::invalid_argument("landmarkUpdate: hypotheses outside 0 .. 1024");
+    if (c.hypotheses > 0 && !(std::isfinite(c.thresh) && c.thresh > 0.0))
+      throw std::invalid_argument("landmarkUpdate: consensus thresh is not finite and > 0");
+    if (c.hypotheses > 0 && c.min_inliers < 2) throw std::invalid_argument("landmarkUpdate: consensus min_inliers < 2");
+  }
   // landmarkPack of the observations' map positions, and the map (landmark ids, Sigma) in this object's buffers
   void mapPack(const std::vector<mapObservation>& obs, const std::vector<mapLandmark>& landmarks, const FixedMatrix<double, 2, 2>* R,
                double chi2_obs, std::vector<double>* gamma, std::vector<int>* flag, msckf_b200_landmarks& lm,
@@ -1263,6 +1302,68 @@ class MSCKFBatch {
     const int rc = msckf_b200_batch_map_landmark_update(batch_, lm.data(), map.data(), r.data());
     if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch map landmark update: " << msckf_b200_last_error() << std::endl;
     else MSCKF<_S>::check(rc, "msckf_b200_batch_map_landmark_update");
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty()) filters_[i]->landmarkAbsorb(r[i]);
+    return r;
+  }
+  // the two MSCKFBatch::landmarkUpdate forms above with a consensus per filter (cons[i], cons_out[i]) as one
+  // msckf_b200_batch_landmark_update_consensus; an invalid consensus or id throws before any device call.  landmarks empty:
+  // the exact map (landmarkObservation), else filter i's landmark list (mapObservation through obs_map).
+  std::vector<msckf_b200_landmark_result> landmarkUpdate(const std::vector<std::vector<landmarkObservation>>& obs,
+                                                         const std::vector<msckf_b200_landmark_consensus>& cons,
+                                                         std::vector<msckf_b200_landmark_consensus_result>& cons_out,
+                                                         const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
+                                                         std::vector<std::vector<double>>* gamma = nullptr,
+                                                         std::vector<std::vector<int>>* flag = nullptr, int max_iter = 1,
+                                                         double tol = 1e-10) {
+    const size_t n = size();
+    if (obs.size() != n || cons.size() != n)
+      throw std::invalid_argument("MSCKFBatch::landmarkUpdate: one observation list and one consensus per filter");
+    for (const auto& c : cons) MSCKF<_S>::checkConsensus(c);
+    if (gamma) gamma->assign(n, std::vector<double>());
+    if (flag) flag->assign(n, std::vector<int>());
+    std::vector<msckf_b200_landmarks> lm(n, msckf_b200_landmarks());
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty())
+        filters_[i]->landmarkPack(obs[i], R, chi2_obs, gamma ? &(*gamma)[i] : nullptr, flag ? &(*flag)[i] : nullptr, lm[i]);
+    for (size_t i = 0; i < n; ++i) { lm[i].max_iter = max_iter; lm[i].tol = tol; }
+    return consensusCall(obs, lm, nullptr, cons, cons_out);
+  }
+  std::vector<msckf_b200_landmark_result> landmarkUpdate(const std::vector<std::vector<mapObservation>>& obs,
+                                                         const std::vector<std::vector<mapLandmark>>& landmarks,
+                                                         const std::vector<msckf_b200_landmark_consensus>& cons,
+                                                         std::vector<msckf_b200_landmark_consensus_result>& cons_out,
+                                                         const FixedMatrix<double, 2, 2>* R = nullptr, double chi2_obs = 0,
+                                                         std::vector<std::vector<double>>* gamma = nullptr,
+                                                         std::vector<std::vector<int>>* flag = nullptr, int max_iter = 1,
+                                                         double tol = 1e-10) {
+    const size_t n = size();
+    if (obs.size() != n || landmarks.size() != n || cons.size() != n)
+      throw std::invalid_argument("MSCKFBatch::landmarkUpdate: one observation list, one landmark list and one consensus per filter");
+    for (const auto& c : cons) MSCKF<_S>::checkConsensus(c);
+    if (gamma) gamma->assign(n, std::vector<double>());
+    if (flag) flag->assign(n, std::vector<int>());
+    std::vector<msckf_b200_landmarks> lm(n, msckf_b200_landmarks());
+    std::vector<msckf_b200_landmark_map> map(n, msckf_b200_landmark_map());
+    for (size_t i = 0; i < n; ++i)
+      if (!obs[i].empty())
+        filters_[i]->mapPack(obs[i], landmarks[i], R, chi2_obs, gamma ? &(*gamma)[i] : nullptr, flag ? &(*flag)[i] : nullptr, lm[i],
+                             map[i]);
+    for (size_t i = 0; i < n; ++i) { lm[i].max_iter = max_iter; lm[i].tol = tol; }
+    return consensusCall(obs, lm, map.data(), cons, cons_out);
+  }
+  template <class Obs>
+  std::vector<msckf_b200_landmark_result> consensusCall(const std::vector<std::vector<Obs>>& obs, std::vector<msckf_b200_landmarks>& lm,
+                                                        const msckf_b200_landmark_map* map,
+                                                        const std::vector<msckf_b200_landmark_consensus>& cons,
+                                                        std::vector<msckf_b200_landmark_consensus_result>& cons_out) {
+    const size_t n = size();
+    flushImu();
+    std::vector<msckf_b200_landmark_result> r(n, msckf_b200_landmark_result());
+    cons_out.assign(n, msckf_b200_landmark_consensus_result());
+    const int rc = msckf_b200_batch_landmark_update_consensus(batch_, lm.data(), map, cons.data(), r.data(), cons_out.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch landmark update: " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_landmark_update_consensus");
     for (size_t i = 0; i < n; ++i)
       if (!obs[i].empty()) filters_[i]->landmarkAbsorb(r[i]);
     return r;

@@ -137,6 +137,18 @@ int msckf_mono_map_update(void* h, int n_obs, const int* state_ids, const int* l
 int msckf_mono_batch_map_update(void* batch, const int* n_obs, const int* state_ids, const int* landmark, const double* z,
                                 const int* n_landmarks, const double* p_L_G, const double* Sigma, const double* R3, double chi2_obs,
                                 int max_iter, double tol, double* gamma, int* flag, msckf_b200_landmark_result* out);
+/* mapped-landmark update with a consensus on the matches (MSCKF::landmarkUpdate with a msckf_b200_landmark_consensus,
+ * msckf_b200_landmark_update_consensus: model, flag 3, errors there), exact map; the other arguments as in
+ * msckf_mono_landmark_update_iter.  _batch_: cons[i] and cons_out[i] per filter, the observation arrays as in
+ * msckf_mono_batch_landmark_update_iter.  An invalid consensus fails before any device call. */
+int msckf_mono_landmark_update_consensus(void* h, int n_obs, const int* state_ids, const double* z, const double* p_L_G,
+                                         const double* R3, double chi2_obs, int max_iter, double tol,
+                                         const msckf_b200_landmark_consensus* cons, double* gamma, int* flag,
+                                         msckf_b200_landmark_result* out, msckf_b200_landmark_consensus_result* cons_out);
+int msckf_mono_batch_landmark_update_consensus(void* batch, const int* n_obs, const int* state_ids, const double* z,
+                                               const double* p_L_G, const double* R3, double chi2_obs, int max_iter, double tol,
+                                               const msckf_b200_landmark_consensus* cons, double* gamma, int* flag,
+                                               msckf_b200_landmark_result* out, msckf_b200_landmark_consensus_result* cons_out);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

@@ -200,6 +200,32 @@ def landmark_map_struct(spec):
     return LandmarkMap(None if lm is None else lm.ctypes.data, S.ctypes.data, len(S)), (lm, S)
 
 
+class LandmarkConsensus(C.Structure):
+    _fields_ = [("hypotheses", C.c_int), ("thresh", C.c_double), ("min_inliers", C.c_int), ("seed", C.c_ulonglong),
+                ("scores", C.c_void_p)]
+
+
+class LandmarkConsensusResult(C.Structure):
+    _fields_ = [("status", C.c_int), ("inliers", C.c_int), ("best", C.c_int), ("valid", C.c_int), ("refit", C.c_int),
+                ("yaw", C.c_double), ("t", C.c_double * 3), ("pivot", C.c_double * 3)]
+
+    def as_dict(self, scores=None):
+        d = {k: getattr(self, k) for k in ("status", "inliers", "best", "valid", "refit", "yaw")}
+        d.update(t=np.array(self.t[:]), pivot=np.array(self.pivot[:]), scores=scores)
+        return d
+
+
+def consensus_struct(cons):
+    """(LandmarkConsensus, the arrays it points into) of cons = None (no consensus) or a dict hypotheses (0..1024), thresh,
+    min_inliers, seed; the arrays are (scores [hypotheses] out,)"""
+    if cons is None or int(cons.get("hypotheses", 0)) == 0:
+        return LandmarkConsensus(0, 0.0, 0, 0, None), ()
+    h = int(cons["hypotheses"])
+    scores = np.zeros(max(h, 0), dtype=np.int32)
+    return LandmarkConsensus(h, float(cons.get("thresh", 0.0)), int(cons.get("min_inliers", 0)), int(cons.get("seed", 0)) % 2 ** 64,
+                             scores.ctypes.data), (scores,)
+
+
 _lib = None
 
 
@@ -415,17 +441,28 @@ class Batch:
                     r.update(o.as_dict())
         return res
 
-    def landmark_update(self, specs, max_iter=None, tol=None):
+    def landmark_update(self, specs, max_iter=None, tol=None, consensus=None):
         """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
         i alone); max_iter / tol, when given, apply to every spec that does not set its own.  When a spec has Sigma_L (see
         landmark_map_struct) the call is msckf_b200_batch_map_landmark_update.  A list of result dicts with "gamma" and "flag"
-        arrays (None for an engine left alone)"""
+        arrays (None for an engine left alone).  consensus (see consensus_struct; also a spec's own "consensus", which comes
+        first): msckf_b200_batch_landmark_update_consensus, and each dict has a "consensus" dict with the hypotheses' scores."""
         n = len(self.engines)
         assert len(specs) == n
         extra = {k: v for k, v in (("max_iter", max_iter), ("tol", tol)) if v is not None}
         st = [landmark_struct(s if s is None else dict(extra, **s)) for s in specs]
         out = (LandmarkResult * n)()
         arr = (Landmarks * n)(*[a for a, _ in st])
+        cs = [s.get("consensus", consensus) if s is not None else consensus for s in specs]
+        if any(c is not None for c in cs):
+            cons = [consensus_struct(c) for c in cs]
+            cout = (LandmarkConsensusResult * n)()
+            maps = [landmark_map_struct(s) for s in specs]
+            check(lib().msckf_b200_batch_landmark_update_consensus(self.h, arr, (LandmarkMap * n)(*[m for m, _ in maps]),
+                                                                   (LandmarkConsensus * n)(*[c for c, _ in cons]), out, cout),
+                  "msckf_b200_batch_landmark_update_consensus")
+            return [None if not k else dict(o.as_dict(), gamma=k[4], flag=k[5], consensus=co.as_dict(ck[0] if ck else None))
+                    for (a, k), o, co, (c, ck) in zip(st, out, cout, cons)]
         if any(s is not None and s.get("Sigma_L") is not None for s in specs):
             maps = [landmark_map_struct(s) for s in specs]
             check(lib().msckf_b200_batch_map_landmark_update(self.h, arr, (LandmarkMap * n)(*[m for m, _ in maps]), out),
@@ -600,14 +637,23 @@ class Engine:
             res.update(iout.as_dict())
         return res
 
-    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0, landmark=None, Sigma_L=None):
+    def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0, landmark=None, Sigma_L=None, consensus=None):
         """msckf_b200_landmark_update: observations of known landmarks p_L [n, 3] at z [n, 2] from window positions clone [n];
         max_iter >= 2 iterates the update (at most max_iter linearisations, converged at max |delta_{i+1} - delta_i| <= tol).
         landmark [n] with Sigma_L (see landmark_map_struct): msckf_b200_map_landmark_update, each landmark's map error
-        marginalised over its observations.
+        marginalised over its observations.  consensus (see consensus_struct): msckf_b200_landmark_update_consensus, and the
+        dict has a "consensus" dict (status, inliers, best, valid, refit, yaw, t, pivot, scores).
         The result as a dict with the per-observation "gamma" and "flag" arrays"""
         a, keep = landmark_struct({"clone": clone, "z": z, "p_L": p_L, "R": R, "chi2_obs": chi2_obs, "max_iter": max_iter, "tol": tol})
         out = LandmarkResult()
+        if consensus is not None:
+            m, mk = landmark_map_struct(None if Sigma_L is None else {"landmark": landmark, "Sigma_L": Sigma_L})
+            c, ck = consensus_struct(consensus)
+            cout = LandmarkConsensusResult()
+            check(lib().msckf_b200_landmark_update_consensus(self.h, C.byref(a), C.byref(m), C.byref(c), C.byref(out), C.byref(cout)),
+                  "msckf_b200_landmark_update_consensus")
+            return dict(out.as_dict(), gamma=keep[4] if keep else np.zeros(0), flag=keep[5] if keep else np.zeros(0, np.int32),
+                        consensus=cout.as_dict(ck[0] if ck else None))
         if Sigma_L is None:
             check(lib().msckf_b200_landmark_update(self.h, C.byref(a), C.byref(out)), "msckf_b200_landmark_update")
         else:

@@ -24,6 +24,7 @@
 #include "feature_kernels.cuh"
 #include "gram_kernels.cuh"
 #include "landmark_kernels.cuh"
+#include "consensus_kernels.cuh"
 #include "nees_kernels.cuh"
 #include "state_kernels.cuh"
 #include "tail_kernels.cuh"
@@ -253,7 +254,9 @@ struct CtxBase {
   virtual int aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
                             msckf_b200_aid_fde_result* out, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) = 0;
   // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
-  virtual int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) = 0;
+  // (cons, cout: the consensus of each member, or NULL)
+  virtual int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out,
+                        const msckf_b200_landmark_consensus* cons = nullptr, msckf_b200_landmark_consensus_result* cout = nullptr) = 0;
   cudaStream_t stream = nullptr;
   long long launches = 0;
   bool pending = false;
@@ -531,7 +534,8 @@ struct Ctx : CtxBase {
   int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what, const msckf_b200_aid_fde* fde = nullptr,
               msckf_b200_aid_fde_result* fout = nullptr, const msckf_b200_aid_iter* iter = nullptr,
               msckf_b200_aid_iter_result* iout = nullptr);
-  int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) override;
+  int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out,
+                const msckf_b200_landmark_consensus* cons, msckf_b200_landmark_consensus_result* cout) override;
   int kernel_times(float* ms, const char** names, int cap) override {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
@@ -1721,6 +1725,11 @@ static_assert(offsetof(mb::LmkOut, status) == offsetof(msckf_b200_landmark_resul
                   offsetof(mb::LmkOut, converged) == offsetof(msckf_b200_landmark_result, converged) &&
                   offsetof(mb::LmkOut, step) == offsetof(msckf_b200_landmark_result, step),
               "mb::LmkOut must have msckf_b200_landmark_result's fields at their offsets");
+static_assert(sizeof(mb::LmkConsOut) == sizeof(msckf_b200_landmark_consensus_result) &&
+                  offsetof(mb::LmkConsOut, refit) == offsetof(msckf_b200_landmark_consensus_result, refit) &&
+                  offsetof(mb::LmkConsOut, yaw) == offsetof(msckf_b200_landmark_consensus_result, yaw) &&
+                  offsetof(mb::LmkConsOut, pivot) == offsetof(msckf_b200_landmark_consensus_result, pivot),
+              "mb::LmkConsOut must be msckf_b200_landmark_consensus_result");
 // one member's call, planned on the host
 struct LmkPlan {
   std::vector<int> perm, grp;  // packed observation j is input observation perm[j]; [G][3] clone, first observation, count
@@ -1730,7 +1739,45 @@ struct LmkPlan {
   std::vector<int> sdesc, pair_of, lms;
   int H = 0, pairs = 0;
   size_t E_len = 0, B_len = 0;
+  // consensus: the member runs one; its sampled observation pairs (packed order) and each observation's group
+  bool cons = false;
+  std::vector<int> hpair, ogrp;
 };
+
+// splitmix64's output function (DESIGN.md 4.17)
+inline uint64_t splitmix64(uint64_t x) {
+  x += 0x9E3779B97F4A7C15ull;
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+
+// the consensus's hypotheses of a member with no observations and its pairs: hypothesis h samples input observations
+// i = u mod n and j = v mod (n - 1), j += 1 when j >= i, with u = splitmix64(seed + 2h), v = splitmix64(seed + 2h + 1), and the
+// pair goes to the device in packed order (fewer than 2 observations: no pair, so no valid hypothesis)
+int lmk_cons_plan(const msckf_b200_landmarks& q, const msckf_b200_landmark_consensus& c, const std::string& who, LmkPlan& p) {
+  if (c.hypotheses < 0 || c.hypotheses > mb::kLmkMaxHyp) return fail(MSCKF_B200_ERR_ARG, "landmark_update: hypotheses outside 0 .. 1024" + who);
+  if (c.hypotheses == 0) return 0;
+  if (!std::isfinite(c.thresh) || !(c.thresh > 0.0)) return fail(MSCKF_B200_ERR_ARG, "landmark_update: consensus thresh is not finite and > 0" + who);
+  if (c.min_inliers < 2) return fail(MSCKF_B200_ERR_ARG, "landmark_update: consensus min_inliers < 2" + who);
+  p.cons = true;
+  const int n = q.n_obs;
+  if (n < 2) return 0;
+  std::vector<int> inv(n);
+  for (int j = 0; j < n; ++j) inv[p.perm[j]] = j;
+  p.hpair.resize(2 * (size_t)c.hypotheses);
+  for (int h = 0; h < c.hypotheses; ++h) {
+    const uint64_t u = splitmix64(c.seed + 2 * (uint64_t)h), v = splitmix64(c.seed + 2 * (uint64_t)h + 1);
+    const int i = (int)(u % (uint64_t)n);
+    int j = (int)(v % (uint64_t)(n - 1));
+    if (j >= i) ++j;
+    p.hpair[2 * h] = inv[i]; p.hpair[2 * h + 1] = inv[j];
+  }
+  p.ogrp.resize(n);
+  for (int g = 0; g < p.G; ++g)
+    for (int k = 0; k < p.grp[3 * g + 2]; ++k) p.ogrp[p.grp[3 * g + 1] + k] = g;
+  return 0;
+}
 
 // Sigma_L given: check the landmark ids and covariances, count the one-clone landmarks' observations per clone (single),
 // and group the landmarks seen from 2 .. 8 clones by their exact clone set (sets in ascending order, landmarks ascending)
@@ -1830,8 +1877,9 @@ int lmk_plan(const msckf_b200_landmarks& q, const msckf_b200_landmark_map* mq, i
 // one member's host addresses in the I/O block: the inputs the host packs and the results it reads back
 struct LmkHost {
   double *obs, *sig, *lsig, *gamma;
-  int *grp, *wrow, *sdesc, *flag;
+  int *grp, *wrow, *sdesc, *flag, *pairs, *ogrp, *score;
   mb::LmkOut* out;
+  mb::LmkConsOut* cres;
 };
 struct LmkSizes { size_t in = 0, res = 0, io = 0, ws = 0; };  // bytes of inputs; offset of the results; I/O block; workspace
 
@@ -1841,7 +1889,7 @@ struct LmkSizes { size_t in = 0, res = 0, io = 0, ws = 0; };  // bytes of inputs
 // also gives each member's host addresses (h) and its arguments' device addresses (a).
 template <class S>
 LmkSizes lmk_layout(const std::vector<int>& idx, const msckf_b200_landmarks* in, const std::vector<LmkPlan>& pl, unsigned char* ioh,
-                    unsigned char* iod, unsigned char* wsd, std::vector<LmkHost>& h, std::vector<mb::LmkMapArgs<S>>& a) {
+                    unsigned char* iod, unsigned char* wsd, std::vector<LmkHost>& h, std::vector<mb::LmkConsArgs<S>>& a) {
   LmkSizes z;
   size_t o = 0, w = 0;  // the cursors in the I/O block and in the workspace
   const auto io = [&](auto& hp, auto& dp, size_t bytes) {  // the next `bytes` of the I/O block, then 16-byte aligned
@@ -1863,6 +1911,10 @@ LmkSizes lmk_layout(const std::vector<int>& idx, const msckf_b200_landmarks* in,
       io(h[i].sdesc, a[i].sdesc, sizeof(int) * p.sdesc.size());
       io(h[i].lsig, a[i].lsig, sizeof(double) * 6 * p.lms.size());
     }
+    if (p.cons) {  // the sampled pairs and each observation's group
+      io(h[i].pairs, a[i].pairs, sizeof(int) * p.hpair.size());
+      io(h[i].ogrp, a[i].ogrp, sizeof(int) * p.ogrp.size());
+    }
     take(a[i].slot, sizeof(double) * mb::kLmkSlot * p.G);
     take(a[i].A, sizeof(double) * (p.ld + n + 1) * p.ld);
     take(a[i].dx, sizeof(double) * n);
@@ -1877,6 +1929,10 @@ LmkSizes lmk_layout(const std::vector<int>& idx, const msckf_b200_landmarks* in,
       take(a[i].B, sizeof(double) * p.B_len); take(a[i].sslot, sizeof(double) * mb::kLmkSetSlot * p.H);
       w = up256(w);
     }
+    if (p.cons) {  // the hypotheses' fits and counts
+      take(a[i].hyp, sizeof(mb::LmkHyp) * p.hpair.size() / 2);
+      w = up256(w);
+    }
   }
   z.in = o;
   o = z.res = up256(o);
@@ -1885,26 +1941,48 @@ LmkSizes lmk_layout(const std::vector<int>& idx, const msckf_b200_landmarks* in,
     io(h[i].out, a[i].out, sizeof(mb::LmkOut));
     io(h[i].gamma, a[i].gamma, sizeof(double) * no);
     io(h[i].flag, a[i].flag, sizeof(int) * no);
+    if (pl[i].cons) {
+      io(h[i].cres, a[i].cres, sizeof(mb::LmkConsOut));
+      io(h[i].score, a[i].score, sizeof(int) * pl[i].hpair.size() / 2);
+    }
   }
   z.io = o; z.ws = w;
   return z;
 }
 
 template <class S>
-int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out) {
+int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out,
+                      const msckf_b200_landmark_consensus* cons, msckf_b200_landmark_consensus_result* cout) {
   if (!in || !out) return fail(MSCKF_B200_ERR_ARG, "landmark_update: null argument");
   RC(members_ready("landmark_update"));
   const int nf = (int)eng.size();
   std::vector<LmkPlan> pl(nf);
   std::vector<LmkHost> h(nf);
-  std::vector<mb::LmkMapArgs<S>> args(nf);  // zeroed; the layout fills in the addresses
+  std::vector<mb::LmkConsArgs<S>> args(nf);  // zeroed; the layout fills in the addresses
   std::vector<int> idx;
+  bool any_cons = false;
   for (int i = 0; i < nf; ++i) {
-    RC(lmk_plan(in[i], map && map[i].Sigma_L ? &map[i] : nullptr, eng[i]->M, " (member " + std::to_string(i) + ")", pl[i]));
+    const std::string who = " (member " + std::to_string(i) + ")";
+    RC(lmk_plan(in[i], map && map[i].Sigma_L ? &map[i] : nullptr, eng[i]->M, who, pl[i]));
+    if (cons) RC(lmk_cons_plan(in[i], cons[i], who, pl[i]));
+  }
+  for (int i = 0; i < nf; ++i) {
+    if (cout) {  // (a member whose consensus runs gets its result and scores below; without observations it fails)
+      memset(&cout[i], 0, sizeof(cout[i]));
+      cout[i].best = -1;
+      if (pl[i].cons) cout[i].status = 1;
+    }
+    if (pl[i].cons && cons[i].scores)
+      for (int k = 0; k < cons[i].hypotheses; ++k) cons[i].scores[k] = -1;
     if (!in[i].n_obs) continue;
     idx.push_back(i);
     static_cast<mb::LmkArgs<S>&>(args[i]) = eng[i]->lmk_args(in[i], pl[i].G, pl[i].ld);
     args[i].H = pl[i].H; args[i].max_iter = in[i].max_iter; args[i].tol = in[i].tol;
+    if (pl[i].cons) {
+      args[i].cons = 1; args[i].thresh = cons[i].thresh; args[i].min_inl = cons[i].min_inliers;
+      args[i].n_obs = in[i].n_obs; args[i].nh = (int)pl[i].hpair.size() / 2;
+      any_cons = true;
+    }
   }
   if (idx.empty()) return 0;
   const LmkSizes z = lmk_layout<S>(idx, in, pl, nullptr, nullptr, nullptr, h, args);
@@ -1929,6 +2007,10 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_
       memcpy(hm.sdesc, p.sdesc.data(), sizeof(int) * p.sdesc.size());
       for (size_t l = 0; l < p.lms.size(); ++l) memcpy(hm.lsig + 6 * l, mq->Sigma_L + 6 * (size_t)p.lms[l], sizeof(double) * 6);
     }
+    if (p.cons) {
+      memcpy(hm.pairs, p.hpair.data(), sizeof(int) * p.hpair.size());
+      memcpy(hm.ogrp, p.ogrp.data(), sizeof(int) * p.ogrp.size());
+    }
   }
   CK(cudaMemcpyAsync(io.d, io.h, z.in, cudaMemcpyHostToDevice, stream));
   per_member(idx, false, [&](int i) { return args[i]; },
@@ -1936,18 +2018,27 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_
                constexpr int NM = (int)std::extent<decltype(std::decay_t<decltype(a)>::m)>::value;
                mb::Members<mb::LmkArgs<S>, NM> b;  // the single linearisation's arguments, as they always were
                mb::Members<mb::LmkItArgs<S>, NM> c;  // the iterated form's
-               int gx = 1, tx = 1, K = 1, hx = 0;  // the largest member's grid; other members' CTAs past their own range exit at once
+               mb::Members<mb::LmkMapArgs<S>, NM> d;  // the map form's
+               int gx = 1, tx = 1, K = 1, hx = 0, hy = 0;  // the largest member's grid; other members' CTAs past their own range exit at once
                for (int j = 0; j < nm; ++j) {
-                 b.m[j] = a.m[j]; c.m[j] = a.m[j];
+                 b.m[j] = a.m[j]; c.m[j] = a.m[j]; d.m[j] = a.m[j];
                  gx = std::max(gx, a.m[j].G);
                  tx = std::max(tx, a.m[j].ntiles);
                  K = std::max(K, a.m[j].max_iter);
                  if (a.m[j].sig) hx = std::max(hx, std::max(1, a.m[j].H));
+                 if (a.m[j].cons) hy = std::max(hy, std::max(1, (a.m[j].nh + mb::kConsWarps - 1) / mb::kConsWarps));
                }
-               // MAP (a member has Sigma_L): clone, set and gain take the map arguments; else b (linearisation 0) and c
-               const auto lin = [&](auto map, const auto& x0, const auto& x1) {
-                 constexpr bool MAP = decltype(map)::value;
-                 mb::k_lmk_clone<S, NM, false, MAP><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(x0);
+               // MAP (a member has Sigma_L): clone, set and gain take the map arguments; else b (linearisation 0) and c.
+               // CONS (a member runs a consensus): k_lmk_hyp and k_lmk_cons, then linearisation 0's clone pre-set by them.
+               const auto lin = [&](auto map, auto cs, const auto& x0, const auto& x1) {
+                 constexpr bool MAP = decltype(map)::value, CONS = decltype(cs)::value;
+                 if constexpr (CONS) {
+                   mb::k_lmk_hyp<S, NM><<<dim3(hy, nm), mb::kConsWarps * 32, 0, stream>>>(a);
+                   mb::k_lmk_cons<S, NM><<<nm, mb::kLmkThreads, 0, stream>>>(a);
+                   mb::k_lmk_clone<S, NM, false, MAP, true><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(a);
+                 } else {
+                   mb::k_lmk_clone<S, NM, false, MAP><<<dim3(gx, nm), mb::kLmkThreads, 0, stream>>>(x0);
+                 }
                  if constexpr (MAP) mb::k_lmk_set<S, NM><<<dim3(hx, nm), mb::kLmkThreads, 0, stream>>>(x0);
                  mb::k_lmk_gain<S, NM, false, MAP><<<nm, mb::kLmkThreads, 0, stream>>>(x0);
                  for (int it = 0; it + 1 < K; ++it) {
@@ -1957,8 +2048,10 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_
                    mb::k_lmk_gain<S, NM, true, MAP><<<nm, mb::kLmkThreads, 0, stream>>>(x1);
                  }
                };
-               if (hx == 0) lin(std::false_type(), b, c);
-               else lin(std::true_type(), a, a);
+               if (hx == 0 && hy == 0) lin(std::false_type(), std::false_type(), b, c);
+               else if (hx == 0) lin(std::false_type(), std::true_type(), b, c);
+               else if (hy == 0) lin(std::true_type(), std::false_type(), d, d);
+               else lin(std::true_type(), std::true_type(), d, d);
                mb::k_lmk_downdate<S, NM><<<dim3(tx, nm), mb::kLmkThreads, 0, stream>>>(b);
              });
   CK(cudaGetLastError());
@@ -1975,6 +2068,11 @@ int Ctx<S>::landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_
     for (int j = 0; j < q.n_obs; ++j) {
       if (q.gamma) q.gamma[pl[i].perm[j]] = h[i].gamma[j];
       if (q.flag) q.flag[pl[i].perm[j]] = h[i].flag[j];
+    }
+    if (pl[i].cons) {
+      if (cout) memcpy(&cout[i], h[i].cres, sizeof(cout[i]));
+      if (cons[i].scores)
+        for (int k = 0; k < cons[i].hypotheses; ++k) cons[i].scores[k] = k < (int)pl[i].hpair.size() / 2 ? h[i].score[k] : -1;
     }
     if (o.numeric && numeric < 0) numeric = i;
   }
@@ -2174,6 +2272,12 @@ int msckf_b200_batch_map_landmark_update(msckf_b200_batch* b, const msckf_b200_l
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->landmarks(lm, map, out);
 }
+int msckf_b200_batch_landmark_update_consensus(msckf_b200_batch* b, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                               const msckf_b200_landmark_consensus* cons, msckf_b200_landmark_result* out,
+                                               msckf_b200_landmark_consensus_result* cons_out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->landmarks(lm, map, out, cons, cons_out);
+}
 
 int msckf_b200_update_batch(msckf_b200_engine** engines, int n, int mode, const msckf_b200_tracks* tracks, msckf_b200_report* reports,
                             int threads) {
@@ -2244,6 +2348,27 @@ int msckf_b200_map_landmark_update(msckf_b200_engine* e, const msckf_b200_landma
   const bool it_ok = lm->max_iter >= 0 && lm->max_iter <= mb::kLmkMaxIter && std::isfinite(lm->tol) && lm->tol >= 0.0;
   if (lm->n_obs == 0 && it_ok) { memset(out, 0, sizeof(*out)); return 0; }
   return e->impl->solo_ctx()->landmarks(lm, map, out);
+}
+// (an empty call with valid settings zeroes the result; a consensus of no observations fails)
+int msckf_b200_landmark_update_consensus(msckf_b200_engine* e, const msckf_b200_landmarks* lm, const msckf_b200_landmark_map* map,
+                                         const msckf_b200_landmark_consensus* cons, msckf_b200_landmark_result* out,
+                                         msckf_b200_landmark_consensus_result* cons_out) {
+  if (!e || !lm || !out) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (!cons || cons->hypotheses == 0) {
+    if (cons_out) { memset(cons_out, 0, sizeof(*cons_out)); cons_out->best = -1; }
+    return msckf_b200_map_landmark_update(e, lm, map, out);
+  }
+  if (lm->n_obs == 0) {
+    LmkPlan p;
+    RC(lmk_plan(*lm, nullptr, e->impl->M, "", p));
+    RC(lmk_cons_plan(*lm, *cons, "", p));
+    memset(out, 0, sizeof(*out));
+    if (cons_out) { memset(cons_out, 0, sizeof(*cons_out)); cons_out->best = -1; cons_out->status = 1; }
+    if (cons->scores)
+      for (int k = 0; k < cons->hypotheses; ++k) cons->scores[k] = -1;
+    return 0;
+  }
+  return e->impl->solo_ctx()->landmarks(lm, map, out, cons, cons_out);
 }
 int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->impl->set_covariance(in); }
 int msckf_b200_get_counters(msckf_b200_engine* e, long long* counters) { return e->impl->get_counters(counters); }

@@ -119,6 +119,34 @@ static_assert(sizeof(Members<LmkMapArgs<double>, kBatchMembers>) <= 32764, "the 
 template <class S, bool IT, bool MAP = false>
 using LmkArgsT = std::conditional_t<MAP, LmkMapArgs<S>, std::conditional_t<IT, LmkItArgs<S>, LmkArgs<S>>>;
 
+// Consensus on the map matches (DESIGN.md 4.17, consensus_kernels.cuh): k_lmk_hyp scores sampled 4-dof corrections of the
+// window, k_lmk_cons picks and refits the best and pre-sets flag 3 on the outliers, which k_lmk_clone<..., CONS> keeps.
+constexpr int kLmkMaxHyp = 1024;  // hypotheses of one member in one call
+struct LmkHyp {
+  double th[4];  // psi, t
+  int count;     // inliers (0 when not valid)
+  int valid;
+};
+// per-member consensus result; msckf_b200_landmark_consensus_result's fields at their offsets
+struct LmkConsOut {
+  int status, inliers, best, valid, refit;
+  double yaw, t[3], pivot[3];
+};
+template <class S>
+struct LmkConsArgs : LmkMapArgs<S> {
+  const int* pairs;  // [nh][2] the sampled observations (packed order)
+  const int* ogrp;   // [n_obs] each observation's group (touched clone) in grp
+  LmkHyp* hyp;       // [nh]
+  LmkConsOut* cres;
+  int* score;        // [nh] out: each hypothesis's inliers, or -1 when it is not valid
+  double thresh;     // inlier when depth > 0 and (z - z^)^T R^-1 (z - z^) <= thresh
+  int n_obs, nh, min_inl;
+  int cons;          // 0: the member runs no consensus (its consensus kernels return at once, its flags are not pre-set)
+};
+static_assert(sizeof(Members<LmkConsArgs<double>, kBatchMembers>) <= 32764, "the consensus kernels' arguments exceed the parameter limit");
+template <class S, bool IT, bool MAP, bool CONS>
+using LmkArgsC = std::conditional_t<CONS, LmkConsArgs<S>, LmkArgsT<S, IT, MAP>>;
+
 __host__ __device__ constexpr int lmk_tiles(int n) { return ((n + kLmkNB - 1) / kLmkNB) * ((n + kLmkNB - 1) / kLmkNB + 1) / 2; }
 
 // one observation against clone pose (C, p_C_G): rows [X | r] (2 x 7), flag (0 used, 1 gated out, 2 behind the camera or not
@@ -180,8 +208,11 @@ __device__ __forceinline__ void lmk_map_R(const double* o, const double* Cr, con
 // MAP: gamma includes F Sigma F^T; a one-clone landmark's rows are whitened by the Cholesky factor of R + F Sigma F^T (exact
 // marginalisation of its position), and the rows of a landmark seen from several clones go to its pair (whitened by L_R, with
 // the flag) instead of the clone's QR.  A member without Sigma runs the exact-map arithmetic.
-template <class S, int NM, bool IT = false, bool MAP = false>
-__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgsT<S, IT, MAP>, NM> a) {
+// CONS (linearisation 0 only): a consensus member's observation pre-set to flag 3 by k_lmk_cons keeps it unless it is flag 2;
+// gamma is written as without consensus.
+template <class S, int NM, bool IT = false, bool MAP = false, bool CONS = false>
+__global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgsC<S, IT, MAP, CONS>, NM> a) {
+  static_assert(!(CONS && IT), "consensus pre-sets linearisation 0's flags only");
   const int f = NM == 1 ? 0 : blockIdx.y, g = blockIdx.x;
   if constexpr (IT) {
     if (a.m[f].max_iter <= 1 || lmk_it_ended(a.m[f].it)) return;
@@ -237,6 +268,10 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
   }
   const double* const Ro = MAP ? Ri : Rm;  // the gate's observation noise
   if (t < cnt) {
+    [[maybe_unused]] int pre = 0;  // CONS: k_lmk_cons's flag
+    if constexpr (CONS) {
+      if (a.m[f].cons) pre = a.m[f].flag[i0 + t];
+    }
     if constexpr (MAP) {
       if (sg) lmk_map_R(obs, Cr, pc, sg + 6 * (size_t)(i0 + t), Ri);
     }
@@ -246,6 +281,9 @@ __global__ void __launch_bounds__(kLmkThreads) k_lmk_clone(const Members<LmkArgs
       if (f0 == 0 && fg == 2) a.m[f].it->stop = 1;
       fg = f0;
     } else {
+      if constexpr (CONS) {
+        if (pre == 3 && fg != 2) fg = 3;
+      }
       a.m[f].gamma[i0 + t] = gam;
       a.m[f].flag[i0 + t] = fg;
     }

@@ -206,13 +206,16 @@ class FilterBatch:
             o0 += c
         return res
 
-    def landmark_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
+    def landmark_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10, consensus=None):
         """MSCKFBatch::landmarkUpdate: obs[i] = (state_ids [n], z [n, 2], p_L [n, 3]) for filter i, or None (filter i left
         alone); R None (each filter's pixel noise) or 2 x 2; one device call for the batch; max_iter >= 2: the iterated update
         (at most max_iter linearisations, converged at max |delta_{i+1} - delta_i| <= tol).  A list of result dicts with
-        "gamma" and "flag" (None for a filter left alone)."""
+        "gamma" and "flag" (None for a filter left alone).  consensus (a capi.consensus_struct dict, or one per filter):
+        msckf_mono_batch_landmark_update_consensus, and each dict has a "consensus" dict."""
         from .capi import LandmarkResult
         n = len(self.filters)
+        if consensus is not None:
+            return self._landmark_consensus(obs, R, chi2_obs, max_iter, tol, consensus)
         assert len(obs) == n
         cnt = np.array([0 if o is None else len(o[0]) for o in obs], dtype=np.int32)
         parts = [o for o in obs if o is not None and len(o[0])]
@@ -231,6 +234,33 @@ class FilterBatch:
         for i in range(n):
             c = int(cnt[i])
             res.append(None if c == 0 else dict(out[i].as_dict(), gamma=gamma[o0:o0 + c].copy(), flag=flag[o0:o0 + c].copy()))
+            o0 += c
+        return res
+
+    def _landmark_consensus(self, obs, R, chi2_obs, max_iter, tol, consensus):
+        from .capi import LandmarkConsensus, LandmarkConsensusResult, LandmarkResult, consensus_struct
+        n = len(self.filters)
+        assert len(obs) == n
+        cl = list(consensus) if isinstance(consensus, (list, tuple)) else [consensus] * n
+        cs = [consensus_struct(c) for c in cl]
+        cnt = np.array([0 if o is None else len(o[0]) for o in obs], dtype=np.int32)
+        parts = [o for o in obs if o is not None and len(o[0])]
+        ids = np.ascontiguousarray(np.concatenate([np.asarray(o[0]) for o in parts]) if parts else np.zeros(1), dtype=np.int32)
+        z = np.ascontiguousarray(np.concatenate([np.asarray(o[1], float).reshape(-1, 2) for o in parts]) if parts else np.zeros((1, 2)))
+        p = np.ascontiguousarray(np.concatenate([np.asarray(o[2], float).reshape(-1, 3) for o in parts]) if parts else np.zeros((1, 3)))
+        r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
+        tot = max(int(cnt.sum()), 1)
+        gamma, flag = np.zeros(tot), np.zeros(tot, dtype=np.int32)
+        out, cout = (LandmarkResult * n)(), (LandmarkConsensusResult * n)()
+        self._call("landmark_update_consensus", cnt.ctypes.data_as(_ip), ids.ctypes.data_as(_ip), z.ctypes.data_as(_dp),
+                   p.ctypes.data_as(_dp), None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs),
+                   C.c_int(int(max_iter)), C.c_double(tol), (LandmarkConsensus * n)(*[c for c, _ in cs]),
+                   gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip), out, cout)
+        res, o0 = [], 0
+        for i in range(n):
+            c = int(cnt[i])
+            res.append(None if c == 0 else dict(out[i].as_dict(), gamma=gamma[o0:o0 + c].copy(), flag=flag[o0:o0 + c].copy(),
+                                                consensus=cout[i].as_dict(cs[i][1][0] if cs[i][1] else None)))
             o0 += c
         return res
 
@@ -477,12 +507,29 @@ class CFilter:
                                         C.byref(out)), "map_update")
         return dict(out.as_dict(), gamma=gamma[:n].copy(), flag=flag[:n].copy())
 
-    def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
+    def landmark_update(self, state_ids, z, p_L, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10, consensus=None):
         """MSCKF::landmarkUpdate (include/msckf_b200.h: msckf_b200_landmark_update): observations of known landmarks p_L [n, 3]
         at z [n, 2] from the images state_ids [n]; R None (the filter's pixel noise) or 2 x 2; chi2_obs > 0: per-observation
         gate; max_iter >= 2: the iterated update.  A dict nis, dx_norm, dof, rows, used, applied, status, iterations,
-        converged, step, gamma [n], flag [n]."""
+        converged, step, gamma [n], flag [n].  consensus (a capi.consensus_struct dict): msckf_mono_landmark_update_consensus,
+        and the dict has a "consensus" dict."""
         from .capi import LandmarkResult
+        if consensus is not None:
+            from .capi import LandmarkConsensusResult, consensus_struct
+            ids = np.ascontiguousarray(state_ids, dtype=np.int32).ravel()
+            n = len(ids)
+            z, pz = _d(np.asarray(z, float).reshape(-1, 2) if n else np.zeros((1, 2)))
+            p, pp = _d(np.asarray(p_L, float).reshape(-1, 3) if n else np.zeros((1, 3)))
+            r3 = None if R is None else np.array([R[0][0], R[1][0], R[1][1]], dtype=np.float64)
+            gamma, flag = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int32)
+            c, ck = consensus_struct(consensus)
+            out, cout = LandmarkResult(), LandmarkConsensusResult()
+            self._chk(self._f("landmark_update_consensus")(self.h, C.c_int(n), ids.ctypes.data_as(_ip), pz, pp,
+                                                           None if r3 is None else r3.ctypes.data_as(_dp), C.c_double(chi2_obs),
+                                                           C.c_int(int(max_iter)), C.c_double(tol), C.byref(c),
+                                                           gamma.ctypes.data_as(_dp), flag.ctypes.data_as(_ip), C.byref(out),
+                                                           C.byref(cout)), "landmark_update_consensus")
+            return dict(out.as_dict(), gamma=gamma[:n].copy(), flag=flag[:n].copy(), consensus=cout.as_dict(ck[0] if ck else None))
         ids = np.ascontiguousarray(state_ids, dtype=np.int32).ravel()
         n = len(ids)
         z, pz = _d(np.asarray(z, float).reshape(-1, 2) if n else np.zeros((1, 2)))

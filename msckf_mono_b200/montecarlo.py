@@ -564,8 +564,14 @@ def _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows):
             "first_bad_pivot": [int(r["first_bad_pivot"]) for r in nees_rows],
             "pos_err2": [float(x) for x in pos_err2],
             "fix_nis": [float(x) for x in fix_nis],
-            "map": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in map_rows] for key in ("nis", "dof", "used", "applied", "n")},
+            "map": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in map_rows]
+                    for key in ("nis", "dof", "used", "applied", "n") + (CONS_KEYS if map_rows and "wrong" in map_rows[0] else ())},
             "odometry": {key: [float(r[key]) if key == "nis" else int(r[key]) for r in odo_rows] for key in ("nis", "dof", "applied")}}
+
+
+# per map update with wrong matches injected or a consensus: wrong matches, those left out of the update (any flag but 0: excluded
+# by consensus, gated out or behind the camera), right ones, those used (flag 0), and the consensus status (-1: none ran)
+CONS_KEYS = ("wrong", "wrong_excluded", "right", "right_kept", "cons_status")
 
 
 def chi2_bounds(total_dof, n, lo=0.025, hi=0.975):
@@ -720,7 +726,8 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         gnss_as_position=False, heading_every=0, heading_sigma=0.01, heading_axis=(1.0, 0.0, 0.0), range_every=0, range_sigma=0.1,
         range_lever=(0.0, 0.0, 0.0), range_delay=0, plane_every=0, plane_sigma=0.02, plane_height=PLANE_HEIGHT, plane_axis=PLANE_AXIS,
         plane_lever=(0.0, 0.0, 0.0), range_outlier_rate=0.0, range_outlier_bias=1.0, gnss_outlier_rate=0.0, gnss_outlier_jump=5.0,
-        fde_alpha=0.0, fde_max_exclude=2, range_start=0, gnss_start=0, aid_iterations=1, aid_tol=1e-10):
+        fde_alpha=0.0, fde_max_exclude=2, range_start=0, gnss_start=0, aid_iterations=1, aid_tol=1e-10, map_outlier_rate=0.0,
+        map_consensus=0, map_consensus_thresh=13.8, map_min_inliers=6):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
@@ -741,7 +748,10 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     observation at map_chi2 > 0, iterated up to map_iterations linearisations; the map carries N(0, map_sigma^2 I) errors and
     is observed from the map_clones newest clones that are still in the window (make_trial); map_uncertain passes
     Sigma = map_sigma^2 I per landmark (MSCKFBatch::landmarkUpdate over mapObservation / mapLandmark), else the map is taken as
-    exact],
+    exact; each map observation is a wrong match with probability map_outlier_rate (its p_L swapped for another map
+    landmark's, drawn from the stream default_rng([seed, k, 12]); no draw when the rate is 0), and map_consensus H > 0 selects the
+    inliers by a consensus of H hypotheses (threshold map_consensus_thresh, min_inliers map_min_inliers, seed [seed, k, frame])
+    before each map update (exact map only); with either, each map row also counts wrong matches left out of the update and right ones used],
     refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.  The first
     map update is also recorded on its own (trial_record's map_first; the state is read just before it).
     Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
@@ -749,6 +759,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     from .capi import AID_POSITION
     from .cview import FilterBatch
     assert not map_uncertain or map_sigma > 0, "map_uncertain needs map_sigma > 0"
+    assert not (map_uncertain and map_consensus), "the consensus runs on the exact-map update here"
     assert not (gnss_as_position and gnss_delay), "gnss_as_position fuses at the IMU: no delay"
     trs = [make_trial(truth, k, seed, fix_every, fix_sigma, map_every, map_stride, odo_every, map_start, map_sigma, map_clones,
                       gnss_every, heading_every, range_every, plane_every, range_start=range_start, gnss_start=gnss_start)
@@ -770,6 +781,23 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
             g_out.append((rg.random(n_fr) < gnss_outlier_rate, rg.uniform(0.0, 2.0 * np.pi, n_fr)))
         else:
             g_out.append(None)
+
+    m_rng = [np.random.default_rng([seed, tr["k"], 12]) if map_outlier_rate > 0 else None for tr in trs]
+    m_pts = [tr.get("map_points", truth["landmarks"][::map_stride]) for tr in trs]
+
+    def map_faults(i, o):
+        """make some of filter i's map matches wrong in place; their mask"""
+        if o is None:
+            return None
+        n = len(o[0])
+        if m_rng[i] is None:
+            return np.zeros(n, dtype=bool)
+        bad = m_rng[i].random(n) < map_outlier_rate
+        pts = m_pts[i]
+        for j in np.flatnonzero(bad):
+            cur = int(np.flatnonzero(np.all(pts == o[2][j], axis=1))[0])
+            o[2][j] = pts[(cur + 1 + int(m_rng[i].integers(len(pts) - 1))) % len(pts)]
+        return bad
 
     def range_faults(i, g, items):
         if r_out[i] is None or not items or items[0]["model"] not in (AID_RANGE, AID_CLONE_RANGE):
@@ -863,16 +891,31 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
                 range_faults if range_outlier_rate > 0 else None, fde, iterate))
         if map_every > 0 and trs[0]["maps"][fi] is not None:
             obs = [map_call(tr, f, fi, map_uncertain, S_map) for tr, f in zip(trs, fs)]
+            track = map_outlier_rate > 0 or map_consensus > 0
+            if track:
+                obs = [None if o is None else (o[0], o[1], np.array(o[2], dtype=np.float64)) for o in obs]
+                wrong = [map_faults(i, o) for i, o in enumerate(obs)]
             if first[0] is None:
                 fb.refreshState()
                 for i, (f, tr) in enumerate(zip(fs, trs)):
                     first[i] = {"frame": fi, "pos_err2_before": float(np.sum((truth_imu_of(truth, tr, fi)[0:3] - f.getImuState()["p_I_G"]) ** 2))}
             if map_uncertain:
                 res = fb.map_update(obs, chi2_obs=map_chi2, max_iter=map_iterations)
+            elif map_consensus > 0:
+                cons = [{"hypotheses": map_consensus, "thresh": map_consensus_thresh, "min_inliers": map_min_inliers,
+                         "seed": int(np.random.SeedSequence([seed, tr["k"], fi]).generate_state(1, np.uint64)[0])} for tr in trs]
+                res = fb.landmark_update(obs, chi2_obs=map_chi2, max_iter=map_iterations, consensus=cons)
             else:
                 res = fb.landmark_update(obs, chi2_obs=map_chi2, max_iter=map_iterations)
             for i, r in enumerate(res):
-                maps[i].append({"nis": 0.0, "dof": 0, "used": 0, "applied": 0, "n": 0} if r is None else dict(r, n=len(r["flag"])))
+                row = {"nis": 0.0, "dof": 0, "used": 0, "applied": 0, "n": 0} if r is None else dict(r, n=len(r["flag"]))
+                if track:
+                    w = wrong[i] if r is not None else np.zeros(0, dtype=bool)
+                    fl = r["flag"] if r is not None else np.zeros(0, dtype=np.int32)
+                    row.update(wrong=int(w.sum()), wrong_excluded=int((w & (fl != 0)).sum()), right=int((~w).sum()),
+                               right_kept=int((~w & (fl == 0)).sum()),
+                               cons_status=int(r["consensus"]["status"]) if r is not None and "consensus" in r else -1)
+                maps[i].append(row)
                 if first[i]["frame"] == fi:
                     first[i].update({k: (float if k == "nis" else int)(r[k]) if r is not None else 0 for k in ("nis", "dof", "iterations", "converged")})
         fb.refreshState()

@@ -9,7 +9,10 @@ max_iter K with tol 0 (so every call makes its K linearisations unless a step is
 linearisations the calls reported and the per-kernel split (k_lmk_step too) for 100 over 5.  Reads the card's name and power
 limit in the same process.  With --map-sigma S, it times the update with map uncertainty instead: 25 and 100 landmarks, each
 seen from the newest 1 and 5 clones, with Sigma = S^2 I (msckf_b200_map_landmark_update) against the same observations with
-Sigma NULL, for 1 / 8 / 32 filters.  Prints one JSON line."""
+Sigma NULL, for 1 / 8 / 32 filters.  With --consensus H ..., it times the update with a consensus of H hypotheses
+(msckf_b200_landmark_update_consensus) against the plain call on the same 100 observations over the newest 5 clones, 30 % of
+them wrong matches, for 1 / 8 / 32 filters, with the per-kernel split (k_lmk_hyp, k_lmk_cons too) at 1 and 32 filters.
+Prints one JSON line."""
 import argparse
 import json
 import subprocess
@@ -112,7 +115,7 @@ def kernel_times(fn, reps=50):
         torch.cuda.synchronize()
     out = {}
     for ev in prof.key_averages():
-        for name in ("k_lmk_clone", "k_lmk_set", "k_lmk_gain", "k_lmk_step", "k_lmk_downdate"):
+        for name in ("k_lmk_hyp", "k_lmk_cons", "k_lmk_clone", "k_lmk_set", "k_lmk_gain", "k_lmk_step", "k_lmk_downdate"):
             if name in ev.key:
                 out[name] = out.get(name, 0.0) + ev.device_time_total / 1e3 / reps  # ms per call
     return out
@@ -192,11 +195,47 @@ def uncertain(sigma):
     print(json.dumps(res), flush=True)
 
 
+def consensus(hs):
+    res = {"gpu": gpu_line(), "dtype": "f64", "clones": M, "obs": 100, "wrong": 0.3, "call_ms": {}, "kernel_ms": {}, "inliers": {}}
+    for nf in (1, 8, 32):
+        for h in [0] + list(hs):  # fresh filters for each setting: the timed calls apply their updates
+            fs, es = filters(nf)
+            b = capi.Batch(es) if nf > 1 else None
+            specs = []
+            for i, e in enumerate(es):
+                rng = np.random.default_rng([nf, i])
+                sp = observations(rng, e, 100, 5)
+                wrong = np.flatnonzero(rng.uniform(size=100) < 0.3)
+                sp["p_L"][wrong] = sp["p_L"][(wrong + 1 + rng.integers(99, size=len(wrong))) % 100]
+                specs.append(sp)
+            cs = None if h == 0 else {"hypotheses": h, "thresh": 13.8, "min_inliers": 10, "seed": 1}
+            key = f"{nf}x100obs/5clones/" + ("plain" if h == 0 else f"consensus{h}")
+            out = []
+            fn = (lambda: out.append(b.landmark_update(specs, consensus=cs))) if b else \
+                (lambda: out.append([es[0].landmark_update(**specs[0], consensus=cs)]))
+            res["call_ms"][key] = timed(fn)
+            if h:
+                res["inliers"][key] = float(np.mean([o["consensus"]["inliers"] for o in out[0]]))  # the first call, on the unchanged filters
+            if nf in (1, 32):
+                try:
+                    res["kernel_ms"][key] = kernel_times(fn)
+                except Exception as ex:  # (the profiler is an extra; the call times above stand on their own)
+                    res["kernel_ms"][key] = f"not measured: {ex}"
+            if b:
+                b.close()
+            for f in fs:
+                f.close()
+    print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--consensus", type=int, nargs="*", default=None, help="time consensus calls of these hypothesis counts")
     ap.add_argument("--iterations", type=int, nargs="*", default=None)
     ap.add_argument("--map-sigma", type=float, default=None, help="time Sigma = s^2 I against Sigma NULL")
     args = ap.parse_args()
+    if args.consensus:
+        return consensus(args.consensus)
     if args.iterations:
         return iterated(args.iterations)
     if args.map_sigma is not None:

@@ -165,6 +165,11 @@ def main():
     ap.add_argument("--map-sigma", type=float, default=0.0, help="each trial's map = the truth map + N(0, s^2 I) per landmark")
     ap.add_argument("--map-uncertain", action="store_true", help="fuse the map with Sigma = s^2 I (else it is taken as exact)")
     ap.add_argument("--map-clones", type=int, default=1, help="observe the map from the K newest clones (K <= --map-every)")
+    ap.add_argument("--map-chi2", type=float, default=0.0, help="> 0: gate each map observation on its own at this chi^2")
+    ap.add_argument("--map-outlier-rate", type=float, default=0.0, help="each map observation a wrong match with this probability")
+    ap.add_argument("--map-consensus", type=int, default=0, help="> 0: select map inliers by a consensus of this many hypotheses")
+    ap.add_argument("--map-consensus-thresh", type=float, default=13.8)
+    ap.add_argument("--map-min-inliers", type=int, default=6)
     ap.add_argument("--odometry-every", type=int, default=0)
     ap.add_argument("--odometry-sigma-v", type=float, default=0.05)
     ap.add_argument("--odometry-sigma-rel", type=float, default=0.01)
@@ -222,7 +227,9 @@ def main():
                         range_outlier_bias=args.range_outlier_bias, gnss_outlier_rate=args.gnss_outlier_rate,
                         gnss_outlier_jump=args.gnss_outlier_jump, fde_alpha=args.fde_alpha, fde_max_exclude=args.fde_max_exclude,
                         range_start=args.range_start, gnss_start=args.gnss_start, aid_iterations=args.aid_iterations,
-                        aid_tol=args.aid_tol)
+                        aid_tol=args.aid_tol, map_chi2=args.map_chi2, map_outlier_rate=args.map_outlier_rate,
+                        map_consensus=args.map_consensus, map_consensus_thresh=args.map_consensus_thresh,
+                        map_min_inliers=args.map_min_inliers)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -236,6 +243,15 @@ def main():
         res["map"] = {"every": args.map_every, "stride": args.map_stride,
                       **{k: s["map"][k] for k in ("mean_anis", "mean_dof", "run_bounds", "updates_inside", "applied", "observations", "gated")}}
         res["map"].update(sigma_m=args.map_sigma, uncertain=args.map_uncertain, clones=args.map_clones)
+        res["map"].update(chi2=args.map_chi2)
+        if args.map_outlier_rate > 0 or args.map_consensus > 0:
+            tot = {k: sum(sum(r["map"][k]) for r in merged.values()) for k in ("wrong", "wrong_excluded", "right", "right_kept")}
+            st = [x for r in merged.values() for x in r["map"]["cons_status"]]
+            res["map"].update(outlier_rate=args.map_outlier_rate, consensus=args.map_consensus,
+                              consensus_thresh=args.map_consensus_thresh, min_inliers=args.map_min_inliers, **tot,
+                              wrong_excluded_share=tot["wrong_excluded"] / max(tot["wrong"], 1),
+                              right_kept_share=tot["right_kept"] / max(tot["right"], 1),
+                              consensus_status={str(v): st.count(v) for v in sorted(set(st))})
         if args.map_start or args.map_iterations != 1:
             res["map"].update(start=args.map_start, iterations=args.map_iterations, first_update=s["map_first"])
     if "odometry" in s:

@@ -19,3 +19,11 @@ timeout 1500 compute-sanitizer --tool racecheck --racecheck-report all --error-e
 echo "racecheck exit $?" >> $OUT/r02_racecheck_pytest.log
 tail -n 3 $OUT/r02_memcheck_pytest.log $OUT/r02_memcheck_side_pytest.log $OUT/r02_racecheck_pytest.log
 tail -n 5 $OUT/r02_memcheck.log $OUT/r02_memcheck_side.log $OUT/r02_racecheck.log
+# the consensus on mapped-landmark matches (k_lmk_hyp, k_lmk_cons, k_lmk_clone<..., CONS>) at every shape of its GPU tests
+timeout 1500 compute-sanitizer --tool memcheck --leak-check no --error-exitcode 9 --log-file $OUT/r02_memcheck_consensus.log \
+  python -m pytest tests/test_landmark_consensus_gpu.py -m gpu -q -x > $OUT/r02_memcheck_consensus_pytest.log 2>&1
+echo "memcheck exit $?" >> $OUT/r02_memcheck_consensus_pytest.log
+timeout 1500 compute-sanitizer --tool racecheck --racecheck-report all --error-exitcode 9 --log-file $OUT/r02_racecheck_consensus.log \
+  python -m pytest tests/test_landmark_consensus_gpu.py -m gpu -q -x > $OUT/r02_racecheck_consensus_pytest.log 2>&1
+echo "racecheck exit $?" >> $OUT/r02_racecheck_consensus_pytest.log
+tail -n 3 $OUT/r02_memcheck_consensus_pytest.log $OUT/r02_racecheck_consensus_pytest.log
