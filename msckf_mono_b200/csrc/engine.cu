@@ -42,7 +42,7 @@ int fail(int code, const std::string& msg) { g_err = msg; return code; }
   } while (0)
 #define RC(call) do { int rc_ = (call); if (rc_ != 0) return rc_; } while (0)
 
-constexpr int kMaxSplit = 16;
+using mb::kMaxSplit;  // split-K chunks of the Gram products (gram_kernels.cuh)
 constexpr int kJacBatchGroup = 32;  // k_jac threads per track in a device batch (DESIGN.md 4.2)
 constexpr int kTailCluster = 8;  // portable cluster size: the serial EKF tail runs on 8 SMs of one GPC
 constexpr size_t kSmemBudget = 220 * 1024;  // dynamic shared memory per CTA, under H100's 227 KB opt-in limit
@@ -1181,7 +1181,7 @@ int Ctx<S>::launch() {
   sh.tri_gx = (Nr + 3) / 4; sh.jac_gx = Nr / (sh.jac_g == 128 ? 1 : 2); sh.rows_gx = Nr; sh.bd_gx = Mmax_;
   const int c = nmax_ - mb::kImuDim, ntile = (c + mb::GT - 1) / mb::GT;
   sh.gram_gx = ntile * (ntile + 1) / 2; sh.gram_gy = nsplit;
-  sh.asm_gx = std::min(4 * num_sms(device), (nmax_ * nmax_ + 255) / 256);
+  sh.asm_gx = mb::asm_ctas(c);
   sh.rows_smem = (unsigned)(sizeof(double) * mb::rows_smem_doubles((Lm + 7) & ~7));
   sh.gemm_g = (nmax_ + 31) / 32;
   sh.syrk_gx = sh.gemm_g * (sh.gemm_g + 1) / 2;  // lower 32 x 32 tile pairs (k_gemm_s, k_syrk)
@@ -1295,7 +1295,7 @@ int Ctx<S>::run_kernels(const LaunchShape& sh) {
     launches++;
     mark("k_gram");
     if (fork) CK(cudaStreamWaitEvent(stream, ev_join, 0));
-    CK(launch_k(mb::k_assemble<S>, dim3(sh.asm_gx, 1, nf), dim3(256), 0, stream, false, 1, A));
+    CK(launch_k(mb::k_assemble<S>, dim3(sh.asm_gx, 1, nf), dim3(mb::kAsmThreads), 0, stream, false, 1, A));
     launches++;
     mark("k_assemble");
     if (fork) CK(cudaStreamWaitEvent(stream, ev_join2, 0));

@@ -22,6 +22,7 @@ namespace mb {
 
 constexpr int GT = 32;   // output tile
 constexpr int GK = 16;   // k-step
+constexpr int kMaxSplit = 16;  // split-K chunks of the Gram products, at most
 
 // Partial Gram products over a K-split: G1p[s] = Z^T Z, G2p[s] = Z^T Yq + Yq^T Z, upper tiles only.
 template <class S>
@@ -113,8 +114,11 @@ __global__ void __launch_bounds__(256) k_gram(const UpdArgs<S>* __restrict__ arg
 }
 
 // The same partial Gram products on the FP64 tensor-core path: mma.sync.aligned.m8n8k4.row.col.f64 (SASS: DMMA), 4 warps per
-// CTA, one 32 x 32 output tile per CTA, each warp a 16 x 16 quadrant = 2 x 2 MMA tiles for G1 and for G2 (12 DMMA per 4-deep
-// k-step against 8 fragment loads; the SIMT form above needs 32 LDS + 48 DFMA warp instructions for the same k-step).
+// CTA, one 32 x 32 output tile per CTA, each warp a 16 x 16 quadrant = 2 x 2 MMA tiles for G1 and for G2, issued as two
+// m16n8k4 per product (6 DMMA per 4-deep k-step against 8 fragment loads; the SIMT form above needs 32 LDS + 48 DFMA warp
+// instructions for the same k-step).  m16n8k4 computes each output as two m8n8k4 would, bit for bit, in half the DMMA
+// instructions: 53.7 -> 49.6 us at a batch of 8 config-B filters, 17.1 -> 15.1 us for one (H100 80GB HBM3, 700 W).
+// 3 CTAs per SM, as without the bound (168 registers).
 // Fragments (PTX ISA, m8n8k4 .f64): A (8x4, row): lane l holds A[l/4][l%4]; B (4x8, col): lane l holds B[l%4][l/4];
 // C/D (8x8): lane l holds C[l/4][2(l%4)] and C[l/4][2(l%4)+1].  Here A = Z^T (or Yq^T) and B = Z (or Yq) of a k-slab
 // staged in shared memory k-major with a row stride of 36 doubles (== 4 mod 16: the 16 lanes of a half warp hit 16 banks pairs).
@@ -123,8 +127,14 @@ constexpr int GL = GT + 4;
 __device__ __forceinline__ void dmma(double (&c)[2], double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c[0]), "+d"(c[1]) : "d"(a), "d"(b));
 }
+// Both 8 x 8 row tiles of a quadrant column in one m16n8k4: rows 0-7 (c0, a[0]) and rows 8-15 (c8, a[1]); lane l holds
+// A[l/4][l%4] and A[8 + l/4][l%4], B[l%4][l/4], C[l/4][2(l%4) + {0,1}] and C[8 + l/4][2(l%4) + {0,1}].
+__device__ __forceinline__ void dmma16(double (&c0)[2], double (&c8)[2], const double (&a)[2], double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(c0[0]), "+d"(c0[1]), "+d"(c8[0]), "+d"(c8[1]) : "d"(a[0]), "d"(a[1]), "d"(b));
+}
 template <class S>
-__global__ void __launch_bounds__(128) k_gram_mma(const UpdArgs<S>* __restrict__ args) {
+__global__ void __launch_bounds__(128, 3) k_gram_mma(const UpdArgs<S>* __restrict__ args) {
   pdl_wait();
   pdl_launch();
   const UpdArgs<S>& A = args[blockIdx.z];
@@ -185,13 +195,11 @@ __global__ void __launch_bounds__(128) k_gram_mma(const UpdArgs<S>* __restrict__
 #pragma unroll
       for (int j = 0; j < 2; ++j) { bz[j] = sZb[ks + fk][wn + 8 * j + fr]; by[j] = sYb[ks + fk][wn + 8 * j + fr]; }
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          dmma(c1[i][j], az[i], bz[j]);
-          dmma(c2[i][j], az[i], by[j]);
-          dmma(c2[i][j], ay[i], bz[j]);
-        }
+      for (int j = 0; j < 2; ++j) {
+        dmma16(c1[0][j], c1[1][j], az, bz[j]);
+        dmma16(c2[0][j], c2[1][j], az, by[j]);
+        dmma16(c2[0][j], c2[1][j], ay, bz[j]);
+      }
     }
     if (diag) {
 #pragma unroll
@@ -276,65 +284,100 @@ __global__ void __launch_bounds__(128) k_blockdiag(const UpdArgs<S>* __restrict_
   }
 }
 
-// Assemble T'' (n x n), r'' (n), R'' (n x n) except the <=15 head rows (k_head fills those afterwards).
+// Assemble T'' (n x n), r'' (n), R'' (n x n) except the <=15 head rows (k_rows fills those beside this kernel).
+// Grid: GT / kAsmRows CTAs per upper 32-tile pair (ta <= tb) of the c x c Gram block, each kAsmRows rows of the tile, then one
+// border CTA (the T'' columns < 15 and r'').  A tile CTA issues the 2 nsplit coalesced row loads of its partials before summing
+// them, in split order from 0.0, and writes its rows of the tile and, for ta < tb, the matching columns of the mirror tile
+// through a shared-memory transpose, so that both stores are coalesced.  The mirror takes the same partial sums and its own
+// block-diagonal term.  A diagonal 32-tile is read in both halves (the Gram kernels write both; G2's (i, j) and (j, i) add
+// Z^T Yq and Yq^T Z in opposite order and need not agree bit for bit).
+// When m <= n (plain uncompressed update) every CTA of the grid zeroes its share of the rows >= m.
+constexpr int kAsmThreads = 256;
+// rows of a tile per CTA: 15.3 us at a batch of 8 config-B filters, 8.5 us for one (8 rows: 16.8 / 7.6 us; 32 rows: 14.5 /
+// 10.5 us; H100 80GB HBM3, 700 W)
+constexpr int kAsmRows = 16;
+__host__ __device__ inline int asm_ctas(int c) {
+  const int ntile = (c + GT - 1) / GT;
+  return ntile * (ntile + 1) / 2 * (GT / kAsmRows) + 1;
+}
 template <class S>
-__device__ __forceinline__ void assemble_work(const UpdArgs<S>& A, int cta, int ncta) {
+__global__ void __launch_bounds__(kAsmThreads) k_assemble(const UpdArgs<S>* __restrict__ args) {
+  pdl_wait();
+  pdl_launch();
+  const UpdArgs<S>& A = args[blockIdx.z];
   if (A.n_tracks == 0) return;
   const int n = A.n, ld = A.ld, nsplit = A.nsplit;
-  const double* __restrict__ G1p = A.G1p;
-  const double* __restrict__ G2p = A.G2p;
   const double* __restrict__ D1 = A.D1;
   const double* __restrict__ D2 = A.D2;
-  const double* __restrict__ bb = A.bb;
-  const int* __restrict__ m_in = A.m_out;
   double* __restrict__ T2 = A.T2;
   double* __restrict__ R2 = A.R2;
   double* __restrict__ r2 = A.r2;
   const int c = n - kImuDim;
-  const int m = *m_in;
-  const bool full = m <= n;  // m <= n: plain uncompressed update, all rows explicit (k_rows), no Gram part
+  const int m = *A.m_out;
+  const int tid = threadIdx.x;
   // The explicit head rows belong to k_rows, which runs BESIDE this kernel (side branch of the graph): rows < hcap of T'', R''
   // and r'', and -- when compressing -- columns < 15 of R'' (the coupling R_hH^T), are neither read nor written here.
-  const int hcap = full ? m : kImuDim, ccap = full ? 0 : kImuDim;
-  const size_t total = (size_t)n * n;
-  for (size_t e = (size_t)cta * 256 + threadIdx.x; e < total; e += (size_t)ncta * 256) {
-    const int a = (int)(e / n), b = (int)(e % n);
-    if (a < hcap) continue;
-    double tv = 0.0, rv = 0.0;
-    if (!full && a >= kImuDim && b >= kImuDim) {
-      const int ac = a - kImuDim, bc = b - kImuDim;
-      // the Gram kernel wrote upper tiles only
-      const bool upper = (ac / GT) <= (bc / GT);
-      const size_t off = upper ? ((size_t)ac * c + bc) : ((size_t)bc * c + ac);
-      double g1 = 0.0, g2 = 0.0;
-      for (int s = 0; s < nsplit; ++s) { g1 += G1p[(size_t)s * c * c + off]; g2 += G2p[(size_t)s * c * c + off]; }
-      double d1 = 0.0, d2 = 0.0;
-      if (ac / 6 == bc / 6) { d1 = D1[36 * (size_t)(ac / 6) + 6 * (ac % 6) + (bc % 6)]; d2 = D2[36 * (size_t)(ac / 6) + 6 * (ac % 6) + (bc % 6)]; }
-      tv = d1 - g1;
-      rv = d2 - g2;
+  if (m <= n) {  // every stacked row explicit (k_rows), no Gram part: rows >= m are zero
+    const size_t total = (size_t)(n - m) * n;
+    for (size_t e = (size_t)blockIdx.x * kAsmThreads + tid; e < total; e += (size_t)gridDim.x * kAsmThreads) {
+      const int a = m + (int)(e / n), b = (int)(e % n);
+      T2[(size_t)a * ld + b] = 0.0;
+      R2[(size_t)a * ld + b] = 0.0;
     }
-    T2[(size_t)a * ld + b] = tv;
-    if (b >= ccap) R2[(size_t)a * ld + b] = rv;
+    for (int a = m + blockIdx.x * kAsmThreads + tid; a < n; a += gridDim.x * kAsmThreads) r2[a] = 0.0;
+    return;
   }
-  // beta = blk(sum X^T r) - Z^T (U^T r); the second term arrives as split-K partials from the Gram kernel's diagonal tiles
-  const double* __restrict__ bzp = A.bzp;
-  for (int a = cta * 256 + threadIdx.x; a < n; a += ncta * 256) {
-    if (a < hcap) continue;
-    double v = 0.0;
-    if (!full && a >= kImuDim) {
-      const int ac = a - kImuDim;
+  constexpr int kParts = GT / kAsmRows;
+  const int ntile = (c + GT - 1) / GT, nwork = ntile * (ntile + 1) / 2 * kParts;
+  if ((int)blockIdx.x > nwork) return;
+  if ((int)blockIdx.x == nwork) {  // border: T'' columns < 15 of rows >= 15, and beta = blk(sum X^T r) - Z^T (U^T r)
+    for (int e = tid; e < c * kImuDim; e += kAsmThreads) T2[(size_t)(kImuDim + e / kImuDim) * ld + e % kImuDim] = 0.0;
+    // Z^T (U^T r) arrives as split-K partials from the Gram kernels' diagonal tiles
+    const double* __restrict__ bzp = A.bzp;
+    for (int ac = tid; ac < c; ac += kAsmThreads) {
       double t = 0.0;
       for (int s = 0; s < nsplit; ++s) t += bzp[(size_t)s * c + ac];
-      v = bb[ac] - t;
+      r2[kImuDim + ac] = A.bb[ac] - t;
     }
-    r2[a] = v;
+    return;
   }
-}
-template <class S>
-__global__ void __launch_bounds__(256) k_assemble(const UpdArgs<S>* __restrict__ args) {
-  pdl_wait();
-  pdl_launch();
-  assemble_work(args[blockIdx.z], blockIdx.x, gridDim.x);
+  int pidx = blockIdx.x / kParts, ta = 0;
+  while (pidx >= ntile - ta) { pidx -= ntile - ta; ++ta; }
+  const int tb = ta + pidx, r0 = (blockIdx.x % kParts) * kAsmRows;
+  __shared__ double sT[GT][kAsmRows + 1], sR[GT][kAsmRows + 1];  // this CTA's columns of the mirror tile
+  const int tx = tid & 31, ty = tid >> 5;
+  const int bc = tb * GT + tx;
+  const size_t cc = (size_t)c * c;
+#pragma unroll 1
+  for (int r = ty; r < kAsmRows; r += kAsmThreads / GT) {
+    const int ac = ta * GT + r0 + r;
+    if (ac < c && bc < c) {
+      const double* __restrict__ p1 = A.G1p + (size_t)ac * c + bc;
+      const double* __restrict__ p2 = A.G2p + (size_t)ac * c + bc;
+      double v1[kMaxSplit], v2[kMaxSplit];
+#pragma unroll
+      for (int s = 0; s < kMaxSplit; ++s)
+        if (s < nsplit) { v1[s] = p1[s * cc]; v2[s] = p2[s * cc]; }
+      double g1 = 0.0, g2 = 0.0;
+#pragma unroll
+      for (int s = 0; s < kMaxSplit; ++s)
+        if (s < nsplit) { g1 += v1[s]; g2 += v2[s]; }
+      const bool blk = ac / 6 == bc / 6;
+      const size_t d = 36 * (size_t)(ac / 6), dab = d + 6 * (ac % 6) + (bc % 6), dba = d + 6 * (bc % 6) + (ac % 6);
+      T2[(size_t)(kImuDim + ac) * ld + kImuDim + bc] = (blk ? D1[dab] : 0.0) - g1;
+      R2[(size_t)(kImuDim + ac) * ld + kImuDim + bc] = (blk ? D2[dab] : 0.0) - g2;
+      if (ta < tb) { sT[tx][r] = (blk ? D1[dba] : 0.0) - g1; sR[tx][r] = (blk ? D2[dba] : 0.0) - g2; }
+    }
+  }
+  if (ta == tb) return;
+  __syncthreads();
+  for (int e = tid; e < GT * kAsmRows; e += kAsmThreads) {
+    const int mr = tb * GT + e / kAsmRows, mc = ta * GT + r0 + e % kAsmRows;
+    if (mr < c && mc < c) {
+      T2[(size_t)(kImuDim + mr) * ld + kImuDim + mc] = sT[e / kAsmRows][e % kAsmRows];
+      R2[(size_t)(kImuDim + mr) * ld + kImuDim + mc] = sR[e / kAsmRows][e % kAsmRows];
+    }
+  }
 }
 
 // Explicit stacked rows ("head rows"), one CTA per feature.
