@@ -59,7 +59,8 @@ def model(th, c, poses, clone, z, p_L, W, jac=False):
     sn, cs = np.sin(th[0]), np.cos(th[0])
     d = np.asarray(p_L, dtype=np.float64) - c - th[1:4]
     u = np.stack([cs * d[:, 0] + sn * d[:, 1], -sn * d[:, 0] + cs * d[:, 1], d[:, 2]], axis=1) + c - poses[clone, 0:3]
-    Cs = np.array([quat_to_rot(poses[k, 3:7]) for k in range(len(poses))])[clone]
+    ks, inv = np.unique(clone, return_inverse=True)  # (the rotations of the clones named only)
+    Cs = np.array([quat_to_rot(poses[k, 3:7]) for k in ks]).reshape(-1, 3, 3)[inv.ravel()]
     p = np.einsum("nij,nj->ni", Cs, u)
     with np.errstate(divide="ignore", invalid="ignore"):
         zh = p[:, 0:2] / p[:, 2:3]
@@ -181,3 +182,184 @@ def planted(rng, poses, counts, th, outlier_rate, noise=0.002, depth=(3.0, 15.0)
     for i in np.flatnonzero(wrong):
         p_L[i] = p_L[(i + 1 + rng.integers(n - 1)) % n]
     return clone, z, p_L, wrong
+
+
+def set_counts(sets):
+    """{clone set (tuple): landmarks} of a list with one clone set per landmark (tests/side_shapes.py's MAP_* lists)"""
+    out = {}
+    for cs in sets:
+        out[tuple(cs)] = out.get(tuple(cs), 0) + 1
+    return out
+
+
+def planted_map(rng, poses, sets, th, swap=(), move=(), push=(), sigma=0.05, noise=0.002, outlier_rate=0.0):
+    """matches of landmarks seen from several clones, as planted() draws them: sets maps a clone set (tuple, <= 8 clones) to
+    its number of landmarks; landmark l has one p_L shared by all its observations, off by the correction th from what the
+    clones see, and a random Sigma_L.  Wrong matches, each passing the host's map checks (one p_L per landmark, one observation
+    per clone, <= 8 clones):
+      swap: landmarks whose p_L is another landmark's (every observation of the landmark wrong);
+      move: (landmark, clone) observations moved to another landmark id that is not seen from that clone (p_L follows the id);
+      push: (landmark, clone) observations whose z is 0.05 off (the match found the wrong keypoint);
+      outlier_rate: each landmark swapped with this probability, on top of `swap`.
+    Landmark ids follow the order of `sets` (set by set).  (clone, z, p_L, landmark, Sigma_L [L, 6], wrong [n] bool), shuffled."""
+    from tests.landmark_map_reference import landmarks_seen_from, tri
+    cs_of, pts, Sig = [], [], []
+    for cs, count in sets.items():
+        for _ in range(count):
+            cs_of.append(tuple(cs))
+            pts.append(landmarks_seen_from(rng, poses, list(cs)))
+            B = rng.normal(size=(3, 3)) * sigma
+            Sig.append(tri(B @ B.T + sigma ** 2 * np.eye(3)))
+    L = len(pts)
+    c = pivot(poses, [k for cs in cs_of for k in cs])
+    seen = np.array(pts)
+    p_map = (rz(th[0]) @ (seen - c).T).T + c + np.asarray(th[1:4])  # each landmark's map position
+    swap = set(swap) | {l for l in range(L) if rng.uniform() < outlier_rate}
+    lm_pL = p_map.copy()
+    for l in sorted(swap):
+        lm_pL[l] = p_map[(l + 1 + rng.integers(L - 1)) % L]
+    clone, z, p_L, lm, wrong = [], [], [], [], []
+    members = {l: set(cs_of[l]) for l in range(L)}
+    moved = {}
+    for (l, k) in move:  # to the next landmark (cyclically) that k does not see and that stays within 8 clones
+        for d in range(1, L):
+            l2 = (l + d) % L
+            if k not in members[l2] and len(members[l2]) < 8 and l2 not in swap:
+                members[l2].add(k)
+                members[l].discard(k)
+                moved[(l, k)] = l2
+                break
+        else:
+            raise ValueError(("no landmark to move to", l, k))
+    for l in range(L):
+        for k in cs_of[l]:
+            pc = quat_to_rot(poses[k, 3:7]) @ (seen[l] - poses[k, 0:3])
+            zz = pc[0:2] / pc[2] + noise * rng.normal(size=2) + (0.05 if (l, k) in push else 0.0)
+            lid = moved.get((l, k), l)
+            clone.append(k); z.append(zz); lm.append(lid); p_L.append(lm_pL[lid])
+            wrong.append(l in swap or (l, k) in moved or (l, k) in push)
+    o = rng.permutation(len(clone))
+    return (np.array(clone, np.int32)[o], np.array(z)[o], np.array(p_L)[o], np.array(lm, np.int32)[o], np.array(Sig),
+            np.array(wrong)[o])
+
+
+def map_checks(clone, p_L, landmark, n_landmarks):
+    """the host's checks of a map call (lmk_map_plan): ids in range, one p_L per landmark, no landmark seen twice from a
+    clone, at most 8 clones per landmark; raises AssertionError"""
+    clone, p_L, landmark = np.asarray(clone), np.asarray(p_L), np.asarray(landmark)
+    assert landmark.min() >= 0 and landmark.max() < n_landmarks
+    for l in np.unique(landmark):
+        sel = landmark == l
+        assert np.all(p_L[sel] == p_L[sel][0]), l
+        assert len(np.unique(clone[sel])) == sel.sum() <= 8, l
+
+
+def pairs_fast(seed, hypotheses, n):
+    """sample_pairs for many hypotheses at once (numpy uint64; the same values)"""
+    with np.errstate(over="ignore"):
+        h = np.arange(hypotheses, dtype=np.uint64)
+        s = np.uint64(seed % 2 ** 64)
+
+        def sm(x):
+            z = x + np.uint64(0x9E3779B97F4A7C15)
+            z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+            z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+            return z ^ (z >> np.uint64(31))
+        u, v = sm(s + np.uint64(2) * h), sm(s + np.uint64(2) * h + np.uint64(1))
+    i = (u % np.uint64(n)).astype(np.int64)
+    j = (v % np.uint64(n - 1)).astype(np.int64)
+    j += j >= i
+    return np.stack([i, j], axis=1)
+
+
+def first_valid_layout(first, hypotheses, n, min_later=0, seeds=range(1, 10000)):
+    """a seed and the observations to plant as degenerate ([n] bool) such that a hypothesis is fittable exactly when neither of
+    its pair is degenerate, and the first such hypothesis is `first`: the good observations are hypothesis `first`'s pair plus,
+    greedily in input order, every observation that closes no pair of an earlier hypothesis.  Searched over `seeds` until at
+    least min_later hypotheses after `first` are fittable too (their ties then meet hypothesis `first` at every level of the
+    arg-max).  (seed, degenerate)"""
+    for seed in seeds:
+        pr = pairs_fast(seed, hypotheses, n)
+        a, b = pr[first]
+        if any({int(x), int(y)} == {int(a), int(b)} for x, y in pr[:first]):
+            continue
+        adj = [set() for _ in range(n)]
+        for x, y in pr[:first]:
+            adj[x].add(int(y)); adj[y].add(int(x))
+        good = {int(a), int(b)}
+        for o in range(n):
+            if o not in good and not (adj[o] & good):
+                good.add(o)
+        deg = np.ones(n, bool)
+        deg[list(good)] = False
+        ok = ~deg[pr[:, 0]] & ~deg[pr[:, 1]]
+        assert np.flatnonzero(ok)[0] == first
+        if ok[first + 1:].sum() >= min_later:
+            return seed, deg
+    raise ValueError(("no seed", first, hypotheses, n))
+
+
+TIE_THRESH = 1e8  # thresh of tied(): every observation in front is an inlier of every valid hypothesis
+
+
+def tied(rng, poses, counts, th, degenerate):
+    """noise-free matches (planted() with noise 0, no wrong match) of the correction th, with the observations marked in
+    `degenerate` moved behind their clone: a pair with one of them has no minimal fit.  At thresh TIE_THRESH every valid
+    hypothesis counts the same inliers, all the observations in front (a few minimal fits of 2 points converge elsewhere
+    or not at all in 8 steps; a tighter thresh would split their counts).  (clone, z, p_L)"""
+    clone = np.concatenate([np.full(c, k) for k, c in sorted(counts.items())]).astype(np.int32)  # input order: clone by clone
+    c = pivot(poses, clone)
+    seen = np.zeros((len(clone), 3))
+    for i, k in enumerate(clone):
+        d = rng.uniform(3.0, 15.0)
+        pc = np.array([rng.uniform(-0.4, 0.4) * d, rng.uniform(-0.3, 0.3) * d, d])
+        seen[i] = quat_to_rot(poses[k, 3:7]).T @ pc + poses[k, 0:3]
+    p_L = (rz(th[0]) @ (seen - c).T).T + c + np.asarray(th[1:4])
+    z = np.array([(quat_to_rot(poses[k, 3:7]) @ (s - poses[k, 0:3])) for k, s in zip(clone, seen)])
+    z = z[:, 0:2] / z[:, 2:3]
+    for i in np.flatnonzero(degenerate):
+        k = clone[i]
+        p_L[i] = 2 * poses[k, 0:3] - p_L[i]  # mirrored through the camera centre: behind it under any small correction
+    return clone, z, p_L
+
+
+def refit_rejected(rng, poses, R, thresh, tries=4000):
+    """a seeded search for a call whose best hypothesis's refit is finite but keeps fewer inliers (c1 < c0), so the
+    hypothesis's own fit stays: 12 matches on clones 2 and 9 (20 % wrong, pixel noise 0.004), 8 hypotheses, consensus seed =
+    the try.  Every e_i of every hypothesis and of the refit lies at least 1e-6 relative from thresh.  (clone, z, p_L, seed,
+    the reference's consensus)"""
+    for seed in range(tries):
+        clone, z, p_L, _ = planted(rng, poses, {2: 6, 9: 6}, [0.02, 0.3, -0.2, 0.1], 0.2, noise=0.004)
+        rf = consensus(poses, clone, z, p_L, R, 8, thresh, 2, seed=seed)
+        if rf["best"] < 0 or rf["refit"] or not np.isfinite(rf["e_refit"]).any():  # (all inf: the refit's fit failed)
+            continue
+        es = np.concatenate([rf["e"].ravel(), rf["e_refit"]])
+        es = es[np.isfinite(es)]
+        if np.any(np.abs(es - thresh) <= 1e-6 * thresh):
+            continue
+        assert (rf["e_refit"] <= thresh).sum() < (rf["e_best"] <= thresh).sum()
+        return clone, z, p_L, seed, rf
+    raise AssertionError("no rejected refit in the search")
+
+
+def map_exclusions(sets, pattern):
+    """planted_map's (swap, move, push) that make the consensus exclude, from a map call over `sets` (one clone set per
+    landmark, tests/side_shapes.py's MAP_* lists; ids in set_counts order):
+      one_observation: one observation of landmark 0 pushed (and, where landmark 1 is seen from 2 clones, one of its
+                       observations moved to another landmark);
+      landmark:        every observation of landmark 1 (its p_L swapped);
+      clone_set:       every landmark of the last clone set (swapped); swap None when that set is the whole call;
+      clone:           every observation of one clone (the first clone of the middle landmark), pushed."""
+    lms = []
+    for cs, count in set_counts(sets).items():
+        lms += [cs] * count
+    if pattern == "one_observation":
+        return (), ([(1, lms[1][0])] if len(lms[1]) == 2 else []), [(0, lms[0][0])]
+    if pattern == "landmark":
+        return [1], [], []
+    if pattern == "clone_set":
+        group = [l for l, cs in enumerate(lms) if cs == lms[-1]]
+        return (None if len(group) == len(lms) else group), [], []
+    assert pattern == "clone", pattern
+    k = lms[len(lms) // 2][0]
+    return (), [], [(l, k) for l, cs in enumerate(lms) if k in cs]

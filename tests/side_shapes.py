@@ -16,7 +16,8 @@ MIRROR = {"kAidSmemMax": ("engine.cu", 32 * 1024), "kAidMaxRows": ("aid_kernels.
           "kLmkMaxPerClone": ("landmark_kernels.cuh", 256), "kLmkMaxObs": ("landmark_kernels.cuh", 4096),
           "kLmkMaxRows": ("landmark_kernels.cuh", 1152), "kLmkMaxPerSet": ("landmark_kernels.cuh", 256),
           "kLmkMaxSets": ("landmark_kernels.cuh", 256), "kLmkMapClones": ("landmark_kernels.cuh", 8),
-          "kLmkNB": ("landmark_kernels.cuh", 32)}
+          "kLmkNB": ("landmark_kernels.cuh", 32), "kLmkThreads": ("landmark_kernels.cuh", 256),
+          "kLmkMaxHyp": ("landmark_kernels.cuh", 1024), "kConsWarps": ("consensus_kernels.cuh", 8)}
 K = {k: v for k, (_, v) in MIRROR.items()}
 
 
@@ -247,6 +248,38 @@ def map_rows(sets):
         else:
             groups[tuple(cs)] = groups.get(tuple(cs), 0) + len(cs)
     return lmk_rows(single, [(len(cs), o) for cs, o in groups.items()])
+
+
+# ---- the consensus on map matches (consensus_kernels.cuh): k_lmk_hyp runs kConsWarps hypotheses (one warp each) per CTA;
+# k_lmk_cons runs one CTA of kLmkThreads per member, strides the hypotheses by kLmkThreads, reduces them by shuffle in a warp
+# and across the kLmkThreads / 32 warps in thread 0, and keeps kLmkMaxObs / kLmkThreads inlier bits per thread
+CONS_WINDOWS = LMK_WINDOWS  # with clones 0, M // 2 and M - 1 observed
+CONS_ALL = {k: 3 for k in range(192)}  # every clone of a 192-clone window touched: k_lmk_hyp's and k_lmk_cons's ps[kMaxKeep] full
+CONS_PER_CLONE = LMK_PER_CLONE  # on clone 191
+CONS_FULL = LMK_FULL  # 4096 observations: every inlier bit of a k_lmk_cons thread in use
+CONS_HYP = (1, 7, 8, 9, 1023, 1024)  # around k_lmk_hyp's CTA edges, and the cap
+CONS_FIRST = (0, 31, 32, 255, 256, 257, 1023)  # the first valid hypothesis: warp, CTA-stride and last-index edges of k_lmk_cons
+CONS_TIE_OBS = 128  # observations of the tie cases (32 on each of 4 clones)
+# map uncertainty: the clone-set shapes, and what the consensus excludes in each (a pattern a shape cannot hold is left out:
+# MAP_FULL_SET's one clone set is the whole call)
+CONS_MAP = {"full_set": MAP_FULL_SET, "sets": MAP_SETS, "rows": MAP_ROWS}
+CONS_MAP_PATTERNS = ("one_observation", "landmark", "clone_set", "clone")
+CONS_GATE = LMK_GATE  # the middle clone's observations all wrong: used rows 30 / 60 under a stride of 36 / 66
+CONS_SWEEP_ROWS = LMK_SWEEP_ROWS  # used rows; wrong matches raise the planned rows past the next panel edge (1152: below it)
+CONS_BATCH = 40  # members: two launch chunks of kBatchMembers and 8
+
+
+def cons_sweep(M, rows):
+    """(right, wrong) clone -> observations whose right ones use `rows` rows (sweep_counts) and whose wrong ones, excluded by
+    the consensus, raise the planned rows by 2 on a clone no right match touches (by 0 at the cap: then one clone's 3 right
+    matches become 2 right and 1 wrong, 2 used rows fewer)"""
+    right = sweep_counts(M, rows)
+    if rows + 2 <= K["kLmkMaxRows"]:
+        return right, {next(k for k in range(M) if k not in right): 1}
+    k = next(iter(right))
+    right = dict(right)
+    right[k] -= 1
+    return right, {k: 1}
 
 
 def lmk_tiles(n):

@@ -1,11 +1,14 @@
 """The consensus on mapped-landmark matches without a GPU: the numpy reference of tests/landmark_consensus_reference.py on its
 own (a planted correction recovered with 0 / 30 / 60 % wrong matches, a minimal fit that reproduces its two observations, the
-sampler's golden pairs), the argument checks of the Python surface, and the runner's outlier draw."""
+sampler's golden pairs), the argument checks of the Python surface, and the runner's outlier draw.  Then the designed cases
+of tests/test_landmark_consensus_shapes_gpu.py on the reference: the multi-clone map builder passes the host's map checks
+and its wrong matches are exactly what the consensus excludes, each tie layout puts the first valid hypothesis at its index,
+and the degenerate pair, rejected refit and min_inliers cases take their branches."""
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import capi
-from tests import landmark_consensus_reference as ref
+from tests import landmark_consensus_reference as ref, landmark_map_reference as mref, side_shapes as ss
 
 R_PIX = np.array([[4.0e-6, 5.0e-7], [5.0e-7, 3.0e-6]])
 THRESH = 13.8  # chi-square, 2 dof, 0.999
@@ -188,3 +191,125 @@ def test_runner_draws_nothing_new_without_wrong_matches():
     cons = [dict(plain[0], wrong=1, wrong_excluded=1, right=3, right_kept=2, cons_status=0)]
     rec = mc.trial_record(nees, [0.01] * 2, map_rows=cons)["map"]
     assert rec["wrong_excluded"] == [1] and rec["right_kept"] == [2] and rec["cons_status"] == [0]
+
+
+# ---- the designed cases of tests/test_landmark_consensus_shapes_gpu.py on the reference -------------------------------------
+def test_pairs_fast_is_the_sampler():
+    for seed, H, n in ((12345, 6, 100), (2 ** 64 - 3, 1024, 4096), (7, 64, 2), (99, 1024, 128)):
+        assert np.array_equal(ref.pairs_fast(seed, H, n), ref.sample_pairs(seed, H, n))
+
+
+@pytest.mark.parametrize("shape", sorted(ss.CONS_MAP))
+def test_planted_map_passes_the_host_checks_and_excludes_as_designed(shape):
+    """every exclusion pattern of a CONS_MAP shape: ids, one p_L per landmark, one observation per clone, <= 8 clones, <= 256
+    clone sets and the planned rows within kLmkMaxRows; the reference's consensus excludes exactly the wrong matches"""
+    rng = np.random.default_rng(11)
+    poses = spread_window(rng, ss.LMK_WINDOW)
+    sets = ss.CONS_MAP[shape]
+    for pattern in ss.CONS_MAP_PATTERNS:
+        swap, move, push = ref.map_exclusions(sets, pattern)
+        if swap is None:
+            assert shape == "full_set" and pattern == "clone_set"
+            continue
+        clone, z, p_L, lm, Sig, wrong = ref.planted_map(rng, poses, ref.set_counts(sets), [0.015, 0.24, -0.15, 0.09], swap=swap,
+                                                        move=move, push=push, noise=0.0005)
+        ref.map_checks(clone, p_L, lm, len(Sig))
+        groups = {tuple(sorted(clone[lm == l])) for l in np.unique(lm)}
+        assert len([g for g in groups if len(g) > 1]) <= ss.K["kLmkMaxSets"]
+        assert mref.rows(clone, lm, np.zeros(len(clone))) <= ss.K["kLmkMaxRows"]
+        assert wrong.any() and (bool(move) == (shape == "sets" and pattern == "one_observation"))
+        out = ref.consensus(poses, clone, z, p_L, R_PIX, 64, THRESH, 2, seed=len(clone))
+        assert out["status"] == 0 and np.array_equal(out["pre"] == 3, wrong), (shape, pattern)
+
+
+def test_planted_map_outliers_of_both_kinds():
+    rng = np.random.default_rng(12)
+    poses = spread_window(rng, 12)
+    sets = {(0, 5): 3, (2, 7, 11): 2, (4,): 2}
+    clone, z, p_L, lm, Sig, wrong = ref.planted_map(rng, poses, sets, [0.0] * 4, swap=[1], move=[(3, 2)])
+    ref.map_checks(clone, p_L, lm, 7)
+    assert np.all(wrong[lm == 1]) and wrong.sum() == 3  # landmark 1 (2 observations) and the moved one
+    moved = np.flatnonzero(wrong & (lm != 1))[0]
+    assert clone[moved] == 2 and lm[moved] != 3 and 2 not in clone[(lm == 3)]
+    assert np.array_equal(p_L[moved], p_L[lm == lm[moved]][0])
+    clone, z, p_L, lm, Sig, wrong = ref.planted_map(rng, poses, sets, [0.0] * 4, outlier_rate=1.0)
+    assert wrong.all()
+    ref.map_checks(clone, p_L, lm, 7)
+
+
+@pytest.mark.parametrize("first", ss.CONS_FIRST)
+def test_tie_layout_puts_the_first_valid_hypothesis_at_its_index(first):
+    """the seed and degenerate set of each (c) case: the sampler's first pair free of degenerate observations is `first`,
+    the reference finds exactly that, every valid hypothesis counts the same inliers, and (but for the last index) ties sit
+    in other warps of k_lmk_cons"""
+    H, n = ss.K["kLmkMaxHyp"], ss.CONS_TIE_OBS
+    seed, deg = ref.first_valid_layout(first, H, n, min_later=0 if first == H - 1 else 8)
+    pr = ref.sample_pairs(seed, H, n)
+    free = ~deg[pr[:, 0]] & ~deg[pr[:, 1]]
+    assert np.flatnonzero(free)[0] == first
+    rng = np.random.default_rng(first)
+    poses = spread_window(rng, 12)
+    clone, z, p_L = ref.tied(rng, poses, {0: 32, 4: 32, 8: 32, 11: 32}, [0.015, 0.24, -0.15, 0.09], deg)
+    out = ref.consensus(poses, clone, z, p_L, R_PIX, H, ref.TIE_THRESH, 2, seed=seed)
+    valid = np.flatnonzero(out["valid"])
+    # (a pair free of them may still fail its fit, e.g. a Gauss-Newton that leaves the front: rare)
+    assert np.all(free[valid]) and (free & ~out["valid"]).sum() <= 0.01 * free.sum()
+    assert out["valid"][first] and out["best"] == first and out["refit"] == 1
+    assert np.all(out["scores"][valid] == (~deg).sum())
+    if first < H - 1:
+        assert len({(h % ss.K["kLmkThreads"]) // 32 for h in valid}) > 1
+
+
+def test_refit_rejected_search_reaches_the_branch():
+    rng = np.random.default_rng(13)
+    poses = spread_window(rng, 12)
+    clone, z, p_L, seed, rf = ref.refit_rejected(rng, poses, R_PIX, 6.0)
+    assert rf["refit"] == 0 and rf["best"] >= 0 and np.isfinite(rf["e_refit"]).any()
+    assert (rf["e_refit"] <= 6.0).sum() < (rf["e_best"] <= 6.0).sum() and rf["inliers"].sum() == (rf["e_best"] <= 6.0).sum()
+    assert np.array_equal(rf["th_final"], rf["th"][rf["best"]])
+
+
+def test_identical_pair_fails_the_cholesky_and_min_inliers_edges():
+    rng = np.random.default_rng(14)
+    poses = spread_window(rng, 12)
+    clone, z, p_L, _ = ref.planted(rng, poses, {2: 10, 9: 10}, [0.015, 0.24, -0.15, 0.09], 0.0)
+    clone[1], z[1], p_L[1] = clone[0], z[0], p_L[0]
+    out = ref.consensus(poses, clone, z, p_L, R_PIX, 1024, THRESH, 2, seed=11)
+    hs = [h for h, p in enumerate(out["pairs"].tolist()) if sorted(p) == [0, 1]]
+    assert hs and not out["valid"][hs].any() and out["valid"].sum() > 900
+    W, c = ref.weight(R_PIX), ref.pivot(poses, clone)
+    assert ref.model(np.zeros(4), c, poses, clone[:2], z[:2], p_L[:2], W)[0].all()  # in front: the Cholesky fails the fit
+    assert not ref.gauss_newton(np.zeros(4), c, poses, clone[:2], z[:2], p_L[:2], W)[1]
+    for copies in (2, 5):
+        o = ref.consensus(poses, np.repeat(clone[:1], copies), np.repeat(z[:1], copies, 0), np.repeat(p_L[:1], copies, 0), R_PIX, 16,
+                          THRESH, 2, seed=7)
+        assert not o["valid"].any() and o["status"] == 1 and np.all(o["pre"] == 3)
+    clone, z, p_L, wrong = ref.planted(rng, poses, {0: 15, 6: 15, 11: 15}, [0.015, 0.24, -0.15, 0.09], 0.3, noise=0.0005)
+    k = int(ref.consensus(poses, clone, z, p_L, R_PIX, 64, THRESH, 2, seed=3)["inliers"].sum())
+    assert k == (~wrong).sum()
+    assert ref.consensus(poses, clone, z, p_L, R_PIX, 64, THRESH, k, seed=3)["status"] == 0
+    assert ref.consensus(poses, clone, z, p_L, R_PIX, 64, THRESH, k + 1, seed=3)["status"] == 1
+
+
+def test_excluded_rows_cases_cross_the_planned_stride():
+    K = ss.K
+    for rows in ss.CONS_SWEEP_ROWS:
+        right, wrong = ss.cons_sweep(ss.LMK_WINDOW, rows)
+        allc = {k: right.get(k, 0) + wrong.get(k, 0) for k in set(right) | set(wrong)}
+        used, planned = ss.lmk_rows(right), ss.lmk_rows(allc)
+        assert planned <= K["kLmkMaxRows"] and sum(allc.values()) <= K["kLmkMaxObs"]
+        assert (used, planned) == ((rows, rows + 2) if rows < K["kLmkMaxRows"] else (rows - 2, rows))
+    for counts in ss.CONS_GATE:
+        mid = sorted(counts)[len(counts) // 2]
+        used = ss.lmk_rows({k: a for k, a in counts.items() if k != mid})
+        assert ss.chunks(ss.lmk_rows(counts)) > ss.chunks(used)
+
+
+def spread_window(rng, M):
+    """window() with the clones' attitudes near one another, as a filter's window is: every landmark of a clone set is seen
+    from each of its clones"""
+    poses = window(rng, M)
+    q0 = poses[0, 3:7]
+    q = q0 + 0.05 * rng.normal(size=(M, 4))
+    poses[:, 3:7] = q / np.linalg.norm(q, axis=1, keepdims=True)
+    return poses
