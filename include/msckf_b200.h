@@ -225,7 +225,9 @@ enum msckf_b200_aid_model {
   MSCKF_B200_AID_RANGE = 11,                 /* stacks only: radio ranging to a surveyed anchor */
   MSCKF_B200_AID_CLONE_RANGE = 12,           /* stacks only */
   MSCKF_B200_AID_PLANE_RANGE = 13,           /* stacks only: a rangefinder over a level plane */
-  MSCKF_B200_AID_CLONE_PLANE_RANGE = 14      /* stacks only */
+  MSCKF_B200_AID_CLONE_PLANE_RANGE = 14,     /* stacks only */
+  MSCKF_B200_AID_GYRO_AT_REST = 15,          /* stacks only: the mean gyro reading of a standstill */
+  MSCKF_B200_AID_ACCEL_AT_REST = 16          /* stacks only: the mean specific force of a standstill */
 };
 typedef struct {
   int model;          /* msckf_b200_aid_model; in a batch, < 0 leaves that member untouched */
@@ -287,23 +289,29 @@ int msckf_b200_batch_aid_update(msckf_b200_batch* b, const msckf_b200_aid* aid, 
  *                           r = rho - rho^; H over dtheta and dp_z (14).  When b_z^2 <= 1e-6 (the beam within ~1e-3 rad of
  *                           parallel to the plane) or rho^ <= 0 (the plane behind the sensor): status 2, NIS NaN, nothing written.
  *   CLONE_PLANE_RANGE       a = clone k; z as PLANE_RANGE with l and f in that clone's camera frame; H over its [dtheta, dp_z].
+ * At-rest models (the IMU readings of a standstill; msckf_b200_standstill_update below forms them), with C = C(q_IG); 3 rows
+ * each, a = b = 0:
+ *   GYRO_AT_REST            z = the mean gyro reading (3): r = z - b_g; H over db_g (3..5) the identity.
+ *   ACCEL_AT_REST           z = the mean specific force (3): h = b_a - C g with the filter's g, r = z - h; H over dtheta -[C g]x
+ *                           and over db_a (9..11) the identity.  It observes roll, pitch and b_a, never yaw (H_theta C g = 0).
+ *                           Both ignore Earth rotation.
  *   A degenerate item ends its member's whole stack (in a batch the other members are applied).  An anchor's position is taken
  *   as exact, and a range as unbiased; a caller with more than 8 anchors in one epoch makes two calls.
  *   A and b that a model does not use must be 0.  (A lever arm or an axis given in the IMU frame, l_I or f_I, is converted to
  *   camera frames with the engine's q_CI and p_C_I (the camera's position in the IMU frame: p_C_G = p_I_G + C(q_IG)^T p_C_I,
  *   C(q_CG) = C(q_CI) C(q_IG)): l_C = C(q_CI) (l_I - p_C_I), f_C = C(q_CI) f_I.)
  * C(q) is Eigen's toRotationMatrix (C(q_CG) maps G to the camera frame).  LINEAR is not allowed in a stack.  R of an item is its
- * own rows x rows block (3, 3, 6, 6, popcount(mask), 6, popcount(mask), popcount(mask), 1, 1, 1, 1, 1, 1 rows), row-major, lower triangle
+ * own rows x rows block (3, 3, 6, 6, popcount(mask), 6, popcount(mask), popcount(mask), 1, 1, 1, 1, 1, 1, 3, 3 rows), row-major, lower triangle
  * read; the struct carries no size, so a caller that passes another size is not caught here (the class forms check it). */
 typedef struct {
   int model;          /* msckf_b200_aid_model except LINEAR */
   int a;              /* CLONE_POSE, RELATIVE_POSE, CLONE_ANTENNA_POSITION, CLONE_HEADING, CLONE_RANGE, CLONE_PLANE_RANGE: clone
-                         position; BODY_VELOCITY, ANTENNA_POSITION: row mask (1..7); else ignored (0 for the GNSS, heading
-                         and range models) */
+                         position; BODY_VELOCITY, ANTENNA_POSITION: row mask (1..7); else ignored (0 for the GNSS, heading,
+                         range and at-rest models) */
   int b;              /* RELATIVE_POSE: the second clone; CLONE_ANTENNA_POSITION: row mask (1..7); else ignored (0 for the
-                         GNSS, heading and range models) */
-  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components), 7, 6 (antenna), 4 (heading), 7 (range)
-                         or 8 (plane range) doubles */
+                         GNSS, heading, range and at-rest models) */
+  const double* z;    /* 3 (VELOCITY, POSITION, BODY_VELOCITY: all three components; GYRO_AT_REST, ACCEL_AT_REST), 7, 6
+                         (antenna), 4 (heading), 7 (range) or 8 (plane range) doubles */
   const double* R;    /* [rows][rows] */
 } msckf_b200_aid_item;
 /* A bad model, a clone outside the window, a == b, an empty mask, more than 8 items or 32 rows, a NULL or non-finite z / R, a zero
@@ -381,7 +389,8 @@ typedef struct {
   double step;           /* the last max |delta_{i+1} - delta_i| (0 for max_iter <= 1) */
 } msckf_b200_aid_iter_result;
 /* Refusals (MSCKF_B200_ERR_ARG, nothing written): everything the call without _iter refuses, iter or iter_out NULL, max_iter
- * outside 0..16, a tol that is not finite and >= 0; an un-fetched update returns MSCKF_B200_ERR_STATE.  A non-finite dx or P
+ * outside 0..16, a tol that is not finite and >= 0, a GYRO_AT_REST or ACCEL_AT_REST item (the iterate carries no biases: a
+ * standstill's rows are linear in b_g and b_a, and nearly so in the attitude); an un-fetched update returns MSCKF_B200_ERR_STATE.  A non-finite dx or P
  * entry returns MSCKF_B200_ERR_NUMERIC with the update applied. */
 int msckf_b200_aid_stack_update_iter(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n_items, double chi2_max,
                                      const msckf_b200_aid_iter* iter, msckf_b200_aid_result* out, msckf_b200_aid_iter_result* iter_out);
@@ -397,6 +406,40 @@ int msckf_b200_batch_aid_stack_update_iter(msckf_b200_batch* b, const msckf_b200
 int msckf_b200_batch_aid_stack_update_fde_iter(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
                                                const msckf_b200_aid_fde* fde, const msckf_b200_aid_iter* iter,
                                                msckf_b200_aid_fde_result* out, msckf_b200_aid_iter_result* iter_out);
+/* ---- standstill: detect that the platform is at rest from the IMU, and fuse a zero-motion update (DESIGN.md 4.18) ----------
+ * readings: k >= 2 IMU readings [k][7] (omega, a, dT) in msckf_b200_propagate_n's layout and the engine's dtype -- the ones
+ * propagated since the previous image.  With R0 the 6 x 6 block diagonal of Q_imu's gyro (rows / columns 0..2) and accelerometer
+ * (6..8) blocks, s = noise_scale and T = sum dT_j, the host forms in fp64, in reading order: the dT-weighted means w^ = sum dT_j
+ * omega_j / T and a^ = sum dT_j a_j / T, and the scatter sigma = sum_j dT_j (y_j - y^)^T (s^2 R0)^-1 (y_j - y^) of y_j = [omega_j; a_j]
+ * (chi-square with 6 (k - 1) dof at rest, whatever the state).  scatter = sigma / (6 (k - 1)) > scatter_max: outcome 1 (moving),
+ * nothing is launched or written.  Otherwise the 9-row stack VELOCITY (z = 0, R = sigma_v^2 I), GYRO_AT_REST (z = w^, R = s^2
+ * R0_g / T), ACCEL_AT_REST (z = a^, R = s^2 R0_a / T) runs as msckf_b200_aid_stack_update with chi2_max as its gate, bit for bit:
+ * outcome 0 applied, 2 gated out (moving: the mean does not fit the state), -1 with stack.status 1 (S not positive definite).
+ * The scatter term and the stack's NIS add up to the NIS of the dense update over all 6k reading rows, and the 9-row update
+ * equals the dense one: the means are sufficient.  The caller skips the frame's vision work on outcome 0 (INTEGRATION.md).
+ * Refusals (MSCKF_B200_ERR_ARG, nothing written): k < 2 or k > 4096, readings NULL, a dT that is not finite and > 0, a
+ * non-finite reading, noise_scale < 1 or not finite, a sigma_v, scatter_max or chi2_max that is not finite and > 0, a gyro or
+ * accelerometer block of Q_imu that is not positive definite; an un-fetched update returns MSCKF_B200_ERR_STATE.  A non-finite
+ * dx or P entry returns MSCKF_B200_ERR_NUMERIC with the result filled and the update applied. */
+typedef struct {
+  double noise_scale;  /* s >= 1: the IMU noise inflation (vibration) */
+  double sigma_v;      /* m/s: the zero-velocity row's standard deviation */
+  double scatter_max;  /* > 0: the largest scatter / (6 (k - 1)) taken as at rest */
+  double chi2_max;     /* > 0: the gate on the 9-row stack's NIS */
+} msckf_b200_standstill;
+typedef struct {
+  msckf_b200_aid_result stack;  /* the 9-row stack, as msckf_b200_aid_stack_update reports it (outcome 1: NIS NaN, dof 0) */
+  double scatter;               /* sigma / (6 (k - 1)) */
+  int outcome;                  /* 0 applied; 1 moving (scatter > scatter_max: nothing launched); 2 moving (stack NIS > chi2_max);
+                                   -1 stack.status 1 */
+} msckf_b200_standstill_result;
+int msckf_b200_standstill_update(msckf_b200_engine* e, const void* readings, int k, const msckf_b200_standstill* cfg,
+                                 msckf_b200_standstill_result* out);
+/* the same for every member of a batch (readings[i] [k[i]][7], out[i]; k[i] = 0 leaves member i untouched and out[i] not
+ * written); every member is validated before anything is launched.  One launch per 32 members that pass the scatter test, none
+ * when no member does. */
+int msckf_b200_batch_standstill_update(msckf_b200_batch* b, const void* const* readings, const int* k, const msckf_b200_standstill* cfg,
+                                       msckf_b200_standstill_result* out);
 /* ---- mapped landmarks: image observations of landmarks whose position is known (prior map, surveyed marker, relocalisation) --
  * Observation i is (clone[i], z[i] normalised image coordinates, p_L_G[i] landmark position in G).  With C = C(q_CG) and p_C_G of
  * that clone: p_C = C (p_L - p_C_G), z^ = p_C[0:2] / p_C[2], r_i = z_i - z^ (calcResidual, msckf.h:960-978), Jacobian the 2 x 6

@@ -522,6 +522,47 @@ class MSCKF {
     R(0, 0) = var;
     return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_CLONE_PLANE_RANGE, k, 0, 1, z, R)}, chi2_max);
   }
+  // the at-rest items on their own (stacks of GYRO_AT_REST / ACCEL_AT_REST): the mean gyro reading, or the mean specific force,
+  // of IMU readings taken at rest, R 3 x 3 (standstillUpdate forms both from the readings)
+  msckf_b200_aid_result gyroAtRestUpdate(const Vector3<double>& omega_mean, const MatrixX<double>& R, double chi2_max = 0) {
+    const double z[3] = {omega_mean(0), omega_mean(1), omega_mean(2)};
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_GYRO_AT_REST, 0, 0, 3, z, R)}, chi2_max);
+  }
+  msckf_b200_aid_result accelAtRestUpdate(const Vector3<double>& a_mean, const MatrixX<double>& R, double chi2_max = 0) {
+    const double z[3] = {a_mean(0), a_mean(1), a_mean(2)};
+    return aidedUpdate(std::vector<msckf_b200_aid_item>{aidItem(MSCKF_B200_AID_ACCEL_AT_REST, 0, 0, 3, z, R)}, chi2_max);
+  }
+  // standstill (not in the reference; msckf_b200_standstill_update: statistics, gate and outcomes there): the IMU readings
+  // propagated since the previous image are tested for rest on their scatter about their mean and, at rest, fused as one
+  // zero-velocity, gyro-bias and specific-force update.  The class only reports: on outcome 0 the caller skips the frame's
+  // augmentState / update / marginalize / prune and keeps propagating (INTEGRATION.md).  Queued readings are handed over
+  // first; readings or a cfg the C-ABI would refuse throw std::invalid_argument before any device call.  Bookkeeping as
+  // aidedUpdate(items).
+  msckf_b200_standstill_result standstillUpdate(const std::vector<imuReading<_S>>& readings, const msckf_b200_standstill& cfg) {
+    std::vector<_S> r;
+    packStandstill(readings, cfg, r, "MSCKF::standstillUpdate");
+    msckf_b200_standstill_result o = {};
+    checkNumeric(msckf_b200_standstill_update(eng(), r.data(), (int)readings.size(), &cfg, &o), "msckf_b200_standstill_update");
+    aidAbsorb(o.stack);
+    return o;
+  }
+  // readings in msckf_b200_propagate_n's layout, after the checks of msckf_b200_standstill_update (std::invalid_argument)
+  static void packStandstill(const std::vector<imuReading<_S>>& readings, const msckf_b200_standstill& cfg, std::vector<_S>& r,
+                             const std::string& what) {
+    if (readings.size() < 2 || readings.size() > 4096) throw std::invalid_argument(what + ": 2 to 4096 readings");
+    if (!(std::isfinite(cfg.noise_scale) && cfg.noise_scale >= 1.0)) throw std::invalid_argument(what + ": noise_scale must be finite and >= 1");
+    if (!(std::isfinite(cfg.sigma_v) && cfg.sigma_v > 0.0)) throw std::invalid_argument(what + ": sigma_v must be finite and > 0");
+    if (!(std::isfinite(cfg.scatter_max) && cfg.scatter_max > 0.0)) throw std::invalid_argument(what + ": scatter_max must be finite and > 0");
+    if (!(std::isfinite(cfg.chi2_max) && cfg.chi2_max > 0.0)) throw std::invalid_argument(what + ": chi2_max must be finite and > 0");
+    r.clear();
+    for (const auto& m : readings) {
+      const _S v[7] = {m.omega(0), m.omega(1), m.omega(2), m.a(0), m.a(1), m.a(2), m.dT};
+      for (int i = 0; i < 7; ++i)
+        if (!std::isfinite((double)v[i])) throw std::invalid_argument(what + ": non-finite reading");
+      if (!(m.dT > 0)) throw std::invalid_argument(what + ": dT must be > 0");
+      r.insert(r.end(), v, v + 7);
+    }
+  }
   // the window position of the clone of image state_id (std::invalid_argument when it is not in the window)
   int windowPosition(int state_id, const char* what) const {
     for (size_t pos = 0; pos < cam_states_.size(); ++pos)
@@ -1249,6 +1290,31 @@ class MSCKFBatch {
     for (size_t i = 0; i < size(); ++i)
       if (!items[i].empty()) filters_[i]->aidAbsorb(r[i].stack);
     return r;
+  }
+  // MSCKF::standstillUpdate of every filter (readings[i] empty: filter i is left alone and result[i] value-initialised) as one
+  // msckf_b200_batch_standstill_update: one launch per 32 filters at rest by their scatter, none when no filter is, one
+  // synchronisation.  Bad readings or a bad cfg throw before any device call.
+  std::vector<msckf_b200_standstill_result> standstillUpdate(const std::vector<std::vector<imuReading<_S>>>& readings,
+                                                             const msckf_b200_standstill& cfg) {
+    const size_t n = size();
+    if (readings.size() != n) throw std::invalid_argument("MSCKFBatch::standstillUpdate: one reading list per filter");
+    std::vector<std::vector<_S>> r(n);
+    std::vector<const void*> p(n, nullptr);
+    std::vector<int> k(n, 0);
+    for (size_t i = 0; i < n; ++i) {
+      if (readings[i].empty()) continue;
+      MSCKF<_S>::packStandstill(readings[i], cfg, r[i], "MSCKFBatch::standstillUpdate");
+      p[i] = r[i].data();
+      k[i] = (int)readings[i].size();
+    }
+    flushImu();
+    std::vector<msckf_b200_standstill_result> o(n, msckf_b200_standstill_result());
+    const int rc = msckf_b200_batch_standstill_update(batch_, p.data(), k.data(), &cfg, o.data());
+    if (rc == MSCKF_B200_ERR_NUMERIC) std::cout << "[msckf_b200] batch standstill update: " << msckf_b200_last_error() << std::endl;
+    else MSCKF<_S>::check(rc, "msckf_b200_batch_standstill_update");
+    for (size_t i = 0; i < n; ++i)
+      if (k[i]) filters_[i]->aidAbsorb(o[i].stack);
+    return o;
   }
   // MSCKF::landmarkUpdate of every filter (obs[i] empty: filter i is left alone) as one msckf_b200_batch_landmark_update: three
   // launches per 32 updated filters and one synchronisation.  gamma / flag (optional) receive one list per filter.  An unknown

@@ -149,6 +149,13 @@ int msckf_mono_batch_landmark_update_consensus(void* batch, const int* n_obs, co
                                                const double* p_L_G, const double* R3, double chi2_obs, int max_iter, double tol,
                                                const msckf_b200_landmark_consensus* cons, double* gamma, int* flag,
                                                msckf_b200_landmark_result* out, msckf_b200_landmark_consensus_result* cons_out);
+/* standstill detection and the zero-motion update (MSCKF::standstillUpdate, msckf_b200_standstill_update: statistics, outcomes
+ * and errors there): k readings [k][7] omega, a, dT (rounded to the filter's scalar type), the ones propagated since the previous
+ * image.  _batch_standstill_update: k[i] per filter (0: filter i is left alone and out[i] is not written), the readings
+ * concatenated in filter order, one device call.  Bad readings or a bad cfg fail before any device call. */
+int msckf_mono_standstill_update(void* h, const double* readings, int k, const msckf_b200_standstill* cfg, msckf_b200_standstill_result* out);
+int msckf_mono_batch_standstill_update(void* batch, const int* k, const double* readings, const msckf_b200_standstill* cfg,
+                                       msckf_b200_standstill_result* out);
 /* the msckf_b200_engine* beneath (for CUDA-event timing on its stream, launch counts, state copies) */
 void* msckf_mono_engine(void* h);
 /* copy the complete filter (host bookkeeping + device state) of src into dst; both must be initialised alike */

@@ -44,6 +44,7 @@ def _truth(truth_imu, truth_poses):
 AID_VELOCITY, AID_POSITION, AID_POSE, AID_CLONE_POSE, AID_LINEAR, AID_BODY_VELOCITY, AID_RELATIVE_POSE = range(7)
 AID_ANTENNA_POSITION, AID_CLONE_ANTENNA_POSITION, AID_HEADING, AID_CLONE_HEADING = range(7, 11)
 AID_RANGE, AID_CLONE_RANGE, AID_PLANE_RANGE, AID_CLONE_PLANE_RANGE = range(11, 15)
+AID_GYRO_AT_REST, AID_ACCEL_AT_REST = 15, 16
 
 
 class Aid(C.Structure):
@@ -83,8 +84,9 @@ def aid_items(items):
     CLONE_ANTENNA_POSITION: the row mask).  z: ANTENNA_POSITION and CLONE_ANTENNA_POSITION p_A_G (3) and the lever arm (3) in
     the body frame, HEADING and CLONE_HEADING psi (1) and the axis (3) in the body frame, RANGE and CLONE_RANGE rho (1), the
     anchor (3) in G and the lever arm (3) in the body frame, PLANE_RANGE and CLONE_PLANE_RANGE rho (1), the plane height h (1),
-    the lever arm (3) and the beam axis (3) in the body frame (include/msckf_b200.h); "a" of CLONE_RANGE and CLONE_PLANE_RANGE
-    is the clone; R of a heading or a range is 1 x 1"""
+    the lever arm (3) and the beam axis (3) in the body frame, GYRO_AT_REST the mean gyro reading (3) and ACCEL_AT_REST the
+    mean specific force (3) of a standstill (include/msckf_b200.h); "a" of CLONE_RANGE and CLONE_PLANE_RANGE is the clone; R of
+    a heading or a range is 1 x 1"""
     arr = (AidItem * max(len(items), 1))()
     keep = []
     for k, it in enumerate(items):
@@ -143,6 +145,25 @@ def fde_struct(fde):
     chi2 = np.asarray(fde["chi2"], dtype=np.float64).ravel()
     assert chi2.size == 32, chi2.size
     return AidFde((C.c_double * 32)(*chi2.tolist()), int(fde["max_exclude"]))
+
+
+class Standstill(C.Structure):
+    _fields_ = [("noise_scale", C.c_double), ("sigma_v", C.c_double), ("scatter_max", C.c_double), ("chi2_max", C.c_double)]
+
+
+class StandstillResult(C.Structure):
+    _fields_ = [("stack", AidResult), ("scatter", C.c_double), ("outcome", C.c_int)]
+
+    def as_dict(self):
+        d = self.stack.as_dict()
+        d.update(scatter=self.scatter, outcome=self.outcome)
+        return d
+
+
+def standstill_struct(cfg):
+    """msckf_b200_standstill of cfg = dict noise_scale (>= 1; default 1), sigma_v (m/s), scatter_max (the largest scatter /
+    (6 (k - 1)) taken as at rest), chi2_max (the gate on the 9-row stack's NIS)"""
+    return Standstill(float(cfg.get("noise_scale", 1.0)), float(cfg["sigma_v"]), float(cfg["scatter_max"]), float(cfg["chi2_max"]))
 
 
 class Landmarks(C.Structure):
@@ -441,6 +462,20 @@ class Batch:
                     r.update(o.as_dict())
         return res
 
+    def standstill_update(self, readings, cfg):
+        """msckf_b200_batch_standstill_update: readings[i] = [k_i, 7] array (omega, a, dT) for engine i, or None / k_i = 0
+        (engine i left alone); cfg as for standstill_struct.  A list of result dicts (the stack's nis, dx_norm, dof, applied,
+        status, then scatter and outcome; None for an engine left alone)."""
+        n = len(self.engines)
+        assert len(readings) == n
+        rs = [np.zeros((0, 7), dtype=e.dtype) if r is None else np.ascontiguousarray(r, dtype=e.dtype).reshape(-1, 7)
+              for r, e in zip(readings, self.engines)]
+        ptrs = (C.c_void_p * n)(*[r.ctypes.data if len(r) else None for r in rs])
+        k = (C.c_int * n)(*[len(r) for r in rs])
+        c, out = standstill_struct(cfg), (StandstillResult * n)()
+        check(lib().msckf_b200_batch_standstill_update(self.h, ptrs, k, C.byref(c), out), "msckf_b200_batch_standstill_update")
+        return [o.as_dict() if len(r) else None for r, o in zip(rs, out)]
+
     def landmark_update(self, specs, max_iter=None, tol=None, consensus=None):
         """msckf_b200_batch_landmark_update: specs[i] for engine i (see landmark_struct; None or no observations leaves engine
         i alone); max_iter / tol, when given, apply to every spec that does not set its own.  When a spec has Sigma_L (see
@@ -636,6 +671,15 @@ class Engine:
         if it is not None:
             res.update(iout.as_dict())
         return res
+
+    def standstill_update(self, readings, cfg):
+        """msckf_b200_standstill_update: readings [k, 7] (omega, a, dT; rounded to the engine's dtype), cfg as for
+        standstill_struct.  The result as a dict: the stack's nis, dx_norm, dof, applied, status, then scatter and outcome."""
+        r = np.ascontiguousarray(readings, dtype=self.dtype).reshape(-1, 7)
+        c, out = standstill_struct(cfg), StandstillResult()
+        check(lib().msckf_b200_standstill_update(self.h, C.c_void_p(r.ctypes.data), C.c_int(len(r)), C.byref(c), C.byref(out)),
+              "msckf_b200_standstill_update")
+        return out.as_dict()
 
     def landmark_update(self, clone, z, p_L, R=None, chi2_obs=0.0, max_iter=0, tol=0.0, landmark=None, Sigma_L=None, consensus=None):
         """msckf_b200_landmark_update: observations of known landmarks p_L [n, 3] at z [n, 2] from window positions clone [n];

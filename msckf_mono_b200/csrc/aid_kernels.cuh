@@ -21,6 +21,7 @@
 // One CTA per member, one launch for everything; one body for a single filter (NM = 1) and a device batch (NM =
 // kBatchMembers), like k_nees.  W^T and dx live in dynamic shared memory where they fit, else in a per-member global workspace.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "nees_kernels.cuh"
 #include "state_kernels.cuh"
@@ -31,7 +32,7 @@ namespace mb {
 enum AidModel {
   kAidVelocity = 0, kAidPosition = 1, kAidPose = 2, kAidClonePose = 3, kAidLinear = 4, kAidBodyVelocity = 5, kAidRelativePose = 6,
   kAidAntennaPosition = 7, kAidCloneAntennaPosition = 8, kAidHeading = 9, kAidCloneHeading = 10,
-  kAidRange = 11, kAidCloneRange = 12, kAidPlaneRange = 13, kAidClonePlaneRange = 14
+  kAidRange = 11, kAidCloneRange = 12, kAidPlaneRange = 13, kAidClonePlaneRange = 14, kAidGyroAtRest = 15, kAidAccelAtRest = 16
 };
 constexpr double kAidHeadingMinHoriz = 1e-6;  // HEADING: d_x^2 + d_y^2 <= this |f|^2 (f within ~1e-3 rad of vertical) is degenerate
 constexpr double kAidRangeMin = 1e-6;         // RANGE: a predicted range at or below this (m) leaves its direction undefined
@@ -118,7 +119,7 @@ struct AidIterOut {
 };
 
 // Where aid_item_rows reads the state from its two pointers (st, poses): the IMU's q_IG, v_I_G, p_I_G and clone k's pose (q, p
-// at offsets 0 and 4).  AidResident: the filter's own (DevState<S>, its poses).
+// at offsets 0 and 4).  AidResident: the filter's own (DevState<S>, its poses), with b_g, b_a and g for the at-rest models.
 template <class S>
 struct AidResident {
   using St = DevState<S>;
@@ -127,9 +128,13 @@ struct AidResident {
   static __device__ const S* v(const St* st, const S*) { return st->v_I_G; }
   static __device__ const S* p(const St* st, const S*) { return st->p_I_G; }
   static __device__ const S* pose(const St*, const S* poses, const AidItem&, int k) { return poses + kPoseStride * k; }
+  static __device__ const S* b_g(const St* st) { return st->b_g; }
+  static __device__ const S* b_a(const St* st) { return st->b_a; }
+  static __device__ const S* g(const St* st) { return st->g; }
 };
 // AidIterate: st is one item's fp64 iterate x^ [+] delta_i (kAidIterX doubles; poses is not read): [0, 7) q, p of the IMU or
-// of clone a, [7, 14) q, p of clone b (RELATIVE_POSE), [14, 17) v_I_G.  Only the poses the item names are there.
+// of clone a, [7, 14) q, p of clone b (RELATIVE_POSE), [14, 17) v_I_G.  Only the poses the item names are there.  It carries no
+// biases, so the at-rest models are not formed at an iterate (the iterated calls refuse them).
 constexpr int kAidIterX = 17;
 struct AidIterate {
   using St = double;
@@ -190,6 +195,9 @@ __device__ __noinline__ void aid_iterate(const AidItem it, const DevState<S>* st
 //                  {x : x_z = h} in G.  b = C^T f / |f|, rho^ = (h - (p + d)_z) / b_z, r = rho - rho^; with d' = C^T (l + rho^ f/|f|)
 //                  (the hit point from the body) and J' = -[d']x C^T: H over dtheta -J'_z / b_z (= e_z^T C^T [l + rho^ f/|f|]x / b_z),
 //                  over dp_z -1 / b_z.  b_z^2 <= kAidPlaneMinBeamZ or rho^ <= 0 (the plane behind the sensor) returns 1 (status 2).
+//   GYRO_AT_REST   z = the mean gyro reading of a standstill (3); r = z - b_g, H over db_g (3..5) the identity
+//   ACCEL_AT_REST  z = the mean specific force of a standstill (3); h = b_a - C g (C = C(q_IG), g the resident gravity), r = z - h;
+//                  H over dtheta -[C g]x (C+ g = C g + [C g]x dtheta), over db_a (9..11) the identity.  H_theta (C g) = 0: no yaw.
 // The state X the rows are formed at: AidResident (the filter's) or AidIterate (an iterate of the iterated form).
 // Returns 0 when the rows are formed.
 // (Out of line, with the item by value: inlined into k_aid<double, 1>, this code made ptxas spill.)
@@ -231,6 +239,35 @@ __device__ __noinline__ int aid_item_rows(const AidItem it, const double* z, con
           col[row][3 + k] = 6 + k; coef[row][3 + k] = C[3 * j + k];
         }
         nnz[row++] = 6;
+      }
+    }
+  } else if (it.model == kAidGyroAtRest || it.model == kAidAccelAtRest) {  // the IMU at rest (AidResident only)
+    if constexpr (std::is_same<X, AidIterate>::value) {
+      return 1;
+    } else {
+      const bool gyro = it.model == kAidGyroAtRest;
+      const auto* b = gyro ? X::b_g(st) : X::b_a(st);
+      double u[3] = {0.0, 0.0, 0.0};  // ACCEL_AT_REST: C g
+      if (!gyro) {
+        const auto* Q = X::q(st, poses);
+        const auto* G = X::g(st);
+        const double q[4] = {(double)Q[0], (double)Q[1], (double)Q[2], (double)Q[3]};
+        double C[9];
+        quat_to_rot(q, C);
+        for (int j = 0; j < 3; ++j) u[j] = C[3 * j] * (double)G[0] + C[3 * j + 1] * (double)G[1] + C[3 * j + 2] * (double)G[2];
+      }
+      const double sk[9] = {0.0, u[2], -u[1], -u[2], 0.0, u[0], u[1], -u[0], 0.0};  // -[C g]x
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const int row = r0 + j;
+        r[row] = z[j] - ((double)b[j] - u[j]);
+        if (gyro) {
+          col[row][0] = 3 + j; coef[row][0] = 1.0; nnz[row] = 1;
+        } else {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) { col[row][k] = k; coef[row][k] = sk[3 * j + k]; }
+          col[row][3] = 9 + j; coef[row][3] = 1.0; nnz[row] = 4;
+        }
       }
     }
   } else if (it.model >= kAidAntennaPosition) {  // the antenna positions, headings and ranges, of the IMU or of clone a

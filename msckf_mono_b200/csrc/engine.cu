@@ -49,6 +49,7 @@ constexpr size_t kSmemBudget = 220 * 1024;  // dynamic shared memory per CTA, un
 // k_aid: W^T and dx in dynamic shared memory up to this many bytes, else in the global workspace (both forms of the kernel;
 // with the FDE form's static shared memory this passes the default 48 KB per CTA, so set_func_attrs raises the limit)
 constexpr size_t kAidSmemMax = 32 * 1024;
+constexpr int kStandstillMaxReadings = 4096;  // IMU readings of one standstill window
 constexpr int kMaxClonesHard = mb::kMaxKeep;  // the keep list of prune() travels as a kernel argument
 constexpr int kMaxGraphs = 8;
 
@@ -181,6 +182,10 @@ int aid_append(AidJob& j, const msckf_b200_aid_item& q, int M, const std::string
       nz = q.model == MSCKF_B200_AID_RANGE || q.model == MSCKF_B200_AID_CLONE_RANGE ? 7 : 8;
       break;
     }
+    case MSCKF_B200_AID_GYRO_AT_REST: case MSCKF_B200_AID_ACCEL_AT_REST:  // three rows each (a and b must be 0)
+      if (q.a != 0 || q.b != 0) return fail(MSCKF_B200_ERR_ARG, w + ": a / b the model does not use must be 0" + who);
+      m = 3;
+      break;
     default: return fail(MSCKF_B200_ERR_ARG, w + ": model not allowed in a stack" + who);
   }
   if (j.m + m > mb::kAidMaxRows) return fail(MSCKF_B200_ERR_ARG, w + ": more than 32 rows" + who);
@@ -253,6 +258,9 @@ struct CtxBase {
   // the stacked form with fault detection and exclusion over the items (msckf_b200_aid_stack_update_fde / _batch_..._fde)
   virtual int aid_stack_fde(const msckf_b200_aid_item* const* items, const int* n_items, const msckf_b200_aid_fde* fde,
                             msckf_b200_aid_fde_result* out, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) = 0;
+  // standstill detection and the 9-row zero-motion stack (msckf_b200_standstill_update / _batch_standstill_update): the scatter
+  // test on the host, then one launch per 32 members at rest, one synchronisation (none when no member is at rest)
+  virtual int standstill(const void* const* readings, const int* k, const msckf_b200_standstill* cfg, msckf_b200_standstill_result* out) = 0;
   // mapped-landmark updates of the members (msckf_b200_landmark_update / _batch_landmark_update): three launches per 32, one synchronisation
   // (cons, cout: the consensus of each member, or NULL)
   virtual int landmarks(const msckf_b200_landmarks* in, const msckf_b200_landmark_map* map, msckf_b200_landmark_result* out,
@@ -531,6 +539,7 @@ struct Ctx : CtxBase {
                     msckf_b200_aid_fde_result* out, const msckf_b200_aid_iter* iter, msckf_b200_aid_iter_result* iout) override;
   int aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n_items, const std::string& w, std::vector<AidJob>& job,
                      const msckf_b200_aid_iter* iter);
+  int standstill(const void* const* readings, const int* k, const msckf_b200_standstill* cfg, msckf_b200_standstill_result* out) override;
   int aid_run(const std::vector<AidJob>& job, msckf_b200_aid_result* out, const char* what, const msckf_b200_aid_fde* fde = nullptr,
               msckf_b200_aid_fde_result* fout = nullptr, const msckf_b200_aid_iter* iter = nullptr,
               msckf_b200_aid_iter_result* iout = nullptr);
@@ -1545,7 +1554,8 @@ static_assert((int)MSCKF_B200_AID_BODY_VELOCITY == (int)mb::kAidBodyVelocity && 
                   (int)MSCKF_B200_AID_HEADING == (int)mb::kAidHeading && (int)MSCKF_B200_AID_CLONE_HEADING == (int)mb::kAidCloneHeading &&
                   (int)MSCKF_B200_AID_RANGE == (int)mb::kAidRange && (int)MSCKF_B200_AID_CLONE_RANGE == (int)mb::kAidCloneRange &&
                   (int)MSCKF_B200_AID_PLANE_RANGE == (int)mb::kAidPlaneRange &&
-                  (int)MSCKF_B200_AID_CLONE_PLANE_RANGE == (int)mb::kAidClonePlaneRange,
+                  (int)MSCKF_B200_AID_CLONE_PLANE_RANGE == (int)mb::kAidClonePlaneRange &&
+                  (int)MSCKF_B200_AID_GYRO_AT_REST == (int)mb::kAidGyroAtRest && (int)MSCKF_B200_AID_ACCEL_AT_REST == (int)mb::kAidAccelAtRest,
               "msckf_b200_aid_model and mb::AidModel differ");
 template <class S>
 int Ctx<S>::aid(const msckf_b200_aid* in, msckf_b200_aid_result* out) {
@@ -1623,10 +1633,127 @@ int Ctx<S>::aid_stack_jobs(const msckf_b200_aid_item* const* items, const int* n
     if (iter && (iter[i].max_iter < 0 || iter[i].max_iter > mb::kAidMaxIter))
       return fail(MSCKF_B200_ERR_ARG, w + ": max_iter outside 0..16" + who);
     if (iter && !(std::isfinite(iter[i].tol) && iter[i].tol >= 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": tol is not finite and >= 0" + who);
-    for (int k = 0; k < n_items[i]; ++k)
-      RC(aid_append(job[i], items[i][k], eng[i]->M, w, " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")"));
+    for (int k = 0; k < n_items[i]; ++k) {
+      const std::string wk = " (member " + std::to_string(i) + ", item " + std::to_string(k) + ")";
+      RC(aid_append(job[i], items[i][k], eng[i]->M, w, wk));
+      // the iterate (mb::AidIterate) carries no biases: the at-rest rows are linear in b_g and b_a and nearly so in the attitude
+      if (iter && (items[i][k].model == MSCKF_B200_AID_GYRO_AT_REST || items[i][k].model == MSCKF_B200_AID_ACCEL_AT_REST))
+        return fail(MSCKF_B200_ERR_ARG, w + ": the at-rest models are not iterated" + wk);
+    }
   }
   return 0;
+}
+
+// A standstill window's statistics (msckf_b200_standstill_update, DESIGN.md 4.18), in fp64 and in reading order: T = sum dT_j,
+// the dT-weighted means of omega and a (the at-rest items' z), their R = s^2 R0 / T, the zero-velocity R and the scatter
+// sigma / (6 (k - 1)) of the readings about their means under s^2 R0 (R0: Q_imu's gyro block, rows / columns 0..2, and
+// accelerometer block, 6..8).  0, or MSCKF_B200_ERR_ARG.
+struct StandstillStats {
+  double T = 0.0, w[3] = {0.0, 0.0, 0.0}, a[3] = {0.0, 0.0, 0.0}, scatter = 0.0;
+  double Rv[9] = {}, Rg[9] = {}, Ra[9] = {};
+};
+template <class S>
+int standstill_stats(const S* r, int k, const S* Q, const msckf_b200_standstill& cfg, StandstillStats& o, const std::string& who) {
+  const std::string w = "standstill_update";
+  for (int j = 0; j < k; ++j) {
+    for (int i = 0; i < 7; ++i)
+      if (!std::isfinite((double)r[7 * j + i])) return fail(MSCKF_B200_ERR_ARG, w + ": non-finite reading" + who);
+    if (!((double)r[7 * j + 6] > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": a dT that is not > 0" + who);
+  }
+  double sw[3] = {0.0, 0.0, 0.0}, sa[3] = {0.0, 0.0, 0.0};
+  for (int j = 0; j < k; ++j) {
+    const double dT = r[7 * j + 6];
+    o.T += dT;
+    for (int i = 0; i < 3; ++i) { sw[i] += dT * (double)r[7 * j + i]; sa[i] += dT * (double)r[7 * j + 3 + i]; }
+  }
+  for (int i = 0; i < 3; ++i) { o.w[i] = sw[i] / o.T; o.a[i] = sa[i] / o.T; }
+  // R0's two blocks and their Cholesky factors (lower triangle read)
+  double L[2][9] = {};
+  const double s2 = cfg.noise_scale * cfg.noise_scale;
+  for (int b = 0; b < 2; ++b) {
+    const int c0 = b == 0 ? 0 : 6;
+    double* R = b == 0 ? o.Rg : o.Ra;
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) R[3 * i + j] = s2 * (double)Q[12 * (c0 + i) + c0 + j] / o.T;
+    for (int j = 0; j < 3; ++j) {
+      double d = Q[12 * (c0 + j) + c0 + j];
+      for (int m = 0; m < j; ++m) d -= L[b][3 * j + m] * L[b][3 * j + m];
+      if (!(d > 0.0) || !std::isfinite(d))
+        return fail(MSCKF_B200_ERR_ARG, w + ": Q_imu's " + (b == 0 ? "gyro" : "accelerometer") + " block is not positive definite" + who);
+      L[b][3 * j + j] = std::sqrt(d);
+      for (int i = j + 1; i < 3; ++i) {
+        double t = Q[12 * (c0 + i) + c0 + j];
+        for (int m = 0; m < j; ++m) t -= L[b][3 * i + m] * L[b][3 * j + m];
+        L[b][3 * i + j] = t / L[b][3 * j + j];
+      }
+    }
+  }
+  double sig = 0.0;
+  for (int j = 0; j < k; ++j) {
+    double q = 0.0;
+    for (int b = 0; b < 2; ++b) {  // |L^-1 (y_j - y^)|^2 of the block
+      const double* m = b == 0 ? o.w : o.a;
+      double x[3];
+      for (int i = 0; i < 3; ++i) {
+        double t = (double)r[7 * j + 3 * b + i] - m[i];
+        for (int c = 0; c < i; ++c) t -= L[b][3 * i + c] * x[c];
+        x[i] = t / L[b][3 * i + i];
+        q += x[i] * x[i];
+      }
+    }
+    sig += (double)r[7 * j + 6] * q;
+  }
+  o.scatter = sig / s2 / (6.0 * (k - 1));
+  const double v2 = cfg.sigma_v * cfg.sigma_v;
+  for (int i = 0; i < 3; ++i) o.Rv[4 * i] = v2;
+  return 0;
+}
+
+template <class S>
+int Ctx<S>::standstill(const void* const* readings, const int* k, const msckf_b200_standstill* cfg, msckf_b200_standstill_result* out) {
+  const std::string w = "standstill_update";
+  if (!readings || !k || !cfg || !out) return fail(MSCKF_B200_ERR_ARG, w + ": null argument");
+  RC(members_ready(w.c_str()));
+  if (!(std::isfinite(cfg->noise_scale) && cfg->noise_scale >= 1.0)) return fail(MSCKF_B200_ERR_ARG, w + ": noise_scale is not finite and >= 1");
+  if (!(std::isfinite(cfg->sigma_v) && cfg->sigma_v > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": sigma_v is not finite and > 0");
+  if (!(std::isfinite(cfg->scatter_max) && cfg->scatter_max > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": scatter_max is not finite and > 0");
+  if (!(std::isfinite(cfg->chi2_max) && cfg->chi2_max > 0.0)) return fail(MSCKF_B200_ERR_ARG, w + ": chi2_max is not finite and > 0");
+  const int nf = (int)eng.size();
+  std::vector<StandstillStats> st(nf);
+  for (int i = 0; i < nf; ++i) {
+    if (k[i] == 0) continue;
+    const std::string who = " (member " + std::to_string(i) + ")";
+    if (k[i] < 2 || k[i] > kStandstillMaxReadings) return fail(MSCKF_B200_ERR_ARG, w + ": 2 to 4096 readings" + who);
+    if (!readings[i]) return fail(MSCKF_B200_ERR_ARG, w + ": null readings" + who);
+    RC(standstill_stats((const S*)readings[i], k[i], eng[i]->h_st->Q_imu, *cfg, st[i], who));
+  }
+  // the members at rest by their scatter: the 9-row stack, gated on chi2_max
+  static const double kZero[3] = {0.0, 0.0, 0.0};
+  std::vector<AidJob> job(nf);
+  for (int i = 0; i < nf; ++i) {
+    if (k[i] == 0 || st[i].scatter > cfg->scatter_max) continue;
+    const std::string who = " (member " + std::to_string(i) + ")";
+    RC(aid_append(job[i], {MSCKF_B200_AID_VELOCITY, 0, 0, kZero, st[i].Rv}, eng[i]->M, w, who));
+    RC(aid_append(job[i], {MSCKF_B200_AID_GYRO_AT_REST, 0, 0, st[i].w, st[i].Rg}, eng[i]->M, w, who));
+    RC(aid_append(job[i], {MSCKF_B200_AID_ACCEL_AT_REST, 0, 0, st[i].a, st[i].Ra}, eng[i]->M, w, who));
+    job[i].chi2_max = cfg->chi2_max;
+  }
+  std::vector<msckf_b200_aid_result> res(nf);
+  const int rc = aid_run(job, res.data(), w.c_str());
+  if (rc != 0 && rc != MSCKF_B200_ERR_NUMERIC) return rc;
+  for (int i = 0; i < nf; ++i) {
+    if (k[i] == 0) continue;
+    msckf_b200_standstill_result& o = out[i];
+    o.scatter = st[i].scatter;
+    if (job[i].n_items == 0) {
+      o.stack = msckf_b200_aid_result{std::nan(""), 0.0, 0, 0, 0};
+      o.outcome = 1;
+    } else {
+      o.stack = res[i];
+      o.outcome = res[i].status == 1 ? -1 : res[i].applied ? 0 : 2;
+    }
+  }
+  return rc;
 }
 
 template <class S>
@@ -2252,6 +2379,11 @@ int msckf_b200_batch_aid_stack_update_iter(msckf_b200_batch* b, const msckf_b200
   if (!b || !iter || !iter_out) return fail(MSCKF_B200_ERR_ARG, "null argument");
   return b->ctx->aid_stack(items, n_items, chi2_max, out, iter, iter_out);
 }
+int msckf_b200_batch_standstill_update(msckf_b200_batch* b, const void* const* readings, const int* k, const msckf_b200_standstill* cfg,
+                                       msckf_b200_standstill_result* out) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return b->ctx->standstill(readings, k, cfg, out);
+}
 int msckf_b200_batch_aid_stack_update_fde(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const int* n_items,
                                           const msckf_b200_aid_fde* fde, msckf_b200_aid_fde_result* out) {
   if (!b) return fail(MSCKF_B200_ERR_ARG, "null argument");
@@ -2337,6 +2469,12 @@ int msckf_b200_aid_stack_update_fde_iter(msckf_b200_engine* e, const msckf_b200_
   if (!e || !iter || !iter_out) return fail(MSCKF_B200_ERR_ARG, "null argument");
   if (n_items < 1) return fail(MSCKF_B200_ERR_ARG, "aid_stack_update_fde_iter: 1 to 8 items per stack");
   return e->impl->solo_ctx()->aid_stack_fde(&items, &n_items, fde, out, iter, iter_out);
+}
+int msckf_b200_standstill_update(msckf_b200_engine* e, const void* readings, int k, const msckf_b200_standstill* cfg,
+                                 msckf_b200_standstill_result* out) {
+  if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  if (k < 2 || k > kStandstillMaxReadings) return fail(MSCKF_B200_ERR_ARG, "standstill_update: 2 to 4096 readings");
+  return e->impl->solo_ctx()->standstill(&readings, &k, cfg, out);
 }
 int msckf_b200_landmark_update(msckf_b200_engine* e, const msckf_b200_landmarks* lm, msckf_b200_landmark_result* out) {
   return msckf_b200_map_landmark_update(e, lm, nullptr, out);

@@ -175,6 +175,20 @@ class FilterBatch:
                     r.update(o.as_dict())
         return res
 
+    def standstill_update(self, readings, cfg):
+        """MSCKFBatch::standstillUpdate: readings[i] = [k_i, 7] (omega, a, dT) for filter i, or None / k_i = 0 (filter i left
+        alone); cfg as for capi.standstill_struct; one device call for the batch.  A list of result dicts (None for a filter
+        left alone)."""
+        from .capi import StandstillResult, standstill_struct
+        n = len(self.filters)
+        assert len(readings) == n
+        rs = [np.zeros((0, 7)) if r is None else np.asarray(r, float).reshape(-1, 7) for r in readings]
+        flat, pr = _d(np.concatenate(rs) if sum(len(r) for r in rs) else np.zeros(7))
+        cnt = np.array([len(r) for r in rs], dtype=np.int32)
+        c, out = standstill_struct(cfg), (StandstillResult * n)()
+        self._call("standstill_update", cnt.ctypes.data_as(_ip), pr, C.byref(c), out)
+        return [o.as_dict() if len(r) else None for r, o in zip(rs, out)]
+
     def map_update(self, obs, R=None, chi2_obs=0.0, max_iter=1, tol=1e-10):
         """MSCKFBatch::landmarkUpdate over mapObservation / mapLandmark: obs[i] = (state_ids [n], landmark [n], z [n, 2],
         p_L [L, 3], Sigma [L, 6] or [L, 3, 3]) for filter i, or None (left alone); one device call for the batch.  A list of
@@ -465,6 +479,15 @@ class CFilter:
         if it is not None:
             res.update(iout.as_dict())
         return res
+
+    def standstill_update(self, readings, cfg):
+        """MSCKF::standstillUpdate (include/msckf_b200.h: msckf_b200_standstill_update): readings [k, 7] (omega, a, dT), cfg
+        as for capi.standstill_struct.  A dict: the stack's nis, dx_norm, dof, applied, status, then scatter and outcome."""
+        from .capi import StandstillResult, standstill_struct
+        r, pr = _d(np.asarray(readings, float).reshape(-1, 7))
+        c, out = standstill_struct(cfg), StandstillResult()
+        self._chk(self._f("standstill_update")(self.h, pr, C.c_int(len(r)), C.byref(c), C.byref(out)), "standstill_update")
+        return out.as_dict()
 
     def body_velocity_update(self, v_I, R, mask=7, chi2_max=0.0):
         """MSCKF::bodyVelocityUpdate: the IMU's velocity v_I in its own frame, rows selected by mask (bits 0..2), R over them"""

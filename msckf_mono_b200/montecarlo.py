@@ -391,10 +391,12 @@ def imu_dict(v):
 
 
 # ---- truth and trials ------------------------------------------------------------------------------------------------------
-def make_truth(n_frames=200, seq=0, max_features=60, max_track_length=20, max_cam_states=20, noise=None):
-    """the noise-free stream, with the truth IMU state per frame (zero biases) and the truth camera pose per state_id"""
+def make_truth(n_frames=200, seq=0, max_features=60, max_track_length=20, max_cam_states=20, noise=None, stop=None):
+    """the noise-free stream, with the truth IMU state per frame (zero biases) and the truth camera pose per state_id.
+    stop = dict(every, frames, ramp): the trajectory stops (synth.StopProfile), and "frame_class" holds per frame the class of
+    the interval since the previous frame: "stationary" (at rest all through), "ramp" or "cruise" (frame 0: None)."""
     wl = synth.make_stream_workload(n_frames=n_frames, seq=seq, max_features=max_features, max_track_length=max_track_length,
-                                    max_cam_states=max_cam_states, pixel_sigma=0.0, imu_noise_frac=0.0)
+                                    max_cam_states=max_cam_states, pixel_sigma=0.0, imu_noise_frac=0.0, stop=stop)
     wl["noise"] = synth.euroc_noise(tuned=True) if noise is None else noise
     traj, cam = wl["traj"], wl["camera"]
     wl["truth_imu"] = np.array([imu_vector(synth.true_imu_state(traj, fr["time"])) for fr in wl["frames"]])
@@ -403,6 +405,9 @@ def make_truth(n_frames=200, seq=0, max_features=60, max_track_length=20, max_ca
         C, p = synth.cam_pose(traj, fr["time"], cam)
         poses.append(np.concatenate([p, synth.rot_to_quat(C)]))
     wl["truth_pose"] = np.array(poses)  # row = state_id (= frame index)
+    if stop is not None:
+        fr = wl["frames"]
+        wl["frame_class"] = [None] + [traj.frame_class(fr[k - 1]["time"], fr[k]["time"]) for k in range(1, len(fr))]
     return wl
 
 
@@ -521,14 +526,20 @@ def truth_imu_of(truth, trial, frame):
 
 # ---- summaries ---------------------------------------------------------------------------------------------------------------
 def trial_record(nees_rows, pos_err2, fix_nis=(), map_rows=(), odo_rows=(), map_first=None, gnss_rows=None, range_rows=None,
-                 range_first=None, gnss_first=None):
+                 range_first=None, gnss_first=None, frame_class=None, standstill_rows=None):
     """one trial's per-frame NEES (list of result dicts), squared position errors, the NIS of its position fixes, of its
     map updates (result dicts of landmark_update: nis, dof, used, applied, plus the observation count n) and of its odometry
     stacks (result dicts of aid_stack_update: nis, dof, applied), as plain lists; map_first (a dict of plain numbers: frame,
     squared position error before and after, nis, dof, iterations, converged) describes the first map update; gnss_rows
     (result dicts of aid_stack_update, dof 0 for an epoch whose clone had left the window) the GNSS stacks, range_rows (the
-    same) the ranging stacks; range_first / gnss_first (as map_first) the first ranging / GNSS stack"""
+    same) the ranging stacks; range_first / gnss_first (as map_first) the first ranging / GNSS stack; frame_class (the truth's
+    per frame, with stops) and standstill_rows (per frame from frame 1 on, result dicts of standstill_update)"""
     rec = _trial_record(nees_rows, pos_err2, fix_nis, map_rows, odo_rows)
+    if frame_class is not None:
+        rec["frame_class"] = list(frame_class)
+    if standstill_rows is not None:
+        rec["standstill"] = {k: [float(r[k]) if k in ("nis", "scatter") else int(r[k]) for r in standstill_rows]
+                             for k in ("nis", "dof", "applied", "outcome", "scatter")}
     for key, first in (("map_first", map_first), ("range_first", range_first), ("gnss_first", gnss_first)):
         if first is not None:
             rec[key] = dict(first)
@@ -651,6 +662,8 @@ def summarize(records):
                            "run_bounds": list(chi2_bounds(int(D.sum()), V.size)),
                            "updates_inside": float(np.mean([l_ <= a <= h_ for a, l_, h_ in zip(anis, lo, hi)])),
                            "applied": float(np.mean([a for o in od for a in o["applied"]]))}
+    if all("frame_class" in records[k] for k in keys):  # the stops: position-error growth over each, and standstill detection
+        out["stops"] = stop_summary([records[k] for k in keys])
     for key in ("gnss", "range"):  # ANIS of the GNSS and of the ranging stacks: the stack's rows per trial and epoch fused
         gn = [records[k].get(key) for k in keys]
         if not all(g is not None and len(g["nis"]) for g in gn):
@@ -672,6 +685,38 @@ def summarize(records):
                     "degenerate": int(sum(s == 2 for g in gn for s in g["status"])),
                     **{c: int(sum(g.get(c, 0) for g in gn)) for c in ("injected", "faults_excluded", "clean_excluded", "faults_missed",
                                                                       "stacks_rejected")}}
+    return out
+
+
+def stop_summary(recs):
+    """Over trial records with frame classes: the stops (maximal runs of stationary frames), the mean growth of the position
+    error |e| over a stop (from the frame before it to its last frame), and with standstill rows the fraction of frames
+    detected (outcome 0) per frame class and the ANIS of the applied stacks against the 9-dof run bounds"""
+    cls = recs[0]["frame_class"]
+    stops, f = [], 1
+    while f < len(cls):
+        if cls[f] == "stationary":
+            g = f
+            while g + 1 < len(cls) and cls[g + 1] == "stationary":
+                g += 1
+            stops.append((f, g))
+            f = g + 1
+        else:
+            f += 1
+    growth = [float(np.sqrt(r["pos_err2"][b]) - np.sqrt(r["pos_err2"][a - 1])) for r in recs for a, b in stops]
+    out = {"stops": [list(s) for s in stops], "frames": {c: int(sum(x == c for x in cls)) for c in ("stationary", "ramp", "cruise")},
+           "pos_err_growth_per_stop": float(np.mean(growth)) if growth else float("nan")}
+    if all("standstill" in r for r in recs):
+        det = {c: [] for c in ("stationary", "ramp", "cruise")}
+        for r in recs:
+            for f, o in enumerate(r["standstill"]["outcome"], start=1):
+                det[cls[f]].append(o == 0)
+        out["detected"] = {c: float(np.mean(v)) if v else float("nan") for c, v in det.items()}
+        V = np.array([x for r in recs for x, a in zip(r["standstill"]["nis"], r["standstill"]["applied"]) if a])
+        out["applied"] = int(V.size)
+        out["anis"] = float(V.mean()) if V.size else float("nan")
+        out["run_bounds"] = list(chi2_bounds(9 * int(V.size), int(V.size))) if V.size else [float("nan")] * 2
+        out["dof"] = 9
     return out
 
 
@@ -727,7 +772,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         range_lever=(0.0, 0.0, 0.0), range_delay=0, plane_every=0, plane_sigma=0.02, plane_height=PLANE_HEIGHT, plane_axis=PLANE_AXIS,
         plane_lever=(0.0, 0.0, 0.0), range_outlier_rate=0.0, range_outlier_bias=1.0, gnss_outlier_rate=0.0, gnss_outlier_jump=5.0,
         fde_alpha=0.0, fde_max_exclude=2, range_start=0, gnss_start=0, aid_iterations=1, aid_tol=1e-10, map_outlier_rate=0.0,
-        map_consensus=0, map_consensus_thresh=13.8, map_min_inliers=6):
+        map_consensus=0, map_consensus_thresh=13.8, map_min_inliers=6, standstill=None):
     """Trials (indices) as one fully batched MSCKFBatch stream: per frame propagate, augmentState, update / addFeatures,
     marginalize, pruneEmptyStates, [every fix_every frames one batched position fix of standard deviation fix_sigma],
     [every odo_every frames one batched odometry stack (odometry_items)],
@@ -752,7 +797,10 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     landmark's, drawn from the stream default_rng([seed, k, 12]); no draw when the rate is 0), and map_consensus H > 0 selects the
     inliers by a consensus of H hypotheses (threshold map_consensus_thresh, min_inliers map_min_inliers, seed [seed, k, frame])
     before each map update (exact map only); with either, each map row also counts wrong matches left out of the update and right ones used],
-    refreshState, then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.  The first
+    refreshState,
+    (standstill = a cfg dict as for capi.standstill_struct: from frame 1 on, before augmentState, one batched standstill update
+    of each filter's readings of the frame interval; a filter at rest (outcome 0) skips that frame's augmentState / update /
+    addFeatures / marginalize / pruneEmptyStates and keeps propagating; no random draw), then one batched NEES with each filter's truth window looked up by the state_ids of getCamStates.  The first
     map update is also recorded on its own (trial_record's map_first; the state is read just before it).
     Returns ({trial: trial_record}, {trial: final (covariance, imu [29], poses [M, 7])})."""
     from . import engine_filter
@@ -842,6 +890,7 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
                                   converged=int(r.get("converged", 0)))
 
     R_fix = (fix_sigma ** 2) * np.eye(3)
+    still = [[] for _ in trs]
     nis = [[] for _ in trs]
     maps = [[] for _ in trs]
     odo = [[] for _ in trs]
@@ -856,12 +905,27 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
         for i, fr in enumerate(frs):
             for (w, a, dT) in fr["imu"]:
                 fb.propagate(i, w, a, dT)
-        fb.augmentState([fr["state_id"] for fr in frs], [fr["time"] for fr in frs])
-        for f, fr in zip(fs, frs):
-            f.update(*fr["update"])
-            f.addFeatures(*fr["add"])
-        fb.marginalize()
-        fb.pruneEmptyStates()
+        skip = [False] * len(trs)
+        if standstill is not None and fi > 0:
+            res = fb.standstill_update([np.array([np.r_[w, a, dT] for (w, a, dT) in fr["imu"]]) for fr in frs], standstill)
+            for i, r in enumerate(res):
+                still[i].append(r)
+                skip[i] = r["outcome"] == 0
+        if not any(skip):
+            fb.augmentState([fr["state_id"] for fr in frs], [fr["time"] for fr in frs])
+            for f, fr in zip(fs, frs):
+                f.update(*fr["update"])
+                f.addFeatures(*fr["add"])
+            fb.marginalize()
+            fb.pruneEmptyStates()
+        elif not all(skip):  # the filters still moving step on their own
+            for f, fr, sk in zip(fs, frs, skip):
+                if not sk:
+                    f.augmentState(fr["state_id"], fr["time"])
+                    f.update(*fr["update"])
+                    f.addFeatures(*fr["add"])
+                    f.marginalize()
+                    f.pruneEmptyStates()
         if fix_every > 0 and trs[0]["fixes"][fi] is not None:
             res = fb.aid_update([{"model": AID_POSITION, "z": tr["fixes"][fi], "R": R_fix} for tr in trs])
             for i, r in enumerate(res):
@@ -936,7 +1000,8 @@ def run(trials, truth, dtype=np.float64, seed=0, on_frame=None, fix_every=0, fix
     fb.close()
     records = {tr["k"]: trial_record(rows[i], err2[i], nis[i], maps[i], odo[i], first[i], None if gnss is None else gnss[i],
                                      None if ranging is None else ranging[i], None if first_r is None else first_r[i],
-                                     None if first_g is None else first_g[i])
+                                     None if first_g is None else first_g[i], truth.get("frame_class"),
+                                     still[i] if standstill is not None else None)
                for i, tr in enumerate(trs)}
     final = {}
     for f, tr in zip(fs, trs):

@@ -155,6 +155,71 @@ class Trajectory:
         return so3_log(self.R_GI(t - h).T @ self.R_GI(t + h)) / (2 * h)
 
 
+class StopProfile:
+    """The trajectory `base` driven through the time warp s(t): stops of `frames` frames every `every` frames, entered and left
+    through quintic ramps of `ramp` frames each, so that the speed s' and s'' are continuous.  Period p starts at t0 + p every
+    frame_dt: (every - frames - 2 ramp) frames at full speed (s' = 1), a ramp down (s' = 1 - q(u), q(u) = 6u^5 - 15u^4 + 10u^3),
+    the stop (s' = 0), a ramp up (s' = q(u)).  Before t0 it runs at full speed.  With s = s(t): pos = base.pos(s),
+    vel = base.vel(s) s', acc = base.acc(s) s'^2 + base.vel(s) s'', R_GI = base.R_GI(s) and omega_body = s' base.omega_body(s),
+    so that a reading at rest is exactly omega = 0, a = -C g."""
+
+    def __init__(self, base, t0, frame_dt, every, frames, ramp):
+        assert ramp >= 1 and frames >= 1 and every >= frames + 2 * ramp + 1, (every, frames, ramp)
+        self.base, self.t0 = base, t0
+        self.r, self.w = base.r, base.w
+        self.P, self.A, self.D, self.S = every * frame_dt, (every - frames - 2 * ramp) * frame_dt, ramp * frame_dt, frames * frame_dt
+
+    def warp(self, t):
+        """(s, s', s'') at time t"""
+        if t < self.t0:
+            return t, 1.0, 0.0
+        n, tau = divmod(t - self.t0, self.P)
+        s0 = self.t0 + n * (self.A + self.D)
+        A, D, S = self.A, self.D, self.S
+        if tau < A:
+            return s0 + tau, 1.0, 0.0
+        if tau < A + D:
+            u = (tau - A) / D
+            return s0 + A + D * (u - (u ** 6 - 3 * u ** 5 + 2.5 * u ** 4)), 1.0 - (6 * u ** 5 - 15 * u ** 4 + 10 * u ** 3), \
+                -(30 * u ** 4 - 60 * u ** 3 + 30 * u ** 2) / D
+        if tau < A + D + S:
+            return s0 + A + 0.5 * D, 0.0, 0.0
+        u = (tau - A - D - S) / D
+        return s0 + A + 0.5 * D + D * (u ** 6 - 3 * u ** 5 + 2.5 * u ** 4), 6 * u ** 5 - 15 * u ** 4 + 10 * u ** 3, \
+            (30 * u ** 4 - 60 * u ** 3 + 30 * u ** 2) / D
+
+    def frame_class(self, ta, tb):
+        """'stationary' when s' = 0 over all of [ta, tb], 'cruise' when s' = 1 over all of it, else 'ramp'"""
+        if ta < self.t0:
+            return "cruise" if tb <= self.t0 + self.A else "ramp"
+        na, a = divmod(ta - self.t0, self.P)
+        nb, b = divmod(tb - self.t0, self.P)
+        eps = 1e-9 * self.P  # (frame times are sums of frame_dt: a boundary may land a rounding error either side)
+        if na == nb and self.A + self.D - eps <= a and b <= self.A + self.D + self.S + eps:
+            return "stationary"
+        if (na == nb and b <= self.A + eps) or (nb == na + 1 and b <= eps and a <= self.A + eps):
+            return "cruise"
+        return "ramp"
+
+    def pos(self, t):
+        return self.base.pos(self.warp(t)[0])
+
+    def vel(self, t):
+        s, s1, _ = self.warp(t)
+        return self.base.vel(s) * s1
+
+    def acc(self, t):
+        s, s1, s2 = self.warp(t)
+        return self.base.acc(s) * s1 * s1 + self.base.vel(s) * s2
+
+    def R_GI(self, t):
+        return self.base.R_GI(self.warp(t)[0])
+
+    def omega_body(self, t):
+        s, s1, _ = self.warp(t)
+        return s1 * self.base.omega_body(s)
+
+
 G_VEC = np.array([0.0, 0.0, -9.81])
 
 
@@ -279,13 +344,14 @@ def visible(C, p, pts_G):
 
 def make_stream_workload(n_frames=200, seq=0, max_features=100, imu_per_frame=10, dT=0.005,
                          pixel_sigma=1.0, imu_noise_frac=0.05, n_landmarks=6000,
-                         max_track_length=50, max_cam_states=30, isotropic=False, dropout=0.02):
+                         max_track_length=50, max_cam_states=30, isotropic=False, dropout=0.02, stop=None):
     """E-sim (SURVEY.md 8d): streamed propagate+update sequence with tracks that appear,
     persist while visible and are lost, <= max_features per frame, ids never reused.
 
     Stands in for EuRoC MH_03 (not on this box).  Feature bookkeeping mimics the front end
     (corner_detector.cpp TrackHandler): `update` receives the still-tracked features,
-    `add` the newly detected ones.
+    `add` the newly detected ones.  stop = dict(every, frames, ramp): the trajectory stops (StopProfile, from the first frame
+    on); None: it never does, and every output is what it was without the option.
     """
     rng = np.random.default_rng(BASE_SEED + seq)
     cam = euroc_camera()
@@ -295,6 +361,8 @@ def make_stream_workload(n_frames=200, seq=0, max_features=100, imu_per_frame=10
     traj = Trajectory()
     t0 = 1.0 + 0.37 * seq
     frame_dt = imu_per_frame * dT
+    if stop is not None:
+        traj = StopProfile(traj, t0, frame_dt, stop["every"], stop["frames"], stop["ramp"])
     # landmark shell 3..15 m around the circle (cylindrical)
     ang = rng.uniform(0, 2 * np.pi, n_landmarks)
     rad = traj.r + rng.uniform(3.0, 15.0, n_landmarks)

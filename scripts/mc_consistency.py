@@ -46,6 +46,13 @@ drifted), and --aid-iterations K iterates the GNSS, ranging and odometry stacks 
 <= --aid-tol); the summary then adds the first ranging / GNSS stack: the position RMSE before and after it, its ANIS, the
 IMU-state ANEES after it, the mean linearisations and the share converged.
 
+With --stop-every F --stop-frames K --stop-ramp R the trajectory stops for K frames every F frames, entered and left through
+quintic ramps of R frames (synth.StopProfile), and the summary adds the mean growth of the position error over a stop.
+--standstill tests every frame interval's IMU readings for rest (msckf_b200_standstill_update with --standstill-noise-scale,
+--standstill-sigma-v, --standstill-scatter-max and --standstill-chi2) and skips the vision work of the frames found at rest; the
+summary adds the fraction of frames detected per class (stationary: at rest all through the interval; ramp; cruise) and the
+applied stacks' ANIS against its 9-dof run bounds.
+
 It also times the batched NEES call (msckf_b200_batch_nees) against the host path (get_covariance + get_state per filter and
 a numpy Cholesky solve) for 8 and 32 config-B members (30 clones: n = 195), and reads the card's name and power limit."""
 import argparse
@@ -200,6 +207,14 @@ def main():
     ap.add_argument("--gnss-start", type=int, default=0, help="fuse no GNSS epoch before this frame")
     ap.add_argument("--aid-iterations", type=int, default=1, help="iterate the GNSS, ranging and odometry stacks (linearisations)")
     ap.add_argument("--aid-tol", type=float, default=1e-10)
+    ap.add_argument("--stop-every", type=int, default=0, help="> 0: the trajectory stops every F frames")
+    ap.add_argument("--stop-frames", type=int, default=40)
+    ap.add_argument("--stop-ramp", type=int, default=5)
+    ap.add_argument("--standstill", action="store_true", help="detect standstills and fuse the zero-motion update")
+    ap.add_argument("--standstill-noise-scale", type=float, default=1.0)
+    ap.add_argument("--standstill-sigma-v", type=float, default=0.01)
+    ap.add_argument("--standstill-scatter-max", type=float, default=2.0)
+    ap.add_argument("--standstill-chi2", type=float, default=27.9, help="the 9-row stack's gate (27.9: chi^2_9 at 0.999)")
     ap.add_argument("--no-timing", action="store_true")
     ap.add_argument("--out", type=Path, default=None)
     args = ap.parse_args()
@@ -211,7 +226,10 @@ def main():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl")
     dtype = np.float32 if args.dtype == "f32" else np.float64
-    truth = mc.make_truth(n_frames=args.frames, seq=args.seq)
+    stop = {"every": args.stop_every, "frames": args.stop_frames, "ramp": args.stop_ramp} if args.stop_every > 0 else None
+    standstill = {"noise_scale": args.standstill_noise_scale, "sigma_v": args.standstill_sigma_v,
+                  "scatter_max": args.standstill_scatter_max, "chi2_max": args.standstill_chi2} if args.standstill else None
+    truth = mc.make_truth(n_frames=args.frames, seq=args.seq, stop=stop)
     t0 = time.perf_counter()
     records, _ = mc.run(shard.sequences_of_rank(args.trials, rank, world), truth, dtype=dtype, seed=args.seed,
                         fix_every=args.position_fix_every, fix_sigma=args.position_fix_sigma, map_every=args.map_every,
@@ -229,7 +247,7 @@ def main():
                         range_start=args.range_start, gnss_start=args.gnss_start, aid_iterations=args.aid_iterations,
                         aid_tol=args.aid_tol, map_chi2=args.map_chi2, map_outlier_rate=args.map_outlier_rate,
                         map_consensus=args.map_consensus, map_consensus_thresh=args.map_consensus_thresh,
-                        map_min_inliers=args.map_min_inliers)
+                        map_min_inliers=args.map_min_inliers, standstill=standstill)
     wall = time.perf_counter() - t0
     merged = shard.gather_summaries(records)
     s = mc.summarize(merged)
@@ -275,6 +293,10 @@ def main():
         res["faults"] = {"range_outlier_rate": args.range_outlier_rate, "range_outlier_bias_m": args.range_outlier_bias,
                          "gnss_outlier_rate": args.gnss_outlier_rate, "gnss_outlier_jump_m": args.gnss_outlier_jump,
                          "fde_alpha": args.fde_alpha, "fde_max_exclude": args.fde_max_exclude}
+    if "stops" in s:
+        res["stops"] = dict(s["stops"], every=args.stop_every, frames_per_stop=args.stop_frames, ramp=args.stop_ramp,
+                            standstill=standstill)
+        res["stops"].pop("stops")
     for c, v in s["components"].items():  # the per-frame bounds of the first frame (the same for every frame of a fixed dimension)
         res["components"][c]["bounds_frame0"] = [v["lower"][0], v["upper"][0]]
     if not args.no_timing and rank == 0:
