@@ -611,8 +611,36 @@ int msckf_b200_rank_pivots(msckf_b200_engine* e, double* out, int cap);
  *                  filter, 32 for a device batch).  The results are bit-identical for every value;
  *              7 = CTAs that run the tail's chains of diagonal blocks: 2 (default where the device accepts clusters of 9: Gamma's
  *                  and S''s chains side by side on two CTAs, seven worker CTAs) or 1 (cluster of 8, both chains on one CTA);
- *                  0 = default.  Same rank decisions; results agree to fp64 rounding. */
+ *                  0 = default.  Same rank decisions; results agree to fp64 rounding;
+ *              8 = stop an update after the compression (testing aid, default off): the kernels up to T'', R'', r'' run, nothing
+ *                  after them, so P, the state and delta-x are left as they were and the report's rank is 0.  Before the kernels
+ *                  every compression workspace of the engine is filled with NaN, so an element no kernel wrote shows up as a NaN
+ *                  in msckf_b200_stage_buffer.  A device batch stops only when every member has the option set; a batch whose
+ *                  members disagree is refused at stage time (MSCKF_B200_ERR_ARG, nothing written). */
 int msckf_b200_set_option(msckf_b200_engine* e, int key, double value);
+/* buffers of the last update's compression stage, for msckf_b200_stage_buffer.  n = 15 + 6M, c = 6M, N tracks, O observations */
+enum {
+  MSCKF_B200_STAGE_T2 = 0,       /* T'' [n][n] fp64 */
+  MSCKF_B200_STAGE_R2 = 1,       /* R'' [n][n] fp64 */
+  MSCKF_B200_STAGE_R2_RHS = 2,   /* r'' [n] fp64 */
+  MSCKF_B200_STAGE_Z = 3,        /* Z = U^T X per track [3N][c] fp64 */
+  MSCKF_B200_STAGE_YQ = 4,       /* Yq [3N][c] fp64 */
+  MSCKF_B200_STAGE_UR = 5,       /* U^T r [3N] fp64 */
+  MSCKF_B200_STAGE_D1 = 6,       /* sum X^T X per clone [M][6][6] fp64 */
+  MSCKF_B200_STAGE_D2 = 7,       /* sum X^T D X per clone [M][6][6] fp64 */
+  MSCKF_B200_STAGE_BB = 8,       /* sum X^T r per clone [M][6] fp64 */
+  MSCKF_B200_STAGE_XG = 9,       /* projected clone Jacobian blocks [O][2][6], the filter's dtype */
+  MSCKF_B200_STAGE_RG = 10,      /* residuals [O][2], the filter's dtype */
+  MSCKF_B200_STAGE_VG = 11,      /* Householder vectors of H_f, per track [2L][3], the filter's dtype */
+  MSCKF_B200_STAGE_TAUG = 12,    /* Householder coefficients [N][3], the filter's dtype */
+  MSCKF_B200_STAGE_ACCEPT = 13,  /* gate flags [N] int */
+  MSCKF_B200_STAGE_ROW_OFF = 14  /* first stacked row of each track [N + 1] int */
+};
+/* copy buffer `which` of the last update into out (at most cap elements; out may be NULL when cap is 0) and return its element
+ * count.  T'', R'', r'' are the compression's outputs after an update with option 8 set; after a full update the later
+ * kernels may have reused them.  0 before an update, or after a stage, window growth or track-capacity growth that followed it;
+ * an un-fetched update returns MSCKF_B200_ERR_STATE, an unknown `which` MSCKF_B200_ERR_ARG. */
+int msckf_b200_stage_buffer(msckf_b200_engine* e, int which, void* out, int cap);
 /* checkpoint / resume: copy the complete filter state of src into dst (same dtype and capacities) */
 int msckf_b200_copy_state(msckf_b200_engine* dst, const msckf_b200_engine* src);
 /* number of kernels launched by this handle so far (bench.py's gpu_launches) */

@@ -602,6 +602,28 @@ class Engine:
     def set_option(self, key, value):
         check(lib().msckf_b200_set_option(self.h, C.c_int(key), C.c_double(value)), "msckf_b200_set_option")
 
+    # msckf_b200_stage_buffer: name -> (which, element type (None: the filter's dtype), trailing shape; "n" = 15 + 6M, "c" = 6M)
+    STAGE_BUFFERS = {"T2": (0, np.float64, ("n",)), "R2": (1, np.float64, ("n",)), "r2": (2, np.float64, ()),
+                     "Z": (3, np.float64, ("c",)), "Yq": (4, np.float64, ("c",)), "ur": (5, np.float64, ()),
+                     "D1": (6, np.float64, (6, 6)), "D2": (7, np.float64, (6, 6)), "bb": (8, np.float64, (6,)),
+                     "Xg": (9, None, (2, 6)), "rg": (10, None, (2,)), "Vg": (11, None, (3,)), "taug": (12, None, (3,)),
+                     "accept": (13, np.int32, ()), "row_off": (14, np.int32, ())}
+
+    def stage_buffer(self, name):
+        """one buffer of the last update's compression stage (see STAGE_BUFFERS and include/msckf_b200.h): T2, R2 [n, n];
+        r2 [n]; Z, Yq [3N, c]; ur [3N]; D1, D2 [M, 6, 6]; bb [M, 6]; Xg [O, 2, 6], rg [O, 2], Vg [2O, 3], taug [N, 3] in the
+        filter's dtype; accept [N], row_off [N + 1]; None when there is no such update"""
+        def count(which):
+            return check(lib().msckf_b200_stage_buffer(self.h, C.c_int(which), None, C.c_int(0)), "msckf_b200_stage_buffer")
+        which, dt, shape = self.STAGE_BUFFERS[name]
+        n = count(which)
+        if n == 0:
+            return None
+        out = np.zeros(n, dtype=self.dtype if dt is None else dt)
+        check(lib().msckf_b200_stage_buffer(self.h, C.c_int(which), out.ctypes.data_as(C.c_void_p), C.c_int(n)), "msckf_b200_stage_buffer")
+        M = count(6) // 36  # the window of that update
+        return out.reshape((-1,) + tuple({"n": 15 + 6 * M, "c": 6 * M}.get(d, d) for d in shape))
+
     def kernel_times(self):
         ms = (C.c_float * 32)()
         names = (C.c_char_p * 32)()

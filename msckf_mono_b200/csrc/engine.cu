@@ -224,7 +224,8 @@ inline size_t tail_smem(int n, int kind) { return kind == 0 ? mb::tail_fused_sme
 
 // grid / shared-memory shape of one (batched) update: what a captured graph is valid for
 struct LaunchShape {
-  int nf, mode, tri_gx, jac_gx, bd_gx, gram_gx, gram_gy, asm_gx, rows_gx, gemm_g, syrk_gx, tail_mask, pdl, gram_mma, jac_g, tail_nch;
+  int nf, mode, tri_gx, jac_gx, bd_gx, gram_gx, gram_gy, asm_gx, rows_gx, gemm_g, syrk_gx, tail_mask, pdl, gram_mma, jac_g, tail_nch,
+      stop;  // option 8: the sequence ends after the compression
   unsigned tri_smem, jac_smem, rows_smem, inj_smem, tail_smem[3];
   const void* args;  // device address of the UpdArgs array (moves only when the input arena is re-allocated)
   bool operator==(const LaunchShape& o) const { return memcmp(this, &o, sizeof(*this)) == 0; }
@@ -285,6 +286,7 @@ struct EngineBase {
   virtual int get_counters(long long*) = 0;
   virtual int last_dx(double*, int) = 0;
   virtual int rank_pivots(double*, int) = 0;
+  virtual int stage_buffer(int, void*, int) = 0;
   virtual int copy_from(const EngineBase*) = 0;
   virtual int sync() = 0;
   virtual int input_buffer(int, int, msckf_b200_tracks*) = 0;
@@ -299,6 +301,10 @@ struct EngineBase {
   bool no_fused_tail = false;  // option 3 = 0: substitution as a separate sweep even where the fused form fits
   int tail_chains = 0;         // option 7: CTAs running the tail's chains of diagonal blocks (1, 2; 0 = 2 where the device takes clusters of 9)
   int jac_group = 0;           // option 6: threads per track in k_jac (32 / 64 / 128; 0 = by batch size)
+  bool stop_after_compression = false;  // option 8: an update ends with T'', R'', r'' (msckf_b200_stage_buffer reads them)
+  // the last launched update's sizes, for msckf_b200_stage_buffer (M < 0: none, or its buffers have been re-staged or reallocated
+  // since); accept lives in the launching context's report arena
+  struct StageRec { int N, O, M; const int* accept; } last_stage = {0, 0, -1, nullptr};
   int dtype = 0, device = 0, Mmax = 0, Tmax = 0, Omax = 0;
   int M = 0;
   double rank_thr = 1e-9;
@@ -437,7 +443,7 @@ struct Ctx : CtxBase {
   cudaStream_t stream2 = nullptr, stream3 = nullptr;  // side branches of the update (k_blockdiag, k_rows run beside k_gram)
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_join2 = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
   int st_mode = -1;
-  bool staged = false, timed_region = false;
+  bool staged = false, timed_region = false, st_stop = false;  // st_stop: option 8 of every member
   WorkerPool pool;
   // graph cache
   struct Cached { LaunchShape shape; cudaGraphExec_t exec; int nodes; unsigned long long stamp; };
@@ -731,6 +737,7 @@ struct Engine : EngineBase {
     CK(cudaSetDevice(device));
     CK(cudaStreamSynchronize(stream));
     const int old_ldp = ldp, old_nmax = nmax, old_M = Mmax;
+    last_stage.M = -1;
     Mmax = std::min(kMaxClonesHard, std::max(need, 2 * Mmax));
     set_dims();
     S *nP = nullptr, *nP2 = nullptr, *nposes = nullptr, *nposes2 = nullptr;
@@ -759,8 +766,19 @@ struct Engine : EngineBase {
     CK(cudaStreamSynchronize(stream));
     if (T > Tmax) Tmax = std::max(T, 2 * Tmax);
     if (O > Omax) Omax = std::max(O, 2 * Omax);
+    last_stage.M = -1;
     free_batchws();
     RC(alloc_batchws());
+    return 0;
+  }
+  // option 8: every compression workspace NaN (bytes 0xFF), so that an element no kernel of the update writes reads as NaN
+  int poison_compression(cudaStream_t s) {
+    const size_t T = Tmax, cmax = 6 * (size_t)Mmax;
+    const std::pair<double*, size_t> ws[] = {
+        {d_Z, 3 * T * cmax}, {d_Yq, 3 * T * cmax}, {d_ur, 3 * T}, {d_G1p, kMaxSplit * cmax * cmax},
+        {d_G2p, kMaxSplit * cmax * cmax + kMaxSplit * cmax} /* + bzp */, {d_D1, 36 * (size_t)Mmax}, {d_D2, 36 * (size_t)Mmax},
+        {d_bb, 6 * (size_t)Mmax}, {d_T2, (size_t)ld * nmax}, {d_R2, (size_t)ld * nmax}, {d_r2, (size_t)nmax}};
+    for (const auto& w : ws) CK(cudaMemsetAsync(w.first, 0xFF, sizeof(double) * w.second, s));
     return 0;
   }
 
@@ -966,6 +984,46 @@ struct Engine : EngineBase {
     for (int i = 0; i < std::min(n, cap); ++i) out[i] = tmp[n + i] > 0.0 ? tmp[i] / tmp[n + i] : 0.0;
     return n;
   }
+  int stage_buffer(int which, void* out, int cap) override {
+    if (busy) return fail(MSCKF_B200_ERR_STATE, "stage_buffer with an un-fetched update pending");
+    if (which < MSCKF_B200_STAGE_T2 || which > MSCKF_B200_STAGE_ROW_OFF) return fail(MSCKF_B200_ERR_ARG, "stage_buffer: unknown buffer");
+    if (cap < 0 || (cap > 0 && !out)) return fail(MSCKF_B200_ERR_ARG, "stage_buffer: bad arguments");
+    const StageRec& r = last_stage;
+    if (r.M < 0) return 0;
+    const int n = 15 + 6 * r.M, c = 6 * r.M, N = r.N, O = r.O;
+    const void* src = nullptr;
+    size_t count = 0, elem = sizeof(double);
+    switch (which) {
+      case MSCKF_B200_STAGE_T2: src = d_T2; count = (size_t)n * n; break;
+      case MSCKF_B200_STAGE_R2: src = d_R2; count = (size_t)n * n; break;
+      case MSCKF_B200_STAGE_R2_RHS: src = d_r2; count = n; break;
+      case MSCKF_B200_STAGE_Z: src = d_Z; count = 3 * (size_t)N * c; break;
+      case MSCKF_B200_STAGE_YQ: src = d_Yq; count = 3 * (size_t)N * c; break;
+      case MSCKF_B200_STAGE_UR: src = d_ur; count = 3 * (size_t)N; break;
+      case MSCKF_B200_STAGE_D1: src = d_D1; count = 36 * (size_t)r.M; break;
+      case MSCKF_B200_STAGE_D2: src = d_D2; count = 36 * (size_t)r.M; break;
+      case MSCKF_B200_STAGE_BB: src = d_bb; count = 6 * (size_t)r.M; break;
+      case MSCKF_B200_STAGE_XG: src = d_Xg; count = 12 * (size_t)O; elem = sizeof(S); break;
+      case MSCKF_B200_STAGE_RG: src = d_rg; count = 2 * (size_t)O; elem = sizeof(S); break;
+      case MSCKF_B200_STAGE_VG: src = d_Vg; count = 6 * (size_t)O; elem = sizeof(S); break;
+      case MSCKF_B200_STAGE_TAUG: src = d_taug; count = 3 * (size_t)N; elem = sizeof(S); break;
+      case MSCKF_B200_STAGE_ACCEPT: src = r.accept; count = N; elem = sizeof(int); break;
+      default: src = d_rowoff; count = (size_t)N + 1; elem = sizeof(int); break;
+    }
+    const size_t k = std::min(count, (size_t)cap);
+    if (k > 0) {
+      CK(cudaSetDevice(device));
+      if (which == MSCKF_B200_STAGE_T2 || which == MSCKF_B200_STAGE_R2) {  // n x n, de-strided from ld
+        const size_t rows = k / n;
+        if (rows) CK(cudaMemcpy2DAsync(out, sizeof(double) * n, src, sizeof(double) * ld, sizeof(double) * n, rows, cudaMemcpyDeviceToHost, stream));
+        if (k % n) CK(cudaMemcpyAsync((double*)out + rows * n, (const double*)src + rows * ld, sizeof(double) * (k % n), cudaMemcpyDeviceToHost, stream));
+      } else {
+        CK(cudaMemcpyAsync(out, src, elem * k, cudaMemcpyDeviceToHost, stream));
+      }
+      CK(cudaStreamSynchronize(stream));
+    }
+    return (int)count;
+  }
   int last_dx(double* out, int cap) override {
     CK(cudaSetDevice(device));
     const int n = 15 + 6 * M;
@@ -1036,6 +1094,7 @@ int Ctx<S>::layout(const std::vector<std::pair<int, int>>& NO) {
     p.rep_off = orp; orp += up256(Plan<S>::rep_bytes(p.N));
   }
   in_used = oi; rep_used = orp;
+  for (auto* e : eng) e->last_stage.M = -1;
   const unsigned char* old = in.d;
   RC(in.ensure(in_used, stream));
   RC(rep.ensure(rep_used, stream));
@@ -1053,6 +1112,8 @@ int Ctx<S>::stage(int mode, const msckf_b200_tracks* tracks, int threads) {
     if (!e) return fail(MSCKF_B200_ERR_STATE, "a member engine of this batch was destroyed");
     if (!e->initialized) return fail(MSCKF_B200_ERR_STATE, "update before initialize");
     if (e->busy) return fail(MSCKF_B200_ERR_STATE, "previous update not fetched");
+    if (e->stop_after_compression != eng[0]->stop_after_compression)
+      return fail(MSCKF_B200_ERR_ARG, "option 8 (stop after the compression) must be the same for every member of a batch");
   }
   CK(cudaSetDevice(device));
   std::vector<std::pair<int, int>> NO(nf);
@@ -1132,6 +1193,7 @@ int Ctx<S>::stage(int mode, const msckf_b200_tracks* tracks, int threads) {
   RC(for_all(pack));
   CK(cudaMemcpyAsync(in.d, in.h, in_used, cudaMemcpyHostToDevice, stream));
   st_mode = mode;
+  st_stop = eng[0]->stop_after_compression;
   staged = true;
   return 0;
 }
@@ -1149,6 +1211,7 @@ int Ctx<S>::launch() {
   LaunchShape sh;
   memset(&sh, 0, sizeof(sh));
   sh.nf = nf; sh.mode = mode; sh.args = d_args();
+  sh.stop = st_stop && mode != MSCKF_B200_TRIANGULATE ? 1 : 0;
   int Nmax = 0, Mmax_ = 0, Lm = 0, nmax_ = 0, nsplit = 1, jac_L = 0, jac_M = 0;
   for (int i = 0; i < nf; ++i) {
     const Plan<S>& p = plan[i];
@@ -1176,8 +1239,13 @@ int Ctx<S>::launch() {
   // a stage or launch that fails on a capacity leaves the last update's diagnostics alone; the window may shrink before they
   // are asked for
   if (mode != MSCKF_B200_TRIANGULATE)
-    for (int i = 0; i < nf; ++i)
-      if (plan[i].N > 0) eng[i]->pivr_n = h_args()[i].n;
+    for (int i = 0; i < nf; ++i) {
+      if (plan[i].N == 0) continue;
+      Engine<S>* e = eng[i];
+      e->last_stage = {plan[i].N, plan[i].O, e->M, plan[i].d_accept};
+      if (sh.stop) RC(e->poison_compression(stream));  // (ahead of the graph: never captured)
+      else e->pivr_n = h_args()[i].n;
+    }
   const int Nr = (Nmax + 15) & ~15;  // rounded track count: kernels exit on blockIdx >= their filter's own N
   // (k_jac's at the SM's allocation granularity of 128 B: a whole KB would cost a batch of 8 config-B filters its tenth CTA per SM)
   sh.tri_smem = (sh.tri_smem + 1023) & ~1023u; sh.jac_smem = (sh.jac_smem + 127) & ~127u;
@@ -1308,6 +1376,7 @@ int Ctx<S>::run_kernels(const LaunchShape& sh) {
     launches++;
     mark("k_assemble");
     if (fork) CK(cudaStreamWaitEvent(stream, ev_join2, 0));
+    if (sh.stop) return 0;
     CK(launch_k(mb::k_gemm_tp<S>, dim3(sh.gemm_g, sh.gemm_g, nf), dim3(mb::kGemmThreads), 0, stream, false, 1, A));
     mark("k_gemm_tp");
     CK(launch_k(mb::k_gemm_s<S>, dim3(sh.syrk_gx, 1, nf), dim3(mb::kGemmThreads), 0, stream, pdl, 1, A));  // lower tile pairs of S''
@@ -1374,7 +1443,7 @@ int Ctx<S>::fetch(msckf_b200_report* reports) {
       if (rep->accepted) memcpy(rep->accepted, p.h_accept, sizeof(int) * N);
       if (rep->gamma) memcpy(rep->gamma, p.h_gamma, sizeof(S) * N);
       rep->m = p.h_mr[0];
-      rep->rank = p.h_mr[1];
+      rep->rank = st_stop ? 0 : p.h_mr[1];  // (option 8: no rank decision was made)
     }
   }
   if (status != 0) return fail(status, "non-finite delta-x or covariance after the update (the update has been applied, like msckf.h:1369-1418 would), or the tail kernel's two chain CTAs lost their hand-off");
@@ -2512,6 +2581,10 @@ int msckf_b200_set_covariance(msckf_b200_engine* e, const void* in) { return e->
 int msckf_b200_get_counters(msckf_b200_engine* e, long long* counters) { return e->impl->get_counters(counters); }
 int msckf_b200_last_delta_x(msckf_b200_engine* e, double* out, int cap) { return e->impl->last_dx(out, cap); }
 int msckf_b200_rank_pivots(msckf_b200_engine* e, double* out, int cap) { return e->impl->rank_pivots(out, cap); }
+int msckf_b200_stage_buffer(msckf_b200_engine* e, int which, void* out, int cap) {
+  if (!e) return fail(MSCKF_B200_ERR_ARG, "null argument");
+  return e->impl->stage_buffer(which, out, cap);
+}
 int msckf_b200_kernel_times(msckf_b200_engine* e, float* ms, const char** names, int cap) { return e->impl->solo_ctx()->kernel_times(ms, names, cap); }
 int msckf_b200_tail_profile(msckf_b200_engine* e, unsigned long long* out, int cap) { return e->impl->tail_profile(out, cap); }
 int msckf_b200_set_option(msckf_b200_engine* e, int key, double value) {
@@ -2521,6 +2594,7 @@ int msckf_b200_set_option(msckf_b200_engine* e, int key, double value) {
   if (key == 3) { e->impl->no_fused_tail = value == 0; return 0; }
   if (key == 4) { e->impl->use_pdl = value != 0; return 0; }
   if (key == 5) { e->impl->gram_mma = value != 0; return 0; }
+  if (key == 8) { e->impl->stop_after_compression = value != 0; return 0; }  // (part of LaunchShape: graphs never mix the two)
   if (key == 7) {
     if (value != 0 && value != 1 && value != 2) return fail(MSCKF_B200_ERR_ARG, "option 7: 0, 1 or 2");
     e->impl->tail_chains = (int)value;

@@ -167,6 +167,7 @@ int msckf_b200_rank_pivots(msckf_b200_engine* e, double* out, int cap) {
   return n;
 }
 int msckf_b200_set_option(msckf_b200_engine*, int, double) { return 0; }
+int msckf_b200_stage_buffer(msckf_b200_engine*, int, void*, int) { return 0; }  // (no update buffers: none recorded)
 int msckf_b200_copy_state(msckf_b200_engine* dst, const msckf_b200_engine* src) { *dst = *src; return 0; }
 long long msckf_b200_launch_count(const msckf_b200_engine* e) { return e->launches; }
 void* msckf_b200_stream(msckf_b200_engine*) { return nullptr; }
