@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/aid_capi.cpp -- aided measurement updates in the C view (include/msckf_mono_c.h,
 // msckf_mono_aid_update / msckf_mono_batch_aid_update): MSCKF<_S>::aidedUpdate and MSCKFBatch<_S>::aidedUpdate over handles
-// created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own translation unit, so that the other view files link
-// against a C-ABI without msckf_b200_aid_update / msckf_b200_batch_aid_update.
+// created by filter_capi.cpp and batch_capi.cpp.  Host code only; calls the engine C-ABI's
+// msckf_b200_aid_update / msckf_b200_batch_aid_update.
 #include <stdexcept>
 #include <vector>
 #include <msckf_mono/msckf.h>

@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/aid_iter_capi.cpp -- iterated stacked aided updates in the C view (include/msckf_mono_c.h,
 // msckf_mono_aid_stack_update_iter / _fde_iter and their batch forms): MSCKF<_S>::aidedUpdate(items, chi2_max | fde, iter,
-// iter_out) and the MSCKFBatch<_S> forms over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own
-// translation unit, so that the other view files link against a C-ABI without the _iter entry points.
+// iter_out) and the MSCKFBatch<_S> forms over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; calls
+// the engine C-ABI's _iter entry points.
 #include <stdexcept>
 #include <vector>
 #include <msckf_mono/msckf.h>

@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/aid_stack_capi.cpp -- stacked aided updates (odometry) in the C view (include/msckf_mono_c.h,
 // msckf_mono_aid_stack_update / _batch_aid_stack_update / _body_velocity_update / _relative_pose_update): MSCKF<_S>::aidedUpdate
 // (items), bodyVelocityUpdate, relativePoseUpdate and MSCKFBatch<_S>::aidedUpdate(items) over handles created by filter_capi.cpp
-// and batch_capi.cpp.  Host code only; its own translation unit, so that the other view files link against a C-ABI without
+// and batch_capi.cpp.  Host code only; calls the engine C-ABI's
 // msckf_b200_aid_stack_update / msckf_b200_batch_aid_stack_update.
 #include <stdexcept>
 #include <vector>

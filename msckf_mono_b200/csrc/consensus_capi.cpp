@@ -1,8 +1,8 @@
 // msckf_mono_b200/csrc/consensus_capi.cpp -- mapped-landmark updates with a consensus on the matches in the C view
 // (include/msckf_mono_c.h, msckf_mono_landmark_update_consensus / msckf_mono_batch_landmark_update_consensus):
 // MSCKF<_S>::landmarkUpdate and MSCKFBatch<_S>::landmarkUpdate with a msckf_b200_landmark_consensus, exact map, on handles
-// created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own translation unit, so that the other view files link
-// against a C-ABI without msckf_b200_landmark_update_consensus / _batch_landmark_update_consensus.
+// created by filter_capi.cpp and batch_capi.cpp.  Host code only; calls the engine C-ABI's
+// msckf_b200_landmark_update_consensus / _batch_landmark_update_consensus.
 #include <stdexcept>
 #include <vector>
 #include <msckf_mono/msckf.h>

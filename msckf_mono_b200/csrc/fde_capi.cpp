@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/fde_capi.cpp -- stacked aided updates with fault detection and exclusion in the C view
 // (include/msckf_mono_c.h, msckf_mono_aid_stack_update_fde / msckf_mono_batch_aid_stack_update_fde): MSCKF<_S>::aidedUpdate(items,
 // fde) and MSCKFBatch<_S>::aidedUpdate(items, fde) over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only;
-// its own translation unit, so that the other view files link against a C-ABI without msckf_b200_aid_stack_update_fde.
+// calls the engine C-ABI's msckf_b200_aid_stack_update_fde / msckf_b200_batch_aid_stack_update_fde.
 #include <stdexcept>
 #include <vector>
 #include <msckf_mono/msckf.h>

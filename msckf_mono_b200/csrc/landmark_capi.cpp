@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/landmark_capi.cpp -- mapped-landmark updates in the C view (include/msckf_mono_c.h,
 // msckf_mono_landmark_update / msckf_mono_batch_landmark_update and their _iter forms): MSCKF<_S>::landmarkUpdate and MSCKFBatch<_S>::landmarkUpdate
-// over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own translation unit, so that the other view
-// files link against a C-ABI without msckf_b200_landmark_update / msckf_b200_batch_landmark_update.
+// over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; calls the engine C-ABI's
+// msckf_b200_landmark_update / msckf_b200_batch_landmark_update.
 #include <stdexcept>
 #include <vector>
 #include <msckf_mono/msckf.h>

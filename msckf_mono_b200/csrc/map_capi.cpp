@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/map_capi.cpp -- mapped-landmark updates with map uncertainty in the C view (include/msckf_mono_c.h,
 // msckf_mono_map_update / msckf_mono_batch_map_update): MSCKF<_S>::landmarkUpdate and MSCKFBatch<_S>::landmarkUpdate over
-// mapObservation / mapLandmark, on handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own translation
-// unit, so that the other view files link against a C-ABI without msckf_b200_map_landmark_update.
+// mapObservation / mapLandmark, on handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; calls the
+// engine C-ABI's msckf_b200_map_landmark_update / msckf_b200_batch_map_landmark_update.
 #include <stdexcept>
 #include <vector>
 #include <msckf_mono/msckf.h>

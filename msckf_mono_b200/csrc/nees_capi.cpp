@@ -1,6 +1,6 @@
 // msckf_mono_b200/csrc/nees_capi.cpp -- consistency against ground truth in the C view (include/msckf_mono_c.h,
 // msckf_mono_nees / msckf_mono_batch_nees): MSCKF<_S>::nees and MSCKFBatch<_S>::nees over handles created by filter_capi.cpp
-// and batch_capi.cpp.  Host code only; its own translation unit, so that the other two link against a C-ABI without
+// and batch_capi.cpp.  Host code only; calls the engine C-ABI's
 // msckf_b200_nees / msckf_b200_batch_nees.
 #include <stdexcept>
 #include <vector>

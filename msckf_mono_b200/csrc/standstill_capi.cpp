@@ -1,7 +1,7 @@
 // msckf_mono_b200/csrc/standstill_capi.cpp -- standstill detection and the zero-motion update in the C view
 // (include/msckf_mono_c.h, msckf_mono_standstill_update / _batch_standstill_update): MSCKF<_S>::standstillUpdate and
-// MSCKFBatch<_S>::standstillUpdate over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; its own
-// translation unit, so that the other view files link against a C-ABI without msckf_b200_standstill_update /
+// MSCKFBatch<_S>::standstillUpdate over handles created by filter_capi.cpp and batch_capi.cpp.  Host code only; calls the
+// engine C-ABI's msckf_b200_standstill_update /
 // msckf_b200_batch_standstill_update.
 #include <stdexcept>
 #include <vector>

@@ -4,8 +4,8 @@
 // ROS node's set-up (/root/reference/src/ros_interface.cpp:250-262 Matrix4 T_cam_imu, :92-116 frame loop) -- written against
 // the drop-in headers of THIS repo.  It touches every boundary symbol those callers use: the type aliases of types.h
 // (Matrix4, Matrix3, Vector3, Quaternion, aligned vectors of Vector2), matrix_utils.h, the class surface with the
-// reference's exact signatures, a const filter, a container of filters.  Linked against tests/stub/stub_engine.cpp (no GPU)
-// it runs a few frames and prints a checksum of the integer bookkeeping.  Compiled twice by
+// reference's exact signatures, a const filter, a container of filters.  Linked against the recording fake of the C-ABI
+// (tests/stub/stub_*.cpp, no GPU) it runs a few frames and prints a checksum of the integer bookkeeping.  Compiled twice by
 // tests/test_dropin_boundary_cpu.py: with the POD stand-ins (MSCKF_B200_NO_EIGEN) and through the Eigen branch against
 // tests/stub/mini_eigen (a mock of the Eigen names, since this image has no Eigen).
 #include <cstdio>

@@ -1,49 +1,28 @@
 // tests/stub/stub_aid_iter.cpp -- TEST INFRASTRUCTURE ONLY.
 // The iterated stacked aided-update calls of include/msckf_b200.h (msckf_b200_aid_stack_update_iter / _fde_iter and their batch
-// forms) for the recording fake tests/stub/stub_engine.cpp, with NO numerics.  Each call checks what the engine checks of its
-// arguments besides the items (a NULL iter or iter_out, max_iter outside 0..16, a tol that is not finite and >= 0, 1 to 8 items)
-// and records per engine: the single and batched calls, the IMU readings the engine had been handed by the last call, that
-// call's max_iter, tol, chi2_max (NaN with FDE), max_exclude (-1 without) and item models.  It answers applied with
-// iterations = max(max_iter, 1), converged 1 and step tol / 2.  Linked with stub_engine.cpp, stub_batch_state.cpp, stub_aid.cpp,
-// stub_aid_stack.cpp and the C view (filter_capi.cpp, batch_capi.cpp, aid_capi.cpp, aid_stack_capi.cpp, fde_capi.cpp,
-// aid_iter_capi.cpp) into tests/stub/libmsckf_aid_iter_view_stub.so by tests/test_aid_iter_cpu.py.  Nothing outside tests/ builds
-// or loads it.
-#include <msckf_b200.h>
+// forms) for the recording fake of the C-ABI (tests/stub/stub.hpp), with NO numerics.  Each call checks what the engine checks
+// of its arguments besides the items (a NULL iter or iter_out, max_iter outside 0..16, a tol that is not finite and >= 0, 1 to
+// 8 items) and records per engine: the single and batched calls, the IMU readings the engine had been handed by the last call,
+// that call's max_iter, tol, chi2_max (NaN with FDE), max_exclude (-1 without) and item models.  It answers applied with
+// iterations = max(max_iter, 1), converged 1 and step tol / 2.  Nothing outside tests/ builds or loads it.
+#include "stub.hpp"
 
 #include <cmath>
-#include <map>
-#include <vector>
-
-// the fake's handles: the same definitions as in stub_engine.cpp (one type across the translation units)
-struct msckf_b200_engine {
-  int dtype = 0, M = 0, max_clones = 0;
-  double imu[19] = {0};
-  std::vector<int> last_len;
-  std::vector<int> buf_off, buf_idx;
-  std::vector<double> buf_obs, buf_pfg;
-  long long imu_readings = 0;
-  int pending = 0, mode = 0;
-  long long updates = 0, launches = 0;
-};
-struct msckf_b200_batch { std::vector<msckf_b200_engine*> es; long long launches = 0; };
 
 namespace {
 constexpr int kRec = 13;  // single, batch, readings at the last call, max_iter, tol, chi2_max, max_exclude, n_items, models[5]
-struct Calls {
-  long long single = 0, batch = 0, readings_at_last = -1;
+struct Calls : stub::Calls {
   double max_iter = NAN, tol = NAN, chi2_max = NAN, max_exclude = NAN;
   std::vector<int> models;
 };
-std::map<const msckf_b200_engine*, Calls> g_calls;
-std::map<const msckf_b200_batch*, long long> g_batch_calls;
+stub::Records<Calls> g_calls;
 
 bool valid(const msckf_b200_aid_item* items, int n, const msckf_b200_aid_iter* iter) {
   return items && n >= 1 && n <= 8 && iter && iter->max_iter >= 0 && iter->max_iter <= 16 && std::isfinite(iter->tol) && iter->tol >= 0.0;
 }
 void record(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n, double chi2_max, const msckf_b200_aid_fde* fde,
             const msckf_b200_aid_iter* iter) {
-  Calls& c = g_calls[e];
-  c.readings_at_last = e->imu_readings;
+  Calls& c = g_calls.last(e);
   c.max_iter = iter->max_iter; c.tol = iter->tol;
   c.chi2_max = fde ? NAN : chi2_max;
   c.max_exclude = fde ? fde->max_exclude : -1;
@@ -66,7 +45,7 @@ int single(msckf_b200_engine* e, const msckf_b200_aid_item* items, int n, double
   record(e, items, n, chi2_max, fde, iter);
   answer(n, out);
   answer(iter, iout);
-  g_calls[e].single++;
+  g_calls.engine[e].single++;
   return 0;
 }
 template <class Out>
@@ -80,9 +59,9 @@ int batch(msckf_b200_batch* b, const msckf_b200_aid_item* const* items, const in
       record(b->es[i], items[i], n_items[i], chi2_max, fde, iter + i);
       answer(n_items[i], out + i);
       answer(iter + i, iout + i);
-      g_calls[b->es[i]].batch++;
+      g_calls.engine[b->es[i]].batch++;
     }
-  g_batch_calls[b]++;
+  g_calls.batch[b]++;
   return 0;
 }
 }  // namespace
@@ -111,10 +90,10 @@ int msckf_b200_batch_aid_stack_update_fde_iter(msckf_b200_batch* b, const msckf_
 // call, that call's max_iter, tol, chi2_max (NaN: FDE), max_exclude (-1: no FDE), item count and first 5 item models; the
 // batched iterated calls made on b
 void msckf_b200_stub_aid_iter_calls(const msckf_b200_engine* e, double* rec) {
-  const Calls c = g_calls.count(e) ? g_calls.at(e) : Calls();
+  const Calls c = g_calls.of(e);
   const double v[8] = {(double)c.single, (double)c.batch, (double)c.readings_at_last, c.max_iter, c.tol, c.chi2_max, c.max_exclude,
                        (double)c.models.size()};
   for (int j = 0; j < kRec; ++j) rec[j] = j < 8 ? v[j] : (j - 8 < (int)c.models.size() ? c.models[j - 8] : NAN);
 }
-long long msckf_b200_stub_batch_aid_iter_calls(const msckf_b200_batch* b) { return g_batch_calls.count(b) ? g_batch_calls.at(b) : 0; }
+long long msckf_b200_stub_batch_aid_iter_calls(const msckf_b200_batch* b) { return g_calls.of(b); }
 }

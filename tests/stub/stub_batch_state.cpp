@@ -1,20 +1,13 @@
 // tests/stub/stub_batch_state.cpp -- TEST INFRASTRUCTURE ONLY.
 // The batched state calls of include/msckf_b200.h (msckf_b200_batch_propagate_n / _augment / _prune / _get_state) for the
-// recording fake tests/stub/stub_engine.cpp, with NO numerics: each validates every member first, then forwards to the
-// fake's single-engine calls, and records one call per batched operation.  Linked with stub_engine.cpp,
-// msckf_mono_b200/csrc/filter_capi.cpp and batch_capi.cpp into tests/stub/libmsckf_batch_view_stub.so by
-// tests/test_batch_stream_cpu.py.  Nothing outside tests/ builds or loads it.
-#include <msckf_b200.h>
+// recording fake of the C-ABI (tests/stub/stub.hpp), with NO numerics: each validates every member first, then forwards to
+// the fake's single-engine calls, and records one call per batched operation.  Nothing outside tests/ builds or loads it.
+#include "stub.hpp"
 
-#include <map>
-#include <vector>
-
-// the fake's batch handle: the same definition as in stub_engine.cpp (one type across the two translation units)
-struct msckf_b200_batch { std::vector<msckf_b200_engine*> es; long long launches = 0; };
+using stub::fail;
 
 namespace {
 std::map<const msckf_b200_batch*, std::vector<long long>> g_calls;  // per batch: propagate_n, augment, prune, get_state
-int fail(int code, const char* why) { (void)why; return code; }  // (the fake's error text belongs to stub_engine.cpp)
 void record(const msckf_b200_batch* b, int op) {
   auto& c = g_calls[b];
   c.resize(4, 0);

@@ -1,28 +1,19 @@
 // tests/stub/stub_engine.cpp -- TEST INFRASTRUCTURE ONLY.
-// A recording fake of the C-ABI of include/msckf_b200.h with NO numerics: it counts clones, remembers the last batch and
-// fabricates a report in which every track is valid and accepted.  Linked with msckf_mono_b200/csrc/filter_capi.cpp into
-// tests/stub/libmsckf_view_stub.so it lets the CPU tests (-m "not gpu") drive the drop-in class shim
-// (include/msckf_mono/msckf.h) and compare its INTEGER bookkeeping -- track lists, clone ids, last_correlated_id,
-// queued tracks, pruneEmptyStates -- with the oracle on a box without a GPU.  It is not a CPU fallback: it never
-// computes a state, a covariance or a residual, and nothing outside tests/ builds or loads it.
-#include <msckf_b200.h>
+// The single-engine calls of the recording fake of the C-ABI of include/msckf_b200.h, with NO numerics: it counts clones,
+// remembers the last batch and fabricates a report in which every track is valid and accepted.  With the other
+// tests/stub/stub_*.cpp it lets the CPU tests (-m "not gpu") drive the drop-in class shim (include/msckf_mono/msckf.h) and
+// compare its INTEGER bookkeeping -- track lists, clone ids, last_correlated_id, queued tracks, pruneEmptyStates -- with the
+// oracle on a box without a GPU.  It is not a CPU fallback: it never computes a state, a covariance or a residual, and nothing
+// outside tests/ builds or loads it (tests/fake_engine.py does).
+#include "stub.hpp"
 
 #include <cstring>
 #include <string>
-#include <vector>
 
-struct msckf_b200_engine {
-  int dtype = 0, M = 0, max_clones = 0;
-  double imu[19] = {0};
-  std::vector<int> last_len;  // observations per track of the pending batch
-  std::vector<int> buf_off, buf_idx;  // msckf_b200_input_buffer: host arrays the caller packs into
-  std::vector<double> buf_obs, buf_pfg;
-  long long imu_readings = 0;
-  int pending = 0, mode = 0;
-  long long updates = 0, launches = 0;
-};
 static thread_local std::string g_err;
-static int fail(int code, const char* msg) { g_err = msg; return code; }
+int stub::fail(int code, const char* msg) { g_err = msg; return code; }
+using stub::fail;
+static stub::Records<> g_jac;  // msckf_b200_jac_group per engine, msckf_b200_batch_jac_occupancy per batch
 template <class T> static void put(void* p, size_t i, double v, int dtype) {
   (void)sizeof(T);
   if (dtype == MSCKF_B200_F32) ((float*)p)[i] = (float)v; else ((double*)p)[i] = v;
@@ -105,7 +96,6 @@ int msckf_b200_update_batch(msckf_b200_engine** es, int n, int mode, const msckf
   for (int i = 0; i < n; ++i) { int rc = msckf_b200_update(es[i], mode, &tr[i], reps ? &reps[i] : nullptr); if (rc) return rc; }
   return 0;
 }
-struct msckf_b200_batch { std::vector<msckf_b200_engine*> es; long long launches = 0; };
 int msckf_b200_batch_create(msckf_b200_engine** es, int n, msckf_b200_batch** out) { auto* b = new msckf_b200_batch(); b->es.assign(es, es + n); *out = b; return 0; }
 int msckf_b200_batch_destroy(msckf_b200_batch* b) { delete b; return 0; }
 int msckf_b200_batch_stage(msckf_b200_batch* b, int mode, const msckf_b200_tracks* tr, int) {
@@ -129,6 +119,17 @@ int msckf_b200_batch_update(msckf_b200_batch* b, int mode, const msckf_b200_trac
 int msckf_b200_batch_kernel_times(msckf_b200_batch*, float*, const char**, int) { return 0; }
 long long msckf_b200_batch_launch_count(const msckf_b200_batch* b) { return b->launches; }
 void* msckf_b200_batch_stream(msckf_b200_batch*) { return nullptr; }
+// no kernel ever runs: both answer "before the first launch"
+int msckf_b200_batch_jac_occupancy(const msckf_b200_batch* b) {
+  if (!b) return fail(MSCKF_B200_ERR_ARG, "stub: null batch");
+  g_jac.batch[b]++;
+  return 0;
+}
+int msckf_b200_jac_group(msckf_b200_engine* e) {
+  if (!e) return fail(MSCKF_B200_ERR_ARG, "stub: null engine");
+  g_jac.last(e).single++;
+  return 0;
+}
 int msckf_b200_kernel_times(msckf_b200_engine*, float*, const char**, int) { return 0; }
 int msckf_b200_tail_profile(msckf_b200_engine*, unsigned long long*, int) { return 0; }
 int msckf_b200_prune(msckf_b200_engine* e, const int* keep, int n_keep) {
@@ -173,4 +174,8 @@ long long msckf_b200_launch_count(const msckf_b200_engine* e) { return e->launch
 void* msckf_b200_stream(msckf_b200_engine*) { return nullptr; }
 int msckf_b200_synchronize(msckf_b200_engine*) { return 0; }
 const char* msckf_b200_last_error(void) { return g_err.c_str(); }
+// test hook: out2 = msckf_b200_jac_group calls on e, msckf_b200_batch_jac_occupancy calls on b
+void msckf_b200_stub_jac_calls(const msckf_b200_engine* e, const msckf_b200_batch* b, long long* out2) {
+  out2[0] = g_jac.of(e).single; out2[1] = g_jac.of(b);
+}
 }

@@ -2,10 +2,9 @@
 MSCKFBatch::aidedUpdate (one C-ABI call per class call, queued IMU readings handed over first, the host mirror refreshed
 afterwards), and the Monte-Carlo runner's position fixes (the trials' other inputs do not change).
 
-The C view is linked against the recording fake of the C-ABI (tests/stub/stub_engine.cpp, stub_batch_state.cpp) plus
-tests/stub/stub_aid.cpp, whose VELOCITY / POSITION "update" copies z into the fake's IMU state."""
+The C view is linked against the recording fake of the C-ABI (tests/fake_engine.py), whose aided calls
+(tests/stub/stub_aid.cpp) copy z of a VELOCITY / POSITION "update" into the fake's IMU state."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,21 +12,8 @@ from scipy import stats
 
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.common import ROOT
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
-
-
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_aid_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "tests" / "stub" / "stub_batch_state.cpp",
-           ROOT / "tests" / "stub" / "stub_aid.cpp", csrc / "filter_capi.cpp", csrc / "batch_capi.cpp", csrc / "aid_capi.cpp"]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", *map(str, src), "-o", str(so)])
-    return so
 
 
 def _calls(f, base=(0, 0)):

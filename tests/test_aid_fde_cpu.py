@@ -1,7 +1,7 @@
 """The numpy FDE over a stack's items (tests/aid_fde_reference.py), without a device: the block w-test against the NIS
 difference, and the outcomes the rounds of msckf_b200_aid_stack_update_fde reach on range stacks with and without NLOS faults;
 capi.fde_thresholds / fde_struct; and what the class and C view forms send to the C-ABI, through the recording fake of
-tests/aid_stack_stub.py."""
+tests/fake_engine.py."""
 import ctypes as C
 
 import numpy as np
@@ -10,7 +10,7 @@ import pytest
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
 from tests import aid_fde_reference as ref
-from tests.aid_stack_stub import recorded, stub_view  # noqa: F401 (stub_view: the fixture)
+from tests.fake_engine import recorded, stub_view  # noqa: F401 (stub_view: the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 CHI2 = capi.fde_thresholds(0.01)

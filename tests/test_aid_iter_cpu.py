@@ -4,7 +4,6 @@ iteration restores the consistency one linearisation loses after drift.  Also wh
 C-ABI, through a recording fake of the iterated entry points (tests/stub/stub_aid_iter.cpp), and the runner's trial inputs
 with --range-start / --gnss-start."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,7 +12,7 @@ from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
 from tests import aid_iter_reference as ref
 from tests.aid_fde_reference import linearise
-from tests.common import ROOT
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 
@@ -104,23 +103,6 @@ def test_anchor_toy_consistency():
 
 
 # ---- the class and C view forms over a fake of the iterated entry points -------------------------------------------------------
-CSRC = ROOT / "msckf_mono_b200" / "csrc"
-STUB_SOURCES = [ROOT / "tests" / "stub" / n for n in ("stub_engine.cpp", "stub_batch_state.cpp", "stub_aid.cpp", "stub_aid_stack.cpp",
-                                                      "stub_aid_iter.cpp")]
-STUB_SOURCES += [CSRC / n for n in ("filter_capi.cpp", "batch_capi.cpp", "aid_capi.cpp", "aid_stack_capi.cpp", "fde_capi.cpp",
-                                    "aid_iter_capi.cpp")]
-STUB_HEADERS = [CSRC / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-
-
-@pytest.fixture(scope="module")
-def iter_view():
-    """the C view linked against the recording fake of the C-ABI plus tests/stub/stub_aid_iter.cpp"""
-    so = ROOT / "tests" / "stub" / "libmsckf_aid_iter_view_stub.so"
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in STUB_SOURCES + STUB_HEADERS):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", f"-I{CSRC}",
-                               *map(str, STUB_SOURCES), "-o", str(so)])
-    return so
 
 
 def _recorded(f):
@@ -143,11 +125,11 @@ def _filters(lib, n, dtype, frames=4):
 
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
-def test_views_pass_the_iteration_options_through(iter_view, dtype):
+def test_views_pass_the_iteration_options_through(stub_view, dtype):
     """MSCKF::aidedUpdate(items, chi2_max | fde, iter, iter_out) and the MSCKFBatch forms through the C view: one C-ABI call per
     class call with the IMU queue handed over first, max_iter / tol / chi2_max / fde passed as given, the results returned;
     options the C-ABI would refuse throw std::invalid_argument in the class before any call"""
-    fs, wl = _filters(iter_view, 3, dtype)
+    fs, wl = _filters(stub_view, 3, dtype)
     rng = np.random.default_rng(9)
     stack = [{"model": capi.AID_RANGE, "z": rng.normal(size=7), "R": np.array([[0.01]])},
              {"model": capi.AID_CLONE_PLANE_RANGE, "a": 2, "z": rng.normal(size=8), "R": np.array([[0.03]])},

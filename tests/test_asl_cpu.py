@@ -64,19 +64,17 @@ def test_player_rejects_missing_folder(engine_lib):
 
 
 def test_player_call_sequence_on_cpu_against_the_oracle(mav0, oracle_lib, tmp_path):
-    """The compiled player's host logic without a GPU: asl_player.cpp linked against tests/stub/stub_engine.cpp (a fake
-    of the C-ABI with no numerics) must hand the class the same frames, IMU readings and tracked / new feature split as
+    """The compiled player's host logic without a GPU: asl_player.cpp linked against the recording fake of the C-ABI
+    (tests/fake_engine.py, no numerics) must hand the class the same frames, IMU readings and tracked / new feature split as
     `synth.drive` hands the oracle: the clone-window size per frame (update / addFeatures / pruneEmptyStates bookkeeping)
     is then identical.  pruneRedundantStates is off here: its decisions depend on poses, which the fake does not compute."""
     import subprocess
     from tests.common import ROOT, make_oracle
+    from tests.fake_engine import build_program
     wl, m = mav0
-    exe = ROOT / "tests" / "stub" / "asl_player_stub"
-    src = [ROOT / "msckf_mono_b200" / "asl" / "asl_player.cpp", ROOT / "tests" / "stub" / "stub_engine.cpp",
-           ROOT / "msckf_mono_b200" / "asl" / "asl_io.hpp", ROOT / "include" / "msckf_mono" / "msckf.h"]
-    if (not exe.exists()) or any(s.stat().st_mtime > exe.stat().st_mtime for s in src):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", f"-I{ROOT / 'include'}", f"-I{ROOT / 'msckf_mono_b200' / 'asl'}",
-                               str(src[0]), str(src[1]), "-o", str(exe)])
+    asl_dir = ROOT / "msckf_mono_b200" / "asl"
+    exe = build_program(ROOT / "tests" / "stub" / "asl_player_stub", [asl_dir / "asl_player.cpp"], deps=[asl_dir / "asl_io.hpp"],
+                        flags=[f"-I{asl_dir}"])
     out = tmp_path / "traj_stub.csv"
     r = subprocess.run([str(exe), "--mav0", m, "--dtype", "f64", "--out", str(out), "--prune-redundant", "0", "--state-id", "frame"],
                        capture_output=True, text=True, timeout=120)

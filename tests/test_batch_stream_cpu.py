@@ -1,34 +1,20 @@
 """Host logic of the batched per-image step (msckf_mono::MSCKFBatch, include/msckf_mono/msckf.h) on a box WITHOUT a GPU.
 
-The C view is linked against `tests/stub/stub_engine.cpp`, the recording fake of the C-ABI (no numerics), like
-test_shim_bookkeeping_cpu.py does, plus `tests/stub/stub_batch_state.cpp`, the fake's batched state calls.  Filters driven through the batch and single filters driven alone on the same streams
+The C view is linked against the recording fake of the C-ABI (no numerics, tests/fake_engine.py), like
+test_shim_bookkeeping_cpu.py does; `tests/stub/stub_batch_state.cpp` holds the fake's batched state calls.  Filters driven through the batch and single filters driven alone on the same streams
 must make the same integer decisions frame by frame, and the batch must reach the C-ABI through one batched call per
 device operation and frame."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.common import ROOT
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 from tests.test_shim_bookkeeping_cpu import _ids, shim_filter
 
 PROPAGATE, AUGMENT, PRUNE, GET_STATE = range(4)
-
-
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_batch_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "tests" / "stub" / "stub_batch_state.cpp",
-           csrc / "filter_capi.cpp", csrc / "batch_capi.cpp"]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", *map(str, src), "-o", str(so)])
-    return so
 
 
 def _calls(fb):

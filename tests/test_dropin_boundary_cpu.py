@@ -11,14 +11,13 @@ import subprocess
 import pytest
 
 from tests.common import ROOT
+from tests.fake_engine import build_program
 
 SRC = ROOT / "tests" / "stub" / "caller_shaped.cpp"
-STUB = ROOT / "tests" / "stub" / "stub_engine.cpp"
 
 
 def build_and_run(tmp_path, name, extra):
-    exe = tmp_path / name
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-Wall", "-Werror=return-type", f"-I{ROOT / 'include'}", *extra, str(SRC), str(STUB), "-o", str(exe)])
+    exe = build_program(tmp_path / name, [SRC], flags=["-Wall", "-Werror=return-type", *extra])
     return subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout
 
 

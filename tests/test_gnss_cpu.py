@@ -3,7 +3,7 @@
 the heading wrap, what the class forms (MSCKF::antennaPositionUpdate, cloneAntennaPositionUpdate, headingUpdate,
 cloneHeadingUpdate) and MSCKFBatch::aidedUpdate(items) send to the C-ABI, and the Monte-Carlo runner's GNSS inputs and summary.
 
-The C view is linked against the recording fake of the C-ABI (tests/aid_stack_stub.py), which records every stacked item in
+The C view is linked against the recording fake of the C-ABI (tests/fake_engine.py), which records every stacked item in
 full and calls the class forms on a view handle."""
 import ctypes as C
 import math
@@ -13,7 +13,7 @@ import pytest
 
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.aid_stack_stub import batch_calls, recorded, stub_view  # noqa: F401 (stub_view: the fixture)
+from tests.fake_engine import batch_calls, recorded, stub_view  # noqa: F401 (stub_view: the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 GNSS = (capi.AID_ANTENNA_POSITION, capi.AID_CLONE_ANTENNA_POSITION, capi.AID_HEADING, capi.AID_CLONE_HEADING)

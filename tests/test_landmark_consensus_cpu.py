@@ -9,6 +9,7 @@ import pytest
 
 from msckf_mono_b200 import capi
 from tests import landmark_consensus_reference as ref, landmark_map_reference as mref, side_shapes as ss
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 
 R_PIX = np.array([[4.0e-6, 5.0e-7], [5.0e-7, 3.0e-6]])
 THRESH = 13.8  # chi-square, 2 dof, 0.999
@@ -90,20 +91,6 @@ def test_consensus_struct():
 
 
 # ---- the class and the C view over a fake C-ABI (tests/stub/stub_landmark_consensus.cpp) -------------------------------------
-@pytest.fixture(scope="module")
-def cons_view():
-    import subprocess
-    from tests.common import ROOT
-    so = ROOT / "tests" / "stub" / "libmsckf_consensus_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "tests" / "stub" / "stub_batch_state.cpp",
-           ROOT / "tests" / "stub" / "stub_landmark_iter.cpp", ROOT / "tests" / "stub" / "stub_landmark_consensus.cpp",
-           csrc / "filter_capi.cpp", csrc / "batch_capi.cpp", csrc / "landmark_capi.cpp", csrc / "consensus_capi.cpp"]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", *map(str, src), "-o", str(so)])
-    return so
 
 
 def _calls(f):
@@ -126,9 +113,9 @@ BAD = [{"hypotheses": 1025, "thresh": 9.0, "min_inliers": 2}, {"hypotheses": 8, 
 
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
-def test_class_maps_ids_and_forwards_the_consensus(cons_view, dtype):
+def test_class_maps_ids_and_forwards_the_consensus(stub_view, dtype):
     from tests.test_landmark_cpu import _filters
-    (f,), wl = _filters(cons_view, 1, dtype, frames=4)
+    (f,), wl = _filters(stub_view, 1, dtype, frames=4)
     z, p = np.tile([0.01, -0.02], (4, 1)), np.tile([1.0, 2.0, 5.0], (4, 1))
     ids = [wl["frames"][k]["state_id"] for k in (2, 0, 2, 1)]
     cb = _calls(f)
@@ -153,10 +140,10 @@ def test_class_maps_ids_and_forwards_the_consensus(cons_view, dtype):
     f.close()
 
 
-def test_batch_makes_one_call(cons_view):
+def test_batch_makes_one_call(stub_view):
     from msckf_mono_b200.cview import FilterBatch
     from tests.test_landmark_cpu import _filters
-    fs, wl = _filters(cons_view, 3, np.float64, frames=4)
+    fs, wl = _filters(stub_view, 3, np.float64, frames=4)
     fb = FilterBatch(fs)
     z, p = np.tile([0.01, -0.02], (3, 1)), np.tile([1.0, 2.0, 5.0], (3, 1))
     sid = [fr["state_id"] for fr in wl["frames"][:3]]

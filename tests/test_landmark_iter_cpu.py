@@ -2,9 +2,8 @@
 linearisation is the dense EKF of tests/test_landmark_gpu.py exactly; a converged result satisfies the Gauss-Newton
 stationarity condition; on the relocalisation toy the single linearisation is inconsistent after a large drift and the
 iterated update is consistent), the class's and the bindings' handling of max_iter / tol over a recording fake of the C-ABI
-(tests/stub/stub_landmark_iter.cpp), and the runner's map_start."""
+(tests/stub/stub_landmark.cpp), and the runner's map_start."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
@@ -12,7 +11,7 @@ from scipy import stats
 
 from msckf_mono_b200 import capi, montecarlo as mc
 from msckf_mono_b200.cview import FilterBatch
-from tests.common import ROOT
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 from tests.landmark_iter_reference import boxminus, boxplus, iekf, relocalisation_trial, stationarity
 from tests.test_aid_gpu import numpy_update
 from tests.test_landmark_cpu import _filters, _obs
@@ -111,20 +110,6 @@ def test_relocalisation_toy(drift_pos, drift_yaw):
     assert lo <= res[10] <= hi
 
 
-@pytest.fixture(scope="module")
-def iter_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_landmark_iter_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "tests" / "stub" / "stub_batch_state.cpp",
-           ROOT / "tests" / "stub" / "stub_landmark_iter.cpp", csrc / "filter_capi.cpp", csrc / "batch_capi.cpp",
-           csrc / "landmark_capi.cpp"]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", *map(str, src), "-o", str(so)])
-    return so
-
-
 def _iter_of(f):
     m, t = C.c_int(), C.c_double()
     f.lib.msckf_b200_stub_landmark_iter(C.c_void_p(f.engineHandle()), C.byref(m), C.byref(t))
@@ -132,8 +117,8 @@ def _iter_of(f):
 
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
-def test_class_passes_max_iter_and_tol(iter_view, dtype):
-    (f,), _ = _filters(iter_view, 1, dtype, frames=4)
+def test_class_passes_max_iter_and_tol(stub_view, dtype):
+    (f,), _ = _filters(stub_view, 1, dtype, frames=4)
     z, p = _obs(3)
     r = f.landmark_update([2, 0, 2], z, p)
     assert _iter_of(f) == (1, 1e-10) and r["iterations"] == 1 and r["converged"] == 0  # the defaults: one linearisation
@@ -145,8 +130,8 @@ def test_class_passes_max_iter_and_tol(iter_view, dtype):
     f.close()
 
 
-def test_batch_passes_max_iter_and_tol(iter_view):
-    fs, _ = _filters(iter_view, 3, np.float64, frames=4)
+def test_batch_passes_max_iter_and_tol(stub_view):
+    fs, _ = _filters(stub_view, 3, np.float64, frames=4)
     fb = FilterBatch(fs)
     z, p = _obs(3)
     res = fb.landmark_update([([0, 1], z[:2], p[:2]), None, ([2], z[:1], p[:1])], max_iter=4, tol=1e-6)

@@ -2,7 +2,6 @@
 its row count, the Python binding's packing of landmark ids and Sigma_L, and the class and C view over a recording stub of
 the C-ABI (tests/stub/stub_landmark_map.cpp).  No GPU."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
@@ -11,7 +10,7 @@ from msckf_mono_b200 import capi, montecarlo as mc
 from msckf_mono_b200.cview import FilterBatch
 from oracle.msckf_numpy import quat_normalized
 from tests import landmark_map_reference as ref
-from tests.common import ROOT
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 from tests.test_aid_gpu import numpy_update
 from tests.test_landmark_cpu import _filters
 from tests.test_landmark_gpu import dense as exact_dense
@@ -126,20 +125,6 @@ def test_binding_packs_landmarks_and_sigma():
     assert C.sizeof(capi.Landmarks) == 80 and C.sizeof(capi.LandmarkMap) == 24
 
 
-@pytest.fixture(scope="module")
-def map_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_landmark_map_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "tests" / "stub" / "stub_batch_state.cpp",
-           ROOT / "tests" / "stub" / "stub_landmark_iter.cpp", ROOT / "tests" / "stub" / "stub_landmark_map.cpp",
-           csrc / "filter_capi.cpp", csrc / "batch_capi.cpp", csrc / "landmark_capi.cpp", csrc / "map_capi.cpp"]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", *map(str, src), "-o", str(so)])
-    return so
-
-
 def _map_calls(f):
     out = (C.c_longlong * 3)()
     f.lib.msckf_b200_stub_map_calls(C.c_void_p(f.engineHandle()), out)
@@ -157,8 +142,8 @@ LMK_S = np.array([[1e-2, 0.0, 2e-2, 0.0, 0.0, 3e-2], [4e-2, 1e-3, 5e-2, 0.0, 2e-
 
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
-def test_class_maps_ids_and_forwards_the_map(map_view, dtype):
-    (f,), wl = _filters(map_view, 1, dtype, frames=4)
+def test_class_maps_ids_and_forwards_the_map(stub_view, dtype):
+    (f,), wl = _filters(stub_view, 1, dtype, frames=4)
     z = np.tile([0.01, -0.02], (3, 1))
     cb = _map_calls(f)  # (the stub keys its records by engine address, which an earlier, closed filter may have had)
     r = f.map_update([2, 0, 2], [1, 0, 0], z, LMK_P, LMK_S)
@@ -183,8 +168,8 @@ def test_class_maps_ids_and_forwards_the_map(map_view, dtype):
     f.close()
 
 
-def test_batch_maps_ids_and_forwards_the_map(map_view):
-    fs, _ = _filters(map_view, 3, np.float64, frames=4)
+def test_batch_maps_ids_and_forwards_the_map(stub_view):
+    fs, _ = _filters(stub_view, 3, np.float64, frames=4)
     fb = FilterBatch(fs)
     z = np.tile([0.01, -0.02], (2, 1))
     S33 = np.stack([ref.sym(s) for s in LMK_S])

@@ -3,14 +3,14 @@ bodyVelocityUpdate, relativePoseUpdate and MSCKFBatch::aidedUpdate(items) (one C
 handed over first, the host mirror refreshed afterwards, state ids mapped to window positions), and the Monte-Carlo runner's
 odometry (the trials' other inputs do not change; the truth odometry agrees with the truth trajectory).
 
-The C view is linked against the recording fake of the C-ABI (tests/aid_stack_stub.py), whose VELOCITY / POSITION items
+The C view is linked against the recording fake of the C-ABI (tests/fake_engine.py), whose VELOCITY / POSITION items
 copy z into the fake's IMU state."""
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import capi, montecarlo as mc, synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.aid_stack_stub import batch_calls, recorded, stub_view  # noqa: F401 (stub_view: the fixture)
+from tests.fake_engine import batch_calls, recorded, stub_view  # noqa: F401 (stub_view: the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 

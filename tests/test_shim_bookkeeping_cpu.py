@@ -2,28 +2,18 @@
 
 The shim keeps every integer decision of the reference on the host (update(): which tracks are residualised and with
 which clones, addFeatures(), pruneEmptyStates(), finish(); msckf.h:215-332, :685-807) and forwards only numerics to the
-C-ABI.  Here the C view of the shim is linked against `tests/stub/stub_engine.cpp` -- a recording fake of the C-ABI
-without any numerics (test infrastructure, not a fallback) -- and driven next to the oracle on the same streams.
+C-ABI.  Here the C view of the shim is linked against the recording fake of the C-ABI built by `tests/fake_engine.py`
+-- without any numerics (test infrastructure, not a fallback) -- and driven next to the oracle on the same streams.
 Everything that does not depend on a computed number must be identical, frame by frame."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import synth
 from msckf_mono_b200.cview import CFilter
-from tests.common import ROOT, make_oracle
-
-
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_view_stub.so"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "msckf_mono_b200" / "csrc" / "filter_capi.cpp",
-           ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h", ROOT / "include" / "msckf_b200.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in src):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", str(src[0]), str(src[1]), "-o", str(so)])
-    return so
+from tests.common import make_oracle
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 
 
 def shim_filter(lib, dtype, max_clones=0):

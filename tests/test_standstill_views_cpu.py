@@ -1,34 +1,19 @@
 """Host side of the standstill update without a GPU: MSCKF::standstillUpdate, MSCKFBatch::standstillUpdate and the at-rest
-class forms through the C view, linked against the recording fake of the C-ABI (tests/stub/stub_engine.cpp,
-stub_batch_state.cpp) plus tests/stub/stub_standstill.cpp.  The readings, the cfg and the result travel unchanged, queued
+class forms through the C view, linked against the recording fake of the C-ABI (tests/fake_engine.py; its standstill calls
+are tests/stub/stub_standstill.cpp).  The readings, the cfg and the result travel unchanged, queued
 IMU readings are handed over first, members without readings are left alone, and bad input is refused before any call."""
 import ctypes as C
-import subprocess
 
 import numpy as np
 import pytest
 
 from msckf_mono_b200 import capi, synth
 from msckf_mono_b200.cview import FilterBatch
-from tests.common import ROOT
+from tests.fake_engine import stub_view  # noqa: F401 (the fixture)
 from tests.test_shim_bookkeeping_cpu import shim_filter
 
 DTYPES = [np.float32, np.float64]
 CFG = {"noise_scale": 1.5, "sigma_v": 0.01, "scatter_max": 2.0, "chi2_max": 30.0}
-
-
-@pytest.fixture(scope="module")
-def stub_view():
-    so = ROOT / "tests" / "stub" / "libmsckf_standstill_view_stub.so"
-    csrc = ROOT / "msckf_mono_b200" / "csrc"
-    src = [ROOT / "tests" / "stub" / "stub_engine.cpp", ROOT / "tests" / "stub" / "stub_batch_state.cpp",
-           ROOT / "tests" / "stub" / "stub_standstill.cpp", csrc / "filter_capi.cpp", csrc / "batch_capi.cpp", csrc / "standstill_capi.cpp"]
-    deps = src + [csrc / "filter_view.hpp", ROOT / "include" / "msckf_mono" / "msckf.h", ROOT / "include" / "msckf_mono" / "types.h",
-                  ROOT / "include" / "msckf_b200.h", ROOT / "include" / "msckf_mono_c.h"]
-    if (not so.exists()) or any(s.stat().st_mtime > so.stat().st_mtime for s in deps):
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{ROOT / 'include'}", f"-I{csrc}", *map(str, src),
-                               "-o", str(so)])
-    return so
 
 
 def _calls(f):
@@ -138,11 +123,12 @@ def test_at_rest_class_forms_send_one_item_and_check_R(stub_view, dtype):
         rc = f.lib.msckf_b200_stub_at_rest_class_call(f.h, C.c_int(which), (C.c_double * 3)(*v), (C.c_double * 9)(*R.ravel()),
                                                       C.c_int(3), C.byref(out))
         assert rc == 0 and out.dof == 3 and out.applied == 1
-        rec = (C.c_double * 15)()
-        assert f.lib.msckf_b200_stub_standstill_items(C.c_void_p(f.engineHandle()), rec, 1) == 1
-        rec = np.array(rec[:])
-        assert rec[0] == model and rec[1] == 0 and rec[2] == 0
-        assert np.array_equal(rec[3:6], v) and np.array_equal(rec[6:15], R.ravel())
+        rec = (C.c_double * (15 * 8))()
+        n = f.lib.msckf_b200_stub_standstill_items(C.c_void_p(f.engineHandle()), rec, 8)
+        rec = np.array(rec[:15 * n]).reshape(n, 15)
+        assert list(rec[:, 0]) == [model]  # one item, of the at-rest model (the fake takes every stack model)
+        assert rec[0, 1] == 0 and rec[0, 2] == 0
+        assert np.array_equal(rec[0, 3:6], v) and np.array_equal(rec[0, 6:15], R.ravel())
     stacks = _calls(f)[0][3]
     out = capi.AidResult()
     rc = f.lib.msckf_b200_stub_at_rest_class_call(f.h, C.c_int(0), (C.c_double * 3)(*v), (C.c_double * 4)(*R[:2, :2].ravel()),
